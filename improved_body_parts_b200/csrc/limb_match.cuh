@@ -146,13 +146,15 @@ __device__ __forceinline__ int match_limb(const Workspace &ws, int n, int k, int
     const int lim = min(nA, nB);
     const size_t baseA = ((size_t)n * ws.K + pa) * ws.capP, baseB = ((size_t)n * ws.K + pb) * ws.capP;
 
-    auto emit = [&](int m, uint32_t ij, int cidx) {  // row [idA, idB, score, i, j, norm] (evaluate.py:267)
+    // the rest of row c [idA, idB, score, i, j, norm] (evaluate.py:267) once o_ij[c] holds (i, j): the score of candidate
+    // cidx and the limb length (the reference's `norm`, :225)
+    auto fill_row = [&](int c, int cidx) {
+        const uint32_t ij = o_ij[c];
         const int i = (int)(ij >> 16), j = (int)(ij & 0xffff);
         const double vx = __dsub_rn(ws.peak_x[baseB + j], ws.peak_x[baseA + i]);
         const double vy = __dsub_rn(ws.peak_y[baseB + j], ws.peak_y[baseA + i]);
-        o_ij[m] = ij;
-        o_score[m] = ws.cand_score[cbase + cidx];
-        o_norm[m] = __dsqrt_rn(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));
+        o_score[c] = ws.cand_score[cbase + cidx];
+        o_norm[c] = __dsqrt_rn(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));
     };
 
     int m = 0;
@@ -173,15 +175,8 @@ __device__ __forceinline__ int match_limb(const Workspace &ws, int n, int k, int
             case 11: case 12: m = match_rounds_keys<12>(o_ij, o_norm, key8, nC, lim, lane); break;
             default: m = match_rounds_keys<16>(o_ij, o_norm, key8, nC, lim, lane); break;
         }
-        __syncwarp();  // the rows were written by different lanes of this warp
-        for (int c = lane; c < m; c += 32) {  // scores and limb lengths (the reference's `norm`, :225) in parallel
-            const uint32_t ij = o_ij[c];
-            o_score[c] = ws.cand_score[cbase + reinterpret_cast<const int *>(o_norm + c)[0]];
-            const int i = (int)(ij >> 16), j = (int)(ij & 0xffff);
-            const double vx = __dsub_rn(ws.peak_x[baseB + j], ws.peak_x[baseA + i]);
-            const double vy = __dsub_rn(ws.peak_y[baseB + j], ws.peak_y[baseA + i]);
-            o_norm[c] = __dsqrt_rn(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));
-        }
+        __syncwarp();  // the rows were written by different lanes of this warp; the rounds left row c's candidate index in o_norm[c]
+        for (int c = lane; c < m; c += 32) fill_row(c, reinterpret_cast<const int *>(o_norm + c)[0]);  // in parallel
     } else if (nC <= 32 * kMatchRegF64) {
         // ---- register path, f64 priorities: (ordered f64 priority bits, tie-break), specialised on the slot count -----
         switch (nslots) {
@@ -195,15 +190,8 @@ __device__ __forceinline__ int match_limb(const Workspace &ws, int n, int k, int
             case 9: case 10: case 11: case 12: m = match_rounds_f64<12>(ws, cbase, o_ij, o_norm, nC, lim, lane); break;
             default: m = match_rounds_f64<kMatchRegF64>(ws, cbase, o_ij, o_norm, nC, lim, lane); break;
         }
-        __syncwarp();
-        for (int c = lane; c < m; c += 32) {  // scores and limb lengths in parallel, as in the f32 path
-            const uint32_t ij = o_ij[c];
-            o_score[c] = ws.cand_score[cbase + reinterpret_cast<const int *>(o_norm + c)[0]];
-            const int i = (int)(ij >> 16), j = (int)(ij & 0xffff);
-            const double vx = __dsub_rn(ws.peak_x[baseB + j], ws.peak_x[baseA + i]);
-            const double vy = __dsub_rn(ws.peak_y[baseB + j], ws.peak_y[baseA + i]);
-            o_norm[c] = __dsqrt_rn(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));
-        }
+        __syncwarp();  // as in the f32 path
+        for (int c = lane; c < m; c += 32) fill_row(c, reinterpret_cast<const int *>(o_norm + c)[0]);
     } else {
         // ---- generic path: re-read the list from L2 every round, 128-bit used masks -------------------
         unsigned long long uA0 = 0, uA1 = 0, uB0 = 0, uB1 = 0;
@@ -234,7 +222,10 @@ __device__ __forceinline__ int match_limb(const Workspace &ws, int n, int k, int
             const int i = bi / nB, j = bi - i * nB;
             if (i < 64) uA0 |= 1ull << i; else uA1 |= 1ull << (i - 64);
             if (j < 64) uB0 |= 1ull << j; else uB1 |= 1ull << (j - 64);
-            if (lane == 0) emit(m, ((uint32_t)i << 16) | (uint32_t)j, bidx);
+            if (lane == 0) {
+                o_ij[m] = ((uint32_t)i << 16) | (uint32_t)j;
+                fill_row(m, bidx);
+            }
             m++;
         }
     }

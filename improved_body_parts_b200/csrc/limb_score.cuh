@@ -36,7 +36,6 @@ struct ScoreArgs {
     const void *paf;
     int64_t img_stride, chan_stride;  // elements
     int H, W, image_base, mid_num, screen;
-    int debug;                                       // only read in -DSPG_DEBUG builds (timing experiments); always 0 otherwise
     int crit1_strict;                                // demo_image.py:288 compares with `>` where evaluate.py:246 uses `>=`
     int exact_warps;                                 // persistent kernel: scorer warps (the rest screen)
     double image_extent, thre2, connect_ration;
@@ -52,13 +51,50 @@ constexpr int kScreenMaxMid = 63;       // per-m tables (maxfail, sample positio
 constexpr int kScreenSamples = SPG_SCREEN_SAMPLES;  // interior samples looked at per pair (build-time: `make variants` for the tuning sweep)
 constexpr int kScreenMaxDim = 2048;     // f32 error of a 1/64-px position stays << 1 unit up to this map size
 
+// per-m constants of the screen (m = number of samples the reference would take for the pair)
+struct alignas(8) ScreenTab {
+    float inv;            // 1 / (m - 1)
+    signed char maxfail;  // failures the connect_ration criterion tolerates
+    unsigned char qn;     // interior samples the screen looks at
+    unsigned char pad[2];
+};
+
+// The per-m tables of both kernels, in this order: rcp[m] = RN(1/m) (phase B), ScreenTab tab[m], ts[m][kScreenSamples]
+// (sample positions of the screen); m = 0 .. kScreenMaxMid.
+__host__ __device__ constexpr size_t screen_tables_bytes() {
+    return (((size_t)(kScreenMaxMid + 1) * (sizeof(double) + sizeof(ScreenTab) + kScreenSamples * sizeof(float))) + 15) & ~(size_t)15;
+}
+
+// Builds row m of the per-m tables.
+__device__ __forceinline__ void build_screen_row(const ScoreArgs &a, int m, double *rcp, ScreenTab *tab, float *ts) {
+    // fewest samples that must exceed thre2: smallest integer >= connect_ration*m in f64, as :246 compares
+    const double need = __dmul_rn(a.connect_ration, (double)m);
+    int need_i = (int)need;
+    if ((double)need_i < need || (a.crit1_strict && (double)need_i == need)) need_i++;  // strict: smallest integer > need
+    rcp[m] = m > 0 ? __ddiv_rn(1.0, (double)m) : 0.0;
+    // up to kScreenSamples samples spread over the interior [lo, hi] (the ends sit on the peaks and rarely fail)
+    const int lo = m / 8, hi = m - 1 - lo;
+    const int qn = max(0, min(kScreenSamples, hi - lo + 1));
+    for (int q = 0; q < kScreenSamples; q++)  // tail clamped: every entry is a valid sample index
+        ts[m * kScreenSamples + q] = (float)(qn > 1 ? lo + (min(q, qn - 1) * (hi - lo)) / (qn - 1) : lo);
+    ScreenTab t;
+    t.inv = m > 1 ? 1.0f / (float)(m - 1) : 0.0f;
+    t.maxfail = (signed char)max(min(m - need_i, 127), -1);
+    t.qn = (unsigned char)qn;
+    t.pad[0] = t.pad[1] = 0;
+    tab[m] = t;
+}
+
 inline size_t score_smem_bytes(size_t plane_bytes, int capP) {
     const size_t plane = (plane_bytes + 127) & ~(size_t)127;
     const size_t peaks = (size_t)capP * (4 * sizeof(double) + 6 * sizeof(float) + 2);
     const size_t words = ((size_t)capP * capP + 31) / 32;
-    const size_t tables = (size_t)(kScreenMaxMid + 1) * (sizeof(double) + (kScreenSamples + 1) * sizeof(float) + 2);
-    return plane + ((peaks + 15) & ~(size_t)15) + ((tables + 15) & ~(size_t)15) +
-           words * (sizeof(uint32_t) + sizeof(uint16_t)) + 16;
+    return plane + ((peaks + 15) & ~(size_t)15) + screen_tables_bytes() + words * (sizeof(uint32_t) + sizeof(uint16_t)) + 16;
+}
+
+// inside the map [0, W-1] x [0, H-1]
+__device__ __forceinline__ bool inside_map(double x, double y, int H, int W) {
+    return x >= 0.0 && x <= (double)(W - 1) && y >= 0.0 && y <= (double)(H - 1);
 }
 
 struct PairGeom {  // one limb's end-point lists in shared memory
@@ -197,6 +233,29 @@ __device__ __forceinline__ bool score_pair_exact(const T *__restrict__ plane, in
     return crit1 && crit2;
 }
 
+// Candidate `pos` of limb slot `out_base`: pair (i, j) with its score and priority, plus the one-word sort key when the
+// priority is an f32 value (TA = float): 32 order-preserving bits + the tie-break fit one word.
+template <typename TA>
+__device__ __forceinline__ void store_candidate(const Workspace &ws, size_t out_base, int pos, int i, int j, double score, double prio) {
+    const uint32_t ij = ((uint32_t)i << 16) | (uint32_t)j;
+    ws.cand_prio[out_base + pos] = prio;
+    ws.cand_score[out_base + pos] = score;
+    ws.cand_ij[out_base + pos] = ij;
+    if (sizeof(TA) == 4) {
+        const uint32_t b = __float_as_uint((float)prio);
+        const uint32_t ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+        ws.cand_key[out_base + pos] = ((unsigned long long)ord << 32) | (unsigned long long)(~ij);
+    }
+}
+
+// Publishes limb `slot` of image n: candidate count (-1 = special_k), survivors of the screen, status bits.
+__device__ __forceinline__ void publish_limb(const Workspace &ws, int n, size_t slot, int ncand, int nsurv, uint32_t flags) {
+    ws.cand_count[slot] = min(ncand, ws.capC);
+    if (ws.surv_count) ws.surv_count[slot] = nsurv;
+    if (ncand > ws.capC) flags |= kStCandOverflow;
+    if (flags) atomicOr(&ws.status[n], flags);
+}
+
 // largest float32 <= t: for float32-stored values v, (double)v > t  <=>  v > screen_threshold(t) -- lets the float32
 // screen apply the float64 comparison of SPG_F32_AS_F64 exactly
 __host__ __device__ inline float f32_not_above(double t) {
@@ -262,23 +321,16 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
     unsigned char *s_ain = reinterpret_cast<unsigned char *>(s_fby + capP);  // end point inside the map
     unsigned char *s_bin = s_ain + capP;
     const size_t peaks_bytes = ((size_t)capP * (4 * sizeof(double) + 6 * sizeof(float) + 2) + 15) & ~(size_t)15;
-    // per-m tables: reciprocals (phase B), screen sample positions, 64/(m-1), #samples, maxfail
-    const size_t tables_bytes = ((size_t)(kScreenMaxMid + 1) * (sizeof(double) + (kScreenSamples + 1) * sizeof(float) + 2) + 15) & ~(size_t)15;
-    double *s_rcp = reinterpret_cast<double *>(after + peaks_bytes);
-    float *s_ts = reinterpret_cast<float *>(s_rcp + (kScreenMaxMid + 1));          // [m][kScreenSamples]
-    float *s_inv64 = s_ts + (size_t)(kScreenMaxMid + 1) * kScreenSamples;           // [m]
-    signed char *s_maxfail = reinterpret_cast<signed char *>(s_inv64 + (kScreenMaxMid + 1));
-    unsigned char *s_qn = reinterpret_cast<unsigned char *>(s_maxfail + (kScreenMaxMid + 1));
-    uint32_t *s_mask = reinterpret_cast<uint32_t *>(after + peaks_bytes + tables_bytes);  // survivor bitmask, bit p = i*nB + j
+    double *s_rcp = reinterpret_cast<double *>(after + peaks_bytes);  // per-m tables (build_screen_row)
+    ScreenTab *s_tab = reinterpret_cast<ScreenTab *>(s_rcp + (kScreenMaxMid + 1));
+    float *s_ts = reinterpret_cast<float *>(s_tab + (kScreenMaxMid + 1));
+    uint32_t *s_mask = reinterpret_cast<uint32_t *>(after + peaks_bytes + screen_tables_bytes());  // survivor bitmask, bit p = i*nB + j
     const int npairs = nA * nB;
     const int nwords = (npairs + 31) >> 5;
     uint16_t *s_prefix = reinterpret_cast<uint16_t *>(s_mask + (((size_t)capP * capP + 31) >> 5));
 
     // end-point lists (refined float coordinates + peak scores), overlapped with the plane copy
     const size_t baseA = ((size_t)n * ws.K + pa) * capP, baseB = ((size_t)n * ws.K + pb) * capP;
-    auto inside = [&](double x, double y) {
-        return x >= 0.0 && x <= (double)(W - 1) && y >= 0.0 && y <= (double)(H - 1);
-    };
     // warp-specialised prologue: warp 0 stages the A list, warp 1 the B list, warps 2-3 build the per-m tables;
     // the other warps go straight to the barrier (the prologue is pure issue overhead for them)
     const bool screen = a.screen && a.mid_num <= kScreenMaxMid && H <= kScreenMaxDim && W <= kScreenMaxDim;
@@ -288,7 +340,7 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
             s_ax[i] = x; s_ay[i] = y;
             s_fax[i] = (float)(x * 64.0); s_fay[i] = (float)(y * 64.0);  // 1/64-px units for the screen
             s_as[i] = ws.peak_score[baseA + i];
-            s_ain[i] = inside(x, y);
+            s_ain[i] = inside_map(x, y, H, W);
         }
     } else if (warp == 1) {
         for (int j = lane; j < nB; j += 32) {
@@ -296,25 +348,11 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
             s_bx[j] = x; s_by[j] = y;
             s_fbx[j] = (float)(x * 64.0); s_fby[j] = (float)(y * 64.0);
             s_bs[j] = ws.peak_score[baseB + j];
-            s_bin[j] = inside(x, y);
+            s_bin[j] = inside_map(x, y, H, W);
         }
     } else if (warp < 4) {
         const int m = tid - 64;
-        if (m <= a.mid_num && m <= kScreenMaxMid) {
-            // fewest samples that must exceed thre2: smallest integer >= connect_ration*m in f64, as :246 compares
-            const double need = __dmul_rn(a.connect_ration, (double)m);
-            int need_i = (int)need;
-            if ((double)need_i < need || (a.crit1_strict && (double)need_i == need)) need_i++;  // strict: smallest integer > need
-            s_maxfail[m] = (signed char)max(min(m - need_i, 127), -1);
-            s_rcp[m] = m > 0 ? __ddiv_rn(1.0, (double)m) : 0.0;
-            s_inv64[m] = m > 1 ? 1.0f / (float)(m - 1) : 0.0f;
-            // screen positions: up to kScreenSamples sample indices spread over the interior [m/8, m-1-m/8]
-            const int lo = m / 8, hi = m - 1 - lo;
-            const int qn = max(0, min(kScreenSamples, hi - lo + 1));
-            s_qn[m] = (unsigned char)qn;
-            for (int q = 0; q < kScreenSamples; q++)
-                s_ts[m * kScreenSamples + q] = (float)(qn > 1 ? lo + (q * (hi - lo)) / (qn - 1) : lo);
-        }
+        if (m <= a.mid_num && m <= kScreenMaxMid) build_screen_row(a, m, s_rcp, s_tab, s_ts);
         if (tid == 64 + 63) s_magic = nB > 1 ? 0xffffffffu / (uint32_t)nB + 1u : 0u;  // ceil(2^32 / nB)
     }
     __syncthreads();
@@ -347,9 +385,10 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
                         if (!longp && !(fabsf(q - r) < 0.49f)) m = -1;  // m within 0.01 of a rounding tie -> survive
                         asm volatile("" : "+r"(m));  // keep ONE copy of the sample loop (no specialisation on m == mid_num)
                         if (m >= 1) {
-                            const int maxfail = s_maxfail[m];
-                            const int qn = s_qn[m];
-                            const float inv = s_inv64[m];
+                            const ScreenTab tb = s_tab[m];
+                            const int maxfail = tb.maxfail;
+                            const int qn = tb.qn;
+                            const float inv = tb.inv;
                             const float sx64 = dx64 * inv, sy64 = dy64 * inv;
                             const float *ts = s_ts + m * kScreenSamples;
                             int fails = 0;
@@ -413,28 +452,11 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
         if (bad) atomicOr(&s_flags, kStSampleIndex);
         if (ok) {
             const int pos = atomicAdd(&s_count, 1);  // warp-aggregated by ptxas (REDUX + one ATOMS)
-            if (pos < ws.capC) {
-                ws.cand_prio[out_base + pos] = prio;
-                ws.cand_score[out_base + pos] = score;
-                const uint32_t ij = ((uint32_t)i << 16) | (uint32_t)j;
-                ws.cand_ij[out_base + pos] = ij;
-                if (sizeof(TA) == 4) {  // the priority is an f32 value: 32 order-preserving bits + the tie-break fit one word
-                    const uint32_t b = __float_as_uint((float)prio);
-                    const uint32_t ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-                    ws.cand_key[out_base + pos] = ((unsigned long long)ord << 32) | (unsigned long long)(~ij);
-                }
-            }
+            if (pos < ws.capC) store_candidate<TA>(ws, out_base, pos, i, j, score, prio);
         }
     }
     __syncthreads();
-    if (tid == 0) {
-        const int total = s_count;
-        ws.cand_count[slot] = min(total, ws.capC);
-        if (ws.surv_count) ws.surv_count[slot] = total_surv;
-        uint32_t f = s_flags;
-        if (total > ws.capC) f |= kStCandOverflow;
-        if (f) atomicOr(&ws.status[n], f);
-    }
+    if (tid == 0) publish_limb(ws, n, slot, s_count, total_surv, s_flags);
 }
 
 }  // namespace spg

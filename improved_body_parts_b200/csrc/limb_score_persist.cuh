@@ -31,12 +31,6 @@
 
 namespace spg {
 
-#ifdef SPG_DEBUG
-#define SPG_DBG(x) (x)
-#else
-#define SPG_DBG(x) false
-#endif
-
 constexpr int kPersistThreads = 1024;
 constexpr int kPersistSlots = 3;   // plane ring
 constexpr int kMetaSlots = 5;      // end-point lists + survivor list + counters ring
@@ -69,28 +63,10 @@ struct alignas(16) MetaSlot {
     uint32_t flags;
 };
 
-// per-m constants of the screen (m = number of samples the reference would take for the pair)
-struct alignas(8) ScreenTab {
-    float inv;            // 1 / (m - 1)
-    signed char maxfail;  // failures the connect_ration criterion tolerates
-    unsigned char qn;     // interior samples the screen looks at
-    unsigned char pad[2];
-};
-
-__host__ __device__ inline size_t persist_tables_bytes() {
-    return (((size_t)(kScreenMaxMid + 1) * (sizeof(double) + kScreenSamples * sizeof(float) + sizeof(ScreenTab))) + 15) &
-           ~(size_t)15;
-}
-constexpr size_t kPersistPlaneOffset =
-    ((((size_t)(kScreenMaxMid + 1) * (sizeof(double) + kScreenSamples * sizeof(float) + sizeof(ScreenTab)) + 15) & ~(size_t)15) +
-     kMetaSlots * sizeof(MetaSlot) + 127) & ~(size_t)127;
+constexpr size_t kPersistPlaneOffset = (screen_tables_bytes() + kMetaSlots * sizeof(MetaSlot) + 127) & ~(size_t)127;
 inline size_t persist_smem_bytes(size_t plane_bytes, int /*capP*/) {
     const size_t plane = (plane_bytes + 127) & ~(size_t)127;
     return kPersistPlaneOffset + kPersistSlots * plane + 128;
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 constexpr uint32_t kScreenBias = 0x4B400000u >> 6;
@@ -187,7 +163,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
     double *s_rcp = reinterpret_cast<double *>(smem_raw);
     ScreenTab *s_tab = reinterpret_cast<ScreenTab *>(s_rcp + (kScreenMaxMid + 1));
     float *s_ts = reinterpret_cast<float *>(s_tab + (kScreenMaxMid + 1));
-    MetaSlot *s_meta = reinterpret_cast<MetaSlot *>(smem_raw + persist_tables_bytes());
+    MetaSlot *s_meta = reinterpret_cast<MetaSlot *>(smem_raw + screen_tables_bytes());
     unsigned char *s_planes = smem_raw + kPersistPlaneOffset;
     const int nE = min(max(a.exact_warps, 1), kWorkerWarps - 1), nS = kWorkerWarps - nE;  // scorer / screener warps
 
@@ -204,24 +180,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         s_bias_bytes = 4u * kScreenBias * (uint32_t)(W + 1);
         fence_mbar_init();
     }
-    if (tid >= 32 && tid < 32 + kScreenMaxMid + 1) {
-        const int m = tid - 32;
-        const double need = __dmul_rn(a.connect_ration, (double)m);  // :246 compares in f64
-        int need_i = (int)need;
-        if ((double)need_i < need || (a.crit1_strict && (double)need_i == need)) need_i++;  // strict: smallest integer > need
-        s_rcp[m] = m > 0 ? __ddiv_rn(1.0, (double)m) : 0.0;
-        // up to kScreenSamples samples spread over the interior [lo, hi] (the ends sit on the peaks and rarely fail)
-        const int lo = m / 8, hi = m - 1 - lo;
-        const int qn = max(0, min(kScreenSamples, hi - lo + 1));
-        for (int q = 0; q < kScreenSamples; q++)  // tail clamped: every entry is a valid sample index
-            s_ts[m * kScreenSamples + q] = (float)(qn > 1 ? lo + (min(q, qn - 1) * (hi - lo)) / (qn - 1) : lo);
-        ScreenTab t;
-        t.inv = m > 1 ? 1.0f / (float)(m - 1) : 0.0f;
-        t.maxfail = (signed char)max(min(m - need_i, 127), -1);
-        t.qn = (unsigned char)qn;
-        t.pad[0] = t.pad[1] = 0;
-        s_tab[m] = t;
-    }
+    if (tid >= 32 && tid < 32 + kScreenMaxMid + 1) build_screen_row(a, tid - 32, s_rcp, s_tab, s_ts);
     __syncthreads();
 
     const int G = gridDim.x;
@@ -261,13 +220,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         auto close_item = [&](int jp) {
             if (lane == 0) {
                 MetaSlot &ms = s_meta[jp % kMetaSlots];
-                const size_t slot = (size_t)ms.hdr.n * L + ms.hdr.k;
-                const int total = ms.ncand;
-                ws.cand_count[slot] = ms.hdr.special ? -1 : min(total, ws.capC);
-                if (ws.surv_count) ws.surv_count[slot] = ms.nsurv;
-                uint32_t f = ms.flags;
-                if (total > ws.capC) f |= kStCandOverflow;
-                if (f) atomicOr(&ws.status[ms.hdr.n], f);
+                publish_limb(ws, ms.hdr.n, (size_t)ms.hdr.n * L + ms.hdr.k, ms.hdr.special ? -1 : ms.ncand, ms.nsurv, ms.flags);
                 ms.nsurv = 0; ms.ncand = 0; ms.bnext = 0; ms.flags = 0;
             }
             __syncwarp();
@@ -304,8 +257,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                     const double xa = r_xa[u], ya = r_ya[u], xb = r_xb[u], yb = r_yb[u];
                     ps.ax[q] = xa; ps.ay[q] = ya; ps.bx[q] = xb; ps.by[q] = yb;
                     ps.as[q] = r_sa[u]; ps.bs[q] = r_sb[u];
-                    const bool ain = xa >= 0.0 && xa <= (double)(W - 1) && ya >= 0.0 && ya <= (double)(H - 1);
-                    const bool bin = xb >= 0.0 && xb <= (double)(W - 1) && yb >= 0.0 && yb <= (double)(H - 1);
+                    const bool ain = inside_map(xa, ya, H, W), bin = inside_map(xb, yb, H, W);
                     ps.fa[q] = ain ? make_float2((float)(xa * 64.0), (float)(ya * 64.0)) : make_float2(-1.0f, 0.0f);
                     ps.fb[q] = bin ? make_float2((float)(xb * 64.0), (float)(yb * 64.0)) : make_float2(-1.0f, 0.0f);
                     ps.ain[q] = ain;
@@ -316,7 +268,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             const bool special = nA == 0 || nB == 0;
             if (lane == 0) {
                 PersistHdr h;
-                h.nA = nA; h.nB = nB; h.npairs = (special || SPG_DBG(a.debug == 1)) ? 0 : nA * nB; h.n = n; h.k = k; h.special = special;
+                h.nA = nA; h.nB = nB; h.npairs = special ? 0 : nA * nB; h.n = n; h.k = k; h.special = special;
                 h.magic = nB > 1 ? 0xffffffffu / (uint32_t)nB + 1u : 0u;
                 h.pad = 0;
                 ms.hdr = h;
@@ -346,17 +298,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             if (ok) {
                 const size_t out_base = ((size_t)h.n * L + h.k) * ws.capC;
                 const int pos = atomicAdd(&ms.ncand, 1);
-                if (pos < ws.capC) {
-                    const uint32_t ij = ((uint32_t)i << 16) | (uint32_t)jj;
-                    ws.cand_prio[out_base + pos] = prio;
-                    ws.cand_score[out_base + pos] = score;
-                    ws.cand_ij[out_base + pos] = ij;
-                    if (sizeof(TA) == 4) {  // one-word sort key: only an f32 priority fits
-                        const uint32_t b = __float_as_uint((float)prio);
-                        const uint32_t ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-                        ws.cand_key[out_base + pos] = ((unsigned long long)ord << 32) | (unsigned long long)(~ij);
-                    }
-                }
+                if (pos < ws.capC) store_candidate<TA>(ws, out_base, pos, i, jj, score, prio);
             }
         };
 
@@ -409,7 +351,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                 const int e = j % kMetaSlots;
                 mbar_wait_sleep(&bar_screened[e], (j / kMetaSlots) & 1);  // every screener has left item j: the list is complete
                 MetaSlot &ms = s_meta[e];
-                const int ns = SPG_DBG(a.debug == 2) ? 0 : min(ms.nsurv, kPersistListCap);
+                const int ns = min(ms.nsurv, kPersistListCap);
                 if (ns > 0) {
                     const T *gplane = plane_of(ms.hdr.n - a.image_base, ms.hdr.k);  // the plane's slot may already hold another item
                     for (;;) {

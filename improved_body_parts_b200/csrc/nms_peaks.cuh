@@ -9,6 +9,9 @@
 // float4 groups and rejects a group with one compare when none of its 4 values reaches thre1 (the
 // common case).  Peaks are appended unordered and then rank-sorted by raster index, which restores
 // np.nonzero's order exactly (peak ids depend on it).  Refinement re-reads the 5x5 box from L2.
+//
+// This header also holds the building blocks of the two persistent forms (nms_peaks_persist.cuh,
+// nms_peaks_banded.cuh): the 8-neighbour test, the peak finisher, the scanners' pass 1 and their role constants.
 #pragma once
 
 #include "common.cuh"
@@ -91,6 +94,124 @@ __device__ __forceinline__ void refine_box(const float *__restrict__ plane, int 
     sc = __fdiv_rn(s32, (float)N);  // score_box.mean() stays f32
 }
 
+// The 8-neighbour test of one float4 group (row y, columns x0 .. x0 + 3), with neighbours clamped to the image: a clamped
+// neighbour is a pixel that is already inside the clipped 3x3 window (or the pixel itself), so the window max is
+// unchanged.  `rows` is addressed by GLOBAL row index.  Peaks are appended to `list` (unordered) through `*cnt`.
+__device__ __forceinline__ void nms_test_group(const float *rows, int y, int x0, int H, int W, float thr, int *cnt, uint32_t *list, int capP) {
+    const float *rc = rows + (size_t)y * W;
+    const float *ru = rows + (size_t)max(y - 1, 0) * W;
+    const float *rd = rows + (size_t)min(y + 1, H - 1) * W;
+    const float4 c4 = *reinterpret_cast<const float4 *>(rc + x0);
+    const float4 u4 = *reinterpret_cast<const float4 *>(ru + x0);
+    const float4 d4 = *reinterpret_cast<const float4 *>(rd + x0);
+    const int xl = max(x0 - 1, 0), xr = min(x0 + 4, W - 1);
+    const float U[6] = {ru[xl], u4.x, u4.y, u4.z, u4.w, ru[xr]};
+    const float C[6] = {rc[xl], c4.x, c4.y, c4.z, c4.w, rc[xr]};
+    const float D[6] = {rd[xl], d4.x, d4.y, d4.z, d4.w, rd[xr]};
+#pragma unroll
+    for (int e = 0; e < 4; e++) {
+        const float v = C[e + 1];
+        // keep = (hmax == heat) & (heat >= thre) (util.py:182); np.nonzero(heat * keep) drops exact zeros.
+        // "all neighbours <= v" (not fmax) so that a NaN neighbour vetoes the peak like torch's max-pool
+        const bool pk = (v >= thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
+                        (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v);
+        if (pk) {
+            const int pos = atomicAdd(cnt, 1);
+            if (pos < capP) list[pos] = (uint32_t)(y * W + x0 + e);
+        }
+    }
+}
+
+// Finishes one peak at raster index `lin` of `plane`: the border test, the refinement (util.py:201-211, from L2) and the
+// four stores at output slot `out`.
+__device__ __forceinline__ void nms_finish_peak(const NmsArgs &a, const float *plane, int H, int W, size_t out, int lin) {
+    const Workspace &ws = a.ws;
+    const int R = a.radius;
+    const int y = lin / W, x = lin - y * W;
+    double rx, ry;
+    float sc;
+    uint32_t anchor = ((uint32_t)y << 16) | (uint32_t)x;
+    if (y + R + 1 > H || y - R < 0 || x + R + 1 > W || x - R < 0) {
+        rx = (double)x;  // util.py:201-202: the box leaves the image -> integer anchor, raw map value
+        ry = (double)y;
+        sc = plane[(size_t)y * W + x];
+        anchor |= 0x80000000u;
+    } else {
+        switch (R) {  // util.py:204-211
+            case 0: refine_box<0>(plane, W, x, y, rx, ry, sc); break;
+            case 1: refine_box<1>(plane, W, x, y, rx, ry, sc); break;
+            case 2: refine_box<2>(plane, W, x, y, rx, ry, sc); break;
+            case 3: refine_box<3>(plane, W, x, y, rx, ry, sc); break;
+            default: refine_box<4>(plane, W, x, y, rx, ry, sc); break;
+        }
+    }
+    ws.peak_x[out] = rx;
+    ws.peak_y[out] = ry;
+    ws.peak_score[out] = sc;
+    ws.peak_anchor[out] = anchor;
+}
+
+// Publishes the peak count of plane (image n, part c).
+__device__ __forceinline__ void nms_publish_count(const NmsArgs &a, int n, int c, int total) {
+    a.ws.peak_count[(size_t)n * a.ws.K + c] = total;
+    if (total > a.ws.capP) atomicOr(&a.ws.status[n], kStPeakOverflow);
+}
+
+// ---- the persistent forms (nms_peaks_persist.cuh, nms_peaks_banded.cuh): one resident 1024-thread CTA per SM with the
+// same roles -- a loader warp, scanner warps, finisher warps -- and a ring of peak lists between scanners and finishers
+constexpr int kNmsPThreads = 1024;
+constexpr int kNmsPFinishers = 3;
+constexpr int kNmsPLists = 2 * kNmsPFinishers;
+constexpr int kNmsPScanners = kNmsPThreads / 32 - 1 - kNmsPFinishers;  // 28
+constexpr int kNmsPMaxIter = 5;  // 32-lane passes of pass 1 over a scanner's share of a plane or band
+
+// Pass 1 of a persistent scanner: the float4 groups g = g0 + it * g_step + lane (it < ITER, g < g_end) of `data` that
+// reach thre1 are queued in `wq`, warp-aggregated, in group order.  First only the votes (one load, three max, one
+// compare, one ballot per 128 elements -- the common case is an empty mask), then the queue from the masks.  Returns the
+// queue length (warp-uniform); the queue is visible to the whole warp.
+template <int ITER>
+__device__ __forceinline__ int nms_queue_groups(const float *data, int g0, int g_step, int g_end, float thr, int lane, uint16_t *wq) {
+    uint32_t am[ITER];
+#pragma unroll
+    for (int it = 0; it < ITER; it++) {
+        const int g = g0 + it * g_step + lane;
+        bool act = false;
+        if (g < g_end) {
+            const float4 c4 = *reinterpret_cast<const float4 *>(data + 4 * (size_t)g);
+            act = fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= thr;
+        }
+        am[it] = __ballot_sync(0xffffffffu, act);
+    }
+    int nq = 0;
+#pragma unroll
+    for (int it = 0; it < ITER; it++) {
+        const uint32_t m = am[it];
+        if (m) {  // warp-uniform
+            if ((m >> lane) & 1u) wq[nq + __popc(m & ((1u << lane) - 1u))] = (uint16_t)(g0 + it * g_step + lane);
+            nq += __popc(m);
+        }
+    }
+    __syncwarp();
+    return nq;
+}
+
+// A persistent finisher's share of plane `item` (= n_local * K + c): lane t takes peaks t, t + 32, ... of the unordered
+// list, ranks each by raster index (= np.nonzero order, evaluate.py:193; indices are unique) and finishes it at its rank.
+__device__ __forceinline__ void nms_finish_plane(const NmsArgs &a, const uint32_t *list, int total, int item, int lane) {
+    const int K = a.ws.K, capP = a.ws.capP;
+    const int n_local = item / K, c = item - n_local * K;
+    const float *plane = a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;  // L2-hot
+    const int np = min(total, capP);
+    const size_t out_base = ((size_t)(a.image_base + n_local) * K + c) * capP;
+    for (int t = lane; t < np; t += 32) {
+        const uint32_t mine = list[t];
+        int rank = 0;
+        for (int u = 0; u < np; u++) rank += list[u] < mine;
+        nms_finish_peak(a, plane, a.H, a.W, out_base + rank, (int)mine);
+    }
+    if (lane == 0) nms_publish_count(a, a.image_base + n_local, c, total);
+}
+
 __global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t bar[kNmsBufs];
@@ -171,34 +292,11 @@ __global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
                 nq += __popc(am);
             }
             __syncwarp();
-            // Neighbour rows/columns are CLAMPED to the image: a clamped neighbour is a pixel that is already
-            // inside the clipped 3x3 window (or the pixel itself), so the window max is unchanged.
+            const float *rows = buf - (size_t)lo * W;  // addressed by global row index
             for (int q = lane; q < nq; q += 32) {
                 const int g = wq[q];
                 const int r = g / W4, xq = g - r * W4;
-                const int y = y0 + r, x0 = 4 * xq;
-                const float *rc = buf + (size_t)(y - lo) * W;
-                const float *ru = buf + (size_t)(max(y - 1, 0) - lo) * W;
-                const float *rd = buf + (size_t)(min(y + 1, H - 1) - lo) * W;
-                const float4 c4 = *reinterpret_cast<const float4 *>(rc + x0);
-                const float4 u4 = *reinterpret_cast<const float4 *>(ru + x0);
-                const float4 d4 = *reinterpret_cast<const float4 *>(rd + x0);
-                const int xl = max(x0 - 1, 0), xr = min(x0 + 4, W - 1);
-                const float U[6] = {ru[xl], u4.x, u4.y, u4.z, u4.w, ru[xr]};
-                const float C[6] = {rc[xl], c4.x, c4.y, c4.z, c4.w, rc[xr]};
-                const float D[6] = {rd[xl], d4.x, d4.y, d4.z, d4.w, rd[xr]};
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const float v = C[e + 1];
-                    // keep = (hmax == heat) & (heat >= thre); np.nonzero(heat * keep) drops exact zeros.
-                    // "all neighbours <= v" (not fmax) so that a NaN neighbour vetoes the peak like torch's max-pool
-                    const bool pk = (v >= a.thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
-                                    (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v);
-                    if (pk) {
-                        const int pos = atomicAdd(&s_count, 1);
-                        if (pos < ws.capP) s_list[pos] = (uint32_t)(y * W + x0 + e);
-                    }
-                }
+                nms_test_group(rows, y0 + r, 4 * xq, H, W, a.thr, &s_count, s_list, ws.capP);
             }
         } else {
             const int cnt = (y1 - y0) * W;
@@ -226,40 +324,9 @@ __global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
         s_sorted[rank] = mine;
     }
     __syncthreads();
-
     const size_t out_base = ((size_t)n * ws.K + c) * ws.capP;
-    const int R = a.radius;
-    for (int t = tid; t < np; t += kNmsThreads) {
-        const int lin = (int)s_sorted[t];
-        const int y = lin / W, x = lin - y * W;
-        double rx, ry;
-        float sc;
-        uint32_t anchor = ((uint32_t)y << 16) | (uint32_t)x;
-        if (y + R + 1 > H || y - R < 0 || x + R + 1 > W || x - R < 0) {
-            // util.py:201-202: the box leaves the image -> integer anchor, raw map value
-            rx = (double)x;
-            ry = (double)y;
-            sc = plane[(size_t)y * W + x];
-            anchor |= 0x80000000u;
-        } else {
-            // util.py:204-211
-            switch (R) {
-                case 0: refine_box<0>(plane, W, x, y, rx, ry, sc); break;
-                case 1: refine_box<1>(plane, W, x, y, rx, ry, sc); break;
-                case 2: refine_box<2>(plane, W, x, y, rx, ry, sc); break;
-                case 3: refine_box<3>(plane, W, x, y, rx, ry, sc); break;
-                default: refine_box<4>(plane, W, x, y, rx, ry, sc); break;
-            }
-        }
-        ws.peak_x[out_base + t] = rx;
-        ws.peak_y[out_base + t] = ry;
-        ws.peak_score[out_base + t] = sc;
-        ws.peak_anchor[out_base + t] = anchor;
-    }
-    if (tid == 0) {
-        ws.peak_count[(size_t)n * ws.K + c] = total;
-        if (total > ws.capP) atomicOr(&ws.status[n], kStPeakOverflow);
-    }
+    for (int t = tid; t < np; t += kNmsThreads) nms_finish_peak(a, plane, H, W, out_base + t, (int)s_sorted[t]);
+    if (tid == 0) nms_publish_count(a, n, c, total);
 }
 
 inline size_t nms_smem_bytes(int band_rows, int H, int W, int capP) {

@@ -23,13 +23,9 @@
 
 namespace spg {
 
-constexpr int kNmsBThreads = 1024;
+// the role constants (kNmsP*) are in nms_peaks.cuh; a band is <= (warps per team) * 32 * kNmsPMaxIter float4 groups
 constexpr int kNmsBMaxSlots = 16;
-constexpr int kNmsBFinishers = 3;
-constexpr int kNmsBLists = 2 * kNmsBFinishers;
-constexpr int kNmsBScanners = kNmsBThreads / 32 - 1 - kNmsBFinishers;  // 28
 constexpr int kNmsBTeams = 4;            // banded form: scanner teams of 7 warps, team g scans the bands t = g, g + 4, ... of the CTA's sequence
-constexpr int kNmsBMaxIter = 5;          // 32-lane passes of a scanner over its share of a band: a band is <= (warps per team) * 32 * 5 float4 groups
 constexpr int kNmsBBandGroups = 1024;    // banded form: target band size in float4 groups (16 KB)
 
 struct NmsBanding {
@@ -40,12 +36,12 @@ struct NmsBanding {
 inline NmsBanding nms_banding(int H, int W, int capP, size_t smem_limit) {
     NmsBanding g{};
     const int W4 = W / 4;
-    const size_t fixed = kNmsBLists * (size_t)capP * sizeof(uint32_t) + (size_t)kNmsBScanners * 32 * kNmsBMaxIter * sizeof(uint16_t) + 64;  // lists + per-warp queues
+    const size_t fixed = kNmsPLists * (size_t)capP * sizeof(uint32_t) + (size_t)kNmsPScanners * 32 * kNmsPMaxIter * sizeof(uint16_t) + 64;  // lists + per-warp queues
     if (smem_limit <= fixed) return g;
     g.teams = kNmsBTeams;
-    const int team_warps = kNmsBScanners / kNmsBTeams;
+    const int team_warps = kNmsPScanners / kNmsBTeams;
     g.band_rows = std::max(1, std::min(H, kNmsBBandGroups / std::max(W4, 1)));
-    if ((size_t)g.band_rows * W4 > (size_t)team_warps * 32 * kNmsBMaxIter) return g;  // a single row wider than a team's reach
+    if ((size_t)g.band_rows * W4 > (size_t)team_warps * 32 * kNmsPMaxIter) return g;  // a single row wider than a team's reach
     g.n_bands = (H + g.band_rows - 1) / g.band_rows;
     g.band_stride = (((size_t)std::min(g.band_rows + 2, H) * W * sizeof(float)) + 127) & ~(size_t)127;
     // a multiple of the team count: band t and band t - slots (same slot) then belong to the same team, which consumes its
@@ -56,85 +52,19 @@ inline NmsBanding nms_banding(int H, int W, int capP, size_t smem_limit) {
     return g;
 }
 
-// pass 2 for one queued float4 group (row y, columns x0 .. x0 + 3): the 8-neighbour test with neighbours clamped to the
-// image (== window clipped to the image); `rows` is addressed by GLOBAL row index.  Peaks go to the plane's list.
-__device__ __forceinline__ void nms_test_group(const float *rows, int y, int x0, int H, int W, float thr, int *cnt, uint32_t *list, int capP) {
-    const float *rc = rows + (size_t)y * W;
-    const float *ru = rows + (size_t)max(y - 1, 0) * W;
-    const float *rd = rows + (size_t)min(y + 1, H - 1) * W;
-    const float4 c4 = *reinterpret_cast<const float4 *>(rc + x0);
-    const float4 u4 = *reinterpret_cast<const float4 *>(ru + x0);
-    const float4 d4 = *reinterpret_cast<const float4 *>(rd + x0);
-    const int xl = max(x0 - 1, 0), xr = min(x0 + 4, W - 1);
-    const float U[6] = {ru[xl], u4.x, u4.y, u4.z, u4.w, ru[xr]};
-    const float C[6] = {rc[xl], c4.x, c4.y, c4.z, c4.w, rc[xr]};
-    const float D[6] = {rd[xl], d4.x, d4.y, d4.z, d4.w, rd[xr]};
-#pragma unroll
-    for (int e = 0; e < 4; e++) {
-        const float v = C[e + 1];
-        // keep = (hmax == heat) & (heat >= thre) (util.py:182); np.nonzero(heat * keep) drops exact zeros
-        const bool pk = (v >= thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
-                        (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v);
-        if (pk) {
-            const int pos = atomicAdd(cnt, 1);
-            if (pos < capP) list[pos] = (uint32_t)(y * W + x0 + e);
-        }
-    }
-}
-
-// The finisher's share of one plane: rank the list by raster index (= np.nonzero order, evaluate.py:193), refine every peak
-// from L2 (util.py:201-211) and write the plane's outputs.  Returns nothing; the caller publishes the count.
-__device__ __forceinline__ void nms_finish_plane(const NmsArgs &a, const uint32_t *list, int total, int item, int lane) {
-    const Workspace &ws = a.ws;
-    const int H = a.H, W = a.W, K = ws.K, capP = ws.capP, R = a.radius;
-    const int n_local = item / K, c = item - n_local * K;
-    const int n = a.image_base + n_local;
-    const float *plane = a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;  // L2-hot
-    const int np = min(total, capP);
-    const size_t out_base = ((size_t)n * K + c) * capP;
-    for (int t = lane; t < np; t += 32) {
-        const uint32_t mine = list[t];
-        int rank = 0;  // raster index rank == np.nonzero order (evaluate.py:193); indices are unique
-        for (int u = 0; u < np; u++) rank += list[u] < mine;
-        const int lin = (int)mine;
-        const int y = lin / W, x = lin - y * W;
-        double rx, ry;
-        float sc;
-        uint32_t anchor = ((uint32_t)y << 16) | (uint32_t)x;
-        if (y + R + 1 > H || y - R < 0 || x + R + 1 > W || x - R < 0) {
-            rx = (double)x;  // util.py:201-202: the box leaves the image -> integer anchor, raw map value
-            ry = (double)y;
-            sc = plane[(size_t)y * W + x];
-            anchor |= 0x80000000u;
-        } else {
-            switch (R) {  // util.py:204-211
-                case 0: refine_box<0>(plane, W, x, y, rx, ry, sc); break;
-                case 1: refine_box<1>(plane, W, x, y, rx, ry, sc); break;
-                case 2: refine_box<2>(plane, W, x, y, rx, ry, sc); break;
-                case 3: refine_box<3>(plane, W, x, y, rx, ry, sc); break;
-                default: refine_box<4>(plane, W, x, y, rx, ry, sc); break;
-            }
-        }
-        ws.peak_x[out_base + rank] = rx;
-        ws.peak_y[out_base + rank] = ry;
-        ws.peak_score[out_base + rank] = sc;
-        ws.peak_anchor[out_base + rank] = anchor;
-    }
-}
-
-__global__ void __launch_bounds__(kNmsBThreads, 1) nms_peaks_banded_kernel(NmsArgs a, int n_items, int n_slots, int n_bands) {
+__global__ void __launch_bounds__(kNmsPThreads, 1) nms_peaks_banded_kernel(NmsArgs a, int n_items, int n_slots, int n_bands) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t bar_full[kNmsBMaxSlots], bar_free[kNmsBMaxSlots], bar_ready[kNmsBLists], bar_lfree[kNmsBLists];
-    __shared__ int s_cnt[kNmsBLists];
+    __shared__ uint64_t bar_full[kNmsBMaxSlots], bar_free[kNmsBMaxSlots], bar_ready[kNmsPLists], bar_lfree[kNmsPLists];
+    __shared__ int s_cnt[kNmsPLists];
 
     const Workspace &ws = a.ws;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int H = a.H, W = a.W, K = ws.K, capP = ws.capP;
     const int BR = a.band_rows, S = n_slots, NB = n_bands;
-    constexpr int T = kNmsBTeams, TW = kNmsBScanners / kNmsBTeams;  // teams, warps per team
+    constexpr int T = kNmsBTeams, TW = kNmsPScanners / kNmsBTeams;  // teams, warps per team
     const size_t band_stride = (((size_t)min(BR + 2, H) * W * sizeof(float)) + 127) & ~(size_t)127;
     uint32_t *s_lists = reinterpret_cast<uint32_t *>(smem_raw + (size_t)S * band_stride);  // [lists][capP]
-    uint16_t *s_queues = reinterpret_cast<uint16_t *>(s_lists + kNmsBLists * (size_t)capP);
+    uint16_t *s_queues = reinterpret_cast<uint16_t *>(s_lists + kNmsPLists * (size_t)capP);
     const int W4 = W >> 2;
     // g / W4 without a division: g < 2^16 here (a band's group count), so umulhi(g, ceil(2^32 / W4)) is exact
     const uint32_t w4_magic = W4 > 1 ? 0xffffffffu / (uint32_t)W4 + 1u : 0u;
@@ -144,8 +74,8 @@ __global__ void __launch_bounds__(kNmsBThreads, 1) nms_peaks_banded_kernel(NmsAr
             mbar_init(&bar_full[s], 1);
             mbar_init(&bar_free[s], TW);
         }
-        for (int l = 0; l < kNmsBLists; l++) {
-            mbar_init(&bar_ready[l], kNmsBScanners);
+        for (int l = 0; l < kNmsPLists; l++) {
+            mbar_init(&bar_ready[l], kNmsPScanners);
             mbar_init(&bar_lfree[l], 1);
             s_cnt[l] = 0;
         }
@@ -174,18 +104,18 @@ __global__ void __launch_bounds__(kNmsBThreads, 1) nms_peaks_banded_kernel(NmsAr
                 }
             }
         }
-    } else if (warp <= kNmsBScanners) {
+    } else if (warp <= kNmsPScanners) {
         // =========================== scanners ===========================
         // Four teams of seven warps; team g takes the bands t = g, g + 4, ... of the CTA's band sequence, so a warp pays the per-band costs (two
         // barrier operations, the queue set-up) once per ~147 float4 groups, as it did with whole planes, while the ring
         // turns over in 17 KB steps.
         const int w = warp - 1, team = w / TW, tw = w - team * TW;
-        uint16_t *wq = s_queues + (size_t)w * (32 * kNmsBMaxIter);
+        uint16_t *wq = s_queues + (size_t)w * (32 * kNmsPMaxIter);
         const float thr = a.thr;
         for (int j = 0; j < nj; j++) {
-            const int l = j % kNmsBLists;
+            const int l = j % kNmsPLists;
             uint32_t *list = s_lists + (size_t)l * capP;
-            if (j >= kNmsBLists) mbar_wait_sleep(&bar_lfree[l], ((j / kNmsBLists) - 1) & 1);
+            if (j >= kNmsPLists) mbar_wait_sleep(&bar_lfree[l], ((j / kNmsPLists) - 1) & 1);
             for (int b = (team - (j * NB) % T + T) % T; b < NB; b += T) {
                 const int t = j * NB + b, round = t / S, s = t - round * S;  // band t (t mod T == team) sits in slot t mod S
                 mbar_wait_sleep(&bar_full[s], round & 1);
@@ -193,31 +123,10 @@ __global__ void __launch_bounds__(kNmsBThreads, 1) nms_peaks_banded_kernel(NmsAr
                 const int groups = (r1 - r0) * W4;
                 // `band` points at the (virtual) start of global row 0, so rows are addressed by their global index
                 const float *band = reinterpret_cast<const float *>(smem_raw + (size_t)s * band_stride) - (size_t)lo * W;
-                // ---- pass 1: queue the float4 groups of this warp's share that reach thre1 (groups are dealt to the team's
-                // warps 32 at a time).  First only the votes (one load, three max, one compare, one ballot per 128 elements
-                // -- the common case is an empty mask), then the queue from the masks.
-                uint32_t am[kNmsBMaxIter];
-#pragma unroll
-                for (int it = 0; it < kNmsBMaxIter; it++) {
-                    const int g = (it * TW + tw) * 32 + lane;
-                    bool act = false;
-                    if (g < groups) {
-                        const float4 c4 = *reinterpret_cast<const float4 *>(band + (size_t)r0 * W + 4 * (size_t)g);
-                        act = fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= thr;
-                    }
-                    am[it] = __ballot_sync(0xffffffffu, act);
-                }
-                int nq = 0;
-#pragma unroll
-                for (int it = 0; it < kNmsBMaxIter; it++) {
-                    const uint32_t m = am[it];
-                    if (m) {  // warp-uniform
-                        if ((m >> lane) & 1u) wq[nq + __popc(m & ((1u << lane) - 1u))] = (uint16_t)((it * TW + tw) * 32 + lane);
-                        nq += __popc(m);
-                    }
-                }
-                __syncwarp();
-                // ---- pass 2: 8-neighbour test (neighbours clamped to the image == window clipped to the image)
+                // pass 1: queue the float4 groups of this warp's share that reach thre1 (groups are dealt to the team's
+                // warps 32 at a time)
+                const int nq = nms_queue_groups<kNmsPMaxIter>(band + (size_t)r0 * W, tw * 32, TW * 32, groups, thr, lane, wq);
+                // pass 2: the 8-neighbour test of the queued groups
                 for (int q = lane; q < nq; q += 32) {
                     const int g = wq[q];
                     const int yl = W4 > 1 ? (int)__umulhi((uint32_t)g, w4_magic) : g, xq = g - yl * W4;
@@ -225,27 +134,22 @@ __global__ void __launch_bounds__(kNmsBThreads, 1) nms_peaks_banded_kernel(NmsAr
                     nms_test_group(band, y, x0, H, W, thr, &s_cnt[l], list, capP);
                 }
                 __syncwarp();
-                if (lane == 0) mbar_arrive_plain(&bar_free[s]);  // the band is not needed any more
+                if (lane == 0) mbar_arrive(&bar_free[s]);  // the band is not needed any more
             }
             __syncwarp();
-            if (lane == 0) mbar_arrive_plain(&bar_ready[l]);      // this warp's peaks of the plane are in the list
+            if (lane == 0) mbar_arrive(&bar_ready[l]);      // this warp's peaks of the plane are in the list
         }
     } else {
         // =========================== finishers ===========================
-        const int f = warp - 1 - kNmsBScanners;
-        for (int j = f; j < nj; j += kNmsBFinishers) {
-            const int l = j % kNmsBLists;
-            mbar_wait_sleep(&bar_ready[l], (j / kNmsBLists) & 1);
-            const int item = (int)blockIdx.x + j * G;
-            const int n = a.image_base + item / K, c = item % K;
-            const int total = s_cnt[l];
-            nms_finish_plane(a, s_lists + (size_t)l * capP, total, item, lane);
+        const int f = warp - 1 - kNmsPScanners;
+        for (int j = f; j < nj; j += kNmsPFinishers) {
+            const int l = j % kNmsPLists;
+            mbar_wait_sleep(&bar_ready[l], (j / kNmsPLists) & 1);
+            nms_finish_plane(a, s_lists + (size_t)l * capP, s_cnt[l], (int)blockIdx.x + j * G, lane);
             __syncwarp();
             if (lane == 0) {
-                ws.peak_count[(size_t)n * K + c] = total;
-                if (total > capP) atomicOr(&ws.status[n], kStPeakOverflow);
                 s_cnt[l] = 0;
-                mbar_arrive_plain(&bar_lfree[l]);  // list + counter may be reused (plane j + kNmsBLists)
+                mbar_arrive(&bar_lfree[l]);  // list + counter may be reused (plane j + kNmsPLists)
             }
         }
     }

@@ -17,22 +17,13 @@
 
 namespace spg {
 
-constexpr int kNmsPThreads = 1024;
-constexpr int kNmsPSlots = 3;
-constexpr int kNmsPFinishers = 3;
-constexpr int kNmsPLists = 2 * kNmsPFinishers;
-constexpr int kNmsPScanners = kNmsPThreads / 32 - 1 - kNmsPFinishers;  // 28
-constexpr int kNmsPMaxIter = 5;  // 32-lane passes over a scanner's slice: 3 planes must fit in shared memory, so a slice is <= 160 float4 groups
+constexpr int kNmsPSlots = 3;  // plane ring; the role constants are in nms_peaks.cuh
 
 inline size_t nms_persist_smem_bytes(int H, int W, int capP) {
     const size_t plane = (((size_t)H * W * sizeof(float)) + 127) & ~(size_t)127;
     const size_t gpw = ((size_t)H * W / 4 + kNmsPScanners - 1) / kNmsPScanners;
     const size_t queues = ((gpw * kNmsPScanners * sizeof(uint16_t)) + 15) & ~(size_t)15;
     return kNmsPSlots * plane + kNmsPLists * (size_t)capP * sizeof(uint32_t) + queues + 64;
-}
-
-__device__ __forceinline__ void mbar_arrive_plain(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 __global__ void __launch_bounds__(kNmsPThreads, 1) nms_peaks_persist_kernel(NmsArgs a, int n_items) {
@@ -99,112 +90,31 @@ __global__ void __launch_bounds__(kNmsPThreads, 1) nms_peaks_persist_kernel(NmsA
             if (j >= kNmsPLists) mbar_wait_sleep(&bar_lfree[l], ((j / kNmsPLists) - 1) & 1);
             const float *buf = reinterpret_cast<const float *>(smem_raw + s * plane_stride);
             uint32_t *list = s_lists + (size_t)l * capP;
-            // ---- pass 1: queue the float4 groups of this warp's slice that reach thre1.  First only the votes (one
-            // load, three max, one compare, one ballot per 128 elements -- the common case is an empty mask), then the
-            // queue from the masks.
-            uint32_t am[kNmsPMaxIter];
-#pragma unroll
-            for (int it = 0; it < kNmsPMaxIter; it++) {
-                const int g = g_lo + it * 32 + lane;
-                bool act = false;
-                if (g < g_hi) {
-                    const float4 c4 = *reinterpret_cast<const float4 *>(buf + 4 * (size_t)g);
-                    act = fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= thr;
-                }
-                am[it] = __ballot_sync(0xffffffffu, act);
-            }
-            int nq = 0;
-#pragma unroll
-            for (int it = 0; it < kNmsPMaxIter; it++) {
-                const uint32_t m = am[it];
-                if (m) {  // warp-uniform
-                    if ((m >> lane) & 1u) wq[nq + __popc(m & ((1u << lane) - 1u))] = (uint16_t)(g_lo + it * 32 + lane);
-                    nq += __popc(m);
-                }
-            }
-            __syncwarp();
-            // ---- pass 2: 8-neighbour test (neighbours clamped to the image == window clipped to the image)
+            // pass 1: queue the float4 groups of this warp's slice (<= 160 groups: 3 planes fit in shared memory) that reach thre1
+            const int nq = nms_queue_groups<kNmsPMaxIter>(buf, g_lo, 32, g_hi, thr, lane, wq);
+            // pass 2: the 8-neighbour test of the queued groups
             for (int q = lane; q < nq; q += 32) {
                 const int g = wq[q];
                 const int y = W4 > 1 ? (int)__umulhi((uint32_t)g, w4_magic) : g, xq = g - y * W4;
-                const int x0 = 4 * xq;
-                const float *rc = buf + (size_t)y * W;
-                const float *ru = buf + (size_t)max(y - 1, 0) * W;
-                const float *rd = buf + (size_t)min(y + 1, H - 1) * W;
-                const float4 c4 = *reinterpret_cast<const float4 *>(rc + x0);
-                const float4 u4 = *reinterpret_cast<const float4 *>(ru + x0);
-                const float4 d4 = *reinterpret_cast<const float4 *>(rd + x0);
-                const int xl = max(x0 - 1, 0), xr = min(x0 + 4, W - 1);
-                const float U[6] = {ru[xl], u4.x, u4.y, u4.z, u4.w, ru[xr]};
-                const float C[6] = {rc[xl], c4.x, c4.y, c4.z, c4.w, rc[xr]};
-                const float D[6] = {rd[xl], d4.x, d4.y, d4.z, d4.w, rd[xr]};
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const float v = C[e + 1];
-                    // keep = (hmax == heat) & (heat >= thre) (util.py:182); np.nonzero(heat * keep) drops exact zeros
-                    const bool pk = (v >= thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
-                                    (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v);
-                    if (pk) {
-                        const int pos = atomicAdd(&s_cnt[l], 1);
-                        if (pos < capP) list[pos] = (uint32_t)(y * W + x0 + e);
-                    }
-                }
+                nms_test_group(buf, y, 4 * xq, H, W, thr, &s_cnt[l], list, capP);
             }
             __syncwarp();
             if (lane == 0) {
-                mbar_arrive_plain(&bar_free[s]);   // the plane is not needed any more
-                mbar_arrive_plain(&bar_ready[l]);  // this warp's peaks are in the list
+                mbar_arrive(&bar_free[s]);   // the plane is not needed any more
+                mbar_arrive(&bar_ready[l]);  // this warp's peaks are in the list
             }
         }
     } else {
         // =========================== finishers ===========================
         const int f = warp - 1 - kNmsPScanners;
-        const int R = a.radius;
         for (int j = f; j < nj; j += kNmsPFinishers) {
             const int l = j % kNmsPLists;
             mbar_wait_sleep(&bar_ready[l], (j / kNmsPLists) & 1);
-            const uint32_t *list = s_lists + (size_t)l * capP;
-            const int item = (int)blockIdx.x + j * G;
-            const int n_local = item / K, c = item - n_local * K;
-            const int n = a.image_base + n_local;
-            const float *plane = a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;  // L2-hot
-            const int total = s_cnt[l];
-            const int np = min(total, capP);
-            const size_t out_base = ((size_t)n * K + c) * capP;
-            for (int t = lane; t < np; t += 32) {
-                const uint32_t mine = list[t];
-                int rank = 0;  // raster index rank == np.nonzero order (evaluate.py:193); indices are unique
-                for (int u = 0; u < np; u++) rank += list[u] < mine;
-                const int lin = (int)mine;
-                const int y = lin / W, x = lin - y * W;
-                double rx, ry;
-                float sc;
-                uint32_t anchor = ((uint32_t)y << 16) | (uint32_t)x;
-                if (y + R + 1 > H || y - R < 0 || x + R + 1 > W || x - R < 0) {
-                    rx = (double)x;  // util.py:201-202: the box leaves the image -> integer anchor, raw map value
-                    ry = (double)y;
-                    sc = plane[(size_t)y * W + x];
-                    anchor |= 0x80000000u;
-                } else {
-                    switch (R) {  // util.py:204-211
-                        case 0: refine_box<0>(plane, W, x, y, rx, ry, sc); break;
-                        case 1: refine_box<1>(plane, W, x, y, rx, ry, sc); break;
-                        case 2: refine_box<2>(plane, W, x, y, rx, ry, sc); break;
-                        case 3: refine_box<3>(plane, W, x, y, rx, ry, sc); break;
-                        default: refine_box<4>(plane, W, x, y, rx, ry, sc); break;
-                    }
-                }
-                ws.peak_x[out_base + rank] = rx;
-                ws.peak_y[out_base + rank] = ry;
-                ws.peak_score[out_base + rank] = sc;
-                ws.peak_anchor[out_base + rank] = anchor;
-            }
+            nms_finish_plane(a, s_lists + (size_t)l * capP, s_cnt[l], (int)blockIdx.x + j * G, lane);
             __syncwarp();
             if (lane == 0) {
-                ws.peak_count[(size_t)n * K + c] = total;
-                if (total > capP) atomicOr(&ws.status[n], kStPeakOverflow);
                 s_cnt[l] = 0;
-                mbar_arrive_plain(&bar_lfree[l]);  // list + counter may be reused (plane j + kNmsPLists)
+                mbar_arrive(&bar_lfree[l]);  // list + counter may be reused (plane j + kNmsPLists)
             }
         }
     }

@@ -56,7 +56,6 @@ struct spg_handle {
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
     int exact_warps = 12; // scorer warps of the persistent limb_score (SPG_EXACT_WARPS)
-    int post_generic_ident = 0;  // SPG_POST_IDENT=0: single-scale identity configurations take postnet_kernel<true,true,*> (A/B timing)
     int ma_warps = kMAMatchWarps;  // matcher warps of the fused kernel (SPG_MA_WARPS, tuning)
     int fuse_ma = 1;      // whole-path calls run the fused match+assemble kernel (SPG_FUSE_MA=0: the two kernels back to back)
     int cand_dtype = SPG_F32;  // dtype of the planes the current candidates were scored on
@@ -129,8 +128,6 @@ int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t cha
     a.chan_stride = chan_stride;
     a.H = H;
     a.W = W;
-    // bands of ~16 KB through a ring of 3 buffers: two bands in flight per CTA while one is scanned, 4 CTAs per SM
-    a.band_rows = std::max(4, std::min(H, 4096 / W));
     a.radius = p->offset_radius;
     a.use_bulk = (W % 4 == 0) && (img_stride % 4 == 0) && (chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(heat) & 15) == 0);
     a.image_base = base;
@@ -155,12 +152,13 @@ int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t cha
         const int items = n * h->ws.K;
         a.band_rows = bg.band_rows;
         SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_banded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bg.smem));
-        nms_peaks_banded_kernel<<<std::min(items, h->sm_count), kNmsBThreads, bg.smem, st>>>(a, items, bg.slots, bg.n_bands);
+        nms_peaks_banded_kernel<<<std::min(items, h->sm_count), kNmsPThreads, bg.smem, st>>>(a, items, bg.slots, bg.n_bands);
         h->stage_kernel[0] = "nms_peaks_banded_kernel";
         h->launches++;
         SPG_CUDA(h, cudaGetLastError());
         return SPG_OK;
     }
+    // bands of ~16 KB through a ring of 3 buffers: two bands in flight per CTA while one is scanned, 4 CTAs per SM
     a.band_rows = std::max(4, std::min(H, 4096 / W));
     const size_t smem = nms_smem_bytes(a.band_rows, H, W, h->ws.capP);
     if (smem > h->smem_optin) return fail(h, SPG_E_INVALID, "map width %d needs %zu B of shared memory per band", W, smem);
@@ -216,10 +214,6 @@ int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, 
     a.connect_ration = p->connect_ration;
     a.screen = h->screen;
     a.crit1_strict = p->crit1_strict != 0;
-    a.debug = 0;
-#ifdef SPG_DEBUG  // timing-only knobs that change results exist only in -DSPG_DEBUG builds (never in the shipped library)
-    if (const char *e = getenv("SPG_DEBUG_PERSIST")) a.debug = atoi(e);
-#endif
     a.exact_warps = h->exact_warps;
     a.ws = h->ws;
     h->cand_dtype = dtype;
@@ -244,8 +238,8 @@ int launch_match(spg_handle *h, int base, int n, cudaStream_t st) {
     return SPG_OK;
 }
 
-int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
-    if (n == 0) return SPG_OK;
+// Arguments of the assemble stage (stand-alone or fused with the matcher); use_bulk is set by the caller.
+AssembleArgs assemble_args(const spg_handle *h, int base, int n, const spg_params *p) {
     AssembleArgs a{};
     a.n_images = n;
     a.image_base = base;
@@ -256,9 +250,15 @@ int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStr
     a.min_parts = p->min_parts;
     a.refresh_len_check = p->refresh_len_check != 0;
     a.wire_flag = h->armed_flag; a.wire_flag_value = h->armed_value; a.done_counter = h->done_counter;
-    h->armed_flag = nullptr;  // one shot
     a.ws = h->ws;
     a.ws.wire_first += base;  // records are indexed by the image's position in the call
+    return a;
+}
+
+int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
+    if (n == 0) return SPG_OK;
+    AssembleArgs a = assemble_args(h, base, n, p);
+    h->armed_flag = nullptr;  // one shot
     a.use_bulk = ((size_t)h->ws.L * h->ws.capP * sizeof(uint32_t)) % 16 == 0;  // bulk copies move multiples of 16 bytes
     const size_t smem = assemble_smem_bytes(h->ws.K, h->ws.capP, h->ws.capR) + assemble_conn_bytes(h->ws.L, h->ws.capP);
     if (smem > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need %zu B of shared memory in assemble (limit %zu)", smem, h->smem_optin);
@@ -272,18 +272,7 @@ int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStr
 
 int launch_match_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
     if (n == 0) return SPG_OK;
-    AssembleArgs a{};
-    a.n_images = n;
-    a.image_base = base;
-    a.len_rate = p->len_rate;
-    a.connection_tole = p->connection_tole;
-    a.min_mean_score = p->min_mean_score;
-    a.remove_recon = p->remove_recon;
-    a.min_parts = p->min_parts;
-    a.refresh_len_check = p->refresh_len_check != 0;
-    a.wire_flag = h->armed_flag; a.wire_flag_value = h->armed_value; a.done_counter = h->done_counter;
-    a.ws = h->ws;
-    a.ws.wire_first += base;
+    AssembleArgs a = assemble_args(h, base, n, p);
     a.use_bulk = ((size_t)h->ws.K * h->ws.capP * sizeof(float)) % 16 == 0;  // bulk copies move multiples of 16 bytes
     const size_t smem = match_assemble_smem_bytes(h->ws.K, h->ws.L, h->ws.capP, h->ws.capR, h->ma_warps);
     if (smem > h->smem_optin) {  // very large capacities: the two stand-alone kernels need less shared memory
@@ -394,7 +383,6 @@ int spg_create(const spg_config *cfg, spg_handle **out) {
     if (const char *e = getenv("SPG_PERSIST")) h->persist = !(e[0] == '0');  // 0: per-item kernels only (A/B tests)
     if (const char *e = getenv("SPG_MA_WARPS")) h->ma_warps = std::max(1, std::min(15, atoi(e)));
     if (const char *e = getenv("SPG_FUSE_MA")) h->fuse_ma = !(e[0] == '0');
-    if (const char *e = getenv("SPG_POST_IDENT")) h->post_generic_ident = atoi(e) == 0;
     if (const char *e = getenv("SPG_EXACT_WARPS")) h->exact_warps = std::max(1, std::min(30, atoi(e)));  // the kernel keeps >= 1 screener
     DeviceGuard guard(h->device);
 
@@ -619,7 +607,6 @@ int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, 
         const size_t need = (size_t)h->cfg.max_batch * ws.K * H * W;
         if (h->heat_acc_elems < need) {
             if (h->heat_acc) cudaFree(h->heat_acc);
-    if (h->done_counter) cudaFree(h->done_counter);
             h->heat_acc = nullptr; h->heat_acc_elems = 0;
             SPG_CUDA(h, cudaMalloc(&h->heat_acc, need * sizeof(double)));
             h->heat_acc_elems = need;
@@ -698,7 +685,7 @@ int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, 
         SPG_CUDA(h, (cudaFuncSetAttribute(postnet_kernel<S_, I_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))); \
         postnet_kernel<S_, I_, F_><<<grid, kPostThreads, smem, st>>>(a);                                                      \
     } while (0)
-            if (single && ident && !h->post_generic_ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
+            if (single && ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
                 a.tile_w = kPostI_TW; a.tile_h = kPostI_TH;
                 a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
                 a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
@@ -711,8 +698,7 @@ int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, 
                 h->stage_kernel[4] = "postnet_x4_ident_kernel";
             } else if (single) {
                 h->stage_kernel[4] = "postnet_kernel";
-                if (ident) { if (all16) SPG_POST_LAUNCH(true, true, true); else SPG_POST_LAUNCH(true, true, false); }
-                else { if (all16) SPG_POST_LAUNCH(true, false, true); else SPG_POST_LAUNCH(true, false, false); }
+                if (all16) SPG_POST_LAUNCH(true, false, true); else SPG_POST_LAUNCH(true, false, false);
             } else {
                 h->stage_kernel[4] = "postnet_kernel";
                 if (ident) { if (all16) SPG_POST_LAUNCH(false, true, true); else SPG_POST_LAUNCH(false, true, false); }

@@ -70,7 +70,9 @@ def test_wire_records_are_the_process_tail(env):
 
 def test_armed_signal_is_published_by_the_assemble_kernel(env):
     """spg_arm_wire_signal: the last CTA of the next assemble launch release-stores the value (here into local memory);
-    one shot -- the following launch leaves the word alone; both the fused and the stand-alone kernel carry it."""
+    one shot -- the following launch leaves the word alone; both the fused and the stand-alone kernel carry it.  A
+    multi-scale postnet at stride 2 between the two armed launches grows the handle's float64 accumulator, which must
+    leave the signal's counter alone."""
     t = env.torch
     heat, paf = env.synth.make_batch(808, 9, 128, 128, 8)
     params = env.skeleton.default_params()
@@ -84,11 +86,16 @@ def test_armed_signal_is_published_by_the_assemble_kernel(env):
         g.group_device(hd, pd, 128, params)            # fused match_assemble
         t.cuda.synchronize()
         assert word.tolist() == [41, 0]
+        first = buf.cpu().numpy()
+        gen = t.Generator().manual_seed(5)
+        net = [t.rand((1, 2, 50, 40, 48), generator=gen).to(env.dev) for _ in range(2)]
+        g.postnet(net, [(76, 90), (70, 84)], (61, 77), stride=2, paf_dtype=t.float64)
         g.group_device(hd, pd, 128, params)            # not armed any more
         g.arm_wire_signal(word.data_ptr() + 8, 77)
         g.assemble(9, params)                          # the stand-alone kernel
         t.cuda.synchronize()
         assert word.tolist() == [41, 77]
+        assert np.array_equal(buf.cpu().numpy(), first)
         rec = env.wire.as_records(buf.cpu().numpy(), 17, g.capR)
         assert (rec["n_persons"] > 0).all()
         g.set_wire_output(None)
