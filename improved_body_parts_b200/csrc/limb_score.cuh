@@ -50,6 +50,11 @@ constexpr int kScreenMaxMid = 63;       // per-m tables (maxfail, sample positio
 #endif
 constexpr int kScreenSamples = SPG_SCREEN_SAMPLES;  // interior samples looked at per pair (build-time: `make variants` for the tuning sweep)
 constexpr int kScreenMaxDim = 2048;     // f32 error of a 1/64-px position stays << 1 unit up to this map size
+// The persistent screen's rows open with this many samples spread evenly over the interior, then take the others in
+// order (build_screen_row).  Same samples, same failures counted: only the order in which a warp's lanes look at them
+// changes.  The order itself was measured not to change the speed; the register allocation ptxas makes of the
+// persistent kernel with this builder does (DESIGN.md §3, K2a).
+constexpr int kScreenSpreadFirst = kScreenSamples < 6 ? kScreenSamples : 6;
 
 // per-m constants of the screen (m = number of samples the reference would take for the pair)
 struct alignas(8) ScreenTab {
@@ -65,18 +70,41 @@ __host__ __device__ constexpr size_t screen_tables_bytes() {
     return (((size_t)(kScreenMaxMid + 1) * (sizeof(double) + sizeof(ScreenTab) + kScreenSamples * sizeof(float))) + 15) & ~(size_t)15;
 }
 
-// Builds row m of the per-m tables.
-__device__ __forceinline__ void build_screen_row(const ScoreArgs &a, int m, double *rcp, ScreenTab *tab, float *ts) {
+// Builds row m of the per-m tables.  spread: the persistent kernel's sample order (kScreenSpreadFirst), else ascending.
+__device__ __forceinline__ void build_screen_row(const ScoreArgs &a, int m, double *rcp, ScreenTab *tab, float *ts, bool spread) {
     // fewest samples that must exceed thre2: smallest integer >= connect_ration*m in f64, as :246 compares
     const double need = __dmul_rn(a.connect_ration, (double)m);
     int need_i = (int)need;
     if ((double)need_i < need || (a.crit1_strict && (double)need_i == need)) need_i++;  // strict: smallest integer > need
     rcp[m] = m > 0 ? __ddiv_rn(1.0, (double)m) : 0.0;
-    // up to kScreenSamples samples spread over the interior [lo, hi] (the ends sit on the peaks and rarely fail)
+    // up to kScreenSamples samples spread over the interior [lo, hi] (the ends sit on the peaks and rarely fail); sample r
+    // of the qn sits at lo + r * (hi - lo) / (qn - 1).  Entries past qn repeat sample qn - 1 (tail clamped: every entry
+    // is a valid sample index).
     const int lo = m / 8, hi = m - 1 - lo;
     const int qn = max(0, min(kScreenSamples, hi - lo + 1));
-    for (int q = 0; q < kScreenSamples; q++)  // tail clamped: every entry is a valid sample index
-        ts[m * kScreenSamples + q] = (float)(qn > 1 ? lo + (min(q, qn - 1) * (hi - lo)) / (qn - 1) : lo);
+    auto put = [&](int q, int r) { ts[m * kScreenSamples + q] = (float)(qn > 1 ? lo + (r * (hi - lo)) / (qn - 1) : lo); };
+    if (!spread) {
+        for (int q = 0; q < kScreenSamples; q++) put(q, min(q, max(qn - 1, 0)));
+    } else {
+        // first s1 samples at ranks ~ q * (qn - 1) / (s1 - 1): the step is >= 1, so they are distinct and the last is
+        // qn - 1; then the ranks not taken yet, ascending; then the tail
+        const int s1 = min(kScreenSpreadFirst, qn);
+        const float step = s1 > 1 ? (float)(qn - 1) / (float)(s1 - 1) : 0.0f;
+        uint32_t taken = 0;  // bit r: sample r is in the first s1
+        for (int q = 0; q < s1; q++) {
+            const int r = min((int)__fadd_rn(__fmul_rn((float)q, step), 0.5f), qn - 1);
+            taken |= 1u << r;
+            put(q, r);
+        }
+        for (int q = s1, r = 0; q < kScreenSamples; q++) {
+            if (q < qn) {
+                while (taken >> r & 1u) r++;
+                put(q, r++);
+            } else {
+                put(q, max(qn - 1, 0));
+            }
+        }
+    }
     ScreenTab t;
     t.inv = m > 1 ? 1.0f / (float)(m - 1) : 0.0f;
     t.maxfail = (signed char)max(min(m - need_i, 127), -1);
@@ -352,7 +380,7 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
         }
     } else if (warp < 4) {
         const int m = tid - 64;
-        if (m <= a.mid_num && m <= kScreenMaxMid) build_screen_row(a, m, s_rcp, s_tab, s_ts);
+        if (m <= a.mid_num && m <= kScreenMaxMid) build_screen_row(a, m, s_rcp, s_tab, s_ts, false);
         if (tid == 64 + 63) s_magic = nB > 1 ? 0xffffffffu / (uint32_t)nB + 1u : 0u;  // ceil(2^32 / nB)
     }
     __syncthreads();

@@ -39,6 +39,13 @@ constexpr int kPersistMaxCapP = 64;
 constexpr int kScreenTailBypass = 4;
 constexpr int kPersistListCap = 1024;  // survivors queued per item; the (rare) excess is evaluated inline by the screener
 
+// Clock trace (`make trace`, tools/trace_limb_score.py): 16 words per item for a CTA's first 64 items.
+// Loader: 0 iteration start, 1 copy issued, 2/3 waits for / got the meta slot of item j - kMetaSlots, 4 lists published,
+// 8 item closed, 9 survivors (value), 10 candidates (value).  Screeners: 5 first past `full`, 6 first / 7 last to leave.
+// Scorers: 11 last to leave.
+constexpr int kTrItemWords = 16, kTrItems = 64;
+#define SPG_TR_ITEM(kind, j, f, dep) do { if ((j) < kTrItems) kind(kTrItemWords * (j) + (f), dep); } while (0)
+
 struct PersistHdr {
     int nA, nB, npairs, n, k, special;
     uint32_t magic;
@@ -180,7 +187,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         s_bias_bytes = 4u * kScreenBias * (uint32_t)(W + 1);
         fence_mbar_init();
     }
-    if (tid >= 32 && tid < 32 + kScreenMaxMid + 1) build_screen_row(a, tid - 32, s_rcp, s_tab, s_ts);
+    if (tid >= 32 && tid < 32 + kScreenMaxMid + 1) build_screen_row(a, tid - 32, s_rcp, s_tab, s_ts, true);
     __syncthreads();
 
     const int G = gridDim.x;
@@ -220,6 +227,9 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         auto close_item = [&](int jp) {
             if (lane == 0) {
                 MetaSlot &ms = s_meta[jp % kMetaSlots];
+                SPG_TR_ITEM(SPG_TR, jp, 8, ms.nsurv);
+                SPG_TR_ITEM(SPG_TRV, jp, 9, ms.nsurv);
+                SPG_TR_ITEM(SPG_TRV, jp, 10, ms.ncand);
                 publish_limb(ws, ms.hdr.n, (size_t)ms.hdr.n * L + ms.hdr.k, ms.hdr.special ? -1 : ms.ncand, ms.nsurv, ms.flags);
                 ms.nsurv = 0; ms.ncand = 0; ms.bnext = 0; ms.flags = 0;
             }
@@ -228,6 +238,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         if (nj > 0) fetch(0);
         for (int j = 0; j < nj; j++) {
             const int s = j % kPersistSlots, e = j % kMetaSlots;
+            SPG_TR_ITEM(SPG_TR, j, 0, j);
             if (j >= kPersistSlots) {  // the plane slot's previous item has been screened
                 const int jp = j - kPersistSlots;
                 mbar_wait_sleep(&bar_screened[jp % kMetaSlots], (jp / kMetaSlots) & 1);
@@ -244,8 +255,11 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                     bulk_g2s(dst + off, gplane + off, bytes, &bar_full[s]);
                 }
             }
+            SPG_TR_ITEM(SPG_TR, j, 1, j);
             if (j >= kMetaSlots) {
+                SPG_TR_ITEM(SPG_TR, j, 2, j);
                 mbar_wait_sleep(&bar_mfree[e], ((j / kMetaSlots) - 1) & 1);
+                SPG_TR_ITEM(SPG_TR, j, 3, j);
                 close_item(j - kMetaSlots);
             }
             MetaSlot &ms = s_meta[e];
@@ -274,6 +288,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                 ms.hdr = h;
             }
             __syncwarp();
+            SPG_TR_ITEM(SPG_TR, j, 4, j);
             if (lane == 0) mbar_arrive(&bar_full[s]);  // arrival 2 of 2: lists + header are in place
             if (j + 1 < nj) fetch(j + 1);              // in flight while the next iteration waits for its slots
         }
@@ -312,6 +327,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                 const int s = j % kPersistSlots, e = j % kMetaSlots;
                 // `full` also means the meta slot's list and counters are recycled (the loader closed item j - kMetaSlots)
                 mbar_wait_sleep(&bar_full[s], (j / kPersistSlots) & 1);
+                SPG_TR_ITEM(SPG_TR_FIRST, j, 5, j);
                 MetaSlot &ms = s_meta[e];
                 const int npairs = ms.hdr.npairs;
                 if (c0 * 32 < npairs) {  // warps without pairs skip the item
@@ -342,6 +358,8 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                     }
                 }
                 __syncwarp();
+                SPG_TR_ITEM(SPG_TR_FIRST, j, 6, j);
+                SPG_TR_ITEM(SPG_TR_LAST, j, 7, j);
                 if (lane == 0) mbar_arrive(&bar_screened[e]);  // release: this warp's survivors are in the list, the plane is no longer read
                 if (++c0 == nS) c0 = 0;
             }
@@ -366,6 +384,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                     }
                 }
                 __syncwarp();
+                SPG_TR_ITEM(SPG_TR_LAST, j, 11, j);
                 if (lane == 0) mbar_arrive(&bar_mfree[e]);  // release: this warp's candidates and counters are visible to the loader
             }
         }

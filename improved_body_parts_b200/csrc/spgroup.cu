@@ -55,7 +55,7 @@ struct spg_handle {
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
-    int exact_warps = 12; // scorer warps of the persistent limb_score (SPG_EXACT_WARPS)
+    int exact_warps = 14; // scorer warps of the persistent limb_score (SPG_EXACT_WARPS; DESIGN.md §8 has the sweep)
     int ma_warps = kMAMatchWarps;  // matcher warps of the fused kernel (SPG_MA_WARPS, tuning)
     int fuse_ma = 1;      // whole-path calls run the fused match+assemble kernel (SPG_FUSE_MA=0: the two kernels back to back)
     int cand_dtype = SPG_F32;  // dtype of the planes the current candidates were scored on
