@@ -16,17 +16,19 @@ namespace spg {
 
 // Clock trace of the first CTAs of a launch (development builds only: `make trace` -> libspgroup_trace.so, which is
 // never loaded by the package).  SPG_TR(slot, dep) stores clock64() once `dep` (any 32-bit value) is available;
-// SPG_TR_FIRST / SPG_TR_LAST keep the earliest / latest such stamp of several warps (the buffer starts zeroed).
+// SPG_TR_FIRST / SPG_TR_LAST keep the earliest / latest such stamp of several warps (the buffer starts zeroed);
+// SPG_TR_ADD sums a value over several warps.
 #ifdef SPG_TRACE
 constexpr int kTraceCtas = 64, kTraceSlots = 1024;
 __device__ unsigned long long g_spg_trace[kTraceCtas * kTraceSlots];
-__device__ __forceinline__ void trace_put(int slot, int dep, int mode) {  // mode 0: store, 1: value, 2: first, 3: last
+__device__ __forceinline__ void trace_put(int slot, int dep, int mode) {  // mode 0: store, 1: value, 2: first, 3: last, 4: add
     if (blockIdx.x < kTraceCtas && (threadIdx.x & 31) == 0) {
         unsigned long long t;
         asm volatile("mov.u64 %0, %%clock64;" : "=l"(t) : "r"(dep) : "memory");
         unsigned long long *w = &g_spg_trace[blockIdx.x * kTraceSlots + slot];
         if (mode == 2) atomicCAS(w, 0ull, t);
         else if (mode == 3) atomicMax(w, t);
+        else if (mode == 4) atomicAdd(w, (unsigned long long)(unsigned)dep);
         else *w = mode == 1 ? (unsigned long long)(unsigned)dep : t;
     }
 }
@@ -34,11 +36,13 @@ __device__ __forceinline__ void trace_put(int slot, int dep, int mode) {  // mod
 #define SPG_TRV(slot, v) ::spg::trace_put((slot), (int)(v), 1)
 #define SPG_TR_FIRST(slot, dep) ::spg::trace_put((slot), (int)(dep), 2)
 #define SPG_TR_LAST(slot, dep) ::spg::trace_put((slot), (int)(dep), 3)
+#define SPG_TR_ADD(slot, v) ::spg::trace_put((slot), (int)(v), 4)
 #else
 #define SPG_TR(slot, dep) do {} while (0)
 #define SPG_TRV(slot, v) do {} while (0)
 #define SPG_TR_FIRST(slot, dep) do {} while (0)
 #define SPG_TR_LAST(slot, dep) do {} while (0)
+#define SPG_TR_ADD(slot, v) do {} while (0)
 #endif
 
 constexpr int kMaxParts = 32;        // K

@@ -122,22 +122,25 @@ __device__ __forceinline__ void nms_test_group(const float *rows, int y, int x0,
     }
 }
 
-// Finishes one peak at raster index `lin` of `plane`: the border test, the refinement (util.py:201-211, from L2) and the
-// four stores at output slot `out`.
-__device__ __forceinline__ void nms_finish_peak(const NmsArgs &a, const float *plane, int H, int W, size_t out, int lin) {
+// Finishes the peak at row y, column x of `plane`: the border test, the refinement (util.py:201-211, from L2) and the
+// four stores at output slot `out`.  R >= 0: the refinement radius (== a.radius) is a compile-time constant, so only
+// one refine_box is compiled in; R < 0: a.radius is dispatched at run time.
+template <int R = -1>
+__device__ __forceinline__ void nms_finish_peak(const NmsArgs &a, const float *plane, int H, int W, size_t out, int y, int x) {
     const Workspace &ws = a.ws;
-    const int R = a.radius;
-    const int y = lin / W, x = lin - y * W;
+    const int r = R >= 0 ? R : a.radius;
     double rx, ry;
     float sc;
     uint32_t anchor = ((uint32_t)y << 16) | (uint32_t)x;
-    if (y + R + 1 > H || y - R < 0 || x + R + 1 > W || x - R < 0) {
+    if (y + r + 1 > H || y - r < 0 || x + r + 1 > W || x - r < 0) {
         rx = (double)x;  // util.py:201-202: the box leaves the image -> integer anchor, raw map value
         ry = (double)y;
         sc = plane[(size_t)y * W + x];
         anchor |= 0x80000000u;
+    } else if constexpr (R >= 0) {
+        refine_box<R>(plane, W, x, y, rx, ry, sc);  // util.py:204-211
     } else {
-        switch (R) {  // util.py:204-211
+        switch (r) {  // util.py:204-211
             case 0: refine_box<0>(plane, W, x, y, rx, ry, sc); break;
             case 1: refine_box<1>(plane, W, x, y, rx, ry, sc); break;
             case 2: refine_box<2>(plane, W, x, y, rx, ry, sc); break;
@@ -197,17 +200,23 @@ __device__ __forceinline__ int nms_queue_groups(const float *data, int g0, int g
 
 // A persistent finisher's share of plane `item` (= n_local * K + c): lane t takes peaks t, t + 32, ... of the unordered
 // list, ranks each by raster index (= np.nonzero order, evaluate.py:193; indices are unique) and finishes it at its rank.
-__device__ __forceinline__ void nms_finish_plane(const NmsArgs &a, const uint32_t *list, int total, int item, int lane) {
-    const int K = a.ws.K, capP = a.ws.capP;
+// R: as in nms_finish_peak.  w4_magic != 0: ceil(2^32 / (W / 4)), and every raster index / 4 is below 2^16, so the row
+// is umulhi(index / 4, w4_magic) (exact there, as in the scanners); 0: the row is index / W.  staged != nullptr: the
+// whole plane in shared memory, which the refinement reads instead of the plane in global memory (L2).
+template <int R = -1>
+__device__ __forceinline__ void nms_finish_plane(const NmsArgs &a, const uint32_t *list, int total, int item, int lane,
+                                                 uint32_t w4_magic, const float *staged = nullptr) {
+    const int K = a.ws.K, capP = a.ws.capP, W = a.W;
     const int n_local = item / K, c = item - n_local * K;
-    const float *plane = a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;  // L2-hot
+    const float *plane = staged ? staged : a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;
     const int np = min(total, capP);
     const size_t out_base = ((size_t)(a.image_base + n_local) * K + c) * capP;
     for (int t = lane; t < np; t += 32) {
         const uint32_t mine = list[t];
         int rank = 0;
         for (int u = 0; u < np; u++) rank += list[u] < mine;
-        nms_finish_peak(a, plane, a.H, a.W, out_base + rank, (int)mine);
+        const int y = w4_magic ? (int)__umulhi(mine >> 2, w4_magic) : (int)mine / W, x = (int)mine - y * W;
+        nms_finish_peak<R>(a, plane, a.H, W, out_base + rank, y, x);
     }
     if (lane == 0) nms_publish_count(a, a.image_base + n_local, c, total);
 }
@@ -325,7 +334,10 @@ __global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
     }
     __syncthreads();
     const size_t out_base = ((size_t)n * ws.K + c) * ws.capP;
-    for (int t = tid; t < np; t += kNmsThreads) nms_finish_peak(a, plane, H, W, out_base + t, (int)s_sorted[t]);
+    for (int t = tid; t < np; t += kNmsThreads) {
+        const int lin = (int)s_sorted[t], y = lin / W;
+        nms_finish_peak(a, plane, H, W, out_base + t, y, lin - y * W);
+    }
     if (tid == 0) nms_publish_count(a, n, c, total);
 }
 

@@ -145,7 +145,7 @@ __global__ void __launch_bounds__(kNmsPThreads, 1) nms_peaks_banded_kernel(NmsAr
         for (int j = f; j < nj; j += kNmsPFinishers) {
             const int l = j % kNmsPLists;
             mbar_wait_sleep(&bar_ready[l], (j / kNmsPLists) & 1);
-            nms_finish_plane(a, s_lists + (size_t)l * capP, s_cnt[l], (int)blockIdx.x + j * G, lane);
+            nms_finish_plane(a, s_lists + (size_t)l * capP, s_cnt[l], (int)blockIdx.x + j * G, lane, 0u);
             __syncwarp();
             if (lane == 0) {
                 s_cnt[l] = 0;

@@ -139,8 +139,16 @@ int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t cha
         // one resident CTA per SM: loader, 28 scanners, 3 finishers over a ring of 3 plane slots
         const size_t psm = nms_persist_smem_bytes(H, W, h->ws.capP);
         const int items = n * h->ws.K;
-        SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        nms_peaks_persist_kernel<<<std::min(items, h->sm_count), kNmsPThreads, psm, st>>>(a, items);
+        void (*kern)(NmsArgs, int) = nms_peaks_persist_kernel<kMaxRefineRadius>;
+        switch (a.radius) {  // one kernel per refinement radius (check_params: 0 .. kMaxRefineRadius)
+            case 0: kern = nms_peaks_persist_kernel<0>; break;
+            case 1: kern = nms_peaks_persist_kernel<1>; break;
+            case 2: kern = nms_peaks_persist_kernel<2>; break;
+            case 3: kern = nms_peaks_persist_kernel<3>; break;
+        }
+        static_assert(kMaxRefineRadius == 4, "one nms_peaks_persist_kernel instantiation per radius");
+        SPG_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
+        kern<<<std::min(items, h->sm_count), kNmsPThreads, psm, st>>>(a, items);
         h->stage_kernel[0] = "nms_peaks_persist_kernel";
         h->launches++;
         SPG_CUDA(h, cudaGetLastError());
