@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
     const size_t slot = (size_t)n * ws.L + k;
     if (nA == 0 || nB == 0) {  // special_k (evaluate.py:272-274)
         if (tid == 0) {
-            ws.cand_count[slot] = -1;
+            publish_limb(ws, n, slot, -1, 0, 0);  // no candidates, no survivors (the slot is never left as it was)
             if (STAGE) mbar_wait(&bar, 0);  // the copy must land before the CTA (and its shared memory) goes away
         }
         return;

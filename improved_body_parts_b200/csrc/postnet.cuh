@@ -4,6 +4,7 @@
 //   split the two outputs (image, mirrored image) into body-part / keypoint channels        (:128-136)
 //   flip ensemble: mirror the second output back, permute its channels, average            (:139-140)
 //   cv2.resize(..., fx=stride, fy=stride, INTER_CUBIC)                                      (:143, :152)
+//   angle != 0 (rotation search): cv2.warpAffine(..., rotate_matrix_reverse, (0, 0))       (:144, :153; postnet_rot_kernel)
 //   crop the padding                                                                        (:148, :157)
 //   cv2.resize(..., (image_w, image_h), INTER_CUBIC)                                        (:149, :158)
 //   heatmap_avg += heatmap / n ; paf_avg += paf / n   (float64 accumulators, :160-161; find_peaks casts the
@@ -71,6 +72,7 @@ struct PostArgs {
     int tile_w, tile_h, tiles_x, tiles_y;
     int chan_chunk;             // stride-4 kernel: channels one CTA walks over (grid.y = ceil(n_out / chan_chunk))
     double sx1, sy1, sx2, sy2;  // source step per destination pixel of the two resizes
+    double rot[6];              // postnet_rot_kernel: the inverse of the item's warp matrix (x4 grid of the output -> of the input)
 };
 
 // interpolateCubic (imgproc/src/resize.cpp), float32, exactly oracle/postnet_port.py::cubic_coeffs
@@ -277,6 +279,313 @@ __device__ __forceinline__ float tap4w(float a0, float a1, float a2, float a3, c
     return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a0, c.x), __fmul_rn(a1, c.y)), __fmul_rn(a2, c.z)), __fmul_rn(a3, c.w));
 }
 
+// ---- building blocks of postnet_kernel and postnet_rot_kernel: one definition each, called by both kernels in the same
+// order.  Functions that end with a barrier say so; every thread of the CTA calls them.
+
+// Second resize of the output tile at (ox0, oy0): per output column / row the weights and the first tap (absolute crop
+// index, unclamped, in .x), and the four weight sets of the x4 resize.  Ends with a barrier.
+__device__ __forceinline__ void post_tabs_resize2(PostTabs &T, const PostScale &S, int ox0, int oy0, int tw, int th, int tid) {
+    if (tid < tw) {
+        float cc[4];
+        T.o2x[tid].x = axis_entry(ox0 + tid, S.sx2, cc);  // first tap (absolute crop column, unclamped) for now
+        T.w2x[tid] = make_float4(cc[0], cc[1], cc[2], cc[3]);
+    } else if (tid >= 64 && tid < 64 + th) {
+        float cc[4];
+        T.o2y[tid - 64].x = axis_entry(oy0 + tid - 64, S.sy2, cc);
+        T.w2y[tid - 64] = make_float4(cc[0], cc[1], cc[2], cc[3]);
+    } else if (tid >= 128 && tid < 132) {
+        float cc[4];
+        axis_entry(4 + (tid - 128), 0.25, cc);  // destination 4 + r: the same fraction as every 4q + r
+        T.wph[tid - 128] = make_float4(cc[0], cc[1], cc[2], cc[3]);
+    }
+    __syncthreads();
+}
+
+// (one thread) the x4 groups that cover columns c_lo..c_hi and rows y_lo..y_hi of the x stride grid, widened to multiples
+// of 4, and the source tile they read
+__device__ __forceinline__ void post_tabs_range(PostTabs &T, const PostScale &S, int c_lo, int c_hi, int y_lo, int y_hi) {
+    const int q_lo = c_lo >> 2, Q = (c_hi >> 2) - q_lo + 1, p_lo = y_lo >> 2, P = (y_hi >> 2) - p_lo + 1;
+    const int sc_lo = max(q_lo - 2, 0), sc_hi = min(q_lo + Q + 1, S.w - 1);
+    const int sr_lo = max(p_lo - 2, 0), sr_hi = min(p_lo + P + 1, S.h - 1);
+    T.rng[0] = q_lo; T.rng[1] = Q; T.rng[2] = p_lo; T.rng[3] = P;
+    T.rng[4] = sc_lo; T.rng[5] = sc_hi - sc_lo + 1; T.rng[6] = sr_lo; T.rng[7] = sr_hi - sr_lo + 1;
+}
+
+// Tap offsets of the four passes, clamps applied here once.  The second resize's are relative to (c_org, y_org), the crop
+// position of element 0 of the buffer passes 3 and 4 read.  Ends with a barrier.
+__device__ __forceinline__ void post_tabs_offsets(PostTabs &T, const PostScale &S, int tw, int th, int c_org, int y_org, int tid) {
+    const int q_lo = T.rng[0], Q = T.rng[1], p_lo = T.rng[2], P = T.rng[3], sc_lo = T.rng[4], sr_lo = T.rng[6];
+    if (tid < tw) {
+        const int b = T.o2x[tid].x;
+        T.o2x[tid] = make_int4(clampi(b, 0, S.crop_w - 1) - c_org, clampi(b + 1, 0, S.crop_w - 1) - c_org,
+                               clampi(b + 2, 0, S.crop_w - 1) - c_org, clampi(b + 3, 0, S.crop_w - 1) - c_org);
+    } else if (tid >= 64 && tid < 64 + th) {
+        const int b = T.o2y[tid - 64].x;
+        T.o2y[tid - 64] = make_int4((clampi(b, 0, S.crop_h - 1) - y_org) * kPostTW, (clampi(b + 1, 0, S.crop_h - 1) - y_org) * kPostTW,
+                                    (clampi(b + 2, 0, S.crop_h - 1) - y_org) * kPostTW, (clampi(b + 3, 0, S.crop_h - 1) - y_org) * kPostTW);
+    } else if (tid >= 128 && tid < 128 + Q) {
+        const int qa = q_lo + tid - 128;
+#pragma unroll
+        for (int k = 0; k < 5; k++) T.o1x[tid - 128][k] = clampi(qa - 2 + k, 0, S.w - 1) - sc_lo;
+    } else if (tid >= 192 && tid < 192 + P) {
+        const int pa = p_lo + tid - 192;
+#pragma unroll
+        for (int k = 0; k < 5; k++) T.o1y[tid - 192][k] = (clampi(pa - 2 + k, 0, S.h - 1) - sr_lo) * kPostF_C1;
+    }
+    __syncthreads();
+}
+
+// T.rng as values: read once per (channel, scale) iteration, before the barriers that would force shared-memory re-reads
+struct PostRange {
+    int q_lo, Q, p_lo, P, sc_lo, CS, sr_lo, RS;
+};
+__device__ __forceinline__ PostRange post_range(const PostTabs &T) {
+    return PostRange{T.rng[0], T.rng[1], T.rng[2], T.rng[3], T.rng[4], T.rng[5], T.rng[6], T.rng[7]};
+}
+
+constexpr int kPostNW = kPostThreads / 32;
+constexpr int kPostKI = (kPostF_RS + kPostNW - 1) / kPostNW;  // source rows per warp
+constexpr int kPostKJ = (kPostF_CS + 31) / 32;                // column passes per row
+constexpr int kPostKY = kPostTH / kPostNW, kPostKX = kPostTW / 32;  // output pixels per thread: rows warp + NW * ky, columns lane + 32 * kx
+
+// global loads of channel c's source tile (image and mirrored image) into registers
+template <bool F16>
+__device__ __forceinline__ void post_prefetch(float (&pv0)[kPostKI][kPostKJ], float (&pv1)[kPostKI][kPostKJ], const PostScale &S,
+                                              const PostTabs &T, const PostArgs &a, int n, int c, int warp, int lane) {
+    const int sc_lo = T.rng[4], CS = T.rng[5], sr_lo = T.rng[6], RS = T.rng[7];
+    const long long base0 = (long long)n * S.img_stride + (long long)a.src_chan[c] * S.chan_stride + (long long)sr_lo * S.w + sc_lo;
+    const long long base1 = (long long)n * S.img_stride + S.pair_stride + (long long)a.flip_chan[c] * S.chan_stride + (long long)sr_lo * S.w + (S.w - 1 - sc_lo);
+#pragma unroll
+    for (int ki = 0; ki < kPostKI; ki++) {
+        const int i = warp + kPostNW * ki;
+#pragma unroll
+        for (int kj = 0; kj < kPostKJ; kj++) {
+            const int j = lane + 32 * kj;
+            if (i < RS && j < CS) {
+                if (F16) {
+                    const __half *p = static_cast<const __half *>(S.net);
+                    pv0[ki][kj] = __half2float(p[base0 + (long long)i * S.w + j]);
+                    pv1[ki][kj] = __half2float(p[base1 + (long long)i * S.w - j]);
+                } else {
+                    const float *p = static_cast<const float *>(S.net);
+                    pv0[ki][kj] = p[base0 + (long long)i * S.w + j];
+                    pv1[ki][kj] = p[base1 + (long long)i * S.w - j];
+                }
+            }
+        }
+    }
+}
+
+// source tile: (out[c] + mirrored_out[flip(c)][:, ::-1]) / 2  (:139-140), float32, from the prefetched registers
+__device__ __forceinline__ void post_commit(float *s0, const float (&pv0)[kPostKI][kPostKJ], const float (&pv1)[kPostKI][kPostKJ],
+                                            const PostRange &R, int warp, int lane) {
+    const int CS = R.CS, RS = R.RS;
+#pragma unroll
+    for (int ki = 0; ki < kPostKI; ki++) {
+        const int i = warp + kPostNW * ki;
+#pragma unroll
+        for (int kj = 0; kj < kPostKJ; kj++) {
+            const int j = lane + 32 * kj;
+            if (i < RS && j < CS) s0[i * kPostF_CS + j] = __fdiv_rn(__fadd_rn(pv0[ki][kj], pv1[ki][kj]), 2.0f);
+        }
+    }
+}
+
+// Passes 1 and 2: the x4 resize of the source tile s0 into the x4 groups R describes, s2 [4P][kPostF_C1], with the four
+// weight sets W of T.wph.  Ends with a barrier.
+__device__ __forceinline__ void post_x4_passes(const PostTabs &T, const PostRange &R, const float4 (&W)[4], const float *s0, float *s1,
+                                               float *s2, int tid, int lane, int warp) {
+    const int Q = R.Q, P = R.P, RS = R.RS;
+    const float4 W0 = W[0], W1 = W[1], W2 = W[2], W3 = W[3];
+    // ---- pass 1: horizontal x4 -- five source values in, four intermediate columns out.  A row's groups beyond the
+    // 32nd (Q <= 36: the x2 scale has 35) do not get a second lane pass of their own: all rows' leftovers are dealt
+    // to the CTA's threads four per row.
+    auto h_item = [&](int i, int q) {
+        const float *row = s0 + i * kPostF_CS;
+        const int *o = T.o1x[q];
+        const float v0 = row[o[0]], v1 = row[o[1]], v2 = row[o[2]], v3 = row[o[3]], v4 = row[o[4]];
+        float4 r;
+        r.x = tap4w(v0, v1, v2, v3, W0);
+        r.y = tap4w(v0, v1, v2, v3, W1);
+        r.z = tap4w(v1, v2, v3, v4, W2);
+        r.w = tap4w(v1, v2, v3, v4, W3);
+        *reinterpret_cast<float4 *>(s1 + i * kPostF_C1 + 4 * q) = r;
+    };
+    for (int i = warp; i < RS; i += kPostNW)
+        if (lane < Q) h_item(i, lane);
+    if (Q > 32) {
+        static_assert(kPostF_Q <= 36 && kPostF_RS * 4 <= kPostThreads, "leftover groups: four per row, one thread each");
+        const int i = tid >> 2, q = 32 + (tid & 3);
+        if (i < RS && q < Q) h_item(i, q);
+    }
+    __syncthreads();
+    // ---- pass 2: vertical x4 -> the x stride grid (what the reference holds after :143 / :152): five 16-byte loads in,
+    // four rows of four columns out
+    auto v_item = [&](int p, int x4) {
+        const int *o = T.o1y[p];
+        const float4 b0 = *reinterpret_cast<const float4 *>(s1 + o[0] + 4 * x4), b1 = *reinterpret_cast<const float4 *>(s1 + o[1] + 4 * x4),
+                     b2 = *reinterpret_cast<const float4 *>(s1 + o[2] + 4 * x4), b3 = *reinterpret_cast<const float4 *>(s1 + o[3] + 4 * x4),
+                     b4 = *reinterpret_cast<const float4 *>(s1 + o[4] + 4 * x4);
+        float *dst = s2 + 4 * p * kPostF_C1 + 4 * x4;
+        *reinterpret_cast<float4 *>(dst) = make_float4(tap4w(b0.x, b1.x, b2.x, b3.x, W0), tap4w(b0.y, b1.y, b2.y, b3.y, W0),
+                                                       tap4w(b0.z, b1.z, b2.z, b3.z, W0), tap4w(b0.w, b1.w, b2.w, b3.w, W0));
+        *reinterpret_cast<float4 *>(dst + kPostF_C1) = make_float4(tap4w(b0.x, b1.x, b2.x, b3.x, W1), tap4w(b0.y, b1.y, b2.y, b3.y, W1),
+                                                                   tap4w(b0.z, b1.z, b2.z, b3.z, W1), tap4w(b0.w, b1.w, b2.w, b3.w, W1));
+        *reinterpret_cast<float4 *>(dst + 2 * kPostF_C1) = make_float4(tap4w(b1.x, b2.x, b3.x, b4.x, W2), tap4w(b1.y, b2.y, b3.y, b4.y, W2),
+                                                                       tap4w(b1.z, b2.z, b3.z, b4.z, W2), tap4w(b1.w, b2.w, b3.w, b4.w, W2));
+        *reinterpret_cast<float4 *>(dst + 3 * kPostF_C1) = make_float4(tap4w(b1.x, b2.x, b3.x, b4.x, W3), tap4w(b1.y, b2.y, b3.y, b4.y, W3),
+                                                                       tap4w(b1.z, b2.z, b3.z, b4.z, W3), tap4w(b1.w, b2.w, b3.w, b4.w, W3));
+    };
+    for (int p = warp; p < P; p += kPostNW)
+        if (lane < Q) v_item(p, lane);
+    if (Q > 32) {
+        static_assert(kPostF_P * 4 <= kPostThreads, "leftover column groups: four per row group, one thread each");
+        const int p = tid >> 2, x4 = 32 + (tid & 3);
+        if (p < P && x4 < Q) v_item(p, x4);
+    }
+    __syncthreads();
+}
+
+// Pass 3: horizontal pass of the second resize over the crop rows the tile needs, s2 -> s3.  Ends with a barrier when it runs.
+template <bool IDENT>
+__device__ __forceinline__ void post_resize2_h(const PostTabs &T, const float *s2, float *s3, bool identity, int tw, int th, int lane, int warp) {
+    if (!IDENT && !identity) {
+        const int yr_lo = T.o2y[0].x / kPostTW, yr_hi = T.o2y[th - 1].w / kPostTW;
+        int4 ox[kPostKX];     // this thread's columns are the same in every row: offsets and weights once per (channel, scale)
+        float4 wx[kPostKX];
+#pragma unroll
+        for (int kx = 0; kx < kPostKX; kx++) {
+            const int x = min(lane + 32 * kx, tw - 1);
+            ox[kx] = T.o2x[x];
+            wx[kx] = T.w2x[x];
+        }
+        for (int Y = yr_lo + warp; Y <= yr_hi; Y += kPostNW) {
+            const float *row = s2 + Y * kPostF_C1;
+#pragma unroll
+            for (int kx = 0; kx < kPostKX; kx++)
+                if (lane + 32 * kx < tw)
+                    s3[Y * kPostTW + lane + 32 * kx] = tap4w(row[ox[kx].x], row[ox[kx].y], row[ox[kx].z], row[ox[kx].w], wx[kx]);
+        }
+        __syncthreads();
+    }
+}
+
+// Where channel c of image n goes: one base pointer per dtype (32-bit offsets from it per thread; the dtype branches are
+// block-uniform), and whether the values stored are float32.
+struct PostOut {
+    size_t pbase;
+    float *f;
+    double *d;
+    bool store_f;
+};
+__device__ __forceinline__ PostOut post_out(const PostArgs &a, int n, int c, int ox0, int oy0, bool more_follow) {
+    const size_t plane = (size_t)a.H * a.W;
+    const bool is_heat = c < a.K;
+    PostOut o;
+    o.pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * a.W + ox0;
+    o.f = is_heat ? a.heat + o.pbase : static_cast<float *>(a.paf) + o.pbase;
+    o.d = (is_heat ? a.heat_acc : static_cast<double *>(a.paf)) + (is_heat && a.heat_acc == nullptr ? 0 : o.pbase);
+    o.store_f = is_heat ? !more_follow : !a.paf_is_f64;
+    return o;
+}
+
+// continuing a scale loop longer than one launch: the float64 sums so far
+template <bool SINGLE>
+__device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, int c,
+                                              size_t pbase, int tw, int th, int lane, int warp) {
+    if (!SINGLE && a.scale_index > 0) {
+        const double *prev = c < a.K ? a.heat_acc : static_cast<const double *>(a.paf);
+#pragma unroll
+        for (int ky = 0; ky < kPostKY; ky++)
+#pragma unroll
+            for (int kx = 0; kx < kPostKX; kx++) {
+                const int y = warp + kPostNW * ky, x = lane + 32 * kx;
+                acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = (y < th && x < tw) ? prev[pbase + (size_t)y * a.W + x] : 0.0;
+            }
+    }
+}
+
+// Pass 4 and epilogue: vertical pass of the second resize (s3; with an identity second resize the crop itself, s2),
+// / n in float32, float64 sum over the scale loop (:160-161) in registers.  SINGLE: the maps are stored from here.
+// (c_org, y_org) is the crop position of element 0 of s2.
+template <bool SINGLE, bool IDENT>
+__device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostTabs &T,
+                                               const float *s2, const float *s3, bool identity, const PostArgs &a, const PostOut &out,
+                                               int ox0, int oy0, int tw, int th, int c_org, int y_org, bool zero_start,
+                                               float nf, float nf_rcp, bool nf_small, int lane, int warp) {
+    float r1[SINGLE ? kPostKY : 1][SINGLE ? kPostKX : 1];  // single scale: the values this thread stores
+#pragma unroll
+    for (int ky = 0; ky < kPostKY; ky++) {
+        const int y = warp + kPostNW * ky;
+        if (y < th) {
+            int4 o = make_int4(0, 0, 0, 0);
+            float4 wy = make_float4(0.f, 1.f, 0.f, 0.f);
+            if (!IDENT && !identity) {
+                o = T.o2y[y];
+                wy = T.w2y[y];
+            }
+            const float *idrow = s2 + (oy0 + y - y_org) * kPostF_C1 + (ox0 - c_org);
+#pragma unroll
+            for (int kx = 0; kx < kPostKX; kx++) {
+                const int x = lane + 32 * kx;
+                if (x < tw) {
+                    float v;
+                    if (IDENT) v = idrow[x];
+                    else v = identity ? idrow[x] : tap4w(s3[o.x + x], s3[o.y + x], s3[o.z + x], s3[o.w + x], wy);
+                    if (SINGLE) {  // avg = 0.0 + v / 1: the float64 value is this float32 one
+                        r1[SINGLE ? ky : 0][SINGLE ? kx : 0] = (a.nan_scrub && v != v) ? 0.0f : v;  // demo_image.py:179-180
+                    } else {
+                        const float part = div_by_scales(v, nf, nf_rcp, nf_small);  // float32 array / Python int -> float32
+                        double sacc = __dadd_rn(zero_start ? 0.0 : acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx], (double)part);
+                        if (a.nan_scrub && sacc != sacc) sacc = 0.0;  // demo_image.py:179-180 scrubs after every scale
+                        acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = sacc;
+                    }
+                }
+            }
+        }
+    }
+    if (SINGLE) {  // one block-uniform branch on the output type, then eight stores at constant offsets from one pointer
+        const int o0 = warp * a.W + lane, dy = kPostNW * a.W;
+        if (out.store_f) {
+            float *op = out.f + o0;
+#pragma unroll
+            for (int ky = 0; ky < kPostKY; ky++)
+#pragma unroll
+                for (int kx = 0; kx < kPostKX; kx++)
+                    if (warp + kPostNW * ky < th && lane + 32 * kx < tw) op[ky * dy + 32 * kx] = r1[SINGLE ? ky : 0][SINGLE ? kx : 0];
+        } else {
+            double *op = out.d + o0;
+#pragma unroll
+            for (int ky = 0; ky < kPostKY; ky++)
+#pragma unroll
+                for (int kx = 0; kx < kPostKX; kx++)
+                    if (warp + kPostNW * ky < th && lane + 32 * kx < tw) op[ky * dy + 32 * kx] = (double)r1[SINGLE ? ky : 0][SINGLE ? kx : 0];
+        }
+    }
+}
+
+// the averaged maps, written once: keypoint maps as float32 (find_peaks' cast, :173), body parts float64 / float32
+template <bool SINGLE>
+__device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a,
+                                               const PostOut &out, int tw, int th, int lane, int warp) {
+    if (!SINGLE) {
+#pragma unroll
+        for (int ky = 0; ky < kPostKY; ky++) {
+            const int y = warp + kPostNW * ky;
+            const int orow = y * a.W;
+#pragma unroll
+            for (int kx = 0; kx < kPostKX; kx++) {
+                const int x = lane + 32 * kx;
+                if (y < th && x < tw) {
+                    const double v = acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx];
+                    if (out.store_f) out.f[orow + x] = (float)v;
+                    else out.d[orow + x] = v;
+                }
+            }
+        }
+    }
+}
+
 // SINGLE: one scale in the whole loop (the reference's default): no float64 sums, the maps are stored from pass 4.
 // IDENT: every fused scale's second resize is the identity (crop == image: weights (0,1,0,0)) -- passes 3 and 4 fall away.
 // F16: the network output is float16.
@@ -291,8 +600,6 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
     float *s3 = s2 + kPostF_R1 * kPostF_C1;                               // after the 2nd resize's h. pass  [4P][kPostTW]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr int NW = kPostThreads / 32;
-    constexpr int KY = kPostTH / NW, KX = kPostTW / 32;  // output pixels per thread: rows warp + NW * ky, columns lane + 32 * kx
     const int tile = blockIdx.x, n = blockIdx.z;
     const int c_begin = blockIdx.y * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
     const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
@@ -304,269 +611,170 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
         PostTabs &T = TT[t];
         const PostScale &S = a.sc[t];
         const bool identity = IDENT || (S.crop_h == a.H && S.crop_w == a.W);  // second resize with scale 1: weights (0, 1, 0, 0)
-        if (tid < tw) {
-            float cc[4];
-            T.o2x[tid].x = axis_entry(ox0 + tid, S.sx2, cc);  // first tap (absolute crop column, unclamped) for now
-            T.w2x[tid] = make_float4(cc[0], cc[1], cc[2], cc[3]);
-        } else if (tid >= 64 && tid < 64 + th) {
-            float cc[4];
-            T.o2y[tid - 64].x = axis_entry(oy0 + tid - 64, S.sy2, cc);
-            T.w2y[tid - 64] = make_float4(cc[0], cc[1], cc[2], cc[3]);
-        } else if (tid >= 128 && tid < 132) {
-            float cc[4];
-            axis_entry(4 + (tid - 128), 0.25, cc);  // destination 4 + r: the same fraction as every 4q + r
-            T.wph[tid - 128] = make_float4(cc[0], cc[1], cc[2], cc[3]);
-        }
-        __syncthreads();
+        post_tabs_resize2(T, S, ox0, oy0, tw, th, tid);
         if (tid == 0) {
-            // crop-coordinate range the tile reads (taps clamped to the cropped array, :148-149), widened to multiples of 4
+            // crop-coordinate range the tile reads (taps clamped to the cropped array, :148-149)
             const int c_lo = identity ? ox0 : clampi(T.o2x[0].x, 0, S.crop_w - 1), c_hi = identity ? ox0 + tw - 1 : clampi(T.o2x[tw - 1].x + 3, 0, S.crop_w - 1);
             const int y_lo = identity ? oy0 : clampi(T.o2y[0].x, 0, S.crop_h - 1), y_hi = identity ? oy0 + th - 1 : clampi(T.o2y[th - 1].x + 3, 0, S.crop_h - 1);
-            const int q_lo = c_lo >> 2, Q = (c_hi >> 2) - q_lo + 1, p_lo = y_lo >> 2, P = (y_hi >> 2) - p_lo + 1;
-            const int sc_lo = max(q_lo - 2, 0), sc_hi = min(q_lo + Q + 1, S.w - 1);
-            const int sr_lo = max(p_lo - 2, 0), sr_hi = min(p_lo + P + 1, S.h - 1);
-            T.rng[0] = q_lo; T.rng[1] = Q; T.rng[2] = p_lo; T.rng[3] = P;
-            T.rng[4] = sc_lo; T.rng[5] = sc_hi - sc_lo + 1; T.rng[6] = sr_lo; T.rng[7] = sr_hi - sr_lo + 1;
+            post_tabs_range(T, S, c_lo, c_hi, y_lo, y_hi);
         }
         __syncthreads();
-        {   // tap offsets of the four passes, clamps applied here once
-            const int q_lo = T.rng[0], Q = T.rng[1], p_lo = T.rng[2], P = T.rng[3], sc_lo = T.rng[4], sr_lo = T.rng[6];
-            const int c_lo_a = 4 * q_lo, y_lo_a = 4 * p_lo;
-            if (tid < tw) {
-                const int b = T.o2x[tid].x;
-                T.o2x[tid] = make_int4(clampi(b, 0, S.crop_w - 1) - c_lo_a, clampi(b + 1, 0, S.crop_w - 1) - c_lo_a,
-                                       clampi(b + 2, 0, S.crop_w - 1) - c_lo_a, clampi(b + 3, 0, S.crop_w - 1) - c_lo_a);
-            } else if (tid >= 64 && tid < 64 + th) {
-                const int b = T.o2y[tid - 64].x;
-                T.o2y[tid - 64] = make_int4((clampi(b, 0, S.crop_h - 1) - y_lo_a) * kPostTW, (clampi(b + 1, 0, S.crop_h - 1) - y_lo_a) * kPostTW,
-                                            (clampi(b + 2, 0, S.crop_h - 1) - y_lo_a) * kPostTW, (clampi(b + 3, 0, S.crop_h - 1) - y_lo_a) * kPostTW);
-            } else if (tid >= 128 && tid < 128 + Q) {
-                const int qa = q_lo + tid - 128;
-#pragma unroll
-                for (int k = 0; k < 5; k++) T.o1x[tid - 128][k] = clampi(qa - 2 + k, 0, S.w - 1) - sc_lo;
-            } else if (tid >= 192 && tid < 192 + P) {
-                const int pa = p_lo + tid - 192;
-#pragma unroll
-                for (int k = 0; k < 5; k++) T.o1y[tid - 192][k] = (clampi(pa - 2 + k, 0, S.h - 1) - sr_lo) * kPostF_C1;
-            }
-        }
-        __syncthreads();
+        post_tabs_offsets(T, S, tw, th, 4 * T.rng[0], 4 * T.rng[2], tid);
     }
     const float nf = (float)a.n_scales, nf_rcp = __fdiv_rn(1.0f, nf);
     const bool nf_small = a.n_scales >= 2 && a.n_scales <= 9;
-    const size_t plane = (size_t)a.H * a.W;
     const bool more_follow = a.scale_index + a.n_fused < a.n_scales;  // only with more than kPostMaxScales scales
 
-    constexpr int KI = (kPostF_RS + NW - 1) / NW;   // source rows per warp
-    constexpr int KJ = (kPostF_CS + 31) / 32;       // column passes per row
-    float pv0[KI][KJ], pv1[KI][KJ];
-    auto prefetch = [&](int c, int t) {
-        const PostScale &S = a.sc[t];
-        const int sc_lo = TT[t].rng[4], CS = TT[t].rng[5], sr_lo = TT[t].rng[6], RS = TT[t].rng[7];
-        const long long base0 = (long long)n * S.img_stride + (long long)a.src_chan[c] * S.chan_stride + (long long)sr_lo * S.w + sc_lo;
-        const long long base1 = (long long)n * S.img_stride + S.pair_stride + (long long)a.flip_chan[c] * S.chan_stride + (long long)sr_lo * S.w + (S.w - 1 - sc_lo);
-#pragma unroll
-        for (int ki = 0; ki < KI; ki++) {
-            const int i = warp + NW * ki;
-#pragma unroll
-            for (int kj = 0; kj < KJ; kj++) {
-                const int j = lane + 32 * kj;
-                if (i < RS && j < CS) {
-                    if (F16) {
-                        const __half *p = static_cast<const __half *>(S.net);
-                        pv0[ki][kj] = __half2float(p[base0 + (long long)i * S.w + j]);
-                        pv1[ki][kj] = __half2float(p[base1 + (long long)i * S.w - j]);
-                    } else {
-                        const float *p = static_cast<const float *>(S.net);
-                        pv0[ki][kj] = p[base0 + (long long)i * S.w + j];
-                        pv1[ki][kj] = p[base1 + (long long)i * S.w - j];
-                    }
-                }
-            }
-        }
-    };
-    if (c_begin < c_end) prefetch(c_begin, 0);
+    float pv0[kPostKI][kPostKJ], pv1[kPostKI][kPostKJ];
+    if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, a.sc[0], TT[0], a, n, c_begin, warp, lane);
 
     for (int c = c_begin; c < c_end; c++) {
-        const bool is_heat = c < a.K;
-        const size_t pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * a.W + ox0;
-        // output rows of this thread (32-bit offsets from one base pointer per channel; the dtype branches are block-uniform)
-        float *const out_f = is_heat ? a.heat + pbase : static_cast<float *>(a.paf) + pbase;
-        double *const out_d = (is_heat ? a.heat_acc : static_cast<double *>(a.paf)) + (is_heat && a.heat_acc == nullptr ? 0 : pbase);
-        const bool store_f = is_heat ? !more_follow : !a.paf_is_f64;
-        double acc[SINGLE ? 1 : KY][SINGLE ? 1 : KX];
-        if (!SINGLE && a.scale_index > 0) {  // continuing a scale loop longer than one launch: the float64 sums so far
-            const double *prev = is_heat ? a.heat_acc : static_cast<const double *>(a.paf);
-#pragma unroll
-            for (int ky = 0; ky < KY; ky++)
-#pragma unroll
-                for (int kx = 0; kx < KX; kx++) {
-                    const int y = warp + NW * ky, x = lane + 32 * kx;
-                    acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = (y < th && x < tw) ? prev[pbase + (size_t)y * a.W + x] : 0.0;
-                }
-        }
+        const PostOut out = post_out(a, n, c, ox0, oy0, more_follow);
+        double acc[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX];
+        post_load_acc<SINGLE>(acc, a, c, out.pbase, tw, th, lane, warp);
         for (int t = 0; t < a.n_fused; t++) {
             const PostTabs &T = TT[t];
             const PostScale &S = a.sc[t];
             const bool identity = IDENT || (S.crop_h == a.H && S.crop_w == a.W);
-            const int q_lo = T.rng[0], Q = T.rng[1], p_lo = T.rng[2], P = T.rng[3], sc_lo = T.rng[4], CS = T.rng[5], sr_lo = T.rng[6], RS = T.rng[7];
-            const int c_lo_a = 4 * q_lo, y_lo_a = 4 * p_lo, C1 = 4 * Q, R1 = 4 * P;
-            const float4 W0 = T.wph[0], W1 = T.wph[1], W2 = T.wph[2], W3 = T.wph[3];
-            // ---- source tile: (out[c] + mirrored_out[flip(c)][:, ::-1]) / 2  (:139-140), float32.  Its global loads were
-            // issued one iteration ago (the chain load -> barrier -> four short passes is latency bound otherwise);
-            // commit them, then put the next iteration's loads in flight under this iteration's passes.
-#pragma unroll
-            for (int ki = 0; ki < KI; ki++) {
-                const int i = warp + NW * ki;
-#pragma unroll
-                for (int kj = 0; kj < KJ; kj++) {
-                    const int j = lane + 32 * kj;
-                    if (i < RS && j < CS) s0[i * kPostF_CS + j] = __fdiv_rn(__fadd_rn(pv0[ki][kj], pv1[ki][kj]), 2.0f);
-                }
-            }
+            const PostRange R = post_range(T);
+            const float4 W[4] = {T.wph[0], T.wph[1], T.wph[2], T.wph[3]};
+            // ---- source tile.  Its global loads were issued one iteration ago (the chain load -> barrier -> four short
+            // passes is latency bound otherwise); commit them, then put the next iteration's loads in flight under this
+            // iteration's passes.
+            post_commit(s0, pv0, pv1, R, warp, lane);
             __syncthreads();
             {
                 int tn = t + 1, cn = c;
                 if (tn == a.n_fused) { tn = 0; cn = c + 1; }
-                if (cn < c_end) prefetch(cn, tn);
+                if (cn < c_end) post_prefetch<F16>(pv0, pv1, a.sc[tn], TT[tn], a, n, cn, warp, lane);
             }
-            // ---- pass 1: horizontal x4 -- five source values in, four intermediate columns out.  A row's groups beyond the
-            // 32nd (Q <= 36: the x2 scale has 35) do not get a second lane pass of their own: all rows' leftovers are dealt
-            // to the CTA's threads four per row.
-            auto h_item = [&](int i, int q) {
-                const float *row = s0 + i * kPostF_CS;
-                const int *o = T.o1x[q];
-                const float v0 = row[o[0]], v1 = row[o[1]], v2 = row[o[2]], v3 = row[o[3]], v4 = row[o[4]];
-                float4 r;
-                r.x = tap4w(v0, v1, v2, v3, W0);
-                r.y = tap4w(v0, v1, v2, v3, W1);
-                r.z = tap4w(v1, v2, v3, v4, W2);
-                r.w = tap4w(v1, v2, v3, v4, W3);
-                *reinterpret_cast<float4 *>(s1 + i * kPostF_C1 + 4 * q) = r;
-            };
-            for (int i = warp; i < RS; i += NW)
-                if (lane < Q) h_item(i, lane);
-            if (Q > 32) {
-                static_assert(kPostF_Q <= 36 && kPostF_RS * 4 <= kPostThreads, "leftover groups: four per row, one thread each");
-                const int i = tid >> 2, q = 32 + (tid & 3);
-                if (i < RS && q < Q) h_item(i, q);
-            }
-            __syncthreads();
-            // ---- pass 2: vertical x4 -> the cropped intermediate (what the reference holds after :148 / :157): five 16-byte
-            // loads in, four rows of four columns out
-            auto v_item = [&](int p, int x4) {
-                const int *o = T.o1y[p];
-                const float4 b0 = *reinterpret_cast<const float4 *>(s1 + o[0] + 4 * x4), b1 = *reinterpret_cast<const float4 *>(s1 + o[1] + 4 * x4),
-                             b2 = *reinterpret_cast<const float4 *>(s1 + o[2] + 4 * x4), b3 = *reinterpret_cast<const float4 *>(s1 + o[3] + 4 * x4),
-                             b4 = *reinterpret_cast<const float4 *>(s1 + o[4] + 4 * x4);
-                float *dst = s2 + 4 * p * kPostF_C1 + 4 * x4;
-                *reinterpret_cast<float4 *>(dst) = make_float4(tap4w(b0.x, b1.x, b2.x, b3.x, W0), tap4w(b0.y, b1.y, b2.y, b3.y, W0),
-                                                               tap4w(b0.z, b1.z, b2.z, b3.z, W0), tap4w(b0.w, b1.w, b2.w, b3.w, W0));
-                *reinterpret_cast<float4 *>(dst + kPostF_C1) = make_float4(tap4w(b0.x, b1.x, b2.x, b3.x, W1), tap4w(b0.y, b1.y, b2.y, b3.y, W1),
-                                                                           tap4w(b0.z, b1.z, b2.z, b3.z, W1), tap4w(b0.w, b1.w, b2.w, b3.w, W1));
-                *reinterpret_cast<float4 *>(dst + 2 * kPostF_C1) = make_float4(tap4w(b1.x, b2.x, b3.x, b4.x, W2), tap4w(b1.y, b2.y, b3.y, b4.y, W2),
-                                                                               tap4w(b1.z, b2.z, b3.z, b4.z, W2), tap4w(b1.w, b2.w, b3.w, b4.w, W2));
-                *reinterpret_cast<float4 *>(dst + 3 * kPostF_C1) = make_float4(tap4w(b1.x, b2.x, b3.x, b4.x, W3), tap4w(b1.y, b2.y, b3.y, b4.y, W3),
-                                                                               tap4w(b1.z, b2.z, b3.z, b4.z, W3), tap4w(b1.w, b2.w, b3.w, b4.w, W3));
-            };
-            for (int p = warp; p < P; p += NW)
-                if (lane < Q) v_item(p, lane);
-            if (Q > 32) {
-                static_assert(kPostF_P * 4 <= kPostThreads, "leftover column groups: four per row group, one thread each");
-                const int p = tid >> 2, x4 = 32 + (tid & 3);
-                if (p < P && x4 < Q) v_item(p, x4);
-            }
-            __syncthreads();
-            // ---- pass 3: horizontal pass of the second resize over the crop rows the tile needs
-            if (!IDENT && !identity) {
-                const int yr_lo = T.o2y[0].x / kPostTW, yr_hi = T.o2y[th - 1].w / kPostTW;
-                int4 ox[KX];     // this thread's columns are the same in every row: offsets and weights once per (channel, scale)
-                float4 wx[KX];
-#pragma unroll
-                for (int kx = 0; kx < KX; kx++) {
-                    const int x = min(lane + 32 * kx, tw - 1);
-                    ox[kx] = T.o2x[x];
-                    wx[kx] = T.w2x[x];
-                }
-                for (int Y = yr_lo + warp; Y <= yr_hi; Y += NW) {
-                    const float *row = s2 + Y * kPostF_C1;
-#pragma unroll
-                    for (int kx = 0; kx < KX; kx++)
-                        if (lane + 32 * kx < tw)
-                            s3[Y * kPostTW + lane + 32 * kx] = tap4w(row[ox[kx].x], row[ox[kx].y], row[ox[kx].z], row[ox[kx].w], wx[kx]);
-                }
-                __syncthreads();
-            }
-            // ---- pass 4: vertical pass, / n in float32, float64 sum over the scale loop (:160-161) in registers
-            const bool zero_start = a.scale_index == 0 && t == 0;
-            float r1[SINGLE ? KY : 1][SINGLE ? KX : 1];  // single scale: the values this thread stores
-#pragma unroll
-            for (int ky = 0; ky < KY; ky++) {
-                const int y = warp + NW * ky;
-                if (y < th) {
-                    int4 o = make_int4(0, 0, 0, 0);
-                    float4 wy = make_float4(0.f, 1.f, 0.f, 0.f);
-                    if (!IDENT && !identity) {
-                        o = T.o2y[y];
-                        wy = T.w2y[y];
-                    }
-                    const float *idrow = s2 + (oy0 + y - y_lo_a) * kPostF_C1 + (ox0 - c_lo_a);
-#pragma unroll
-                    for (int kx = 0; kx < KX; kx++) {
-                        const int x = lane + 32 * kx;
-                        if (x < tw) {
-                            float v;
-                            if (IDENT) v = idrow[x];
-                            else v = identity ? idrow[x] : tap4w(s3[o.x + x], s3[o.y + x], s3[o.z + x], s3[o.w + x], wy);
-                            if (SINGLE) {  // avg = 0.0 + v / 1: the float64 value is this float32 one
-                                r1[SINGLE ? ky : 0][SINGLE ? kx : 0] = (a.nan_scrub && v != v) ? 0.0f : v;  // demo_image.py:179-180
-                            } else {
-                                const float part = div_by_scales(v, nf, nf_rcp, nf_small);  // float32 array / Python int -> float32
-                                double sacc = __dadd_rn(zero_start ? 0.0 : acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx], (double)part);
-                                if (a.nan_scrub && sacc != sacc) sacc = 0.0;  // demo_image.py:179-180 scrubs after every scale
-                                acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = sacc;
-                            }
-                        }
-                    }
-                }
-            }
-            if (SINGLE) {  // one block-uniform branch on the output type, then eight stores at constant offsets from one pointer
-                const int o0 = warp * a.W + lane, dy = NW * a.W;
-                if (store_f) {
-                    float *op = out_f + o0;
-#pragma unroll
-                    for (int ky = 0; ky < KY; ky++)
-#pragma unroll
-                        for (int kx = 0; kx < KX; kx++)
-                            if (warp + NW * ky < th && lane + 32 * kx < tw) op[ky * dy + 32 * kx] = r1[SINGLE ? ky : 0][SINGLE ? kx : 0];
-                } else {
-                    double *op = out_d + o0;
-#pragma unroll
-                    for (int ky = 0; ky < KY; ky++)
-#pragma unroll
-                        for (int kx = 0; kx < KX; kx++)
-                            if (warp + NW * ky < th && lane + 32 * kx < tw) op[ky * dy + 32 * kx] = (double)r1[SINGLE ? ky : 0][SINGLE ? kx : 0];
-                }
-            }
+            post_x4_passes(T, R, W, s0, s1, s2, tid, lane, warp);  // -> the cropped intermediate (what the reference holds after :148 / :157)
+            post_resize2_h<IDENT>(T, s2, s3, identity, tw, th, lane, warp);
+            post_resize2_v<SINGLE, IDENT>(acc, T, s2, s3, identity, a, out, ox0, oy0, tw, th, 4 * R.q_lo, 4 * R.p_lo,
+                                          a.scale_index == 0 && t == 0, nf, nf_rcp, nf_small, lane, warp);
             __syncthreads();  // s0..s3 are reused by the next scale / channel
         }
-        // ---- the averaged maps, written once: keypoint maps as float32 (find_peaks' cast, :173), body parts float64 / float32
-        if (!SINGLE) {
-#pragma unroll
-            for (int ky = 0; ky < KY; ky++) {
-                const int y = warp + NW * ky;
-                const int orow = y * a.W;
-#pragma unroll
-                for (int kx = 0; kx < KX; kx++) {
-                    const int x = lane + 32 * kx;
-                    if (y < th && x < tw) {
-                        const double v = acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx];
-                        if (store_f) out_f[orow + x] = (float)v;
-                        else out_d[orow + x] = v;
-                    }
-                }
-            }
+        post_store_acc<SINGLE>(acc, a, out, tw, th, lane, warp);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// An item of the rotation search (evaluate.py:107-158, angle != 0), stride 4, one item per launch: between the x4 resize
+// and the crop the maps go through cv2.warpAffine(map, rotate_matrix_reverse, (0, 0)), INTER_LINEAR, BORDER_CONSTANT 0,
+// on the x4 grid (Hp x Wp = 4h x 4w, output grid = input grid).  The x4 maps still never exist in memory.  Per output tile:
+//   1. the crop span [c_lo, c_hi] x [y_lo, y_hi] the tile's second resize reads (the tables postnet_kernel uses);
+//   2. the box of the x4 grid whose values the warp of that span reads.  Box argument: pixel (x, y) reads the taps
+//      (sx + j, sy + i), i, j in {0, 1}, with sx = ((rhe(1024 (m1 y + m2)) + 16 + rhe(1024 m0 x)) >> 5) >> 5.  The two
+//      roundings and the +16 move 1024 * u (u = m0 x + m1 y + m2) by at most 17, so sx lies within one pixel of floor(u)
+//      (likewise sy of v = m3 x + m4 y + m5).  u and v are affine, so over the span they take their extremes at its
+//      corners: every tap lies in [floor(u_min) - 1, floor(u_max) + 2] x [floor(v_min) - 1, floor(v_max) + 2].  The box
+//      adds one more pixel on each side against the rounding of the corner values themselves and is clipped to the grid
+//      (taps outside the grid read 0 and need no value);
+//   3. the box's x4 values into shared memory with the same passes as postnet_kernel, from a flip-averaged source tile;
+//   4. the warp gathers the span from them (OpenCV's fixed point, bit for bit: oracle/postnet_rotation_port.py);
+//   5. the second resize and the epilogue of postnet_kernel: / n in float32, float64 sums that continue through memory
+//      between launches, keypoint maps cast to float32 by the last item, nan_scrub.
+// The host picks a tile whose span and box fit the buffers (a rotation grows the box by at most sqrt(2) per axis).
+constexpr int kPostR_R1 = 64;  // rows of the warped span (its columns: kPostF_C1)
+constexpr size_t postR_smem_bytes() {
+    return sizeof(PostTabs) + sizeof(float) * ((size_t)kPostF_RS * kPostF_CS + (size_t)kPostF_RS * kPostF_C1 +
+                                               (size_t)kPostF_R1 * kPostF_C1 + (size_t)kPostR_R1 * kPostF_C1);
+}
+static_assert(kPostR_R1 * kPostTW <= kPostF_RS * (kPostF_CS + kPostF_C1), "pass 3's output fits where the source tile was");
+
+template <bool SINGLE, bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a) {
+    extern __shared__ __align__(16) unsigned char post_smem[];
+    PostTabs &T = *reinterpret_cast<PostTabs *>(post_smem);
+    float *s0 = reinterpret_cast<float *>(post_smem + sizeof(PostTabs));  // source tile, flip-averaged [RS][kPostF_CS]
+    float *s1 = s0 + kPostF_RS * kPostF_CS;                   // after the horizontal x4 pass        [RS][kPostF_C1]
+    float *su = s1 + kPostF_RS * kPostF_C1;                   // the box of the x4 grid              [4P][kPostF_C1]
+    float *sr = su + kPostF_R1 * kPostF_C1;                   // the warped crop span                [kPostR_R1][kPostF_C1]
+    float *s3 = s0;                                           // after the 2nd resize's h. pass      [kPostR_R1][kPostTW]
+    __shared__ int span[4];                                   // c_lo, y_lo, columns, rows of the crop span
+    __shared__ int colA[kPostF_C1], colB[kPostF_C1], rowX[kPostR_R1], rowY[kPostR_R1];  // fixed-point coordinate terms
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tile = blockIdx.x, n = blockIdx.z;
+    const int c_begin = blockIdx.y * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
+    const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
+    const int ox0 = tx * a.tile_w, oy0 = ty * a.tile_h;
+    const int tw = min(a.tile_w, a.W - ox0), th = min(a.tile_h, a.H - oy0);
+    const PostScale &S = a.sc[0];
+    const bool identity = S.crop_h == a.H && S.crop_w == a.W;
+    const int Wp = 4 * S.w, Hp = 4 * S.h;
+    const double m0 = a.rot[0], m1 = a.rot[1], m2 = a.rot[2], m3 = a.rot[3], m4 = a.rot[4], m5 = a.rot[5];
+
+    post_tabs_resize2(T, S, ox0, oy0, tw, th, tid);
+    if (tid == 0) {
+        const int c_lo = identity ? ox0 : clampi(T.o2x[0].x, 0, S.crop_w - 1), c_hi = identity ? ox0 + tw - 1 : clampi(T.o2x[tw - 1].x + 3, 0, S.crop_w - 1);
+        const int y_lo = identity ? oy0 : clampi(T.o2y[0].x, 0, S.crop_h - 1), y_hi = identity ? oy0 + th - 1 : clampi(T.o2y[th - 1].x + 3, 0, S.crop_h - 1);
+        span[0] = c_lo; span[1] = y_lo; span[2] = c_hi - c_lo + 1; span[3] = y_hi - y_lo + 1;
+        double u_lo = INFINITY, u_hi = -INFINITY, v_lo = INFINITY, v_hi = -INFINITY;
+        for (int k = 0; k < 4; k++) {
+            const double x = (k & 1) ? c_hi : c_lo, y = (k & 2) ? y_hi : y_lo;
+            const double u = m0 * x + m1 * y + m2, v = m3 * x + m4 * y + m5;
+            u_lo = fmin(u_lo, u); u_hi = fmax(u_hi, u); v_lo = fmin(v_lo, v); v_hi = fmax(v_hi, v);
         }
+        // clipped in double first: a box far outside the grid must not overflow the conversion
+        auto clip = [](double e, int hi) { return (int)fmin(fmax(e, 0.0), (double)hi); };
+        post_tabs_range(T, S, clip(floor(u_lo) - 2.0, Wp - 1), clip(floor(u_hi) + 3.0, Wp - 1), clip(floor(v_lo) - 2.0, Hp - 1),
+                        clip(floor(v_hi) + 3.0, Hp - 1));
+    }
+    __syncthreads();
+    const int c_lo = span[0], y_lo = span[1], C1 = span[2], R1 = span[3];
+    // per column rhe(1024 m0 x), rhe(1024 m3 x); per row rhe(1024 (m1 y + m2)) + 16, rhe(1024 (m4 y + m5)) + 16
+    // (warpAffine's adelta / bdelta and X0 / Y0; __double2int_rn rounds ties to even like cvRound)
+    for (int i = tid; i < C1; i += kPostThreads) {
+        const double x = (double)(c_lo + i);
+        colA[i] = __double2int_rn(__dmul_rn(__dmul_rn(m0, x), 1024.0));
+        colB[i] = __double2int_rn(__dmul_rn(__dmul_rn(m3, x), 1024.0));
+    }
+    for (int i = tid; i < R1; i += kPostThreads) {
+        const double y = (double)(y_lo + i);
+        rowX[i] = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m1, y), m2), 1024.0)) + 16;
+        rowY[i] = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m4, y), m5), 1024.0)) + 16;
+    }
+    post_tabs_offsets(T, S, tw, th, c_lo, y_lo, tid);
+
+    const float nf = (float)a.n_scales, nf_rcp = __fdiv_rn(1.0f, nf);
+    const bool nf_small = a.n_scales >= 2 && a.n_scales <= 9;
+    const bool more_follow = a.scale_index + 1 < a.n_scales;
+    const PostRange R = post_range(T);
+    const float4 W[4] = {T.wph[0], T.wph[1], T.wph[2], T.wph[3]};
+    const int bx0 = 4 * R.q_lo, by0 = 4 * R.p_lo;
+
+    float pv0[kPostKI][kPostKJ], pv1[kPostKI][kPostKJ];
+    if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c_begin, warp, lane);
+    for (int c = c_begin; c < c_end; c++) {
+        const PostOut out = post_out(a, n, c, ox0, oy0, more_follow);
+        double acc[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX];
+        post_load_acc<SINGLE>(acc, a, c, out.pbase, tw, th, lane, warp);
+        post_commit(s0, pv0, pv1, R, warp, lane);
+        __syncthreads();
+        if (c + 1 < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c + 1, warp, lane);
+        post_x4_passes(T, R, W, s0, s1, su, tid, lane, warp);
+        // ---- the warp: the crop span from the box, taps outside the x4 grid read 0 (evaluate.py:144-146, :153-155)
+        for (int e = tid; e < R1 * C1; e += kPostThreads) {
+            const int Y = e / C1, X = e - Y * C1;
+            const int xf = (rowX[Y] + colA[X]) >> 5, yf = (rowY[Y] + colB[X]) >> 5;
+            const int sx = clampi(xf >> 5, -32768, 32767), sy = clampi(yf >> 5, -32768, 32767);  // saturate_cast<short>
+            const float fx = __fmul_rn((float)(xf & 31), 0.03125f), fy = __fmul_rn((float)(yf & 31), 0.03125f);
+            const float gx = __fsub_rn(1.0f, fx), gy = __fsub_rn(1.0f, fy);
+            const bool x0in = sx >= 0 && sx < Wp, x1in = sx + 1 >= 0 && sx + 1 < Wp;
+            const bool y0in = sy >= 0 && sy < Hp, y1in = sy + 1 >= 0 && sy + 1 < Hp;
+            const float *u = su + (sy - by0) * kPostF_C1 + (sx - bx0);
+            const float t00 = (y0in && x0in) ? u[0] : 0.0f, t01 = (y0in && x1in) ? u[1] : 0.0f;
+            const float t10 = (y1in && x0in) ? u[kPostF_C1] : 0.0f, t11 = (y1in && x1in) ? u[kPostF_C1 + 1] : 0.0f;
+            sr[Y * kPostF_C1 + X] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t00, __fmul_rn(gy, gx)), __fmul_rn(t01, __fmul_rn(gy, fx))),
+                                                        __fmul_rn(t10, __fmul_rn(fy, gx))), __fmul_rn(t11, __fmul_rn(fy, fx)));
+        }
+        __syncthreads();
+        post_resize2_h<false>(T, sr, s3, identity, tw, th, lane, warp);
+        post_resize2_v<SINGLE, false>(acc, T, sr, s3, identity, a, out, ox0, oy0, tw, th, c_lo, y_lo, a.scale_index == 0, nf,
+                                      nf_rcp, nf_small, lane, warp);
+        __syncthreads();  // s0 / s3, su and sr are reused by the next channel
+        post_store_acc<SINGLE>(acc, a, out, tw, th, lane, warp);
     }
 }
 

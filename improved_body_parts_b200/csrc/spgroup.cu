@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -597,8 +598,34 @@ const char *spg_stage_kernel(const spg_handle *h, int32_t stage) { return (h && 
 // ---- post-network stage ------------------------------------------------------------------------
 int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, int32_t W, float *heat_out, void *paf_out,
                 int32_t paf_dtype, void *stream) {
+    return spg_postnet_rotated(h, d, nullptr, n, H, W, heat_out, paf_out, paf_dtype, stream);
+}
+
+// warpAffine's inversion of its matrix (imgproc/src/imgwarp.cpp), in its operation order (this file's host code is built
+// without FMA contraction): the kernel then repeats its fixed-point coordinates bit for bit
+static void invert_affine(const double *M, double *m) {
+    for (int i = 0; i < 6; i++) m[i] = M[i];
+    double D = m[0] * m[4] - m[1] * m[3];
+    D = D != 0 ? 1.0 / D : 0.0;
+    const double A11 = m[4] * D, A22 = m[0] * D;
+    m[0] = A11; m[1] *= -D; m[3] *= -D; m[4] = A22;
+    const double b1 = -m[0] * m[2] - m[1] * m[5], b2 = -m[3] * m[2] - m[4] * m[5];
+    m[2] = b1; m[5] = b2;
+}
+
+int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_postnet_rotation *rot, int32_t n, int32_t H, int32_t W,
+                        float *heat_out, void *paf_out, int32_t paf_dtype, void *stream) {
     if (!h) return SPG_E_INVALID;
     if (!d || !d->scales || d->n_scales < 1 || !d->flip_paf_ord || !d->flip_heat_ord) return fail(h, SPG_E_INVALID, "postnet descriptor incomplete");
+    bool any_rot = false;
+    for (int t = 0; rot && t < d->n_scales; t++) {
+        if ((rot[t].apply != 0 && rot[t].apply != 1) || rot[t].reserved != 0)
+            return fail(h, SPG_E_INVALID, "rotation %d: apply must be 0 or 1 and reserved 0", t);
+        for (int k = 0; k < 6; k++)
+            if (!std::isfinite(rot[t].matrix[k])) return fail(h, SPG_E_INVALID, "rotation %d: matrix entry %d is not finite", t, k);
+        if (rot[t].apply && d->stride != 4) return fail(h, SPG_E_INVALID, "rotation %d: rotated items need stride 4", t);
+        any_rot = any_rot || rot[t].apply;
+    }
     if ((!heat_out || !paf_out) && n > 0) return fail(h, SPG_E_INVALID, "heat_out/paf_out is NULL");
     if (paf_dtype != SPG_F32 && paf_dtype != SPG_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32 or SPG_F64");
     if (paf_dtype == SPG_F32 && d->n_scales != 1)
@@ -611,7 +638,7 @@ int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, 
     if (ws.K + ws.L > kMaxNetChannels) return fail(h, SPG_E_INVALID, "too many channels for postnet");
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales)) {  // float64 keypoint sums that outlive a launch
+    if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
         const size_t need = (size_t)h->cfg.max_batch * ws.K * H * W;
         if (h->heat_acc_elems < need) {
             if (h->heat_acc) cudaFree(h->heat_acc);
@@ -660,10 +687,57 @@ int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, 
     };
     const bool fast = d->stride == 4;  // the reference's model: four-phase kernel; other strides: table-driven generic kernel
     if (fast) {
-        // the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales
-        for (int t0 = 0; t0 < d->n_scales; t0 += kPostMaxScales) {
-            a.n_fused = std::min(kPostMaxScales, d->n_scales - t0);
+        // the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales.  With a
+        // rotated item every item is a launch of its own, in item order: rotated ones postnet_rot_kernel, the others
+        // postnet_kernel; the float64 sums continue through memory.
+        const int group = any_rot ? 1 : kPostMaxScales;
+        for (int t0 = 0; t0 < d->n_scales; t0 += group) {
+            a.n_fused = std::min(group, d->n_scales - t0);
             a.scale_index = t0;
+            if (any_rot && rot[t0].apply) {
+                a.sc[0] = scale_of(d->scales[t0]);
+                const PostScale &S = a.sc[0];
+                invert_affine(rot[t0].matrix, a.rot);
+                // the largest tile (up to 64 x 32) whose crop span and rotated box fit the kernel's buffers: a span of cw x ch
+                // crop pixels reads a box of |m0| cw + |m1| ch (+ 7, the box's margins) columns of the x4 grid, and its x4
+                // groups add up to two more
+                const bool ident = S.crop_h == H && S.crop_w == W;
+                auto fits = [&](int tw, int th) {
+                    const double cw = ident ? tw : tw * S.sx2 + 5.0, ch = ident ? th : th * S.sy2 + 5.0;
+                    const double bw = std::fabs(a.rot[0]) * cw + std::fabs(a.rot[1]) * ch + 7.0;
+                    const double bh = std::fabs(a.rot[3]) * cw + std::fabs(a.rot[4]) * ch + 7.0;
+                    return cw <= kPostF_C1 && ch <= kPostR_R1 && bw / 4.0 + 2.0 <= kPostF_Q && bh / 4.0 + 2.0 <= kPostF_P;
+                };
+                int tw = kPostTW, th = kPostTH;
+                while (!fits(tw, th) && (tw > 1 || th > 1)) {
+                    if (tw * S.sx2 >= th * S.sy2 && tw > 1) tw--;
+                    else if (th > 1) th--;
+                    else tw--;
+                }
+                if (!fits(tw, th)) return fail(h, SPG_E_INVALID, "rotation %d: the crop is too large for the image to warp it", t0);
+                a.tile_w = tw; a.tile_h = th;
+                a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
+                a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
+                if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
+                const long long tiles = (long long)a.tiles_x * a.tiles_y * n;
+                const int n_chunks = (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * 16 + tiles - 1) / tiles));
+                a.chan_chunk = (a.n_out + n_chunks - 1) / n_chunks;
+                dim3 grid((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
+                const size_t smem = postR_smem_bytes();
+#define SPG_ROT_LAUNCH(S_, F_)                                                                                                \
+    do {                                                                                                                      \
+        SPG_CUDA(h, (cudaFuncSetAttribute(postnet_rot_kernel<S_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))); \
+        postnet_rot_kernel<S_, F_><<<grid, kPostThreads, smem, st>>>(a);                                                      \
+    } while (0)
+                const bool single = d->n_scales == 1;
+                if (single) { if (S.net_is_f16) SPG_ROT_LAUNCH(true, true); else SPG_ROT_LAUNCH(true, false); }
+                else { if (S.net_is_f16) SPG_ROT_LAUNCH(false, true); else SPG_ROT_LAUNCH(false, false); }
+#undef SPG_ROT_LAUNCH
+                h->stage_kernel[4] = "postnet_rot_kernel";
+                h->launches++;
+                SPG_CUDA(h, cudaGetLastError());
+                continue;
+            }
             a.tile_w = kPostTW; a.tile_h = kPostTH;
             for (int t = 0; t < a.n_fused; t++) {
                 a.sc[t] = scale_of(d->scales[t0 + t]);

@@ -30,7 +30,8 @@ EXPORTS = (
     "spg_assemble", "spg_upload_peaks", "spg_upload_connections", "spg_download_peaks", "spg_download_connections",
     "spg_download_people", "spg_download_status", "spg_launch_count", "spg_stage_kernel", "spg_wire_record_bytes",
     "spg_set_wire_output", "spg_wire_create", "spg_wire_open", "spg_wire_close", "spg_wire_destroy", "spg_wire_signal",
-    "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal")
+    "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal",
+    "spg_postnet_rotated")
 
 
 class GroupingError(RuntimeError):
@@ -60,6 +61,10 @@ class _PostnetDesc(C.Structure):
     _fields_ = [("n_scales", C.c_int32), ("scales", C.POINTER(_PostnetScale)), ("stride", C.c_int32),
                 ("paf_chan0", C.c_int32), ("heat_chan0", C.c_int32), ("flip_paf_ord", C.POINTER(C.c_int32)),
                 ("flip_heat_ord", C.POINTER(C.c_int32)), ("nan_scrub", C.c_int32)]
+
+
+class _PostnetRotation(C.Structure):
+    _fields_ = [("apply", C.c_int32), ("reserved", C.c_int32), ("matrix", C.c_double * 6)]
 
 
 class _DeviceView(C.Structure):
@@ -100,6 +105,8 @@ def load_library() -> C.CDLL:
         lib.spg_wire_destroy.argtypes = [C.c_int32, C.c_void_p]
         lib.spg_wire_signal.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
         lib.spg_wire_wait.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
+        lib.spg_postnet_rotated.argtypes = [C.c_void_p, C.POINTER(_PostnetDesc), C.POINTER(_PostnetRotation), C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
         if lib.spg_abi_version() != ABI_VERSION:
             raise GroupingError("libspgroup.so ABI version mismatch")
         _lib = lib
@@ -421,12 +428,14 @@ class Grouper:
     # -- post-network stage ---------------------------------------------------------------------------
     def postnet(self, net_outs, crops, out_hw, *, stride: int = 4, paf_dtype=None, heat_out=None, paf_out=None,
                 paf_chan0: int = 0, heat_chan0: Optional[int] = None, flip_paf_ord=None, flip_heat_ord=None,
-                nan_scrub: bool = False, stream=None):
+                nan_scrub: bool = False, stream=None, rotations=None):
         """The scale loop of ``predict()`` after the forward pass (evaluate.py:126-161) on the device.
 
-        ``net_outs``: one CUDA tensor ``[N, 2, C, h, w]`` (float32 / float16; image, mirrored image) per scale;
-        ``crops``: per scale ``(crop_h, crop_w)`` = ``imageToTest.shape[:2]``; ``out_hw``: the image size.
-        Returns ``(heat [N,K,H,W] float32, paf [N,L,H,W])`` -- ``paf`` float32 for a single scale (pass
+        ``net_outs``: one CUDA tensor ``[N, 2, C, h, w]`` (float32 / float16; image, mirrored image) per item of
+        ``product(multiplier, rotate_angle)``; ``crops``: per item ``(crop_h, crop_w)`` = ``imageToTest.shape[:2]``;
+        ``out_hw``: the image size.  ``rotations``: ``None``, or per item ``None`` (angle 0) or the 2x3 matrix the
+        reference warps that item's x stride maps with (``rotate_matrix_reverse``, evaluate.py:115, :144, :153).
+        Returns ``(heat [N,K,H,W] float32, paf [N,L,H,W])`` -- ``paf`` float32 for a single item (pass
         ``paf_as_f64=True`` to the grouping calls: the reference's float64 values are exactly these), float64 otherwise.
         """
         import torch
@@ -466,10 +475,21 @@ class Grouper:
             raise GroupingError("heat_out / paf_out must be contiguous tensors of the requested dtype")
         desc = _PostnetDesc(len(net_outs), scales, int(stride), int(paf_chan0), int(heat_chan0),
                             fp.ctypes.data_as(C.POINTER(C.c_int32)), fh.ctypes.data_as(C.POINTER(C.c_int32)), int(bool(nan_scrub)))
-        rc = self._lib.spg_postnet(self._h, C.byref(desc), C.c_int32(N), C.c_int32(H), C.c_int32(W),
-                                   C.c_void_p(heat_out.data_ptr()), C.c_void_p(paf_out.data_ptr()),
-                                   C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
-        self._check(rc, "spg_postnet")
+        rot = None
+        if rotations is not None:
+            if len(rotations) != len(net_outs):
+                raise GroupingError("one rotation entry (None or a 2x3 matrix) per item expected")
+            rot = (_PostnetRotation * len(net_outs))()
+            for t, m in enumerate(rotations):
+                if m is not None:
+                    m = np.asarray(m, np.float64)
+                    if m.shape != (2, 3):
+                        raise GroupingError("a rotation matrix is 2x3")
+                    rot[t] = _PostnetRotation(1, 0, (C.c_double * 6)(*m.reshape(6).tolist()))
+        rc = self._lib.spg_postnet_rotated(self._h, C.byref(desc), rot, C.c_int32(N), C.c_int32(H), C.c_int32(W),
+                                           C.c_void_p(heat_out.data_ptr()), C.c_void_p(paf_out.data_ptr()),
+                                           C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
+        self._check(rc, "spg_postnet_rotated")
         return heat_out, paf_out
 
     # -- stages -------------------------------------------------------------------------------------

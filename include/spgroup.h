@@ -146,7 +146,7 @@ typedef struct spg_postnet_scale {
     int32_t crop_h, crop_w;         /* imageToTest size: padded size minus pad[2] / pad[3] (evaluate.py:148) */
 } spg_postnet_scale;
 typedef struct spg_postnet_desc {
-    int32_t n_scales;               /* len(multiplier) * len(rotate_angle); rotation is not supported (angle == 0) */
+    int32_t n_scales;               /* items: len(multiplier) * len(rotate_angle), in product() order (scale-major) */
     const spg_postnet_scale *scales;
     int32_t stride;                 /* model_params['stride'] (4) */
     int32_t paf_chan0, heat_chan0;  /* first body-part / keypoint channel of the network output (0 / 30, config.py:101-103) */
@@ -161,6 +161,18 @@ typedef struct spg_postnet_desc {
  * Interpolation follows OpenCV's generic bicubic path (A = -0.75) operation for operation in float32. */
 int spg_postnet(spg_handle *h, const spg_postnet_desc *desc, int32_t n_images, int32_t height, int32_t width,
                 float *heat_out, void *paf_out, int32_t paf_dtype, void *stream);
+/* The rotation search (rotation_search != [0], evaluate.py:107-158): per item, whether its x stride maps go through
+ * cv2.warpAffine(map, matrix, (0, 0)) (INTER_LINEAR, BORDER_CONSTANT 0) before the crop.  The warp follows OpenCV's
+ * fixed-point algorithm bit for bit.  Rotated items need stride 4. */
+typedef struct spg_postnet_rotation {
+    int32_t apply;      /* 0: angle == 0, the item is not warped (evaluate.py:115,144,153); 1: warped */
+    int32_t reserved;   /* 0 */
+    double matrix[6];   /* row-major 2x3 matrix evaluate.py passes to cv2.warpAffine for the maps (rotate_matrix_reverse) */
+} spg_postnet_rotation;
+/* spg_postnet with rot [desc->n_scales] (NULL: no item is rotated; spg_postnet is this call with NULL). */
+int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *desc, const spg_postnet_rotation *rot,
+                        int32_t n_images, int32_t height, int32_t width, float *heat_out, void *paf_out,
+                        int32_t paf_dtype, void *stream);
 
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
