@@ -682,6 +682,26 @@ constexpr size_t postR_smem_bytes() {
 }
 static_assert(kPostR_R1 * kPostTW <= kPostF_RS * (kPostF_CS + kPostF_C1), "pass 3's output fits where the source tile was");
 
+// One destination pixel of warpAffine's INTER_LINEAR (imgproc/src/imgwarp.cpp) on a w x h grid: (xs, ys) are its source
+// coordinates in OpenCV's fixed point, X0 + adelta and Y0 + bdelta (1/1024 px, the +16 rounding term included).  The grid's
+// value (y, x) is val(g[(y - y0) * pitch + (x - x0) * CS]); taps outside the grid read 0 (BORDER_CONSTANT) and are never
+// loaded.  Every product and sum is rounded to float32, left to right.  Shared by the inverse warp of the maps
+// (postnet_rot_kernel) and the forward warp of the input image (prenet.cuh).
+template <int CS, typename T, typename Val>
+__device__ __forceinline__ float warp_linear(int xs, int ys, int w, int h, const T *g, int pitch, int x0, int y0, const Val &val) {
+    const int xf = xs >> 5, yf = ys >> 5;
+    const int sx = clampi(xf >> 5, -32768, 32767), sy = clampi(yf >> 5, -32768, 32767);  // saturate_cast<short>
+    const float fx = __fmul_rn((float)(xf & 31), 0.03125f), fy = __fmul_rn((float)(yf & 31), 0.03125f);
+    const float gx = __fsub_rn(1.0f, fx), gy = __fsub_rn(1.0f, fy);
+    const bool x0in = sx >= 0 && sx < w, x1in = sx + 1 >= 0 && sx + 1 < w;
+    const bool y0in = sy >= 0 && sy < h, y1in = sy + 1 >= 0 && sy + 1 < h;
+    const T *u = g + (sy - y0) * pitch + (sx - x0) * CS;
+    const float t00 = (y0in && x0in) ? val(u[0]) : 0.0f, t01 = (y0in && x1in) ? val(u[CS]) : 0.0f;
+    const float t10 = (y1in && x0in) ? val(u[pitch]) : 0.0f, t11 = (y1in && x1in) ? val(u[pitch + CS]) : 0.0f;
+    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t00, __fmul_rn(gy, gx)), __fmul_rn(t01, __fmul_rn(gy, fx))),
+                               __fmul_rn(t10, __fmul_rn(fy, gx))), __fmul_rn(t11, __fmul_rn(fy, fx)));
+}
+
 template <bool SINGLE, bool F16>
 __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a) {
     extern __shared__ __align__(16) unsigned char post_smem[];
@@ -757,17 +777,8 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
         // ---- the warp: the crop span from the box, taps outside the x4 grid read 0 (evaluate.py:144-146, :153-155)
         for (int e = tid; e < R1 * C1; e += kPostThreads) {
             const int Y = e / C1, X = e - Y * C1;
-            const int xf = (rowX[Y] + colA[X]) >> 5, yf = (rowY[Y] + colB[X]) >> 5;
-            const int sx = clampi(xf >> 5, -32768, 32767), sy = clampi(yf >> 5, -32768, 32767);  // saturate_cast<short>
-            const float fx = __fmul_rn((float)(xf & 31), 0.03125f), fy = __fmul_rn((float)(yf & 31), 0.03125f);
-            const float gx = __fsub_rn(1.0f, fx), gy = __fsub_rn(1.0f, fy);
-            const bool x0in = sx >= 0 && sx < Wp, x1in = sx + 1 >= 0 && sx + 1 < Wp;
-            const bool y0in = sy >= 0 && sy < Hp, y1in = sy + 1 >= 0 && sy + 1 < Hp;
-            const float *u = su + (sy - by0) * kPostF_C1 + (sx - bx0);
-            const float t00 = (y0in && x0in) ? u[0] : 0.0f, t01 = (y0in && x1in) ? u[1] : 0.0f;
-            const float t10 = (y1in && x0in) ? u[kPostF_C1] : 0.0f, t11 = (y1in && x1in) ? u[kPostF_C1 + 1] : 0.0f;
-            sr[Y * kPostF_C1 + X] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t00, __fmul_rn(gy, gx)), __fmul_rn(t01, __fmul_rn(gy, fx))),
-                                                        __fmul_rn(t10, __fmul_rn(fy, gx))), __fmul_rn(t11, __fmul_rn(fy, fx)));
+            sr[Y * kPostF_C1 + X] = warp_linear<1>(rowX[Y] + colA[X], rowY[Y] + colB[X], Wp, Hp, su, kPostF_C1, bx0, by0,
+                                                   [](float v) { return v; });
         }
         __syncthreads();
         post_resize2_h<false>(T, sr, s3, identity, tw, th, lane, warp);

@@ -28,6 +28,7 @@
 #include "nms_peaks_persist.cuh"
 #include "nms_peaks_banded.cuh"
 #include "postnet.cuh"
+#include "prenet.cuh"
 
 using namespace spg;
 
@@ -50,9 +51,11 @@ struct spg_handle {
     unsigned long long armed_value = 0;
     double *heat_acc = nullptr;  // postnet: float64 accumulator of the keypoint maps over the scale loop
     size_t heat_acc_elems = 0;
+    unsigned char *pre_grid = nullptr;  // prenet: the padded uint8 images of a rotated item, grown on demand
+    size_t pre_grid_bytes = 0;
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
-    const char *stage_kernel[5] = {"", "", "", "", ""};  // nms_peaks, limb_score, limb_match, assemble, post-network
+    const char *stage_kernel[6] = {"", "", "", "", "", ""};  // nms_peaks, limb_score, limb_match, assemble, post-, pre-network
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
@@ -444,6 +447,7 @@ void spg_destroy(spg_handle *h) {
     if (h->in_heat) cudaFree(h->in_heat);
     if (h->in_paf) cudaFree(h->in_paf);
     if (h->heat_acc) cudaFree(h->heat_acc);
+    if (h->pre_grid) cudaFree(h->pre_grid);
     if (h->done_counter) cudaFree(h->done_counter);
     for (auto &s : h->streams)
         if (s) cudaStreamDestroy(s);
@@ -593,7 +597,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 
 int64_t spg_launch_count(const spg_handle *h) { return h ? h->launches : 0; }
 
-const char *spg_stage_kernel(const spg_handle *h, int32_t stage) { return (h && stage >= 0 && stage < 5) ? h->stage_kernel[stage] : ""; }
+const char *spg_stage_kernel(const spg_handle *h, int32_t stage) { return (h && stage >= 0 && stage < 6) ? h->stage_kernel[stage] : ""; }
 
 // ---- post-network stage ------------------------------------------------------------------------
 int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, int32_t W, float *heat_out, void *paf_out,
@@ -807,6 +811,82 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         postnet_generic_kernel<<<grid, kPostThreads, 0, st>>>(a);
         h->stage_kernel[4] = "postnet_generic_kernel";
         h->launches++;
+        SPG_CUDA(h, cudaGetLastError());
+    }
+    return SPG_OK;
+}
+
+// ---- pre-network stage -------------------------------------------------------------------------
+int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_t row_stride, int32_t n, int32_t height,
+               int32_t width, int32_t max_downsample, int32_t pad_value, const spg_prenet_item *items, int32_t n_items,
+               void *stream) {
+    if (!h) return SPG_E_INVALID;
+    if (n < 0 || n > 65535) return fail(h, SPG_E_INVALID, "n_images %d outside [0, 65535]", n);
+    if (height < 1 || width < 1 || height > 32767 || width > 32767)
+        return fail(h, SPG_E_INVALID, "image %dx%d outside [1, 32767]", height, width);
+    if (max_downsample < 1 || max_downsample > 32767) return fail(h, SPG_E_INVALID, "max_downsample %d outside [1, 32767]", max_downsample);
+    if (pad_value < 0 || pad_value > 255) return fail(h, SPG_E_INVALID, "pad_value %d outside [0, 255]", pad_value);
+    if (n_items < 0 || (n_items > 0 && !items)) return fail(h, SPG_E_INVALID, "items is NULL or n_items negative");
+    if (n > 0 && !image) return fail(h, SPG_E_INVALID, "image_dev is NULL");
+    if (row_stride < 3LL * width || image_stride < 0) return fail(h, SPG_E_INVALID, "row_stride below width * 3 or image_stride negative");
+    // validate every item before the first launch; the geometry is cv2.resize's and util.padRightDownCorner's
+    std::vector<PreArgs> args((size_t)n_items);
+    size_t grid_need = 0;
+    for (int t = 0; t < n_items; t++) {
+        const spg_prenet_item &it = items[t];
+        if (!std::isfinite(it.scale) || !(it.scale > 0)) return fail(h, SPG_E_INVALID, "item %d: scale must be finite and positive", t);
+        if ((it.rotate != 0 && it.rotate != 1) || it.reserved != 0)
+            return fail(h, SPG_E_INVALID, "item %d: rotate must be 0 or 1 and reserved 0", t);
+        for (int k = 0; k < 6; k++)
+            if (!std::isfinite(it.matrix[k])) return fail(h, SPG_E_INVALID, "item %d: matrix entry %d is not finite", t, k);
+        const double rh = (double)height * it.scale, rw = (double)width * it.scale;  // dsize = saturate_cast<int>(size * fx)
+        if (!(rh < 32767.5 && rw < 32767.5)) return fail(h, SPG_E_INVALID, "item %d: padded image above 32767 pixels a side", t);
+        PreArgs &a = args[t];
+        a.H1 = (int)std::nearbyint(rh);
+        a.W1 = (int)std::nearbyint(rw);
+        if (a.H1 < 1 || a.W1 < 1) return fail(h, SPG_E_INVALID, "item %d: the resized image is empty (%dx%d)", t, a.H1, a.W1);
+        a.Hp = (a.H1 + max_downsample - 1) / max_downsample * max_downsample;
+        a.Wp = (a.W1 + max_downsample - 1) / max_downsample * max_downsample;
+        if (a.Hp > 32767 || a.Wp > 32767 || (long long)a.Hp * a.Wp * 3 > 0x7fffffffLL)
+            return fail(h, SPG_E_INVALID, "item %d: padded image %dx%d above 32767 pixels a side or 2^31 values", t, a.Hp, a.Wp);
+        if (!it.out) return fail(h, SPG_E_INVALID, "item %d: out is NULL", t);
+        const long long pair = 2LL * a.Hp * a.Wp * 3;
+        if (n > 1 && it.out_image_stride < pair)
+            return fail(h, SPG_E_INVALID, "item %d: out_image_stride %lld below the pair's %lld elements", t, (long long)it.out_image_stride, pair);
+        a.src = image; a.img_stride = image_stride; a.row_stride = row_stride; a.h = height; a.w = width;
+        a.copy = a.H1 == height && a.W1 == width;  // cv2.resize: dsize == ssize is a copy
+        a.n_body = a.W1 * 3 / kPreLanes * kPreLanes;
+        a.pad_value = pad_value;
+        a.scale = 1.0 / it.scale;  // resize keeps scale = 1 / inv_scale, not src / dst
+        a.out = it.out; a.out_stride = it.out_image_stride;
+        if (it.rotate) {
+            invert_affine(it.matrix, a.rot);
+            grid_need = std::max(grid_need, (size_t)n * a.Hp * a.Wp * 3);
+        }
+    }
+    if (n == 0 || n_items == 0) return SPG_OK;
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (h->pre_grid_bytes < grid_need) {
+        if (h->pre_grid) cudaFree(h->pre_grid);
+        h->pre_grid = nullptr; h->pre_grid_bytes = 0;
+        SPG_CUDA(h, cudaMalloc(&h->pre_grid, grid_need));
+        h->pre_grid_bytes = grid_need;
+    }
+    for (int t = 0; t < n_items; t++) {
+        PreArgs &a = args[t];
+        a.grid = h->pre_grid;
+        const dim3 grid((unsigned)((a.Wp + kPreThreads - 1) / kPreThreads), (unsigned)a.Hp, (unsigned)n);
+        if (items[t].rotate) {
+            prenet_resize_kernel<<<grid, kPreThreads, 0, st>>>(a);
+            prenet_kernel<true><<<grid, kPreThreads, 0, st>>>(a);
+            h->launches += 2;
+            h->stage_kernel[5] = "prenet_kernel<true>";
+        } else {
+            prenet_kernel<false><<<grid, kPreThreads, 0, st>>>(a);
+            h->launches++;
+            h->stage_kernel[5] = "prenet_kernel<false>";
+        }
         SPG_CUDA(h, cudaGetLastError());
     }
     return SPG_OK;

@@ -28,17 +28,23 @@ from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
 _device = 0
 _variant = "evaluate"
+_input_stage = "host"
 _groupers: Dict[int, Grouper] = {}
 CAP_PEAKS, CAP_CANDS, CAP_ROWS = 128, 4096, 128
 MAX_DIM = 32767  # the C ABI's limit; the workspace does not depend on the map size, so ONE handle serves every image size
 
 
 def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optional[int] = None,
-              variant: Optional[str] = None) -> None:
-    """Select the limb table (default: the Canonical ``limbs_conn``, config/config.py:94), the CUDA device and the
+              variant: Optional[str] = None, input_stage: Optional[str] = None) -> None:
+    """Select the limb table (default: the Canonical ``limbs_conn``, config/config.py:94), the CUDA device, the
     behavioural variant: ``"evaluate"`` (evaluate.py, the default) or ``"demo"`` (demo_image.py's inlined copy, which
-    differs at :288, :414-415 and :533 -- SURVEY.md 3.2)."""
-    global _limbs, _device, _variant
+    differs at :288, :414-415 and :533 -- SURVEY.md 3.2), and where ``predict`` builds the network's input:
+    ``"host"`` (cv2, the default) or ``"device"`` (``spg_prenet``)."""
+    global _limbs, _device, _variant, _input_stage
+    if input_stage is not None:
+        if input_stage not in ("host", "device"):
+            raise ValueError("input_stage must be 'host' or 'device'")
+        _input_stage = input_stage
     if limbs is not None:
         _limbs = tuple((int(a), int(b)) for a, b in limbs)
     if device is not None:
@@ -114,20 +120,66 @@ def pad_right_down_corner(img: np.ndarray, stride: int, pad_value: int) -> Tuple
     return np.pad(img, ((0, pad[2]), (0, pad[3]), (0, 0)), constant_values=pad_value), pad
 
 
-def predict(image, params, model, model_params, heat_layers=None, paf_layers=None, input_image_path=None):
+#: pinned staging of the uint8 image for ``predict(input_stage="device")`` and the event of its last upload
+_staging: Dict[str, object] = {}
+
+
+def _upload_image(image: np.ndarray):
+    """Host uint8 ``[H, W, 3]`` image -> CUDA tensor, through a pinned buffer that grows on demand (one copy, async)."""
+    import torch
+    arr = np.ascontiguousarray(image, np.uint8)
+    buf, ev = _staging.get("buf"), _staging.get("event")
+    if ev is not None:
+        ev.synchronize()  # the previous upload has left the buffer
+    if buf is None or buf.numel() < arr.size:
+        buf = torch.empty(arr.size, dtype=torch.uint8, pin_memory=True)
+        _staging["buf"] = buf
+    host = buf[:arr.size].view(arr.shape)
+    host.numpy()[...] = arr
+    dev = host.to(f"cuda:{_device}", non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(_device))
+    _staging["event"] = ev
+    return dev
+
+
+def predict(image, params, model, model_params, heat_layers=None, paf_layers=None, input_image_path=None,
+            input_stage: Optional[str] = None):
     """evaluate.py:83-166 with everything after the forward pass on the device.
 
     Same arguments as the reference's ``predict``.  For every item of ``product(multiplier, rotate_angle)`` (:87-90) the
-    image is scaled, padded and -- for ``angle != 0`` -- rotated exactly as there (cv2, host, :98-117), and the network
-    runs on it and its mirror (:118-124).  The flip ensemble, both bicubic resizes, the inverse rotation of the maps, the
-    crop and the float64 average over the items (:126-161) happen in ``spg_postnet_rotated`` -- the maps never visit the
-    host.  Returns two ``DeviceMaps`` (heatmap, paf) that ``find_peaks`` / ``find_connections`` / ``group`` accept."""
+    image is scaled, padded and -- for ``angle != 0`` -- rotated exactly as there, and the network runs on it and its
+    mirror (:118-124).  With ``input_stage="host"`` (the default, see ``configure``) that input is built with cv2 on
+    the host (:98-117); with ``"device"`` the uint8 image goes up once (``image`` may also be a uint8 CUDA tensor) and
+    ``spg_prenet`` builds every item's pair on the GPU, with OpenCV's generic resize path (the IPP build of the
+    reference's wheels differs from it by at most 1 LSB in some pixels).  The flip ensemble, both bicubic resizes, the
+    inverse rotation of the maps, the crop and the float64 average over the items (:126-161) happen in
+    ``spg_postnet_rotated`` -- the maps never visit the host.  Returns two ``DeviceMaps`` (heatmap, paf) that
+    ``find_peaks`` / ``find_connections`` / ``group`` accept."""
     import itertools
 
-    import cv2
     import torch
+    stage = _input_stage if input_stage is None else input_stage
+    if stage not in ("host", "device"):
+        raise ValueError("input_stage must be 'host' or 'device'")
     g = _grouper()
     multiplier = [x * model_params["boxsize"] / image.shape[0] for x in params["scale_search"]]
+    if stage == "device":
+        img = image if isinstance(image, torch.Tensor) else _upload_image(image)
+        items = g.prenet(img.to(f"cuda:{_device}"), multiplier, params["rotation_search"],
+                         max_downsample=int(model_params["max_downsample"]), pad_value=int(model_params["padValue"]))
+        outs = []
+        for pair, _, _ in items:
+            with torch.no_grad():
+                out = model(pair)[-1][0]  # last stack, finest scale (:126)
+            if out.dtype not in (torch.float32, torch.float16):
+                out = out.float()
+            outs.append(out[None].contiguous())
+        heat, paf = g.postnet(outs, [c for _, c, _ in items], tuple(int(v) for v in image.shape[:2]),
+                              stride=int(model_params["stride"]), nan_scrub=_variant == "demo",
+                              rotations=[r for _, _, r in items])
+        return DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)
+    import cv2
     outs, crops, rotations = [], [], []
     for scale, angle in itertools.product(multiplier, params["rotation_search"]):
         if scale * image.shape[0] > 2600 or scale * image.shape[1] > 3800:  # evaluate.py:94-96
@@ -300,13 +352,14 @@ def keypoint_heatmap_nms(heat, kernel: int = 3, thre: float = 0.1):
     return out.to(heat.device)
 
 
-def install(evaluate_module, device_predict: bool = False) -> None:
+def install(evaluate_module, device_predict: bool = False, device_input: bool = False) -> None:
     """Rebind ``find_peaks / find_connections / find_people`` of an imported reference ``evaluate`` module.
 
     ``limbSeq`` is taken from the module (evaluate.py:54) so alternative skeletons keep working.  With
     ``device_predict`` the module's ``predict`` (:83-166) is replaced as well: the network of the module (the global
-    ``posenet`` the reference's own predict uses, :124) feeds the device post-network stage and the maps stay on the GPU."""
-    configure(limbs=getattr(evaluate_module, "limbSeq", _limbs))
+    ``posenet`` the reference's own predict uses, :124) feeds the device post-network stage and the maps stay on the GPU.
+    ``device_input`` (with ``device_predict``) also builds the network's input on the GPU (``input_stage="device"``)."""
+    configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host")
     evaluate_module.find_peaks = find_peaks
     evaluate_module.find_connections = find_connections
     evaluate_module.find_people = find_people

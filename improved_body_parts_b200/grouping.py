@@ -31,7 +31,7 @@ EXPORTS = (
     "spg_download_people", "spg_download_status", "spg_launch_count", "spg_stage_kernel", "spg_wire_record_bytes",
     "spg_set_wire_output", "spg_wire_create", "spg_wire_open", "spg_wire_close", "spg_wire_destroy", "spg_wire_signal",
     "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal",
-    "spg_postnet_rotated")
+    "spg_postnet_rotated", "spg_prenet")
 
 
 class GroupingError(RuntimeError):
@@ -65,6 +65,11 @@ class _PostnetDesc(C.Structure):
 
 class _PostnetRotation(C.Structure):
     _fields_ = [("apply", C.c_int32), ("reserved", C.c_int32), ("matrix", C.c_double * 6)]
+
+
+class _PrenetItem(C.Structure):
+    _fields_ = [("scale", C.c_double), ("rotate", C.c_int32), ("reserved", C.c_int32), ("matrix", C.c_double * 6),
+                ("out", C.c_void_p), ("out_image_stride", C.c_int64)]
 
 
 class _DeviceView(C.Structure):
@@ -107,6 +112,8 @@ def load_library() -> C.CDLL:
         lib.spg_wire_wait.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
         lib.spg_postnet_rotated.argtypes = [C.c_void_p, C.POINTER(_PostnetDesc), C.POINTER(_PostnetRotation), C.c_int32,
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+        lib.spg_prenet.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_int32, C.POINTER(_PrenetItem), C.c_int32, C.c_void_p]
         if lib.spg_abi_version() != ABI_VERSION:
             raise GroupingError("libspgroup.so ABI version mismatch")
         _lib = lib
@@ -491,6 +498,71 @@ class Grouper:
                                            C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
         self._check(rc, "spg_postnet_rotated")
         return heat_out, paf_out
+
+    # -- pre-network stage ----------------------------------------------------------------------------
+    @property
+    def prenet_kernel(self) -> str:
+        """Name of the kernel the last pre-network launch used (``""`` before the first)."""
+        return (self._lib.spg_stage_kernel(self._h, 5) or b"").decode()
+
+    def prenet(self, image, scales, angles, *, max_downsample: int, pad_value: int, out=None, stream=None):
+        """The item loop of ``predict()`` before the forward pass (evaluate.py:94-121) on the device.
+
+        ``image``: ``[N, H, W, 3]`` or ``[H, W, 3]`` uint8 CUDA tensor (BGR as read) with contiguous rows; ``scales`` the
+        reference's ``multiplier`` and ``angles`` its ``rotate_angle``: one item per entry of ``product(scales, angles)``
+        (:90), each scale clamped as at :94-96.  ``out``: optional per-item output tensors to reuse.  Returns per item
+        ``(pair, crop, rotate_matrix_reverse)``: ``pair`` the ``[N, 2, Hp, Wp, 3]`` float32 tensor the network receives
+        (image, mirror; ``[2, Hp, Wp, 3]`` for a 3-D ``image``), ``crop`` = ``imageToTest.shape[:2]`` and the reverse
+        matrix (``None`` for angle 0) -- the ``crops`` and ``rotations`` ``postnet`` takes.  Asynchronous on ``stream``.
+        """
+        import itertools
+
+        import torch
+        if not getattr(image, "is_cuda", False) or image.dtype != torch.uint8 or image.dim() not in (3, 4):
+            raise GroupingError("image must be a [N,H,W,3] or [H,W,3] uint8 CUDA tensor")
+        if image.device.index != self.device:
+            raise GroupingError(f"image lives on cuda:{image.device.index}, the handle on cuda:{self.device}")
+        batched = image.dim() == 4
+        img = image if batched else image[None]
+        N, h, w, cn = (int(v) for v in img.shape)
+        if cn != 3 or img.stride(3) != 1 or img.stride(2) != 3:
+            raise GroupingError("image must have 3 channels and contiguous rows (channel stride 1, pixel stride 3)")
+        md, pv = int(max_downsample), int(pad_value)
+        if md < 1:
+            raise GroupingError("max_downsample must be >= 1")
+        pairs = list(itertools.product(scales, angles))
+        if out is not None and len(out) != len(pairs):
+            raise GroupingError("one output tensor per item expected")
+        items = (_PrenetItem * max(len(pairs), 1))()
+        dev = torch.device("cuda", self.device)
+        results = []
+        for t, (scale, angle) in enumerate(pairs):
+            scale = float(scale)
+            if scale * h > 2600 or scale * w > 3800:  # evaluate.py:94-96
+                scale = min(2600 / h, 3800 / w)
+            # the library checks the scale and the geometry; this only sizes the output
+            H1, W1 = (int(np.rint(h * scale)), int(np.rint(w * scale))) if np.isfinite(scale) and scale > 0 else (0, 0)
+            Hp, Wp = -(-H1 // md) * md, -(-W1 // md) * md
+            forward = reverse = None
+            if angle != 0:  # evaluate.py:108-110, the centre's x and y swapped as there
+                import cv2
+                centre = (Hp / 2, Wp / 2)
+                forward, reverse = cv2.getRotationMatrix2D(centre, angle, 1), cv2.getRotationMatrix2D(centre, -angle, 1)
+            if out is not None:
+                o = out[t] if batched else out[t][None]
+                if o.dtype != torch.float32 or not o.is_cuda or o.device.index != self.device or \
+                        tuple(o.shape) != (N, 2, max(Hp, 0), max(Wp, 0), 3) or not o[0].is_contiguous():
+                    raise GroupingError(f"out[{t}] must be a float32 [N,2,{Hp},{Wp},3] CUDA tensor with contiguous images")
+            else:
+                o = torch.empty((N, 2, max(Hp, 0), max(Wp, 0), 3), dtype=torch.float32, device=dev)
+            m = (C.c_double * 6)(*(np.asarray(forward, np.float64).reshape(6).tolist() if forward is not None else [0.0] * 6))
+            items[t] = _PrenetItem(scale, int(forward is not None), 0, m, o.data_ptr(), o.stride(0))
+            results.append((o if batched else o[0], (H1, W1), reverse))
+        rc = self._lib.spg_prenet(self._h, C.c_void_p(img.data_ptr()), C.c_int64(img.stride(0)), C.c_int64(img.stride(1)),
+                                  C.c_int32(N), C.c_int32(h), C.c_int32(w), C.c_int32(md), C.c_int32(pv), items,
+                                  C.c_int32(len(pairs)), self._stream_ptr(stream))
+        self._check(rc, "spg_prenet")
+        return results
 
     # -- stages -------------------------------------------------------------------------------------
     def nms_peaks(self, heat, params=None, stream=None) -> None:

@@ -174,6 +174,28 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *desc, const spg_p
                         int32_t n_images, int32_t height, int32_t width, float *heat_out, void *paf_out,
                         int32_t paf_dtype, void *stream);
 
+/* ---- pre-network stage: the item loop of predict() before the forward pass, evaluate.py:94-121 ------------ */
+/* One (scale, angle) item of product(multiplier, rotate_angle) (evaluate.py:90). */
+typedef struct spg_prenet_item {
+    double scale;               /* fx = fy of cv2.resize, after the 2600 / 3800 clamp (evaluate.py:94-96) */
+    int32_t rotate;             /* 0: angle == 0, no warp; 1: cv2.warpAffine(input_img, matrix, (0, 0)) (:108-111) */
+    int32_t reserved;           /* 0 */
+    double matrix[6];           /* row-major 2x3 FORWARD matrix evaluate.py:109 passes to warpAffine (rotate_matrix) */
+    float *out;                 /* [n_images][2][Hp][Wp][3] float32: the image, then its mirror (:116-119) */
+    int64_t out_image_stride;   /* elements between images (>= 2 * Hp * Wp * 3 when n_images > 1) */
+} spg_prenet_item;
+/* image_dev [n_images][height][width][3] uint8 (BGR as read), rows of width * 3 contiguous bytes row_stride bytes apart,
+ * images image_stride bytes apart.  Per item: cv2.resize(image, (0, 0), fx=scale, fy=scale, INTER_CUBIC) to
+ * H1 = cvRound(height * scale) x W1 = cvRound(width * scale) (:98), padded below / right with pad_value to
+ * Hp x Wp, multiples of max_downsample (:99-100), divided by 255 in float32 (:105), warped for rotate = 1 (the padded
+ * grid, taps outside it read 0) and mirrored.  The resize follows OpenCV's GENERIC uint8 path bit for bit (the IPP build
+ * differs by at most 1 LSB); the warp follows its fixed-point algorithm bit for bit.  The library computes the geometry;
+ * the host inverts the matrix in warpAffine's operation order.  Asynchronous on `stream`; a handle-owned scratch grid
+ * for rotated items grows on demand and lives until spg_destroy. */
+int spg_prenet(spg_handle *h, const uint8_t *image_dev, int64_t image_stride, int64_t row_stride, int32_t n_images,
+               int32_t height, int32_t width, int32_t max_downsample, int32_t pad_value, const spg_prenet_item *items,
+               int32_t n_items, void *stream);
+
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
 int spg_nms_peaks(spg_handle *h, const float *heat_dev, int64_t image_stride, int64_t chan_stride,
@@ -258,7 +280,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage);
+ * 4 post-network stage, 5 pre-network stage);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 
