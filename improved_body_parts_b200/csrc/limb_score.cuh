@@ -292,8 +292,11 @@ __host__ __device__ inline float f32_not_above(double t) {
     return f;
 }
 
-template <typename T, bool STAGE, typename TA = T>
-__global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs a) {
+// The per-limb schedule: the CTA scores limb k of image n_local of `a` (plane a.paf + n_local * img_stride +
+// k * chan_stride, geometry a.H x a.W, a.image_extent) and writes to slot a.image_base + n_local.  `ws` is a.ws, passed
+// apart so that a kernel's per-CTA copy of the arguments never has its limb table indexed (that would put it in local memory).
+template <typename T, bool STAGE, typename TA>
+__device__ __forceinline__ void limb_score_plane(const ScoreArgs &a, const Workspace &ws, int n_local, int k) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t bar;
     __shared__ int s_count;
@@ -301,10 +304,7 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
     __shared__ int s_total_surv;
     __shared__ uint32_t s_magic;
 
-    const Workspace &ws = a.ws;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int k = blockIdx.x % ws.L;
-    const int n_local = blockIdx.x / ws.L;
     const int n = a.image_base + n_local;
     const int H = a.H, W = a.W, capP = ws.capP;
     // Start the plane copy before anything that depends on a global load: it is the longest latency of the CTA.
@@ -485,6 +485,38 @@ __global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs 
     }
     __syncthreads();
     if (tid == 0) publish_limb(ws, n, slot, s_count, total_surv, s_flags);
+}
+
+template <typename T, bool STAGE, typename TA = T>
+__global__ void __launch_bounds__(kScoreThreads, 3) limb_score_kernel(ScoreArgs a) {
+    limb_score_plane<T, STAGE, TA>(a, a.ws, blockIdx.x / a.ws.L, blockIdx.x % a.ws.L);
+}
+
+// ---- ragged batches: images of different sizes in one launch (the counterpart of nms_peaks_ragged_kernel) ----
+struct ScoreImage {
+    const void *paf;
+    int64_t chan_stride;  // elements
+    double image_extent;
+    int H, W, slot;
+};
+constexpr int kScoreRaggedMaxImages = 128;  // ScoreArgs + 128 x 40 B of kernel parameter
+struct ScoreRagged {
+    ScoreImage img[kScoreRaggedMaxImages];
+};
+
+// Block b: limb b % L of image r.img[b / L] (largest plane first), scored with that image's geometry and extent.
+template <typename T, bool STAGE, typename TA = T>
+__global__ void __launch_bounds__(kScoreThreads, 3) limb_score_ragged_kernel(ScoreArgs a, const __grid_constant__ ScoreRagged r) {
+    const ScoreImage &im = r.img[blockIdx.x / a.ws.L];
+    ScoreArgs b = a;  // score_pair_exact reads the extent from the arguments
+    b.paf = im.paf;
+    b.img_stride = 0;
+    b.chan_stride = im.chan_stride;
+    b.H = im.H;
+    b.W = im.W;
+    b.image_extent = im.image_extent;
+    b.image_base = im.slot;
+    limb_score_plane<T, STAGE, TA>(b, a.ws, 0, blockIdx.x % a.ws.L);
 }
 
 }  // namespace spg

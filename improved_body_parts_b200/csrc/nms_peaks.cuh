@@ -221,15 +221,15 @@ __device__ __forceinline__ void nms_finish_plane(const NmsArgs &a, const uint32_
     if (lane == 0) nms_publish_count(a, a.image_base + n_local, c, total);
 }
 
-__global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
+// The per-plane schedule: the CTA finds the peaks of part c of image n_local of `a` (plane a.heat + n_local * img_stride
+// + c * chan_stride, geometry a.H x a.W in bands of a.band_rows) and writes them to slot a.image_base + n_local.
+__device__ __forceinline__ void nms_peaks_plane(const NmsArgs &a, int n_local, int c) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t bar[kNmsBufs];
     __shared__ int s_count;
 
     const Workspace &ws = a.ws;
     const int tid = threadIdx.x;
-    const int c = blockIdx.x % ws.K;
-    const int n_local = blockIdx.x / ws.K;
     const int n = a.image_base + n_local;
     const int H = a.H, W = a.W, br = a.band_rows;
     const float *plane = a.heat + (int64_t)n_local * a.img_stride + (int64_t)c * a.chan_stride;
@@ -339,6 +339,40 @@ __global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
         nms_finish_peak(a, plane, H, W, out_base + t, y, lin - y * W);
     }
     if (tid == 0) nms_publish_count(a, n, c, total);
+}
+
+__global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_kernel(NmsArgs a) {
+    nms_peaks_plane(a, blockIdx.x / a.ws.K, blockIdx.x % a.ws.K);
+}
+
+// ---- ragged batches: images of different sizes in one launch ----
+// One image of a ragged launch: its plane base, channel stride and geometry, and the slot its results go to.
+struct NmsImage {
+    const float *heat;
+    int64_t chan_stride;  // elements
+    int H, W, band_rows, use_bulk, slot;
+};
+// Images per ragged launch; the descriptors travel as a kernel parameter (NmsArgs + 128 x 40 B, well inside the
+// 32 764 bytes CUDA 12.1 allows), so a call returns with nothing of the caller's left to copy.
+constexpr int kRaggedMaxImages = 128;
+struct NmsRagged {
+    NmsImage img[kRaggedMaxImages];
+};
+
+// Block b: image r.img[b / K], part b % K.  The host orders the images by plane size, largest first, so the longest
+// CTAs enter the queue first; the order decides scheduling only.
+__global__ void __launch_bounds__(kNmsThreads, 4) nms_peaks_ragged_kernel(NmsArgs a, const __grid_constant__ NmsRagged r) {
+    const NmsImage &im = r.img[blockIdx.x / a.ws.K];
+    NmsArgs b = a;
+    b.heat = im.heat;
+    b.img_stride = 0;
+    b.chan_stride = im.chan_stride;
+    b.H = im.H;
+    b.W = im.W;
+    b.band_rows = im.band_rows;
+    b.use_bulk = im.use_bulk;
+    b.image_base = im.slot;
+    nms_peaks_plane(b, 0, blockIdx.x % a.ws.K);
 }
 
 inline size_t nms_smem_bytes(int band_rows, int H, int W, int capP) {

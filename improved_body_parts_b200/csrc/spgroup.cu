@@ -314,6 +314,33 @@ int run_all(spg_handle *h, const float *heat, int64_t his, int64_t hcs, const vo
     return SPG_OK;
 }
 
+template <typename T, bool STAGE, typename TA>
+int launch_score_ragged_t(spg_handle *h, const ScoreArgs &a, const std::vector<ScoreImage> &imgs, size_t smem,
+                          cudaStream_t st) {
+    if (imgs.empty()) return SPG_OK;
+    if (STAGE) SPG_CUDA(h, (cudaFuncSetAttribute(limb_score_ragged_kernel<T, STAGE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
+    for (size_t i0 = 0; i0 < imgs.size(); i0 += kScoreRaggedMaxImages) {
+        const int cnt = (int)std::min<size_t>(kScoreRaggedMaxImages, imgs.size() - i0);
+        ScoreRagged r{};
+        std::copy(imgs.begin() + i0, imgs.begin() + i0 + cnt, r.img);
+        limb_score_ragged_kernel<T, STAGE, TA><<<cnt * h->ws.L, kScoreThreads, smem, st>>>(a, r);
+        h->launches++;
+        SPG_CUDA(h, cudaGetLastError());
+    }
+    h->stage_kernel[1] = sizeof(T) == 8 ? (STAGE ? "limb_score_ragged_kernel<double,true>" : "limb_score_ragged_kernel<double,false>")
+                         : sizeof(TA) == 4 ? (STAGE ? "limb_score_ragged_kernel<float,true>" : "limb_score_ragged_kernel<float,false>")
+                                           : (STAGE ? "limb_score_ragged_kernel<float,true,double>" : "limb_score_ragged_kernel<float,false,double>");
+    return SPG_OK;
+}
+
+template <typename T, typename TA = T>
+int launch_score_ragged(spg_handle *h, const ScoreArgs &a, const std::vector<ScoreImage> &staged, size_t staged_smem,
+                        const std::vector<ScoreImage> &sampled, cudaStream_t st) {
+    int rc;
+    if ((rc = launch_score_ragged_t<T, true, TA>(h, a, staged, staged_smem, st))) return rc;
+    return launch_score_ragged_t<T, false, TA>(h, a, sampled, score_smem_bytes(0, h->ws.capP), st);
+}
+
 __global__ void wire_signal_kernel(unsigned long long *word, unsigned long long value) {
     __threadfence_system();  // everything earlier on the stream has completed; order it before the flag for every observer
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(word), "l"(value) : "memory");
@@ -966,6 +993,101 @@ int spg_group_batch(spg_handle *h, const float *heat, int64_t his, int64_t hcs, 
     if ((rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = run_all(h, heat, his, hcs, paf, dtype, pis, pcs, 0, n, H, W, extent, p, static_cast<cudaStream_t>(stream)))) return rc;
+    h->stage = 4;
+    return SPG_OK;
+}
+
+// ---- ragged batches --------------------------------------------------------------------------------
+// K1 and K2a run their per-plane schedules with the geometry taken per image from descriptors passed as kernel
+// parameters; match_assemble reads no geometry and runs as for spg_group_batch.  Images go into each launch largest
+// plane first (longest job first over the CTA queue); every CTA writes to its image's own slot.
+int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int32_t dtype, const spg_params *p, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images %d outside [0, max_batch=%d]", n, h->cfg.max_batch);
+    if (!images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
+    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
+    int rc;
+    if ((rc = check_params(h, p))) return rc;
+    const Workspace &ws = h->ws;
+    const size_t esz = dtype == SPG_F64 ? 8 : 4;
+    const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
+    // validate every image and build the descriptors before the first launch
+    std::vector<int> order((size_t)n);
+    for (int i = 0; i < n; i++) {
+        const spg_image_maps &im = images[i];
+        if (!im.heat || !im.paf) return fail(h, SPG_E_INVALID, "image %d: heat/paf is NULL", i);
+        if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
+            return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
+        const int br = std::max(4, std::min((int)im.height, 4096 / (int)im.width));
+        const size_t smem = nms_smem_bytes(br, im.height, im.width, ws.capP);
+        if (smem > h->smem_optin)
+            return fail(h, SPG_E_INVALID, "image %d: map width %d needs %zu B of shared memory per band (limit %zu)", i, im.width, smem, h->smem_optin);
+        order[i] = i;
+    }
+    if (score_smem_bytes(0, ws.capP) > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need too much shared memory in limb scoring");
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
+        return (int64_t)images[x].height * images[x].width > (int64_t)images[y].height * images[y].width;
+    });
+    std::vector<NmsImage> nms;
+    std::vector<ScoreImage> staged, sampled;
+    size_t nms_smem = 0, staged_smem = 0;
+    nms.reserve(n);
+    for (int i : order) {
+        const spg_image_maps &im = images[i];
+        const int H = im.height, W = im.width;
+        NmsImage d{};
+        d.heat = im.heat; d.chan_stride = im.heat_chan_stride; d.H = H; d.W = W; d.slot = i;
+        d.band_rows = std::max(4, std::min(H, 4096 / W));
+        d.use_bulk = (W % 4 == 0) && (im.heat_chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(im.heat) & 15) == 0);
+        nms_smem = std::max(nms_smem, nms_smem_bytes(d.band_rows, H, W, ws.capP));
+        nms.push_back(d);
+        ScoreImage s{};
+        s.paf = im.paf; s.chan_stride = im.paf_chan_stride; s.image_extent = im.image_extent; s.H = H; s.W = W; s.slot = i;
+        // the conditions of launch_score_t's staged kernel, per image
+        const size_t plane_bytes = (size_t)H * W * esz, smem = score_smem_bytes(plane_bytes, ws.capP);
+        const bool aligned = (plane_bytes % 16 == 0) && ((im.paf_chan_stride * esz) % 16 == 0) &&
+                             ((reinterpret_cast<uintptr_t>(im.paf) & 15) == 0) && plane_bytes < (1u << 20);
+        if (aligned && smem <= h->smem_optin) {
+            staged.push_back(s);
+            staged_smem = std::max(staged_smem, smem);
+        } else {
+            sampled.push_back(s);
+        }
+    }
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SPG_CUDA(h, cudaMemsetAsync(ws.status, 0, sizeof(uint32_t) * (size_t)n, st));
+    if (n == 0) return SPG_OK;
+    NmsArgs na{};
+    na.radius = p->offset_radius;
+    na.thr = (float)p->thre1;
+    na.ws = ws;
+    SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_ragged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nms_smem));
+    for (size_t i0 = 0; i0 < nms.size(); i0 += kRaggedMaxImages) {
+        const int cnt = (int)std::min<size_t>(kRaggedMaxImages, nms.size() - i0);
+        NmsRagged r{};
+        std::copy(nms.begin() + i0, nms.begin() + i0 + cnt, r.img);
+        nms_peaks_ragged_kernel<<<cnt * ws.K, kNmsThreads, nms_smem, st>>>(na, r);
+        h->launches++;
+        SPG_CUDA(h, cudaGetLastError());
+    }
+    h->stage_kernel[0] = "nms_peaks_ragged_kernel";
+    ScoreArgs sa{};
+    sa.mid_num = p->mid_num;
+    sa.thre2 = p->thre2;
+    sa.connect_ration = p->connect_ration;
+    sa.screen = h->screen;
+    sa.crit1_strict = p->crit1_strict != 0;
+    sa.exact_warps = h->exact_warps;
+    sa.ws = ws;
+    h->cand_dtype = dtype;
+    if (dtype == SPG_F64) rc = launch_score_ragged<double>(h, sa, staged, staged_smem, sampled, st);
+    else if (dtype == SPG_F32_AS_F64) rc = launch_score_ragged<float, double>(h, sa, staged, staged_smem, sampled, st);
+    else rc = launch_score_ragged<float>(h, sa, staged, staged_smem, sampled, st);
+    if (rc) return rc;
+    if (h->fuse_ma) rc = launch_match_assemble(h, 0, n, p, st);
+    else if (!(rc = launch_match(h, 0, n, st))) rc = launch_assemble(h, 0, n, p, st);
+    if (rc) return rc;
     h->stage = 4;
     return SPG_OK;
 }

@@ -30,6 +30,7 @@ _device = 0
 _variant = "evaluate"
 _input_stage = "host"
 _groupers: Dict[int, Grouper] = {}
+_ragged: Dict[int, Grouper] = {}  # the handle of the batched calls (group_many / predict_many), per device
 CAP_PEAKS, CAP_CANDS, CAP_ROWS = 128, 4096, 128
 MAX_DIM = 32767  # the C ABI's limit; the workspace does not depend on the map size, so ONE handle serves every image size
 
@@ -53,9 +54,10 @@ def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optiona
         if variant not in ("evaluate", "demo"):
             raise ValueError("variant must be 'evaluate' or 'demo'")
         _variant = variant
-    for g in _groupers.values():
+    for g in list(_groupers.values()) + list(_ragged.values()):
         g.close()
     _groupers.clear()
+    _ragged.clear()
 
 
 def _grouper(H: int = 0, W: int = 0) -> Grouper:
@@ -69,6 +71,19 @@ def _grouper(H: int = 0, W: int = 0) -> Grouper:
     return g
 
 
+def _grouper_many(n: int) -> Grouper:
+    """The handle of the batched calls on the current device; its max_batch grows on demand (the max_batch=1 handle of
+    the three call-site functions stays as it is)."""
+    g = _ragged.get(_device)
+    if g is None or g.max_batch < n:
+        if g is not None:
+            g.close()
+        g = Grouper(_limbs, NUM_PARTS, COCO_FROM_PART, max_batch=max(int(n), 1), max_h=MAX_DIM, max_w=MAX_DIM,
+                    max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS, device=_device)
+        _ragged[_device] = g
+    return g
+
+
 def _params(params):
     """The reference's params dict -> what the library runs with (the demo variant adds its three deviations)."""
     if isinstance(params, GroupParams):
@@ -76,9 +91,13 @@ def _params(params):
     return GroupParams.demo(params) if _variant == "demo" else params
 
 
-def _check(r: GroupResult) -> None:
-    if r.status[0]:
-        raise GroupingError(f"grouping capacity exceeded or invalid sample index (status {int(r.status[0]):#x}); "
+def _check(r: GroupResult, n: int = 0) -> None:
+    _check_status(int(r.status[n]))
+
+
+def _check_status(status: int) -> None:
+    if status:
+        raise GroupingError(f"grouping capacity exceeded or invalid sample index (status {status:#x}); "
                             f"capacities: {CAP_PEAKS} peaks/part, {CAP_CANDS} candidates/limb, {CAP_ROWS} person rows")
 
 
@@ -310,6 +329,115 @@ def group(heatmap_avg, paf_avg, image_extent, params):
     return r.as_reference_structures(0)
 
 
+def _ragged_maps(maps):
+    """(heat, paf) pairs of ``DeviceMaps`` or host ``[H, W, C]`` arrays -> device tensors + whether paf is float32
+    storage of float64 values (one answer for the whole call)."""
+    pairs, as_f64 = [], set()
+    for heat, paf in maps:
+        if isinstance(heat, DeviceMaps):
+            h = heat.tensor
+        else:
+            h = _maps_to_device(heat, NUM_PARTS, np.float32)
+        if isinstance(paf, DeviceMaps):
+            p = paf.tensor
+            as_f64.add(paf.as_f64)
+        else:
+            p = _maps_to_device(paf, len(_limbs), np.float64 if np.asarray(paf).dtype == np.float64 else np.float32)
+            as_f64.add(False)
+        pairs.append((h, p))
+    if len(as_f64) > 1:
+        raise GroupingError("the body-part maps of one call must all be float32, float32-held float64 or float64")
+    return pairs, as_f64 == {True}
+
+
+def group_many(maps, image_extents, params):
+    """``group()`` for several images of different sizes in ONE grouping call (``spg_group_ragged``) and one download.
+
+    ``maps``: per image a ``(heatmap_avg, paf_avg)`` pair -- the ``DeviceMaps`` ``predict`` returns or host ``[H, W, C]``
+    arrays; ``image_extents``: per image ``oriImg.shape[0]``.  Returns one ``(all_peaks, connection_all, special_k,
+    subset, candidate)`` per image, equal to what ``group()`` returns for it."""
+    pairs, as_f64 = _ragged_maps(maps)
+    g = _grouper_many(len(pairs))
+    _state.clear()
+    g.group_ragged(pairs, image_extents, _params(params), paf_as_f64=as_f64)
+    r = g.fetch(len(pairs))
+    out = []
+    for i in range(len(pairs)):
+        _check(r, i)
+        out.append(r.as_reference_structures(i))
+    return out
+
+
+#: device buffers of the wire records ``predict_many`` downloads, per device
+_records: Dict[int, object] = {}
+
+
+def _people_of_batch(maps, extents, params) -> list:
+    """One ragged grouping call for a batch of images, their wire records in one device-to-host copy, and per image
+    ``process()``'s return value (evaluate.py:523-543)."""
+    import torch
+
+    from . import wire
+    pairs, as_f64 = _ragged_maps(maps)
+    g = _grouper_many(len(pairs))
+    rec_bytes = g.wire_record_bytes()
+    buf = _records.get(_device)
+    if buf is None or buf.shape[0] < len(pairs) or buf.shape[1] != rec_bytes:
+        buf = torch.empty((max(len(pairs), g.max_batch), rec_bytes), dtype=torch.uint8, device=f"cuda:{_device}")
+        _records[_device] = buf
+    _state.clear()
+    g.set_wire_output(buf.data_ptr())
+    try:
+        g.group_ragged(pairs, extents, _params(params), paf_as_f64=as_f64)
+    finally:
+        g.set_wire_output(None)
+    recs = wire.as_records(buf[:len(pairs)].cpu().numpy(), g.J, g.capR)
+    out = []
+    for rec in recs:
+        _check_status(int(rec["status"]))
+        out.append(wire.people_of(rec))
+    return out
+
+
+def predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers,
+                 batch: int = 16, image_name=None):
+    """evaluate.py:550-560 with the grouping of ``batch`` images at a time in one call.
+
+    Same arguments, assert and result as the reference's ``predict_many``: ``{image_id: [([17 x (x, y)], score)]}`` in
+    ``validation_ids`` order, with ``np.float64`` coordinates and scores and integer ``(0, 0)`` for a missing joint, so
+    ``format_results`` writes the same file.  Per image: ``cv2.imread`` and ``predict`` (the maps stay on the device);
+    every ``batch`` images and at the end: one ``group_many``-style ragged call, the batch's wire records in one copy.
+    A non-zero status raises ``GroupingError``.  ``image_name(coco, image_id)`` gives the file name (default:
+    ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()`` is not called, so the reference's
+    ``batch_time`` meter is not updated."""
+    import os
+
+    import cv2
+    assert (not set(validation_ids).difference(set(coco.getImgIds())))
+    if int(batch) < 1:
+        raise ValueError("batch must be >= 1")
+    keypoints = {}
+    pending = []  # (image_id, heatmap, paf, oriImg.shape[0])
+
+    def flush():
+        if pending:
+            people = _people_of_batch([(h, p) for _, h, p, _ in pending], [e for _, _, _, e in pending], params)
+            for (iid, _, _, _), kp in zip(pending, people):
+                keypoints[iid] = kp
+            pending.clear()
+
+    for image_id in validation_ids:
+        name = image_name(coco, image_id) if image_name is not None else coco.imgs[image_id]["file_name"]
+        path = os.path.join(images_directory, name)
+        ori = cv2.imread(path)  # B,G,R order (evaluate.py:502)
+        heat, paf = predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path)
+        pending.append((image_id, heat, paf, ori.shape[0]))
+        if len(pending) >= int(batch):
+            flush()
+    flush()
+    return keypoints
+
+
 def keypoints(subset, candidate):
     """Tail of process() (evaluate.py:523-543): [(17 x (x, y) in COCO order, score)]."""
     out = []
@@ -352,13 +480,18 @@ def keypoint_heatmap_nms(heat, kernel: int = 3, thre: float = 0.1):
     return out.to(heat.device)
 
 
-def install(evaluate_module, device_predict: bool = False, device_input: bool = False) -> None:
+def install(evaluate_module, device_predict: bool = False, device_input: bool = False, batch: int = 1) -> None:
     """Rebind ``find_peaks / find_connections / find_people`` of an imported reference ``evaluate`` module.
 
     ``limbSeq`` is taken from the module (evaluate.py:54) so alternative skeletons keep working.  With
     ``device_predict`` the module's ``predict`` (:83-166) is replaced as well: the network of the module (the global
     ``posenet`` the reference's own predict uses, :124) feeds the device post-network stage and the maps stay on the GPU.
-    ``device_input`` (with ``device_predict``) also builds the network's input on the GPU (``input_stage="device"``)."""
+    ``device_input`` (with ``device_predict``) also builds the network's input on the GPU (``input_stage="device"``).
+    ``batch > 1`` (with ``device_predict``) also replaces ``predict_many`` (:550-560) by ``predict_many`` above, which
+    groups ``batch`` images per call; it uses the module's ``posenet`` and ``get_image_name`` and leaves the module's
+    ``batch_time`` meter alone."""
+    if int(batch) > 1 and not device_predict:
+        raise ValueError("batch > 1 needs device_predict=True: the batched grouping takes the maps predict() leaves on the device")
     configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host")
     evaluate_module.find_peaks = find_peaks
     evaluate_module.find_connections = find_connections
@@ -368,3 +501,9 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
             return predict(image, params, getattr(evaluate_module, "posenet", model), model_params, heat_layers,
                            paf_layers, input_image_path)
         evaluate_module.predict = _predict
+    if int(batch) > 1:
+        def _predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers):
+            return predict_many(coco, images_directory, validation_ids, params, getattr(evaluate_module, "posenet", model),
+                                model_params, heat_layers, paf_layers, batch=int(batch),
+                                image_name=getattr(evaluate_module, "get_image_name", None))
+        evaluate_module.predict_many = _predict_many

@@ -31,7 +31,7 @@ EXPORTS = (
     "spg_download_people", "spg_download_status", "spg_launch_count", "spg_stage_kernel", "spg_wire_record_bytes",
     "spg_set_wire_output", "spg_wire_create", "spg_wire_open", "spg_wire_close", "spg_wire_destroy", "spg_wire_signal",
     "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal",
-    "spg_postnet_rotated", "spg_prenet")
+    "spg_postnet_rotated", "spg_prenet", "spg_group_ragged")
 
 
 class GroupingError(RuntimeError):
@@ -70,6 +70,11 @@ class _PostnetRotation(C.Structure):
 class _PrenetItem(C.Structure):
     _fields_ = [("scale", C.c_double), ("rotate", C.c_int32), ("reserved", C.c_int32), ("matrix", C.c_double * 6),
                 ("out", C.c_void_p), ("out_image_stride", C.c_int64)]
+
+
+class _ImageMaps(C.Structure):
+    _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
+                ("paf_chan_stride", C.c_int64), ("height", C.c_int32), ("width", C.c_int32), ("image_extent", C.c_double)]
 
 
 class _DeviceView(C.Structure):
@@ -114,6 +119,8 @@ def load_library() -> C.CDLL:
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
         lib.spg_prenet.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.POINTER(_PrenetItem), C.c_int32, C.c_void_p]
+        lib.spg_group_ragged.argtypes = [C.c_void_p, C.POINTER(_ImageMaps), C.c_int32, C.c_int32, C.POINTER(_Params),
+                                         C.c_void_p]
         if lib.spg_abi_version() != ABI_VERSION:
             raise GroupingError("libspgroup.so ABI version mismatch")
         _lib = lib
@@ -404,6 +411,45 @@ class Grouper:
         self._check(rc, "spg_group_batch")
         self._peaks_shape = (N, H, W)
         self._last_n = N
+
+    def group_ragged(self, maps, image_extents, params=None, stream=None, paf_as_f64: bool = False) -> None:
+        """``group_device`` for images of different sizes in one asynchronous call; image i's results in slot i.
+
+        ``maps``: per image a ``(heat, paf)`` pair of CUDA tensors, ``[C, H, W]`` or ``[1, C, H, W]`` with contiguous
+        rows (channel slices of the network's output work), heat float32 and paf float32 / float64 -- one paf dtype for
+        the whole call.  ``image_extents``: per image the reference's ``oriImg.shape[0]``.  Each image's results equal
+        those of ``group_device`` on that image alone.  ``fetch(n)`` / ``as_reference_structures(i)`` read them back."""
+        import torch
+        maps = list(maps)
+        extents = [float(e) for e in image_extents]
+        if len(extents) != len(maps):
+            raise GroupingError(f"{len(maps)} images but {len(extents)} image extents")
+        if len(maps) > self.max_batch:
+            raise GroupingError(f"{len(maps)} images, the handle was created for {self.max_batch}")
+        arr = (_ImageMaps * max(len(maps), 1))()
+        dtype = None
+        for i, (heat, paf) in enumerate(maps):
+            heat = heat[None] if heat.dim() == 3 else heat
+            paf = paf[None] if paf.dim() == 3 else paf
+            try:
+                self._check_maps(heat, "heat", self.K, (torch.float32,))
+                self._check_maps(paf, "paf", self.L, (torch.float32, torch.float64))
+            except GroupingError as e:
+                raise GroupingError(f"image {i}: {e}") from None
+            if heat.shape[0] != 1 or paf.shape[0] != 1 or tuple(paf.shape[2:]) != tuple(heat.shape[2:]):
+                raise GroupingError(f"image {i}: heat and paf must be one image each, of the same size")
+            d = self._paf_dtype(paf, paf_as_f64)
+            if dtype is not None and d != dtype:
+                raise GroupingError(f"image {i}: every image of a call needs the same paf dtype")
+            dtype = d
+            arr[i] = _ImageMaps(heat.data_ptr(), paf.data_ptr(), heat.stride(1), paf.stride(1), heat.shape[2],
+                                heat.shape[3], extents[i])
+        p = params_struct(params)
+        rc = self._lib.spg_group_ragged(self._h, arr, C.c_int32(len(maps)), C.c_int32(F32 if dtype is None else dtype),
+                                        C.byref(p), self._stream_ptr(stream))
+        self._check(rc, "spg_group_ragged")
+        self._peaks_shape = None
+        self._last_n = len(maps)
 
     def group_host(self, heat: np.ndarray, paf: np.ndarray, image_extent: float, params=None, out=None) -> dict:
         """Host maps in, person lists out (H2D / kernels / D2H pipelined inside the library).  Synchronous.

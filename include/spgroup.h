@@ -122,6 +122,23 @@ int spg_group_batch(spg_handle *h, const float *heat_dev, int64_t heat_image_str
                     int32_t n_images, int32_t height, int32_t width, double image_extent,
                     const spg_params *params, void *stream);
 
+/* One image of a ragged call: its own maps, size and extent.  evaluate.py groups every validation image at its own
+ * resolution (process(), evaluate.py:501-543), so a batch of them has no common size. */
+typedef struct spg_image_maps {
+    const float *heat;          /* [>=K][H][W] float32, rows contiguous, planes heat_chan_stride elements apart */
+    const void *paf;            /* [>=L][H][W] of the call's paf_dtype, planes paf_chan_stride elements apart   */
+    int64_t heat_chan_stride, paf_chan_stride;
+    int32_t height, width;
+    double image_extent;        /* this image's oriImg.shape[0] (evaluate.py:510) */
+} spg_image_maps;
+
+/* peaks -> connections -> people for n_images maps of different sizes; image i's results in slot i, equal to what
+ * spg_group_batch returns for that image alone (the candidate arrays aside: they are unordered).  Every image is
+ * validated before the first launch; SPG_E_INVALID names the first bad one.  Asynchronous on `stream`; `images` may be
+ * reused as soon as the call returns.  Wire output and the armed wire signal apply as for spg_group_batch. */
+int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n_images, int32_t paf_dtype,
+                     const spg_params *params, void *stream);
+
 /* host inputs (pinned for full overlap; pageable works): H2D in chunks overlapped with the kernels, results
  * copied back into the caller's arrays (any of which may be NULL).  Synchronous.
  *   heat_host [N][K][H][W] f32, paf_host [N][L][H][W] f32|f64

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Run the reference's ``evaluate.py`` UNCHANGED with its grouping stage on the H100 path.
 
-    python tools/run_evaluate_b200.py --reference /path/to/Improved-Body-Parts [--config utils/config] [--check]
+    python tools/run_evaluate_b200.py --reference /path/to/Improved-Body-Parts [--config utils/config] [--check] [--batch N]
 
 What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is never modified:
 
@@ -11,7 +11,9 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
    and ``GetConfig``, ``:52``) and restores ``CUDA_VISIBLE_DEVICES``, which the module pins to "0" (``:28``) -- one
    process per GPU needs its own device;
 3. ``dropin.install(evaluate)``: rebinds ``evaluate.find_peaks / find_connections / find_people`` (looked up by name
-   at the call sites ``:509-511``) and takes ``limbSeq`` from the module (``:54``);
+   at the call sites ``:509-511``) and takes ``limbSeq`` from the module (``:54``); with ``--batch N`` (N > 1) it also
+   replaces ``predict`` by the device one and ``predict_many`` (``:550-560``) by ``dropin.predict_many``, which groups
+   N images per call;
 4. fills the globals ``evaluate.__main__`` would set (``:643-646``): ``params, model_params`` from the reference's own
    ``utils/config`` through ``skeleton.read_reference_ini`` (``utils/config_reader.py:7`` hard-codes the author's path),
    ``show_eval_speed``;
@@ -58,7 +60,7 @@ def _stub_missing() -> list:
 
 
 def prepare(reference_root: str, config_path: str = None, device: int = None, install: bool = True,
-            replace_format_results: bool = False):
+            replace_format_results: bool = False, batch: int = 1):
     """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites."""
     reference_root = os.path.abspath(reference_root)
     if not os.path.isfile(os.path.join(reference_root, "evaluate.py")):
@@ -85,7 +87,10 @@ def prepare(reference_root: str, config_path: str = None, device: int = None, in
     if install:
         if device is not None:
             dropin.configure(device=device)
-        dropin.install(evaluate)
+        if batch > 1:  # the batched grouping takes the maps the device predict() leaves on the GPU
+            dropin.install(evaluate, device_predict=True, batch=batch)
+        else:
+            dropin.install(evaluate)
     evaluate.params, evaluate.model_params = skeleton.read_reference_ini(
         config_path or os.path.join(reference_root, "utils", "config"))
     evaluate.show_eval_speed = False
@@ -102,8 +107,12 @@ def main() -> None:
     ap.add_argument("--config", default=None, help="the reference's utils/config INI (default: <reference>/utils/config)")
     ap.add_argument("--device", type=int, default=None)
     ap.add_argument("--check", action="store_true", help="group one synthetic image through evaluate's call sites on the GPU")
+    ap.add_argument("--batch", type=int, default=1,
+                    help="images per grouping call in predict_many (> 1 implies the device predict; default 1)")
     a = ap.parse_args()
-    ev = prepare(a.reference, a.config, a.device)
+    if a.batch < 1:
+        ap.error("--batch must be >= 1")
+    ev = prepare(a.reference, a.config, a.device, batch=a.batch)
     print(f"evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
           f"find_peaks -> {ev.find_peaks.__module__}.{ev.find_peaks.__name__}")
     if a.check:
