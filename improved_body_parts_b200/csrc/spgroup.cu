@@ -36,6 +36,15 @@ static_assert(sizeof(spg_params) == sizeof(spg::Params), "spg_params layout");
 
 static thread_local std::string g_create_error;
 
+// the stage numbers of spg_stage_kernel (include/spgroup.h)
+enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageCount };
+
+// device scratch that grows on demand (grow) and lives until spg_destroy
+struct Scratch {
+    void *p = nullptr;
+    size_t bytes = 0;
+};
+
 struct spg_handle {
     spg_config cfg{};
     int device = 0;
@@ -43,19 +52,15 @@ struct spg_handle {
     size_t smem_optin = 0;
     Workspace ws{};
     std::vector<void *> allocs;
-    // staging for spg_group_host
-    void *in_heat = nullptr, *in_paf = nullptr;
-    size_t in_heat_bytes = 0, in_paf_bytes = 0;
+    Scratch in_heat, in_paf;  // staging for spg_group_host
     unsigned int *done_counter = nullptr;          // "last CTA done" counter of the in-kernel wire signal
     unsigned long long *armed_flag = nullptr;      // spg_arm_wire_signal: consumed by the next assemble launch
     unsigned long long armed_value = 0;
-    double *heat_acc = nullptr;  // postnet: float64 accumulator of the keypoint maps over the scale loop
-    size_t heat_acc_elems = 0;
-    unsigned char *pre_grid = nullptr;  // prenet: the padded uint8 images of a rotated item, grown on demand
-    size_t pre_grid_bytes = 0;
+    Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
+    Scratch pre_grid;  // prenet: the padded uint8 images of a rotated item
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
-    const char *stage_kernel[6] = {"", "", "", "", "", ""};  // nms_peaks, limb_score, limb_match, assemble, post-, pre-network
+    const char *stage_kernel[kStageCount] = {"", "", "", "", "", ""};
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
@@ -107,8 +112,38 @@ struct DeviceGuard {
     }
 };
 
-int check_dims(spg_handle *h, int n, int H, int W) {
+int grow(spg_handle *h, Scratch &s, size_t bytes) {
+    if (s.bytes >= bytes) return SPG_OK;
+    if (s.p) cudaFree(s.p);
+    s.p = nullptr;
+    s.bytes = 0;
+    SPG_CUDA(h, cudaMalloc(&s.p, bytes));
+    s.bytes = bytes;
+    return SPG_OK;
+}
+
+// Every kernel launch on a handle goes through here: it raises the kernel's dynamic shared memory limit to `smem`,
+// launches, records `name` as the kernel of `stage` (spg_stage_kernel), counts the launch (spg_launch_count) and turns
+// a launch error into the call's error.
+template <typename... P, typename... A>
+int launch(spg_handle *h, int stage, const char *name, void (*kern)(P...), dim3 grid, int block, size_t smem, cudaStream_t st,
+           const A &...args) {
+    if (smem > 0) SPG_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, block, smem, st>>>(args...);
+    h->stage_kernel[stage] = name;
+    h->launches++;
+    SPG_CUDA(h, cudaGetLastError());
+    return SPG_OK;
+}
+
+int check_batch(spg_handle *h, int n) {
     if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images %d outside [0, max_batch=%d]", n, h->cfg.max_batch);
+    return SPG_OK;
+}
+
+int check_dims(spg_handle *h, int n, int H, int W) {
+    int rc;
+    if ((rc = check_batch(h, n))) return rc;
     if (H < 2 || W < 2 || H > h->cfg.max_h || W > h->cfg.max_w || H > 32767 || W > 32767)
         return fail(h, SPG_E_INVALID, "map %dx%d outside [2, %dx%d]", H, W, h->cfg.max_h, h->cfg.max_w);
     return SPG_OK;
@@ -122,132 +157,131 @@ int check_params(spg_handle *h, const spg_params *p) {
     return SPG_OK;
 }
 
-// ---- stage launchers on absolute image range [base, base+n) with chunk-local input pointers ----
-int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_stride, int base, int n, int H, int W,
-               const spg_params *p, cudaStream_t st) {
-    if (n == 0) return SPG_OK;
-    NmsArgs a{};
-    a.heat = heat;
-    a.img_stride = img_stride;
-    a.chan_stride = chan_stride;
-    a.H = H;
-    a.W = W;
-    a.radius = p->offset_radius;
-    a.use_bulk = (W % 4 == 0) && (img_stride % 4 == 0) && (chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(heat) & 15) == 0);
-    a.image_base = base;
-    a.thr = (float)p->thre1;
-    a.ws = h->ws;
-    if (h->persist && a.use_bulk && nms_persist_smem_bytes(H, W, h->ws.capP) <= h->smem_optin && (size_t)H * W / 4 < 65536 &&
+// the dtype of the body-part planes: an index into kScoreKernels
+int check_dtype(spg_handle *h, int dtype) {
+    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64)
+        return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
+    return SPG_OK;
+}
+
+// The limb-scoring kernels for one dtype of body-part planes, with the names spg_stage_kernel reports.  Index 0 of a
+// pair samples the planes through L2, index 1 stages each plane in shared memory.
+struct ScoreKernels {
+    size_t esz;  // bytes per plane element
+    void (*item[2])(ScoreArgs);
+    const char *item_name[2];
+    void (*ragged[2])(ScoreArgs, ScoreRagged);
+    const char *ragged_name[2];
+    void (*persist)(ScoreArgs, int);  // f32 planes only
+    const char *persist_name;
+};
+
+static_assert(SPG_F32 == 0 && SPG_F64 == 1 && SPG_F32_AS_F64 == 2, "kScoreKernels is indexed by the dtype");
+const ScoreKernels kScoreKernels[3] = {
+    {4, {limb_score_kernel<float, false>, limb_score_kernel<float, true>},
+     {"limb_score_kernel<float,false>", "limb_score_kernel<float,true>"},
+     {limb_score_ragged_kernel<float, false>, limb_score_ragged_kernel<float, true>},
+     {"limb_score_ragged_kernel<float,false>", "limb_score_ragged_kernel<float,true>"},
+     limb_score_persist_kernel<float>, "limb_score_persist_kernel<float>"},
+    {8, {limb_score_kernel<double, false>, limb_score_kernel<double, true>},
+     {"limb_score_kernel<double,false>", "limb_score_kernel<double,true>"},
+     {limb_score_ragged_kernel<double, false>, limb_score_ragged_kernel<double, true>},
+     {"limb_score_ragged_kernel<double,false>", "limb_score_ragged_kernel<double,true>"},
+     nullptr, ""},
+    {4, {limb_score_kernel<float, false, double>, limb_score_kernel<float, true, double>},
+     {"limb_score_kernel<float,false,double>", "limb_score_kernel<float,true,double>"},
+     {limb_score_ragged_kernel<float, false, double>, limb_score_ragged_kernel<float, true, double>},
+     {"limb_score_ragged_kernel<float,false,double>", "limb_score_ragged_kernel<float,true,double>"},
+     limb_score_persist_kernel<double>, "limb_score_persist_kernel<double>"},
+};
+
+// one kernel per refinement radius (check_params: 0 .. kMaxRefineRadius)
+void (*const kNmsPersistKernels[])(NmsArgs, int) = {nms_peaks_persist_kernel<0>, nms_peaks_persist_kernel<1>, nms_peaks_persist_kernel<2>,
+                                                    nms_peaks_persist_kernel<3>, nms_peaks_persist_kernel<4>};
+static_assert(kMaxRefineRadius == 4, "one nms_peaks_persist_kernel instantiation per radius");
+
+// ---- schedules: the kernel, band rows, bulk-copy flag and shared memory a stage uses for planes of one geometry ----
+// `persistent` allows the persistent kernels (one resident CTA per SM over a ring of plane or band slots; SPG_PERSIST=0
+// turns them off).  Ragged launches pass false: their CTAs take the plane geometry per image, which only the per-plane
+// kernels do.
+struct NmsPlan {
+    enum { kPersist, kBanded, kBands } kind;
+    int band_rows, use_bulk;
+    size_t smem;
+    NmsBanding bg;
+};
+
+// `image` >= 0 names the image of a ragged call in the error
+int plan_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_stride, int H, int W, bool persistent, int image,
+             NmsPlan *pl) {
+    const int capP = h->ws.capP;
+    *pl = NmsPlan{};
+    pl->use_bulk = (W % 4 == 0) && (img_stride % 4 == 0) && (chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(heat) & 15) == 0);
+    const bool persist = persistent && h->persist && pl->use_bulk;
+    if (persist && nms_persist_smem_bytes(H, W, capP) <= h->smem_optin && (size_t)H * W / 4 < 65536 &&
         (size_t)H * W * sizeof(float) < (1u << 20) &&
         ((size_t)H * W / 4 + kNmsPScanners - 1) / kNmsPScanners <= (size_t)32 * kNmsPMaxIter) {
         // one resident CTA per SM: loader, 28 scanners, 3 finishers over a ring of 3 plane slots
-        const size_t psm = nms_persist_smem_bytes(H, W, h->ws.capP);
-        const int items = n * h->ws.K;
-        void (*kern)(NmsArgs, int) = nms_peaks_persist_kernel<kMaxRefineRadius>;
-        switch (a.radius) {  // one kernel per refinement radius (check_params: 0 .. kMaxRefineRadius)
-            case 0: kern = nms_peaks_persist_kernel<0>; break;
-            case 1: kern = nms_peaks_persist_kernel<1>; break;
-            case 2: kern = nms_peaks_persist_kernel<2>; break;
-            case 3: kern = nms_peaks_persist_kernel<3>; break;
-        }
-        static_assert(kMaxRefineRadius == 4, "one nms_peaks_persist_kernel instantiation per radius");
-        SPG_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        kern<<<std::min(items, h->sm_count), kNmsPThreads, psm, st>>>(a, items);
-        h->stage_kernel[0] = "nms_peaks_persist_kernel";
-        h->launches++;
-        SPG_CUDA(h, cudaGetLastError());
+        pl->kind = NmsPlan::kPersist;
+        pl->smem = nms_persist_smem_bytes(H, W, capP);
         return SPG_OK;
     }
-    const NmsBanding bg = (h->persist && a.use_bulk) ? nms_banding(H, W, h->ws.capP, h->smem_optin - 1024) : NmsBanding{};
-    if (bg.slots >= kNmsBTeams) {
+    if (persist) pl->bg = nms_banding(H, W, capP, h->smem_optin - 1024);
+    if (pl->bg.slots >= kNmsBTeams) {
         // planes that do not fit three times: the same roles over a ring of ~17 KB band slots, four scanner teams
-        const int items = n * h->ws.K;
-        a.band_rows = bg.band_rows;
-        SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_banded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bg.smem));
-        nms_peaks_banded_kernel<<<std::min(items, h->sm_count), kNmsPThreads, bg.smem, st>>>(a, items, bg.slots, bg.n_bands);
-        h->stage_kernel[0] = "nms_peaks_banded_kernel";
-        h->launches++;
-        SPG_CUDA(h, cudaGetLastError());
+        pl->kind = NmsPlan::kBanded;
+        pl->band_rows = pl->bg.band_rows;
+        pl->smem = pl->bg.smem;
         return SPG_OK;
     }
     // bands of ~16 KB through a ring of 3 buffers: two bands in flight per CTA while one is scanned, 4 CTAs per SM
-    a.band_rows = std::max(4, std::min(H, 4096 / W));
-    const size_t smem = nms_smem_bytes(a.band_rows, H, W, h->ws.capP);
-    if (smem > h->smem_optin) return fail(h, SPG_E_INVALID, "map width %d needs %zu B of shared memory per band", W, smem);
-    SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    nms_peaks_kernel<<<n * h->ws.K, kNmsThreads, smem, st>>>(a);
-    h->stage_kernel[0] = "nms_peaks_kernel";
-    h->launches++;
-    SPG_CUDA(h, cudaGetLastError());
-    return SPG_OK;
+    pl->kind = NmsPlan::kBands;
+    pl->band_rows = std::max(4, std::min(H, 4096 / W));
+    pl->smem = nms_smem_bytes(pl->band_rows, H, W, capP);
+    if (pl->smem <= h->smem_optin) return SPG_OK;
+    if (image < 0)
+        return fail(h, SPG_E_INVALID, "map width %d needs %zu B of shared memory per band (limit %zu)", W, pl->smem, h->smem_optin);
+    return fail(h, SPG_E_INVALID, "image %d: map width %d needs %zu B of shared memory per band (limit %zu)", image, W, pl->smem,
+                h->smem_optin);
 }
 
-template <typename T, typename TA = T>
-int launch_score_t(spg_handle *h, const ScoreArgs &a, int n, cudaStream_t st) {
-    const size_t plane_bytes = (size_t)a.H * a.W * sizeof(T);
-    const size_t staged = score_smem_bytes(plane_bytes, h->ws.capP);
-    const bool aligned = (plane_bytes % 16 == 0) && ((a.img_stride * sizeof(T)) % 16 == 0) && ((a.chan_stride * sizeof(T)) % 16 == 0) &&
-                         ((reinterpret_cast<uintptr_t>(a.paf) & 15) == 0) && plane_bytes < (1u << 20);
-    const int grid = n * h->ws.L;
-    if (sizeof(T) == 4 && h->persist && aligned && h->ws.capP <= kPersistMaxCapP &&
-        persist_smem_bytes(plane_bytes, h->ws.capP) <= h->smem_optin) {
-        // one resident CTA per SM walking a ring of 3 plane slots (loader / screeners / scorers)
-        const size_t smem = persist_smem_bytes(plane_bytes, h->ws.capP);
-        SPG_CUDA(h, cudaFuncSetAttribute(limb_score_persist_kernel<TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        limb_score_persist_kernel<TA><<<std::min(grid, h->sm_count), kPersistThreads, smem, st>>>(a, grid);
-        h->stage_kernel[1] = sizeof(TA) == 4 ? "limb_score_persist_kernel<float>" : "limb_score_persist_kernel<double>";
-    } else if (aligned && staged <= h->smem_optin) {
-        SPG_CUDA(h, (cudaFuncSetAttribute(limb_score_kernel<T, true, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)staged)));
-        limb_score_kernel<T, true, TA><<<grid, kScoreThreads, staged, st>>>(a);
-        h->stage_kernel[1] = sizeof(T) == 8 ? "limb_score_kernel<double,true>" : sizeof(TA) == 4 ? "limb_score_kernel<float,true>" : "limb_score_kernel<float,true,double>";
-    } else {  // plane larger than shared memory (or unaligned): sample through L2
-        const size_t smem = score_smem_bytes(0, h->ws.capP);
-        limb_score_kernel<T, false, TA><<<grid, kScoreThreads, smem, st>>>(a);
-        h->stage_kernel[1] = sizeof(T) == 8 ? "limb_score_kernel<double,false>" : sizeof(TA) == 4 ? "limb_score_kernel<float,false>" : "limb_score_kernel<float,false,double>";
-    }
-    h->launches++;
-    SPG_CUDA(h, cudaGetLastError());
-    return SPG_OK;
+struct ScorePlan {
+    enum { kSampled, kStaged, kPersist } kind;  // kSampled and kStaged index the pairs of ScoreKernels
+    size_t smem;
+};
+
+ScorePlan plan_score(const spg_handle *h, const ScoreKernels &k, const void *paf, int64_t img_stride, int64_t chan_stride, int H,
+                     int W, bool persistent) {
+    const int capP = h->ws.capP;
+    const size_t plane_bytes = (size_t)H * W * k.esz;
+    const bool aligned = (plane_bytes % 16 == 0) && ((img_stride * k.esz) % 16 == 0) && ((chan_stride * k.esz) % 16 == 0) &&
+                         ((reinterpret_cast<uintptr_t>(paf) & 15) == 0) && plane_bytes < (1u << 20);
+    if (persistent && h->persist && k.persist && aligned && capP <= kPersistMaxCapP && persist_smem_bytes(plane_bytes, capP) <= h->smem_optin)
+        return {ScorePlan::kPersist, persist_smem_bytes(plane_bytes, capP)};  // one resident CTA per SM walking a ring of 3 plane slots (loader / screeners / scorers)
+    const size_t staged = score_smem_bytes(plane_bytes, capP);
+    if (aligned && staged <= h->smem_optin) return {ScorePlan::kStaged, staged};
+    return {ScorePlan::kSampled, score_smem_bytes(0, capP)};  // plane larger than shared memory (or unaligned): sample through L2
 }
 
-int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, int64_t chan_stride, int base, int n, int H,
-                 int W, double extent, const spg_params *p, cudaStream_t st) {
-    if (n == 0) return SPG_OK;
+// ---- kernel arguments from the parameters; the launchers add the planes and the image range ----
+NmsArgs nms_args(const spg_handle *h, const spg_params *p) {
+    NmsArgs a{};
+    a.radius = p->offset_radius;
+    a.thr = (float)p->thre1;
+    a.ws = h->ws;
+    return a;
+}
+
+ScoreArgs score_args(const spg_handle *h, const spg_params *p) {
     ScoreArgs a{};
-    a.paf = paf;
-    a.img_stride = img_stride;
-    a.chan_stride = chan_stride;
-    a.H = H;
-    a.W = W;
-    a.image_base = base;
     a.mid_num = p->mid_num;
-    a.image_extent = extent;
     a.thre2 = p->thre2;
     a.connect_ration = p->connect_ration;
     a.screen = h->screen;
     a.crit1_strict = p->crit1_strict != 0;
     a.exact_warps = h->exact_warps;
     a.ws = h->ws;
-    h->cand_dtype = dtype;
-    if (dtype == SPG_F64) return launch_score_t<double>(h, a, n, st);
-    if (dtype == SPG_F32_AS_F64) return launch_score_t<float, double>(h, a, n, st);
-    return launch_score_t<float>(h, a, n, st);
-}
-
-int launch_match(spg_handle *h, int base, int n, cudaStream_t st) {
-    if (n == 0) return SPG_OK;
-    MatchArgs a{};
-    a.n_images = n;
-    a.image_base = base;
-    a.keys_valid = h->cand_dtype == SPG_F32;
-    a.ws = h->ws;
-    const int warps = n * h->ws.L;
-    const int blocks = (warps * 32 + kMatchThreads - 1) / kMatchThreads;
-    limb_match_kernel<<<blocks, kMatchThreads, 0, st>>>(a);
-    h->stage_kernel[2] = "limb_match_kernel";
-    h->launches++;
-    SPG_CUDA(h, cudaGetLastError());
-    return SPG_OK;
+    return a;
 }
 
 // Arguments of the assemble stage (stand-alone or fused with the matcher); use_bulk is set by the caller.
@@ -267,6 +301,83 @@ AssembleArgs assemble_args(const spg_handle *h, int base, int n, const spg_param
     return a;
 }
 
+// ---- stage launchers on absolute image range [base, base+n) with chunk-local input pointers ----
+int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_stride, int base, int n, int H, int W,
+               const spg_params *p, cudaStream_t st) {
+    if (n == 0) return SPG_OK;
+    NmsPlan pl;
+    int rc;
+    if ((rc = plan_nms(h, heat, img_stride, chan_stride, H, W, true, -1, &pl))) return rc;
+    NmsArgs a = nms_args(h, p);
+    a.heat = heat;
+    a.img_stride = img_stride;
+    a.chan_stride = chan_stride;
+    a.H = H;
+    a.W = W;
+    a.band_rows = pl.band_rows;
+    a.use_bulk = pl.use_bulk;
+    a.image_base = base;
+    const int items = n * h->ws.K;
+    switch (pl.kind) {
+        case NmsPlan::kPersist:
+            return launch(h, kStageNms, "nms_peaks_persist_kernel", kNmsPersistKernels[a.radius], std::min(items, h->sm_count),
+                          kNmsPThreads, pl.smem, st, a, items);
+        case NmsPlan::kBanded:
+            return launch(h, kStageNms, "nms_peaks_banded_kernel", nms_peaks_banded_kernel, std::min(items, h->sm_count), kNmsPThreads,
+                          pl.smem, st, a, items, pl.bg.slots, pl.bg.n_bands);
+        default:
+            return launch(h, kStageNms, "nms_peaks_kernel", nms_peaks_kernel, items, kNmsThreads, pl.smem, st, a);
+    }
+}
+
+int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, int64_t chan_stride, int base, int n, int H,
+                 int W, double extent, const spg_params *p, cudaStream_t st) {
+    if (n == 0) return SPG_OK;
+    const ScoreKernels &k = kScoreKernels[dtype];
+    ScoreArgs a = score_args(h, p);
+    a.paf = paf;
+    a.img_stride = img_stride;
+    a.chan_stride = chan_stride;
+    a.H = H;
+    a.W = W;
+    a.image_base = base;
+    a.image_extent = extent;
+    h->cand_dtype = dtype;
+    const ScorePlan pl = plan_score(h, k, paf, img_stride, chan_stride, H, W, true);
+    const int grid = n * h->ws.L;
+    if (pl.kind == ScorePlan::kPersist)
+        return launch(h, kStageScore, k.persist_name, k.persist, std::min(grid, h->sm_count), kPersistThreads, pl.smem, st, a, grid);
+    return launch(h, kStageScore, k.item_name[pl.kind], k.item[pl.kind], grid, kScoreThreads, pl.smem, st, a);
+}
+
+// Images of a ragged call, as many per launch as the descriptor struct holds (it travels as the kernel parameter), with
+// `per_image` CTAs each.
+template <typename Args, typename Ragged, typename Image>
+int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), int per_image, int block, size_t smem,
+                  cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
+    constexpr size_t cap = sizeof(Ragged::img) / sizeof(Image);
+    for (size_t i0 = 0; i0 < imgs.size(); i0 += cap) {
+        const size_t cnt = std::min(cap, imgs.size() - i0);
+        Ragged r{};
+        std::copy(imgs.begin() + i0, imgs.begin() + i0 + cnt, r.img);
+        int rc;
+        if ((rc = launch(h, stage, name, kern, (int)cnt * per_image, block, smem, st, a, r))) return rc;
+    }
+    return SPG_OK;
+}
+
+int launch_match(spg_handle *h, int base, int n, cudaStream_t st) {
+    if (n == 0) return SPG_OK;
+    MatchArgs a{};
+    a.n_images = n;
+    a.image_base = base;
+    a.keys_valid = h->cand_dtype == SPG_F32;
+    a.ws = h->ws;
+    const int warps = n * h->ws.L;
+    const int blocks = (warps * 32 + kMatchThreads - 1) / kMatchThreads;
+    return launch(h, kStageMatch, "limb_match_kernel", limb_match_kernel, blocks, kMatchThreads, 0, st, a);
+}
+
 int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
     if (n == 0) return SPG_OK;
     AssembleArgs a = assemble_args(h, base, n, p);
@@ -274,12 +385,7 @@ int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStr
     a.use_bulk = ((size_t)h->ws.L * h->ws.capP * sizeof(uint32_t)) % 16 == 0;  // bulk copies move multiples of 16 bytes
     const size_t smem = assemble_smem_bytes(h->ws.K, h->ws.capP, h->ws.capR) + assemble_conn_bytes(h->ws.L, h->ws.capP);
     if (smem > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need %zu B of shared memory in assemble (limit %zu)", smem, h->smem_optin);
-    SPG_CUDA(h, cudaFuncSetAttribute(assemble_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    assemble_kernel<<<n, kAssembleThreads, smem, st>>>(a);
-    h->stage_kernel[3] = "assemble_kernel";
-    h->launches++;
-    SPG_CUDA(h, cudaGetLastError());
-    return SPG_OK;
+    return launch(h, kStageAssemble, "assemble_kernel", assemble_kernel, n, kAssembleThreads, smem, st, a);
 }
 
 int launch_match_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
@@ -293,13 +399,17 @@ int launch_match_assemble(spg_handle *h, int base, int n, const spg_params *p, c
         return launch_assemble(h, base, n, p, st);  // consumes the armed signal itself
     }
     h->armed_flag = nullptr;  // one shot
-    SPG_CUDA(h, cudaFuncSetAttribute(match_assemble_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    match_assemble_kernel<<<n, 32 * (1 + h->ma_warps), smem, st>>>(a, h->cand_dtype == SPG_F32);
-    h->stage_kernel[2] = "match_assemble_kernel";
-    h->stage_kernel[3] = "";
-    h->launches++;
-    SPG_CUDA(h, cudaGetLastError());
-    return SPG_OK;
+    h->stage_kernel[kStageAssemble] = "";
+    return launch(h, kStageMatch, "match_assemble_kernel", match_assemble_kernel, n, 32 * (1 + h->ma_warps), smem, st, a,
+                  h->cand_dtype == SPG_F32);
+}
+
+// persons from the scored candidates: the fused kernel, or the matcher and the assembler back to back (SPG_FUSE_MA=0)
+int launch_people(spg_handle *h, int base, int n, const spg_params *p, cudaStream_t st) {
+    if (h->fuse_ma) return launch_match_assemble(h, base, n, p, st);
+    int rc;
+    if ((rc = launch_match(h, base, n, st))) return rc;
+    return launch_assemble(h, base, n, p, st);
 }
 
 int run_all(spg_handle *h, const float *heat, int64_t his, int64_t hcs, const void *paf, int dtype, int64_t pis, int64_t pcs,
@@ -308,37 +418,7 @@ int run_all(spg_handle *h, const float *heat, int64_t his, int64_t hcs, const vo
     SPG_CUDA(h, cudaMemsetAsync(h->ws.status + base, 0, sizeof(uint32_t) * (size_t)n, st));
     if ((rc = launch_nms(h, heat, his, hcs, base, n, H, W, p, st))) return rc;
     if ((rc = launch_score(h, paf, dtype, pis, pcs, base, n, H, W, extent, p, st))) return rc;
-    if (h->fuse_ma) return launch_match_assemble(h, base, n, p, st);
-    if ((rc = launch_match(h, base, n, st))) return rc;
-    if ((rc = launch_assemble(h, base, n, p, st))) return rc;
-    return SPG_OK;
-}
-
-template <typename T, bool STAGE, typename TA>
-int launch_score_ragged_t(spg_handle *h, const ScoreArgs &a, const std::vector<ScoreImage> &imgs, size_t smem,
-                          cudaStream_t st) {
-    if (imgs.empty()) return SPG_OK;
-    if (STAGE) SPG_CUDA(h, (cudaFuncSetAttribute(limb_score_ragged_kernel<T, STAGE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
-    for (size_t i0 = 0; i0 < imgs.size(); i0 += kScoreRaggedMaxImages) {
-        const int cnt = (int)std::min<size_t>(kScoreRaggedMaxImages, imgs.size() - i0);
-        ScoreRagged r{};
-        std::copy(imgs.begin() + i0, imgs.begin() + i0 + cnt, r.img);
-        limb_score_ragged_kernel<T, STAGE, TA><<<cnt * h->ws.L, kScoreThreads, smem, st>>>(a, r);
-        h->launches++;
-        SPG_CUDA(h, cudaGetLastError());
-    }
-    h->stage_kernel[1] = sizeof(T) == 8 ? (STAGE ? "limb_score_ragged_kernel<double,true>" : "limb_score_ragged_kernel<double,false>")
-                         : sizeof(TA) == 4 ? (STAGE ? "limb_score_ragged_kernel<float,true>" : "limb_score_ragged_kernel<float,false>")
-                                           : (STAGE ? "limb_score_ragged_kernel<float,true,double>" : "limb_score_ragged_kernel<float,false,double>");
-    return SPG_OK;
-}
-
-template <typename T, typename TA = T>
-int launch_score_ragged(spg_handle *h, const ScoreArgs &a, const std::vector<ScoreImage> &staged, size_t staged_smem,
-                        const std::vector<ScoreImage> &sampled, cudaStream_t st) {
-    int rc;
-    if ((rc = launch_score_ragged_t<T, true, TA>(h, a, staged, staged_smem, st))) return rc;
-    return launch_score_ragged_t<T, false, TA>(h, a, sampled, score_smem_bytes(0, h->ws.capP), st);
+    return launch_people(h, base, n, p, st);
 }
 
 __global__ void wire_signal_kernel(unsigned long long *word, unsigned long long value) {
@@ -471,10 +551,8 @@ void spg_destroy(spg_handle *h) {
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
     for (void *p : h->allocs) cudaFree(p);
-    if (h->in_heat) cudaFree(h->in_heat);
-    if (h->in_paf) cudaFree(h->in_paf);
-    if (h->heat_acc) cudaFree(h->heat_acc);
-    if (h->pre_grid) cudaFree(h->pre_grid);
+    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid})
+        if (s->p) cudaFree(s->p);
     if (h->done_counter) cudaFree(h->done_counter);
     for (auto &s : h->streams)
         if (s) cudaStreamDestroy(s);
@@ -624,7 +702,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 
 int64_t spg_launch_count(const spg_handle *h) { return h ? h->launches : 0; }
 
-const char *spg_stage_kernel(const spg_handle *h, int32_t stage) { return (h && stage >= 0 && stage < 6) ? h->stage_kernel[stage] : ""; }
+const char *spg_stage_kernel(const spg_handle *h, int32_t stage) { return (h && stage >= 0 && stage < kStageCount) ? h->stage_kernel[stage] : ""; }
 
 // ---- post-network stage ------------------------------------------------------------------------
 int spg_postnet(spg_handle *h, const spg_postnet_desc *d, int32_t n, int32_t H, int32_t W, float *heat_out, void *paf_out,
@@ -642,6 +720,21 @@ static void invert_affine(const double *M, double *m) {
     m[0] = A11; m[1] *= -D; m[3] *= -D; m[4] = A22;
     const double b1 = -m[0] * m[2] - m[1] * m[5], b2 = -m[3] * m[2] - m[4] * m[5];
     m[2] = b1; m[5] = b2;
+}
+
+// The grid over output tiles of a.tile_w x a.tile_h: a CTA builds its tile's tables once and walks over a chunk of
+// channels -- as many as still leave ~ctas_per_sm CTAs per SM in the grid (a few resident: several waves).
+// ctas_per_sm 0: one channel per CTA.
+static int postnet_grid(spg_handle *h, PostArgs &a, int n, int ctas_per_sm, dim3 *grid) {
+    a.tiles_x = (a.W + a.tile_w - 1) / a.tile_w;
+    a.tiles_y = (a.H + a.tile_h - 1) / a.tile_h;
+    if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
+    const long long tiles = (long long)a.tiles_x * a.tiles_y * n;
+    const int n_chunks = ctas_per_sm == 0 ? a.n_out
+                                          : (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * ctas_per_sm + tiles - 1) / tiles));
+    a.chan_chunk = (a.n_out + n_chunks - 1) / n_chunks;
+    *grid = dim3((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
+    return SPG_OK;
 }
 
 int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_postnet_rotation *rot, int32_t n, int32_t H, int32_t W,
@@ -670,13 +763,7 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
-        const size_t need = (size_t)h->cfg.max_batch * ws.K * H * W;
-        if (h->heat_acc_elems < need) {
-            if (h->heat_acc) cudaFree(h->heat_acc);
-            h->heat_acc = nullptr; h->heat_acc_elems = 0;
-            SPG_CUDA(h, cudaMalloc(&h->heat_acc, need * sizeof(double)));
-            h->heat_acc_elems = need;
-        }
+        if ((rc = grow(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double)))) return rc;
     }
     // validate every scale and fill the common arguments
     PostArgs a{};
@@ -691,7 +778,7 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         a.src_chan[ws.K + k] = (short)(d->paf_chan0 + k);
         a.flip_chan[ws.K + k] = (short)(d->paf_chan0 + d->flip_paf_ord[k]);
     }
-    a.heat = heat_out; a.paf = paf_out; a.heat_acc = h->heat_acc; a.paf_is_f64 = paf_dtype == SPG_F64;
+    a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p); a.paf_is_f64 = paf_dtype == SPG_F64;
     a.n_scales = d->n_scales; a.nan_scrub = d->nan_scrub != 0;
     a.sx1 = 1.0 / (double)d->stride; a.sy1 = a.sx1;  // cv2.resize(fx = stride): scale = 1/fx
     for (int t = 0; t < d->n_scales; t++) {
@@ -716,6 +803,8 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         const double c1 = std::min((double)cap1, ((double)cap0 - 7.0) / s1) - margin;  // intermediate span allowed
         return std::max(1, std::min(maxd, (int)(c1 / std::max(s2, 1e-6))));
     };
+    dim3 grid;
+    const bool single = d->n_scales == 1;
     const bool fast = d->stride == 4;  // the reference's model: four-phase kernel; other strides: table-driven generic kernel
     if (fast) {
         // the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales.  With a
@@ -747,26 +836,10 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
                 }
                 if (!fits(tw, th)) return fail(h, SPG_E_INVALID, "rotation %d: the crop is too large for the image to warp it", t0);
                 a.tile_w = tw; a.tile_h = th;
-                a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
-                a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
-                if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
-                const long long tiles = (long long)a.tiles_x * a.tiles_y * n;
-                const int n_chunks = (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * 16 + tiles - 1) / tiles));
-                a.chan_chunk = (a.n_out + n_chunks - 1) / n_chunks;
-                dim3 grid((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
-                const size_t smem = postR_smem_bytes();
-#define SPG_ROT_LAUNCH(S_, F_)                                                                                                \
-    do {                                                                                                                      \
-        SPG_CUDA(h, (cudaFuncSetAttribute(postnet_rot_kernel<S_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))); \
-        postnet_rot_kernel<S_, F_><<<grid, kPostThreads, smem, st>>>(a);                                                      \
-    } while (0)
-                const bool single = d->n_scales == 1;
-                if (single) { if (S.net_is_f16) SPG_ROT_LAUNCH(true, true); else SPG_ROT_LAUNCH(true, false); }
-                else { if (S.net_is_f16) SPG_ROT_LAUNCH(false, true); else SPG_ROT_LAUNCH(false, false); }
-#undef SPG_ROT_LAUNCH
-                h->stage_kernel[4] = "postnet_rot_kernel";
-                h->launches++;
-                SPG_CUDA(h, cudaGetLastError());
+                if ((rc = postnet_grid(h, a, n, 16, &grid))) return rc;
+                void (*rot_kern)(PostArgs) = single ? (S.net_is_f16 ? postnet_rot_kernel<true, true> : postnet_rot_kernel<true, false>)
+                                                    : (S.net_is_f16 ? postnet_rot_kernel<false, true> : postnet_rot_kernel<false, false>);
+                if ((rc = launch(h, kStagePostnet, "postnet_rot_kernel", rot_kern, grid, kPostThreads, postR_smem_bytes(), st, a))) return rc;
                 continue;
             }
             a.tile_w = kPostTW; a.tile_h = kPostTH;
@@ -775,15 +848,6 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
                 a.tile_w = std::min(a.tile_w, tile_dim(a.sc[t].sx2, a.sx1, kPostF_C1, kPostF_CS, kPostTW, 13.0));
                 a.tile_h = std::min(a.tile_h, tile_dim(a.sc[t].sy2, a.sy1, kPostF_R1, kPostF_RS, kPostTH, 13.0));
             }
-            a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
-            a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
-            if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
-            // a CTA builds its tile's tables once and walks over a chunk of channels -- as many as still leave
-            // ~16 CTAs per SM in the grid (3 resident: several waves)
-            const long long tiles = (long long)a.tiles_x * a.tiles_y * n;
-            const int n_chunks = (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * 16 + tiles - 1) / tiles));
-            a.chan_chunk = (a.n_out + n_chunks - 1) / n_chunks;
-            dim3 grid((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
             bool ident = true, any16 = false, all16 = true;
             for (int t = 0; t < a.n_fused; t++) {
                 ident = ident && a.sc[t].crop_h == H && a.sc[t].crop_w == W;
@@ -791,35 +855,19 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
                 all16 = all16 && a.sc[t].net_is_f16;
             }
             if (any16 != all16) return fail(h, SPG_E_INVALID, "the network outputs of all scales must have the same dtype");
-            const bool single = d->n_scales == 1;
-            const size_t smem = postF_smem_bytes(single ? 1 : kPostMaxScales);
-#define SPG_POST_LAUNCH(S_, I_, F_)                                                                                           \
-    do {                                                                                                                      \
-        SPG_CUDA(h, (cudaFuncSetAttribute(postnet_kernel<S_, I_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))); \
-        postnet_kernel<S_, I_, F_><<<grid, kPostThreads, smem, st>>>(a);                                                      \
-    } while (0)
             if (single && ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
                 a.tile_w = kPostI_TW; a.tile_h = kPostI_TH;
-                a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
-                a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
-                const long long tiles_i = (long long)a.tiles_x * a.tiles_y * n;
-                const int chunks_i = (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * 32 + tiles_i - 1) / tiles_i));
-                a.chan_chunk = (a.n_out + chunks_i - 1) / chunks_i;
-                dim3 grid_i((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
-                if (all16) postnet_x4_ident_kernel<true><<<grid_i, kPostThreads, 0, st>>>(a);
-                else postnet_x4_ident_kernel<false><<<grid_i, kPostThreads, 0, st>>>(a);
-                h->stage_kernel[4] = "postnet_x4_ident_kernel";
-            } else if (single) {
-                h->stage_kernel[4] = "postnet_kernel";
-                if (all16) SPG_POST_LAUNCH(true, false, true); else SPG_POST_LAUNCH(true, false, false);
+                if ((rc = postnet_grid(h, a, n, 32, &grid))) return rc;
+                rc = launch(h, kStagePostnet, "postnet_x4_ident_kernel", all16 ? postnet_x4_ident_kernel<true> : postnet_x4_ident_kernel<false>,
+                            grid, kPostThreads, 0, st, a);
             } else {
-                h->stage_kernel[4] = "postnet_kernel";
-                if (ident) { if (all16) SPG_POST_LAUNCH(false, true, true); else SPG_POST_LAUNCH(false, true, false); }
-                else { if (all16) SPG_POST_LAUNCH(false, false, true); else SPG_POST_LAUNCH(false, false, false); }
+                if ((rc = postnet_grid(h, a, n, 16, &grid))) return rc;
+                void (*kern)(PostArgs) = single  ? (all16 ? postnet_kernel<true, false, true> : postnet_kernel<true, false, false>)
+                                         : ident ? (all16 ? postnet_kernel<false, true, true> : postnet_kernel<false, true, false>)
+                                                 : (all16 ? postnet_kernel<false, false, true> : postnet_kernel<false, false, false>);
+                rc = launch(h, kStagePostnet, "postnet_kernel", kern, grid, kPostThreads, postF_smem_bytes(single ? 1 : kPostMaxScales), st, a);
             }
-#undef SPG_POST_LAUNCH
-            h->launches++;
-            SPG_CUDA(h, cudaGetLastError());
+            if (rc) return rc;
         }
         return SPG_OK;
     }
@@ -830,15 +878,9 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         a.scale_index = t;
         a.tile_w = tile_dim(a.sx2, a.sx1, kPostC1, kPostCS, kPostTW, 7.0);
         a.tile_h = tile_dim(a.sy2, a.sy1, kPostR1, kPostRS, kPostTH, 7.0);
-        a.tiles_x = (W + a.tile_w - 1) / a.tile_w;
-        a.tiles_y = (H + a.tile_h - 1) / a.tile_h;
-        if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
-        a.chan_chunk = 1;
-        dim3 grid((unsigned)(a.tiles_x * a.tiles_y), (unsigned)a.n_out, (unsigned)n);
-        postnet_generic_kernel<<<grid, kPostThreads, 0, st>>>(a);
-        h->stage_kernel[4] = "postnet_generic_kernel";
-        h->launches++;
-        SPG_CUDA(h, cudaGetLastError());
+        if ((rc = postnet_grid(h, a, n, 0, &grid)) ||
+            (rc = launch(h, kStagePostnet, "postnet_generic_kernel", postnet_generic_kernel, grid, kPostThreads, 0, st, a)))
+            return rc;
     }
     return SPG_OK;
 }
@@ -894,27 +936,19 @@ int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_
     if (n == 0 || n_items == 0) return SPG_OK;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (h->pre_grid_bytes < grid_need) {
-        if (h->pre_grid) cudaFree(h->pre_grid);
-        h->pre_grid = nullptr; h->pre_grid_bytes = 0;
-        SPG_CUDA(h, cudaMalloc(&h->pre_grid, grid_need));
-        h->pre_grid_bytes = grid_need;
-    }
+    int rc;
+    if ((rc = grow(h, h->pre_grid, grid_need))) return rc;
     for (int t = 0; t < n_items; t++) {
         PreArgs &a = args[t];
-        a.grid = h->pre_grid;
+        a.grid = static_cast<unsigned char *>(h->pre_grid.p);
         const dim3 grid((unsigned)((a.Wp + kPreThreads - 1) / kPreThreads), (unsigned)a.Hp, (unsigned)n);
         if (items[t].rotate) {
-            prenet_resize_kernel<<<grid, kPreThreads, 0, st>>>(a);
-            prenet_kernel<true><<<grid, kPreThreads, 0, st>>>(a);
-            h->launches += 2;
-            h->stage_kernel[5] = "prenet_kernel<true>";
-        } else {
-            prenet_kernel<false><<<grid, kPreThreads, 0, st>>>(a);
-            h->launches++;
-            h->stage_kernel[5] = "prenet_kernel<false>";
+            if ((rc = launch(h, kStagePrenet, "prenet_resize_kernel", prenet_resize_kernel, grid, kPreThreads, 0, st, a)) ||
+                (rc = launch(h, kStagePrenet, "prenet_kernel<true>", prenet_kernel<true>, grid, kPreThreads, 0, st, a)))
+                return rc;
+        } else if ((rc = launch(h, kStagePrenet, "prenet_kernel<false>", prenet_kernel<false>, grid, kPreThreads, 0, st, a))) {
+            return rc;
         }
-        SPG_CUDA(h, cudaGetLastError());
     }
     return SPG_OK;
 }
@@ -938,9 +972,9 @@ int spg_limb_score(spg_handle *h, const void *paf, int32_t dtype, int64_t image_
                    int32_t W, double extent, const spg_params *p, void *stream) {
     if (!h) return SPG_E_INVALID;
     if (!paf && n > 0) return fail(h, SPG_E_INVALID, "paf_dev is NULL");
-    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
-    if (h->stage < 1) return fail(h, SPG_E_STATE, "spg_limb_score needs peaks (spg_nms_peaks or spg_upload_peaks) first");
     int rc;
+    if ((rc = check_dtype(h, dtype))) return rc;
+    if (h->stage < 1) return fail(h, SPG_E_STATE, "spg_limb_score needs peaks (spg_nms_peaks or spg_upload_peaks) first");
     if ((rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = launch_score(h, paf, dtype, image_stride, chan_stride, 0, n, H, W, extent, p, static_cast<cudaStream_t>(stream)))) return rc;
@@ -952,8 +986,7 @@ int spg_limb_match(spg_handle *h, int32_t n, const spg_params *p, void *stream) 
     if (!h) return SPG_E_INVALID;
     if (h->stage < 2) return fail(h, SPG_E_STATE, "spg_limb_match needs spg_limb_score first");
     int rc;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
-    if ((rc = check_params(h, p))) return rc;
+    if ((rc = check_batch(h, n)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = launch_match(h, 0, n, static_cast<cudaStream_t>(stream)))) return rc;
     h->stage = std::max(h->stage, 3);
@@ -964,8 +997,7 @@ int spg_assemble(spg_handle *h, int32_t n, const spg_params *p, void *stream) {
     if (!h) return SPG_E_INVALID;
     if (h->stage < 3) return fail(h, SPG_E_STATE, "spg_assemble needs connections (spg_limb_match or spg_upload_connections) first");
     int rc;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
-    if ((rc = check_params(h, p))) return rc;
+    if ((rc = check_batch(h, n)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = launch_assemble(h, 0, n, p, static_cast<cudaStream_t>(stream)))) return rc;
     h->stage = 4;
@@ -976,8 +1008,7 @@ int spg_match_assemble(spg_handle *h, int32_t n, const spg_params *p, void *stre
     if (!h) return SPG_E_INVALID;
     if (h->stage < 2) return fail(h, SPG_E_STATE, "spg_match_assemble needs spg_limb_score first");
     int rc;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
-    if ((rc = check_params(h, p))) return rc;
+    if ((rc = check_batch(h, n)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = launch_match_assemble(h, 0, n, p, static_cast<cudaStream_t>(stream)))) return rc;
     h->stage = 4;
@@ -988,9 +1019,8 @@ int spg_group_batch(spg_handle *h, const float *heat, int64_t his, int64_t hcs, 
                     int32_t n, int32_t H, int32_t W, double extent, const spg_params *p, void *stream) {
     if (!h) return SPG_E_INVALID;
     if ((!heat || !paf) && n > 0) return fail(h, SPG_E_INVALID, "heat_dev/paf_dev is NULL");
-    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
     int rc;
-    if ((rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
+    if ((rc = check_dtype(h, dtype)) || (rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     if ((rc = run_all(h, heat, his, hcs, paf, dtype, pis, pcs, 0, n, H, W, extent, p, static_cast<cudaStream_t>(stream)))) return rc;
     h->stage = 4;
@@ -1003,25 +1033,22 @@ int spg_group_batch(spg_handle *h, const float *heat, int64_t his, int64_t hcs, 
 // plane first (longest job first over the CTA queue); every CTA writes to its image's own slot.
 int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int32_t dtype, const spg_params *p, void *stream) {
     if (!h) return SPG_E_INVALID;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images %d outside [0, max_batch=%d]", n, h->cfg.max_batch);
-    if (!images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
-    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
     int rc;
-    if ((rc = check_params(h, p))) return rc;
+    if ((rc = check_batch(h, n))) return rc;
+    if (!images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
+    if ((rc = check_dtype(h, dtype)) || (rc = check_params(h, p))) return rc;
     const Workspace &ws = h->ws;
-    const size_t esz = dtype == SPG_F64 ? 8 : 4;
+    const ScoreKernels &k = kScoreKernels[dtype];
     const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
-    // validate every image and build the descriptors before the first launch
+    // validate every image before the first launch
     std::vector<int> order((size_t)n);
+    NmsPlan np;
     for (int i = 0; i < n; i++) {
         const spg_image_maps &im = images[i];
         if (!im.heat || !im.paf) return fail(h, SPG_E_INVALID, "image %d: heat/paf is NULL", i);
         if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
             return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
-        const int br = std::max(4, std::min((int)im.height, 4096 / (int)im.width));
-        const size_t smem = nms_smem_bytes(br, im.height, im.width, ws.capP);
-        if (smem > h->smem_optin)
-            return fail(h, SPG_E_INVALID, "image %d: map width %d needs %zu B of shared memory per band (limit %zu)", i, im.width, smem, h->smem_optin);
+        if ((rc = plan_nms(h, im.heat, 0, im.heat_chan_stride, im.height, im.width, false, i, &np))) return rc;
         order[i] = i;
     }
     if (score_smem_bytes(0, ws.capP) > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need too much shared memory in limb scoring");
@@ -1035,21 +1062,17 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
     for (int i : order) {
         const spg_image_maps &im = images[i];
         const int H = im.height, W = im.width;
+        plan_nms(h, im.heat, 0, im.heat_chan_stride, H, W, false, i, &np);  // succeeded in the validation above
         NmsImage d{};
-        d.heat = im.heat; d.chan_stride = im.heat_chan_stride; d.H = H; d.W = W; d.slot = i;
-        d.band_rows = std::max(4, std::min(H, 4096 / W));
-        d.use_bulk = (W % 4 == 0) && (im.heat_chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(im.heat) & 15) == 0);
-        nms_smem = std::max(nms_smem, nms_smem_bytes(d.band_rows, H, W, ws.capP));
+        d.heat = im.heat; d.chan_stride = im.heat_chan_stride; d.H = H; d.W = W; d.band_rows = np.band_rows; d.use_bulk = np.use_bulk; d.slot = i;
+        nms_smem = std::max(nms_smem, np.smem);
         nms.push_back(d);
         ScoreImage s{};
         s.paf = im.paf; s.chan_stride = im.paf_chan_stride; s.image_extent = im.image_extent; s.H = H; s.W = W; s.slot = i;
-        // the conditions of launch_score_t's staged kernel, per image
-        const size_t plane_bytes = (size_t)H * W * esz, smem = score_smem_bytes(plane_bytes, ws.capP);
-        const bool aligned = (plane_bytes % 16 == 0) && ((im.paf_chan_stride * esz) % 16 == 0) &&
-                             ((reinterpret_cast<uintptr_t>(im.paf) & 15) == 0) && plane_bytes < (1u << 20);
-        if (aligned && smem <= h->smem_optin) {
+        const ScorePlan sp = plan_score(h, k, im.paf, 0, im.paf_chan_stride, H, W, false);
+        if (sp.kind == ScorePlan::kStaged) {
             staged.push_back(s);
-            staged_smem = std::max(staged_smem, smem);
+            staged_smem = std::max(staged_smem, sp.smem);
         } else {
             sampled.push_back(s);
         }
@@ -1058,36 +1081,16 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SPG_CUDA(h, cudaMemsetAsync(ws.status, 0, sizeof(uint32_t) * (size_t)n, st));
     if (n == 0) return SPG_OK;
-    NmsArgs na{};
-    na.radius = p->offset_radius;
-    na.thr = (float)p->thre1;
-    na.ws = ws;
-    SPG_CUDA(h, cudaFuncSetAttribute(nms_peaks_ragged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nms_smem));
-    for (size_t i0 = 0; i0 < nms.size(); i0 += kRaggedMaxImages) {
-        const int cnt = (int)std::min<size_t>(kRaggedMaxImages, nms.size() - i0);
-        NmsRagged r{};
-        std::copy(nms.begin() + i0, nms.begin() + i0 + cnt, r.img);
-        nms_peaks_ragged_kernel<<<cnt * ws.K, kNmsThreads, nms_smem, st>>>(na, r);
-        h->launches++;
-        SPG_CUDA(h, cudaGetLastError());
-    }
-    h->stage_kernel[0] = "nms_peaks_ragged_kernel";
-    ScoreArgs sa{};
-    sa.mid_num = p->mid_num;
-    sa.thre2 = p->thre2;
-    sa.connect_ration = p->connect_ration;
-    sa.screen = h->screen;
-    sa.crit1_strict = p->crit1_strict != 0;
-    sa.exact_warps = h->exact_warps;
-    sa.ws = ws;
+    if ((rc = launch_ragged(h, kStageNms, "nms_peaks_ragged_kernel", nms_peaks_ragged_kernel, ws.K, kNmsThreads, nms_smem, st,
+                            nms_args(h, p), nms)))
+        return rc;
     h->cand_dtype = dtype;
-    if (dtype == SPG_F64) rc = launch_score_ragged<double>(h, sa, staged, staged_smem, sampled, st);
-    else if (dtype == SPG_F32_AS_F64) rc = launch_score_ragged<float, double>(h, sa, staged, staged_smem, sampled, st);
-    else rc = launch_score_ragged<float>(h, sa, staged, staged_smem, sampled, st);
-    if (rc) return rc;
-    if (h->fuse_ma) rc = launch_match_assemble(h, 0, n, p, st);
-    else if (!(rc = launch_match(h, 0, n, st))) rc = launch_assemble(h, 0, n, p, st);
-    if (rc) return rc;
+    const ScoreArgs sa = score_args(h, p);
+    if ((rc = launch_ragged(h, kStageScore, k.ragged_name[1], k.ragged[1], ws.L, kScoreThreads, staged_smem, st, sa, staged)) ||
+        (rc = launch_ragged(h, kStageScore, k.ragged_name[0], k.ragged[0], ws.L, kScoreThreads, score_smem_bytes(0, ws.capP), st, sa,
+                            sampled)) ||
+        (rc = launch_people(h, 0, n, p, st)))
+        return rc;
     h->stage = 4;
     return SPG_OK;
 }
@@ -1102,36 +1105,22 @@ int spg_group_host(spg_handle *h, const float *heat_host, const void *paf_host, 
                    double extent, const spg_params *p, int32_t *out_n, double *out_xy, double *out_score, uint32_t *out_status) {
     if (!h) return SPG_E_INVALID;
     if ((!heat_host || !paf_host) && n > 0) return fail(h, SPG_E_INVALID, "heat_host/paf_host is NULL");
-    if (dtype != SPG_F32 && dtype != SPG_F64 && dtype != SPG_F32_AS_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32, SPG_F64 or SPG_F32_AS_F64");
     int rc;
-    if ((rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
+    if ((rc = check_dtype(h, dtype)) || (rc = check_dims(h, n, H, W)) || (rc = check_params(h, p))) return rc;
     DeviceGuard guard(h->device);
     const Workspace &ws = h->ws;
     const size_t plane = (size_t)H * W;
-    const size_t esz = dtype == SPG_F64 ? 8 : 4;
-    const size_t heat_img = (size_t)ws.K * plane * sizeof(float), paf_img = (size_t)ws.L * plane * esz;
+    const size_t heat_img = (size_t)ws.K * plane * sizeof(float), paf_img = (size_t)ws.L * plane * kScoreKernels[dtype].esz;
     // chunk so that copy(c+1) overlaps kernels(c); keep at least ~8 chunks for large batches
     const int chunk = std::max(1, std::min(n, std::max(8, n / 8)));
-    const size_t need_heat = 2 * (size_t)chunk * heat_img, need_paf = 2 * (size_t)chunk * paf_img;
-    if (h->in_heat_bytes < need_heat) {
-        if (h->in_heat) cudaFree(h->in_heat);
-        h->in_heat = nullptr; h->in_heat_bytes = 0;
-        SPG_CUDA(h, cudaMalloc(&h->in_heat, need_heat));
-        h->in_heat_bytes = need_heat;
-    }
-    if (h->in_paf_bytes < need_paf) {
-        if (h->in_paf) cudaFree(h->in_paf);
-        h->in_paf = nullptr; h->in_paf_bytes = 0;
-        SPG_CUDA(h, cudaMalloc(&h->in_paf, need_paf));
-        h->in_paf_bytes = need_paf;
-    }
+    if ((rc = grow(h, h->in_heat, 2 * (size_t)chunk * heat_img)) || (rc = grow(h, h->in_paf, 2 * (size_t)chunk * paf_img))) return rc;
     const size_t RSJ = (size_t)ws.capR * ws.J * 2;
     int ci = 0;
     for (int base = 0; base < n; base += chunk, ci++) {
         const int m = std::min(chunk, n - base);
         cudaStream_t st = h->streams[ci & 1];
-        unsigned char *dh = static_cast<unsigned char *>(h->in_heat) + (size_t)(ci & 1) * chunk * heat_img;
-        unsigned char *dp = static_cast<unsigned char *>(h->in_paf) + (size_t)(ci & 1) * chunk * paf_img;
+        unsigned char *dh = static_cast<unsigned char *>(h->in_heat.p) + (size_t)(ci & 1) * chunk * heat_img;
+        unsigned char *dp = static_cast<unsigned char *>(h->in_paf.p) + (size_t)(ci & 1) * chunk * paf_img;
         // stream order protects the staging buffers: chunk ci reuses the buffers of chunk ci-2 on the same stream
         SPG_CUDA(h, cudaMemcpyAsync(dh, reinterpret_cast<const unsigned char *>(heat_host) + (size_t)base * heat_img, (size_t)m * heat_img, cudaMemcpyHostToDevice, st));
         SPG_CUDA(h, cudaMemcpyAsync(dp, static_cast<const unsigned char *>(paf_host) + (size_t)base * paf_img, (size_t)m * paf_img, cudaMemcpyHostToDevice, st));
@@ -1226,7 +1215,7 @@ int spg_upload_connections(spg_handle *h, int32_t img, const int32_t *conn_count
 
 int spg_download_peaks(spg_handle *h, int32_t n, int32_t *peak_count, double *x, double *y, float *score, uint32_t *anchor, void *stream) {
     if (!h) return SPG_E_INVALID;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
+    if (const int rc = check_batch(h, n)) return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const Workspace &ws = h->ws;
@@ -1242,7 +1231,7 @@ int spg_download_peaks(spg_handle *h, int32_t n, int32_t *peak_count, double *x,
 
 int spg_download_connections(spg_handle *h, int32_t n, int32_t *conn_count, int32_t *cand_count, uint32_t *ij, double *score, double *norm, void *stream) {
     if (!h) return SPG_E_INVALID;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
+    if (const int rc = check_batch(h, n)) return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const Workspace &ws = h->ws;
@@ -1258,7 +1247,7 @@ int spg_download_connections(spg_handle *h, int32_t n, int32_t *conn_count, int3
 
 int spg_download_people(spg_handle *h, int32_t n, int32_t *n_persons, double *subset, double *people_xy, double *people_score, void *stream) {
     if (!h) return SPG_E_INVALID;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
+    if (const int rc = check_batch(h, n)) return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const Workspace &ws = h->ws;
@@ -1272,7 +1261,7 @@ int spg_download_people(spg_handle *h, int32_t n, int32_t *n_persons, double *su
 
 int spg_download_status(spg_handle *h, int32_t n, uint32_t *status, void *stream) {
     if (!h) return SPG_E_INVALID;
-    if (n < 0 || n > h->cfg.max_batch) return fail(h, SPG_E_INVALID, "n_images out of range");
+    if (const int rc = check_batch(h, n)) return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SPG_D2H(status, h->ws.status, (size_t)n);
