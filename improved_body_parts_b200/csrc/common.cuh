@@ -37,12 +37,29 @@ __device__ __forceinline__ void trace_put(int slot, int dep, int mode) {  // mod
 #define SPG_TR_FIRST(slot, dep) ::spg::trace_put((slot), (int)(dep), 2)
 #define SPG_TR_LAST(slot, dep) ::spg::trace_put((slot), (int)(dep), 3)
 #define SPG_TR_ADD(slot, v) ::spg::trace_put((slot), (int)(v), 4)
+// Start and exit time of every CTA (up to kTraceSpanCtas) of a launch, in %globaltimer nanoseconds: unlike clock64 one
+// clock for all SMs, so CTAs on different SMs can be compared.  SPG_TR_CTA_START: thread 0 at entry; SPG_TR_CTA_EXIT:
+// every warp at its end, the latest stays.
+constexpr int kTraceSpanCtas = 1024;
+__device__ unsigned long long g_spg_cta_span[kTraceSpanCtas * 2];
+__device__ __forceinline__ void trace_cta(int exit) {
+    if (blockIdx.x < kTraceSpanCtas && (threadIdx.x & 31) == 0 && (exit || threadIdx.x == 0)) {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
+        if (exit) atomicMax(&g_spg_cta_span[2 * blockIdx.x + 1], t);
+        else g_spg_cta_span[2 * blockIdx.x] = t;
+    }
+}
+#define SPG_TR_CTA_START() ::spg::trace_cta(0)
+#define SPG_TR_CTA_EXIT() ::spg::trace_cta(1)
 #else
 #define SPG_TR(slot, dep) do {} while (0)
 #define SPG_TRV(slot, v) do {} while (0)
 #define SPG_TR_FIRST(slot, dep) do {} while (0)
 #define SPG_TR_LAST(slot, dep) do {} while (0)
 #define SPG_TR_ADD(slot, v) do {} while (0)
+#define SPG_TR_CTA_START() do {} while (0)
+#define SPG_TR_CTA_EXIT() do {} while (0)
 #endif
 
 constexpr int kMaxParts = 32;        // K

@@ -3,7 +3,7 @@
 // Same arithmetic and outputs as limb_score_kernel (limb_score.cuh: conservative f32 screen, then the
 // reference's exact evaluation of the survivors, evaluate.py:211-255); different schedule.  The one-CTA-per-
 // (image, limb) kernel pays a prologue per item and serialises load -> screen -> exact inside a CTA.  Here one
-// CTA per SM stays resident and walks over its items (item = image * L + limb, strided by the grid) with
+// CTA per SM stays resident and walks over the items it draws from a device-side queue (item = image * L + limb) with
 // three roles and two rings:
 //
 //   loader    (warp 0)     issues the plane's bulk copy (TMA, SASS UBLKCP) into one of 3 plane slots as soon as the
@@ -152,13 +152,17 @@ __device__ __forceinline__ void screen_pair(const ScreenCtx &c, int pc, bool val
 }
 
 // TA = float: f32 planes, f32 arithmetic; double: f32 planes evaluated in float64 (SPG_F32_AS_F64).
+// Items are dealt from a device-side queue: queue[0] is the next ticket (ticket = item = image * L + limb), queue[1]
+// counts the CTAs that have drawn a ticket >= n_items; the last of them resets both to 0 for the next launch.  Both
+// words are 0 when the kernel starts.
 template <typename TA>
-__global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(ScoreArgs a, int n_items) {
+__global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(ScoreArgs a, int n_items, unsigned int *queue) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     // full: plane copy landed + lists published; screened: every screener has left the item -- its survivor list is
     // complete (scorers) and its plane slot can be refilled (loader); mfree: every scorer has left the meta slot
     __shared__ uint64_t bar_full[kPersistSlots], bar_screened[kMetaSlots], bar_mfree[kMetaSlots];
     __shared__ uint32_t s_bias_bytes;  // 4 * kScreenBias * (W + 1)
+    SPG_TR_CTA_START();
 
     using T = float;
     const Workspace &ws = a.ws;
@@ -190,8 +194,6 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
     if (tid >= 32 && tid < 32 + kScreenMaxMid + 1) build_screen_row(a, tid - 32, s_rcp, s_tab, s_ts, true);
     __syncthreads();
 
-    const int G = gridDim.x;
-    const int nj = ((int)blockIdx.x < n_items) ? (n_items - 1 - (int)blockIdx.x) / G + 1 : 0;
     const bool screen = a.screen && a.mid_num <= kScreenMaxMid && H <= kScreenMaxDim && W <= kScreenMaxDim;
     const T thre2 = sizeof(TA) == 8 ? f32_not_above(a.thre2) : (T)a.thre2;  // the screen's float32 threshold
     const TA thre2_exact = (TA)a.thre2;
@@ -204,9 +206,17 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
         constexpr int kMaxE = kPersistMaxCapP / 32;  // list entries per lane
         double r_xa[kMaxE], r_ya[kMaxE], r_xb[kMaxE], r_yb[kMaxE];
         float r_sa[kMaxE], r_sb[kMaxE];
-        int r_cntA = 0, r_cntB = 0;
-        auto fetch = [&](int j) {
-            const int item = (int)blockIdx.x + j * G;
+        int r_cntA = 0, r_cntB = 0, r_item = 0;
+        // Draws the CTA's next item from the queue and loads its end-point lists into registers.  Items go to whichever
+        // CTA asks first, so every SM stays busy until the queue is empty: with a fixed stride of G = 132 CTAs over
+        // item = image * 30 + limb, CTA c would only ever score the limbs k = c (mod 6), and limbs differ a lot in how
+        // many pairs survive the screen.  A ticket >= n_items ends the CTA's items (its lists load item n_items - 1,
+        // unused).
+        auto fetch = [&]() {
+            int t = 0;
+            if (lane == 0) t = (int)atomicAdd(queue, 1u);
+            r_item = __shfl_sync(0xffffffffu, t, 0);
+            const int item = min(r_item, n_items - 1);
             const int n_local = item / L, k = item - n_local * L;
             const int n = a.image_base + n_local;
             const int pa = ws.limbs[2 * k], pb = ws.limbs[2 * k + 1];
@@ -235,22 +245,27 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             }
             __syncwarp();
         };
-        if (nj > 0) fetch(0);
-        for (int j = 0; j < nj; j++) {
+        // Item j of the CTA goes through plane slot j % kPersistSlots and meta slot j % kMetaSlots.  Once the queue is
+        // empty, one more "item" is published: a header with npairs = -1 and no plane, which tells the screeners (and
+        // through them the scorers) that there are no more items.
+        fetch();
+        int j = 0;
+        for (;; j++) {
             const int s = j % kPersistSlots, e = j % kMetaSlots;
             SPG_TR_ITEM(SPG_TR, j, 0, j);
             if (j >= kPersistSlots) {  // the plane slot's previous item has been screened
                 const int jp = j - kPersistSlots;
                 mbar_wait_sleep(&bar_screened[jp % kMetaSlots], (jp / kMetaSlots) & 1);
             }
-            const int item = (int)blockIdx.x + j * G;
-            const int n_local = item / L, k = item - n_local * L;
+            const bool live = r_item < n_items;
+            const int n_local = r_item / L, k = r_item - n_local * L;
             const int n = a.image_base + n_local;
             if (lane == 0) {  // plane first (arrival 1 of 2 on `full`, carries the byte count)
                 const unsigned char *gplane = reinterpret_cast<const unsigned char *>(plane_of(n_local, k));
                 unsigned char *dst = s_planes + s * plane_stride;
-                mbar_expect_tx(&bar_full[s], (uint32_t)plane_bytes);
-                for (size_t off = 0; off < plane_bytes; off += kBulkChunkBytes) {
+                const size_t bytes_in = live ? plane_bytes : 0;
+                mbar_expect_tx(&bar_full[s], (uint32_t)bytes_in);
+                for (size_t off = 0; off < bytes_in; off += kBulkChunkBytes) {
                     const uint32_t bytes = (uint32_t)min((size_t)kBulkChunkBytes, plane_bytes - off);
                     bulk_g2s(dst + off, gplane + off, bytes, &bar_full[s]);
                 }
@@ -282,7 +297,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             const bool special = nA == 0 || nB == 0;
             if (lane == 0) {
                 PersistHdr h;
-                h.nA = nA; h.nB = nB; h.npairs = special ? 0 : nA * nB; h.n = n; h.k = k; h.special = special;
+                h.nA = nA; h.nB = nB; h.npairs = !live ? -1 : special ? 0 : nA * nB; h.n = n; h.k = k; h.special = special;
                 h.magic = nB > 1 ? 0xffffffffu / (uint32_t)nB + 1u : 0u;
                 h.pad = 0;
                 ms.hdr = h;
@@ -290,11 +305,20 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             __syncwarp();
             SPG_TR_ITEM(SPG_TR, j, 4, j);
             if (lane == 0) mbar_arrive(&bar_full[s]);  // arrival 2 of 2: lists + header are in place
-            if (j + 1 < nj) fetch(j + 1);              // in flight while the next iteration waits for its slots
+            if (!live) break;
+            fetch();  // in flight while the next iteration waits for its slots
         }
-        for (int jp = max(0, nj - kMetaSlots); jp < nj; jp++) {  // the items still in the meta ring
+        for (int jp = max(0, j - kMetaSlots + 1); jp < j; jp++) {  // the items still in the meta ring (j: the end header)
             mbar_wait_sleep(&bar_mfree[jp % kMetaSlots], (jp / kMetaSlots) & 1);
             close_item(jp);
+        }
+        if (lane == 0) {  // this CTA has drawn its last ticket
+            __threadfence();
+            if (atomicAdd(queue + 1, 1u) == gridDim.x - 1) {  // so has every other: reset the queue for the next launch
+                __threadfence();
+                *(volatile unsigned int *)queue = 0u;
+                *(volatile unsigned int *)(queue + 1) = 0u;
+            }
         }
     } else {
         // exact evaluation of one pair + candidate append.  `plane` is the shared-memory copy for a screener whose
@@ -323,7 +347,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             // moves the odd second chunk of an item (pairs beyond 32 * nS) to a different warp every item.  Screeners
             // never wait for each other: their only wait is `full`.
             int c0 = warp - 1;
-            for (int j = 0; j < nj; j++) {
+            for (int j = 0;; j++) {
                 const int s = j % kPersistSlots, e = j % kMetaSlots;
                 // `full` also means the meta slot's list and counters are recycled (the loader closed item j - kMetaSlots)
                 mbar_wait_sleep(&bar_full[s], (j / kPersistSlots) & 1);
@@ -361,14 +385,16 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
                 SPG_TR_ITEM(SPG_TR_FIRST, j, 6, j);
                 SPG_TR_ITEM(SPG_TR_LAST, j, 7, j);
                 if (lane == 0) mbar_arrive(&bar_screened[e]);  // release: this warp's survivors are in the list, the plane is no longer read
+                if (npairs < 0) break;  // the end header (passed on to the scorers by the arrival above)
                 if (++c0 == nS) c0 = 0;
             }
         } else {
             // =========================== scorers ===========================
-            for (int j = 0; j < nj; j++) {
+            for (int j = 0;; j++) {
                 const int e = j % kMetaSlots;
                 mbar_wait_sleep(&bar_screened[e], (j / kMetaSlots) & 1);  // every screener has left item j: the list is complete
                 MetaSlot &ms = s_meta[e];
+                if (ms.hdr.npairs < 0) break;  // the end header
                 const int ns = min(ms.nsurv, kPersistListCap);
                 if (ns > 0) {
                     const T *gplane = plane_of(ms.hdr.n - a.image_base, ms.hdr.k);  // the plane's slot may already hold another item
@@ -389,6 +415,7 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             }
         }
     }
+    SPG_TR_CTA_EXIT();
 }
 
 }  // namespace spg

@@ -54,6 +54,7 @@ struct spg_handle {
     std::vector<void *> allocs;
     Scratch in_heat, in_paf;  // staging for spg_group_host
     unsigned int *done_counter = nullptr;          // "last CTA done" counter of the in-kernel wire signal
+    unsigned int *score_queue = nullptr;           // 2 x 2 words: item queues of limb_score_persist_kernel (launch_score)
     unsigned long long *armed_flag = nullptr;      // spg_arm_wire_signal: consumed by the next assemble launch
     unsigned long long armed_value = 0;
     Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
@@ -172,7 +173,7 @@ struct ScoreKernels {
     const char *item_name[2];
     void (*ragged[2])(ScoreArgs, ScoreRagged);
     const char *ragged_name[2];
-    void (*persist)(ScoreArgs, int);  // f32 planes only
+    void (*persist)(ScoreArgs, int, unsigned int *);  // f32 planes only
     const char *persist_name;
 };
 
@@ -345,8 +346,13 @@ int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, 
     h->cand_dtype = dtype;
     const ScorePlan pl = plan_score(h, k, paf, img_stride, chan_stride, H, W, true);
     const int grid = n * h->ws.L;
-    if (pl.kind == ScorePlan::kPersist)
-        return launch(h, kStageScore, k.persist_name, k.persist, std::min(grid, h->sm_count), kPersistThreads, pl.smem, st, a, grid);
+    if (pl.kind == ScorePlan::kPersist) {
+        // The kernel leaves its queue at 0 for the next launch on the same stream.  spg_group_host's chunks run on the
+        // handle's two streams and may overlap, so the second stream has a queue of its own.
+        unsigned int *queue = h->score_queue + (st == h->streams[1] ? 2 : 0);
+        return launch(h, kStageScore, k.persist_name, k.persist, std::min(grid, h->sm_count), kPersistThreads, pl.smem, st, a, grid,
+                      queue);
+    }
     return launch(h, kStageScore, k.item_name[pl.kind], k.item[pl.kind], grid, kScoreThreads, pl.smem, st, a);
 }
 
@@ -458,6 +464,17 @@ int spg_trace_read(unsigned long long *out, size_t n_words, int clear) {
     }
     return 0;
 }
+// (start, exit) %globaltimer pairs of the first kTraceSpanCtas CTAs of the traced launches (SPG_TR_CTA_*)
+int spg_trace_read_spans(unsigned long long *out, size_t n_words, int clear) {
+    const size_t n = std::min(n_words, (size_t)2 * spg::kTraceSpanCtas);
+    if (cudaMemcpyFromSymbol(out, spg::g_spg_cta_span, n * sizeof(unsigned long long)) != cudaSuccess) return -1;
+    if (clear) {
+        void *p = nullptr;
+        if (cudaGetSymbolAddress(&p, spg::g_spg_cta_span) != cudaSuccess) return -1;
+        if (cudaMemset(p, 0, sizeof(spg::g_spg_cta_span)) != cudaSuccess) return -1;
+    }
+    return 0;
+}
 #endif
 
 int spg_abi_version(void) { return SPG_ABI_VERSION; }
@@ -531,10 +548,12 @@ int spg_create(const spg_config *cfg, spg_handle **out) {
     A(dalloc(h, &ws.people_xy, N * cR * std::max<size_t>(J, 1) * 2));
     A(dalloc(h, &ws.people_score, N * cR));
     A(dalloc(h, &ws.status, N));
+    A(dalloc(h, &h->score_queue, 4));
     for (size_t i = 0; i < L * 2; i++) ws.limbs[i] = (int16_t)cfg->limbs[i];
     for (size_t g = 0; g < J; g++) ws.out_from_part[g] = (int16_t)cfg->out_from_part[g];
     if (rc == SPG_OK && cudaMemset(ws.status, 0, sizeof(uint32_t) * N) != cudaSuccess) rc = SPG_E_CUDA;
     if (rc == SPG_OK && cudaMemset(ws.peak_count, 0, sizeof(int32_t) * N * K) != cudaSuccess) rc = SPG_E_CUDA;
+    if (rc == SPG_OK && cudaMemset(h->score_queue, 0, sizeof(unsigned int) * 4) != cudaSuccess) rc = SPG_E_CUDA;
     for (int s = 0; s < 2 && rc == SPG_OK; s++)
         if (cudaStreamCreateWithFlags(&h->streams[s], cudaStreamNonBlocking) != cudaSuccess) rc = SPG_E_CUDA;
     if (rc != SPG_OK) {

@@ -9,6 +9,10 @@ after a warm-up pass and splits, per traced CTA (the first 64) and item, the pla
   exact     last screener gone -> last scorer gone (the meta slot, not the plane slot, is held)
   mfree     the loader waiting for a meta slot to come back from the scorers
 
+It also times every CTA's start and exit with %globaltimer (one clock for all SMs) over SPAN_LAUNCHES launches and
+prints the kernel span, the mean and the latest CTA exit and the mean exit per class blockIdx.x mod 6 (item = image * 30
++ limb: under a fixed grid stride of 132 CTAs, class c would only ever score the limbs k = c mod 6).
+
 usage: python tools/trace_limb_score.py [persons] [out.json]"""
 import ctypes as C, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,21 +31,33 @@ prm = skeleton.default_params()
 g = grouping.Grouper(max_batch=NB, max_person_rows=64)
 lib = grouping.load_library()
 lib.spg_trace_read.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
+lib.spg_trace_read_spans.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
+SPAN_CTAS, SPAN_LAUNCHES, CLASSES = 1024, 20, 6   # kTraceSpanCtas
 buf = np.zeros(CTAS * SLOTS, dtype=np.uint64)
+spans = np.zeros(2 * SPAN_CTAS, dtype=np.uint64)
 for _ in range(3):
     g.group_device(hd, pd, 128, prm)
 torch.cuda.synchronize()
 assert lib.spg_trace_read(buf.ctypes.data, buf.size, 1) == 0
+assert lib.spg_trace_read_spans(spans.ctypes.data, spans.size, 1) == 0
 assert "persist" in g.stage_kernels()[1]
-g.limb_score(pd, 128, prm)
-torch.cuda.synchronize()
-assert lib.spg_trace_read(buf.ctypes.data, buf.size, 1) == 0
+exits, kspan = [], []   # per launch: CTA exits after the earliest CTA start (us), kernel span (us)
+for i in range(SPAN_LAUNCHES):
+    g.limb_score(pd, 128, prm)
+    torch.cuda.synchronize()
+    if i == 0:
+        assert lib.spg_trace_read(buf.ctypes.data, buf.size, 1) == 0
+    assert lib.spg_trace_read_spans(spans.ctypes.data, spans.size, 1) == 0
+    s = spans.reshape(SPAN_CTAS, 2).astype(np.int64)
+    s = s[: int(np.count_nonzero(s[:, 0]))]
+    exits.append((s[:, 1] - s[:, 0].min()) / 1e3)
+    kspan.append((s[:, 1].max() - s[:, 0].min()) / 1e3)
 tr = buf.reshape(CTAS, SLOTS // W, W).astype(np.int64)
 
 rows = []
 for b in range(CTAS):
     t = tr[b]
-    nj = int(np.count_nonzero(t[:, 1]))
+    nj = int(np.count_nonzero(t[:, 8]))   # items closed (the end-of-queue header is published but never closed)
     t0 = int(t[0, 0])
     for j in range(nj):
         x = t[j]
@@ -65,3 +81,9 @@ print("cycles per item (mean): slot cycle %.0f = copy %.0f + screen %.0f + wait 
 print("  exact phase after the screen %.0f, loader stalled on mfree %.0f, loader stalled before the copy %.0f" % (
     mean("exact"), mean("mfree"), mean("issue_stall")))
 print("  survivors per item %.1f, candidates per item %.1f" % (mean("surv"), mean("cand")))
+ex = np.mean(exits, axis=0)   # per CTA, mean over the launches
+cls = [float(np.mean(ex[c::CLASSES])) for c in range(CLASSES)]
+print(f"CTA spans (%globaltimer, {len(ex)} CTAs, mean of {SPAN_LAUNCHES} launches, us): kernel span {np.mean(kspan):.1f}, "
+      f"CTA exit mean {ex.mean():.1f} / latest {ex.max():.1f} / earliest {ex.min():.1f} "
+      f"(latest - mean = {100 * (ex.max() - ex.mean()) / np.mean(kspan):.1f} % of the span)")
+print("  mean exit per class blockIdx.x mod %d: %s" % (CLASSES, " / ".join(f"{c}: {v:.1f}" for c, v in enumerate(cls))))
