@@ -470,6 +470,19 @@ __device__ __forceinline__ void post_resize2_h(const PostTabs &T, const float *s
     }
 }
 
+// One image of a ragged launch (postnet_ragged_kernel, postnet_x4_ident_ragged_kernel): one scale, its output planes
+// [K][H][W] / [L][H][W], its own tiling, and the first CTA (blockIdx.x) of its tiles in the launch.  The helpers and
+// kernel bodies below read an image's fields from `im`: the per-launch kernels pass their PostArgs (the same field
+// names), the ragged kernels their image's PostImage.
+struct PostImage {
+    PostScale sc[1];
+    int H, W;
+    float *heat;
+    void *paf;
+    int tile_w, tile_h, tiles_x, tiles_y;
+    int first_cta;
+};
+
 // Where channel c of image n goes: one base pointer per dtype (32-bit offsets from it per thread; the dtype branches are
 // block-uniform), and whether the values stored are float32.
 struct PostOut {
@@ -478,29 +491,30 @@ struct PostOut {
     double *d;
     bool store_f;
 };
-__device__ __forceinline__ PostOut post_out(const PostArgs &a, int n, int c, int ox0, int oy0, bool more_follow) {
-    const size_t plane = (size_t)a.H * a.W;
+template <class I>
+__device__ __forceinline__ PostOut post_out(const PostArgs &a, const I &im, int n, int c, int ox0, int oy0, bool more_follow) {
+    const size_t plane = (size_t)im.H * im.W;
     const bool is_heat = c < a.K;
     PostOut o;
-    o.pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * a.W + ox0;
-    o.f = is_heat ? a.heat + o.pbase : static_cast<float *>(a.paf) + o.pbase;
-    o.d = (is_heat ? a.heat_acc : static_cast<double *>(a.paf)) + (is_heat && a.heat_acc == nullptr ? 0 : o.pbase);
+    o.pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * im.W + ox0;
+    o.f = is_heat ? im.heat + o.pbase : static_cast<float *>(im.paf) + o.pbase;
+    o.d = (is_heat ? a.heat_acc : static_cast<double *>(im.paf)) + (is_heat && a.heat_acc == nullptr ? 0 : o.pbase);
     o.store_f = is_heat ? !more_follow : !a.paf_is_f64;
     return o;
 }
 
 // continuing a scale loop longer than one launch: the float64 sums so far
-template <bool SINGLE>
-__device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, int c,
-                                              size_t pbase, int tw, int th, int lane, int warp) {
+template <bool SINGLE, class I>
+__device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, const I &im,
+                                              int c, size_t pbase, int tw, int th, int lane, int warp) {
     if (!SINGLE && a.scale_index > 0) {
-        const double *prev = c < a.K ? a.heat_acc : static_cast<const double *>(a.paf);
+        const double *prev = c < a.K ? a.heat_acc : static_cast<const double *>(im.paf);
 #pragma unroll
         for (int ky = 0; ky < kPostKY; ky++)
 #pragma unroll
             for (int kx = 0; kx < kPostKX; kx++) {
                 const int y = warp + kPostNW * ky, x = lane + 32 * kx;
-                acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = (y < th && x < tw) ? prev[pbase + (size_t)y * a.W + x] : 0.0;
+                acc[SINGLE ? 0 : ky][SINGLE ? 0 : kx] = (y < th && x < tw) ? prev[pbase + (size_t)y * im.W + x] : 0.0;
             }
     }
 }
@@ -508,9 +522,10 @@ __device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY
 // Pass 4 and epilogue: vertical pass of the second resize (s3; with an identity second resize the crop itself, s2),
 // / n in float32, float64 sum over the scale loop (:160-161) in registers.  SINGLE: the maps are stored from here.
 // (c_org, y_org) is the crop position of element 0 of s2.
-template <bool SINGLE, bool IDENT>
+template <bool SINGLE, bool IDENT, class I>
 __device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostTabs &T,
-                                               const float *s2, const float *s3, bool identity, const PostArgs &a, const PostOut &out,
+                                               const float *s2, const float *s3, bool identity, const PostArgs &a, const I &im,
+                                               const PostOut &out,
                                                int ox0, int oy0, int tw, int th, int c_org, int y_org, bool zero_start,
                                                float nf, float nf_rcp, bool nf_small, int lane, int warp) {
     float r1[SINGLE ? kPostKY : 1][SINGLE ? kPostKX : 1];  // single scale: the values this thread stores
@@ -545,7 +560,7 @@ __device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostK
         }
     }
     if (SINGLE) {  // one block-uniform branch on the output type, then eight stores at constant offsets from one pointer
-        const int o0 = warp * a.W + lane, dy = kPostNW * a.W;
+        const int o0 = warp * im.W + lane, dy = kPostNW * im.W;
         if (out.store_f) {
             float *op = out.f + o0;
 #pragma unroll
@@ -565,14 +580,14 @@ __device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostK
 }
 
 // the averaged maps, written once: keypoint maps as float32 (find_peaks' cast, :173), body parts float64 / float32
-template <bool SINGLE>
-__device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a,
+template <bool SINGLE, class I>
+__device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const I &im,
                                                const PostOut &out, int tw, int th, int lane, int warp) {
     if (!SINGLE) {
 #pragma unroll
         for (int ky = 0; ky < kPostKY; ky++) {
             const int y = warp + kPostNW * ky;
-            const int orow = y * a.W;
+            const int orow = y * im.W;
 #pragma unroll
             for (int kx = 0; kx < kPostKX; kx++) {
                 const int x = lane + 32 * kx;
@@ -589,8 +604,9 @@ __device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : 
 // SINGLE: one scale in the whole loop (the reference's default): no float64 sums, the maps are stored from pass 4.
 // IDENT: every fused scale's second resize is the identity (crop == image: weights (0,1,0,0)) -- passes 3 and 4 fall away.
 // F16: the network output is float16.
-template <bool SINGLE, bool IDENT, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
+// One CTA: tile `tile` of image `im` (slot n of its output planes), channel chunk `chunk`.
+template <bool SINGLE, bool IDENT, bool F16, class I>
+__device__ __forceinline__ void postnet_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
     constexpr int kTabs = SINGLE ? 1 : kPostMaxScales;
     extern __shared__ __align__(16) unsigned char post_smem[];
     PostTabs *TT = reinterpret_cast<PostTabs *>(post_smem);
@@ -600,17 +616,16 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
     float *s3 = s2 + kPostF_R1 * kPostF_C1;                               // after the 2nd resize's h. pass  [4P][kPostTW]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = blockIdx.x, n = blockIdx.z;
-    const int c_begin = blockIdx.y * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
-    const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
-    const int ox0 = tx * a.tile_w, oy0 = ty * a.tile_h;
-    const int tw = min(a.tile_w, a.W - ox0), th = min(a.tile_h, a.H - oy0);
+    const int c_begin = chunk * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
+    const int ty = tile / im.tiles_x, tx = tile - ty * im.tiles_x;
+    const int ox0 = tx * im.tile_w, oy0 = ty * im.tile_h;
+    const int tw = min(im.tile_w, im.W - ox0), th = min(im.tile_h, im.H - oy0);
 
     // ---- once per CTA and scale: everything that depends on the tile position only
     for (int t = 0; t < a.n_fused; t++) {
         PostTabs &T = TT[t];
-        const PostScale &S = a.sc[t];
-        const bool identity = IDENT || (S.crop_h == a.H && S.crop_w == a.W);  // second resize with scale 1: weights (0, 1, 0, 0)
+        const PostScale &S = im.sc[t];
+        const bool identity = IDENT || (S.crop_h == im.H && S.crop_w == im.W);  // second resize with scale 1: weights (0, 1, 0, 0)
         post_tabs_resize2(T, S, ox0, oy0, tw, th, tid);
         if (tid == 0) {
             // crop-coordinate range the tile reads (taps clamped to the cropped array, :148-149)
@@ -626,16 +641,16 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
     const bool more_follow = a.scale_index + a.n_fused < a.n_scales;  // only with more than kPostMaxScales scales
 
     float pv0[kPostKI][kPostKJ], pv1[kPostKI][kPostKJ];
-    if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, a.sc[0], TT[0], a, n, c_begin, warp, lane);
+    if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, im.sc[0], TT[0], a, n, c_begin, warp, lane);
 
     for (int c = c_begin; c < c_end; c++) {
-        const PostOut out = post_out(a, n, c, ox0, oy0, more_follow);
+        const PostOut out = post_out(a, im, n, c, ox0, oy0, more_follow);
         double acc[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX];
-        post_load_acc<SINGLE>(acc, a, c, out.pbase, tw, th, lane, warp);
+        post_load_acc<SINGLE>(acc, a, im, c, out.pbase, tw, th, lane, warp);
         for (int t = 0; t < a.n_fused; t++) {
             const PostTabs &T = TT[t];
-            const PostScale &S = a.sc[t];
-            const bool identity = IDENT || (S.crop_h == a.H && S.crop_w == a.W);
+            const PostScale &S = im.sc[t];
+            const bool identity = IDENT || (S.crop_h == im.H && S.crop_w == im.W);
             const PostRange R = post_range(T);
             const float4 W[4] = {T.wph[0], T.wph[1], T.wph[2], T.wph[3]};
             // ---- source tile.  Its global loads were issued one iteration ago (the chain load -> barrier -> four short
@@ -646,16 +661,21 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
             {
                 int tn = t + 1, cn = c;
                 if (tn == a.n_fused) { tn = 0; cn = c + 1; }
-                if (cn < c_end) post_prefetch<F16>(pv0, pv1, a.sc[tn], TT[tn], a, n, cn, warp, lane);
+                if (cn < c_end) post_prefetch<F16>(pv0, pv1, im.sc[tn], TT[tn], a, n, cn, warp, lane);
             }
             post_x4_passes(T, R, W, s0, s1, s2, tid, lane, warp);  // -> the cropped intermediate (what the reference holds after :148 / :157)
             post_resize2_h<IDENT>(T, s2, s3, identity, tw, th, lane, warp);
-            post_resize2_v<SINGLE, IDENT>(acc, T, s2, s3, identity, a, out, ox0, oy0, tw, th, 4 * R.q_lo, 4 * R.p_lo,
+            post_resize2_v<SINGLE, IDENT>(acc, T, s2, s3, identity, a, im, out, ox0, oy0, tw, th, 4 * R.q_lo, 4 * R.p_lo,
                                           a.scale_index == 0 && t == 0, nf, nf_rcp, nf_small, lane, warp);
             __syncthreads();  // s0..s3 are reused by the next scale / channel
         }
-        post_store_acc<SINGLE>(acc, a, out, tw, th, lane, warp);
+        post_store_acc<SINGLE>(acc, im, out, tw, th, lane, warp);
     }
+}
+
+template <bool SINGLE, bool IDENT, bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
+    postnet_tile<SINGLE, IDENT, F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -767,9 +787,9 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
     float pv0[kPostKI][kPostKJ], pv1[kPostKI][kPostKJ];
     if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c_begin, warp, lane);
     for (int c = c_begin; c < c_end; c++) {
-        const PostOut out = post_out(a, n, c, ox0, oy0, more_follow);
+        const PostOut out = post_out(a, a, n, c, ox0, oy0, more_follow);
         double acc[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX];
-        post_load_acc<SINGLE>(acc, a, c, out.pbase, tw, th, lane, warp);
+        post_load_acc<SINGLE>(acc, a, a, c, out.pbase, tw, th, lane, warp);
         post_commit(s0, pv0, pv1, R, warp, lane);
         __syncthreads();
         if (c + 1 < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c + 1, warp, lane);
@@ -782,7 +802,7 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
         }
         __syncthreads();
         post_resize2_h<false>(T, sr, s3, identity, tw, th, lane, warp);
-        post_resize2_v<SINGLE, false>(acc, T, sr, s3, identity, a, out, ox0, oy0, tw, th, c_lo, y_lo, a.scale_index == 0, nf,
+        post_resize2_v<SINGLE, false>(acc, T, sr, s3, identity, a, a, out, ox0, oy0, tw, th, c_lo, y_lo, a.scale_index == 0, nf,
                                       nf_rcp, nf_small, lane, warp);
         __syncthreads();  // s0 / s3, su and sr are reused by the next channel
         post_store_acc<SINGLE>(acc, a, out, tw, th, lane, warp);
@@ -804,20 +824,20 @@ constexpr int kPostI_RS = kPostI_P + 4, kPostI_CS = kPostI_Q + 4;  // source til
 constexpr int kPostI_S0 = kPostI_CS;                // row stride of the source tile in shared memory
 constexpr int kPostI_LD = (kPostI_RS * kPostI_CS + kPostThreads - 1) / kPostThreads;  // source elements per thread
 
-template <bool F16>
-__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostArgs a) {
+// One CTA: tile `tile` of image `im` (slot n of its output planes), channel chunk `chunk`.
+template <bool F16, class I>
+__device__ __forceinline__ void postnet_x4_ident_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
     __shared__ float s0[2][kPostI_RS * kPostI_S0];                  // source tile, flip-averaged
     __shared__ __align__(16) float s1[2][kPostI_RS * kPostI_TW];   // after the horizontal pass
     __shared__ int s_o1x[kPostI_Q + 1][5], s_o1y[kPostI_P][5];
     __shared__ float4 s_wph[4];
 
     const int tid = threadIdx.x;
-    const PostScale &S = a.sc[0];
-    const int tile = blockIdx.x, n = blockIdx.z;
-    const int c_begin = blockIdx.y * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
-    const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
+    const PostScale &S = im.sc[0];
+    const int c_begin = chunk * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
+    const int ty = tile / im.tiles_x, tx = tile - ty * im.tiles_x;
     const int ox0 = tx * kPostI_TW, oy0 = ty * kPostI_TH;
-    const int tw = min(kPostI_TW, a.W - ox0), th = min(kPostI_TH, a.H - oy0);
+    const int tw = min(kPostI_TW, im.W - ox0), th = min(kPostI_TH, im.H - oy0);
     // crop columns ox0 .. ox0 + tw - 1 = intermediate groups q_lo .. q_lo + Q - 1 (ox0, oy0 are multiples of 4)
     const int q_lo = ox0 >> 2, Q = ((ox0 + tw - 1) >> 2) - q_lo + 1, p_lo = oy0 >> 2, P = ((oy0 + th - 1) >> 2) - p_lo + 1;
     const int sc_lo = max(q_lo - 2, 0), sc_hi = min(q_lo + Q + 1, S.w - 1), sr_lo = max(p_lo - 2, 0), sr_hi = min(p_lo + P + 1, S.h - 1);
@@ -853,7 +873,7 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
         v0 = s_o1y[p2][0] + 4 * x2; v1 = s_o1y[p2][1] + 4 * x2; v2 = s_o1y[p2][2] + 4 * x2; v3 = s_o1y[p2][3] + 4 * x2; v4 = s_o1y[p2][4] + 4 * x2;
     }
     // 16-byte stores need all of the tile's columns and 16-byte aligned rows (W a multiple of 4; float64 rows: always then)
-    const bool vec = tw == kPostI_TW && (a.W & 3) == 0;
+    const bool vec = tw == kPostI_TW && (im.W & 3) == 0;
     // source elements of this thread (row-major over the RS x CS tile)
     long long g0[kPostI_LD], g1[kPostI_LD];
     int sdst[kPostI_LD];
@@ -885,8 +905,8 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
             }
         }
     };
-    const size_t plane = (size_t)a.H * a.W;
-    const size_t othread = (size_t)(oy0 + 4 * p2) * a.W + ox0 + 4 * x2;  // first output of the pass-2 item
+    const size_t plane = (size_t)im.H * im.W;
+    const size_t othread = (size_t)(oy0 + 4 * p2) * im.W + ox0 + 4 * x2;  // first output of the pass-2 item
     // One barrier per channel: the interval between two barriers runs the horizontal pass of channel c (source tile buffer
     // `buf` -> s1[buf]), the vertical pass + stores of channel c - 1 (s1[buf ^ 1]), commits channel c + 1's source tile (loaded
     // one interval ago) to the other s0 buffer and puts channel c + 2's loads in flight.
@@ -940,11 +960,11 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
             const bool is_heat = cp < a.K;
             const size_t pbase = (is_heat ? ((size_t)n * a.K + cp) * plane : ((size_t)n * (a.n_out - a.K) + (cp - a.K)) * plane) + othread;
             if (is_heat || !a.paf_is_f64) {
-                float *of = (is_heat ? a.heat : static_cast<float *>(a.paf)) + pbase;
+                float *of = (is_heat ? im.heat : static_cast<float *>(im.paf)) + pbase;
                 if (vec) {
 #pragma unroll
                     for (int k = 0; k < 4; k++)
-                        if (4 * p2 + k < th) *reinterpret_cast<float4 *>(of + (size_t)k * a.W) = r[k];
+                        if (4 * p2 + k < th) *reinterpret_cast<float4 *>(of + (size_t)k * im.W) = r[k];
                 } else {
 #pragma unroll
                     for (int k = 0; k < 4; k++) {
@@ -952,17 +972,17 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
                             const float e[4] = {r[k].x, r[k].y, r[k].z, r[k].w};
 #pragma unroll
                             for (int x = 0; x < 4; x++)
-                                if (4 * x2 + x < tw) of[(size_t)k * a.W + x] = e[x];
+                                if (4 * x2 + x < tw) of[(size_t)k * im.W + x] = e[x];
                         }
                     }
                 }
             } else {
-                double *od = static_cast<double *>(a.paf) + pbase;
+                double *od = static_cast<double *>(im.paf) + pbase;
                 if (vec) {
 #pragma unroll
                     for (int k = 0; k < 4; k++) {
                         if (4 * p2 + k < th) {
-                            double2 *q = reinterpret_cast<double2 *>(od + (size_t)k * a.W);
+                            double2 *q = reinterpret_cast<double2 *>(od + (size_t)k * im.W);
                             q[0] = make_double2((double)r[k].x, (double)r[k].y);
                             q[1] = make_double2((double)r[k].z, (double)r[k].w);
                         }
@@ -974,7 +994,7 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
                             const float e[4] = {r[k].x, r[k].y, r[k].z, r[k].w};
 #pragma unroll
                             for (int x = 0; x < 4; x++)
-                                if (4 * x2 + x < tw) od[(size_t)k * a.W + x] = (double)e[x];
+                                if (4 * x2 + x < tw) od[(size_t)k * im.W + x] = (double)e[x];
                         }
                     }
                 }
@@ -986,6 +1006,48 @@ __global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostA
         }
         __syncthreads();
     }
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostArgs a) {
+    postnet_x4_ident_tile<F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Ragged batches: one single-scale, unrotated, stride-4 item per image, images of different sizes in one launch (what
+// predict() runs per image, for a batch of images).  grid.x walks the images' tiles back to back, grid.y the channel
+// chunks (one chunk size per launch).  Each CTA runs the per-launch kernel's body on its image's geometry, so every image
+// gets exactly the maps a launch of its own gives it.  The host puts identity items (crop == image) and the others in
+// separate launches, largest image first.
+// Images per launch; the descriptors travel as a kernel parameter (PostArgs + 64 x 136 B, inside the 32 764 bytes CUDA
+// 12.1 allows), so a call returns with nothing of the caller's left to copy.
+constexpr int kPostRaggedMaxImages = 64;
+struct PostRagged {
+    int n;                                  // images of this launch
+    PostImage img[kPostRaggedMaxImages];    // first_cta increasing
+};
+
+// the image whose tiles hold CTA `cta`: the last one whose first CTA is <= cta
+__device__ __forceinline__ const PostImage &post_ragged_image(const PostRagged &r, int cta) {
+    int lo = 0, hi = r.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (r.img[mid].first_cta <= cta) lo = mid;
+        else hi = mid - 1;
+    }
+    return r.img[lo];
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_ragged_kernel(PostArgs a, const __grid_constant__ PostRagged r) {
+    const PostImage &im = post_ragged_image(r, blockIdx.x);
+    postnet_x4_ident_tile<F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_ragged_kernel(PostArgs a, const __grid_constant__ PostRagged r) {
+    const PostImage &im = post_ragged_image(r, blockIdx.x);
+    postnet_tile<true, false, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 
 }  // namespace spg

@@ -356,20 +356,30 @@ int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, 
     return launch(h, kStageScore, k.item_name[pl.kind], k.item[pl.kind], grid, kScoreThreads, pl.smem, st, a);
 }
 
-// Images of a ragged call, as many per launch as the descriptor struct holds (it travels as the kernel parameter), with
-// `per_image` CTAs each.
-template <typename Args, typename Ragged, typename Image>
-int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), int per_image, int block, size_t smem,
-                  cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
+// Images of a ragged call, as many per launch as the descriptor struct holds (it travels as the kernel parameter).
+// place(r, k, x) puts image k of the launch's descriptors r at grid.x position x and returns its CTA count; grid.y is
+// grid_y.  The caller keeps a launch inside the grid limits (the validation of its images).
+template <typename Args, typename Ragged, typename Image, typename Place>
+int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), Place place, int grid_y, int block,
+                  size_t smem, cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
     constexpr size_t cap = sizeof(Ragged::img) / sizeof(Image);
     for (size_t i0 = 0; i0 < imgs.size(); i0 += cap) {
         const size_t cnt = std::min(cap, imgs.size() - i0);
         Ragged r{};
         std::copy(imgs.begin() + i0, imgs.begin() + i0 + cnt, r.img);
+        int x = 0;
+        for (size_t k = 0; k < cnt; k++) x += place(r, (int)k, x);
         int rc;
-        if ((rc = launch(h, stage, name, kern, (int)cnt * per_image, block, smem, st, a, r))) return rc;
+        if ((rc = launch(h, stage, name, kern, dim3((unsigned)x, (unsigned)grid_y), block, smem, st, a, r))) return rc;
     }
     return SPG_OK;
+}
+
+// ... with `per_image` CTAs each
+template <typename Args, typename Ragged, typename Image>
+int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), int per_image, int block, size_t smem,
+                  cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
+    return launch_ragged(h, stage, name, kern, [per_image](Ragged &, int, int) { return per_image; }, 1, block, smem, st, a, imgs);
 }
 
 int launch_match(spg_handle *h, int base, int n, cudaStream_t st) {
@@ -744,15 +754,69 @@ static void invert_affine(const double *M, double *m) {
 // The grid over output tiles of a.tile_w x a.tile_h: a CTA builds its tile's tables once and walks over a chunk of
 // channels -- as many as still leave ~ctas_per_sm CTAs per SM in the grid (a few resident: several waves).
 // ctas_per_sm 0: one channel per CTA.
+static int post_chan_chunk(const spg_handle *h, int n_out, long long tiles, int ctas_per_sm) {
+    const int n_chunks = ctas_per_sm == 0 ? n_out
+                                          : (int)std::min<long long>(n_out, std::max<long long>(1, ((long long)h->sm_count * ctas_per_sm + tiles - 1) / tiles));
+    return (n_out + n_chunks - 1) / n_chunks;
+}
+
 static int postnet_grid(spg_handle *h, PostArgs &a, int n, int ctas_per_sm, dim3 *grid) {
     a.tiles_x = (a.W + a.tile_w - 1) / a.tile_w;
     a.tiles_y = (a.H + a.tile_h - 1) / a.tile_h;
     if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
-    const long long tiles = (long long)a.tiles_x * a.tiles_y * n;
-    const int n_chunks = ctas_per_sm == 0 ? a.n_out
-                                          : (int)std::min<long long>(a.n_out, std::max<long long>(1, ((long long)h->sm_count * ctas_per_sm + tiles - 1) / tiles));
-    a.chan_chunk = (a.n_out + n_chunks - 1) / n_chunks;
+    a.chan_chunk = post_chan_chunk(h, a.n_out, (long long)a.tiles_x * a.tiles_y * n, ctas_per_sm);
     *grid = dim3((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
+    return SPG_OK;
+}
+
+// CTAs per SM the channel chunks aim at: the identity kernel (4 resident per SM) and the four-phase kernel (2 resident)
+constexpr int kPostIdentCtasPerSm = 32, kPostCtasPerSm = 16;
+
+// output tile of the four-phase kernels: as large as the shared-memory tiles of the intermediate / source allow
+static int post_tile_dim(double s2, double s1, int cap1, int cap0, int maxd, double margin) {
+    const double c1 = std::min((double)cap1, ((double)cap0 - 7.0) / s1) - margin;  // intermediate span allowed
+    return std::max(1, std::min(maxd, (int)(c1 / std::max(s2, 1e-6))));
+}
+
+// shrink the four-phase kernel's output tile (tw x th) until it fits item S's second resize
+static void post_tile_fit(const PostScale &S, double s1, int &tw, int &th) {
+    tw = std::min(tw, post_tile_dim(S.sx2, s1, kPostF_C1, kPostF_CS, kPostTW, 13.0));
+    th = std::min(th, post_tile_dim(S.sy2, s1, kPostF_R1, kPostF_RS, kPostTH, 13.0));
+}
+
+// one item's network output and the steps of its resize to the H x W image
+static PostScale post_scale(const void *net, int dtype, int64_t img_stride, int64_t pair_stride, int64_t chan_stride, int h, int w,
+                            int crop_h, int crop_w, int H, int W) {
+    PostScale s{};
+    s.net = net; s.net_is_f16 = dtype == SPG_F16;
+    s.img_stride = img_stride; s.pair_stride = pair_stride; s.chan_stride = chan_stride;
+    s.h = h; s.w = w; s.crop_h = crop_h; s.crop_w = crop_w;
+    // cv2.resize(dsize): inv_scale = dst/src, scale = 1/inv_scale (two roundings, as OpenCV)
+    s.sx2 = 1.0 / ((double)W / (double)crop_w);
+    s.sy2 = 1.0 / ((double)H / (double)crop_h);
+    return s;
+}
+
+static bool post_crop_fits(int h, int w, int crop_h, int crop_w, int stride) {
+    return h >= 1 && w >= 1 && crop_h >= 1 && crop_w >= 1 && crop_h <= h * stride && crop_w <= w * stride;
+}
+
+// the output channels (K keypoint, then L body part) and the network channels each one averages, validated
+static int post_channels(spg_handle *h, int paf_chan0, int heat_chan0, const int32_t *flip_paf_ord, const int32_t *flip_heat_ord,
+                         PostArgs &a) {
+    const Workspace &ws = h->ws;
+    if (ws.K + ws.L > kMaxNetChannels) return fail(h, SPG_E_INVALID, "too many channels for postnet");
+    a.n_out = ws.K + ws.L; a.K = ws.K;
+    for (int c = 0; c < ws.K; c++) {
+        if (flip_heat_ord[c] < 0 || flip_heat_ord[c] >= ws.K) return fail(h, SPG_E_INVALID, "flip_heat_ord[%d] out of range", c);
+        a.src_chan[c] = (short)(heat_chan0 + c);
+        a.flip_chan[c] = (short)(heat_chan0 + flip_heat_ord[c]);
+    }
+    for (int k = 0; k < ws.L; k++) {
+        if (flip_paf_ord[k] < 0 || flip_paf_ord[k] >= ws.L) return fail(h, SPG_E_INVALID, "flip_paf_ord[%d] out of range", k);
+        a.src_chan[ws.K + k] = (short)(paf_chan0 + k);
+        a.flip_chan[ws.K + k] = (short)(paf_chan0 + flip_paf_ord[k]);
+    }
     return SPG_OK;
 }
 
@@ -778,25 +842,15 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     if ((rc = check_dims(h, n, H, W))) return rc;
     if (n == 0) return SPG_OK;
     const Workspace &ws = h->ws;
-    if (ws.K + ws.L > kMaxNetChannels) return fail(h, SPG_E_INVALID, "too many channels for postnet");
+    // validate every scale and fill the common arguments
+    PostArgs a{};
+    if ((rc = post_channels(h, d->paf_chan0, d->heat_chan0, d->flip_paf_ord, d->flip_heat_ord, a))) return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
         if ((rc = grow(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double)))) return rc;
     }
-    // validate every scale and fill the common arguments
-    PostArgs a{};
-    a.stride = d->stride; a.H = H; a.W = W; a.n_out = ws.K + ws.L; a.K = ws.K;
-    for (int c = 0; c < ws.K; c++) {
-        if (d->flip_heat_ord[c] < 0 || d->flip_heat_ord[c] >= ws.K) return fail(h, SPG_E_INVALID, "flip_heat_ord[%d] out of range", c);
-        a.src_chan[c] = (short)(d->heat_chan0 + c);
-        a.flip_chan[c] = (short)(d->heat_chan0 + d->flip_heat_ord[c]);
-    }
-    for (int k = 0; k < ws.L; k++) {
-        if (d->flip_paf_ord[k] < 0 || d->flip_paf_ord[k] >= ws.L) return fail(h, SPG_E_INVALID, "flip_paf_ord[%d] out of range", k);
-        a.src_chan[ws.K + k] = (short)(d->paf_chan0 + k);
-        a.flip_chan[ws.K + k] = (short)(d->paf_chan0 + d->flip_paf_ord[k]);
-    }
+    a.stride = d->stride; a.H = H; a.W = W;
     a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p); a.paf_is_f64 = paf_dtype == SPG_F64;
     a.n_scales = d->n_scales; a.nan_scrub = d->nan_scrub != 0;
     a.sx1 = 1.0 / (double)d->stride; a.sy1 = a.sx1;  // cv2.resize(fx = stride): scale = 1/fx
@@ -804,23 +858,11 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         const spg_postnet_scale &sc = d->scales[t];
         if (!sc.net_out) return fail(h, SPG_E_INVALID, "scale %d: net_out is NULL", t);
         if (sc.dtype != SPG_F32 && sc.dtype != SPG_F16) return fail(h, SPG_E_INVALID, "scale %d: network output must be SPG_F32 or SPG_F16", t);
-        if (sc.h < 1 || sc.w < 1 || sc.crop_h < 1 || sc.crop_w < 1 || sc.crop_h > sc.h * d->stride || sc.crop_w > sc.w * d->stride)
+        if (!post_crop_fits(sc.h, sc.w, sc.crop_h, sc.crop_w, d->stride))
             return fail(h, SPG_E_INVALID, "scale %d: crop %dx%d does not fit the up-sampled %dx%d output", t, sc.crop_h, sc.crop_w, sc.h * d->stride, sc.w * d->stride);
     }
     auto scale_of = [&](const spg_postnet_scale &sc) {
-        PostScale s{};
-        s.net = sc.net_out; s.net_is_f16 = sc.dtype == SPG_F16;
-        s.img_stride = sc.image_stride; s.pair_stride = sc.pair_stride; s.chan_stride = sc.chan_stride;
-        s.h = sc.h; s.w = sc.w; s.crop_h = sc.crop_h; s.crop_w = sc.crop_w;
-        // cv2.resize(dsize): inv_scale = dst/src, scale = 1/inv_scale (two roundings, as OpenCV)
-        s.sx2 = 1.0 / ((double)W / (double)sc.crop_w);
-        s.sy2 = 1.0 / ((double)H / (double)sc.crop_h);
-        return s;
-    };
-    // output tile: as large as the shared-memory tiles of the intermediate / source allow
-    auto tile_dim = [&](double s2, double s1, int cap1, int cap0, int maxd, double margin) {
-        const double c1 = std::min((double)cap1, ((double)cap0 - 7.0) / s1) - margin;  // intermediate span allowed
-        return std::max(1, std::min(maxd, (int)(c1 / std::max(s2, 1e-6))));
+        return post_scale(sc.net_out, sc.dtype, sc.image_stride, sc.pair_stride, sc.chan_stride, sc.h, sc.w, sc.crop_h, sc.crop_w, H, W);
     };
     dim3 grid;
     const bool single = d->n_scales == 1;
@@ -864,8 +906,7 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
             a.tile_w = kPostTW; a.tile_h = kPostTH;
             for (int t = 0; t < a.n_fused; t++) {
                 a.sc[t] = scale_of(d->scales[t0 + t]);
-                a.tile_w = std::min(a.tile_w, tile_dim(a.sc[t].sx2, a.sx1, kPostF_C1, kPostF_CS, kPostTW, 13.0));
-                a.tile_h = std::min(a.tile_h, tile_dim(a.sc[t].sy2, a.sy1, kPostF_R1, kPostF_RS, kPostTH, 13.0));
+                post_tile_fit(a.sc[t], a.sx1, a.tile_w, a.tile_h);
             }
             bool ident = true, any16 = false, all16 = true;
             for (int t = 0; t < a.n_fused; t++) {
@@ -876,11 +917,11 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
             if (any16 != all16) return fail(h, SPG_E_INVALID, "the network outputs of all scales must have the same dtype");
             if (single && ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
                 a.tile_w = kPostI_TW; a.tile_h = kPostI_TH;
-                if ((rc = postnet_grid(h, a, n, 32, &grid))) return rc;
+                if ((rc = postnet_grid(h, a, n, kPostIdentCtasPerSm, &grid))) return rc;
                 rc = launch(h, kStagePostnet, "postnet_x4_ident_kernel", all16 ? postnet_x4_ident_kernel<true> : postnet_x4_ident_kernel<false>,
                             grid, kPostThreads, 0, st, a);
             } else {
-                if ((rc = postnet_grid(h, a, n, 16, &grid))) return rc;
+                if ((rc = postnet_grid(h, a, n, kPostCtasPerSm, &grid))) return rc;
                 void (*kern)(PostArgs) = single  ? (all16 ? postnet_kernel<true, false, true> : postnet_kernel<true, false, false>)
                                          : ident ? (all16 ? postnet_kernel<false, true, true> : postnet_kernel<false, true, false>)
                                                  : (all16 ? postnet_kernel<false, false, true> : postnet_kernel<false, false, false>);
@@ -895,10 +936,93 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
         a.net = s.net; a.net_is_f16 = s.net_is_f16; a.img_stride = s.img_stride; a.pair_stride = s.pair_stride; a.chan_stride = s.chan_stride;
         a.h = s.h; a.w = s.w; a.crop_h = s.crop_h; a.crop_w = s.crop_w; a.sx2 = s.sx2; a.sy2 = s.sy2;
         a.scale_index = t;
-        a.tile_w = tile_dim(a.sx2, a.sx1, kPostC1, kPostCS, kPostTW, 7.0);
-        a.tile_h = tile_dim(a.sy2, a.sy1, kPostR1, kPostRS, kPostTH, 7.0);
+        a.tile_w = post_tile_dim(a.sx2, a.sx1, kPostC1, kPostCS, kPostTW, 7.0);
+        a.tile_h = post_tile_dim(a.sy2, a.sy1, kPostR1, kPostRS, kPostTH, 7.0);
         if ((rc = postnet_grid(h, a, n, 0, &grid)) ||
             (rc = launch(h, kStagePostnet, "postnet_generic_kernel", postnet_generic_kernel, grid, kPostThreads, 0, st, a)))
+            return rc;
+    }
+    return SPG_OK;
+}
+
+// Ragged batches of single-item images: the identity items (crop == image) in postnet_x4_ident_ragged_kernel launches,
+// the others in postnet_ragged_kernel launches -- the kernels and tiles spg_postnet picks for each image alone -- images
+// largest first, one channel chunk per kernel for all its launches.
+int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *images, int32_t n, int32_t paf_dtype,
+                       void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    if ((rc = check_batch(h, n))) return rc;
+    if (!images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
+    if (!cm || !cm->flip_paf_ord || !cm->flip_heat_ord) return fail(h, SPG_E_INVALID, "postnet common descriptor incomplete");
+    if (cm->stride != 4) return fail(h, SPG_E_INVALID, "the ragged post-network stage needs stride 4 (got %d)", cm->stride);
+    if (cm->net_dtype != SPG_F32 && cm->net_dtype != SPG_F16) return fail(h, SPG_E_INVALID, "network output must be SPG_F32 or SPG_F16");
+    if (paf_dtype != SPG_F32 && paf_dtype != SPG_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32 or SPG_F64");
+    PostArgs a{};
+    if ((rc = post_channels(h, cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord, a))) return rc;
+    a.stride = 4; a.n_fused = 1; a.n_scales = 1; a.scale_index = 0;
+    a.paf_is_f64 = paf_dtype == SPG_F64; a.nan_scrub = cm->nan_scrub != 0;
+    a.sx1 = 0.25; a.sy1 = 0.25;
+    // validate every image before the first launch
+    const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
+    std::vector<int> order((size_t)n);
+    std::vector<PostImage> descs((size_t)n);
+    for (int i = 0; i < n; i++) {
+        const spg_postnet_image &im = images[i];
+        if (!im.net_out || !im.heat_out || !im.paf_out) return fail(h, SPG_E_INVALID, "image %d: net_out/heat_out/paf_out is NULL", i);
+        // the kernels store rows of 4 values with 16-byte stores (postnet_x4_ident_tile)
+        if ((reinterpret_cast<uintptr_t>(im.heat_out) & 15) || (reinterpret_cast<uintptr_t>(im.paf_out) & 15))
+            return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out must be 16-byte aligned", i);
+        if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
+            return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
+        if (!post_crop_fits(im.h, im.w, im.crop_h, im.crop_w, 4))
+            return fail(h, SPG_E_INVALID, "image %d: crop %dx%d does not fit the up-sampled %dx%d output", i, im.crop_h, im.crop_w, 4 * im.h, 4 * im.w);
+        if (im.pair_stride < 0 || im.chan_stride < 0) return fail(h, SPG_E_INVALID, "image %d: negative stride", i);
+        PostImage &d = descs[(size_t)i];
+        d.sc[0] = post_scale(im.net_out, cm->net_dtype, 0, im.pair_stride, im.chan_stride, im.h, im.w, im.crop_h, im.crop_w, im.height, im.width);
+        d.H = im.height; d.W = im.width; d.heat = im.heat_out; d.paf = im.paf_out;
+        if (im.crop_h == im.height && im.crop_w == im.width) {
+            d.tile_w = kPostI_TW; d.tile_h = kPostI_TH;
+        } else {
+            d.tile_w = kPostTW; d.tile_h = kPostTH;
+            post_tile_fit(d.sc[0], a.sx1, d.tile_w, d.tile_h);
+        }
+        d.tiles_x = (d.W + d.tile_w - 1) / d.tile_w;
+        d.tiles_y = (d.H + d.tile_h - 1) / d.tile_h;
+        if ((long long)d.tiles_x * d.tiles_y * kPostRaggedMaxImages > 0x7fffffffLL)
+            return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
+        order[(size_t)i] = i;
+    }
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
+        return (int64_t)images[x].height * images[x].width > (int64_t)images[y].height * images[y].width;
+    });
+    std::vector<PostImage> ident, other;
+    long long ident_tiles = 0, other_tiles = 0;
+    for (int i : order) {
+        const PostImage &d = descs[(size_t)i];
+        const bool id = images[i].crop_h == d.H && images[i].crop_w == d.W;
+        (id ? ident : other).push_back(d);
+        (id ? ident_tiles : other_tiles) += (long long)d.tiles_x * d.tiles_y;
+    }
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool f16 = cm->net_dtype == SPG_F16;
+    auto place = [](PostRagged &r, int k, int x) {
+        r.img[k].first_cta = x;
+        r.n = k + 1;
+        return r.img[k].tiles_x * r.img[k].tiles_y;
+    };
+    if (!ident.empty()) {
+        a.chan_chunk = post_chan_chunk(h, a.n_out, ident_tiles, kPostIdentCtasPerSm);
+        if ((rc = launch_ragged(h, kStagePostnet, "postnet_x4_ident_ragged_kernel",
+                                f16 ? postnet_x4_ident_ragged_kernel<true> : postnet_x4_ident_ragged_kernel<false>, place,
+                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, 0, st, a, ident)))
+            return rc;
+    }
+    if (!other.empty()) {
+        a.chan_chunk = post_chan_chunk(h, a.n_out, other_tiles, kPostCtasPerSm);
+        if ((rc = launch_ragged(h, kStagePostnet, "postnet_ragged_kernel", f16 ? postnet_ragged_kernel<true> : postnet_ragged_kernel<false>,
+                                place, (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, postF_smem_bytes(1), st, a, other)))
             return rc;
     }
     return SPG_OK;

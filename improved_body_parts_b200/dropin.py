@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .grouping import Grouper, GroupingError, GroupResult
+from .grouping import Grouper, GroupingError, GroupResult, clamp_scale, input_geometry
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -198,30 +198,137 @@ def predict(image, params, model, model_params, heat_layers=None, paf_layers=Non
                               stride=int(model_params["stride"]), nan_scrub=_variant == "demo",
                               rotations=[r for _, _, r in items])
         return DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)
-    import cv2
     outs, crops, rotations = [], [], []
     for scale, angle in itertools.product(multiplier, params["rotation_search"]):
-        if scale * image.shape[0] > 2600 or scale * image.shape[1] > 3800:  # evaluate.py:94-96
-            scale = min(2600 / image.shape[0], 3800 / image.shape[1])
-        image_to_test = cv2.resize(image, (0, 0), fx=scale, fy=scale, interpolation=cv2.INTER_CUBIC)
-        padded, _ = pad_right_down_corner(image_to_test, model_params["max_downsample"], model_params["padValue"])
-        input_img = np.float32(padded / 255)
-        reverse = None
-        if angle != 0:  # evaluate.py:113-117, the centre's x and y swapped as there
-            centre = (input_img.shape[0] / 2, input_img.shape[1] / 2)
-            reverse = cv2.getRotationMatrix2D(centre, -angle, 1)
-            input_img = cv2.warpAffine(input_img, cv2.getRotationMatrix2D(centre, angle, 1), (0, 0))
-        pair = np.concatenate((input_img[None, ...], input_img[:, ::-1, :].copy()[None, ...]), axis=0)
+        pair, crop, reverse = _host_pair(image, clamp_scale(scale, image.shape[:2]), angle, model_params)
         with torch.no_grad():
-            out = model(torch.from_numpy(pair).to(f"cuda:{_device}"))[-1][0]  # last stack, finest scale (:126)
-        if out.dtype not in (torch.float32, torch.float16):
-            out = out.float()
+            out = _network_output(model, torch.from_numpy(pair).to(f"cuda:{_device}"))
         outs.append(out[None].contiguous())
-        crops.append(image_to_test.shape[:2])
+        crops.append(crop)
         rotations.append(reverse)
     heat, paf = g.postnet(outs, crops, image.shape[:2], stride=int(model_params["stride"]), nan_scrub=_variant == "demo",
                           rotations=rotations)
     return DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)
+
+
+def _host_pair(image: np.ndarray, scale: float, angle: float, model_params, out: Optional[np.ndarray] = None):
+    """evaluate.py:98-117 for one item with cv2 on the host: ``(pair, crop, rotate_matrix_reverse)`` -- ``pair`` the
+    ``[2, Hp, Wp, 3]`` float32 network input (image, mirror), written into ``out`` when given; ``crop`` =
+    ``imageToTest.shape[:2]``; the reverse matrix is ``None`` for angle 0.  ``scale`` is already clamped."""
+    import cv2
+    image_to_test = cv2.resize(image, (0, 0), fx=scale, fy=scale, interpolation=cv2.INTER_CUBIC)
+    padded, _ = pad_right_down_corner(image_to_test, model_params["max_downsample"], model_params["padValue"])
+    input_img = np.float32(padded / 255)
+    reverse = None
+    if angle != 0:  # evaluate.py:113-117, the centre's x and y swapped as there
+        centre = (input_img.shape[0] / 2, input_img.shape[1] / 2)
+        reverse = cv2.getRotationMatrix2D(centre, -angle, 1)
+        input_img = cv2.warpAffine(input_img, cv2.getRotationMatrix2D(centre, angle, 1), (0, 0))
+    if out is None:
+        out = np.empty((2,) + input_img.shape, np.float32)
+    out[0] = input_img
+    out[1] = input_img[:, ::-1, :]
+    return out, image_to_test.shape[:2], reverse
+
+
+def _network_output(model, x):
+    """The network's maps for the input batch ``x`` (evaluate.py:124-126): the last stack's finest scale, float32 unless
+    the network answers in float16."""
+    import torch
+    out = model(x)[-1][0]
+    if out.dtype not in (torch.float32, torch.float16):
+        out = out.float()
+    return out
+
+
+def _single_item(params, model_params) -> bool:
+    """One unrotated item per image at stride 4: the configuration ``predict_batch`` batches (the reference's default)."""
+    return len(params["scale_search"]) == 1 and len(params["rotation_search"]) == 1 and \
+        params["rotation_search"][0] == 0 and int(model_params["stride"]) == 4
+
+
+def plan_buckets(image_shapes, params, model_params):
+    """The batches of ``predict_batch``: per image ``(multiplier, scale, H1, W1, Hp, Wp)`` of its one item (the
+    multiplier of evaluate.py:87, the scale after the clamp of :94-96, the crop size and the padded network input size of
+    :98-100), and the images grouped by network input size ``{(Hp, Wp): [image index, ...]}`` in order of first
+    appearance."""
+    plan, buckets = [], {}
+    for i, shape in enumerate(image_shapes):
+        h, w = int(shape[0]), int(shape[1])
+        multiplier = params["scale_search"][0] * model_params["boxsize"] / h
+        scale = clamp_scale(multiplier, (h, w))
+        geo = input_geometry(h, w, scale, int(model_params["max_downsample"]))
+        plan.append((multiplier, scale) + geo)
+        buckets.setdefault(geo[2:], []).append(i)
+    return plan, buckets
+
+
+def _pinned_pairs(n_floats: int):
+    """A pinned float32 staging buffer of at least ``n_floats`` for ``predict_batch``'s host input stage, once the copy
+    out of its previous contents has left it."""
+    import torch
+    buf, ev = _staging.get("pairs"), _staging.get("pairs_event")
+    if ev is not None:
+        ev.synchronize()
+    if buf is None or buf.numel() < n_floats:
+        buf = torch.empty(n_floats, dtype=torch.float32, pin_memory=True)
+        _staging["pairs"] = buf
+    return buf
+
+
+def predict_batch(images, params, model, model_params, *, forward_batch: int, input_stage: Optional[str] = None):
+    """``predict`` for several images at once: one ``(heatmap, paf)`` pair of ``DeviceMaps`` per image, in input order.
+
+    With one unrotated item per image at stride 4 (the reference's settings), images whose network inputs have the same
+    padded size ``(Hp, Wp)`` share forward passes of at most ``forward_batch`` images (``2 * forward_batch`` samples:
+    each image and its mirror), and one ``spg_postnet_ragged`` call runs the post-network stage of the whole batch,
+    reading each image's pair out of its forward pass in place.  The inputs are built per image as ``predict`` builds
+    them (``input_stage`` as there) into one tensor per size.  Every kernel treats each image on its own, so the maps
+    equal ``predict``'s bit for bit when the network's output for a sample does not depend on the batch it runs in (a
+    network under cuDNN may pick another algorithm for another batch size).  Other configurations (several scales, a
+    rotation search, another stride) run ``predict`` per image."""
+    import torch
+    stage = _input_stage if input_stage is None else input_stage
+    if stage not in ("host", "device"):
+        raise ValueError("input_stage must be 'host' or 'device'")
+    if int(forward_batch) < 1:
+        raise ValueError("forward_batch must be >= 1")
+    images = list(images)
+    if not _single_item(params, model_params):
+        return [predict(img, params, model, model_params, input_stage=stage) for img in images]
+    fb = int(forward_batch)
+    md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
+    plan, buckets = plan_buckets([img.shape[:2] for img in images], params, model_params)
+    g = _grouper_many(len(images))
+    dev = f"cuda:{_device}"
+    entries = [None] * len(images)
+    for (Hp, Wp), idx in buckets.items():
+        k = len(idx)
+        x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
+        crops = []
+        if stage == "host":
+            host = _pinned_pairs(x.numel())[:x.numel()].view(x.shape)
+            for j, i in enumerate(idx):
+                crops.append(_host_pair(images[i], plan[i][1], 0, model_params, out=host[2 * j:2 * j + 2].numpy())[1])
+            x.copy_(host, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(_device))
+            _staging["pairs_event"] = ev
+        else:
+            for j, i in enumerate(idx):
+                img = images[i] if isinstance(images[i], torch.Tensor) else _upload_image(images[i])
+                (_, crop, _), = g.prenet(img.to(dev), [plan[i][0]], [0], max_downsample=md, pad_value=pv,
+                                         out=[x[2 * j:2 * j + 2]])
+                crops.append(crop)
+        for c0 in range(0, k, fb):
+            c1 = min(k, c0 + fb)
+            with torch.no_grad():
+                out = _network_output(model, x[2 * c0:2 * c1]).contiguous()
+            for j in range(c0, c1):
+                i = idx[j]
+                entries[i] = (out[2 * (j - c0):2 * (j - c0) + 2], crops[j], tuple(int(v) for v in images[i].shape[:2]))
+    maps = g.postnet_ragged(entries, nan_scrub=_variant == "demo")
+    return [(DeviceMaps(heat, False), DeviceMaps(paf, True)) for heat, paf in maps]
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:
@@ -400,29 +507,35 @@ def _people_of_batch(maps, extents, params) -> list:
 
 
 def predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers,
-                 batch: int = 16, image_name=None):
+                 batch: int = 16, image_name=None, forward_batch: int = 1):
     """evaluate.py:550-560 with the grouping of ``batch`` images at a time in one call.
 
     Same arguments, assert and result as the reference's ``predict_many``: ``{image_id: [([17 x (x, y)], score)]}`` in
     ``validation_ids`` order, with ``np.float64`` coordinates and scores and integer ``(0, 0)`` for a missing joint, so
     ``format_results`` writes the same file.  Per image: ``cv2.imread`` and ``predict`` (the maps stay on the device);
     every ``batch`` images and at the end: one ``group_many``-style ragged call, the batch's wire records in one copy.
-    A non-zero status raises ``GroupingError``.  ``image_name(coco, image_id)`` gives the file name (default:
-    ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()`` is not called, so the reference's
-    ``batch_time`` meter is not updated."""
+    ``forward_batch > 1`` runs ``predict_batch`` on each group of ``batch`` images instead of ``predict`` per image (see
+    there for when its maps equal ``predict``'s).  A non-zero status raises ``GroupingError``.  ``image_name(coco,
+    image_id)`` gives the file name (default: ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()``
+    is not called, so the reference's ``batch_time`` meter is not updated."""
     import os
 
     import cv2
     assert (not set(validation_ids).difference(set(coco.getImgIds())))
     if int(batch) < 1:
         raise ValueError("batch must be >= 1")
+    if int(forward_batch) < 1:
+        raise ValueError("forward_batch must be >= 1")
     keypoints = {}
-    pending = []  # (image_id, heatmap, paf, oriImg.shape[0])
+    pending = []  # (image_id, (heatmap, paf) -- or the image itself for predict_batch, oriImg.shape[0])
 
     def flush():
         if pending:
-            people = _people_of_batch([(h, p) for _, h, p, _ in pending], [e for _, _, _, e in pending], params)
-            for (iid, _, _, _), kp in zip(pending, people):
+            maps = [m for _, m, _ in pending]
+            if int(forward_batch) > 1:
+                maps = predict_batch(maps, dict(params), model, dict(model_params), forward_batch=int(forward_batch))
+            people = _people_of_batch(maps, [e for _, _, e in pending], params)
+            for (iid, _, _), kp in zip(pending, people):
                 keypoints[iid] = kp
             pending.clear()
 
@@ -430,8 +543,11 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
         name = image_name(coco, image_id) if image_name is not None else coco.imgs[image_id]["file_name"]
         path = os.path.join(images_directory, name)
         ori = cv2.imread(path)  # B,G,R order (evaluate.py:502)
-        heat, paf = predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path)
-        pending.append((image_id, heat, paf, ori.shape[0]))
+        if int(forward_batch) > 1:
+            pending.append((image_id, ori, ori.shape[0]))
+        else:
+            pending.append((image_id, predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path),
+                            ori.shape[0]))
         if len(pending) >= int(batch):
             flush()
     flush()
@@ -480,7 +596,8 @@ def keypoint_heatmap_nms(heat, kernel: int = 3, thre: float = 0.1):
     return out.to(heat.device)
 
 
-def install(evaluate_module, device_predict: bool = False, device_input: bool = False, batch: int = 1) -> None:
+def install(evaluate_module, device_predict: bool = False, device_input: bool = False, batch: int = 1,
+            forward_batch: int = 1) -> None:
     """Rebind ``find_peaks / find_connections / find_people`` of an imported reference ``evaluate`` module.
 
     ``limbSeq`` is taken from the module (evaluate.py:54) so alternative skeletons keep working.  With
@@ -489,9 +606,15 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     ``device_input`` (with ``device_predict``) also builds the network's input on the GPU (``input_stage="device"``).
     ``batch > 1`` (with ``device_predict``) also replaces ``predict_many`` (:550-560) by ``predict_many`` above, which
     groups ``batch`` images per call; it uses the module's ``posenet`` and ``get_image_name`` and leaves the module's
-    ``batch_time`` meter alone."""
+    ``batch_time`` meter alone.  ``forward_batch > 1`` (with ``device_predict`` and ``batch > 1``) makes that
+    ``predict_many`` run the network on up to ``forward_batch`` images of the same input size at once
+    (``predict_batch``)."""
     if int(batch) > 1 and not device_predict:
         raise ValueError("batch > 1 needs device_predict=True: the batched grouping takes the maps predict() leaves on the device")
+    if int(forward_batch) < 1:
+        raise ValueError("forward_batch must be >= 1")
+    if int(forward_batch) > 1 and (not device_predict or int(batch) < 2):
+        raise ValueError("forward_batch > 1 needs device_predict=True and batch > 1: it batches predict_many's forward passes")
     configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host")
     evaluate_module.find_peaks = find_peaks
     evaluate_module.find_connections = find_connections
@@ -505,5 +628,5 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
         def _predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers):
             return predict_many(coco, images_directory, validation_ids, params, getattr(evaluate_module, "posenet", model),
                                 model_params, heat_layers, paf_layers, batch=int(batch),
-                                image_name=getattr(evaluate_module, "get_image_name", None))
+                                image_name=getattr(evaluate_module, "get_image_name", None), forward_batch=int(forward_batch))
         evaluate_module.predict_many = _predict_many

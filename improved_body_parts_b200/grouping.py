@@ -31,7 +31,7 @@ EXPORTS = (
     "spg_download_people", "spg_download_status", "spg_launch_count", "spg_stage_kernel", "spg_wire_record_bytes",
     "spg_set_wire_output", "spg_wire_create", "spg_wire_open", "spg_wire_close", "spg_wire_destroy", "spg_wire_signal",
     "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal",
-    "spg_postnet_rotated", "spg_prenet", "spg_group_ragged")
+    "spg_postnet_rotated", "spg_prenet", "spg_group_ragged", "spg_postnet_ragged")
 
 
 class GroupingError(RuntimeError):
@@ -65,6 +65,18 @@ class _PostnetDesc(C.Structure):
 
 class _PostnetRotation(C.Structure):
     _fields_ = [("apply", C.c_int32), ("reserved", C.c_int32), ("matrix", C.c_double * 6)]
+
+
+class _PostnetCommon(C.Structure):
+    _fields_ = [("stride", C.c_int32), ("paf_chan0", C.c_int32), ("heat_chan0", C.c_int32),
+                ("flip_paf_ord", C.POINTER(C.c_int32)), ("flip_heat_ord", C.POINTER(C.c_int32)), ("nan_scrub", C.c_int32),
+                ("net_dtype", C.c_int32)]
+
+
+class _PostnetImage(C.Structure):
+    _fields_ = [("net_out", C.c_void_p), ("pair_stride", C.c_int64), ("chan_stride", C.c_int64), ("h", C.c_int32),
+                ("w", C.c_int32), ("crop_h", C.c_int32), ("crop_w", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+                ("heat_out", C.c_void_p), ("paf_out", C.c_void_p)]
 
 
 class _PrenetItem(C.Structure):
@@ -117,6 +129,8 @@ def load_library() -> C.CDLL:
         lib.spg_wire_wait.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
         lib.spg_postnet_rotated.argtypes = [C.c_void_p, C.POINTER(_PostnetDesc), C.POINTER(_PostnetRotation), C.c_int32,
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+        lib.spg_postnet_ragged.argtypes = [C.c_void_p, C.POINTER(_PostnetCommon), C.POINTER(_PostnetImage), C.c_int32,
+                                           C.c_int32, C.c_void_p]
         lib.spg_prenet.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.POINTER(_PrenetItem), C.c_int32, C.c_void_p]
         lib.spg_group_ragged.argtypes = [C.c_void_p, C.POINTER(_ImageMaps), C.c_int32, C.c_int32, C.POINTER(_Params),
@@ -137,6 +151,23 @@ def params_struct(params) -> _Params:
         gp = GroupParams.from_dict(dict(params))
     return _Params(gp.thre1, gp.thre2, gp.connect_ration, gp.len_rate, gp.connection_tole, gp.min_mean_score,
                    gp.mid_num, gp.offset_radius, gp.remove_recon, gp.min_parts, gp.crit1_strict, gp.refresh_len_check)
+
+
+def clamp_scale(scale: float, image_hw) -> float:
+    """evaluate.py:94-96: an item whose resized image would exceed 2600 rows or 3800 columns is shrunk to fit."""
+    h, w = image_hw
+    if scale * h > 2600 or scale * w > 3800:
+        scale = min(2600 / h, 3800 / w)
+    return scale
+
+
+def input_geometry(h: int, w: int, scale: float, max_downsample: int) -> Tuple[int, int, int, int]:
+    """``(H1, W1, Hp, Wp)`` of one item (evaluate.py:98-100): the size of ``cv2.resize(image, (0, 0), fx=scale,
+    fy=scale)`` (``cvRound``: ties to even) = the crop, and that size padded up to multiples of ``max_downsample`` = the
+    network's input."""
+    H1, W1 = int(np.rint(h * scale)), int(np.rint(w * scale))
+    md = int(max_downsample)
+    return H1, W1, -(-H1 // md) * md, -(-W1 // md) * md
 
 
 def _vp(a: Optional[np.ndarray]):
@@ -492,7 +523,6 @@ class Grouper:
         ``paf_as_f64=True`` to the grouping calls: the reference's float64 values are exactly these), float64 otherwise.
         """
         import torch
-        from .skeleton import FLIP_HEAT_ORD, FLIP_PAF_ORD, NUM_LIMBS
         if len(net_outs) != len(crops) or not net_outs:
             raise GroupingError("one crop size per scale expected")
         H, W = (int(v) for v in out_hw)
@@ -504,10 +534,7 @@ class Grouper:
         if paf_dtype == torch.float32 and not single:
             raise GroupingError("float32 body-part planes hold the reference's float64 values only for a single scale")
         heat_chan0 = self.L if heat_chan0 is None else heat_chan0
-        fp = np.ascontiguousarray(np.asarray(FLIP_PAF_ORD if flip_paf_ord is None else flip_paf_ord, np.int32)[:self.L])
-        fh = np.ascontiguousarray(np.asarray(FLIP_HEAT_ORD if flip_heat_ord is None else flip_heat_ord, np.int32)[:self.K])
-        if flip_paf_ord is None and self.L != NUM_LIMBS:
-            raise GroupingError("flip_paf_ord is needed for a non-canonical skeleton")
+        fp, fh = self._flip_orders(flip_paf_ord, flip_heat_ord)
         scales = (_PostnetScale * len(net_outs))()
         for t, (o, (ch, cw)) in enumerate(zip(net_outs, crops)):
             if not o.is_cuda or o.device.index != self.device or o.dim() != 5 or o.shape[0] != N or o.shape[1] != 2:
@@ -544,6 +571,72 @@ class Grouper:
                                            C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
         self._check(rc, "spg_postnet_rotated")
         return heat_out, paf_out
+
+    def _flip_orders(self, flip_paf_ord, flip_heat_ord):
+        """The flip permutations of the body-part / keypoint channels (default: the canonical skeleton's)."""
+        from .skeleton import FLIP_HEAT_ORD, FLIP_PAF_ORD, NUM_LIMBS
+        if flip_paf_ord is None and self.L != NUM_LIMBS:
+            raise GroupingError("flip_paf_ord is needed for a non-canonical skeleton")
+        fp = np.ascontiguousarray(np.asarray(FLIP_PAF_ORD if flip_paf_ord is None else flip_paf_ord, np.int32)[:self.L])
+        fh = np.ascontiguousarray(np.asarray(FLIP_HEAT_ORD if flip_heat_ord is None else flip_heat_ord, np.int32)[:self.K])
+        return fp, fh
+
+    def postnet_ragged(self, images, *, stride: int = 4, paf_dtype=None, outs=None, paf_chan0: int = 0,
+                       heat_chan0: Optional[int] = None, flip_paf_ord=None, flip_heat_ord=None, nan_scrub: bool = False,
+                       stream=None):
+        """``postnet`` for a batch of images of different sizes with one item each (one scale, no rotation) in one
+        asynchronous call (``spg_postnet_ragged``).
+
+        ``images``: per image ``(net_out, (crop_h, crop_w), (H, W))`` -- ``net_out`` the ``[2, C, h, w]`` CUDA tensor of
+        its pair (float32 / float16, one dtype per call; slices of a shared ``[2k, C, h, w]`` batch output work without
+        copies).  ``outs``: optional per-image ``(heat, paf)`` contiguous tensors to write into.  Returns per image
+        ``(heat [1,K,H,W] float32, paf [1,L,H,W])``, equal to what ``postnet`` returns for that image alone; ``paf`` is
+        float32 by default (float32 storage of the float64 values, ``paf_as_f64=True`` for the grouping calls)."""
+        import torch
+        images = list(images)
+        if outs is not None and len(outs) != len(images):
+            raise GroupingError("one (heat, paf) output pair per image expected")
+        if len(images) > self.max_batch:
+            raise GroupingError(f"{len(images)} images, the handle was created for {self.max_batch}")
+        paf_dtype = torch.float32 if paf_dtype is None else paf_dtype
+        if paf_dtype not in (torch.float32, torch.float64):
+            raise GroupingError("paf_dtype must be float32 or float64")
+        heat_chan0 = self.L if heat_chan0 is None else heat_chan0
+        fp, fh = self._flip_orders(flip_paf_ord, flip_heat_ord)
+        dev = torch.device("cuda", self.device)
+        arr = (_PostnetImage * max(len(images), 1))()
+        net_dtype, results = None, []
+        for i, (o, (ch, cw), (H, W)) in enumerate(images):
+            H, W = int(H), int(W)
+            if not o.is_cuda or o.device.index != self.device or o.dim() != 4 or o.shape[0] != 2:
+                raise GroupingError(f"image {i}: network output must be a [2,C,h,w] CUDA tensor on the handle's device")
+            if o.stride(3) != 1 or o.stride(2) != o.shape[3]:
+                raise GroupingError(f"image {i}: network output rows must be contiguous")
+            if o.dtype not in (torch.float32, torch.float16):
+                raise GroupingError(f"image {i}: network output must be float32 or float16")
+            if net_dtype is not None and o.dtype != net_dtype:
+                raise GroupingError(f"image {i}: every network output of a call needs the same dtype")
+            net_dtype = o.dtype
+            if o.shape[1] < max(heat_chan0 + self.K, paf_chan0 + self.L):
+                raise GroupingError(f"image {i}: network output has too few channels")
+            if outs is not None:
+                heat, paf = outs[i]
+            else:
+                heat = torch.empty((1, self.K, H, W), dtype=torch.float32, device=dev)
+                paf = torch.empty((1, self.L, H, W), dtype=paf_dtype, device=dev)
+            if not (heat.is_contiguous() and paf.is_contiguous()) or heat.dtype != torch.float32 or paf.dtype != paf_dtype \
+                    or heat.numel() != self.K * H * W or paf.numel() != self.L * H * W:
+                raise GroupingError(f"image {i}: heat / paf outputs must be contiguous float32 [K,H,W] / {paf_dtype} [L,H,W]")
+            arr[i] = _PostnetImage(o.data_ptr(), o.stride(0), o.stride(1), o.shape[2], o.shape[3], int(ch), int(cw), H, W,
+                                   heat.data_ptr(), paf.data_ptr())
+            results.append((heat, paf))
+        common = _PostnetCommon(int(stride), int(paf_chan0), int(heat_chan0), fp.ctypes.data_as(C.POINTER(C.c_int32)),
+                                fh.ctypes.data_as(C.POINTER(C.c_int32)), int(bool(nan_scrub)),
+                                F16 if net_dtype == torch.float16 else F32)
+        rc = self._lib.spg_postnet_ragged(self._h, C.byref(common), arr, C.c_int32(len(images)),
+                                          C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
+        self._check(rc, "spg_postnet_ragged")
+        return results
 
     # -- pre-network stage ----------------------------------------------------------------------------
     @property
@@ -583,12 +676,9 @@ class Grouper:
         dev = torch.device("cuda", self.device)
         results = []
         for t, (scale, angle) in enumerate(pairs):
-            scale = float(scale)
-            if scale * h > 2600 or scale * w > 3800:  # evaluate.py:94-96
-                scale = min(2600 / h, 3800 / w)
+            scale = clamp_scale(float(scale), (h, w))
             # the library checks the scale and the geometry; this only sizes the output
-            H1, W1 = (int(np.rint(h * scale)), int(np.rint(w * scale))) if np.isfinite(scale) and scale > 0 else (0, 0)
-            Hp, Wp = -(-H1 // md) * md, -(-W1 // md) * md
+            H1, W1, Hp, Wp = input_geometry(h, w, scale, md) if np.isfinite(scale) and scale > 0 else (0, 0, 0, 0)
             forward = reverse = None
             if angle != 0:  # evaluate.py:108-110, the centre's x and y swapped as there
                 import cv2

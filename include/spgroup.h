@@ -190,6 +190,32 @@ typedef struct spg_postnet_rotation {
 int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *desc, const spg_postnet_rotation *rot,
                         int32_t n_images, int32_t height, int32_t width, float *heat_out, void *paf_out,
                         int32_t paf_dtype, void *stream);
+/* Ragged batches: predict()'s post-network stage for images of different sizes in one call, one item per image (a single
+ * scale, no rotation: the reference's default, utils/config).  What the images share: */
+typedef struct spg_postnet_common {
+    int32_t stride;                 /* model_params['stride']: must be 4 */
+    int32_t paf_chan0, heat_chan0;  /* as spg_postnet_desc */
+    const int32_t *flip_paf_ord;    /* [n_limbs] */
+    const int32_t *flip_heat_ord;   /* [n_parts] */
+    int32_t nan_scrub;              /* as spg_postnet_desc */
+    int32_t net_dtype;              /* SPG_F32 | SPG_F16: the dtype of every image's network output */
+} spg_postnet_common;
+/* One image: the network's output for its pair and where its maps go. */
+typedef struct spg_postnet_image {
+    const void *net_out;            /* [2][C][h][w] (image, mirrored image), rows contiguous (row stride w) */
+    int64_t pair_stride, chan_stride; /* elements */
+    int32_t h, w;                   /* network output size = padded input size / 4 */
+    int32_t crop_h, crop_w;         /* imageToTest size (evaluate.py:148) */
+    int32_t height, width;          /* image size = map size */
+    float *heat_out;                /* [n_parts][height][width] float32, 16-byte aligned */
+    void *paf_out;                  /* [n_limbs][height][width] of the call's paf_dtype, 16-byte aligned */
+} spg_postnet_image;
+/* Image i's maps equal those spg_postnet gives for it alone (n_scales = 1).  paf_dtype: SPG_F32 (float32 storage of the
+ * float64 values, as for a single scale: pass SPG_F32_AS_F64 to the grouping calls) or SPG_F64.  Every image is validated
+ * before the first launch; SPG_E_INVALID names the first bad one.  Asynchronous on `stream` (never synchronises);
+ * `images` may be reused as soon as the call returns. */
+int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *common, const spg_postnet_image *images,
+                       int32_t n_images, int32_t paf_dtype, void *stream);
 
 /* ---- pre-network stage: the item loop of predict() before the forward pass, evaluate.py:94-121 ------------ */
 /* One (scale, angle) item of product(multiplier, rotate_angle) (evaluate.py:90). */

@@ -2,6 +2,7 @@
 """Run the reference's ``evaluate.py`` UNCHANGED with its grouping stage on the H100 path.
 
     python tools/run_evaluate_b200.py --reference /path/to/Improved-Body-Parts [--config utils/config] [--check] [--batch N]
+                                      [--forward-batch M]
 
 What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is never modified:
 
@@ -13,7 +14,8 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
 3. ``dropin.install(evaluate)``: rebinds ``evaluate.find_peaks / find_connections / find_people`` (looked up by name
    at the call sites ``:509-511``) and takes ``limbSeq`` from the module (``:54``); with ``--batch N`` (N > 1) it also
    replaces ``predict`` by the device one and ``predict_many`` (``:550-560``) by ``dropin.predict_many``, which groups
-   N images per call;
+   N images per call; ``--forward-batch M`` (M > 1, with N > 1) also runs the network on up to M images of the same
+   input size at once (``dropin.predict_batch``);
 4. fills the globals ``evaluate.__main__`` would set (``:643-646``): ``params, model_params`` from the reference's own
    ``utils/config`` through ``skeleton.read_reference_ini`` (``utils/config_reader.py:7`` hard-codes the author's path),
    ``show_eval_speed``;
@@ -60,7 +62,7 @@ def _stub_missing() -> list:
 
 
 def prepare(reference_root: str, config_path: str = None, device: int = None, install: bool = True,
-            replace_format_results: bool = False, batch: int = 1):
+            replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1):
     """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites."""
     reference_root = os.path.abspath(reference_root)
     if not os.path.isfile(os.path.join(reference_root, "evaluate.py")):
@@ -88,7 +90,8 @@ def prepare(reference_root: str, config_path: str = None, device: int = None, in
         if device is not None:
             dropin.configure(device=device)
         if batch > 1:  # the batched grouping takes the maps the device predict() leaves on the GPU
-            dropin.install(evaluate, device_predict=True, batch=batch)
+            extra = dict(forward_batch=forward_batch) if forward_batch > 1 else {}
+            dropin.install(evaluate, device_predict=True, batch=batch, **extra)
         else:
             dropin.install(evaluate)
     evaluate.params, evaluate.model_params = skeleton.read_reference_ini(
@@ -109,10 +112,16 @@ def main() -> None:
     ap.add_argument("--check", action="store_true", help="group one synthetic image through evaluate's call sites on the GPU")
     ap.add_argument("--batch", type=int, default=1,
                     help="images per grouping call in predict_many (> 1 implies the device predict; default 1)")
+    ap.add_argument("--forward-batch", type=int, default=1,
+                    help="images per network forward pass in predict_many (> 1 needs --batch > 1; default 1)")
     a = ap.parse_args()
     if a.batch < 1:
         ap.error("--batch must be >= 1")
-    ev = prepare(a.reference, a.config, a.device, batch=a.batch)
+    if a.forward_batch < 1:
+        ap.error("--forward-batch must be >= 1")
+    if a.forward_batch > 1 and a.batch < 2:
+        ap.error("--forward-batch > 1 needs --batch > 1")
+    ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch)
     print(f"evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
           f"find_peaks -> {ev.find_peaks.__module__}.{ev.find_peaks.__name__}")
     if a.check:
