@@ -22,17 +22,30 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .grouping import Grouper, GroupingError, GroupResult, clamp_scale, input_geometry
+from . import wire
+from .grouping import Grouper, GroupingError, clamp_scale, input_geometry
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
 _device = 0
 _variant = "evaluate"
 _input_stage = "host"
-_groupers: Dict[int, Grouper] = {}
+_groupers: Dict[int, Grouper] = {}  # the max_batch=1 handle of the per-image calls, per device
 _ragged: Dict[int, Grouper] = {}  # the handle of the batched calls (group_many / predict_many), per device
 CAP_PEAKS, CAP_CANDS, CAP_ROWS = 128, 4096, 128
 MAX_DIM = 32767  # the C ABI's limit; the workspace does not depend on the map size, so ONE handle serves every image size
+
+
+def _stage(input_stage: str) -> str:
+    if input_stage not in ("host", "device"):
+        raise ValueError("input_stage must be 'host' or 'device'")
+    return input_stage
+
+
+def _forward_batch(n) -> int:
+    if int(n) < 1:
+        raise ValueError("forward_batch must be >= 1")
+    return int(n)
 
 
 def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optional[int] = None,
@@ -43,9 +56,7 @@ def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optiona
     ``"host"`` (cv2, the default) or ``"device"`` (``spg_prenet``)."""
     global _limbs, _device, _variant, _input_stage
     if input_stage is not None:
-        if input_stage not in ("host", "device"):
-            raise ValueError("input_stage must be 'host' or 'device'")
-        _input_stage = input_stage
+        _input_stage = _stage(input_stage)
     if limbs is not None:
         _limbs = tuple((int(a), int(b)) for a, b in limbs)
     if device is not None:
@@ -60,27 +71,28 @@ def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optiona
     _ragged.clear()
 
 
-def _grouper(H: int = 0, W: int = 0) -> Grouper:
+def _new_grouper(max_batch: int) -> Grouper:
+    return Grouper(_limbs, NUM_PARTS, COCO_FROM_PART, max_batch=max_batch, max_h=MAX_DIM, max_w=MAX_DIM,
+                   max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS, device=_device)
+
+
+def _grouper() -> Grouper:
     """The one native handle of the current device (evaluate.py runs over images of hundreds of different sizes: a
     handle per size, as in round 1, grew device memory and streams without bound)."""
     g = _groupers.get(_device)
     if g is None:
-        g = Grouper(_limbs, NUM_PARTS, COCO_FROM_PART, max_batch=1, max_h=MAX_DIM, max_w=MAX_DIM,
-                    max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS, device=_device)
-        _groupers[_device] = g
+        g = _groupers[_device] = _new_grouper(1)
     return g
 
 
 def _grouper_many(n: int) -> Grouper:
-    """The handle of the batched calls on the current device; its max_batch grows on demand (the max_batch=1 handle of
-    the three call-site functions stays as it is)."""
+    """The handle of the batched calls on the current device; its max_batch grows on demand.  The max_batch=1 handle of
+    the per-image calls stays separate: spg_postnet_rotated sizes its float64 accumulator by the handle's max_batch."""
     g = _ragged.get(_device)
     if g is None or g.max_batch < n:
         if g is not None:
             g.close()
-        g = Grouper(_limbs, NUM_PARTS, COCO_FROM_PART, max_batch=max(int(n), 1), max_h=MAX_DIM, max_w=MAX_DIM,
-                    max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS, device=_device)
-        _ragged[_device] = g
+        g = _ragged[_device] = _new_grouper(max(int(n), 1))
     return g
 
 
@@ -91,10 +103,6 @@ def _params(params):
     return GroupParams.demo(params) if _variant == "demo" else params
 
 
-def _check(r: GroupResult, n: int = 0) -> None:
-    _check_status(int(r.status[n]))
-
-
 def _check_status(status: int) -> None:
     if status:
         raise GroupingError(f"grouping capacity exceeded or invalid sample index (status {status:#x}); "
@@ -102,7 +110,7 @@ def _check_status(status: int) -> None:
 
 
 def _maps_to_device(hwc: np.ndarray, channels: int, dtype):
-    """``[H, W, C]`` host maps (what predict() returns) -> ``[1, channels, H, W]`` device planes of ``dtype``.
+    """``[H, W, C]`` host maps (what predict() returns) -> ``[1, channels, H, W]`` device planes of torch ``dtype``.
 
     The array goes up as it is and is transposed / cast on the device: a numpy transpose of a 512x512x30 float64 array
     on the host costs more than the whole device path.  The float64 -> float32 cast rounds to nearest even on both sides."""
@@ -111,8 +119,24 @@ def _maps_to_device(hwc: np.ndarray, channels: int, dtype):
     if arr.dtype not in (np.float32, np.float64):
         arr = arr.astype(np.float64)
     t = torch.from_numpy(np.ascontiguousarray(arr)).to(f"cuda:{_device}")
-    want = torch.float32 if dtype == np.float32 else torch.float64
-    return t[:, :, :channels].permute(2, 0, 1).to(want).contiguous()[None]
+    return t[:, :, :channels].permute(2, 0, 1).to(dtype).contiguous()[None]
+
+
+def _heat_tensor(heat):
+    """``DeviceMaps`` or host ``[H, W, >=18]`` keypoint maps -> ``[1, 18, H, W]`` float32 device planes (the cast of
+    evaluate.py:173)."""
+    import torch
+    return heat.tensor if isinstance(heat, DeviceMaps) else _maps_to_device(heat, NUM_PARTS, torch.float32)
+
+
+def _paf_tensor(paf):
+    """``DeviceMaps`` or host ``[H, W, L]`` body-part maps -> ``(device planes, as_f64)``: host float64 maps stay
+    float64, any other host maps become float32; ``as_f64`` says the planes are float32 storage of float64 values."""
+    import torch
+    if isinstance(paf, DeviceMaps):
+        return paf.tensor, paf.as_f64
+    dtype = torch.float64 if np.asarray(paf).dtype == np.float64 else torch.float32
+    return _maps_to_device(paf, len(_limbs), dtype), False
 
 
 class DeviceMaps:
@@ -139,26 +163,39 @@ def pad_right_down_corner(img: np.ndarray, stride: int, pad_value: int) -> Tuple
     return np.pad(img, ((0, pad[2]), (0, pad[3]), (0, 0)), constant_values=pad_value), pad
 
 
-#: pinned staging of the uint8 image for ``predict(input_stage="device")`` and the event of its last upload
-_staging: Dict[str, object] = {}
+#: pinned host staging per slot ("image", "pairs") as ``(buffer, event of the last copy out of it)``
+_staging: Dict[str, tuple] = {}
+
+
+def _pinned(slot: str, n: int, dtype):
+    """A pinned buffer of ``n`` elements of ``dtype`` for ``slot`` (grown on demand), once the slot's last copy has left
+    it.  Record the next copy out of it with ``_copied(slot)``."""
+    import torch
+    buf, ev = _staging.get(slot, (None, None))
+    if ev is not None:
+        ev.synchronize()
+    if buf is None or buf.numel() < n:
+        buf = torch.empty(n, dtype=dtype, pin_memory=True)
+    _staging[slot] = (buf, ev)
+    return buf[:n]
+
+
+def _copied(slot: str) -> None:
+    """Mark the copy just enqueued on the current stream out of ``slot``'s buffer."""
+    import torch
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(_device))
+    _staging[slot] = (_staging[slot][0], ev)
 
 
 def _upload_image(image: np.ndarray):
-    """Host uint8 ``[H, W, 3]`` image -> CUDA tensor, through a pinned buffer that grows on demand (one copy, async)."""
+    """Host uint8 ``[H, W, 3]`` image -> CUDA tensor, through a pinned buffer (one copy, async)."""
     import torch
     arr = np.ascontiguousarray(image, np.uint8)
-    buf, ev = _staging.get("buf"), _staging.get("event")
-    if ev is not None:
-        ev.synchronize()  # the previous upload has left the buffer
-    if buf is None or buf.numel() < arr.size:
-        buf = torch.empty(arr.size, dtype=torch.uint8, pin_memory=True)
-        _staging["buf"] = buf
-    host = buf[:arr.size].view(arr.shape)
+    host = _pinned("image", arr.size, torch.uint8).view(arr.shape)
     host.numpy()[...] = arr
     dev = host.to(f"cuda:{_device}", non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record(torch.cuda.current_stream(_device))
-    _staging["event"] = ev
+    _copied("image")
     return dev
 
 
@@ -175,40 +212,36 @@ def predict(image, params, model, model_params, heat_layers=None, paf_layers=Non
     inverse rotation of the maps, the crop and the float64 average over the items (:126-161) happen in
     ``spg_postnet_rotated`` -- the maps never visit the host.  Returns two ``DeviceMaps`` (heatmap, paf) that
     ``find_peaks`` / ``find_connections`` / ``group`` accept."""
-    import itertools
-
     import torch
-    stage = _input_stage if input_stage is None else input_stage
-    if stage not in ("host", "device"):
-        raise ValueError("input_stage must be 'host' or 'device'")
+    stage = _stage(_input_stage if input_stage is None else input_stage)
     g = _grouper()
     multiplier = [x * model_params["boxsize"] / image.shape[0] for x in params["scale_search"]]
     if stage == "device":
         img = image if isinstance(image, torch.Tensor) else _upload_image(image)
         items = g.prenet(img.to(f"cuda:{_device}"), multiplier, params["rotation_search"],
                          max_downsample=int(model_params["max_downsample"]), pad_value=int(model_params["padValue"]))
-        outs = []
-        for pair, _, _ in items:
-            with torch.no_grad():
-                out = model(pair)[-1][0]  # last stack, finest scale (:126)
-            if out.dtype not in (torch.float32, torch.float16):
-                out = out.float()
-            outs.append(out[None].contiguous())
-        heat, paf = g.postnet(outs, [c for _, c, _ in items], tuple(int(v) for v in image.shape[:2]),
-                              stride=int(model_params["stride"]), nan_scrub=_variant == "demo",
-                              rotations=[r for _, _, r in items])
-        return DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)
+    else:
+        items = _host_items(image, multiplier, params["rotation_search"], model_params)
     outs, crops, rotations = [], [], []
-    for scale, angle in itertools.product(multiplier, params["rotation_search"]):
-        pair, crop, reverse = _host_pair(image, clamp_scale(scale, image.shape[:2]), angle, model_params)
+    for pair, crop, reverse in items:
         with torch.no_grad():
-            out = _network_output(model, torch.from_numpy(pair).to(f"cuda:{_device}"))
-        outs.append(out[None].contiguous())
+            outs.append(_network_output(model, pair)[None].contiguous())
         crops.append(crop)
         rotations.append(reverse)
     heat, paf = g.postnet(outs, crops, image.shape[:2], stride=int(model_params["stride"]), nan_scrub=_variant == "demo",
                           rotations=rotations)
     return DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)
+
+
+def _host_items(image: np.ndarray, multiplier, angles, model_params):
+    """The items of ``product(multiplier, angles)`` built with cv2 on the host, each pair moved to the device as it is
+    yielded: a generator, so that the next item's cv2 work overlaps the network's kernels for this one."""
+    import itertools
+
+    import torch
+    for scale, angle in itertools.product(multiplier, angles):
+        pair, crop, reverse = _host_pair(image, clamp_scale(scale, image.shape[:2]), angle, model_params)
+        yield torch.from_numpy(pair).to(f"cuda:{_device}"), crop, reverse
 
 
 def _host_pair(image: np.ndarray, scale: float, angle: float, model_params, out: Optional[np.ndarray] = None):
@@ -263,19 +296,6 @@ def plan_buckets(image_shapes, params, model_params):
     return plan, buckets
 
 
-def _pinned_pairs(n_floats: int):
-    """A pinned float32 staging buffer of at least ``n_floats`` for ``predict_batch``'s host input stage, once the copy
-    out of its previous contents has left it."""
-    import torch
-    buf, ev = _staging.get("pairs"), _staging.get("pairs_event")
-    if ev is not None:
-        ev.synchronize()
-    if buf is None or buf.numel() < n_floats:
-        buf = torch.empty(n_floats, dtype=torch.float32, pin_memory=True)
-        _staging["pairs"] = buf
-    return buf
-
-
 def predict_batch(images, params, model, model_params, *, forward_batch: int, input_stage: Optional[str] = None):
     """``predict`` for several images at once: one ``(heatmap, paf)`` pair of ``DeviceMaps`` per image, in input order.
 
@@ -288,15 +308,11 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     network under cuDNN may pick another algorithm for another batch size).  Other configurations (several scales, a
     rotation search, another stride) run ``predict`` per image."""
     import torch
-    stage = _input_stage if input_stage is None else input_stage
-    if stage not in ("host", "device"):
-        raise ValueError("input_stage must be 'host' or 'device'")
-    if int(forward_batch) < 1:
-        raise ValueError("forward_batch must be >= 1")
+    stage = _stage(_input_stage if input_stage is None else input_stage)
+    fb = _forward_batch(forward_batch)
     images = list(images)
     if not _single_item(params, model_params):
         return [predict(img, params, model, model_params, input_stage=stage) for img in images]
-    fb = int(forward_batch)
     md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
     plan, buckets = plan_buckets([img.shape[:2] for img in images], params, model_params)
     g = _grouper_many(len(images))
@@ -307,13 +323,11 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
         x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
         crops = []
         if stage == "host":
-            host = _pinned_pairs(x.numel())[:x.numel()].view(x.shape)
+            host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
             for j, i in enumerate(idx):
                 crops.append(_host_pair(images[i], plan[i][1], 0, model_params, out=host[2 * j:2 * j + 2].numpy())[1])
             x.copy_(host, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(torch.cuda.current_stream(_device))
-            _staging["pairs_event"] = ev
+            _copied("pairs")
         else:
             for j, i in enumerate(idx):
                 img = images[i] if isinstance(images[i], torch.Tensor) else _upload_image(images[i])
@@ -343,12 +357,10 @@ def _upload_peaks(g: Grouper, all_peaks) -> None:
 # ---- the three reference functions ---------------------------------------------------------------------
 def find_peaks(heatmap_avg, params):
     """evaluate.py:169-203.  ``heatmap_avg [H,W,>=18]`` -> list[18] of [(x, y, score, id), ...]."""
-    H, W = heatmap_avg.shape[:2]
-    g = _grouper(H, W)
-    heat = heatmap_avg.tensor if isinstance(heatmap_avg, DeviceMaps) else _maps_to_device(heatmap_avg, NUM_PARTS, np.float32)
-    g.nms_peaks(heat, _params(params))  # the cast is evaluate.py:173
+    g = _grouper()
+    g.nms_peaks(_heat_tensor(heatmap_avg), _params(params))
     r = g.fetch(1)
-    _check(r)
+    _check_status(r.status[0])
     all_peaks = r.as_reference_structures(0)[0]
     _state.clear()
     _state.update(peaks=all_peaks, handle=g)
@@ -357,17 +369,13 @@ def find_peaks(heatmap_avg, params):
 
 def find_connections(all_peaks, paf_avg, image_width, params):
     """evaluate.py:206-276.  ``paf_avg [H,W,L]`` float32 or float64 -> (connection_all, special_k)."""
-    H, W = paf_avg.shape[:2]
-    g = _grouper(H, W)
+    g = _grouper()
     _upload_peaks(g, all_peaks)
-    if isinstance(paf_avg, DeviceMaps):
-        g.limb_score(paf_avg.tensor, image_width, _params(params), paf_as_f64=paf_avg.as_f64)
-    else:
-        dtype = np.float64 if np.asarray(paf_avg).dtype == np.float64 else np.float32
-        g.limb_score(_maps_to_device(paf_avg, len(_limbs), dtype), image_width, _params(params))
+    paf, as_f64 = _paf_tensor(paf_avg)
+    g.limb_score(paf, image_width, _params(params), paf_as_f64=as_f64)
     g.limb_match(1, _params(params))
     r = g.fetch(1)
-    _check(r)
+    _check_status(r.status[0])
     # ids in the rows are those of the caller's all_peaks (:267), not positions in our tables
     _, conns, special, _, _ = r.as_reference_structures(0)
     for k, rows in enumerate(conns):
@@ -387,7 +395,7 @@ def find_people(connection_all, special_k, all_peaks, params):
             and _state.get("handle") is g:  # evaluate.py:509-511 handing our own objects back: everything is still on the device
         g.assemble(1, _params(params))
         r = g.fetch(1)
-        _check(r)
+        _check_status(r.status[0])
         return r.subset[0, :int(r.n_persons[0])].copy(), np.array([item for sublist in all_peaks for item in sublist])
     _upload_peaks(g, all_peaks)
     special = set(int(k) for k in special_k)
@@ -405,7 +413,7 @@ def find_people(connection_all, special_k, all_peaks, params):
                          np.concatenate(sc) if sc else np.zeros(0), np.concatenate(nm) if nm else np.zeros(0))
     g.assemble(1, _params(params))
     r = g.fetch(1)
-    _check(r)
+    _check_status(r.status[0])
     subset = r.subset[0, :int(r.n_persons[0])].copy()
     candidate = np.array([item for sublist in all_peaks for item in sublist])  # evaluate.py:283, verbatim semantics
     # subset holds positions in the flattened table; the reference stores the peaks' own ids there (equal unless
@@ -422,17 +430,13 @@ def group(heatmap_avg, paf_avg, image_extent, params):
     """Fused peaks -> connections -> people: one upload, four kernels, one download.
 
     Returns ``(all_peaks, connection_all, special_k, subset, candidate)`` exactly as the three calls would."""
-    H, W = heatmap_avg.shape[:2]
-    g = _grouper(H, W)
+    g = _grouper()
     _state.clear()
-    if isinstance(heatmap_avg, DeviceMaps):
-        g.group_device(heatmap_avg.tensor, paf_avg.tensor, image_extent, _params(params), paf_as_f64=paf_avg.as_f64)
-    else:
-        dtype = np.float64 if np.asarray(paf_avg).dtype == np.float64 else np.float32
-        g.group_device(_maps_to_device(heatmap_avg, NUM_PARTS, np.float32), _maps_to_device(paf_avg, len(_limbs), dtype),
-                       image_extent, _params(params))
+    heat = _heat_tensor(heatmap_avg)
+    paf, as_f64 = _paf_tensor(paf_avg)
+    g.group_device(heat, paf, image_extent, _params(params), paf_as_f64=as_f64)
     r = g.fetch(1)
-    _check(r)
+    _check_status(r.status[0])
     return r.as_reference_structures(0)
 
 
@@ -441,20 +445,41 @@ def _ragged_maps(maps):
     storage of float64 values (one answer for the whole call)."""
     pairs, as_f64 = [], set()
     for heat, paf in maps:
-        if isinstance(heat, DeviceMaps):
-            h = heat.tensor
-        else:
-            h = _maps_to_device(heat, NUM_PARTS, np.float32)
-        if isinstance(paf, DeviceMaps):
-            p = paf.tensor
-            as_f64.add(paf.as_f64)
-        else:
-            p = _maps_to_device(paf, len(_limbs), np.float64 if np.asarray(paf).dtype == np.float64 else np.float32)
-            as_f64.add(False)
+        h = _heat_tensor(heat)
+        p, f64 = _paf_tensor(paf)
         pairs.append((h, p))
+        as_f64.add(f64)
     if len(as_f64) > 1:
         raise GroupingError("the body-part maps of one call must all be float32, float32-held float64 or float64")
     return pairs, as_f64 == {True}
+
+
+#: device buffers of the wire records ``predict_many`` downloads, per device
+_records: Dict[int, object] = {}
+
+
+def _group_ragged(maps, image_extents, params, records: bool = False):
+    """The maps of a batch of images to the device and one ragged grouping call (``spg_group_ragged``) on the batched
+    handle: ``(handle, n_images, wire)``.  With ``records`` the call also writes image i's wire record to row i of
+    ``wire``, a per-device buffer; without, ``wire`` is None."""
+    import torch
+    pairs, as_f64 = _ragged_maps(maps)
+    g = _grouper_many(len(pairs))
+    _state.clear()
+    buf = None
+    if records:
+        rec_bytes = g.wire_record_bytes()
+        buf = _records.get(_device)
+        if buf is None or buf.shape[0] < len(pairs) or buf.shape[1] != rec_bytes:
+            buf = torch.empty((max(len(pairs), g.max_batch), rec_bytes), dtype=torch.uint8, device=f"cuda:{_device}")
+            _records[_device] = buf
+        g.set_wire_output(buf.data_ptr())
+    try:
+        g.group_ragged(pairs, image_extents, _params(params), paf_as_f64=as_f64)
+    finally:
+        if records:
+            g.set_wire_output(None)
+    return g, len(pairs), buf
 
 
 def group_many(maps, image_extents, params):
@@ -463,45 +488,22 @@ def group_many(maps, image_extents, params):
     ``maps``: per image a ``(heatmap_avg, paf_avg)`` pair -- the ``DeviceMaps`` ``predict`` returns or host ``[H, W, C]``
     arrays; ``image_extents``: per image ``oriImg.shape[0]``.  Returns one ``(all_peaks, connection_all, special_k,
     subset, candidate)`` per image, equal to what ``group()`` returns for it."""
-    pairs, as_f64 = _ragged_maps(maps)
-    g = _grouper_many(len(pairs))
-    _state.clear()
-    g.group_ragged(pairs, image_extents, _params(params), paf_as_f64=as_f64)
-    r = g.fetch(len(pairs))
+    g, n, _ = _group_ragged(maps, image_extents, params)
+    r = g.fetch(n)
     out = []
-    for i in range(len(pairs)):
-        _check(r, i)
+    for i in range(n):
+        _check_status(r.status[i])
         out.append(r.as_reference_structures(i))
     return out
-
-
-#: device buffers of the wire records ``predict_many`` downloads, per device
-_records: Dict[int, object] = {}
 
 
 def _people_of_batch(maps, extents, params) -> list:
     """One ragged grouping call for a batch of images, their wire records in one device-to-host copy, and per image
     ``process()``'s return value (evaluate.py:523-543)."""
-    import torch
-
-    from . import wire
-    pairs, as_f64 = _ragged_maps(maps)
-    g = _grouper_many(len(pairs))
-    rec_bytes = g.wire_record_bytes()
-    buf = _records.get(_device)
-    if buf is None or buf.shape[0] < len(pairs) or buf.shape[1] != rec_bytes:
-        buf = torch.empty((max(len(pairs), g.max_batch), rec_bytes), dtype=torch.uint8, device=f"cuda:{_device}")
-        _records[_device] = buf
-    _state.clear()
-    g.set_wire_output(buf.data_ptr())
-    try:
-        g.group_ragged(pairs, extents, _params(params), paf_as_f64=as_f64)
-    finally:
-        g.set_wire_output(None)
-    recs = wire.as_records(buf[:len(pairs)].cpu().numpy(), g.J, g.capR)
+    g, n, buf = _group_ragged(maps, extents, params, records=True)
     out = []
-    for rec in recs:
-        _check_status(int(rec["status"]))
+    for rec in wire.as_records(buf[:n].cpu().numpy(), g.J, g.capR):
+        _check_status(rec["status"])
         out.append(wire.people_of(rec))
     return out
 
@@ -524,16 +526,15 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
     assert (not set(validation_ids).difference(set(coco.getImgIds())))
     if int(batch) < 1:
         raise ValueError("batch must be >= 1")
-    if int(forward_batch) < 1:
-        raise ValueError("forward_batch must be >= 1")
+    fb = _forward_batch(forward_batch)
     keypoints = {}
     pending = []  # (image_id, (heatmap, paf) -- or the image itself for predict_batch, oriImg.shape[0])
 
     def flush():
         if pending:
             maps = [m for _, m, _ in pending]
-            if int(forward_batch) > 1:
-                maps = predict_batch(maps, dict(params), model, dict(model_params), forward_batch=int(forward_batch))
+            if fb > 1:
+                maps = predict_batch(maps, dict(params), model, dict(model_params), forward_batch=fb)
             people = _people_of_batch(maps, [e for _, _, e in pending], params)
             for (iid, _, _), kp in zip(pending, people):
                 keypoints[iid] = kp
@@ -543,7 +544,7 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
         name = image_name(coco, image_id) if image_name is not None else coco.imgs[image_id]["file_name"]
         path = os.path.join(images_directory, name)
         ori = cv2.imread(path)  # B,G,R order (evaluate.py:502)
-        if int(forward_batch) > 1:
+        if fb > 1:
             pending.append((image_id, ori, ori.shape[0]))
         else:
             pending.append((image_id, predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path),
@@ -575,14 +576,14 @@ def keypoint_heatmap_nms(heat, kernel: int = 3, thre: float = 0.1):
         raise GroupingError("only the 3x3 NMS the reference uses is implemented")
     if heat.dim() != 4 or heat.shape[0] != 1:
         raise GroupingError("expected a [1,C,H,W] tensor")
-    C, H, W = heat.shape[1:]
+    C = heat.shape[1]
     g = Grouper(((0, 0),), C, (0,), max_batch=1, max_h=MAX_DIM, max_w=MAX_DIM, max_peaks_per_part=CAP_PEAKS,
-                device=_device) if C != NUM_PARTS else _grouper(H, W)
+                device=_device) if C != NUM_PARTS else _grouper()
     src = heat.to(f"cuda:{_device}", torch.float32).contiguous()
     _state.clear()
     g.nms_peaks(src, dict(thre1=float(thre), offset_radius=0))
     r = g.fetch(1)
-    _check(r)
+    _check_status(r.status[0])
     out = torch.zeros_like(src)
     for c in range(C):
         n = int(min(r.peak_count[0, c], r.peak_anchor.shape[2]))
@@ -611,9 +612,8 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     (``predict_batch``)."""
     if int(batch) > 1 and not device_predict:
         raise ValueError("batch > 1 needs device_predict=True: the batched grouping takes the maps predict() leaves on the device")
-    if int(forward_batch) < 1:
-        raise ValueError("forward_batch must be >= 1")
-    if int(forward_batch) > 1 and (not device_predict or int(batch) < 2):
+    fb = _forward_batch(forward_batch)
+    if fb > 1 and (not device_predict or int(batch) < 2):
         raise ValueError("forward_batch > 1 needs device_predict=True and batch > 1: it batches predict_many's forward passes")
     configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host")
     evaluate_module.find_peaks = find_peaks
@@ -628,5 +628,5 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
         def _predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers):
             return predict_many(coco, images_directory, validation_ids, params, getattr(evaluate_module, "posenet", model),
                                 model_params, heat_layers, paf_layers, batch=int(batch),
-                                image_name=getattr(evaluate_module, "get_image_name", None), forward_batch=int(forward_batch))
+                                image_name=getattr(evaluate_module, "get_image_name", None), forward_batch=fb)
         evaluate_module.predict_many = _predict_many

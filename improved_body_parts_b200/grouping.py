@@ -14,6 +14,7 @@ from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
+from . import wire
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -22,16 +23,6 @@ ABI_VERSION = 2
 
 ST_PEAK_OVERFLOW, ST_CAND_OVERFLOW, ST_ROW_OVERFLOW, ST_SAMPLE_INDEX, ST_ASSERT, ST_WIRE_OVERFLOW = 1, 2, 4, 8, 16, 32
 F32, F64, F32_AS_F64, F16 = 0, 1, 2, 3
-
-#: every symbol include/spgroup.h declares (checked by tests/test_abi.py against the built library)
-EXPORTS = (
-    "spg_create", "spg_destroy", "spg_last_error", "spg_abi_version", "spg_get_device_view", "spg_group_batch",
-    "spg_group_host", "spg_host_alloc", "spg_host_free", "spg_nms_peaks", "spg_limb_score", "spg_limb_match",
-    "spg_assemble", "spg_upload_peaks", "spg_upload_connections", "spg_download_peaks", "spg_download_connections",
-    "spg_download_people", "spg_download_status", "spg_launch_count", "spg_stage_kernel", "spg_wire_record_bytes",
-    "spg_set_wire_output", "spg_wire_create", "spg_wire_open", "spg_wire_close", "spg_wire_destroy", "spg_wire_signal",
-    "spg_wire_wait", "spg_postnet", "spg_match_assemble", "spg_wire_signal_many", "spg_arm_wire_signal",
-    "spg_postnet_rotated", "spg_prenet", "spg_group_ragged", "spg_postnet_ragged")
 
 
 class GroupingError(RuntimeError):
@@ -97,6 +88,51 @@ class _DeviceView(C.Structure):
                                           "n_persons", "people_xy", "people_score", "status")]
 
 
+_ptr, _i32, _i64, _u64, _f64, _int, _P = C.c_void_p, C.c_int32, C.c_int64, C.c_uint64, C.c_double, C.c_int, C.POINTER
+
+#: export name -> (restype, argtypes) of every function include/spgroup.h declares (tests/test_abi.py checks the table
+#: against the header and the built library).  Handles, streams and data pointers are all ``c_void_p``.
+_PROTOTYPES = {
+    "spg_create": (_int, [_P(_Config), _P(C.c_void_p)]),
+    "spg_destroy": (None, [_ptr]),
+    "spg_last_error": (C.c_char_p, [_ptr]),
+    "spg_abi_version": (_int, []),
+    "spg_get_device_view": (_int, [_ptr, _P(_DeviceView)]),
+    "spg_group_batch": (_int, [_ptr, _ptr, _i64, _i64, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
+    "spg_group_ragged": (_int, [_ptr, _P(_ImageMaps), _i32, _i32, _P(_Params), _ptr]),
+    "spg_group_host": (_int, [_ptr, _ptr, _ptr, _i32, _i32, _i32, _i32, _f64, _P(_Params), _ptr, _ptr, _ptr, _ptr]),
+    "spg_host_alloc": (_int, [_P(C.c_void_p), _u64]),
+    "spg_host_free": (_int, [_ptr]),
+    "spg_postnet": (_int, [_ptr, _P(_PostnetDesc), _i32, _i32, _i32, _ptr, _ptr, _i32, _ptr]),
+    "spg_postnet_rotated": (_int, [_ptr, _P(_PostnetDesc), _P(_PostnetRotation), _i32, _i32, _i32, _ptr, _ptr, _i32, _ptr]),
+    "spg_postnet_ragged": (_int, [_ptr, _P(_PostnetCommon), _P(_PostnetImage), _i32, _i32, _ptr]),
+    "spg_prenet": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _P(_PrenetItem), _i32, _ptr]),
+    "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
+    "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
+    "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
+    "spg_assemble": (_int, [_ptr, _i32, _P(_Params), _ptr]),
+    "spg_match_assemble": (_int, [_ptr, _i32, _P(_Params), _ptr]),
+    "spg_upload_peaks": (_int, [_ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_upload_connections": (_int, [_ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_download_peaks": (_int, [_ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_download_connections": (_int, [_ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_download_people": (_int, [_ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_download_status": (_int, [_ptr, _i32, _ptr, _ptr]),
+    "spg_wire_record_bytes": (_i64, [_ptr]),
+    "spg_set_wire_output": (_int, [_ptr, _ptr, _i64, _i32]),
+    "spg_arm_wire_signal": (_int, [_ptr, _ptr, _u64]),
+    "spg_wire_create": (_int, [_i32, _u64, _P(C.c_void_p), C.c_char_p]),
+    "spg_wire_open": (_int, [_i32, C.c_char_p, _P(C.c_void_p)]),
+    "spg_wire_close": (_int, [_ptr]),
+    "spg_wire_destroy": (_int, [_i32, _ptr]),
+    "spg_wire_signal": (_int, [_i32, _ptr, _u64, _ptr]),
+    "spg_wire_signal_many": (_int, [_i32, _P(C.c_void_p), _i32, _u64, _ptr]),
+    "spg_wire_wait": (_int, [_i32, _ptr, _u64, _ptr]),
+    "spg_launch_count": (_i64, [_ptr]),
+    "spg_stage_kernel": (C.c_char_p, [_ptr, _i32]),
+}
+EXPORTS = tuple(_PROTOTYPES)
+
 _lib = None
 
 
@@ -108,33 +144,9 @@ def load_library() -> C.CDLL:
             raise GroupingError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; "
                                 f"g.build()'` (or `make -C improved_body_parts_b200/csrc`).  There is no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
-        lib.spg_last_error.restype = C.c_char_p
-        lib.spg_last_error.argtypes = [C.c_void_p]
-        lib.spg_launch_count.restype = C.c_int64
-        lib.spg_launch_count.argtypes = [C.c_void_p]
-        lib.spg_stage_kernel.restype = C.c_char_p
-        lib.spg_stage_kernel.argtypes = [C.c_void_p, C.c_int32]
-        lib.spg_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
-        lib.spg_destroy.argtypes = [C.c_void_p]
-        lib.spg_destroy.restype = None
-        lib.spg_wire_record_bytes.restype = C.c_int64
-        lib.spg_wire_record_bytes.argtypes = [C.c_void_p]
-        lib.spg_set_wire_output.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32]
-        lib.spg_arm_wire_signal.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
-        lib.spg_wire_create.argtypes = [C.c_int32, C.c_uint64, C.POINTER(C.c_void_p), C.c_char_p]
-        lib.spg_wire_open.argtypes = [C.c_int32, C.c_char_p, C.POINTER(C.c_void_p)]
-        lib.spg_wire_close.argtypes = [C.c_void_p]
-        lib.spg_wire_destroy.argtypes = [C.c_int32, C.c_void_p]
-        lib.spg_wire_signal.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
-        lib.spg_wire_wait.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p]
-        lib.spg_postnet_rotated.argtypes = [C.c_void_p, C.POINTER(_PostnetDesc), C.POINTER(_PostnetRotation), C.c_int32,
-                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
-        lib.spg_postnet_ragged.argtypes = [C.c_void_p, C.POINTER(_PostnetCommon), C.POINTER(_PostnetImage), C.c_int32,
-                                           C.c_int32, C.c_void_p]
-        lib.spg_prenet.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                   C.c_int32, C.POINTER(_PrenetItem), C.c_int32, C.c_void_p]
-        lib.spg_group_ragged.argtypes = [C.c_void_p, C.POINTER(_ImageMaps), C.c_int32, C.c_int32, C.POINTER(_Params),
-                                         C.c_void_p]
+        for name, (restype, argtypes) in _PROTOTYPES.items():
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = restype, argtypes
         if lib.spg_abi_version() != ABI_VERSION:
             raise GroupingError("libspgroup.so ABI version mismatch")
         _lib = lib
@@ -172,6 +184,21 @@ def input_geometry(h: int, w: int, scale: float, max_downsample: int) -> Tuple[i
 
 def _vp(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _stream_handle(stream, device: int) -> int:
+    """The ``cudaStream_t`` of ``stream`` (a torch stream or a raw handle); ``None``: ``device``'s current stream."""
+    if stream is None:
+        import torch
+        stream = torch.cuda.current_stream(device)  # the handle's device, not torch's current one
+    return int(getattr(stream, "cuda_stream", stream))
+
+
+def _check(rc: int, what: str, handle=None) -> None:
+    """Raise for a non-zero return code, with the library's message (``handle`` None: the handle-less calls' slot)."""
+    if rc != 0:
+        msg = load_library().spg_last_error(handle)
+        raise GroupingError(f"{what} failed ({rc}): {msg.decode() if msg else ''}")
 
 
 class _CudaView:
@@ -255,49 +282,40 @@ class GroupResult:
 # ---- peer memory + stream-ordered signalling (the NVLink gather; sharding.py drives it) ------------------------
 def wire_create(device: int, nbytes: int) -> Tuple[int, bytes]:
     """Zero-filled device buffer other processes can map: ``(device address, 64-byte IPC handle)``."""
-    lib = load_library()
     ptr, hd = C.c_void_p(), C.create_string_buffer(64)
-    if lib.spg_wire_create(C.c_int32(device), C.c_uint64(nbytes), C.byref(ptr), hd) != 0:
-        raise GroupingError("spg_wire_create failed: " + (lib.spg_last_error(None) or b"").decode())
+    _check(load_library().spg_wire_create(device, nbytes, C.byref(ptr), hd), "spg_wire_create")
     return int(ptr.value), hd.raw
 
 
 def wire_open(device: int, ipc_handle: bytes) -> int:
-    lib = load_library()
     ptr = C.c_void_p()
-    if lib.spg_wire_open(C.c_int32(device), C.c_char_p(ipc_handle), C.byref(ptr)) != 0:
-        raise GroupingError("spg_wire_open failed: " + (lib.spg_last_error(None) or b"").decode())
+    _check(load_library().spg_wire_open(device, ipc_handle, C.byref(ptr)), "spg_wire_open")
     return int(ptr.value)
 
 
 def wire_close(peer_ptr: int) -> None:
-    load_library().spg_wire_close(C.c_void_p(peer_ptr))
+    load_library().spg_wire_close(peer_ptr)
 
 
 def wire_destroy(device: int, dev_ptr: int) -> None:
-    load_library().spg_wire_destroy(C.c_int32(device), C.c_void_p(dev_ptr))
+    load_library().spg_wire_destroy(device, dev_ptr)
 
 
 def wire_signal(device: int, word_ptr: int, value: int, stream) -> None:
     """Release-store ``value`` into a 64-bit word (local or peer memory) after everything earlier on ``stream``."""
-    if load_library().spg_wire_signal(C.c_int32(device), C.c_void_p(word_ptr), C.c_uint64(value),
-                                      C.c_void_p(int(getattr(stream, "cuda_stream", stream)))) != 0:
-        raise GroupingError("spg_wire_signal failed")
+    _check(load_library().spg_wire_signal(device, word_ptr, value, _stream_handle(stream, device)), "spg_wire_signal")
 
 
 def wire_signal_many(device: int, word_ptrs: Sequence[int], value: int, stream) -> None:
     """One launch that release-stores ``value`` into every word of ``word_ptrs`` (<= 32, local or peer memory)."""
-    arr = (C.c_void_p * len(word_ptrs))(*[C.c_void_p(p) for p in word_ptrs])
-    if load_library().spg_wire_signal_many(C.c_int32(device), arr, C.c_int32(len(word_ptrs)), C.c_uint64(value),
-                                           C.c_void_p(int(getattr(stream, "cuda_stream", stream)))) != 0:
-        raise GroupingError("spg_wire_signal_many failed")
+    arr = (C.c_void_p * len(word_ptrs))(*word_ptrs)
+    _check(load_library().spg_wire_signal_many(device, arr, len(word_ptrs), value, _stream_handle(stream, device)),
+           "spg_wire_signal_many")
 
 
 def wire_wait(device: int, word_ptr: int, value: int, stream) -> None:
     """Make ``stream`` wait until the LOCAL 64-bit word is >= ``value`` (a stream memory operation, no SM involved)."""
-    if load_library().spg_wire_wait(C.c_int32(device), C.c_void_p(word_ptr), C.c_uint64(value),
-                                    C.c_void_p(int(getattr(stream, "cuda_stream", stream)))) != 0:
-        raise GroupingError("spg_wire_wait failed")
+    _check(load_library().spg_wire_wait(device, word_ptr, value, _stream_handle(stream, device)), "spg_wire_wait")
 
 
 def device_bytes_view(ptr: int, nbytes: int, device: int):
@@ -326,9 +344,8 @@ class Grouper:
                       self.capP, self.capC, self.capR)
         rc = self._lib.spg_create(C.byref(cfg), C.byref(self._h))
         if rc != 0:
-            msg = self._lib.spg_last_error(None)
             self._h = C.c_void_p()
-            raise GroupingError(f"spg_create failed ({rc}): {msg.decode() if msg else ''}")
+            _check(rc, "spg_create")
 
     # -- lifetime ------------------------------------------------------------------------------
     def close(self) -> None:
@@ -348,11 +365,6 @@ class Grouper:
     def __exit__(self, *exc):
         self.close()
 
-    def _check(self, rc: int, what: str) -> None:
-        if rc != 0:
-            msg = self._lib.spg_last_error(self._h)
-            raise GroupingError(f"{what} failed ({rc}): {msg.decode() if msg else ''}")
-
     @property
     def launch_count(self) -> int:
         return int(self._lib.spg_launch_count(self._h))
@@ -368,27 +380,22 @@ class Grouper:
     # -- wire records (include/spgroup.h; wire.py is the host-side view) -------------------------------
     def wire_record_bytes(self, rows: Optional[int] = None) -> int:
         """Bytes of one image's record with ``rows`` person rows (default: ``max_person_rows``)."""
-        return 8 + int(self.capR if rows is None else rows) * (2 * self.J + 2) * 8
+        return wire.record_bytes(self.J, self.capR if rows is None else rows)
 
     def set_wire_output(self, dev_ptr: Optional[int], first_record: int = 0, rows: Optional[int] = None) -> None:
         """Make the assemble stage also write one wire record per image to ``dev_ptr`` (a raw device address: local
         memory or a peer GPU's buffer opened with ``wire_open``); ``None`` switches it off."""
-        rc = self._lib.spg_set_wire_output(self._h, C.c_void_p(dev_ptr or 0), C.c_int64(first_record),
-                                           C.c_int32(self.capR if rows is None else rows))
-        self._check(rc, "spg_set_wire_output")
+        rc = self._lib.spg_set_wire_output(self._h, dev_ptr, first_record, self.capR if rows is None else rows)
+        _check(rc, "spg_set_wire_output", self._h)
 
     def arm_wire_signal(self, word_ptr: Optional[int], value: int = 0) -> None:
         """The next single-launch assemble stage release-stores ``value`` into the 64-bit word at ``word_ptr`` (local or
         peer memory) when its last CTA is done: the "records landed" signal without a separate kernel.  One shot."""
-        rc = self._lib.spg_arm_wire_signal(self._h, C.c_void_p(word_ptr or 0), C.c_uint64(value))
-        self._check(rc, "spg_arm_wire_signal")
+        _check(self._lib.spg_arm_wire_signal(self._h, word_ptr, value), "spg_arm_wire_signal", self._h)
 
     # -- helpers ---------------------------------------------------------------------------------
-    def _stream_ptr(self, stream) -> C.c_void_p:
-        if stream is None:
-            import torch
-            stream = torch.cuda.current_stream(self.device)  # the handle's device, not torch's current one
-        return C.c_void_p(int(getattr(stream, "cuda_stream", stream)))
+    def _stream_ptr(self, stream) -> int:
+        return _stream_handle(stream, self.device)
 
     def _check_maps(self, t, name: str, channels: int, dtypes) -> None:
         """Shape / dtype / channel checks shared by the whole-path and the stage entry points."""
@@ -419,6 +426,21 @@ class Grouper:
             return F64
         raise GroupingError("body-part maps must be float32 or float64")
 
+    def _check_net_out(self, o, channels: int, n: Optional[int] = None, prefix: str = "") -> None:
+        """A network output the post-network stage reads: ``[N,2,C,h,w]`` (``n`` images) or, for ``n=None``, one pair
+        ``[2,C,h,w]``; float32 / float16 on the handle's device, rows contiguous, at least ``channels`` channels."""
+        import torch
+        lead = (2,) if n is None else (n, 2)
+        if not o.is_cuda or o.device.index != self.device or o.dim() != len(lead) + 3 or tuple(o.shape[:len(lead)]) != lead:
+            layout = "[2,C,h,w]" if n is None else "[N,2,C,h,w]"
+            raise GroupingError(f"{prefix}network output must be a {layout} CUDA tensor on the handle's device")
+        if o.stride(-1) != 1 or o.stride(-2) != o.shape[-1]:
+            raise GroupingError(f"{prefix}network output rows must be contiguous")
+        if o.dtype not in (torch.float32, torch.float16):
+            raise GroupingError(f"{prefix}network output must be float32 or float16")
+        if o.shape[-3] < channels:
+            raise GroupingError(f"{prefix}network output has too few channels")
+
     # -- whole path --------------------------------------------------------------------------------
     def group_device(self, heat, paf, image_extent: float, params=None, stream=None, paf_as_f64: bool = False) -> None:
         """peaks -> connections -> people on device-resident maps; asynchronous on ``stream``.
@@ -434,12 +456,10 @@ class Grouper:
         if paf.shape[0] != N or tuple(paf.shape[2:]) != (H, W):
             raise GroupingError("heat/paf shapes do not agree")
         p = params_struct(params)
-        rc = self._lib.spg_group_batch(self._h, C.c_void_p(heat.data_ptr()), C.c_int64(heat.stride(0)),
-                                       C.c_int64(heat.stride(1)), C.c_void_p(paf.data_ptr()),
-                                       C.c_int32(self._paf_dtype(paf, paf_as_f64)), C.c_int64(paf.stride(0)), C.c_int64(paf.stride(1)),
-                                       C.c_int32(N), C.c_int32(H), C.c_int32(W), C.c_double(float(image_extent)),
-                                       C.byref(p), self._stream_ptr(stream))
-        self._check(rc, "spg_group_batch")
+        rc = self._lib.spg_group_batch(self._h, heat.data_ptr(), heat.stride(0), heat.stride(1), paf.data_ptr(),
+                                       self._paf_dtype(paf, paf_as_f64), paf.stride(0), paf.stride(1), N, H, W,
+                                       float(image_extent), C.byref(p), self._stream_ptr(stream))
+        _check(rc, "spg_group_batch", self._h)
         self._peaks_shape = (N, H, W)
         self._last_n = N
 
@@ -476,9 +496,9 @@ class Grouper:
             arr[i] = _ImageMaps(heat.data_ptr(), paf.data_ptr(), heat.stride(1), paf.stride(1), heat.shape[2],
                                 heat.shape[3], extents[i])
         p = params_struct(params)
-        rc = self._lib.spg_group_ragged(self._h, arr, C.c_int32(len(maps)), C.c_int32(F32 if dtype is None else dtype),
-                                        C.byref(p), self._stream_ptr(stream))
-        self._check(rc, "spg_group_ragged")
+        rc = self._lib.spg_group_ragged(self._h, arr, len(maps), F32 if dtype is None else dtype, C.byref(p),
+                                        self._stream_ptr(stream))
+        _check(rc, "spg_group_ragged", self._h)
         self._peaks_shape = None
         self._last_n = len(maps)
 
@@ -502,10 +522,9 @@ class Grouper:
         o_sc = out.setdefault("people_score", np.zeros((N, self.capR), np.float64))
         o_st = out.setdefault("status", np.zeros((N,), np.uint32))
         p = params_struct(params)
-        rc = self._lib.spg_group_host(self._h, _vp(heat), _vp(paf), C.c_int32(F64 if paf.dtype == np.float64 else F32),
-                                      C.c_int32(N), C.c_int32(H), C.c_int32(W), C.c_double(float(image_extent)),
-                                      C.byref(p), _vp(o_n), _vp(o_xy), _vp(o_sc), _vp(o_st))
-        self._check(rc, "spg_group_host")
+        rc = self._lib.spg_group_host(self._h, _vp(heat), _vp(paf), F64 if paf.dtype == np.float64 else F32, N, H, W,
+                                      float(image_extent), C.byref(p), _vp(o_n), _vp(o_xy), _vp(o_sc), _vp(o_st))
+        _check(rc, "spg_group_host", self._h)
         self._last_n = N
         return out
 
@@ -537,14 +556,7 @@ class Grouper:
         fp, fh = self._flip_orders(flip_paf_ord, flip_heat_ord)
         scales = (_PostnetScale * len(net_outs))()
         for t, (o, (ch, cw)) in enumerate(zip(net_outs, crops)):
-            if not o.is_cuda or o.device.index != self.device or o.dim() != 5 or o.shape[0] != N or o.shape[1] != 2:
-                raise GroupingError("network output must be a [N,2,C,h,w] CUDA tensor on the handle's device")
-            if o.stride(4) != 1 or o.stride(3) != o.shape[4]:
-                raise GroupingError("network output rows must be contiguous")
-            if o.dtype not in (torch.float32, torch.float16):
-                raise GroupingError("network output must be float32 or float16")
-            if o.shape[2] < max(heat_chan0 + self.K, paf_chan0 + self.L):
-                raise GroupingError("network output has too few channels")
+            self._check_net_out(o, max(heat_chan0 + self.K, paf_chan0 + self.L), N)
             scales[t] = _PostnetScale(o.data_ptr(), F32 if o.dtype == torch.float32 else F16, o.stride(0), o.stride(1),
                                       o.stride(2), o.shape[3], o.shape[4], int(ch), int(cw))
         if heat_out is None:
@@ -566,10 +578,9 @@ class Grouper:
                     if m.shape != (2, 3):
                         raise GroupingError("a rotation matrix is 2x3")
                     rot[t] = _PostnetRotation(1, 0, (C.c_double * 6)(*m.reshape(6).tolist()))
-        rc = self._lib.spg_postnet_rotated(self._h, C.byref(desc), rot, C.c_int32(N), C.c_int32(H), C.c_int32(W),
-                                           C.c_void_p(heat_out.data_ptr()), C.c_void_p(paf_out.data_ptr()),
-                                           C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
-        self._check(rc, "spg_postnet_rotated")
+        rc = self._lib.spg_postnet_rotated(self._h, C.byref(desc), rot, N, H, W, heat_out.data_ptr(), paf_out.data_ptr(),
+                                           F32 if paf_dtype == torch.float32 else F64, self._stream_ptr(stream))
+        _check(rc, "spg_postnet_rotated", self._h)
         return heat_out, paf_out
 
     def _flip_orders(self, flip_paf_ord, flip_heat_ord):
@@ -608,17 +619,10 @@ class Grouper:
         net_dtype, results = None, []
         for i, (o, (ch, cw), (H, W)) in enumerate(images):
             H, W = int(H), int(W)
-            if not o.is_cuda or o.device.index != self.device or o.dim() != 4 or o.shape[0] != 2:
-                raise GroupingError(f"image {i}: network output must be a [2,C,h,w] CUDA tensor on the handle's device")
-            if o.stride(3) != 1 or o.stride(2) != o.shape[3]:
-                raise GroupingError(f"image {i}: network output rows must be contiguous")
-            if o.dtype not in (torch.float32, torch.float16):
-                raise GroupingError(f"image {i}: network output must be float32 or float16")
+            self._check_net_out(o, max(heat_chan0 + self.K, paf_chan0 + self.L), prefix=f"image {i}: ")
             if net_dtype is not None and o.dtype != net_dtype:
                 raise GroupingError(f"image {i}: every network output of a call needs the same dtype")
             net_dtype = o.dtype
-            if o.shape[1] < max(heat_chan0 + self.K, paf_chan0 + self.L):
-                raise GroupingError(f"image {i}: network output has too few channels")
             if outs is not None:
                 heat, paf = outs[i]
             else:
@@ -633,9 +637,9 @@ class Grouper:
         common = _PostnetCommon(int(stride), int(paf_chan0), int(heat_chan0), fp.ctypes.data_as(C.POINTER(C.c_int32)),
                                 fh.ctypes.data_as(C.POINTER(C.c_int32)), int(bool(nan_scrub)),
                                 F16 if net_dtype == torch.float16 else F32)
-        rc = self._lib.spg_postnet_ragged(self._h, C.byref(common), arr, C.c_int32(len(images)),
-                                          C.c_int32(F32 if paf_dtype == torch.float32 else F64), self._stream_ptr(stream))
-        self._check(rc, "spg_postnet_ragged")
+        rc = self._lib.spg_postnet_ragged(self._h, C.byref(common), arr, len(images),
+                                          F32 if paf_dtype == torch.float32 else F64, self._stream_ptr(stream))
+        _check(rc, "spg_postnet_ragged", self._h)
         return results
 
     # -- pre-network stage ----------------------------------------------------------------------------
@@ -694,10 +698,9 @@ class Grouper:
             m = (C.c_double * 6)(*(np.asarray(forward, np.float64).reshape(6).tolist() if forward is not None else [0.0] * 6))
             items[t] = _PrenetItem(scale, int(forward is not None), 0, m, o.data_ptr(), o.stride(0))
             results.append((o if batched else o[0], (H1, W1), reverse))
-        rc = self._lib.spg_prenet(self._h, C.c_void_p(img.data_ptr()), C.c_int64(img.stride(0)), C.c_int64(img.stride(1)),
-                                  C.c_int32(N), C.c_int32(h), C.c_int32(w), C.c_int32(md), C.c_int32(pv), items,
-                                  C.c_int32(len(pairs)), self._stream_ptr(stream))
-        self._check(rc, "spg_prenet")
+        rc = self._lib.spg_prenet(self._h, img.data_ptr(), img.stride(0), img.stride(1), N, h, w, md, pv, items, len(pairs),
+                                  self._stream_ptr(stream))
+        _check(rc, "spg_prenet", self._h)
         return results
 
     # -- stages -------------------------------------------------------------------------------------
@@ -708,10 +711,9 @@ class Grouper:
         N, _, H, W = heat.shape
         self._peaks_shape = (N, H, W)
         p = params_struct(params)
-        rc = self._lib.spg_nms_peaks(self._h, C.c_void_p(heat.data_ptr()), C.c_int64(heat.stride(0)),
-                                     C.c_int64(heat.stride(1)), C.c_int32(N), C.c_int32(H), C.c_int32(W), C.byref(p),
+        rc = self._lib.spg_nms_peaks(self._h, heat.data_ptr(), heat.stride(0), heat.stride(1), N, H, W, C.byref(p),
                                      self._stream_ptr(stream))
-        self._check(rc, "spg_nms_peaks")
+        _check(rc, "spg_nms_peaks", self._h)
         self._last_n = N
 
     def limb_score(self, paf, image_extent: float, params=None, stream=None, paf_as_f64: bool = False) -> None:
@@ -723,29 +725,27 @@ class Grouper:
         if ps is not None and (ps[0] < N or ps[1:] != (H, W)):
             raise GroupingError(f"paf is {N}x{H}x{W} but the peaks on the device come from {ps[0]}x{ps[1]}x{ps[2]} heat maps")
         p = params_struct(params)
-        rc = self._lib.spg_limb_score(self._h, C.c_void_p(paf.data_ptr()), C.c_int32(self._paf_dtype(paf, paf_as_f64)),
-                                      C.c_int64(paf.stride(0)), C.c_int64(paf.stride(1)), C.c_int32(N), C.c_int32(H),
-                                      C.c_int32(W), C.c_double(float(image_extent)), C.byref(p), self._stream_ptr(stream))
-        self._check(rc, "spg_limb_score")
+        rc = self._lib.spg_limb_score(self._h, paf.data_ptr(), self._paf_dtype(paf, paf_as_f64), paf.stride(0),
+                                      paf.stride(1), N, H, W, float(image_extent), C.byref(p), self._stream_ptr(stream))
+        _check(rc, "spg_limb_score", self._h)
         self._last_n = N
 
     def limb_match(self, n_images: int, params=None, stream=None) -> None:
         """Matching half of find_connections (evaluate.py:259-274)."""
         p = params_struct(params)
-        self._check(self._lib.spg_limb_match(self._h, C.c_int32(n_images), C.byref(p), self._stream_ptr(stream)),
-                    "spg_limb_match")
+        _check(self._lib.spg_limb_match(self._h, n_images, C.byref(p), self._stream_ptr(stream)),
+               "spg_limb_match", self._h)
 
     def assemble(self, n_images: int, params=None, stream=None) -> None:
         """find_people + process() tail (evaluate.py:279-498, 523-543)."""
         p = params_struct(params)
-        self._check(self._lib.spg_assemble(self._h, C.c_int32(n_images), C.byref(p), self._stream_ptr(stream)),
-                    "spg_assemble")
+        _check(self._lib.spg_assemble(self._h, n_images, C.byref(p), self._stream_ptr(stream)), "spg_assemble", self._h)
 
     def match_assemble(self, n_images: int, params=None, stream=None) -> None:
         """limb_match + assemble fused in one kernel (what the whole-path calls run)."""
         p = params_struct(params)
-        self._check(self._lib.spg_match_assemble(self._h, C.c_int32(n_images), C.byref(p), self._stream_ptr(stream)),
-                    "spg_match_assemble")
+        _check(self._lib.spg_match_assemble(self._h, n_images, C.byref(p), self._stream_ptr(stream)),
+               "spg_match_assemble", self._h)
 
     # -- state transfer ---------------------------------------------------------------------------------
     def upload_peaks(self, image_index: int, part_count, x, y, score, stream=None) -> None:
@@ -754,16 +754,16 @@ class Grouper:
         x = np.ascontiguousarray(x, np.float64)
         y = np.ascontiguousarray(y, np.float64)
         s = np.ascontiguousarray(score, np.float32)
-        self._check(self._lib.spg_upload_peaks(self._h, C.c_int32(image_index), _vp(pc), _vp(x), _vp(y), _vp(s),
-                                               self._stream_ptr(stream)), "spg_upload_peaks")
+        _check(self._lib.spg_upload_peaks(self._h, image_index, _vp(pc), _vp(x), _vp(y), _vp(s),
+                                          self._stream_ptr(stream)), "spg_upload_peaks", self._h)
 
     def upload_connections(self, image_index: int, conn_count, ij, score, norm, stream=None) -> None:
         cc = np.ascontiguousarray(conn_count, np.int32)
         ij = np.ascontiguousarray(ij, np.int32).reshape(-1, 2)
         sc = np.ascontiguousarray(score, np.float64)
         nm = np.ascontiguousarray(norm, np.float64)
-        self._check(self._lib.spg_upload_connections(self._h, C.c_int32(image_index), _vp(cc), _vp(ij), _vp(sc), _vp(nm),
-                                                     self._stream_ptr(stream)), "spg_upload_connections")
+        _check(self._lib.spg_upload_connections(self._h, image_index, _vp(cc), _vp(ij), _vp(sc), _vp(nm),
+                                                self._stream_ptr(stream)), "spg_upload_connections", self._h)
 
     def fetch(self, n_images: Optional[int] = None, stream=None) -> GroupResult:
         """Synchronise and copy every result of the last call to the host."""
@@ -778,21 +778,21 @@ class Grouper:
             conn_score=np.zeros((N, L, cP)), conn_norm=np.zeros((N, L, cP)), n_persons=np.zeros((N,), np.int32),
             subset=np.zeros((N, cR, K + 2, 2)), people_xy=np.zeros((N, cR, J, 2)), people_score=np.zeros((N, cR)),
             status=np.zeros((N,), np.uint32))
-        self._check(self._lib.spg_download_peaks(self._h, C.c_int32(N), _vp(r.peak_count), _vp(r.peak_x), _vp(r.peak_y),
-                                                 _vp(r.peak_score), _vp(r.peak_anchor), st), "spg_download_peaks")
-        self._check(self._lib.spg_download_connections(self._h, C.c_int32(N), _vp(r.conn_count), _vp(r.cand_count),
-                                                       _vp(r.conn_ij), _vp(r.conn_score), _vp(r.conn_norm), st),
-                    "spg_download_connections")
-        self._check(self._lib.spg_download_people(self._h, C.c_int32(N), _vp(r.n_persons), _vp(r.subset), _vp(r.people_xy),
-                                                  _vp(r.people_score), st), "spg_download_people")
-        self._check(self._lib.spg_download_status(self._h, C.c_int32(N), _vp(r.status), st), "spg_download_status")
+        _check(self._lib.spg_download_peaks(self._h, N, _vp(r.peak_count), _vp(r.peak_x), _vp(r.peak_y), _vp(r.peak_score),
+                                            _vp(r.peak_anchor), st), "spg_download_peaks", self._h)
+        _check(self._lib.spg_download_connections(self._h, N, _vp(r.conn_count), _vp(r.cand_count), _vp(r.conn_ij),
+                                                  _vp(r.conn_score), _vp(r.conn_norm), st),
+               "spg_download_connections", self._h)
+        _check(self._lib.spg_download_people(self._h, N, _vp(r.n_persons), _vp(r.subset), _vp(r.people_xy),
+                                             _vp(r.people_score), st), "spg_download_people", self._h)
+        _check(self._lib.spg_download_status(self._h, N, _vp(r.status), st), "spg_download_status", self._h)
         return r
 
     def device_tensors(self) -> dict:
         """Zero-copy torch views of the device-resident person lists (what the NCCL gather sends)."""
         import torch
         v = _DeviceView()
-        self._check(self._lib.spg_get_device_view(self._h, C.byref(v)), "spg_get_device_view")
+        _check(self._lib.spg_get_device_view(self._h, C.byref(v)), "spg_get_device_view", self._h)
         dev = torch.device("cuda", self.device)
         N, cR, J, K = self.max_batch, self.capR, self.J, self.K
 

@@ -6,6 +6,8 @@ import re
 import numpy as np
 import pytest
 
+from improved_body_parts_b200 import grouping
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -29,24 +31,67 @@ def test_library_exports_every_declared_symbol():
     assert lib.spg_abi_version() == grouping.ABI_VERSION
 
 
+#: ctypes mirror in grouping.py -> the struct of include/spgroup.h it mirrors
+MIRRORS = {grouping._Config: "spg_config", grouping._Params: "spg_params", grouping._DeviceView: "spg_device_view",
+           grouping._ImageMaps: "spg_image_maps", grouping._PostnetScale: "spg_postnet_scale",
+           grouping._PostnetDesc: "spg_postnet_desc", grouping._PostnetRotation: "spg_postnet_rotation",
+           grouping._PostnetCommon: "spg_postnet_common", grouping._PostnetImage: "spg_postnet_image",
+           grouping._PrenetItem: "spg_prenet_item"}
+#: layouts pinned by value too: sizeof, then the offset of every field
+PINNED = {"spg_postnet_rotation": [56, 0, 4, 8], "spg_prenet_item": [80, 0, 8, 12, 16, 64, 72]}
+
+
 def test_struct_layouts_match_the_header(tmp_path):
-    """ctypes mirrors vs the real header: compile a C probe that prints sizeof/offsetof."""
+    """Every ctypes mirror against the real header: one generated C probe prints sizeof and the offset of every field of
+    each mirrored struct."""
     import subprocess
 
-    from improved_body_parts_b200 import grouping
-
-    probe = tmp_path / "probe.c"
-    probe.write_text(
-        '#include <stdio.h>\n#include <stddef.h>\n#include "spgroup.h"\n'
-        'int main(void){printf("%zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(spg_config), sizeof(spg_params), '
-        'sizeof(spg_device_view), offsetof(spg_config, limbs), offsetof(spg_config, out_from_part), '
-        'offsetof(spg_config, max_batch), offsetof(spg_params, mid_num), offsetof(spg_device_view, peak_x));return 0;}\n')
-    exe = tmp_path / "probe"
+    mirrors = {c for c in vars(grouping).values() if isinstance(c, type) and issubclass(c, ctypes.Structure)}
+    assert mirrors == set(MIRRORS)
+    lines = []
+    for cls, name in MIRRORS.items():
+        args = ", ".join([f"sizeof({name})"] + [f"offsetof({name}, {f})" for f, _ in cls._fields_])
+        lines.append(f'printf("{name}{" %zu" * (1 + len(cls._fields_))}\\n", {args});')
+    probe, exe = tmp_path / "probe.c", tmp_path / "probe"
+    probe.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "spgroup.h"\nint main(void){\n' + "\n".join(lines) +
+                     "\nreturn 0;}\n")
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(probe), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
-    C, V, P = grouping._Config, grouping._DeviceView, grouping._Params
-    assert got == [ctypes.sizeof(C), ctypes.sizeof(P), ctypes.sizeof(V), C.limbs.offset, C.out_from_part.offset,
-                   C.max_batch.offset, P.mid_num.offset, V.peak_x.offset]
+    got = {name: [int(v) for v in vals] for name, *vals in
+           (line.split() for line in subprocess.check_output([str(exe)], text=True).splitlines())}
+    want = {name: [ctypes.sizeof(cls)] + [getattr(cls, f).offset for f, _ in cls._fields_] for cls, name in MIRRORS.items()}
+    assert got == want
+    for name, layout in PINNED.items():
+        assert got[name] == layout, name
+
+
+_C_SCALARS = {"int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "double": ctypes.c_double}
+_C_RESULTS = {"int": ctypes.c_int, "void": None, "int64_t": ctypes.c_int64, "const char *": ctypes.c_char_p}
+
+
+def _prototypes():
+    """name -> (return type, [parameter declarations]) of every function include/spgroup.h declares."""
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "spgroup.h")).read(), flags=re.S)
+    out = {}
+    for ret, name, params in re.findall(r"^([\w ]*?\**)\s*\b(spg_\w+)\s*\(([^)]*)\)\s*;", src, flags=re.M):
+        params = " ".join(params.split())
+        out[name] = (ret.strip(), [] if params == "void" else [p.strip() for p in params.split(",")])
+    return out
+
+
+def test_prototype_table_matches_the_header():
+    """The binding's argtypes / restype of every export against its C prototype: the parameter count, and per parameter
+    its kind -- a pointer (arrays such as ``ipc_handle[64]`` included) or the exact integer / floating-point type."""
+    protos = _prototypes()
+    assert sorted(protos) == sorted(grouping.EXPORTS)
+    for name, (ret, params) in protos.items():
+        restype, argtypes = grouping._PROTOTYPES[name]
+        assert restype is _C_RESULTS[ret], name
+        assert len(argtypes) == len(params), name
+        for decl, t in zip(params, argtypes):
+            if "*" in decl or "[" in decl:
+                assert t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer), (name, decl, t)
+            else:
+                assert t is _C_SCALARS[decl.rsplit(" ", 1)[0]], (name, decl, t)
 
 
 def test_no_gpu_means_a_loud_failure_not_a_fallback():

@@ -1,13 +1,9 @@
-"""CPU: the rotation search's warp (oracle/postnet_rotation_port.py) against OpenCV, and the C ABI's rotation struct.
+"""CPU: the rotation search's warp (oracle/postnet_rotation_port.py) against OpenCV.
 
 ``cv2.warpAffine`` on float32 maps is OpenCV's generic fixed-point warp, which the port restates: the bar is BIT-IDENTICAL
 maps (compared as uint32, so NaN payloads and signed zeros count), NaN and inf included.  The item chain
 (evaluate.py:143-158: resize, warp, crop, resize) is checked against the reference's lines written out with cv2.
 """
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
@@ -17,7 +13,6 @@ from improved_body_parts_b200 import skeleton
 from oracle import postnet_port as pp
 from oracle import postnet_rotation_port as pr
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GRIDS = [(640, 896), (256, 256), (257, 131), (131, 257)]
 ANGLES = [-45, -30, -7.5, 0.5, 13, 30, 90, 180]
 
@@ -105,17 +100,3 @@ def test_item_chain_places_the_warp_between_the_resizes(hw, crop, image, angle):
     plain = pr.post_network_item(out, 4, padded, pad, image, 30, 48, skeleton.FLIP_PAF_ORD, skeleton.FLIP_HEAT_ORD[:18])
     base = pp.post_network_scale(out, 4, padded, pad, image, 30, 48, skeleton.FLIP_PAF_ORD, skeleton.FLIP_HEAT_ORD[:18])
     assert all(np.array_equal(_bits(a), _bits(b)) for a, b in zip(plain, base))
-
-
-def test_rotation_struct_layout_matches_the_header(tmp_path):
-    from improved_body_parts_b200 import grouping
-
-    probe = tmp_path / "probe.c"
-    probe.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "spgroup.h"\n'
-                     'int main(void){printf("%zu %zu %zu\\n", sizeof(spg_postnet_rotation), '
-                     'offsetof(spg_postnet_rotation, reserved), offsetof(spg_postnet_rotation, matrix));return 0;}\n')
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(probe), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
-    R = grouping._PostnetRotation
-    assert got == [ctypes.sizeof(R), R.reserved.offset, R.matrix.offset] == [56, 4, 8]

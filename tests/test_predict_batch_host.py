@@ -1,6 +1,5 @@
-"""CPU: the host side of the batched predict(): the ctypes mirrors of spg_postnet_ragged's structs, the bucket planner
-of ``dropin.predict_batch`` and the launcher's ``--forward-batch``."""
-import ctypes
+"""CPU: the host side of the batched predict(): the bucket planner of ``dropin.predict_batch`` and the launcher's
+``--forward-batch``."""
 import os
 import subprocess
 import sys
@@ -11,26 +10,6 @@ import pytest
 from oracle import prenet_port as pn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def test_postnet_ragged_structs_match_the_header(tmp_path):
-    from improved_body_parts_b200 import grouping
-
-    probe = tmp_path / "probe.c"
-    fields_i = ("net_out", "pair_stride", "chan_stride", "h", "w", "crop_h", "crop_w", "height", "width", "heat_out", "paf_out")
-    fields_c = ("stride", "paf_chan0", "heat_chan0", "flip_paf_ord", "flip_heat_ord", "nan_scrub", "net_dtype")
-    offs = " ".join(["%zu"] * (2 + len(fields_i) + len(fields_c)))
-    args = ", ".join(["sizeof(spg_postnet_image)", "sizeof(spg_postnet_common)"] +
-                     [f"offsetof(spg_postnet_image, {f})" for f in fields_i] +
-                     [f"offsetof(spg_postnet_common, {f})" for f in fields_c])
-    probe.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "spgroup.h"\n'
-                     f'int main(void){{printf("{offs}\\n", {args});return 0;}}\n')
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(probe), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
-    I, Cm = grouping._PostnetImage, grouping._PostnetCommon
-    assert got == [ctypes.sizeof(I), ctypes.sizeof(Cm)] + [getattr(I, f).offset for f in fields_i] + \
-        [getattr(Cm, f).offset for f in fields_c]
 
 
 def test_bucket_planner_is_the_prenet_geometry():

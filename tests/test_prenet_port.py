@@ -1,22 +1,16 @@
-"""CPU: the input side of predict() (oracle/prenet_port.py) against OpenCV, and the C ABI's prenet item struct.
+"""CPU: the input side of predict() (oracle/prenet_port.py) against OpenCV.
 
 ``cv2.resize`` of uint8 images with IPP switched off is OpenCV's generic path, which the port restates: the bar is
 BIT-IDENTICAL images.  With IPP on (what the reference's wheels run) every pixel is within 1 LSB.  The item chain
 (evaluate.py:94-121: clamp, resize, pad, / 255, warp, mirror) is checked against the reference's lines written out
 with cv2.
 """
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 cv2 = pytest.importorskip("cv2")
 
 from oracle import prenet_port as pn
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture
@@ -160,20 +154,3 @@ def test_pad_value_goes_through_the_table():
     assert crop == (9, 13) and pad == [0, 0, 7, 3]
     assert (pair[0, 9:, :, :] == np.float32(200 / 255)).all() and (pair[0, :, 13:, :] == np.float32(200 / 255)).all()
     assert np.array_equal(pair[1], pair[0, :, ::-1, :])
-
-
-def test_prenet_item_struct_layout_matches_the_header(tmp_path):
-    from improved_body_parts_b200 import grouping
-
-    probe = tmp_path / "probe.c"
-    probe.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "spgroup.h"\n'
-                     'int main(void){printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(spg_prenet_item), '
-                     'offsetof(spg_prenet_item, rotate), offsetof(spg_prenet_item, reserved), '
-                     'offsetof(spg_prenet_item, matrix), offsetof(spg_prenet_item, out), '
-                     'offsetof(spg_prenet_item, out_image_stride));return 0;}\n')
-    exe = tmp_path / "probe"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(probe), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
-    S = grouping._PrenetItem
-    assert got == [ctypes.sizeof(S), S.rotate.offset, S.reserved.offset, S.matrix.offset, S.out.offset,
-                   S.out_image_stride.offset] == [80, 8, 12, 16, 64, 72]
