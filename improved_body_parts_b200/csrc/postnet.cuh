@@ -50,13 +50,8 @@ struct PostScale {              // one entry of the scale loop (evaluate.py:90)
 };
 
 struct PostArgs {
-    const void *net;            // (generic kernel: the one scale of this launch; the stride-4 kernel reads `sc`)
-    int net_is_f16;
-    long long img_stride, pair_stride, chan_stride;
-    int h, w;
-    int stride;                 // model_params['stride']
-    int crop_h, crop_w;
-    PostScale sc[kPostMaxScales];  // stride-4 kernel: the scales summed inside ONE launch, in the order of the scale loop
+    PostScale sc[kPostMaxScales];  // the scales summed inside ONE launch, in the order of the scale loop (stride 4 fuses up to
+                                   // kPostMaxScales; the generic and the rotated kernel take one)
     int n_fused;                // entries of `sc` in this launch; scale_index is the index of sc[0] in the whole loop
     int H, W;                   // image size = output size
     int n_out;                  // output channels handled: K keypoint + L body-part
@@ -71,7 +66,7 @@ struct PostArgs {
     int nan_scrub;              // demo_image.py:179-180: NaN -> 0 after the accumulation
     int tile_w, tile_h, tiles_x, tiles_y;
     int chan_chunk;             // stride-4 kernel: channels one CTA walks over (grid.y = ceil(n_out / chan_chunk))
-    double sx1, sy1, sx2, sy2;  // source step per destination pixel of the two resizes
+    double sx1, sy1;            // source step per destination pixel of the x stride resize (the second resize's: sc[t])
     double rot[6];              // postnet_rot_kernel: the inverse of the item's warp matrix (x4 grid of the output -> of the input)
 };
 
@@ -120,16 +115,17 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
     const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
     const int ox0 = tx * a.tile_w, oy0 = ty * a.tile_h;
     const int tw = min(a.tile_w, a.W - ox0), th = min(a.tile_h, a.H - oy0);
-    const bool identity = a.crop_h == a.H && a.crop_w == a.W;  // second resize with scale 1: weights (0, 1, 0, 0)
+    const PostScale &S = a.sc[0];
+    const bool identity = S.crop_h == a.H && S.crop_w == a.W;  // second resize with scale 1: weights (0, 1, 0, 0)
 
     // ---- tables of the second resize for this tile's output columns / rows
-    if (tid < tw) t2x[tid].s = axis_entry(ox0 + tid, a.sx2, t2x[tid].c);
-    if (tid >= 64 && tid < 64 + th) t2y[tid - 64].s = axis_entry(oy0 + tid - 64, a.sy2, t2y[tid - 64].c);
+    if (tid < tw) t2x[tid].s = axis_entry(ox0 + tid, S.sx2, t2x[tid].c);
+    if (tid >= 64 && tid < 64 + th) t2y[tid - 64].s = axis_entry(oy0 + tid - 64, S.sy2, t2y[tid - 64].c);
     __syncthreads();
     if (tid == 0) {
         // crop-coordinate range the tile reads (taps clamped to the cropped array, :148-149)
-        const int c_lo = identity ? ox0 : clampi(t2x[0].s, 0, a.crop_w - 1), c_hi = identity ? ox0 + tw - 1 : clampi(t2x[tw - 1].s + 3, 0, a.crop_w - 1);
-        const int rr_lo = identity ? oy0 : clampi(t2y[0].s, 0, a.crop_h - 1), rr_hi = identity ? oy0 + th - 1 : clampi(t2y[th - 1].s + 3, 0, a.crop_h - 1);
+        const int c_lo = identity ? ox0 : clampi(t2x[0].s, 0, S.crop_w - 1), c_hi = identity ? ox0 + tw - 1 : clampi(t2x[tw - 1].s + 3, 0, S.crop_w - 1);
+        const int rr_lo = identity ? oy0 : clampi(t2y[0].s, 0, S.crop_h - 1), rr_hi = identity ? oy0 + th - 1 : clampi(t2y[th - 1].s + 3, 0, S.crop_h - 1);
         r_lo[0] = c_lo; r_lo[1] = c_hi - c_lo + 1;
         r_lo[2] = rr_lo; r_lo[3] = rr_hi - rr_lo + 1;
     }
@@ -139,26 +135,26 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
     if (tid < C1) t1x[tid].s = axis_entry(c_lo + tid, a.sx1, t1x[tid].c);
     if (tid >= 128 && tid < 128 + R1) t1y[tid - 128].s = axis_entry(y_lo + tid - 128, a.sy1, t1y[tid - 128].c);
     __syncthreads();
-    const int sc_lo = clampi(t1x[0].s, 0, a.w - 1), sc_hi = clampi(t1x[C1 - 1].s + 3, 0, a.w - 1);
-    const int sr_lo = clampi(t1y[0].s, 0, a.h - 1), sr_hi = clampi(t1y[R1 - 1].s + 3, 0, a.h - 1);
+    const int sc_lo = clampi(t1x[0].s, 0, S.w - 1), sc_hi = clampi(t1x[C1 - 1].s + 3, 0, S.w - 1);
+    const int sr_lo = clampi(t1y[0].s, 0, S.h - 1), sr_hi = clampi(t1y[R1 - 1].s + 3, 0, S.h - 1);
     const int CS = sc_hi - sc_lo + 1, RS = sr_hi - sr_lo + 1;
 
     // ---- source tile: (out[c] + mirrored_out[flip(c)][:, ::-1]) / 2  (:139-140), float32
     {
-        const long long base0 = (long long)n * a.img_stride + (long long)a.src_chan[c] * a.chan_stride;
-        const long long base1 = (long long)n * a.img_stride + a.pair_stride + (long long)a.flip_chan[c] * a.chan_stride;
+        const long long base0 = (long long)n * S.img_stride + (long long)a.src_chan[c] * S.chan_stride;
+        const long long base1 = (long long)n * S.img_stride + S.pair_stride + (long long)a.flip_chan[c] * S.chan_stride;
         for (int e = tid; e < RS * CS; e += kPostThreads) {
             const int i = e / CS, j = e - i * CS;
             const int y = sr_lo + i, x = sc_lo + j;
             float v0, v1;
-            if (a.net_is_f16) {
-                const __half *p = static_cast<const __half *>(a.net);
-                v0 = __half2float(p[base0 + (long long)y * a.w + x]);
-                v1 = __half2float(p[base1 + (long long)y * a.w + (a.w - 1 - x)]);
+            if (S.net_is_f16) {
+                const __half *p = static_cast<const __half *>(S.net);
+                v0 = __half2float(p[base0 + (long long)y * S.w + x]);
+                v1 = __half2float(p[base1 + (long long)y * S.w + (S.w - 1 - x)]);
             } else {
-                const float *p = static_cast<const float *>(a.net);
-                v0 = p[base0 + (long long)y * a.w + x];
-                v1 = p[base1 + (long long)y * a.w + (a.w - 1 - x)];
+                const float *p = static_cast<const float *>(S.net);
+                v0 = p[base0 + (long long)y * S.w + x];
+                v1 = p[base1 + (long long)y * S.w + (S.w - 1 - x)];
             }
             s0[i * kPostCS + j] = __fdiv_rn(__fadd_rn(v0, v1), 2.0f);
         }
@@ -169,8 +165,8 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
         const int i = e / C1, X = e - i * C1;
         const AxisTab &t = t1x[X];
         const float *row = s0 + i * kPostCS - sc_lo;
-        s1[i * kPostC1 + X] = tap4(row[clampi(t.s, 0, a.w - 1)], row[clampi(t.s + 1, 0, a.w - 1)], row[clampi(t.s + 2, 0, a.w - 1)],
-                                   row[clampi(t.s + 3, 0, a.w - 1)], t.c);
+        s1[i * kPostC1 + X] = tap4(row[clampi(t.s, 0, S.w - 1)], row[clampi(t.s + 1, 0, S.w - 1)], row[clampi(t.s + 2, 0, S.w - 1)],
+                                   row[clampi(t.s + 3, 0, S.w - 1)], t.c);
     }
     __syncthreads();
     // ---- pass 2: vertical x stride -> the cropped intermediate (what the reference holds after :148 / :157)
@@ -178,8 +174,8 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
         const int Y = e / C1, X = e - Y * C1;
         const AxisTab &t = t1y[Y];
         const float *col = s1 + X - sr_lo * kPostC1;
-        s2[Y * kPostC1 + X] = tap4(col[clampi(t.s, 0, a.h - 1) * kPostC1], col[clampi(t.s + 1, 0, a.h - 1) * kPostC1],
-                                   col[clampi(t.s + 2, 0, a.h - 1) * kPostC1], col[clampi(t.s + 3, 0, a.h - 1) * kPostC1], t.c);
+        s2[Y * kPostC1 + X] = tap4(col[clampi(t.s, 0, S.h - 1) * kPostC1], col[clampi(t.s + 1, 0, S.h - 1) * kPostC1],
+                                   col[clampi(t.s + 2, 0, S.h - 1) * kPostC1], col[clampi(t.s + 3, 0, S.h - 1) * kPostC1], t.c);
     }
     __syncthreads();
     // ---- pass 3: horizontal pass of the second resize (clamped to the cropped array)
@@ -188,8 +184,8 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
             const int Y = e / tw, x = e - Y * tw;
             const AxisTab &t = t2x[x];
             const float *row = s2 + Y * kPostC1 - c_lo;
-            s3[Y * kPostTW + x] = tap4(row[clampi(t.s, 0, a.crop_w - 1)], row[clampi(t.s + 1, 0, a.crop_w - 1)],
-                                       row[clampi(t.s + 2, 0, a.crop_w - 1)], row[clampi(t.s + 3, 0, a.crop_w - 1)], t.c);
+            s3[Y * kPostTW + x] = tap4(row[clampi(t.s, 0, S.crop_w - 1)], row[clampi(t.s + 1, 0, S.crop_w - 1)],
+                                       row[clampi(t.s + 2, 0, S.crop_w - 1)], row[clampi(t.s + 3, 0, S.crop_w - 1)], t.c);
         }
         __syncthreads();
     }
@@ -207,8 +203,8 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
         } else {
             const AxisTab &t = t2y[y];
             const float *col = s3 + x - y_lo * kPostTW;
-            v = tap4(col[clampi(t.s, 0, a.crop_h - 1) * kPostTW], col[clampi(t.s + 1, 0, a.crop_h - 1) * kPostTW],
-                     col[clampi(t.s + 2, 0, a.crop_h - 1) * kPostTW], col[clampi(t.s + 3, 0, a.crop_h - 1) * kPostTW], t.c);
+            v = tap4(col[clampi(t.s, 0, S.crop_h - 1) * kPostTW], col[clampi(t.s + 1, 0, S.crop_h - 1) * kPostTW],
+                     col[clampi(t.s + 2, 0, S.crop_h - 1) * kPostTW], col[clampi(t.s + 3, 0, S.crop_h - 1) * kPostTW], t.c);
         }
         const size_t o = pbase + (size_t)(oy0 + y) * a.W + (ox0 + x);
         const float part = __fdiv_rn(v, nf);  // float32 array / Python int -> float32

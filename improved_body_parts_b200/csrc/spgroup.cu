@@ -751,37 +751,36 @@ static void invert_affine(const double *M, double *m) {
     m[2] = b1; m[5] = b2;
 }
 
-// The grid over output tiles of a.tile_w x a.tile_h: a CTA builds its tile's tables once and walks over a chunk of
-// channels -- as many as still leave ~ctas_per_sm CTAs per SM in the grid (a few resident: several waves).
-// ctas_per_sm 0: one channel per CTA.
+// Channels per CTA: a CTA builds its tile's tables once and walks over a chunk of channels -- as many as still leave
+// ~ctas_per_sm CTAs per SM over `tiles` tiles (a few resident: several waves).  ctas_per_sm 0: one channel per CTA.
 static int post_chan_chunk(const spg_handle *h, int n_out, long long tiles, int ctas_per_sm) {
     const int n_chunks = ctas_per_sm == 0 ? n_out
                                           : (int)std::min<long long>(n_out, std::max<long long>(1, ((long long)h->sm_count * ctas_per_sm + tiles - 1) / tiles));
     return (n_out + n_chunks - 1) / n_chunks;
 }
 
+// the tiles_x x tiles_y output tiles of tile_w x tile_h that cover an H x W image; returns their number
+static long long post_tiles(int H, int W, int tile_w, int tile_h, int &tiles_x, int &tiles_y) {
+    tiles_x = (W + tile_w - 1) / tile_w;
+    tiles_y = (H + tile_h - 1) / tile_h;
+    return (long long)tiles_x * tiles_y;
+}
+
 static int postnet_grid(spg_handle *h, PostArgs &a, int n, int ctas_per_sm, dim3 *grid) {
-    a.tiles_x = (a.W + a.tile_w - 1) / a.tile_w;
-    a.tiles_y = (a.H + a.tile_h - 1) / a.tile_h;
-    if ((long long)a.tiles_x * a.tiles_y > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
-    a.chan_chunk = post_chan_chunk(h, a.n_out, (long long)a.tiles_x * a.tiles_y * n, ctas_per_sm);
-    *grid = dim3((unsigned)(a.tiles_x * a.tiles_y), (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
+    const long long tiles = post_tiles(a.H, a.W, a.tile_w, a.tile_h, a.tiles_x, a.tiles_y);
+    if (tiles > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
+    a.chan_chunk = post_chan_chunk(h, a.n_out, tiles * n, ctas_per_sm);
+    *grid = dim3((unsigned)tiles, (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
     return SPG_OK;
 }
 
-// CTAs per SM the channel chunks aim at: the identity kernel (4 resident per SM) and the four-phase kernel (2 resident)
+// CTAs per SM the channel chunks aim at: the identity kernel (4 resident per SM) and the four-phase kernels (2 resident)
 constexpr int kPostIdentCtasPerSm = 32, kPostCtasPerSm = 16;
 
 // output tile of the four-phase kernels: as large as the shared-memory tiles of the intermediate / source allow
 static int post_tile_dim(double s2, double s1, int cap1, int cap0, int maxd, double margin) {
     const double c1 = std::min((double)cap1, ((double)cap0 - 7.0) / s1) - margin;  // intermediate span allowed
     return std::max(1, std::min(maxd, (int)(c1 / std::max(s2, 1e-6))));
-}
-
-// shrink the four-phase kernel's output tile (tw x th) until it fits item S's second resize
-static void post_tile_fit(const PostScale &S, double s1, int &tw, int &th) {
-    tw = std::min(tw, post_tile_dim(S.sx2, s1, kPostF_C1, kPostF_CS, kPostTW, 13.0));
-    th = std::min(th, post_tile_dim(S.sy2, s1, kPostF_R1, kPostF_RS, kPostTH, 13.0));
 }
 
 // one item's network output and the steps of its resize to the H x W image
@@ -797,13 +796,22 @@ static PostScale post_scale(const void *net, int dtype, int64_t img_stride, int6
     return s;
 }
 
-static bool post_crop_fits(int h, int w, int crop_h, int crop_w, int stride) {
-    return h >= 1 && w >= 1 && crop_h >= 1 && crop_w >= 1 && crop_h <= h * stride && crop_w <= w * stride;
+// A scale's or an image's network output ("<what> <i>" in the error): present, float32 or float16, and its crop inside
+// the h x w output up-sampled by `stride`
+static int check_net_out(spg_handle *h, const char *what, int i, const void *net, int dtype, int hn, int wn, int crop_h, int crop_w,
+                         int stride) {
+    if (!net) return fail(h, SPG_E_INVALID, "%s %d: net_out is NULL", what, i);
+    if (dtype != SPG_F32 && dtype != SPG_F16) return fail(h, SPG_E_INVALID, "%s %d: network output must be SPG_F32 or SPG_F16", what, i);
+    if (hn < 1 || wn < 1 || crop_h < 1 || crop_w < 1 || crop_h > hn * stride || crop_w > wn * stride)
+        return fail(h, SPG_E_INVALID, "%s %d: crop %dx%d does not fit the up-sampled %dx%d output", what, i, crop_h, crop_w, hn * stride,
+                    wn * stride);
+    return SPG_OK;
 }
 
-// the output channels (K keypoint, then L body part) and the network channels each one averages, validated
-static int post_channels(spg_handle *h, int paf_chan0, int heat_chan0, const int32_t *flip_paf_ord, const int32_t *flip_heat_ord,
-                         PostArgs &a) {
+// The arguments every launch of a call shares: the output channels (K keypoint, then L body part) and the network
+// channels each one averages, validated; the scale count, NaN scrub, body-part dtype and the x stride resize's step.
+static int post_common(spg_handle *h, int stride, int n_scales, int paf_chan0, int heat_chan0, const int32_t *flip_paf_ord,
+                       const int32_t *flip_heat_ord, int nan_scrub, int paf_dtype, PostArgs &a) {
     const Workspace &ws = h->ws;
     if (ws.K + ws.L > kMaxNetChannels) return fail(h, SPG_E_INVALID, "too many channels for postnet");
     a.n_out = ws.K + ws.L; a.K = ws.K;
@@ -816,6 +824,90 @@ static int post_channels(spg_handle *h, int paf_chan0, int heat_chan0, const int
         if (flip_paf_ord[k] < 0 || flip_paf_ord[k] >= ws.L) return fail(h, SPG_E_INVALID, "flip_paf_ord[%d] out of range", k);
         a.src_chan[ws.K + k] = (short)(paf_chan0 + k);
         a.flip_chan[ws.K + k] = (short)(paf_chan0 + flip_paf_ord[k]);
+    }
+    a.n_scales = n_scales; a.nan_scrub = nan_scrub != 0; a.paf_is_f64 = paf_dtype == SPG_F64;
+    a.sx1 = 1.0 / (double)stride; a.sy1 = a.sx1;  // cv2.resize(fx = stride): scale = 1/fx
+    return SPG_OK;
+}
+
+// The kernel families of the post-network stage (PostPlan::family), each with its kernels by template flags
+// [single][ident][f16] (nullptr: not instantiated) and its single-scale ragged kernels by [f16], under the names
+// spg_stage_kernel reports.
+enum : int { kPostIdent, kPostFourPhase, kPostRotated, kPostGeneric };
+struct PostKernels {
+    const char *name;
+    void (*fn[2][2][2])(PostArgs);
+    const char *ragged_name;
+    void (*ragged[2])(PostArgs, PostRagged);
+};
+static const PostKernels kPostKernels[4] = {
+    {"postnet_x4_ident_kernel", {{}, {{}, {postnet_x4_ident_kernel<false>, postnet_x4_ident_kernel<true>}}},
+     "postnet_x4_ident_ragged_kernel", {postnet_x4_ident_ragged_kernel<false>, postnet_x4_ident_ragged_kernel<true>}},
+    {"postnet_kernel",
+     {{{postnet_kernel<false, false, false>, postnet_kernel<false, false, true>}, {postnet_kernel<false, true, false>, postnet_kernel<false, true, true>}},
+      {{postnet_kernel<true, false, false>, postnet_kernel<true, false, true>}, {}}},
+     "postnet_ragged_kernel", {postnet_ragged_kernel<false>, postnet_ragged_kernel<true>}},
+    {"postnet_rot_kernel",
+     {{{postnet_rot_kernel<false, false>, postnet_rot_kernel<false, true>}, {}}, {{postnet_rot_kernel<true, false>, postnet_rot_kernel<true, true>}, {}}},
+     "", {}},
+    {"postnet_generic_kernel", {{{postnet_generic_kernel}}}, "", {}},
+};
+
+struct PostPlan {
+    int family;
+    bool single, ident, f16;  // the kernel's template flags (kPostKernels[family].fn)
+    int tile_w, tile_h;
+    int ctas_per_sm;          // target of the channel chunk (post_chan_chunk)
+    size_t smem;              // dynamic shared memory
+};
+
+// The schedule of one launch over the n_fused scales sc of an H x W image; rot: the inverse warp matrix of a rotated item.
+// `single`: one scale in the whole scale loop; `item` names the item in the error.
+static int plan_post(spg_handle *h, const PostScale *sc, int n_fused, bool single, int stride, int H, int W, const double *rot,
+                     int item, PostPlan *pl) {
+    const double s1 = 1.0 / (double)stride;  // PostArgs::sx1 (post_common)
+    if (stride != 4) {
+        *pl = PostPlan{kPostGeneric, false, false, false, post_tile_dim(sc[0].sx2, s1, kPostC1, kPostCS, kPostTW, 7.0),
+                       post_tile_dim(sc[0].sy2, s1, kPostR1, kPostRS, kPostTH, 7.0), 0, 0};
+        return SPG_OK;
+    }
+    const PostScale &S = sc[0];
+    if (rot) {
+        // the largest tile (up to 64 x 32) whose crop span and rotated box fit the kernel's buffers: a span of cw x ch
+        // crop pixels reads a box of |m0| cw + |m1| ch (+ 7, the box's margins) columns of the x4 grid, and its x4
+        // groups add up to two more
+        const bool ident = S.crop_h == H && S.crop_w == W;
+        auto fits = [&](int tw, int th) {
+            const double cw = ident ? tw : tw * S.sx2 + 5.0, ch = ident ? th : th * S.sy2 + 5.0;
+            const double bw = std::fabs(rot[0]) * cw + std::fabs(rot[1]) * ch + 7.0;
+            const double bh = std::fabs(rot[3]) * cw + std::fabs(rot[4]) * ch + 7.0;
+            return cw <= kPostF_C1 && ch <= kPostR_R1 && bw / 4.0 + 2.0 <= kPostF_Q && bh / 4.0 + 2.0 <= kPostF_P;
+        };
+        int tw = kPostTW, th = kPostTH;
+        while (!fits(tw, th) && (tw > 1 || th > 1)) {
+            if (tw * S.sx2 >= th * S.sy2 && tw > 1) tw--;
+            else if (th > 1) th--;
+            else tw--;
+        }
+        if (!fits(tw, th)) return fail(h, SPG_E_INVALID, "rotation %d: the crop is too large for the image to warp it", item);
+        *pl = PostPlan{kPostRotated, single, false, S.net_is_f16 != 0, tw, th, kPostCtasPerSm, postR_smem_bytes()};
+        return SPG_OK;
+    }
+    bool ident = true, any16 = false, all16 = true;
+    for (int t = 0; t < n_fused; t++) {
+        ident = ident && sc[t].crop_h == H && sc[t].crop_w == W;
+        any16 = any16 || sc[t].net_is_f16;
+        all16 = all16 && sc[t].net_is_f16;
+    }
+    if (any16 != all16) return fail(h, SPG_E_INVALID, "the network outputs of all scales must have the same dtype");
+    if (single && ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
+        *pl = PostPlan{kPostIdent, true, true, all16, kPostI_TW, kPostI_TH, kPostIdentCtasPerSm, 0};
+        return SPG_OK;
+    }
+    *pl = PostPlan{kPostFourPhase, single, ident, all16, kPostTW, kPostTH, kPostCtasPerSm, postF_smem_bytes(single ? 1 : kPostMaxScales)};
+    for (int t = 0; t < n_fused; t++) {  // as large as every scale's second resize allows
+        pl->tile_w = std::min(pl->tile_w, post_tile_dim(sc[t].sx2, s1, kPostF_C1, kPostF_CS, kPostTW, 13.0));
+        pl->tile_h = std::min(pl->tile_h, post_tile_dim(sc[t].sy2, s1, kPostF_R1, kPostF_RS, kPostTH, 13.0));
     }
     return SPG_OK;
 }
@@ -844,110 +936,46 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     const Workspace &ws = h->ws;
     // validate every scale and fill the common arguments
     PostArgs a{};
-    if ((rc = post_channels(h, d->paf_chan0, d->heat_chan0, d->flip_paf_ord, d->flip_heat_ord, a))) return rc;
+    if ((rc = post_common(h, d->stride, d->n_scales, d->paf_chan0, d->heat_chan0, d->flip_paf_ord, d->flip_heat_ord, d->nan_scrub,
+                          paf_dtype, a)))
+        return rc;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
         if ((rc = grow(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double)))) return rc;
     }
-    a.stride = d->stride; a.H = H; a.W = W;
-    a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p); a.paf_is_f64 = paf_dtype == SPG_F64;
-    a.n_scales = d->n_scales; a.nan_scrub = d->nan_scrub != 0;
-    a.sx1 = 1.0 / (double)d->stride; a.sy1 = a.sx1;  // cv2.resize(fx = stride): scale = 1/fx
+    a.H = H; a.W = W; a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p);
     for (int t = 0; t < d->n_scales; t++) {
         const spg_postnet_scale &sc = d->scales[t];
-        if (!sc.net_out) return fail(h, SPG_E_INVALID, "scale %d: net_out is NULL", t);
-        if (sc.dtype != SPG_F32 && sc.dtype != SPG_F16) return fail(h, SPG_E_INVALID, "scale %d: network output must be SPG_F32 or SPG_F16", t);
-        if (!post_crop_fits(sc.h, sc.w, sc.crop_h, sc.crop_w, d->stride))
-            return fail(h, SPG_E_INVALID, "scale %d: crop %dx%d does not fit the up-sampled %dx%d output", t, sc.crop_h, sc.crop_w, sc.h * d->stride, sc.w * d->stride);
+        if ((rc = check_net_out(h, "scale", t, sc.net_out, sc.dtype, sc.h, sc.w, sc.crop_h, sc.crop_w, d->stride))) return rc;
     }
-    auto scale_of = [&](const spg_postnet_scale &sc) {
-        return post_scale(sc.net_out, sc.dtype, sc.image_stride, sc.pair_stride, sc.chan_stride, sc.h, sc.w, sc.crop_h, sc.crop_w, H, W);
-    };
-    dim3 grid;
-    const bool single = d->n_scales == 1;
-    const bool fast = d->stride == 4;  // the reference's model: four-phase kernel; other strides: table-driven generic kernel
-    if (fast) {
-        // the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales.  With a
-        // rotated item every item is a launch of its own, in item order: rotated ones postnet_rot_kernel, the others
-        // postnet_kernel; the float64 sums continue through memory.
-        const int group = any_rot ? 1 : kPostMaxScales;
-        for (int t0 = 0; t0 < d->n_scales; t0 += group) {
-            a.n_fused = std::min(group, d->n_scales - t0);
-            a.scale_index = t0;
-            if (any_rot && rot[t0].apply) {
-                a.sc[0] = scale_of(d->scales[t0]);
-                const PostScale &S = a.sc[0];
-                invert_affine(rot[t0].matrix, a.rot);
-                // the largest tile (up to 64 x 32) whose crop span and rotated box fit the kernel's buffers: a span of cw x ch
-                // crop pixels reads a box of |m0| cw + |m1| ch (+ 7, the box's margins) columns of the x4 grid, and its x4
-                // groups add up to two more
-                const bool ident = S.crop_h == H && S.crop_w == W;
-                auto fits = [&](int tw, int th) {
-                    const double cw = ident ? tw : tw * S.sx2 + 5.0, ch = ident ? th : th * S.sy2 + 5.0;
-                    const double bw = std::fabs(a.rot[0]) * cw + std::fabs(a.rot[1]) * ch + 7.0;
-                    const double bh = std::fabs(a.rot[3]) * cw + std::fabs(a.rot[4]) * ch + 7.0;
-                    return cw <= kPostF_C1 && ch <= kPostR_R1 && bw / 4.0 + 2.0 <= kPostF_Q && bh / 4.0 + 2.0 <= kPostF_P;
-                };
-                int tw = kPostTW, th = kPostTH;
-                while (!fits(tw, th) && (tw > 1 || th > 1)) {
-                    if (tw * S.sx2 >= th * S.sy2 && tw > 1) tw--;
-                    else if (th > 1) th--;
-                    else tw--;
-                }
-                if (!fits(tw, th)) return fail(h, SPG_E_INVALID, "rotation %d: the crop is too large for the image to warp it", t0);
-                a.tile_w = tw; a.tile_h = th;
-                if ((rc = postnet_grid(h, a, n, 16, &grid))) return rc;
-                void (*rot_kern)(PostArgs) = single ? (S.net_is_f16 ? postnet_rot_kernel<true, true> : postnet_rot_kernel<true, false>)
-                                                    : (S.net_is_f16 ? postnet_rot_kernel<false, true> : postnet_rot_kernel<false, false>);
-                if ((rc = launch(h, kStagePostnet, "postnet_rot_kernel", rot_kern, grid, kPostThreads, postR_smem_bytes(), st, a))) return rc;
-                continue;
-            }
-            a.tile_w = kPostTW; a.tile_h = kPostTH;
-            for (int t = 0; t < a.n_fused; t++) {
-                a.sc[t] = scale_of(d->scales[t0 + t]);
-                post_tile_fit(a.sc[t], a.sx1, a.tile_w, a.tile_h);
-            }
-            bool ident = true, any16 = false, all16 = true;
-            for (int t = 0; t < a.n_fused; t++) {
-                ident = ident && a.sc[t].crop_h == H && a.sc[t].crop_w == W;
-                any16 = any16 || a.sc[t].net_is_f16;
-                all16 = all16 && a.sc[t].net_is_f16;
-            }
-            if (any16 != all16) return fail(h, SPG_E_INVALID, "the network outputs of all scales must have the same dtype");
-            if (single && ident) {  // the reference's default: its own kernel (two passes, per-thread state hoisted)
-                a.tile_w = kPostI_TW; a.tile_h = kPostI_TH;
-                if ((rc = postnet_grid(h, a, n, kPostIdentCtasPerSm, &grid))) return rc;
-                rc = launch(h, kStagePostnet, "postnet_x4_ident_kernel", all16 ? postnet_x4_ident_kernel<true> : postnet_x4_ident_kernel<false>,
-                            grid, kPostThreads, 0, st, a);
-            } else {
-                if ((rc = postnet_grid(h, a, n, kPostCtasPerSm, &grid))) return rc;
-                void (*kern)(PostArgs) = single  ? (all16 ? postnet_kernel<true, false, true> : postnet_kernel<true, false, false>)
-                                         : ident ? (all16 ? postnet_kernel<false, true, true> : postnet_kernel<false, true, false>)
-                                                 : (all16 ? postnet_kernel<false, false, true> : postnet_kernel<false, false, false>);
-                rc = launch(h, kStagePostnet, "postnet_kernel", kern, grid, kPostThreads, postF_smem_bytes(single ? 1 : kPostMaxScales), st, a);
-            }
-            if (rc) return rc;
+    // At stride 4 the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales.
+    // With a rotated item, or at another stride, every item is a launch of its own, in item order; the float64 sums
+    // continue through memory.
+    const int group = d->stride == 4 && !any_rot ? kPostMaxScales : 1;
+    for (int t0 = 0; t0 < d->n_scales; t0 += group) {
+        a.n_fused = std::min(group, d->n_scales - t0);
+        a.scale_index = t0;
+        for (int t = 0; t < a.n_fused; t++) {
+            const spg_postnet_scale &sc = d->scales[t0 + t];
+            a.sc[t] = post_scale(sc.net_out, sc.dtype, sc.image_stride, sc.pair_stride, sc.chan_stride, sc.h, sc.w, sc.crop_h, sc.crop_w, H, W);
         }
-        return SPG_OK;
-    }
-    for (int t = 0; t < d->n_scales; t++) {  // generic kernel: one launch per scale, float64 accumulators in memory
-        const PostScale s = scale_of(d->scales[t]);
-        a.net = s.net; a.net_is_f16 = s.net_is_f16; a.img_stride = s.img_stride; a.pair_stride = s.pair_stride; a.chan_stride = s.chan_stride;
-        a.h = s.h; a.w = s.w; a.crop_h = s.crop_h; a.crop_w = s.crop_w; a.sx2 = s.sx2; a.sy2 = s.sy2;
-        a.scale_index = t;
-        a.tile_w = post_tile_dim(a.sx2, a.sx1, kPostC1, kPostCS, kPostTW, 7.0);
-        a.tile_h = post_tile_dim(a.sy2, a.sy1, kPostR1, kPostRS, kPostTH, 7.0);
-        if ((rc = postnet_grid(h, a, n, 0, &grid)) ||
-            (rc = launch(h, kStagePostnet, "postnet_generic_kernel", postnet_generic_kernel, grid, kPostThreads, 0, st, a)))
-            return rc;
+        const bool rotated = any_rot && rot[t0].apply;
+        if (rotated) invert_affine(rot[t0].matrix, a.rot);
+        PostPlan pl;
+        dim3 grid;
+        if ((rc = plan_post(h, a.sc, a.n_fused, d->n_scales == 1, d->stride, H, W, rotated ? a.rot : nullptr, t0, &pl))) return rc;
+        a.tile_w = pl.tile_w; a.tile_h = pl.tile_h;
+        if ((rc = postnet_grid(h, a, n, pl.ctas_per_sm, &grid))) return rc;
+        const PostKernels &k = kPostKernels[pl.family];
+        if ((rc = launch(h, kStagePostnet, k.name, k.fn[pl.single][pl.ident][pl.f16], grid, kPostThreads, pl.smem, st, a))) return rc;
     }
     return SPG_OK;
 }
 
-// Ragged batches of single-item images: the identity items (crop == image) in postnet_x4_ident_ragged_kernel launches,
-// the others in postnet_ragged_kernel launches -- the kernels and tiles spg_postnet picks for each image alone -- images
-// largest first, one channel chunk per kernel for all its launches.
+// Ragged batches of single-item images: each family's images (plan_post: the kernel and tile spg_postnet picks for each
+// image alone) in its ragged kernel's launches, identity items (crop == image) first, images largest first, one channel
+// chunk per family for all its launches.
 int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *images, int32_t n, int32_t paf_dtype,
                        void *stream) {
     if (!h) return SPG_E_INVALID;
@@ -959,70 +987,53 @@ int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_po
     if (cm->net_dtype != SPG_F32 && cm->net_dtype != SPG_F16) return fail(h, SPG_E_INVALID, "network output must be SPG_F32 or SPG_F16");
     if (paf_dtype != SPG_F32 && paf_dtype != SPG_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32 or SPG_F64");
     PostArgs a{};
-    if ((rc = post_channels(h, cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord, a))) return rc;
-    a.stride = 4; a.n_fused = 1; a.n_scales = 1; a.scale_index = 0;
-    a.paf_is_f64 = paf_dtype == SPG_F64; a.nan_scrub = cm->nan_scrub != 0;
-    a.sx1 = 0.25; a.sy1 = 0.25;
+    if ((rc = post_common(h, 4, 1, cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord, cm->nan_scrub, paf_dtype, a)))
+        return rc;
+    a.n_fused = 1;
     // validate every image before the first launch
     const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
-    std::vector<int> order((size_t)n);
-    std::vector<PostImage> descs((size_t)n);
+    std::vector<PostImage> imgs[2];  // by family: kPostIdent, kPostFourPhase
+    long long tiles[2] = {0, 0};
+    PostPlan plans[2];               // one scale per image: the same chunk target and shared memory for a family's images
     for (int i = 0; i < n; i++) {
         const spg_postnet_image &im = images[i];
-        if (!im.net_out || !im.heat_out || !im.paf_out) return fail(h, SPG_E_INVALID, "image %d: net_out/heat_out/paf_out is NULL", i);
+        if (!im.heat_out || !im.paf_out) return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out is NULL", i);
         // the kernels store rows of 4 values with 16-byte stores (postnet_x4_ident_tile)
         if ((reinterpret_cast<uintptr_t>(im.heat_out) & 15) || (reinterpret_cast<uintptr_t>(im.paf_out) & 15))
             return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out must be 16-byte aligned", i);
         if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
             return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
-        if (!post_crop_fits(im.h, im.w, im.crop_h, im.crop_w, 4))
-            return fail(h, SPG_E_INVALID, "image %d: crop %dx%d does not fit the up-sampled %dx%d output", i, im.crop_h, im.crop_w, 4 * im.h, 4 * im.w);
+        if ((rc = check_net_out(h, "image", i, im.net_out, cm->net_dtype, im.h, im.w, im.crop_h, im.crop_w, 4))) return rc;
         if (im.pair_stride < 0 || im.chan_stride < 0) return fail(h, SPG_E_INVALID, "image %d: negative stride", i);
-        PostImage &d = descs[(size_t)i];
+        PostImage d{};
         d.sc[0] = post_scale(im.net_out, cm->net_dtype, 0, im.pair_stride, im.chan_stride, im.h, im.w, im.crop_h, im.crop_w, im.height, im.width);
         d.H = im.height; d.W = im.width; d.heat = im.heat_out; d.paf = im.paf_out;
-        if (im.crop_h == im.height && im.crop_w == im.width) {
-            d.tile_w = kPostI_TW; d.tile_h = kPostI_TH;
-        } else {
-            d.tile_w = kPostTW; d.tile_h = kPostTH;
-            post_tile_fit(d.sc[0], a.sx1, d.tile_w, d.tile_h);
-        }
-        d.tiles_x = (d.W + d.tile_w - 1) / d.tile_w;
-        d.tiles_y = (d.H + d.tile_h - 1) / d.tile_h;
-        if ((long long)d.tiles_x * d.tiles_y * kPostRaggedMaxImages > 0x7fffffffLL)
+        PostPlan pl;
+        if ((rc = plan_post(h, d.sc, 1, true, 4, d.H, d.W, nullptr, i, &pl))) return rc;
+        d.tile_w = pl.tile_w; d.tile_h = pl.tile_h;
+        const long long t = post_tiles(d.H, d.W, d.tile_w, d.tile_h, d.tiles_x, d.tiles_y);
+        if (t * kPostRaggedMaxImages > 0x7fffffffLL)
             return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
-        order[(size_t)i] = i;
-    }
-    std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
-        return (int64_t)images[x].height * images[x].width > (int64_t)images[y].height * images[y].width;
-    });
-    std::vector<PostImage> ident, other;
-    long long ident_tiles = 0, other_tiles = 0;
-    for (int i : order) {
-        const PostImage &d = descs[(size_t)i];
-        const bool id = images[i].crop_h == d.H && images[i].crop_w == d.W;
-        (id ? ident : other).push_back(d);
-        (id ? ident_tiles : other_tiles) += (long long)d.tiles_x * d.tiles_y;
+        imgs[pl.family].push_back(d);
+        tiles[pl.family] += t;
+        plans[pl.family] = pl;
     }
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool f16 = cm->net_dtype == SPG_F16;
     auto place = [](PostRagged &r, int k, int x) {
         r.img[k].first_cta = x;
         r.n = k + 1;
         return r.img[k].tiles_x * r.img[k].tiles_y;
     };
-    if (!ident.empty()) {
-        a.chan_chunk = post_chan_chunk(h, a.n_out, ident_tiles, kPostIdentCtasPerSm);
-        if ((rc = launch_ragged(h, kStagePostnet, "postnet_x4_ident_ragged_kernel",
-                                f16 ? postnet_x4_ident_ragged_kernel<true> : postnet_x4_ident_ragged_kernel<false>, place,
-                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, 0, st, a, ident)))
-            return rc;
-    }
-    if (!other.empty()) {
-        a.chan_chunk = post_chan_chunk(h, a.n_out, other_tiles, kPostCtasPerSm);
-        if ((rc = launch_ragged(h, kStagePostnet, "postnet_ragged_kernel", f16 ? postnet_ragged_kernel<true> : postnet_ragged_kernel<false>,
-                                place, (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, postF_smem_bytes(1), st, a, other)))
+    for (int f : {kPostIdent, kPostFourPhase}) {
+        if (imgs[f].empty()) continue;
+        std::stable_sort(imgs[f].begin(), imgs[f].end(), [](const PostImage &x, const PostImage &y) {
+            return (int64_t)x.H * x.W > (int64_t)y.H * y.W;
+        });
+        const PostKernels &k = kPostKernels[f];
+        a.chan_chunk = post_chan_chunk(h, a.n_out, tiles[f], plans[f].ctas_per_sm);
+        if ((rc = launch_ragged(h, kStagePostnet, k.ragged_name, k.ragged[cm->net_dtype == SPG_F16], place,
+                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, plans[f].smem, st, a, imgs[f])))
             return rc;
     }
     return SPG_OK;
