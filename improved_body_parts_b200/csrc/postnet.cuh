@@ -479,6 +479,26 @@ struct PostImage {
     int first_cta;
 };
 
+// One image of a multi-item ragged launch (postnet_items_ragged_kernel, postnet_rot_ragged_kernel): the image's items in
+// this launch's group (a.n_fused of them; the rotated kernel takes one), its own float64 keypoint sums and, for a rotated
+// item, its own inverse warp matrix (the rotation centre depends on the image's padded size).
+struct PostItemsImage {
+    PostScale sc[kPostMaxScales];
+    int H, W;
+    float *heat;
+    void *paf;
+    double *heat_acc;           // [K][H][W] float64 scratch of sums that outlive a launch, or nullptr
+    int tile_w, tile_h, tiles_x, tiles_y;
+    int first_cta;
+    double rot[6];
+};
+
+// The float64 keypoint sums that outlive a launch: the launch's scratch (slot n of it) for the per-launch and the
+// single-item ragged kernels, the image's own for the multi-item ragged kernels.
+__device__ __forceinline__ double *post_heat_acc(const PostArgs &a, const PostArgs &) { return a.heat_acc; }
+__device__ __forceinline__ double *post_heat_acc(const PostArgs &a, const PostImage &) { return a.heat_acc; }
+__device__ __forceinline__ double *post_heat_acc(const PostArgs &, const PostItemsImage &im) { return im.heat_acc; }
+
 // Where channel c of image n goes: one base pointer per dtype (32-bit offsets from it per thread; the dtype branches are
 // block-uniform), and whether the values stored are float32.
 struct PostOut {
@@ -494,7 +514,7 @@ __device__ __forceinline__ PostOut post_out(const PostArgs &a, const I &im, int 
     PostOut o;
     o.pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * im.W + ox0;
     o.f = is_heat ? im.heat + o.pbase : static_cast<float *>(im.paf) + o.pbase;
-    o.d = (is_heat ? a.heat_acc : static_cast<double *>(im.paf)) + (is_heat && a.heat_acc == nullptr ? 0 : o.pbase);
+    o.d = (is_heat ? post_heat_acc(a, im) : static_cast<double *>(im.paf)) + (is_heat && post_heat_acc(a, im) == nullptr ? 0 : o.pbase);
     o.store_f = is_heat ? !more_follow : !a.paf_is_f64;
     return o;
 }
@@ -504,7 +524,7 @@ template <bool SINGLE, class I>
 __device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, const I &im,
                                               int c, size_t pbase, int tw, int th, int lane, int warp) {
     if (!SINGLE && a.scale_index > 0) {
-        const double *prev = c < a.K ? a.heat_acc : static_cast<const double *>(im.paf);
+        const double *prev = c < a.K ? post_heat_acc(a, im) : static_cast<const double *>(im.paf);
 #pragma unroll
         for (int ky = 0; ky < kPostKY; ky++)
 #pragma unroll
@@ -718,8 +738,9 @@ __device__ __forceinline__ float warp_linear(int xs, int ys, int w, int h, const
                                __fmul_rn(t10, __fmul_rn(fy, gx))), __fmul_rn(t11, __fmul_rn(fy, fx)));
 }
 
-template <bool SINGLE, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a) {
+// One CTA: tile `tile` of the rotated item of image `im` (slot n of its output planes), channel chunk `chunk`.
+template <bool SINGLE, bool F16, class I>
+__device__ __forceinline__ void postnet_rot_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
     extern __shared__ __align__(16) unsigned char post_smem[];
     PostTabs &T = *reinterpret_cast<PostTabs *>(post_smem);
     float *s0 = reinterpret_cast<float *>(post_smem + sizeof(PostTabs));  // source tile, flip-averaged [RS][kPostF_CS]
@@ -731,15 +752,14 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
     __shared__ int colA[kPostF_C1], colB[kPostF_C1], rowX[kPostR_R1], rowY[kPostR_R1];  // fixed-point coordinate terms
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = blockIdx.x, n = blockIdx.z;
-    const int c_begin = blockIdx.y * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
-    const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
-    const int ox0 = tx * a.tile_w, oy0 = ty * a.tile_h;
-    const int tw = min(a.tile_w, a.W - ox0), th = min(a.tile_h, a.H - oy0);
-    const PostScale &S = a.sc[0];
-    const bool identity = S.crop_h == a.H && S.crop_w == a.W;
+    const int c_begin = chunk * a.chan_chunk, c_end = min(c_begin + a.chan_chunk, a.n_out);
+    const int ty = tile / im.tiles_x, tx = tile - ty * im.tiles_x;
+    const int ox0 = tx * im.tile_w, oy0 = ty * im.tile_h;
+    const int tw = min(im.tile_w, im.W - ox0), th = min(im.tile_h, im.H - oy0);
+    const PostScale &S = im.sc[0];
+    const bool identity = S.crop_h == im.H && S.crop_w == im.W;
     const int Wp = 4 * S.w, Hp = 4 * S.h;
-    const double m0 = a.rot[0], m1 = a.rot[1], m2 = a.rot[2], m3 = a.rot[3], m4 = a.rot[4], m5 = a.rot[5];
+    const double m0 = im.rot[0], m1 = im.rot[1], m2 = im.rot[2], m3 = im.rot[3], m4 = im.rot[4], m5 = im.rot[5];
 
     post_tabs_resize2(T, S, ox0, oy0, tw, th, tid);
     if (tid == 0) {
@@ -783,9 +803,9 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
     float pv0[kPostKI][kPostKJ], pv1[kPostKI][kPostKJ];
     if (c_begin < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c_begin, warp, lane);
     for (int c = c_begin; c < c_end; c++) {
-        const PostOut out = post_out(a, a, n, c, ox0, oy0, more_follow);
+        const PostOut out = post_out(a, im, n, c, ox0, oy0, more_follow);
         double acc[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX];
-        post_load_acc<SINGLE>(acc, a, a, c, out.pbase, tw, th, lane, warp);
+        post_load_acc<SINGLE>(acc, a, im, c, out.pbase, tw, th, lane, warp);
         post_commit(s0, pv0, pv1, R, warp, lane);
         __syncthreads();
         if (c + 1 < c_end) post_prefetch<F16>(pv0, pv1, S, T, a, n, c + 1, warp, lane);
@@ -798,11 +818,16 @@ __global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a
         }
         __syncthreads();
         post_resize2_h<false>(T, sr, s3, identity, tw, th, lane, warp);
-        post_resize2_v<SINGLE, false>(acc, T, sr, s3, identity, a, a, out, ox0, oy0, tw, th, c_lo, y_lo, a.scale_index == 0, nf,
+        post_resize2_v<SINGLE, false>(acc, T, sr, s3, identity, a, im, out, ox0, oy0, tw, th, c_lo, y_lo, a.scale_index == 0, nf,
                                       nf_rcp, nf_small, lane, warp);
         __syncthreads();  // s0 / s3, su and sr are reused by the next channel
-        post_store_acc<SINGLE>(acc, a, out, tw, th, lane, warp);
+        post_store_acc<SINGLE>(acc, im, out, tw, th, lane, warp);
     }
+}
+
+template <bool SINGLE, bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a) {
+    postnet_rot_tile<SINGLE, F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1024,7 +1049,8 @@ struct PostRagged {
 };
 
 // the image whose tiles hold CTA `cta`: the last one whose first CTA is <= cta
-__device__ __forceinline__ const PostImage &post_ragged_image(const PostRagged &r, int cta) {
+template <class R>
+__device__ __forceinline__ const auto &post_ragged_image(const R &r, int cta) {
     int lo = 0, hi = r.n - 1;
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
@@ -1044,6 +1070,34 @@ template <bool F16>
 __global__ void __launch_bounds__(kPostThreads, 2) postnet_ragged_kernel(PostArgs a, const __grid_constant__ PostRagged r) {
     const PostImage &im = post_ragged_image(r, blockIdx.x);
     postnet_tile<true, false, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Ragged batches of multi-item images (predict()'s multi-scale and rotation search for a batch of images): every image
+// has the same items (one product(multiplier, rotate_angle)), so a launch covers one group of items -- up to
+// kPostMaxScales fused unrotated items, or one item when any is rotated -- for many images of different sizes.  The
+// float64 sums of the items in one launch stay in registers (postnet_tile); sums that outlive a launch go through each
+// image's own keypoint scratch (PostItemsImage::heat_acc) and its float64 body-part planes.  Each CTA runs the per-launch
+// kernel's body on its image's geometry: every image gets exactly the maps spg_postnet_rotated gives it alone.
+// Images per launch: as many descriptors as fit next to PostArgs in the 32 764 bytes of kernel parameters.
+constexpr int kPostParamBytes = 32764;
+constexpr int kPostItemsMaxImages = (int)((kPostParamBytes - sizeof(PostArgs) - 8) / sizeof(PostItemsImage));
+struct PostItemsRagged {
+    int n;                                      // images of this launch
+    PostItemsImage img[kPostItemsMaxImages];    // first_cta increasing
+};
+static_assert(sizeof(PostArgs) + sizeof(PostItemsRagged) <= kPostParamBytes, "a launch's parameters fit the kernel-parameter limit");
+
+template <bool IDENT, bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_items_ragged_kernel(PostArgs a, const __grid_constant__ PostItemsRagged r) {
+    const PostItemsImage &im = post_ragged_image(r, blockIdx.x);
+    postnet_tile<false, IDENT, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
+}
+
+template <bool SINGLE, bool F16>
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_ragged_kernel(PostArgs a, const __grid_constant__ PostItemsRagged r) {
+    const PostItemsImage &im = post_ragged_image(r, blockIdx.x);
+    postnet_rot_tile<SINGLE, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 
 }  // namespace spg

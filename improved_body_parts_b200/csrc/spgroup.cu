@@ -831,26 +831,34 @@ static int post_common(spg_handle *h, int stride, int n_scales, int paf_chan0, i
 }
 
 // The kernel families of the post-network stage (PostPlan::family), each with its kernels by template flags
-// [single][ident][f16] (nullptr: not instantiated) and its single-scale ragged kernels by [f16], under the names
-// spg_stage_kernel reports.
+// [single][ident][f16] (nullptr: not instantiated), its single-scale ragged kernels by [f16] and its multi-item ragged
+// kernels by the same flags as its per-launch kernels, under the names spg_stage_kernel reports.
 enum : int { kPostIdent, kPostFourPhase, kPostRotated, kPostGeneric };
 struct PostKernels {
     const char *name;
     void (*fn[2][2][2])(PostArgs);
     const char *ragged_name;
     void (*ragged[2])(PostArgs, PostRagged);
+    const char *items_name;
+    void (*items[2][2][2])(PostArgs, PostItemsRagged);
 };
 static const PostKernels kPostKernels[4] = {
     {"postnet_x4_ident_kernel", {{}, {{}, {postnet_x4_ident_kernel<false>, postnet_x4_ident_kernel<true>}}},
-     "postnet_x4_ident_ragged_kernel", {postnet_x4_ident_ragged_kernel<false>, postnet_x4_ident_ragged_kernel<true>}},
+     "postnet_x4_ident_ragged_kernel", {postnet_x4_ident_ragged_kernel<false>, postnet_x4_ident_ragged_kernel<true>}, "", {}},
     {"postnet_kernel",
      {{{postnet_kernel<false, false, false>, postnet_kernel<false, false, true>}, {postnet_kernel<false, true, false>, postnet_kernel<false, true, true>}},
       {{postnet_kernel<true, false, false>, postnet_kernel<true, false, true>}, {}}},
-     "postnet_ragged_kernel", {postnet_ragged_kernel<false>, postnet_ragged_kernel<true>}},
+     "postnet_ragged_kernel", {postnet_ragged_kernel<false>, postnet_ragged_kernel<true>},
+     "postnet_items_ragged_kernel",
+     {{{postnet_items_ragged_kernel<false, false>, postnet_items_ragged_kernel<false, true>},
+       {postnet_items_ragged_kernel<true, false>, postnet_items_ragged_kernel<true, true>}}}},
     {"postnet_rot_kernel",
      {{{postnet_rot_kernel<false, false>, postnet_rot_kernel<false, true>}, {}}, {{postnet_rot_kernel<true, false>, postnet_rot_kernel<true, true>}, {}}},
-     "", {}},
-    {"postnet_generic_kernel", {{{postnet_generic_kernel}}}, "", {}},
+     "", {},
+     "postnet_rot_ragged_kernel",
+     {{{postnet_rot_ragged_kernel<false, false>, postnet_rot_ragged_kernel<false, true>}, {}},
+      {{postnet_rot_ragged_kernel<true, false>, postnet_rot_ragged_kernel<true, true>}, {}}}},
+    {"postnet_generic_kernel", {{{postnet_generic_kernel}}}, "", {}, "", {}},
 };
 
 struct PostPlan {
@@ -1034,6 +1042,132 @@ int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_po
         a.chan_chunk = post_chan_chunk(h, a.n_out, tiles[f], plans[f].ctas_per_sm);
         if ((rc = launch_ragged(h, kStagePostnet, k.ragged_name, k.ragged[cm->net_dtype == SPG_F16], place,
                                 (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, plans[f].smem, st, a, imgs[f])))
+            return rc;
+    }
+    return SPG_OK;
+}
+
+// Ragged batches of multi-item images: spg_postnet_rotated's schedule for every image at once.  The items go in groups
+// -- kPostMaxScales fused unrotated items, or one item per group when any is rotated -- and within a group each image goes
+// in the family and tile plan_post picks for it alone, largest first, as many per launch as PostItemsRagged holds.  One
+// unrotated item per image is spg_postnet_ragged.
+int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *items,
+                             const spg_postnet_rotation *rot, int32_t n, int32_t n_items, int32_t paf_dtype, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    if ((rc = check_batch(h, n))) return rc;
+    if (n > 0 && (!items || n_items < 1)) return fail(h, SPG_E_INVALID, "items is NULL or n_items %d below 1", n_items);
+    if (!cm || !cm->flip_paf_ord || !cm->flip_heat_ord) return fail(h, SPG_E_INVALID, "postnet common descriptor incomplete");
+    if (cm->stride != 4) return fail(h, SPG_E_INVALID, "the ragged post-network stage needs stride 4 (got %d)", cm->stride);
+    if (cm->net_dtype != SPG_F32 && cm->net_dtype != SPG_F16) return fail(h, SPG_E_INVALID, "network output must be SPG_F32 or SPG_F16");
+    if (paf_dtype != SPG_F32 && paf_dtype != SPG_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32 or SPG_F64");
+    if (paf_dtype == SPG_F32 && n_items > 1)
+        return fail(h, SPG_E_INVALID, "float32 body-part planes hold the reference's float64 values only for a single item");
+    PostArgs a{};
+    if ((rc = post_common(h, 4, std::max(n_items, 1), cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord,
+                          cm->nan_scrub, paf_dtype, a)))
+        return rc;
+    // validate every image and item before the first launch
+    bool any_rot = false;
+    for (int i = 0; rot && i < n; i++) {
+        for (int t = 0; t < n_items; t++) {
+            const spg_postnet_rotation &r = rot[(size_t)i * n_items + t];
+            if ((r.apply != 0 && r.apply != 1) || r.reserved != 0)
+                return fail(h, SPG_E_INVALID, "image %d item %d: rotation apply must be 0 or 1 and reserved 0", i, t);
+            for (int k = 0; k < 6; k++)
+                if (!std::isfinite(r.matrix[k])) return fail(h, SPG_E_INVALID, "image %d item %d: matrix entry %d is not finite", i, t, k);
+            if (r.apply != rot[t].apply)
+                return fail(h, SPG_E_INVALID, "image %d item %d: rotated in some images and not in others (one rotation_search per call)", i, t);
+            any_rot = any_rot || r.apply;
+        }
+    }
+    const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
+    std::vector<size_t> acc_off((size_t)n);  // each image's float64 keypoint sums in the handle's scratch
+    size_t acc_total = 0;
+    for (int i = 0; i < n; i++) {
+        const spg_postnet_image &im = items[(size_t)i * n_items];
+        for (int t = 0; t < n_items; t++) {
+            const spg_postnet_image &it = items[(size_t)i * n_items + t];
+            if (!it.heat_out || !it.paf_out) return fail(h, SPG_E_INVALID, "image %d item %d: heat_out/paf_out is NULL", i, t);
+            if (it.height != im.height || it.width != im.width || it.heat_out != im.heat_out || it.paf_out != im.paf_out)
+                return fail(h, SPG_E_INVALID, "image %d item %d: height/width/heat_out/paf_out differ from the image's item 0", i, t);
+            char what[32];
+            snprintf(what, sizeof what, "image %d item", i);
+            if ((rc = check_net_out(h, what, t, it.net_out, cm->net_dtype, it.h, it.w, it.crop_h, it.crop_w, 4))) return rc;
+            if (it.pair_stride < 0 || it.chan_stride < 0) return fail(h, SPG_E_INVALID, "image %d item %d: negative stride", i, t);
+        }
+        // the kernels store rows of 4 values with 16-byte stores (postnet_x4_ident_tile)
+        if ((reinterpret_cast<uintptr_t>(im.heat_out) & 15) || (reinterpret_cast<uintptr_t>(im.paf_out) & 15))
+            return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out must be 16-byte aligned", i);
+        if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
+            return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
+        acc_off[i] = acc_total;
+        acc_total += (size_t)h->ws.K * im.height * im.width;
+    }
+    if (n == 0) return SPG_OK;
+    if (n_items == 1 && !any_rot) return spg_postnet_ragged(h, cm, items, n, paf_dtype, stream);
+    // the schedule of every launch, planned (and checked) before the first one: per item group, one launch list per kernel
+    struct Group {
+        int t0, n_fused;
+        PostPlan plan;
+        long long tiles;
+        std::vector<PostItemsImage> imgs;
+    };
+    std::vector<Group> groups;
+    const int per_group = any_rot ? 1 : kPostMaxScales;
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double *acc = nullptr;
+    if (n_items > 1 && (n_items > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
+        if ((rc = grow(h, h->heat_acc, acc_total * sizeof(double)))) return rc;
+        acc = static_cast<double *>(h->heat_acc.p);
+    }
+    for (int t0 = 0; t0 < n_items; t0 += per_group) {
+        const int nf = std::min(per_group, n_items - t0);
+        const bool rotated = any_rot && rot[t0].apply;
+        const size_t first = groups.size();
+        for (int i = 0; i < n; i++) {
+            const spg_postnet_image &im = items[(size_t)i * n_items];
+            PostItemsImage d{};
+            for (int t = 0; t < nf; t++) {
+                const spg_postnet_image &it = items[(size_t)i * n_items + t0 + t];
+                d.sc[t] = post_scale(it.net_out, cm->net_dtype, 0, it.pair_stride, it.chan_stride, it.h, it.w, it.crop_h, it.crop_w,
+                                     im.height, im.width);
+            }
+            d.H = im.height; d.W = im.width; d.heat = im.heat_out; d.paf = im.paf_out;
+            d.heat_acc = acc ? acc + acc_off[i] : nullptr;
+            if (rotated) invert_affine(rot[(size_t)i * n_items + t0].matrix, d.rot);
+            PostPlan pl;
+            if ((rc = plan_post(h, d.sc, nf, n_items == 1, 4, d.H, d.W, rotated ? d.rot : nullptr, t0, &pl)))
+                return fail(h, rc, "image %d item %d: %s", i, t0, std::string(h->err).c_str());
+            d.tile_w = pl.tile_w; d.tile_h = pl.tile_h;
+            const long long tl = post_tiles(d.H, d.W, d.tile_w, d.tile_h, d.tiles_x, d.tiles_y);
+            if (tl * kPostItemsMaxImages > 0x7fffffffLL)
+                return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
+            size_t g = first;
+            while (g < groups.size() && !(groups[g].plan.family == pl.family && groups[g].plan.single == pl.single &&
+                                          groups[g].plan.ident == pl.ident))
+                g++;
+            if (g == groups.size()) groups.push_back(Group{t0, nf, pl, 0, {}});
+            groups[g].imgs.push_back(d);
+            groups[g].tiles += tl;
+        }
+    }
+    auto place = [](PostItemsRagged &r, int k, int x) {
+        r.img[k].first_cta = x;
+        r.n = k + 1;
+        return r.img[k].tiles_x * r.img[k].tiles_y;
+    };
+    for (Group &g : groups) {
+        std::stable_sort(g.imgs.begin(), g.imgs.end(), [](const PostItemsImage &x, const PostItemsImage &y) {
+            return (int64_t)x.H * x.W > (int64_t)y.H * y.W;
+        });
+        const PostKernels &k = kPostKernels[g.plan.family];
+        a.n_fused = g.n_fused;
+        a.scale_index = g.t0;
+        a.chan_chunk = post_chan_chunk(h, a.n_out, g.tiles, g.plan.ctas_per_sm);
+        if ((rc = launch_ragged(h, kStagePostnet, k.items_name, k.items[g.plan.single][g.plan.ident][g.plan.f16], place,
+                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, g.plan.smem, st, a, g.imgs)))
             return rc;
     }
     return SPG_OK;

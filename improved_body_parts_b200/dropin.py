@@ -296,6 +296,28 @@ def plan_buckets(image_shapes, params, model_params):
     return plan, buckets
 
 
+def plan_items(image_shapes, params, model_params):
+    """The batches of ``predict_batch`` for any ``scale_search x rotation_search``: per image, per item of
+    ``product(multiplier, rotation_search)`` (evaluate.py:87-90) ``(multiplier, scale, angle, H1, W1, Hp, Wp)`` -- the
+    scale after the clamp of :94-96, the crop size and the padded network input size of :98-100 -- and the items grouped
+    by network input size ``{(Hp, Wp): [(image index, item index), ...]}`` in order of first appearance.  The rotated and
+    unrotated items of one scale share a bucket: the rotation happens inside the padded input."""
+    import itertools
+    plan, buckets = [], {}
+    md = int(model_params["max_downsample"])
+    for i, shape in enumerate(image_shapes):
+        h, w = int(shape[0]), int(shape[1])
+        items = []
+        multiplier = [x * model_params["boxsize"] / h for x in params["scale_search"]]
+        for t, (m, angle) in enumerate(itertools.product(multiplier, params["rotation_search"])):
+            scale = clamp_scale(m, (h, w))
+            geo = input_geometry(h, w, scale, md)
+            items.append((m, scale, angle) + geo)
+            buckets.setdefault(geo[2:], []).append((i, t))
+        plan.append(items)
+    return plan, buckets
+
+
 def predict_batch(images, params, model, model_params, *, forward_batch: int, input_stage: Optional[str] = None):
     """``predict`` for several images at once: one ``(heatmap, paf)`` pair of ``DeviceMaps`` per image, in input order.
 
@@ -303,16 +325,28 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     padded size ``(Hp, Wp)`` share forward passes of at most ``forward_batch`` images (``2 * forward_batch`` samples:
     each image and its mirror), and one ``spg_postnet_ragged`` call runs the post-network stage of the whole batch,
     reading each image's pair out of its forward pass in place.  The inputs are built per image as ``predict`` builds
-    them (``input_stage`` as there) into one tensor per size.  Every kernel treats each image on its own, so the maps
-    equal ``predict``'s bit for bit when the network's output for a sample does not depend on the batch it runs in (a
-    network under cuDNN may pick another algorithm for another batch size).  Other configurations (several scales, a
-    rotation search, another stride) run ``predict`` per image."""
+    them (``input_stage`` as there) into one tensor per size.
+
+    Any other ``scale_search x rotation_search`` at stride 4 (the reference's multi-scale and rotation search) is batched
+    the same way per item: the items of every image are grouped by padded input size (``plan_items``; an item's rotation
+    does not change its size), each size's forward passes take at most ``forward_batch`` items, and one
+    ``spg_postnet_ragged_items`` call averages every image's items.  The inputs are built per size with cv2
+    (``input_stage="host"``) or by one ``spg_prenet`` call per image that writes each item into its slot
+    (``"device"``).  A size's input tensor is released after its forward passes, but every network output lives until
+    the post-network call: at ``scale_search = [0.5, 1, 1.5, 2]``, boxsize 640, float32 that is about 100 MB per
+    480 x 640 image, and the device input stage holds about as much again of inputs until the forward passes.
+
+    Every kernel treats each image on its own, so the maps equal ``predict``'s bit for bit when the network's output for
+    a sample does not depend on the batch it runs in (a network under cuDNN may pick another algorithm for another batch
+    size).  Another stride runs ``predict`` per image."""
     import torch
     stage = _stage(_input_stage if input_stage is None else input_stage)
     fb = _forward_batch(forward_batch)
     images = list(images)
     if not _single_item(params, model_params):
-        return [predict(img, params, model, model_params, input_stage=stage) for img in images]
+        if int(model_params["stride"]) != 4:
+            return [predict(img, params, model, model_params, input_stage=stage) for img in images]
+        return _predict_batch_items(images, params, model, model_params, fb, stage)
     md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
     plan, buckets = plan_buckets([img.shape[:2] for img in images], params, model_params)
     g = _grouper_many(len(images))
@@ -343,6 +377,59 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
                 entries[i] = (out[2 * (j - c0):2 * (j - c0) + 2], crops[j], tuple(int(v) for v in images[i].shape[:2]))
     maps = g.postnet_ragged(entries, nan_scrub=_variant == "demo")
     return [(DeviceMaps(heat, False), DeviceMaps(paf, True)) for heat, paf in maps]
+
+
+def _predict_batch_items(images, params, model, model_params, fb: int, stage: str):
+    """``predict_batch`` for several items per image (or one rotated item) at stride 4; see there."""
+    import torch
+    if not images:
+        return []
+    plan, buckets = plan_items([img.shape[:2] for img in images], params, model_params)
+    n_items = len(plan[0])
+    g = _grouper_many(len(images))
+    dev = f"cuda:{_device}"
+    crops = [[None] * n_items for _ in images]
+    reverses = [[None] * n_items for _ in images]
+    inputs = {}  # (Hp, Wp) -> [2 * items, Hp, Wp, 3] network input
+    if stage == "device":
+        md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
+        inputs = {(Hp, Wp): torch.empty((2 * len(members), Hp, Wp, 3), dtype=torch.float32, device=dev)
+                  for (Hp, Wp), members in buckets.items()}
+        slots = [[None] * n_items for _ in images]
+        for key, members in buckets.items():
+            for j, (i, t) in enumerate(members):
+                slots[i][t] = inputs[key][2 * j:2 * j + 2]
+        for i, image in enumerate(images):
+            img = image if isinstance(image, torch.Tensor) else _upload_image(image)
+            multiplier = [x * model_params["boxsize"] / image.shape[0] for x in params["scale_search"]]
+            for t, (_, crop, reverse) in enumerate(g.prenet(img.to(dev), multiplier, params["rotation_search"],
+                                                             max_downsample=md, pad_value=pv, out=slots[i])):
+                crops[i][t], reverses[i][t] = crop, reverse
+    entries = [[None] * n_items for _ in images]
+    for key, members in buckets.items():
+        k = len(members)
+        if stage == "host":
+            x = torch.empty((2 * k,) + key + (3,), dtype=torch.float32, device=dev)
+            host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
+            for j, (i, t) in enumerate(members):
+                _, scale, angle = plan[i][t][:3]
+                _, crops[i][t], reverses[i][t] = _host_pair(images[i], scale, angle, model_params,
+                                                            out=host[2 * j:2 * j + 2].numpy())
+            x.copy_(host, non_blocking=True)
+            _copied("pairs")
+        else:
+            x = inputs.pop(key)
+        for c0 in range(0, k, fb):
+            c1 = min(k, c0 + fb)
+            with torch.no_grad():
+                out = _network_output(model, x[2 * c0:2 * c1]).contiguous()
+            for j in range(c0, c1):
+                i, t = members[j]
+                entries[i][t] = (out[2 * (j - c0):2 * (j - c0) + 2], crops[i][t], reverses[i][t])
+        del x
+    maps = g.postnet_ragged_items([(entries[i], tuple(int(v) for v in img.shape[:2])) for i, img in enumerate(images)],
+                                  nan_scrub=_variant == "demo")
+    return [(DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)) for heat, paf in maps]
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:
@@ -516,9 +603,9 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
     ``validation_ids`` order, with ``np.float64`` coordinates and scores and integer ``(0, 0)`` for a missing joint, so
     ``format_results`` writes the same file.  Per image: ``cv2.imread`` and ``predict`` (the maps stay on the device);
     every ``batch`` images and at the end: one ``group_many``-style ragged call, the batch's wire records in one copy.
-    ``forward_batch > 1`` runs ``predict_batch`` on each group of ``batch`` images instead of ``predict`` per image (see
-    there for when its maps equal ``predict``'s).  A non-zero status raises ``GroupingError``.  ``image_name(coco,
-    image_id)`` gives the file name (default: ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()``
+    ``forward_batch > 1`` runs ``predict_batch`` on each group of ``batch`` images instead of ``predict`` per image, for
+    any ``scale_search`` and ``rotation_search`` at stride 4 (see there for when its maps equal ``predict``'s).  A
+    non-zero status raises ``GroupingError``.  ``image_name(coco, image_id)`` gives the file name (default: ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()``
     is not called, so the reference's ``batch_time`` meter is not updated."""
     import os
 
@@ -608,8 +695,8 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     ``batch > 1`` (with ``device_predict``) also replaces ``predict_many`` (:550-560) by ``predict_many`` above, which
     groups ``batch`` images per call; it uses the module's ``posenet`` and ``get_image_name`` and leaves the module's
     ``batch_time`` meter alone.  ``forward_batch > 1`` (with ``device_predict`` and ``batch > 1``) makes that
-    ``predict_many`` run the network on up to ``forward_batch`` images of the same input size at once
-    (``predict_batch``)."""
+    ``predict_many`` run the network on up to ``forward_batch`` items (images, or with a multi-scale or rotation search
+    their scaled and rotated copies) of the same input size at once (``predict_batch``)."""
     if int(batch) > 1 and not device_predict:
         raise ValueError("batch > 1 needs device_predict=True: the batched grouping takes the maps predict() leaves on the device")
     fb = _forward_batch(forward_batch)

@@ -216,6 +216,16 @@ typedef struct spg_postnet_image {
  * `images` may be reused as soon as the call returns. */
 int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *common, const spg_postnet_image *images,
                        int32_t n_images, int32_t paf_dtype, void *stream);
+/* Ragged batches with several items per image: the multi-scale and rotation search (scale_search, rotation_search) for
+ * images of different sizes in one call.  items [n_images][n_items] in product(multiplier, rotate_angle) order: the
+ * items of one image share height, width, heat_out and paf_out.  rot [n_images][n_items] as spg_postnet_rotated's, or
+ * NULL (no item rotated); item t is rotated in every image or in none.  Image i's maps equal those spg_postnet_rotated
+ * gives for it alone.  paf_dtype SPG_F64, or SPG_F32 for n_items == 1.  Validation, asynchrony and reuse of `items` /
+ * `rot` as spg_postnet_ragged; the handle's float64 keypoint scratch grows on demand to the batch's sum of
+ * n_parts * height * width when the sums outlive a launch (more than 4 items, or a rotated one). */
+int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *common, const spg_postnet_image *items,
+                             const spg_postnet_rotation *rot, int32_t n_images, int32_t n_items, int32_t paf_dtype,
+                             void *stream);
 
 /* ---- pre-network stage: the item loop of predict() before the forward pass, evaluate.py:94-121 ------------ */
 /* One (scale, angle) item of product(multiplier, rotate_angle) (evaluate.py:90). */

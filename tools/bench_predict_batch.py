@@ -5,7 +5,9 @@ of forward_batch images, one ragged post-network call per group).
 
 Workload: --images seeded random uint8 images, shapes drawn from a fixed table of COCO val2017 sizes, at the reference's
 settings (utils/config: boxsize 640, max_downsample 64, scale_search [1], rotation_search [0], stride 4), so every image
-is resized to 640 rows and the images fall into a few network input sizes.  The network is imhn.IMHN with the
+is resized to 640 rows and the images fall into a few network input sizes.  --scale-search and --rotation-search (comma
+lists) select the reference's accuracy mode instead, e.g. 0.5,1,1.5,2 or 0,30,-30: every image then has one item per
+(scale, angle), and the batched mode groups the items by input size (``dropin.plan_items``).  The network is imhn.IMHN with the
 reference's random initialisation, bf16 autocast, channels-last, no CUDA graph.  The input stage is --input-stage
 (default device: spg_prenet per image).  Every group of --group images is grouped with one ragged call
 (``predict_many``'s batching).
@@ -20,6 +22,7 @@ images).  Also the largest absolute difference between the per-image and the bat
 one input size): the network's numerics across batch sizes.  The card's name and power limit are read in the same run.
 
 usage: python tools/bench_predict_batch.py [--images 48] [--group 16] [--rounds 3] [--forward-batches 2,4,8,16]
+                                           [--scale-search 1] [--rotation-search 0]
                                            [--out profiles/predict_batch.json]"""
 import argparse
 import json
@@ -35,7 +38,6 @@ sys.path.insert(0, ROOT)
 
 SHAPES = [(480, 640), (640, 480), (427, 640), (640, 427), (612, 612), (375, 500), (640, 640), (500, 375), (360, 640),
           (426, 640)]
-PARAMS_REF = dict(scale_search=[1.0], rotation_search=[0.0])
 MODEL_PARAMS_REF = dict(boxsize=640, stride=4, max_downsample=64, padValue=128)
 
 
@@ -66,6 +68,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--forward-batches", default="2,4,8,16")
     ap.add_argument("--input-stage", default="device", choices=("host", "device"))
+    ap.add_argument("--scale-search", default="1", help="comma list (utils/config scale_search)")
+    ap.add_argument("--rotation-search", default="0", help="comma list of angles (utils/config rotation_search)")
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "predict_batch.json"))
     a = ap.parse_args()
     import torch
@@ -78,14 +82,16 @@ def main():
     rng = np.random.default_rng(2029)
     images = [rng.integers(0, 256, size=SHAPES[int(rng.integers(len(SHAPES)))] + (3,), dtype=np.uint8)
               for _ in range(a.images)]
-    params = dict(skeleton.default_params(), **PARAMS_REF)
+    params = dict(skeleton.default_params(), scale_search=[float(v) for v in a.scale_search.split(",")],
+                  rotation_search=[float(v) for v in a.rotation_search.split(",")])
     runner = imhn.Runner(imhn.IMHN().init_like_reference_(0), device="cuda:0", use_graph=False)
 
     def model(x):
         return [[runner(x)]]
 
-    _, buckets = dropin.plan_buckets([im.shape[:2] for im in images], params, MODEL_PARAMS_REF)
-    print(f"workload: {a.images} images, input sizes {{(Hp, Wp): images}} = "
+    _, buckets = dropin.plan_items([im.shape[:2] for im in images], params, MODEL_PARAMS_REF)
+    print(f"workload: {a.images} images, scale_search {params['scale_search']}, rotation_search "
+          f"{params['rotation_search']}, input sizes {{(Hp, Wp): items}} = "
           f"{ {k: len(v) for k, v in buckets.items()} }", flush=True)
     groups = [list(range(i, min(i + a.group, a.images))) for i in range(0, a.images, a.group)]
     fbs = [int(k) for k in a.forward_batches.split(",")]
@@ -135,7 +141,8 @@ def main():
         net_diff = float((whole - pairs).abs().max())
     name, pl = card()
     res = {"card": name, "power_limit": pl, "images": a.images, "group": a.group, "rounds": a.rounds,
-           "input_stage": a.input_stage, "input_sizes": {f"{k[0]}x{k[1]}": len(v) for k, v in buckets.items()},
+           "input_stage": a.input_stage, "scale_search": params["scale_search"],
+           "rotation_search": params["rotation_search"], "input_sizes": {f"{k[0]}x{k[1]}": len(v) for k, v in buckets.items()},
            "max_abs_diff_maps": map_diff, "max_abs_diff_network": net_diff, "network_diff_batch": list(x.shape),
            "modes": {}}
     print(f"{name}, power limit {pl}; {a.images} images in groups of {a.group}, input stage {a.input_stage}")

@@ -15,7 +15,8 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
    at the call sites ``:509-511``) and takes ``limbSeq`` from the module (``:54``); with ``--batch N`` (N > 1) it also
    replaces ``predict`` by the device one and ``predict_many`` (``:550-560``) by ``dropin.predict_many``, which groups
    N images per call; ``--forward-batch M`` (M > 1, with N > 1) also runs the network on up to M images of the same
-   input size at once (``dropin.predict_batch``);
+   input size at once (``dropin.predict_batch``; with several scales or a rotation search in ``utils/config``, up to M
+   items: the images' scaled and rotated copies);
 4. fills the globals ``evaluate.__main__`` would set (``:643-646``): ``params, model_params`` from the reference's own
    ``utils/config`` through ``skeleton.read_reference_ini`` (``utils/config_reader.py:7`` hard-codes the author's path),
    ``show_eval_speed``;
