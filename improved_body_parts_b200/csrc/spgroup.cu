@@ -20,6 +20,7 @@
 
 #include "assemble.cuh"
 #include "common.cuh"
+#include "group_unbounded.cuh"
 #include "limb_match.cuh"
 #include "limb_score.cuh"
 #include "limb_score_persist.cuh"
@@ -59,6 +60,11 @@ struct spg_handle {
     unsigned long long armed_value = 0;
     Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
     Scratch pre_grid;  // prenet: the padded uint8 images of a rotated item
+    // the capacity-free tier (spg_group_unbounded): fixed-size words, tables sized by the peak counts, the candidate list
+    // with the sort's scratch, the person table and outputs; `ub_ws` describes the last call's results
+    Scratch ub_small, ub_peaks, ub_cands, ub_people;
+    Workspace ub_ws{};
+    bool ub_valid = false;
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
     const char *stage_kernel[kStageCount] = {"", "", "", "", "", ""};
@@ -580,7 +586,7 @@ void spg_destroy(spg_handle *h) {
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
     for (void *p : h->allocs) cudaFree(p);
-    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid})
+    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid, &h->ub_small, &h->ub_peaks, &h->ub_cands, &h->ub_people})
         if (s->p) cudaFree(s->p);
     if (h->done_counter) cudaFree(h->done_counter);
     for (auto &s : h->streams)
@@ -1554,6 +1560,244 @@ int spg_download_status(spg_handle *h, int32_t n, uint32_t *status, void *stream
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SPG_D2H(status, h->ws.status, (size_t)n);
     SPG_CUDA(h, cudaStreamSynchronize(st));
+    return SPG_OK;
+}
+
+}  // extern "C"
+
+// ---- the capacity-free tier (group_unbounded.cuh) ------------------------------------------------------------------
+namespace {
+
+// Lays arrays out in one Scratch, each 256-byte aligned: a pass with base == nullptr measures, a pass with the grown
+// buffer hands out the pointers.
+struct Carver {
+    unsigned char *base = nullptr;
+    size_t bytes = 0;
+    template <typename T>
+    T *take(size_t count) {
+        const size_t o = (bytes + 255) & ~(size_t)255;
+        bytes = o + std::max<size_t>(count, 1) * sizeof(T);
+        return base ? reinterpret_cast<T *>(base + o) : nullptr;
+    }
+};
+
+template <typename F>
+int carve(spg_handle *h, Scratch &s, F &&layout) {
+    Carver m;
+    layout(m);
+    int rc;
+    if ((rc = grow(h, s, m.bytes))) return rc;
+    Carver c;
+    c.base = static_cast<unsigned char *>(s.p);
+    layout(c);
+    return SPG_OK;
+}
+
+// [dtype][write]: the scoring kernel for the plane's storage / arithmetic types (kScoreKernels' dtype order)
+void (*const kUbScoreKernels[3][2])(UbArgs, ScoreArgs) = {
+    {ub_score_kernel<float, float, false>, ub_score_kernel<float, float, true>},
+    {ub_score_kernel<double, double, false>, ub_score_kernel<double, double, true>},
+    {ub_score_kernel<float, double, false>, ub_score_kernel<float, double, true>},
+};
+
+}  // namespace
+
+extern "C" {
+
+int spg_group_unbounded(spg_handle *h, const spg_image_maps *im, int32_t dtype, const spg_params *p, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    h->ub_valid = false;
+    int rc;
+    if (!im || !im->heat || !im->paf) return fail(h, SPG_E_INVALID, "image maps or their heat/paf are NULL");
+    if ((rc = check_dtype(h, dtype)) || (rc = check_params(h, p))) return rc;
+    const int H = im->height, W = im->width;
+    if (H < 2 || W < 2 || H > 32767 || W > 32767) return fail(h, SPG_E_INVALID, "map %dx%d outside [2, 32767x32767]", H, W);
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int K = h->ws.K, L = h->ws.L, J = h->ws.J;
+    Workspace ws = h->ws;  // skeleton of the handle, arrays of the tier
+    ws.max_batch = 1;
+    ws.capC = 0;
+    ws.surv_count = nullptr;
+    ws.wire = nullptr;
+    ws.wire_first = 0;
+    ws.wire_rows = 0;
+    int64_t *seg_off = nullptr;
+    if ((rc = carve(h, h->ub_small, [&](Carver &c) {
+             ws.peak_count = c.take<int32_t>(K);
+             ws.status = c.take<uint32_t>(1);
+             ws.n_persons = c.take<int32_t>(1);
+             ws.conn_count = c.take<int32_t>(L);
+             ws.cand_count = c.take<int32_t>(L);
+             seg_off = c.take<int64_t>(L + 1);
+         })))
+        return rc;
+    UbArgs u{};
+    u.heat = im->heat;
+    u.paf = im->paf;
+    u.heat_chan_stride = im->heat_chan_stride;
+    u.paf_chan_stride = im->paf_chan_stride;
+    u.H = H;
+    u.W = W;
+    u.seg_off = seg_off;
+    NmsArgs na = nms_args(h, p);
+    na.H = H;
+    na.W = W;
+
+    // 1. peak counts, then the peak tables sized by the largest part
+    SPG_CUDA(h, cudaMemsetAsync(ws.status, 0, sizeof(uint32_t), st));
+    u.ws = ws;
+    if ((rc = launch(h, kStageNms, "ub_peaks_kernel<count>", ub_peaks_kernel<false>, K, kUbPeakThreads, 0, st, u, na))) return rc;
+    std::vector<int32_t> counts((size_t)K);
+    SPG_CUDA(h, cudaMemcpyAsync(counts.data(), ws.peak_count, sizeof(int32_t) * K, cudaMemcpyDeviceToHost, st));
+    SPG_CUDA(h, cudaStreamSynchronize(st));
+    const int P = std::max(1, *std::max_element(counts.begin(), counts.end()));
+    if (P > kUbMaxPeaks) return fail(h, SPG_E_INVALID, "a part has %d peaks; the unbounded tier holds at most %d per part", P, kUbMaxPeaks);
+    ws.capP = P;
+    if ((rc = carve(h, h->ub_peaks, [&](Carver &c) {
+             ws.peak_x = c.take<double>((size_t)K * P);
+             ws.peak_y = c.take<double>((size_t)K * P);
+             ws.peak_score = c.take<float>((size_t)K * P);
+             ws.peak_anchor = c.take<uint32_t>((size_t)K * P);
+             ws.conn_ij = c.take<uint32_t>((size_t)L * P);
+             ws.conn_score = c.take<double>((size_t)L * P);
+             ws.conn_norm = c.take<double>((size_t)L * P);
+             u.row_count = c.take<int32_t>((size_t)L * P);
+             u.row_off = c.take<int64_t>((size_t)L * P);
+             u.used = c.take<unsigned char>((size_t)L * 2 * P);
+         })))
+        return rc;
+    u.ws = ws;
+    na.ws = ws;
+    if ((rc = launch(h, kStageNms, "ub_peaks_kernel<write>", ub_peaks_kernel<true>, K, kUbPeakThreads, 0, st, u, na))) return rc;
+
+    // 2. candidates per pair row, their offsets in generation order, then the candidates themselves
+    ScoreArgs sa = score_args(h, p);
+    sa.H = H;
+    sa.W = W;
+    sa.image_extent = im->image_extent;
+    sa.ws = ws;
+    const dim3 sgrid((unsigned)L, (unsigned)((P + kUbScoreThreads - 1) / kUbScoreThreads));
+    SPG_CUDA(h, cudaMemsetAsync(u.row_count, 0, sizeof(int32_t) * (size_t)L * P, st));
+    if ((rc = launch(h, kStageScore, "ub_score_kernel<count>", kUbScoreKernels[dtype][0], sgrid, kUbScoreThreads, 0, st, u, sa)))
+        return rc;
+    std::vector<int32_t> row_count((size_t)L * P);
+    SPG_CUDA(h, cudaMemcpyAsync(row_count.data(), u.row_count, sizeof(int32_t) * row_count.size(), cudaMemcpyDeviceToHost, st));
+    SPG_CUDA(h, cudaStreamSynchronize(st));
+    std::vector<int64_t> row_off(row_count.size()), segs((size_t)L + 1);
+    int64_t n_cand = 0;
+    for (int k = 0; k < L; k++) {
+        segs[k] = n_cand;
+        for (int i = 0; i < P; i++) {
+            row_off[(size_t)k * P + i] = n_cand;
+            n_cand += row_count[(size_t)k * P + i];
+        }
+    }
+    segs[L] = n_cand;
+    if (n_cand > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "%lld candidates; the unbounded tier sorts at most 2^31 - 1", (long long)n_cand);
+    SPG_CUDA(h, cudaMemcpyAsync(const_cast<int64_t *>(u.row_off), row_off.data(), sizeof(int64_t) * row_off.size(), cudaMemcpyHostToDevice, st));
+    SPG_CUDA(h, cudaMemcpyAsync(seg_off, segs.data(), sizeof(int64_t) * segs.size(), cudaMemcpyHostToDevice, st));
+    size_t sort_bytes = 0;
+    SPG_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairsDescending(
+                    nullptr, sort_bytes, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, (const uint32_t *)nullptr,
+                    (uint32_t *)nullptr, (int)n_cand, L, seg_off, seg_off + 1, 0, 64, st));
+    void *sort_tmp = nullptr;
+    uint32_t *sorted = nullptr;
+    if ((rc = carve(h, h->ub_cands, [&](Carver &c) {
+             ws.cand_prio = c.take<double>((size_t)n_cand);
+             ws.cand_score = c.take<double>((size_t)n_cand);
+             ws.cand_ij = c.take<uint32_t>((size_t)n_cand);
+             ws.cand_key = c.take<unsigned long long>((size_t)n_cand);
+             u.cand_key_out = c.take<unsigned long long>((size_t)n_cand);
+             u.cand_idx = c.take<uint32_t>((size_t)n_cand);
+             sorted = c.take<uint32_t>((size_t)n_cand);
+             sort_tmp = c.take<unsigned char>(sort_bytes);
+         })))
+        return rc;
+    u.sorted = sorted;
+    u.ws = ws;
+    if ((rc = launch(h, kStageScore, "ub_score_kernel<write>", kUbScoreKernels[dtype][1], sgrid, kUbScoreThreads, 0, st, u, sa)))
+        return rc;
+
+    // 3. each limb's candidates by priority (stable: ties stay in generation order), then the greedy matching
+    if (n_cand > 0)
+        SPG_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairsDescending(sort_tmp, sort_bytes, ws.cand_key, u.cand_key_out, u.cand_idx, sorted,
+                                                                       (int)n_cand, L, seg_off, seg_off + 1, 0, 64, st));
+    SPG_CUDA(h, cudaMemsetAsync(u.used, 0, (size_t)L * 2 * P, st));
+    if ((rc = launch(h, kStageMatch, "ub_match_kernel", ub_match_kernel, 1, kMaxLimbs, 0, st, u))) return rc;
+
+    // 4. the person table, one row per accepted connection, and the assembly
+    std::vector<int32_t> conn_count((size_t)L);
+    SPG_CUDA(h, cudaMemcpyAsync(conn_count.data(), ws.conn_count, sizeof(int32_t) * L, cudaMemcpyDeviceToHost, st));
+    SPG_CUDA(h, cudaStreamSynchronize(st));
+    int64_t n_conn = 0;
+    for (int k = 0; k < L; k++) n_conn += std::max(conn_count[k], 0);
+    if (n_conn > kUbMaxRows) return fail(h, SPG_E_INVALID, "%lld connections; the unbounded tier's person table holds at most %d rows",
+                                         (long long)n_conn, kUbMaxRows);
+    const int R = std::max(1, (int)n_conn);
+    ws.capR = R;
+    PersonTable &t = u.table;
+    t.K = K;
+    t.capP = P;
+    t.capR = R;
+    if ((rc = carve(h, h->ub_people, [&](Carver &c) {
+             ws.subset = c.take<double>((size_t)R * (K + 2) * 2);
+             ws.people_xy = c.take<double>((size_t)R * std::max(J, 1) * 2);
+             ws.people_score = c.take<double>((size_t)R);
+             t.row = c.take<RowRec>((size_t)R);
+             t.slot = c.take<SlotRec>((size_t)K * R);
+             t.pscore = c.take<double>((size_t)R);
+             t.ps = c.take<float>((size_t)K * P);
+             t.postA = c.take<int>((size_t)R);
+             t.postB = c.take<int>((size_t)R);
+             t.off = c.take<int>((size_t)K + 1);
+             t.owner = c.take<short>((size_t)K * P);
+         })))
+        return rc;
+    t.px = ws.peak_x;
+    t.py = ws.peak_y;
+    u.ws = ws;
+    AssembleArgs aa = assemble_args(h, 0, 1, p);
+    aa.wire_flag = nullptr;  // the tier writes no wire record and consumes no armed signal
+    aa.done_counter = nullptr;
+    aa.ws = ws;
+    if ((rc = launch(h, kStageAssemble, "ub_assemble_kernel", ub_assemble_kernel, 1, kUbAssembleThreads, 0, st, u, aa))) return rc;
+    h->ub_ws = ws;
+    h->ub_valid = true;
+    return SPG_OK;
+}
+
+int spg_download_unbounded(spg_handle *h, spg_unbounded_sizes *sizes, int32_t *peak_count, double *x, double *y, float *score,
+                           uint32_t *anchor, int32_t *conn_count, int32_t *cand_count, uint32_t *ij, double *conn_score,
+                           double *conn_norm, double *subset, double *people_xy, double *people_score, void *stream) {
+    if (!h || !sizes) return SPG_E_INVALID;
+    if (!h->ub_valid) return fail(h, SPG_E_STATE, "no spg_group_unbounded call has succeeded on this handle");
+    DeviceGuard guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const Workspace &ws = h->ub_ws;
+    const size_t KP = (size_t)ws.K * ws.capP, LP = (size_t)ws.L * ws.capP;
+    int32_t n_persons = 0;
+    uint32_t status = 0;
+    SPG_CUDA(h, cudaMemcpyAsync(&n_persons, ws.n_persons, sizeof n_persons, cudaMemcpyDeviceToHost, st));
+    SPG_CUDA(h, cudaMemcpyAsync(&status, ws.status, sizeof status, cudaMemcpyDeviceToHost, st));
+    SPG_D2H(peak_count, ws.peak_count, ws.K);
+    SPG_D2H(x, ws.peak_x, KP);
+    SPG_D2H(y, ws.peak_y, KP);
+    SPG_D2H(score, ws.peak_score, KP);
+    SPG_D2H(anchor, ws.peak_anchor, KP);
+    SPG_D2H(conn_count, ws.conn_count, ws.L);
+    SPG_D2H(cand_count, ws.cand_count, ws.L);
+    SPG_D2H(ij, ws.conn_ij, LP);
+    SPG_D2H(conn_score, ws.conn_score, LP);
+    SPG_D2H(conn_norm, ws.conn_norm, LP);
+    SPG_D2H(subset, ws.subset, (size_t)ws.capR * (ws.K + 2) * 2);
+    SPG_D2H(people_xy, ws.people_xy, (size_t)ws.capR * ws.J * 2);
+    SPG_D2H(people_score, ws.people_score, (size_t)ws.capR);
+    SPG_CUDA(h, cudaStreamSynchronize(st));
+    sizes->cap_peaks = ws.capP;
+    sizes->cap_rows = ws.capR;
+    sizes->n_persons = n_persons;
+    sizes->status = status;
     return SPG_OK;
 }
 

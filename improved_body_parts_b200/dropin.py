@@ -18,6 +18,7 @@ There is no CPU path: without the CUDA library / an sm_90 GPU these functions ra
 """
 from __future__ import annotations
 
+import dataclasses
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -107,6 +108,51 @@ def _check_status(status: int) -> None:
     if status:
         raise GroupingError(f"grouping capacity exceeded or invalid sample index (status {status:#x}); "
                             f"capacities: {CAP_PEAKS} peaks/part, {CAP_CANDS} candidates/limb, {CAP_ROWS} person rows")
+
+
+#: status bits of an image that went past the handle's capacities (SPG_ST_PEAK_OVERFLOW | SPG_ST_CAND_OVERFLOW |
+#: SPG_ST_ROW_OVERFLOW): such an image is regrouped on the capacity-free tier (``Grouper.group_unbounded``)
+CAPACITY_BITS = 0x7
+
+
+def _over_capacity(status) -> bool:
+    return bool(int(status) & CAPACITY_BITS)
+
+
+def _unbounded(heat, paf, as_f64: bool, image_extent, params):
+    """One image's device maps regrouped on the capacity-free tier: a one-image ``GroupResult``.  Its status can only
+    carry the bits the reference raises for, which ``_check_status`` turns into ``GroupingError``."""
+    return _grouper().group_unbounded(heat, paf, image_extent, _params(params), paf_as_f64=as_f64)
+
+
+def _group_params(params) -> GroupParams:
+    p = _params(params)
+    return p if isinstance(p, GroupParams) else GroupParams.from_dict(dict(p or {}))
+
+
+def _chain_params(params) -> GroupParams:
+    """``params`` of a later stage with the peak-finding fields find_peaks ran with: what the tier regroups a chained
+    image with, so that its peaks are the ones find_peaks returned."""
+    return dataclasses.replace(_group_params(params), **_state["peak_params"])
+
+
+def _tier_unavailable(stage: str, status) -> GroupingError:
+    return GroupingError(f"{stage}: the image exceeds the grouping capacities (status {int(status):#x}; {CAP_PEAKS} "
+                         f"peaks/part, {CAP_CANDS} candidates/limb, {CAP_ROWS} person rows) and the capacity-free tier "
+                         f"needs the maps of the image: chain find_peaks -> find_connections -> find_people on each "
+                         f"other's return values, or call group()")
+
+
+def _people_of_result(r) -> list:
+    """``process()``'s return value (evaluate.py:523-543) from a one-image ``GroupResult``, in the form
+    ``wire.people_of`` gives it: ``np.float64`` coordinates and score, integer ``(0, 0)`` for a missing joint."""
+    out = []
+    for j in range(int(r.n_persons[0])):
+        row = r.subset[0, j]
+        pts = [(np.float64(x), np.float64(y)) if row[part, 0] >= 0 else (0, 0)
+               for part, (x, y) in zip(COCO_FROM_PART, r.people_xy[0, j])]
+        out.append((pts, np.float64(r.people_score[0, j])))
+    return out
 
 
 def _maps_to_device(hwc: np.ndarray, channels: int, dtype):
@@ -444,25 +490,52 @@ def _upload_peaks(g: Grouper, all_peaks) -> None:
 # ---- the three reference functions ---------------------------------------------------------------------
 def find_peaks(heatmap_avg, params):
     """evaluate.py:169-203.  ``heatmap_avg [H,W,>=18]`` -> list[18] of [(x, y, score, id), ...]."""
+    import torch
     g = _grouper()
-    g.nms_peaks(_heat_tensor(heatmap_avg), _params(params))
+    heat = _heat_tensor(heatmap_avg)
+    g.nms_peaks(heat, _params(params))
     r = g.fetch(1)
-    _check_status(r.status[0])
+    tier = _over_capacity(r.status[0])
+    if tier:  # every peak of the image from the capacity-free tier; no body-part maps yet, so zero planes stand in
+        zeros = torch.zeros((1, len(_limbs)) + tuple(heat.shape[2:]), dtype=torch.float32, device=heat.device)
+        r = _unbounded(heat, zeros, False, heat.shape[2], params)
+    else:
+        _check_status(r.status[0])
     all_peaks = r.as_reference_structures(0)[0]
+    gp = _group_params(params)
     _state.clear()
-    _state.update(peaks=all_peaks, handle=g)
+    _state.update(peaks=all_peaks, handle=g, heat=heat, tier_peaks=tier,
+                  peak_params=dict(thre1=gp.thre1, offset_radius=gp.offset_radius))
     return all_peaks
+
+
+def _chained_peaks(g: Grouper, all_peaks) -> bool:
+    """``all_peaks`` is what our own find_peaks returned last, on handle ``g``, with its heat maps kept."""
+    return _state.get("peaks") is all_peaks and _state.get("handle") is g and "heat" in _state
 
 
 def find_connections(all_peaks, paf_avg, image_width, params):
     """evaluate.py:206-276.  ``paf_avg [H,W,L]`` float32 or float64 -> (connection_all, special_k)."""
     g = _grouper()
-    _upload_peaks(g, all_peaks)
+    chained = _chained_peaks(g, all_peaks)
     paf, as_f64 = _paf_tensor(paf_avg)
-    g.limb_score(paf, image_width, _params(params), paf_as_f64=as_f64)
-    g.limb_match(1, _params(params))
-    r = g.fetch(1)
+    tier = chained and bool(_state.get("tier_peaks"))
+    if not tier:
+        _upload_peaks(g, all_peaks)
+        g.limb_score(paf, image_width, _params(params), paf_as_f64=as_f64)
+        g.limb_match(1, _params(params))
+        r = g.fetch(1)
+        if _over_capacity(r.status[0]):
+            if not chained:
+                raise _tier_unavailable("find_connections", r.status[0])
+            tier = True
+    if tier:
+        gp = _chain_params(params)
+        r = _unbounded(_state["heat"], paf, as_f64, image_width, gp)
+        _state.update(tier=r, tier_params=gp)  # find_people takes its persons from the same call
     _check_status(r.status[0])
+    if chained:
+        _state.update(paf=paf, as_f64=as_f64, extent=image_width)
     # ids in the rows are those of the caller's all_peaks (:267), not positions in our tables
     _, conns, special, _, _ = r.as_reference_structures(0)
     for k, rows in enumerate(conns):
@@ -480,8 +553,18 @@ def find_people(connection_all, special_k, all_peaks, params):
     g = _grouper()  # assembly does not depend on the map size
     if _state.get("conns") is connection_all and _state.get("special") is special_k and _state.get("peaks") is all_peaks \
             and _state.get("handle") is g:  # evaluate.py:509-511 handing our own objects back: everything is still on the device
-        g.assemble(1, _params(params))
-        r = g.fetch(1)
+        r = _state.get("tier")
+        if r is None:
+            g.assemble(1, _params(params))
+            r = g.fetch(1)
+            if _over_capacity(r.status[0]):
+                if "paf" not in _state:
+                    raise _tier_unavailable("find_people", r.status[0])
+                r = None
+        if r is None or _state.get("tier_params") not in (None, _chain_params(params)):
+            gp = _chain_params(params)  # the persons of the tier, with find_people's own assembly parameters
+            r = _unbounded(_state["heat"], _state["paf"], _state["as_f64"], _state["extent"], gp)
+            _state.update(tier=r, tier_params=gp)
         _check_status(r.status[0])
         return r.subset[0, :int(r.n_persons[0])].copy(), np.array([item for sublist in all_peaks for item in sublist])
     _upload_peaks(g, all_peaks)
@@ -500,6 +583,8 @@ def find_people(connection_all, special_k, all_peaks, params):
                          np.concatenate(sc) if sc else np.zeros(0), np.concatenate(nm) if nm else np.zeros(0))
     g.assemble(1, _params(params))
     r = g.fetch(1)
+    if _over_capacity(r.status[0]):
+        raise _tier_unavailable("find_people", r.status[0])
     _check_status(r.status[0])
     subset = r.subset[0, :int(r.n_persons[0])].copy()
     candidate = np.array([item for sublist in all_peaks for item in sublist])  # evaluate.py:283, verbatim semantics
@@ -523,6 +608,8 @@ def group(heatmap_avg, paf_avg, image_extent, params):
     paf, as_f64 = _paf_tensor(paf_avg)
     g.group_device(heat, paf, image_extent, _params(params), paf_as_f64=as_f64)
     r = g.fetch(1)
+    if _over_capacity(r.status[0]):
+        r = _unbounded(heat, paf, as_f64, image_extent, params)
     _check_status(r.status[0])
     return r.as_reference_structures(0)
 
@@ -547,8 +634,9 @@ _records: Dict[int, object] = {}
 
 def _group_ragged(maps, image_extents, params, records: bool = False):
     """The maps of a batch of images to the device and one ragged grouping call (``spg_group_ragged``) on the batched
-    handle: ``(handle, n_images, wire)``.  With ``records`` the call also writes image i's wire record to row i of
-    ``wire``, a per-device buffer; without, ``wire`` is None."""
+    handle: ``(handle, n_images, wire, regroup)``.  With ``records`` the call also writes image i's wire record to row i
+    of ``wire``, a per-device buffer; without, ``wire`` is None.  ``regroup(i)`` regroups image i on the capacity-free
+    tier from the device maps of the call."""
     import torch
     pairs, as_f64 = _ragged_maps(maps)
     g = _grouper_many(len(pairs))
@@ -566,7 +654,10 @@ def _group_ragged(maps, image_extents, params, records: bool = False):
     finally:
         if records:
             g.set_wire_output(None)
-    return g, len(pairs), buf
+
+    def regroup(i: int):
+        return _unbounded(pairs[i][0], pairs[i][1], as_f64, image_extents[i], params)
+    return g, len(pairs), buf, regroup
 
 
 def group_many(maps, image_extents, params):
@@ -575,10 +666,16 @@ def group_many(maps, image_extents, params):
     ``maps``: per image a ``(heatmap_avg, paf_avg)`` pair -- the ``DeviceMaps`` ``predict`` returns or host ``[H, W, C]``
     arrays; ``image_extents``: per image ``oriImg.shape[0]``.  Returns one ``(all_peaks, connection_all, special_k,
     subset, candidate)`` per image, equal to what ``group()`` returns for it."""
-    g, n, _ = _group_ragged(maps, image_extents, params)
+    image_extents = list(image_extents)
+    g, n, _, regroup = _group_ragged(maps, image_extents, params)
     r = g.fetch(n)
     out = []
     for i in range(n):
+        if _over_capacity(r.status[i]):
+            ri = regroup(i)
+            _check_status(ri.status[0])
+            out.append(ri.as_reference_structures(0))
+            continue
         _check_status(r.status[i])
         out.append(r.as_reference_structures(i))
     return out
@@ -587,9 +684,15 @@ def group_many(maps, image_extents, params):
 def _people_of_batch(maps, extents, params) -> list:
     """One ragged grouping call for a batch of images, their wire records in one device-to-host copy, and per image
     ``process()``'s return value (evaluate.py:523-543)."""
-    g, n, buf = _group_ragged(maps, extents, params, records=True)
+    extents = list(extents)
+    g, n, buf, regroup = _group_ragged(maps, extents, params, records=True)
     out = []
-    for rec in wire.as_records(buf[:n].cpu().numpy(), g.J, g.capR):
+    for i, rec in enumerate(wire.as_records(buf[:n].cpu().numpy(), g.J, g.capR)):
+        if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
+            ri = regroup(i)
+            _check_status(ri.status[0])
+            out.append(_people_of_result(ri))
+            continue
         _check_status(rec["status"])
         out.append(wire.people_of(rec))
     return out

@@ -100,6 +100,9 @@ _PROTOTYPES = {
     "spg_get_device_view": (_int, [_ptr, _P(_DeviceView)]),
     "spg_group_batch": (_int, [_ptr, _ptr, _i64, _i64, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_group_ragged": (_int, [_ptr, _P(_ImageMaps), _i32, _i32, _P(_Params), _ptr]),
+    "spg_group_unbounded": (_int, [_ptr, _P(_ImageMaps), _i32, _P(_Params), _ptr]),
+    # spg_unbounded_sizes is four 32-bit words: cap_peaks, cap_rows, n_persons, status (uint32)
+    "spg_download_unbounded": (_int, [_ptr, _P(C.c_int32)] + [_ptr] * 14),
     "spg_group_host": (_int, [_ptr, _ptr, _ptr, _i32, _i32, _i32, _i32, _f64, _P(_Params), _ptr, _ptr, _ptr, _ptr]),
     "spg_host_alloc": (_int, [_P(C.c_void_p), _u64]),
     "spg_host_free": (_int, [_ptr]),
@@ -503,6 +506,46 @@ class Grouper:
         _check(rc, "spg_group_ragged", self._h)
         self._peaks_shape = None
         self._last_n = len(maps)
+
+    def group_unbounded(self, heat, paf, image_extent: float, params=None, paf_as_f64: bool = False,
+                        stream=None) -> GroupResult:
+        """One image on the capacity-free tier (``spg_group_unbounded``): the reference's answer whatever the image's
+        number of peaks, candidates and persons, where the other calls set a capacity status bit.  Synchronous.
+
+        ``heat`` / ``paf``: the image's maps as for ``group_ragged`` (``[C, H, W]`` or ``[1, C, H, W]``).  Returns a
+        one-image ``GroupResult`` with the tier's sizes (``peak_x.shape[2]`` = the largest part's peak count,
+        ``subset.shape[1]`` = the person table's rows), so ``as_reference_structures(0)`` and ``keypoints(0)`` read it
+        as they read ``fetch``'s.  The handle's results of earlier calls are left as they were."""
+        import torch
+        heat = heat[None] if heat.dim() == 3 else heat
+        paf = paf[None] if paf.dim() == 3 else paf
+        self._check_maps(heat, "heat", self.K, (torch.float32,))
+        self._check_maps(paf, "paf", self.L, (torch.float32, torch.float64))
+        if heat.shape[0] != 1 or paf.shape[0] != 1 or tuple(paf.shape[2:]) != tuple(heat.shape[2:]):
+            raise GroupingError("heat and paf must be one image each, of the same size")
+        im = _ImageMaps(heat.data_ptr(), paf.data_ptr(), heat.stride(1), paf.stride(1), heat.shape[2], heat.shape[3],
+                        float(image_extent))
+        p = params_struct(params)
+        st = self._stream_ptr(stream)
+        _check(self._lib.spg_group_unbounded(self._h, C.byref(im), self._paf_dtype(paf, paf_as_f64), C.byref(p), st),
+               "spg_group_unbounded", self._h)
+        sz = (C.c_int32 * 4)()  # spg_unbounded_sizes: cap_peaks, cap_rows, n_persons, status
+        _check(self._lib.spg_download_unbounded(self._h, sz, *([None] * 13), st), "spg_download_unbounded", self._h)
+        K, L, J, cP, cR = self.K, self.L, self.J, int(sz[0]), int(sz[1])
+        r = GroupResult(
+            K=K, L=L, limbs=self.limbs, peak_count=np.zeros((1, K), np.int32), peak_x=np.zeros((1, K, cP)),
+            peak_y=np.zeros((1, K, cP)), peak_score=np.zeros((1, K, cP), np.float32),
+            peak_anchor=np.zeros((1, K, cP), np.uint32), conn_count=np.zeros((1, L), np.int32),
+            cand_count=np.zeros((1, L), np.int32), conn_ij=np.zeros((1, L, cP), np.uint32),
+            conn_score=np.zeros((1, L, cP)), conn_norm=np.zeros((1, L, cP)),
+            n_persons=np.array([sz[2]], np.int32), subset=np.zeros((1, cR, K + 2, 2)),
+            people_xy=np.zeros((1, cR, J, 2)), people_score=np.zeros((1, cR)),
+            status=np.array([sz[3] & 0xffffffff], np.uint32))
+        _check(self._lib.spg_download_unbounded(
+            self._h, sz, _vp(r.peak_count), _vp(r.peak_x), _vp(r.peak_y), _vp(r.peak_score), _vp(r.peak_anchor),
+            _vp(r.conn_count), _vp(r.cand_count), _vp(r.conn_ij), _vp(r.conn_score), _vp(r.conn_norm), _vp(r.subset),
+            _vp(r.people_xy), _vp(r.people_score), st), "spg_download_unbounded", self._h)
+        return r
 
     def group_host(self, heat: np.ndarray, paf: np.ndarray, image_extent: float, params=None, out=None) -> dict:
         """Host maps in, person lists out (H2D / kernels / D2H pipelined inside the library).  Synchronous.

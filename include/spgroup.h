@@ -139,6 +139,36 @@ typedef struct spg_image_maps {
 int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n_images, int32_t paf_dtype,
                      const spg_params *params, void *stream);
 
+/* ---- the capacity-free tier: one image whatever its number of peaks, candidates and persons ---------------------
+ * The calls above hold at most max_peaks_per_part peaks per part (<= 128), max_cands_per_limb candidates per limb and
+ * max_person_rows rows (<= 128); an image past one of them gets SPG_ST_PEAK_OVERFLOW / SPG_ST_CAND_OVERFLOW /
+ * SPG_ST_ROW_OVERFLOW and undefined outputs.  spg_group_unbounded regroups such an image with every list sized from the
+ * image itself, bit-identical to the reference as the bounded path is: peaks -> connections -> people of `image` (its
+ * maps, size and image_extent) on `stream`.  The host sizes each stage's tables from the previous stage's counts, so the
+ * call synchronises `stream` three times; the tables belong to the handle, grow on demand and live until spg_destroy.
+ * The tier's status word carries SPG_ST_SAMPLE_INDEX and SPG_ST_ASSERT as the bounded path sets them, never a capacity
+ * bit.  Its own limits -- at most 65535 peaks per part ((i, j) of a connection are packed in 16 bits each), 32767
+ * accepted connections per image (the person table has one row per connection) and 2^31 - 1 candidates -- and a failed
+ * allocation make the call return an error, never undefined output.  Maps: 2 <= height, width <= 32767; the handle's
+ * max_h / max_w do not apply. */
+int spg_group_unbounded(spg_handle *h, const spg_image_maps *image, int32_t paf_dtype, const spg_params *params,
+                        void *stream);
+typedef struct spg_unbounded_sizes {
+    int32_t cap_peaks;  /* peak arrays are [K][cap_peaks], connection arrays [L][cap_peaks] */
+    int32_t cap_rows;   /* person arrays are [cap_rows][...] */
+    int32_t n_persons;  /* persons after the prune */
+    uint32_t status;    /* SPG_ST_* bits of the image */
+} spg_unbounded_sizes;
+/* The last spg_group_unbounded call's results, laid out as the spg_download_* arrays of ONE image with the tier's sizes:
+ * peak_count [K], x / y / score / anchor [K][cap_peaks], conn_count / cand_count [L], ij / conn_score / conn_norm
+ * [L][cap_peaks], subset [cap_rows][K+2][2], people_xy [cap_rows][J][2], people_score [cap_rows].  `sizes` is always
+ * filled; NULL arrays are skipped, so a first call with NULL arrays gives the sizes to allocate.  Synchronises `stream`.
+ * SPG_E_STATE before the first successful spg_group_unbounded. */
+int spg_download_unbounded(spg_handle *h, spg_unbounded_sizes *sizes, int32_t *peak_count, double *x, double *y,
+                           float *score, uint32_t *anchor, int32_t *conn_count, int32_t *cand_count, uint32_t *ij,
+                           double *conn_score, double *conn_norm, double *subset, double *people_xy,
+                           double *people_score, void *stream);
+
 /* host inputs (pinned for full overlap; pageable works): H2D in chunks overlapped with the kernels, results
  * copied back into the caller's arrays (any of which may be NULL).  Synchronous.
  *   heat_host [N][K][H][W] f32, paf_host [N][L][H][W] f32|f64
