@@ -802,15 +802,25 @@ static PostScale post_scale(const void *net, int dtype, int64_t img_stride, int6
     return s;
 }
 
-// A scale's or an image's network output ("<what> <i>" in the error): present, float32 or float16, and its crop inside
-// the h x w output up-sampled by `stride`
-static int check_net_out(spg_handle *h, const char *what, int i, const void *net, int dtype, int hn, int wn, int crop_h, int crop_w,
+// A scale's or an item's network output (`what` names it in the error): present, float32 or float16, and its crop
+// inside the h x w output up-sampled by `stride`
+static int check_net_out(spg_handle *h, const char *what, const void *net, int dtype, int hn, int wn, int crop_h, int crop_w,
                          int stride) {
-    if (!net) return fail(h, SPG_E_INVALID, "%s %d: net_out is NULL", what, i);
-    if (dtype != SPG_F32 && dtype != SPG_F16) return fail(h, SPG_E_INVALID, "%s %d: network output must be SPG_F32 or SPG_F16", what, i);
+    if (!net) return fail(h, SPG_E_INVALID, "%s: net_out is NULL", what);
+    if (dtype != SPG_F32 && dtype != SPG_F16) return fail(h, SPG_E_INVALID, "%s: network output must be SPG_F32 or SPG_F16", what);
     if (hn < 1 || wn < 1 || crop_h < 1 || crop_w < 1 || crop_h > hn * stride || crop_w > wn * stride)
-        return fail(h, SPG_E_INVALID, "%s %d: crop %dx%d does not fit the up-sampled %dx%d output", what, i, crop_h, crop_w, hn * stride,
+        return fail(h, SPG_E_INVALID, "%s: crop %dx%d does not fit the up-sampled %dx%d output", what, crop_h, crop_w, hn * stride,
                     wn * stride);
+    return SPG_OK;
+}
+
+// A rotation entry: apply 0 or 1, reserved 0 and a finite matrix.  `what` names the entry in the error and `apply` its
+// apply field.
+static int check_rotation(spg_handle *h, const char *what, const char *apply, const spg_postnet_rotation &r) {
+    if ((r.apply != 0 && r.apply != 1) || r.reserved != 0)
+        return fail(h, SPG_E_INVALID, "%s: %s must be 0 or 1 and reserved 0", what, apply);
+    for (int k = 0; k < 6; k++)
+        if (!std::isfinite(r.matrix[k])) return fail(h, SPG_E_INVALID, "%s: matrix entry %d is not finite", what, k);
     return SPG_OK;
 }
 
@@ -931,11 +941,11 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     if (!h) return SPG_E_INVALID;
     if (!d || !d->scales || d->n_scales < 1 || !d->flip_paf_ord || !d->flip_heat_ord) return fail(h, SPG_E_INVALID, "postnet descriptor incomplete");
     bool any_rot = false;
+    int rc;
+    char what[32];
     for (int t = 0; rot && t < d->n_scales; t++) {
-        if ((rot[t].apply != 0 && rot[t].apply != 1) || rot[t].reserved != 0)
-            return fail(h, SPG_E_INVALID, "rotation %d: apply must be 0 or 1 and reserved 0", t);
-        for (int k = 0; k < 6; k++)
-            if (!std::isfinite(rot[t].matrix[k])) return fail(h, SPG_E_INVALID, "rotation %d: matrix entry %d is not finite", t, k);
+        snprintf(what, sizeof what, "rotation %d", t);
+        if ((rc = check_rotation(h, what, "apply", rot[t]))) return rc;
         if (rot[t].apply && d->stride != 4) return fail(h, SPG_E_INVALID, "rotation %d: rotated items need stride 4", t);
         any_rot = any_rot || rot[t].apply;
     }
@@ -944,7 +954,6 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     if (paf_dtype == SPG_F32 && d->n_scales != 1)
         return fail(h, SPG_E_INVALID, "float32 body-part planes hold the reference's float64 values only for a single scale");
     if (d->stride < 1 || d->stride > 16) return fail(h, SPG_E_INVALID, "stride outside [1,16]");
-    int rc;
     if ((rc = check_dims(h, n, H, W))) return rc;
     if (n == 0) return SPG_OK;
     const Workspace &ws = h->ws;
@@ -961,7 +970,8 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     a.H = H; a.W = W; a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p);
     for (int t = 0; t < d->n_scales; t++) {
         const spg_postnet_scale &sc = d->scales[t];
-        if ((rc = check_net_out(h, "scale", t, sc.net_out, sc.dtype, sc.h, sc.w, sc.crop_h, sc.crop_w, d->stride))) return rc;
+        snprintf(what, sizeof what, "scale %d", t);
+        if ((rc = check_net_out(h, what, sc.net_out, sc.dtype, sc.h, sc.w, sc.crop_h, sc.crop_w, d->stride))) return rc;
     }
     // At stride 4 the scale loop runs INSIDE the kernel (groups of kPostMaxScales): one tile geometry for all fused scales.
     // With a rotated item, or at another stride, every item is a launch of its own, in item order; the float64 sums
@@ -987,78 +997,14 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     return SPG_OK;
 }
 
-// Ragged batches of single-item images: each family's images (plan_post: the kernel and tile spg_postnet picks for each
-// image alone) in its ragged kernel's launches, identity items (crop == image) first, images largest first, one channel
-// chunk per family for all its launches.
-int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *images, int32_t n, int32_t paf_dtype,
-                       void *stream) {
-    if (!h) return SPG_E_INVALID;
-    int rc;
-    if ((rc = check_batch(h, n))) return rc;
-    if (!images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
-    if (!cm || !cm->flip_paf_ord || !cm->flip_heat_ord) return fail(h, SPG_E_INVALID, "postnet common descriptor incomplete");
-    if (cm->stride != 4) return fail(h, SPG_E_INVALID, "the ragged post-network stage needs stride 4 (got %d)", cm->stride);
-    if (cm->net_dtype != SPG_F32 && cm->net_dtype != SPG_F16) return fail(h, SPG_E_INVALID, "network output must be SPG_F32 or SPG_F16");
-    if (paf_dtype != SPG_F32 && paf_dtype != SPG_F64) return fail(h, SPG_E_INVALID, "paf_dtype must be SPG_F32 or SPG_F64");
-    PostArgs a{};
-    if ((rc = post_common(h, 4, 1, cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord, cm->nan_scrub, paf_dtype, a)))
-        return rc;
-    a.n_fused = 1;
-    // validate every image before the first launch
-    const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
-    std::vector<PostImage> imgs[2];  // by family: kPostIdent, kPostFourPhase
-    long long tiles[2] = {0, 0};
-    PostPlan plans[2];               // one scale per image: the same chunk target and shared memory for a family's images
-    for (int i = 0; i < n; i++) {
-        const spg_postnet_image &im = images[i];
-        if (!im.heat_out || !im.paf_out) return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out is NULL", i);
-        // the kernels store rows of 4 values with 16-byte stores (postnet_x4_ident_tile)
-        if ((reinterpret_cast<uintptr_t>(im.heat_out) & 15) || (reinterpret_cast<uintptr_t>(im.paf_out) & 15))
-            return fail(h, SPG_E_INVALID, "image %d: heat_out/paf_out must be 16-byte aligned", i);
-        if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
-            return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
-        if ((rc = check_net_out(h, "image", i, im.net_out, cm->net_dtype, im.h, im.w, im.crop_h, im.crop_w, 4))) return rc;
-        if (im.pair_stride < 0 || im.chan_stride < 0) return fail(h, SPG_E_INVALID, "image %d: negative stride", i);
-        PostImage d{};
-        d.sc[0] = post_scale(im.net_out, cm->net_dtype, 0, im.pair_stride, im.chan_stride, im.h, im.w, im.crop_h, im.crop_w, im.height, im.width);
-        d.H = im.height; d.W = im.width; d.heat = im.heat_out; d.paf = im.paf_out;
-        PostPlan pl;
-        if ((rc = plan_post(h, d.sc, 1, true, 4, d.H, d.W, nullptr, i, &pl))) return rc;
-        d.tile_w = pl.tile_w; d.tile_h = pl.tile_h;
-        const long long t = post_tiles(d.H, d.W, d.tile_w, d.tile_h, d.tiles_x, d.tiles_y);
-        if (t * kPostRaggedMaxImages > 0x7fffffffLL)
-            return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
-        imgs[pl.family].push_back(d);
-        tiles[pl.family] += t;
-        plans[pl.family] = pl;
-    }
-    DeviceGuard guard(h->device);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    auto place = [](PostRagged &r, int k, int x) {
-        r.img[k].first_cta = x;
-        r.n = k + 1;
-        return r.img[k].tiles_x * r.img[k].tiles_y;
-    };
-    for (int f : {kPostIdent, kPostFourPhase}) {
-        if (imgs[f].empty()) continue;
-        std::stable_sort(imgs[f].begin(), imgs[f].end(), [](const PostImage &x, const PostImage &y) {
-            return (int64_t)x.H * x.W > (int64_t)y.H * y.W;
-        });
-        const PostKernels &k = kPostKernels[f];
-        a.chan_chunk = post_chan_chunk(h, a.n_out, tiles[f], plans[f].ctas_per_sm);
-        if ((rc = launch_ragged(h, kStagePostnet, k.ragged_name, k.ragged[cm->net_dtype == SPG_F16], place,
-                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, plans[f].smem, st, a, imgs[f])))
-            return rc;
-    }
-    return SPG_OK;
-}
-
-// Ragged batches of multi-item images: spg_postnet_rotated's schedule for every image at once.  The items go in groups
-// -- kPostMaxScales fused unrotated items, or one item per group when any is rotated -- and within a group each image goes
-// in the family and tile plan_post picks for it alone, largest first, as many per launch as PostItemsRagged holds.  One
-// unrotated item per image is spg_postnet_ragged.
-int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *items,
-                             const spg_postnet_rotation *rot, int32_t n, int32_t n_items, int32_t paf_dtype, void *stream) {
+// Ragged batches, over items[n][n_items] and rot (NULL, or one entry per item): spg_postnet_rotated's schedule for every
+// image at once.  The items go in groups -- kPostMaxScales fused unrotated items, or one item per group when any is
+// rotated -- and within a group each image goes in the family and tile plan_post picks for it alone.  A group's images
+// are bucketed by kernel, identity family first, and each bucket's images go largest first, as many per launch as its
+// kernel's descriptor struct holds, with one channel chunk for all its launches.  One unrotated item per image takes
+// the single-scale ragged kernels.
+static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *items,
+                          const spg_postnet_rotation *rot, int32_t n, int32_t n_items, int32_t paf_dtype, void *stream) {
     if (!h) return SPG_E_INVALID;
     int rc;
     if ((rc = check_batch(h, n))) return rc;
@@ -1073,17 +1019,20 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
     if ((rc = post_common(h, 4, std::max(n_items, 1), cm->paf_chan0, cm->heat_chan0, cm->flip_paf_ord, cm->flip_heat_ord,
                           cm->nan_scrub, paf_dtype, a)))
         return rc;
-    // validate every image and item before the first launch
+    // validate every image and item before the first launch; errors name "image i", or "image i item t" of several items
+    char what[48];
+    auto name = [&](int i, int t) {
+        if (n_items == 1) snprintf(what, sizeof what, "image %d", i);
+        else snprintf(what, sizeof what, "image %d item %d", i, t);
+        return what;
+    };
     bool any_rot = false;
     for (int i = 0; rot && i < n; i++) {
         for (int t = 0; t < n_items; t++) {
             const spg_postnet_rotation &r = rot[(size_t)i * n_items + t];
-            if ((r.apply != 0 && r.apply != 1) || r.reserved != 0)
-                return fail(h, SPG_E_INVALID, "image %d item %d: rotation apply must be 0 or 1 and reserved 0", i, t);
-            for (int k = 0; k < 6; k++)
-                if (!std::isfinite(r.matrix[k])) return fail(h, SPG_E_INVALID, "image %d item %d: matrix entry %d is not finite", i, t, k);
+            if ((rc = check_rotation(h, name(i, t), "rotation apply", r))) return rc;
             if (r.apply != rot[t].apply)
-                return fail(h, SPG_E_INVALID, "image %d item %d: rotated in some images and not in others (one rotation_search per call)", i, t);
+                return fail(h, SPG_E_INVALID, "%s: rotated in some images and not in others (one rotation_search per call)", name(i, t));
             any_rot = any_rot || r.apply;
         }
     }
@@ -1094,13 +1043,11 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
         const spg_postnet_image &im = items[(size_t)i * n_items];
         for (int t = 0; t < n_items; t++) {
             const spg_postnet_image &it = items[(size_t)i * n_items + t];
-            if (!it.heat_out || !it.paf_out) return fail(h, SPG_E_INVALID, "image %d item %d: heat_out/paf_out is NULL", i, t);
+            if (!it.heat_out || !it.paf_out) return fail(h, SPG_E_INVALID, "%s: heat_out/paf_out is NULL", name(i, t));
             if (it.height != im.height || it.width != im.width || it.heat_out != im.heat_out || it.paf_out != im.paf_out)
-                return fail(h, SPG_E_INVALID, "image %d item %d: height/width/heat_out/paf_out differ from the image's item 0", i, t);
-            char what[32];
-            snprintf(what, sizeof what, "image %d item", i);
-            if ((rc = check_net_out(h, what, t, it.net_out, cm->net_dtype, it.h, it.w, it.crop_h, it.crop_w, 4))) return rc;
-            if (it.pair_stride < 0 || it.chan_stride < 0) return fail(h, SPG_E_INVALID, "image %d item %d: negative stride", i, t);
+                return fail(h, SPG_E_INVALID, "%s: height/width/heat_out/paf_out differ from the image's item 0", name(i, t));
+            if ((rc = check_net_out(h, name(i, t), it.net_out, cm->net_dtype, it.h, it.w, it.crop_h, it.crop_w, 4))) return rc;
+            if (it.pair_stride < 0 || it.chan_stride < 0) return fail(h, SPG_E_INVALID, "%s: negative stride", name(i, t));
         }
         // the kernels store rows of 4 values with 16-byte stores (postnet_x4_ident_tile)
         if ((reinterpret_cast<uintptr_t>(im.heat_out) & 15) || (reinterpret_cast<uintptr_t>(im.paf_out) & 15))
@@ -1111,15 +1058,15 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
         acc_total += (size_t)h->ws.K * im.height * im.width;
     }
     if (n == 0) return SPG_OK;
-    if (n_items == 1 && !any_rot) return spg_postnet_ragged(h, cm, items, n, paf_dtype, stream);
     // the schedule of every launch, planned (and checked) before the first one: per item group, one launch list per kernel
-    struct Group {
+    struct Bucket {
         int t0, n_fused;
+        bool single_scale;  // one unrotated item per image: the single-scale ragged kernels
         PostPlan plan;
         long long tiles;
         std::vector<PostItemsImage> imgs;
     };
-    std::vector<Group> groups;
+    std::vector<Bucket> buckets;
     const int per_group = any_rot ? 1 : kPostMaxScales;
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1131,7 +1078,8 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
     for (int t0 = 0; t0 < n_items; t0 += per_group) {
         const int nf = std::min(per_group, n_items - t0);
         const bool rotated = any_rot && rot[t0].apply;
-        const size_t first = groups.size();
+        const bool single_scale = n_items == 1 && !rotated;
+        const size_t first = buckets.size();
         for (int i = 0; i < n; i++) {
             const spg_postnet_image &im = items[(size_t)i * n_items];
             PostItemsImage d{};
@@ -1145,38 +1093,67 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
             if (rotated) invert_affine(rot[(size_t)i * n_items + t0].matrix, d.rot);
             PostPlan pl;
             if ((rc = plan_post(h, d.sc, nf, n_items == 1, 4, d.H, d.W, rotated ? d.rot : nullptr, t0, &pl)))
-                return fail(h, rc, "image %d item %d: %s", i, t0, std::string(h->err).c_str());
+                return fail(h, rc, "%s: %s", name(i, t0), std::string(h->err).c_str());
             d.tile_w = pl.tile_w; d.tile_h = pl.tile_h;
             const long long tl = post_tiles(d.H, d.W, d.tile_w, d.tile_h, d.tiles_x, d.tiles_y);
-            if (tl * kPostItemsMaxImages > 0x7fffffffLL)
+            if (tl * (single_scale ? kPostRaggedMaxImages : kPostItemsMaxImages) > 0x7fffffffLL)
                 return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
-            size_t g = first;
-            while (g < groups.size() && !(groups[g].plan.family == pl.family && groups[g].plan.single == pl.single &&
-                                          groups[g].plan.ident == pl.ident))
-                g++;
-            if (g == groups.size()) groups.push_back(Group{t0, nf, pl, 0, {}});
-            groups[g].imgs.push_back(d);
-            groups[g].tiles += tl;
+            size_t b = first;
+            while (b < buckets.size() && !(buckets[b].plan.family == pl.family && buckets[b].plan.single == pl.single &&
+                                           buckets[b].plan.ident == pl.ident))
+                b++;
+            if (b == buckets.size()) buckets.push_back(Bucket{t0, nf, single_scale, pl, 0, {}});
+            buckets[b].imgs.push_back(d);
+            buckets[b].tiles += tl;
         }
+        // identity family first; the buckets of fused or rotated items are of one family each and keep their order
+        std::stable_sort(buckets.begin() + first, buckets.end(), [](const Bucket &x, const Bucket &y) {
+            return x.plan.family < y.plan.family;
+        });
     }
-    auto place = [](PostItemsRagged &r, int k, int x) {
+    auto place = [](auto &r, int k, int x) {
         r.img[k].first_cta = x;
         r.n = k + 1;
         return r.img[k].tiles_x * r.img[k].tiles_y;
     };
-    for (Group &g : groups) {
-        std::stable_sort(g.imgs.begin(), g.imgs.end(), [](const PostItemsImage &x, const PostItemsImage &y) {
+    for (Bucket &b : buckets) {
+        std::stable_sort(b.imgs.begin(), b.imgs.end(), [](const PostItemsImage &x, const PostItemsImage &y) {
             return (int64_t)x.H * x.W > (int64_t)y.H * y.W;
         });
-        const PostKernels &k = kPostKernels[g.plan.family];
-        a.n_fused = g.n_fused;
-        a.scale_index = g.t0;
-        a.chan_chunk = post_chan_chunk(h, a.n_out, g.tiles, g.plan.ctas_per_sm);
-        if ((rc = launch_ragged(h, kStagePostnet, k.items_name, k.items[g.plan.single][g.plan.ident][g.plan.f16], place,
-                                (a.n_out + a.chan_chunk - 1) / a.chan_chunk, kPostThreads, g.plan.smem, st, a, g.imgs)))
-            return rc;
+        const PostKernels &k = kPostKernels[b.plan.family];
+        a.n_fused = b.n_fused;
+        a.scale_index = b.t0;
+        a.chan_chunk = post_chan_chunk(h, a.n_out, b.tiles, b.plan.ctas_per_sm);
+        const int chunks = (a.n_out + a.chan_chunk - 1) / a.chan_chunk;
+        if (b.single_scale) {
+            std::vector<PostImage> imgs(b.imgs.size());
+            for (size_t j = 0; j < imgs.size(); j++) {
+                const PostItemsImage &d = b.imgs[j];
+                PostImage &s = imgs[j];
+                s.sc[0] = d.sc[0];
+                s.H = d.H; s.W = d.W; s.heat = d.heat; s.paf = d.paf;
+                s.tile_w = d.tile_w; s.tile_h = d.tile_h; s.tiles_x = d.tiles_x; s.tiles_y = d.tiles_y;
+            }
+            rc = launch_ragged(h, kStagePostnet, k.ragged_name, k.ragged[b.plan.f16], place, chunks, kPostThreads, b.plan.smem, st, a,
+                               imgs);
+        } else {
+            rc = launch_ragged(h, kStagePostnet, k.items_name, k.items[b.plan.single][b.plan.ident][b.plan.f16], place, chunks,
+                               kPostThreads, b.plan.smem, st, a, b.imgs);
+        }
+        if (rc) return rc;
     }
     return SPG_OK;
+}
+
+int spg_postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *images, int32_t n, int32_t paf_dtype,
+                       void *stream) {
+    if (h && !images && n > 0) return fail(h, SPG_E_INVALID, "images is NULL");
+    return postnet_ragged(h, cm, images, nullptr, n, 1, paf_dtype, stream);
+}
+
+int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *items,
+                             const spg_postnet_rotation *rot, int32_t n, int32_t n_items, int32_t paf_dtype, void *stream) {
+    return postnet_ragged(h, cm, items, rot, n, n_items, paf_dtype, stream);
 }
 
 // ---- pre-network stage -------------------------------------------------------------------------

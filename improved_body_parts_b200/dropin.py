@@ -320,28 +320,6 @@ def _network_output(model, x):
     return out
 
 
-def _single_item(params, model_params) -> bool:
-    """One unrotated item per image at stride 4: the configuration ``predict_batch`` batches (the reference's default)."""
-    return len(params["scale_search"]) == 1 and len(params["rotation_search"]) == 1 and \
-        params["rotation_search"][0] == 0 and int(model_params["stride"]) == 4
-
-
-def plan_buckets(image_shapes, params, model_params):
-    """The batches of ``predict_batch``: per image ``(multiplier, scale, H1, W1, Hp, Wp)`` of its one item (the
-    multiplier of evaluate.py:87, the scale after the clamp of :94-96, the crop size and the padded network input size of
-    :98-100), and the images grouped by network input size ``{(Hp, Wp): [image index, ...]}`` in order of first
-    appearance."""
-    plan, buckets = [], {}
-    for i, shape in enumerate(image_shapes):
-        h, w = int(shape[0]), int(shape[1])
-        multiplier = params["scale_search"][0] * model_params["boxsize"] / h
-        scale = clamp_scale(multiplier, (h, w))
-        geo = input_geometry(h, w, scale, int(model_params["max_downsample"]))
-        plan.append((multiplier, scale) + geo)
-        buckets.setdefault(geo[2:], []).append(i)
-    return plan, buckets
-
-
 def plan_items(image_shapes, params, model_params):
     """The batches of ``predict_batch`` for any ``scale_search x rotation_search``: per image, per item of
     ``product(multiplier, rotation_search)`` (evaluate.py:87-90) ``(multiplier, scale, angle, H1, W1, Hp, Wp)`` -- the
@@ -367,20 +345,14 @@ def plan_items(image_shapes, params, model_params):
 def predict_batch(images, params, model, model_params, *, forward_batch: int, input_stage: Optional[str] = None):
     """``predict`` for several images at once: one ``(heatmap, paf)`` pair of ``DeviceMaps`` per image, in input order.
 
-    With one unrotated item per image at stride 4 (the reference's settings), images whose network inputs have the same
-    padded size ``(Hp, Wp)`` share forward passes of at most ``forward_batch`` images (``2 * forward_batch`` samples:
-    each image and its mirror), and one ``spg_postnet_ragged`` call runs the post-network stage of the whole batch,
-    reading each image's pair out of its forward pass in place.  The inputs are built per image as ``predict`` builds
-    them (``input_stage`` as there) into one tensor per size.
-
-    Any other ``scale_search x rotation_search`` at stride 4 (the reference's multi-scale and rotation search) is batched
-    the same way per item: the items of every image are grouped by padded input size (``plan_items``; an item's rotation
-    does not change its size), each size's forward passes take at most ``forward_batch`` items, and one
-    ``spg_postnet_ragged_items`` call averages every image's items.  The inputs are built per size with cv2
-    (``input_stage="host"``) or by one ``spg_prenet`` call per image that writes each item into its slot
-    (``"device"``).  A size's input tensor is released after its forward passes, but every network output lives until
-    the post-network call: at ``scale_search = [0.5, 1, 1.5, 2]``, boxsize 640, float32 that is about 100 MB per
-    480 x 640 image, and the device input stage holds about as much again of inputs until the forward passes.
+    At stride 4 the items of every image -- one per element of ``scale_search x rotation_search`` -- are grouped by
+    padded network input size (``plan_items``; an item's rotation does not change its size).  For each size in turn its
+    items' inputs are built into one tensor as ``predict`` builds them (``input_stage`` as there: cv2 on the host, or one
+    ``spg_prenet`` call per item that writes the item into its slot), forward passes take at most ``forward_batch``
+    items (``2 * forward_batch`` samples: each item and its mirror), and the tensor is released.  One
+    ``spg_postnet_ragged_items`` call then runs the post-network stage of the whole batch, reading each item's pair out
+    of its forward pass in place.  Every network output lives until that call: at ``scale_search = [0.5, 1, 1.5, 2]``,
+    boxsize 640, float32 that is about 100 MB per 480 x 640 image.
 
     Every kernel treats each image on its own, so the maps equal ``predict``'s bit for bit when the network's output for
     a sample does not depend on the batch it runs in (a network under cuDNN may pick another algorithm for another batch
@@ -389,91 +361,45 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     stage = _stage(_input_stage if input_stage is None else input_stage)
     fb = _forward_batch(forward_batch)
     images = list(images)
-    if not _single_item(params, model_params):
-        if int(model_params["stride"]) != 4:
-            return [predict(img, params, model, model_params, input_stage=stage) for img in images]
-        return _predict_batch_items(images, params, model, model_params, fb, stage)
-    md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
-    plan, buckets = plan_buckets([img.shape[:2] for img in images], params, model_params)
-    g = _grouper_many(len(images))
-    dev = f"cuda:{_device}"
-    entries = [None] * len(images)
-    for (Hp, Wp), idx in buckets.items():
-        k = len(idx)
-        x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
-        crops = []
-        if stage == "host":
-            host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
-            for j, i in enumerate(idx):
-                crops.append(_host_pair(images[i], plan[i][1], 0, model_params, out=host[2 * j:2 * j + 2].numpy())[1])
-            x.copy_(host, non_blocking=True)
-            _copied("pairs")
-        else:
-            for j, i in enumerate(idx):
-                img = images[i] if isinstance(images[i], torch.Tensor) else _upload_image(images[i])
-                (_, crop, _), = g.prenet(img.to(dev), [plan[i][0]], [0], max_downsample=md, pad_value=pv,
-                                         out=[x[2 * j:2 * j + 2]])
-                crops.append(crop)
-        for c0 in range(0, k, fb):
-            c1 = min(k, c0 + fb)
-            with torch.no_grad():
-                out = _network_output(model, x[2 * c0:2 * c1]).contiguous()
-            for j in range(c0, c1):
-                i = idx[j]
-                entries[i] = (out[2 * (j - c0):2 * (j - c0) + 2], crops[j], tuple(int(v) for v in images[i].shape[:2]))
-    maps = g.postnet_ragged(entries, nan_scrub=_variant == "demo")
-    return [(DeviceMaps(heat, False), DeviceMaps(paf, True)) for heat, paf in maps]
-
-
-def _predict_batch_items(images, params, model, model_params, fb: int, stage: str):
-    """``predict_batch`` for several items per image (or one rotated item) at stride 4; see there."""
-    import torch
-    if not images:
-        return []
+    if int(model_params["stride"]) != 4:
+        return [predict(img, params, model, model_params, input_stage=stage) for img in images]
     plan, buckets = plan_items([img.shape[:2] for img in images], params, model_params)
-    n_items = len(plan[0])
     g = _grouper_many(len(images))
     dev = f"cuda:{_device}"
-    crops = [[None] * n_items for _ in images]
-    reverses = [[None] * n_items for _ in images]
-    inputs = {}  # (Hp, Wp) -> [2 * items, Hp, Wp, 3] network input
-    if stage == "device":
-        md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
-        inputs = {(Hp, Wp): torch.empty((2 * len(members), Hp, Wp, 3), dtype=torch.float32, device=dev)
-                  for (Hp, Wp), members in buckets.items()}
-        slots = [[None] * n_items for _ in images]
-        for key, members in buckets.items():
-            for j, (i, t) in enumerate(members):
-                slots[i][t] = inputs[key][2 * j:2 * j + 2]
-        for i, image in enumerate(images):
-            img = image if isinstance(image, torch.Tensor) else _upload_image(image)
-            multiplier = [x * model_params["boxsize"] / image.shape[0] for x in params["scale_search"]]
-            for t, (_, crop, reverse) in enumerate(g.prenet(img.to(dev), multiplier, params["rotation_search"],
-                                                             max_downsample=md, pad_value=pv, out=slots[i])):
-                crops[i][t], reverses[i][t] = crop, reverse
-    entries = [[None] * n_items for _ in images]
-    for key, members in buckets.items():
+    md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
+    uploaded = {}  # device input stage: image index -> its uint8 CUDA image, from its first bucket to its last one
+    last = {i: key for key, members in buckets.items() for i, _ in members}
+    entries = [[None] * len(items) for items in plan]
+    for (Hp, Wp), members in buckets.items():
         k = len(members)
+        x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
+        built = []  # per member (crop, rotate_matrix_reverse)
         if stage == "host":
-            x = torch.empty((2 * k,) + key + (3,), dtype=torch.float32, device=dev)
             host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
             for j, (i, t) in enumerate(members):
                 _, scale, angle = plan[i][t][:3]
-                _, crops[i][t], reverses[i][t] = _host_pair(images[i], scale, angle, model_params,
-                                                            out=host[2 * j:2 * j + 2].numpy())
+                built.append(_host_pair(images[i], scale, angle, model_params, out=host[2 * j:2 * j + 2].numpy())[1:])
             x.copy_(host, non_blocking=True)
             _copied("pairs")
         else:
-            x = inputs.pop(key)
+            for j, (i, t) in enumerate(members):
+                if i not in uploaded:
+                    uploaded[i] = (images[i] if isinstance(images[i], torch.Tensor) else _upload_image(images[i])).to(dev)
+                multiplier, _, angle = plan[i][t][:3]
+                (_, crop, reverse), = g.prenet(uploaded[i], [multiplier], [angle], max_downsample=md, pad_value=pv,
+                                               out=[x[2 * j:2 * j + 2]])
+                built.append((crop, reverse))
+            for i in {i for i, _ in members if last[i] == (Hp, Wp)}:
+                del uploaded[i]
         for c0 in range(0, k, fb):
             c1 = min(k, c0 + fb)
             with torch.no_grad():
                 out = _network_output(model, x[2 * c0:2 * c1]).contiguous()
             for j in range(c0, c1):
                 i, t = members[j]
-                entries[i][t] = (out[2 * (j - c0):2 * (j - c0) + 2], crops[i][t], reverses[i][t])
+                entries[i][t] = (out[2 * (j - c0):2 * (j - c0) + 2],) + built[j]
         del x
-    maps = g.postnet_ragged_items([(entries[i], tuple(int(v) for v in img.shape[:2])) for i, img in enumerate(images)],
+    maps = g.postnet_ragged_items([(e, tuple(int(v) for v in img.shape[:2])) for e, img in zip(entries, images)],
                                   nan_scrub=_variant == "demo")
     return [(DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)) for heat, paf in maps]
 

@@ -641,57 +641,21 @@ class Grouper:
                        heat_chan0: Optional[int] = None, flip_paf_ord=None, flip_heat_ord=None, nan_scrub: bool = False,
                        stream=None):
         """``postnet`` for a batch of images of different sizes with one item each (one scale, no rotation) in one
-        asynchronous call (``spg_postnet_ragged``).
+        asynchronous call.
 
         ``images``: per image ``(net_out, (crop_h, crop_w), (H, W))`` -- ``net_out`` the ``[2, C, h, w]`` CUDA tensor of
         its pair (float32 / float16, one dtype per call; slices of a shared ``[2k, C, h, w]`` batch output work without
         copies).  ``outs``: optional per-image ``(heat, paf)`` contiguous tensors to write into.  Returns per image
         ``(heat [1,K,H,W] float32, paf [1,L,H,W])``, equal to what ``postnet`` returns for that image alone; ``paf`` is
         float32 by default (float32 storage of the float64 values, ``paf_as_f64=True`` for the grouping calls)."""
-        import torch
-        images = list(images)
-        if outs is not None and len(outs) != len(images):
-            raise GroupingError("one (heat, paf) output pair per image expected")
-        if len(images) > self.max_batch:
-            raise GroupingError(f"{len(images)} images, the handle was created for {self.max_batch}")
-        paf_dtype = torch.float32 if paf_dtype is None else paf_dtype
-        if paf_dtype not in (torch.float32, torch.float64):
-            raise GroupingError("paf_dtype must be float32 or float64")
-        heat_chan0 = self.L if heat_chan0 is None else heat_chan0
-        fp, fh = self._flip_orders(flip_paf_ord, flip_heat_ord)
-        dev = torch.device("cuda", self.device)
-        arr = (_PostnetImage * max(len(images), 1))()
-        net_dtype, results = None, []
-        for i, (o, (ch, cw), (H, W)) in enumerate(images):
-            H, W = int(H), int(W)
-            self._check_net_out(o, max(heat_chan0 + self.K, paf_chan0 + self.L), prefix=f"image {i}: ")
-            if net_dtype is not None and o.dtype != net_dtype:
-                raise GroupingError(f"image {i}: every network output of a call needs the same dtype")
-            net_dtype = o.dtype
-            if outs is not None:
-                heat, paf = outs[i]
-            else:
-                heat = torch.empty((1, self.K, H, W), dtype=torch.float32, device=dev)
-                paf = torch.empty((1, self.L, H, W), dtype=paf_dtype, device=dev)
-            if not (heat.is_contiguous() and paf.is_contiguous()) or heat.dtype != torch.float32 or paf.dtype != paf_dtype \
-                    or heat.numel() != self.K * H * W or paf.numel() != self.L * H * W:
-                raise GroupingError(f"image {i}: heat / paf outputs must be contiguous float32 [K,H,W] / {paf_dtype} [L,H,W]")
-            arr[i] = _PostnetImage(o.data_ptr(), o.stride(0), o.stride(1), o.shape[2], o.shape[3], int(ch), int(cw), H, W,
-                                   heat.data_ptr(), paf.data_ptr())
-            results.append((heat, paf))
-        common = _PostnetCommon(int(stride), int(paf_chan0), int(heat_chan0), fp.ctypes.data_as(C.POINTER(C.c_int32)),
-                                fh.ctypes.data_as(C.POINTER(C.c_int32)), int(bool(nan_scrub)),
-                                F16 if net_dtype == torch.float16 else F32)
-        rc = self._lib.spg_postnet_ragged(self._h, C.byref(common), arr, len(images),
-                                          F32 if paf_dtype == torch.float32 else F64, self._stream_ptr(stream))
-        _check(rc, "spg_postnet_ragged", self._h)
-        return results
+        return self._postnet_ragged([([(o, crop, None)], hw) for o, crop, hw in images], stride, paf_dtype, outs, paf_chan0,
+                                    heat_chan0, flip_paf_ord, flip_heat_ord, nan_scrub, stream)
 
     def postnet_ragged_items(self, images, *, paf_dtype=None, outs=None, paf_chan0: int = 0,
                              heat_chan0: Optional[int] = None, flip_paf_ord=None, flip_heat_ord=None,
                              nan_scrub: bool = False, stream=None):
         """``postnet`` for a batch of images of different sizes with several items each -- the multi-scale and rotation
-        search of ``predict()`` -- in one asynchronous call (``spg_postnet_ragged_items``, stride 4).
+        search of ``predict()`` -- in one asynchronous call (stride 4).
 
         ``images``: per image ``(items, (H, W))``; ``items``: per item of ``product(multiplier, rotate_angle)`` a
         ``(net_out, (crop_h, crop_w), rotate_matrix_reverse or None)`` triple -- what ``prenet`` returns with the
@@ -700,6 +664,13 @@ class Grouper:
         per-image ``(heat, paf)`` contiguous tensors to write into.  Returns per image ``(heat [1,K,H,W] float32,
         paf [1,L,H,W])``, equal to what ``postnet(..., rotations=...)`` returns for that image alone; ``paf`` is
         float64 for more than one item and float32 for a single one, as there."""
+        return self._postnet_ragged(images, 4, paf_dtype, outs, paf_chan0, heat_chan0, flip_paf_ord, flip_heat_ord,
+                                    nan_scrub, stream)
+
+    def _postnet_ragged(self, images, stride, paf_dtype, outs, paf_chan0, heat_chan0, flip_paf_ord, flip_heat_ord,
+                        nan_scrub, stream):
+        """``postnet_ragged_items`` at any ``stride`` (the C call rejects all but 4): one ``spg_postnet_ragged_items``
+        call.  Errors name ``image i``, or ``image i item t`` when the images have several items."""
         import torch
         images = list(images)
         if outs is not None and len(outs) != len(images):
@@ -732,9 +703,10 @@ class Grouper:
                     or heat.numel() != self.K * H * W or paf.numel() != self.L * H * W:
                 raise GroupingError(f"image {i}: heat / paf outputs must be contiguous float32 [K,H,W] / {paf_dtype} [L,H,W]")
             for t, (o, (ch, cw), m) in enumerate(items):
-                self._check_net_out(o, max(heat_chan0 + self.K, paf_chan0 + self.L), prefix=f"image {i} item {t}: ")
+                prefix = f"image {i}: " if n_items == 1 else f"image {i} item {t}: "
+                self._check_net_out(o, max(heat_chan0 + self.K, paf_chan0 + self.L), prefix=prefix)
                 if net_dtype is not None and o.dtype != net_dtype:
-                    raise GroupingError(f"image {i} item {t}: every network output of a call needs the same dtype")
+                    raise GroupingError(f"{prefix}every network output of a call needs the same dtype")
                 net_dtype = o.dtype
                 k = i * n_items + t
                 arr[k] = _PostnetImage(o.data_ptr(), o.stride(0), o.stride(1), o.shape[2], o.shape[3], int(ch), int(cw), H, W,
@@ -742,11 +714,11 @@ class Grouper:
                 if m is not None:
                     m = np.asarray(m, np.float64)
                     if m.shape != (2, 3):
-                        raise GroupingError(f"image {i} item {t}: a rotation matrix is 2x3")
+                        raise GroupingError(f"{prefix}a rotation matrix is 2x3")
                     rot[k] = _PostnetRotation(1, 0, (C.c_double * 6)(*m.reshape(6).tolist()))
                     any_rot = True
             results.append((heat, paf))
-        common = _PostnetCommon(4, int(paf_chan0), int(heat_chan0), fp.ctypes.data_as(C.POINTER(C.c_int32)),
+        common = _PostnetCommon(int(stride), int(paf_chan0), int(heat_chan0), fp.ctypes.data_as(C.POINTER(C.c_int32)),
                                 fh.ctypes.data_as(C.POINTER(C.c_int32)), int(bool(nan_scrub)),
                                 F16 if net_dtype == torch.float16 else F32)
         rc = self._lib.spg_postnet_ragged_items(self._h, C.byref(common), arr, rot if any_rot else None, len(images), n_items,

@@ -1,5 +1,6 @@
-"""GPU: ``dropin.predict_batch`` -- predict() for a batch of images: one forward pass per input size (in chunks of
-``forward_batch`` images) and one ragged post-network call -- against ``predict`` per image.
+"""GPU: ``dropin.predict_batch`` -- predict() for a batch of images, any ``scale_search x rotation_search``: one forward
+pass per chunk of ``forward_batch`` items of one input size and one ragged post-network call -- against ``predict`` per
+image.
 
 The network is a stand-in whose output for a sample does not depend on the batch it runs in: network-like maps keyed on
 the input size, plus a small term taken by indexing and scaling from the sample's own input (elementwise float32 is exact
@@ -14,6 +15,9 @@ from test_gpu_ragged import _stand_in_evaluate, _typed
 pytestmark = pytest.mark.gpu
 
 MODEL_PARAMS = dict(boxsize=160, stride=4, max_downsample=32, padValue=128)
+
+SEARCHES = {"1 item": ([1.0], [0.0]), "2 scales": ([1.0, 0.5], [0.0]), "5 scales": ([0.5, 1.0, 1.5, 2.0, 2.5], [0.0]),
+            "3 angles": ([1.0], [0.0, 30.0, -30.0]), "2 scales x 2 angles": ([1.0, 0.5], [0.0, 30.0])}
 
 
 class StandIn:
@@ -39,17 +43,17 @@ def env(cuda_device):
 
     dropin.configure(device=0, limbs=dropin.LIMBS)
     yield types.SimpleNamespace(torch=torch, dropin=dropin, skeleton=skeleton, synth=synth, dev=cuda_device)
-    dropin.configure(input_stage="host")
+    dropin.configure(input_stage="host", variant="evaluate")
 
 
 # boxsize 160: (120, 160), (60, 80), (90, 120) share a 160 x 224 input; (160, 120), (80, 60) a 160 x 128 one; images 160
-# rows high are identity items (crop == image)
+# rows high are identity items (crop == image) at scale 1
 SHAPES = [(120, 160), (160, 120), (60, 80), (160, 200), (90, 120), (80, 60), (160, 97), (150, 200), (33, 250), (160, 200)]
 
 
-def _images(seed=0):
+def _images(seed=0, shapes=SHAPES):
     rng = np.random.default_rng(seed)
-    return [rng.integers(0, 256, size=(H, W, 3), dtype=np.uint8) for H, W in SHAPES]
+    return [rng.integers(0, 256, size=(H, W, 3), dtype=np.uint8) for H, W in shapes]
 
 
 def _assert_maps_equal(got, want):
@@ -58,44 +62,80 @@ def _assert_maps_equal(got, want):
         for a, b, name in ((gh, wh, "heat"), (gp, wp, "paf")):
             assert a.as_f64 == b.as_f64 and a.shape == b.shape, f"image {i}: {name}"
             x, y = a.tensor.cpu().numpy(), b.tensor.cpu().numpy()
-            assert x.dtype == y.dtype and np.array_equal(x, y, equal_nan=True), f"image {i} {SHAPES[i]}: {name}"
+            assert x.dtype == y.dtype and np.array_equal(x, y, equal_nan=True), f"image {i}: {name}"
 
 
+def _expected_calls(buckets, forward_batch):
+    calls = []
+    for (Hp, Wp), members in buckets.items():
+        for c0 in range(0, len(members), forward_batch):
+            calls.append((2 * min(forward_batch, len(members) - c0), Hp, Wp, 3))
+    return calls
+
+
+@pytest.mark.parametrize("search", list(SEARCHES))
 @pytest.mark.parametrize("stage", ["host", "device"])
 @pytest.mark.parametrize("forward_batch", [2, 16])
-def test_predict_batch_equals_predict(env, stage, forward_batch):
+def test_predict_batch_equals_predict(env, search, stage, forward_batch):
     d, t = env.dropin, env.torch
-    params = dict(env.skeleton.default_params(), scale_search=[1.0], rotation_search=[0.0])
+    scales, angles = SEARCHES[search]
+    params = dict(env.skeleton.default_params(), scale_search=scales, rotation_search=angles)
     imgs = _images(1)
     model = StandIn(t, env.synth)
     want = [d.predict(img, params, model, MODEL_PARAMS, input_stage=stage) for img in imgs]
     model.calls.clear()
     got = d.predict_batch(imgs, params, model, MODEL_PARAMS, forward_batch=forward_batch, input_stage=stage)
     _assert_maps_equal(got, want)
-    # one forward pass per chunk of at most forward_batch images of one input size, sizes in order of first appearance
-    _, buckets = d.plan_buckets([im.shape[:2] for im in imgs], params, MODEL_PARAMS)
-    expect = []
-    for (Hp, Wp), idx in buckets.items():
-        for c0 in range(0, len(idx), forward_batch):
-            expect.append((2 * min(forward_batch, len(idx) - c0), Hp, Wp, 3))
-    assert model.calls == expect
-    assert any(len(idx) > 2 for idx in buckets.values()) and len(buckets) >= 3
+    # one forward pass per chunk of at most forward_batch items of one input size, sizes in order of first appearance
+    _, buckets = d.plan_items([im.shape[:2] for im in imgs], params, MODEL_PARAMS)
+    assert model.calls == _expected_calls(buckets, forward_batch)
+    assert any(len(m) > 2 for m in buckets.values()) and len(buckets) >= 3
 
 
-@pytest.mark.parametrize("params_update", [dict(scale_search=[1.0, 0.5], rotation_search=[0.0]),
-                                           dict(scale_search=[1.0], rotation_search=[0.0, 30.0])])
-def test_multi_item_configurations_run_predict_per_image(env, params_update):
+@pytest.mark.parametrize("params_update,stride", [(dict(scale_search=[1.0, 0.5], rotation_search=[0.0]), 4),
+                                                  (dict(scale_search=[1.0], rotation_search=[0.0, 30.0]), 4),
+                                                  (dict(scale_search=[1.0], rotation_search=[0.0]), 8),
+                                                  (dict(scale_search=[1.0, 0.5], rotation_search=[0.0]), 8)])
+def test_predict_batch_equals_predict_at_any_stride(env, params_update, stride):
+    """At stride 4 the items are batched; at another stride (no rotation there) every image runs ``predict``, one pair
+    per forward pass."""
     d, t = env.dropin, env.torch
     params = dict(env.skeleton.default_params(), **params_update)
+    model_params = dict(MODEL_PARAMS, stride=stride)
     imgs = _images(2)[:5]
     model = StandIn(t, env.synth)
+    want = [d.predict(img, params, model, model_params) for img in imgs]
+    model.calls.clear()
+    got = d.predict_batch(imgs, params, model, model_params, forward_batch=8)
+    _assert_maps_equal(got, want)
+    assert (max(c[0] for c in model.calls) > 2) == (stride == 4)
+
+
+def test_demo_variant(env):
+    d, t = env.dropin, env.torch
+    d.configure(variant="demo")
+    params = dict(env.skeleton.default_params(), scale_search=[1.0, 0.5, 1.5], rotation_search=[0.0, 30.0])
+    imgs = _images(4, SHAPES[:6])
+    model = StandIn(t, env.synth)
     want = [d.predict(img, params, model, MODEL_PARAMS) for img in imgs]
-    got = d.predict_batch(imgs, params, model, MODEL_PARAMS, forward_batch=8)
+    got = d.predict_batch(imgs, params, model, MODEL_PARAMS, forward_batch=4)
     _assert_maps_equal(got, want)
 
 
-@pytest.mark.parametrize("batch,forward_batch", [(3, 2), (16, 4)])
-def test_predict_many_with_forward_batch_equals_the_per_image_path(env, tmp_path, batch, forward_batch):
+def test_uint8_cuda_tensors_on_the_device_stage(env):
+    d, t = env.dropin, env.torch
+    params = dict(env.skeleton.default_params(), scale_search=[1.0, 0.5], rotation_search=[0.0, -30.0])
+    imgs = _images(5, SHAPES[:5])
+    model = StandIn(t, env.synth)
+    want = [d.predict(img, params, model, MODEL_PARAMS, input_stage="device") for img in imgs]
+    got = d.predict_batch([t.from_numpy(im).to(env.dev) for im in imgs], params, model, MODEL_PARAMS, forward_batch=3,
+                          input_stage="device")
+    _assert_maps_equal(got, want)
+
+
+@pytest.mark.parametrize("search,batch,forward_batch", [("1 item", 3, 2), ("1 item", 16, 4), ("2 scales", 6, 4),
+                                                        ("2 scales x 2 angles", 6, 4)])
+def test_predict_many_with_forward_batch_equals_the_per_image_path(env, tmp_path, search, batch, forward_batch):
     import cv2
     from improved_body_parts_b200 import wire
 
@@ -107,7 +147,8 @@ def test_predict_many_with_forward_batch_equals_the_per_image_path(env, tmp_path
         cv2.imwrite(str(tmp_path / f"{iid:012d}.png"), rng.integers(0, 255, size=(H, W, 3), dtype=np.uint8))
         coco.imgs[iid] = {"file_name": f"{iid:012d}.png"}
     ids = list(coco.imgs)[::-1]
-    params = dict(env.skeleton.default_params(), scale_search=[1.0], rotation_search=[0.0])
+    scales, angles = SEARCHES[search]
+    params = dict(env.skeleton.default_params(), scale_search=scales, rotation_search=angles)
     model = StandIn(env.torch, env.synth)
 
     mod = _stand_in_evaluate(env.skeleton, d)

@@ -62,17 +62,32 @@ def test_buckets_hold_every_item_once_in_first_appearance_order():
     assert b == {(640, 896): [(0, 0), (0, 1)], (320, 448): [(0, 2), (0, 3)]}
 
 
-def test_single_item_plan_agrees_with_plan_buckets():
+def test_bucket_planner_is_the_prenet_geometry():
+    """One item per image: (multiplier, scale, angle, H1, W1, Hp, Wp) equals cv2.resize's size (cvRound) and its
+    padding, the 2600 / 3800 clamp included, and images are bucketed by (Hp, Wp) in order of first appearance."""
     from improved_body_parts_b200 import dropin
 
-    shapes = _shapes()
-    for scale, md in ((1.0, 64), (0.5, 32), (2.0, 64), (1.3, 16)):
-        params = dict(scale_search=[scale], rotation_search=[0.0])
-        model_params = dict(boxsize=640, max_downsample=md, stride=4)
-        plan_b, buckets_b = dropin.plan_buckets(shapes, params, model_params)
-        plan_i, buckets_i = dropin.plan_items(shapes, params, model_params)
-        assert [p[:2] + p[3:] for (p,) in plan_i] == plan_b
-        assert [p[2] for (p,) in plan_i] == [0.0] * len(shapes)
-        assert {k: [i for i, t in v] for k, v in buckets_i.items()} == buckets_b
-        assert list(buckets_i) == list(buckets_b)
-        assert all(t == 0 for v in buckets_i.values() for _, t in v)
+    rng = np.random.default_rng(3)
+    shapes = [(480, 640), (640, 480), (427, 640), (640, 427), (612, 612), (375, 500), (640, 640), (1, 1), (3, 7000),
+              (5000, 20), (333, 333), (641, 639)] + [tuple(int(v) for v in rng.integers(1, 2000, 2)) for _ in range(200)]
+    for boxsize, scale_search, md in ((640, 1.0, 64), (368, 1.0, 8), (640, 0.5, 32), (640, 2.0, 64), (160, 1.3, 16)):
+        params = dict(scale_search=[scale_search], rotation_search=[0.0])
+        model_params = dict(boxsize=boxsize, max_downsample=md, stride=4)
+        plan, buckets = dropin.plan_items(shapes, params, model_params)
+        assert len(plan) == len(shapes)
+        seen = []
+        for i, (h, w) in enumerate(shapes):
+            multiplier = scale_search * boxsize / h
+            scale = pn.clamp_scale(multiplier, (h, w))
+            H1, W1 = pn.resized_size(h, w, scale)
+            Hp, Wp = -(-H1 // md) * md, -(-W1 // md) * md
+            assert plan[i] == [(multiplier, scale, 0.0, H1, W1, Hp, Wp)], (h, w, boxsize, scale_search, md)
+            assert (i, 0) in buckets[(Hp, Wp)]
+            if (Hp, Wp) not in seen:
+                seen.append((Hp, Wp))
+        assert list(buckets) == seen
+        assert sorted(m for ms in buckets.values() for m in ms) == [(i, 0) for i in range(len(shapes))]
+    # the reference's settings: images with one aspect ratio share an input size
+    _, b = dropin.plan_items([(480, 640), (240, 320), (640, 480), (960, 1280)],
+                             dict(scale_search=[1.0], rotation_search=[0.0]), dict(boxsize=640, max_downsample=64))
+    assert b == {(640, 896): [(0, 0), (1, 0), (3, 0)], (640, 512): [(2, 0)]}
