@@ -18,8 +18,12 @@
 // postnet_rot_kernel, on the padded grid (taps outside it read 0, not the pad value).  The pair is bit-identical to the
 // port's (tests/test_gpu_prenet.py).
 //
-// An unrotated item is one launch of prenet_kernel<false>: a thread computes one padded pixel straight from the source
-// and stores it to the image and to the mirror.  A rotated item first writes its padded uint8 image to the handle's
+// The stage is ragged: a launch covers many members -- one (scale, angle) item of one source image each -- whose
+// sources and padded sizes may all differ.  Each member has a descriptor (PreMember) in a table that travels as the
+// kernel parameter; grid.x walks each member's CTAs (one per kPreThreads pixels of one padded row) back to back, and a
+// CTA finds its member by binary search over the table's first_cta (post_ragged_image).  A CTA belongs to one member.
+// Unrotated members are one launch of prenet_kernel<false>: a thread computes one padded pixel straight from the source
+// and stores it to the image and to the mirror.  Rotated members first write their padded uint8 images to the handle's
 // scratch grid (prenet_resize_kernel); prenet_kernel<true> then warps from the grid.  Every output float is stored once.
 #pragma once
 
@@ -30,21 +34,42 @@ namespace spg {
 constexpr int kPreThreads = 128;
 constexpr int kPreLanes = 8;  // values per vector iteration of VResizeCubicVec_32s8u (v_int16 at the SSE baseline)
 
-struct PreArgs {
-    const unsigned char *src;      // [N] images of h rows of w x 3 bytes
-    long long img_stride, row_stride;  // bytes
+// One member: one item of one source image.
+struct PreMember {
+    const unsigned char *src;      // the source: h rows of w x 3 bytes
+    unsigned char *grid;           // rotated members: [Hp][Wp][3] the padded uint8 image (the handle's scratch)
+    float *out;                    // [2][Hp][Wp][3]
+    long long row_stride;          // bytes
+    double scale;                  // 1 / fx, either axis
+    double rot[6];                 // rotated members: the inverse of the forward matrix (output pixel -> padded grid)
     int h, w;                      // source size
     int H1, W1;                    // resized size (imageToTest)
     int Hp, Wp;                    // padded size
     int copy;                      // H1 == h and W1 == w: cv2.resize copies
     int n_body;                    // values of an interleaved resized row on the vector path: (W1 * 3) / 8 * 8
     int pad_value;
-    double scale;                  // 1 / fx, either axis
-    unsigned char *grid;           // rotated items: [N][Hp][Wp][3] the padded uint8 image
-    float *out;                    // [N][2][Hp][Wp][3]
-    long long out_stride;          // elements between images
-    double rot[6];                 // rotated items: the inverse of the forward matrix (output pixel -> padded grid)
+    int tiles_x;                   // CTAs per padded row: ceil(Wp / kPreThreads)
+    int first_cta;                 // the member's first grid.x position in its launch
 };
+
+// Members per launch: as many descriptors as fit in the 32 764 bytes of kernel parameters, so a call returns with nothing
+// of the caller's left to copy.
+constexpr int kPreParamBytes = 32764;
+constexpr int kPreMaxMembers = (int)((kPreParamBytes - 8) / sizeof(PreMember));
+struct PreRagged {
+    int n;                                // members of this launch
+    PreMember img[kPreMaxMembers];        // first_cta increasing
+};
+static_assert(sizeof(PreRagged) <= kPreParamBytes, "a launch's parameters fit the kernel-parameter limit");
+
+// the member of CTA blockIdx.x and the pixel (y, x) of its padded image this thread computes
+__device__ __forceinline__ const PreMember &prenet_member(const PreRagged &r, int &y, int &x) {
+    const PreMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const int cta = (int)blockIdx.x - a.first_cta;
+    y = cta / a.tiles_x;
+    x = (cta - y * a.tiles_x) * kPreThreads + (int)threadIdx.x;
+    return a;
+}
 
 // byte -> float32(byte / 255), the quotient rounded in double and then to float32 as numpy does
 __device__ __forceinline__ void prenet_lut(float *lut) {
@@ -53,7 +78,7 @@ __device__ __forceinline__ void prenet_lut(float *lut) {
 }
 
 // pixel (y, x) of the padded uint8 image of `img`: the resized image's or the pad value
-__device__ __forceinline__ void prenet_pixel(const PreArgs &a, const unsigned char *img, int y, int x, int v[3]) {
+__device__ __forceinline__ void prenet_pixel(const PreMember &a, const unsigned char *img, int y, int x, int v[3]) {
     if (y >= a.H1 || x >= a.W1) {
         v[0] = v[1] = v[2] = a.pad_value;
         return;
@@ -100,22 +125,24 @@ __device__ __forceinline__ void prenet_pixel(const PreArgs &a, const unsigned ch
     }
 }
 
-// rotated items: the padded uint8 image into the scratch grid
-__global__ void __launch_bounds__(kPreThreads) prenet_resize_kernel(PreArgs a) {
-    const int x = blockIdx.x * kPreThreads + threadIdx.x, y = blockIdx.y, n = blockIdx.z;
+// rotated members: the padded uint8 image into the scratch grid
+__global__ void __launch_bounds__(kPreThreads) prenet_resize_kernel(const __grid_constant__ PreRagged r) {
+    int y, x;
+    const PreMember &a = prenet_member(r, y, x);
     if (x >= a.Wp) return;
     int v[3];
-    prenet_pixel(a, a.src + n * a.img_stride, y, x, v);
-    unsigned char *g = a.grid + (((long long)n * a.Hp + y) * a.Wp + x) * 3;
+    prenet_pixel(a, a.src, y, x, v);
+    unsigned char *g = a.grid + ((long long)y * a.Wp + x) * 3;
     g[0] = (unsigned char)v[0]; g[1] = (unsigned char)v[1]; g[2] = (unsigned char)v[2];
 }
 
 // one pixel of the pair per thread: stored to the image at (y, x) and to the mirror at (y, Wp - 1 - x)
 template <bool ROT>
-__global__ void __launch_bounds__(kPreThreads) prenet_kernel(PreArgs a) {
+__global__ void __launch_bounds__(kPreThreads) prenet_kernel(const __grid_constant__ PreRagged r) {
     __shared__ float lut[256];
     prenet_lut(lut);
-    const int x = blockIdx.x * kPreThreads + threadIdx.x, y = blockIdx.y, n = blockIdx.z;
+    int y, x;
+    const PreMember &a = prenet_member(r, y, x);
     if (x >= a.Wp) return;
     float f[3];
     if (ROT) {
@@ -125,17 +152,16 @@ __global__ void __launch_bounds__(kPreThreads) prenet_kernel(PreArgs a) {
                        __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.rot[1], yd), a.rot[2]), 1024.0)) + 16;
         const int ys = __double2int_rn(__dmul_rn(__dmul_rn(a.rot[3], xd), 1024.0)) +
                        __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.rot[4], yd), a.rot[5]), 1024.0)) + 16;
-        const unsigned char *g = a.grid + (long long)n * a.Hp * a.Wp * 3;
 #pragma unroll
         for (int ch = 0; ch < 3; ch++)
-            f[ch] = warp_linear<3>(xs, ys, a.Wp, a.Hp, g + ch, 3 * a.Wp, 0, 0, [&](unsigned char v) { return lut[v]; });
+            f[ch] = warp_linear<3>(xs, ys, a.Wp, a.Hp, a.grid + ch, 3 * a.Wp, 0, 0, [&](unsigned char v) { return lut[v]; });
     } else {
         int v[3];
-        prenet_pixel(a, a.src + n * a.img_stride, y, x, v);
+        prenet_pixel(a, a.src, y, x, v);
         f[0] = lut[v[0]]; f[1] = lut[v[1]]; f[2] = lut[v[2]];
     }
-    float *o = a.out + n * a.out_stride + ((long long)y * a.Wp + x) * 3;
-    float *m = a.out + n * a.out_stride + ((long long)(a.Hp + y) * a.Wp + (a.Wp - 1 - x)) * 3;
+    float *o = a.out + ((long long)y * a.Wp + x) * 3;
+    float *m = a.out + ((long long)(a.Hp + y) * a.Wp + (a.Wp - 1 - x)) * 3;
     o[0] = f[0]; o[1] = f[1]; o[2] = f[2];
     m[0] = f[0]; m[1] = f[1]; m[2] = f[2];
 }

@@ -59,7 +59,7 @@ struct spg_handle {
     unsigned long long *armed_flag = nullptr;      // spg_arm_wire_signal: consumed by the next assemble launch
     unsigned long long armed_value = 0;
     Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
-    Scratch pre_grid;  // prenet: the padded uint8 images of a rotated item
+    Scratch pre_grid;  // prenet: the padded uint8 images of a launch's rotated members
     // the capacity-free tier (spg_group_unbounded): fixed-size words, tables sized by the peak counts, the candidate list
     // with the sort's scratch, the person table and outputs; `ub_ws` describes the last call's results
     Scratch ub_small, ub_peaks, ub_cands, ub_people;
@@ -1157,6 +1157,135 @@ int spg_postnet_ragged_items(spg_handle *h, const spg_postnet_common *cm, const 
 }
 
 // ---- pre-network stage -------------------------------------------------------------------------
+namespace {
+
+// One member's descriptor: the checks every item of spg_prenet and every member of spg_prenet_ragged passes (`what` and
+// `index` name it in the error) and the geometry of cv2.resize and util.padRightDownCorner.  The caller sets src and
+// row_stride.
+int prenet_member(spg_handle *h, const char *what, int index, int height, int width, int max_downsample, int pad_value,
+                  double scale, int rotate, int reserved, const double *matrix, float *out, PreMember &a) {
+    if (!std::isfinite(scale) || !(scale > 0)) return fail(h, SPG_E_INVALID, "%s %d: scale must be finite and positive", what, index);
+    if ((rotate != 0 && rotate != 1) || reserved != 0)
+        return fail(h, SPG_E_INVALID, "%s %d: rotate must be 0 or 1 and reserved 0", what, index);
+    for (int k = 0; k < 6; k++)
+        if (!std::isfinite(matrix[k])) return fail(h, SPG_E_INVALID, "%s %d: matrix entry %d is not finite", what, index, k);
+    const double rh = (double)height * scale, rw = (double)width * scale;  // dsize = saturate_cast<int>(size * fx)
+    if (!(rh < 32767.5 && rw < 32767.5)) return fail(h, SPG_E_INVALID, "%s %d: padded image above 32767 pixels a side", what, index);
+    a = PreMember{};
+    a.H1 = (int)std::nearbyint(rh);
+    a.W1 = (int)std::nearbyint(rw);
+    if (a.H1 < 1 || a.W1 < 1) return fail(h, SPG_E_INVALID, "%s %d: the resized image is empty (%dx%d)", what, index, a.H1, a.W1);
+    a.Hp = (a.H1 + max_downsample - 1) / max_downsample * max_downsample;
+    a.Wp = (a.W1 + max_downsample - 1) / max_downsample * max_downsample;
+    if (a.Hp > 32767 || a.Wp > 32767 || (long long)a.Hp * a.Wp * 3 > 0x7fffffffLL)
+        return fail(h, SPG_E_INVALID, "%s %d: padded image %dx%d above 32767 pixels a side or 2^31 values", what, index, a.Hp, a.Wp);
+    if (!out) return fail(h, SPG_E_INVALID, "%s %d: out is NULL", what, index);
+    a.h = height; a.w = width;
+    a.copy = a.H1 == height && a.W1 == width;  // cv2.resize: dsize == ssize is a copy
+    a.n_body = a.W1 * 3 / kPreLanes * kPreLanes;
+    a.pad_value = pad_value;
+    a.scale = 1.0 / scale;  // resize keeps scale = 1 / inv_scale, not src / dst
+    a.out = out;
+    a.tiles_x = (a.Wp + kPreThreads - 1) / kPreThreads;
+    if (rotate) invert_affine(matrix, a.rot);
+    return SPG_OK;
+}
+
+// The launches of validated members.  Unrotated members go in chunks of one prenet_kernel<false> launch; rotated ones in
+// chunks of a prenet_resize_kernel launch, which writes each member's padded uint8 image to its own part of the
+// handle's scratch grid (grown to the largest chunk's total), and a prenet_kernel<true> launch that warps from it.  A
+// chunk holds as many members as one launch's table; every chunk is planned and checked before the first launch.
+int prenet_launch(spg_handle *h, std::vector<PreMember> &ms, const std::vector<char> &rotated, cudaStream_t st) {
+    struct Chunk {
+        bool rot;
+        std::vector<int> members;
+    };
+    std::vector<Chunk> chunks;
+    std::vector<size_t> grid_at(ms.size());  // rotated members: the offset of the member's image in the scratch grid
+    size_t grid_need = 0;
+    for (int rot = 0; rot < 2; rot++) {
+        size_t grid_bytes = 0;
+        long long ctas = 0;
+        for (int i = 0; i < (int)ms.size(); i++) {
+            if (rotated[i] != rot) continue;
+            PreMember &a = ms[i];
+            if (chunks.empty() || chunks.back().rot != (rot != 0) || chunks.back().members.size() == (size_t)kPreMaxMembers) {
+                chunks.push_back(Chunk{rot != 0, {}});
+                grid_bytes = 0;
+                ctas = 0;
+            }
+            a.first_cta = (int)ctas;
+            ctas += (long long)a.tiles_x * a.Hp;
+            if (ctas > 0x7fffffffLL)
+                return fail(h, SPG_E_INVALID, "member %d: the %lld CTAs of its launch are above grid.x's 2^31 - 1", i, ctas);
+            if (rot) {
+                grid_at[i] = grid_bytes;
+                grid_bytes += (size_t)a.Hp * a.Wp * 3;
+                grid_need = std::max(grid_need, grid_bytes);
+            }
+            chunks.back().members.push_back(i);
+        }
+    }
+    if (chunks.empty()) return SPG_OK;
+    int rc;
+    if ((rc = grow(h, h->pre_grid, grid_need))) return rc;
+    for (const Chunk &c : chunks) {
+        PreRagged r{};
+        r.n = (int)c.members.size();
+        int x = 0;
+        for (int k = 0; k < r.n; k++) {
+            r.img[k] = ms[c.members[k]];
+            if (c.rot) r.img[k].grid = static_cast<unsigned char *>(h->pre_grid.p) + grid_at[c.members[k]];
+            x = r.img[k].first_cta + r.img[k].tiles_x * r.img[k].Hp;
+        }
+        const dim3 grid((unsigned)x);
+        if (c.rot) {
+            if ((rc = launch(h, kStagePrenet, "prenet_resize_kernel", prenet_resize_kernel, grid, kPreThreads, 0, st, r)) ||
+                (rc = launch(h, kStagePrenet, "prenet_kernel<true>", prenet_kernel<true>, grid, kPreThreads, 0, st, r)))
+                return rc;
+        } else if ((rc = launch(h, kStagePrenet, "prenet_kernel<false>", prenet_kernel<false>, grid, kPreThreads, 0, st, r))) {
+            return rc;
+        }
+    }
+    return SPG_OK;
+}
+
+int check_prenet_common(spg_handle *h, int32_t max_downsample, int32_t pad_value) {
+    if (max_downsample < 1 || max_downsample > 32767) return fail(h, SPG_E_INVALID, "max_downsample %d outside [1, 32767]", max_downsample);
+    if (pad_value < 0 || pad_value > 255) return fail(h, SPG_E_INVALID, "pad_value %d outside [0, 255]", pad_value);
+    return SPG_OK;
+}
+
+}  // namespace
+
+int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, const spg_prenet_member *members,
+                      int32_t n_members, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    if ((rc = check_prenet_common(h, max_downsample, pad_value))) return rc;
+    if (n_members < 0 || (n_members > 0 && !members)) return fail(h, SPG_E_INVALID, "members is NULL or n_members negative");
+    // validate every member before the first launch
+    std::vector<PreMember> ms((size_t)n_members);
+    std::vector<char> rotated((size_t)n_members);
+    for (int i = 0; i < n_members; i++) {
+        const spg_prenet_member &m = members[i];
+        if (m.height < 1 || m.width < 1 || m.height > 32767 || m.width > 32767)
+            return fail(h, SPG_E_INVALID, "member %d: image %dx%d outside [1, 32767]", i, m.height, m.width);
+        if (!m.image) return fail(h, SPG_E_INVALID, "member %d: image is NULL", i);
+        if (m.row_stride < 3LL * m.width) return fail(h, SPG_E_INVALID, "member %d: row_stride below width * 3", i);
+        if ((rc = prenet_member(h, "member", i, m.height, m.width, max_downsample, pad_value, m.scale, m.rotate, m.reserved,
+                                m.matrix, m.out, ms[i])))
+            return rc;
+        ms[i].src = m.image;
+        ms[i].row_stride = m.row_stride;
+        rotated[i] = (char)m.rotate;
+    }
+    if (n_members == 0) return SPG_OK;
+    DeviceGuard guard(h->device);
+    return prenet_launch(h, ms, rotated, static_cast<cudaStream_t>(stream));
+}
+
+// n_images x n_items members of one image size on the ragged path
 int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_t row_stride, int32_t n, int32_t height,
                int32_t width, int32_t max_downsample, int32_t pad_value, const spg_prenet_item *items, int32_t n_items,
                void *stream) {
@@ -1164,64 +1293,36 @@ int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_
     if (n < 0 || n > 65535) return fail(h, SPG_E_INVALID, "n_images %d outside [0, 65535]", n);
     if (height < 1 || width < 1 || height > 32767 || width > 32767)
         return fail(h, SPG_E_INVALID, "image %dx%d outside [1, 32767]", height, width);
-    if (max_downsample < 1 || max_downsample > 32767) return fail(h, SPG_E_INVALID, "max_downsample %d outside [1, 32767]", max_downsample);
-    if (pad_value < 0 || pad_value > 255) return fail(h, SPG_E_INVALID, "pad_value %d outside [0, 255]", pad_value);
+    int rc;
+    if ((rc = check_prenet_common(h, max_downsample, pad_value))) return rc;
     if (n_items < 0 || (n_items > 0 && !items)) return fail(h, SPG_E_INVALID, "items is NULL or n_items negative");
     if (n > 0 && !image) return fail(h, SPG_E_INVALID, "image_dev is NULL");
     if (row_stride < 3LL * width || image_stride < 0) return fail(h, SPG_E_INVALID, "row_stride below width * 3 or image_stride negative");
-    // validate every item before the first launch; the geometry is cv2.resize's and util.padRightDownCorner's
-    std::vector<PreArgs> args((size_t)n_items);
-    size_t grid_need = 0;
+    // validate every item before the first launch
+    std::vector<PreMember> ms;
+    std::vector<char> rotated;
+    ms.reserve((size_t)n * n_items);
+    rotated.reserve((size_t)n * n_items);
     for (int t = 0; t < n_items; t++) {
         const spg_prenet_item &it = items[t];
-        if (!std::isfinite(it.scale) || !(it.scale > 0)) return fail(h, SPG_E_INVALID, "item %d: scale must be finite and positive", t);
-        if ((it.rotate != 0 && it.rotate != 1) || it.reserved != 0)
-            return fail(h, SPG_E_INVALID, "item %d: rotate must be 0 or 1 and reserved 0", t);
-        for (int k = 0; k < 6; k++)
-            if (!std::isfinite(it.matrix[k])) return fail(h, SPG_E_INVALID, "item %d: matrix entry %d is not finite", t, k);
-        const double rh = (double)height * it.scale, rw = (double)width * it.scale;  // dsize = saturate_cast<int>(size * fx)
-        if (!(rh < 32767.5 && rw < 32767.5)) return fail(h, SPG_E_INVALID, "item %d: padded image above 32767 pixels a side", t);
-        PreArgs &a = args[t];
-        a.H1 = (int)std::nearbyint(rh);
-        a.W1 = (int)std::nearbyint(rw);
-        if (a.H1 < 1 || a.W1 < 1) return fail(h, SPG_E_INVALID, "item %d: the resized image is empty (%dx%d)", t, a.H1, a.W1);
-        a.Hp = (a.H1 + max_downsample - 1) / max_downsample * max_downsample;
-        a.Wp = (a.W1 + max_downsample - 1) / max_downsample * max_downsample;
-        if (a.Hp > 32767 || a.Wp > 32767 || (long long)a.Hp * a.Wp * 3 > 0x7fffffffLL)
-            return fail(h, SPG_E_INVALID, "item %d: padded image %dx%d above 32767 pixels a side or 2^31 values", t, a.Hp, a.Wp);
-        if (!it.out) return fail(h, SPG_E_INVALID, "item %d: out is NULL", t);
+        PreMember a;
+        if ((rc = prenet_member(h, "item", t, height, width, max_downsample, pad_value, it.scale, it.rotate, it.reserved, it.matrix,
+                                it.out, a)))
+            return rc;
         const long long pair = 2LL * a.Hp * a.Wp * 3;
         if (n > 1 && it.out_image_stride < pair)
             return fail(h, SPG_E_INVALID, "item %d: out_image_stride %lld below the pair's %lld elements", t, (long long)it.out_image_stride, pair);
-        a.src = image; a.img_stride = image_stride; a.row_stride = row_stride; a.h = height; a.w = width;
-        a.copy = a.H1 == height && a.W1 == width;  // cv2.resize: dsize == ssize is a copy
-        a.n_body = a.W1 * 3 / kPreLanes * kPreLanes;
-        a.pad_value = pad_value;
-        a.scale = 1.0 / it.scale;  // resize keeps scale = 1 / inv_scale, not src / dst
-        a.out = it.out; a.out_stride = it.out_image_stride;
-        if (it.rotate) {
-            invert_affine(it.matrix, a.rot);
-            grid_need = std::max(grid_need, (size_t)n * a.Hp * a.Wp * 3);
+        a.row_stride = row_stride;
+        for (int i = 0; i < n; i++) {
+            ms.push_back(a);
+            ms.back().src = image + (int64_t)i * image_stride;
+            ms.back().out = it.out + (int64_t)i * it.out_image_stride;
+            rotated.push_back((char)it.rotate);
         }
     }
-    if (n == 0 || n_items == 0) return SPG_OK;
+    if (ms.empty()) return SPG_OK;
     DeviceGuard guard(h->device);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc;
-    if ((rc = grow(h, h->pre_grid, grid_need))) return rc;
-    for (int t = 0; t < n_items; t++) {
-        PreArgs &a = args[t];
-        a.grid = static_cast<unsigned char *>(h->pre_grid.p);
-        const dim3 grid((unsigned)((a.Wp + kPreThreads - 1) / kPreThreads), (unsigned)a.Hp, (unsigned)n);
-        if (items[t].rotate) {
-            if ((rc = launch(h, kStagePrenet, "prenet_resize_kernel", prenet_resize_kernel, grid, kPreThreads, 0, st, a)) ||
-                (rc = launch(h, kStagePrenet, "prenet_kernel<true>", prenet_kernel<true>, grid, kPreThreads, 0, st, a)))
-                return rc;
-        } else if ((rc = launch(h, kStagePrenet, "prenet_kernel<false>", prenet_kernel<false>, grid, kPreThreads, 0, st, a))) {
-            return rc;
-        }
-    }
-    return SPG_OK;
+    return prenet_launch(h, ms, rotated, static_cast<cudaStream_t>(stream));
 }
 
 // ---- stages ------------------------------------------------------------------------------------

@@ -234,15 +234,26 @@ def _copied(slot: str) -> None:
     _staging[slot] = (_staging[slot][0], ev)
 
 
-def _upload_image(image: np.ndarray):
-    """Host uint8 ``[H, W, 3]`` image -> CUDA tensor, through a pinned buffer (one copy, async)."""
+def _upload_images(images) -> list:
+    """The ``[H, W, 3]`` uint8 CUDA image of every entry of ``images``: CUDA tensors as they are (on the current device),
+    host images packed into one pinned buffer and sent up with one asynchronous copy into one device buffer, of which
+    each gets a view."""
     import torch
-    arr = np.ascontiguousarray(image, np.uint8)
-    host = _pinned("image", arr.size, torch.uint8).view(arr.shape)
-    host.numpy()[...] = arr
-    dev = host.to(f"cuda:{_device}", non_blocking=True)
-    _copied("image")
-    return dev
+    dev = f"cuda:{_device}"
+    out = [img.to(dev) if isinstance(img, torch.Tensor) else None for img in images]
+    host_imgs = {i: np.ascontiguousarray(img, np.uint8) for i, img in enumerate(images) if out[i] is None}
+    if host_imgs:
+        host = _pinned("image", sum(a.size for a in host_imgs.values()), torch.uint8)
+        staged, at, off = host.numpy(), {}, 0
+        for i, a in host_imgs.items():
+            staged[off:off + a.size] = a.reshape(-1)
+            at[i] = off
+            off += a.size
+        packed = host.to(dev, non_blocking=True)
+        _copied("image")
+        for i, a in host_imgs.items():
+            out[i] = packed[at[i]:at[i] + a.size].view(a.shape)
+    return out
 
 
 def predict(image, params, model, model_params, heat_layers=None, paf_layers=None, input_image_path=None,
@@ -263,8 +274,7 @@ def predict(image, params, model, model_params, heat_layers=None, paf_layers=Non
     g = _grouper()
     multiplier = [x * model_params["boxsize"] / image.shape[0] for x in params["scale_search"]]
     if stage == "device":
-        img = image if isinstance(image, torch.Tensor) else _upload_image(image)
-        items = g.prenet(img.to(f"cuda:{_device}"), multiplier, params["rotation_search"],
+        items = g.prenet(_upload_images([image])[0], multiplier, params["rotation_search"],
                          max_downsample=int(model_params["max_downsample"]), pad_value=int(model_params["padValue"]))
     else:
         items = _host_items(image, multiplier, params["rotation_search"], model_params)
@@ -348,7 +358,8 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     At stride 4 the items of every image -- one per element of ``scale_search x rotation_search`` -- are grouped by
     padded network input size (``plan_items``; an item's rotation does not change its size).  For each size in turn its
     items' inputs are built into one tensor as ``predict`` builds them (``input_stage`` as there: cv2 on the host, or one
-    ``spg_prenet`` call per item that writes the item into its slot), forward passes take at most ``forward_batch``
+    ``spg_prenet_ragged`` call per size that writes every item into its slot; the call's host images go up together,
+    through one pinned buffer and one copy), forward passes take at most ``forward_batch``
     items (``2 * forward_batch`` samples: each item and its mirror), and the tensor is released.  One
     ``spg_postnet_ragged_items`` call then runs the post-network stage of the whole batch, reading each item's pair out
     of its forward pass in place.  Every network output lives until that call: at ``scale_search = [0.5, 1, 1.5, 2]``,
@@ -367,14 +378,13 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     g = _grouper_many(len(images))
     dev = f"cuda:{_device}"
     md, pv = int(model_params["max_downsample"]), int(model_params["padValue"])
-    uploaded = {}  # device input stage: image index -> its uint8 CUDA image, from its first bucket to its last one
-    last = {i: key for key, members in buckets.items() for i, _ in members}
+    uploaded = _upload_images(images) if stage == "device" else None
     entries = [[None] * len(items) for items in plan]
     for (Hp, Wp), members in buckets.items():
         k = len(members)
         x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
-        built = []  # per member (crop, rotate_matrix_reverse)
         if stage == "host":
+            built = []  # per member (crop, rotate_matrix_reverse)
             host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
             for j, (i, t) in enumerate(members):
                 _, scale, angle = plan[i][t][:3]
@@ -382,15 +392,9 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
             x.copy_(host, non_blocking=True)
             _copied("pairs")
         else:
-            for j, (i, t) in enumerate(members):
-                if i not in uploaded:
-                    uploaded[i] = (images[i] if isinstance(images[i], torch.Tensor) else _upload_image(images[i])).to(dev)
-                multiplier, _, angle = plan[i][t][:3]
-                (_, crop, reverse), = g.prenet(uploaded[i], [multiplier], [angle], max_downsample=md, pad_value=pv,
-                                               out=[x[2 * j:2 * j + 2]])
-                built.append((crop, reverse))
-            for i in {i for i, _ in members if last[i] == (Hp, Wp)}:
-                del uploaded[i]
+            pairs = g.prenet_ragged([(uploaded[i], plan[i][t][0], plan[i][t][2]) for i, t in members], max_downsample=md,
+                                    pad_value=pv, out=[x[2 * j:2 * j + 2] for j in range(k)])
+            built = [(crop, reverse) for _, crop, reverse in pairs]
         for c0 in range(0, k, fb):
             c1 = min(k, c0 + fb)
             with torch.no_grad():

@@ -75,6 +75,13 @@ class _PrenetItem(C.Structure):
                 ("out", C.c_void_p), ("out_image_stride", C.c_int64)]
 
 
+#: one ``spg_prenet_member`` (include/spgroup.h) per record: a ragged call fills hundreds of them, which a numpy record
+#: array takes without a Python object per member
+PRENET_MEMBER = np.dtype([("image", np.uint64), ("row_stride", np.int64), ("height", np.int32), ("width", np.int32),
+                          ("scale", np.float64), ("rotate", np.int32), ("reserved", np.int32), ("matrix", np.float64, (6,)),
+                          ("out", np.uint64)], align=True)
+
+
 class _ImageMaps(C.Structure):
     _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
                 ("paf_chan_stride", C.c_int64), ("height", C.c_int32), ("width", C.c_int32), ("image_extent", C.c_double)]
@@ -112,6 +119,7 @@ _PROTOTYPES = {
     "spg_postnet_ragged_items": (_int, [_ptr, _P(_PostnetCommon), _P(_PostnetImage), _P(_PostnetRotation), _i32, _i32, _i32,
                                         _ptr]),
     "spg_prenet": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _P(_PrenetItem), _i32, _ptr]),
+    "spg_prenet_ragged": (_int, [_ptr, _i32, _i32, _ptr, _i32, _ptr]),  # members: a PRENET_MEMBER array
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -185,6 +193,21 @@ def input_geometry(h: int, w: int, scale: float, max_downsample: int) -> Tuple[i
     H1, W1 = int(np.rint(h * scale)), int(np.rint(w * scale))
     md = int(max_downsample)
     return H1, W1, -(-H1 // md) * md, -(-W1 // md) * md
+
+
+def prenet_item(h: int, w: int, scale: float, angle: float, max_downsample: int):
+    """One pre-network item of an ``h x w`` image (evaluate.py:94-110): ``(scale, (H1, W1, Hp, Wp), forward, reverse)``
+    -- the scale after the clamp of :94-96, the crop and padded network input sizes of :98-100 (zeros for a scale that
+    is not finite and positive, which the library rejects), and for ``angle != 0`` the forward 2x3 matrix warpAffine
+    takes and the reverse one ``postnet`` takes (the centre's x and y swapped as at :108-110), else ``None`` twice."""
+    scale = clamp_scale(float(scale), (h, w))
+    geo = input_geometry(h, w, scale, max_downsample) if np.isfinite(scale) and scale > 0 else (0, 0, 0, 0)
+    forward = reverse = None
+    if angle != 0:
+        import cv2
+        centre = (geo[2] / 2, geo[3] / 2)
+        forward, reverse = cv2.getRotationMatrix2D(centre, angle, 1), cv2.getRotationMatrix2D(centre, -angle, 1)
+    return scale, geo, forward, reverse
 
 
 def _vp(a: Optional[np.ndarray]):
@@ -761,24 +784,11 @@ class Grouper:
         if out is not None and len(out) != len(pairs):
             raise GroupingError("one output tensor per item expected")
         items = (_PrenetItem * max(len(pairs), 1))()
-        dev = torch.device("cuda", self.device)
         results = []
         for t, (scale, angle) in enumerate(pairs):
-            scale = clamp_scale(float(scale), (h, w))
-            # the library checks the scale and the geometry; this only sizes the output
-            H1, W1, Hp, Wp = input_geometry(h, w, scale, md) if np.isfinite(scale) and scale > 0 else (0, 0, 0, 0)
-            forward = reverse = None
-            if angle != 0:  # evaluate.py:108-110, the centre's x and y swapped as there
-                import cv2
-                centre = (Hp / 2, Wp / 2)
-                forward, reverse = cv2.getRotationMatrix2D(centre, angle, 1), cv2.getRotationMatrix2D(centre, -angle, 1)
-            if out is not None:
-                o = out[t] if batched else out[t][None]
-                if o.dtype != torch.float32 or not o.is_cuda or o.device.index != self.device or \
-                        tuple(o.shape) != (N, 2, max(Hp, 0), max(Wp, 0), 3) or not o[0].is_contiguous():
-                    raise GroupingError(f"out[{t}] must be a float32 [N,2,{Hp},{Wp},3] CUDA tensor with contiguous images")
-            else:
-                o = torch.empty((N, 2, max(Hp, 0), max(Wp, 0), 3), dtype=torch.float32, device=dev)
+            scale, (H1, W1, Hp, Wp), forward, reverse = prenet_item(h, w, scale, angle, md)
+            o = self._prenet_out(None if out is None else out[t] if batched else out[t][None], (N, 2, Hp, Wp, 3),
+                                 f"out[{t}]", f"[N,2,{Hp},{Wp},3] CUDA tensor with contiguous images")
             m = (C.c_double * 6)(*(np.asarray(forward, np.float64).reshape(6).tolist() if forward is not None else [0.0] * 6))
             items[t] = _PrenetItem(scale, int(forward is not None), 0, m, o.data_ptr(), o.stride(0))
             results.append((o if batched else o[0], (H1, W1), reverse))
@@ -786,6 +796,52 @@ class Grouper:
                                   self._stream_ptr(stream))
         _check(rc, "spg_prenet", self._h)
         return results
+
+    def prenet_ragged(self, members, *, max_downsample: int, pad_value: int, out=None, stream=None):
+        """``prenet`` for images of different sizes, each with its own items, in one asynchronous call.
+
+        ``members``: per member ``(image, scale, angle)`` -- ``image`` a ``[H, W, 3]`` uint8 CUDA tensor (BGR as read)
+        with contiguous rows, ``scale`` a ``multiplier`` entry (clamped as at evaluate.py:94-96) and ``angle`` a
+        ``rotate_angle`` entry; several members may read one image.  ``out``: optional per-member ``[2, Hp, Wp, 3]``
+        float32 contiguous tensors to write into (slices of one batch tensor work).  Returns per member the
+        ``(pair, crop, rotate_matrix_reverse)`` triple ``prenet`` returns for that image and item alone."""
+        import torch
+        members = list(members)
+        if out is not None and len(out) != len(members):
+            raise GroupingError("one output tensor per member expected")
+        md, pv = int(max_downsample), int(pad_value)
+        if md < 1:
+            raise GroupingError("max_downsample must be >= 1")
+        arr = np.zeros(max(len(members), 1), PRENET_MEMBER)
+        results = []
+        for i, (image, scale, angle) in enumerate(members):
+            if not getattr(image, "is_cuda", False) or image.dtype != torch.uint8 or image.dim() != 3:
+                raise GroupingError(f"member {i}: image must be a [H,W,3] uint8 CUDA tensor")
+            if image.device.index != self.device:
+                raise GroupingError(f"member {i}: image lives on cuda:{image.device.index}, the handle on cuda:{self.device}")
+            h, w, cn = (int(v) for v in image.shape)
+            if cn != 3 or image.stride(2) != 1 or image.stride(1) != 3:
+                raise GroupingError(f"member {i}: image must have 3 channels and contiguous rows")
+            scale, (H1, W1, Hp, Wp), forward, reverse = prenet_item(h, w, scale, angle, md)
+            o = self._prenet_out(None if out is None else out[i], (2, Hp, Wp, 3), f"out[{i}]",
+                                 f"contiguous [2,{Hp},{Wp},3] CUDA tensor")
+            arr[i] = (image.data_ptr(), image.stride(0), h, w, scale, int(forward is not None), 0,
+                      np.zeros(6) if forward is None else np.asarray(forward, np.float64).reshape(6), o.data_ptr())
+            results.append((o, (H1, W1), reverse))
+        rc = self._lib.spg_prenet_ragged(self._h, md, pv, arr.ctypes.data, len(members), self._stream_ptr(stream))
+        _check(rc, "spg_prenet_ragged", self._h)
+        return results
+
+    def _prenet_out(self, o, shape, name, form):
+        """A pre-network output of ``shape`` on the handle's device: ``o`` checked (the leading pair contiguous), or a new
+        tensor for ``None``."""
+        import torch
+        if o is None:
+            return torch.empty(shape, dtype=torch.float32, device=torch.device("cuda", self.device))
+        if o.dtype != torch.float32 or not o.is_cuda or o.device.index != self.device or tuple(o.shape) != shape or \
+                not o[(0,) * (len(shape) - 4)].is_contiguous():
+            raise GroupingError(f"{name} must be a float32 {form}")
+        return o
 
     # -- stages -------------------------------------------------------------------------------------
     def nms_peaks(self, heat, params=None, stream=None) -> None:

@@ -278,6 +278,25 @@ typedef struct spg_prenet_item {
 int spg_prenet(spg_handle *h, const uint8_t *image_dev, int64_t image_stride, int64_t row_stride, int32_t n_images,
                int32_t height, int32_t width, int32_t max_downsample, int32_t pad_value, const spg_prenet_item *items,
                int32_t n_items, void *stream);
+/* One member of a ragged pre-network call: one (scale, angle) item of one image. */
+typedef struct spg_prenet_member {
+    const uint8_t *image;       /* [height][width][3] uint8 device image (BGR as read), rows row_stride bytes apart */
+    int64_t row_stride;         /* >= width * 3 */
+    int32_t height, width;
+    double scale;               /* as spg_prenet_item */
+    int32_t rotate;             /* as spg_prenet_item */
+    int32_t reserved;           /* 0 */
+    double matrix[6];           /* as spg_prenet_item */
+    float *out;                 /* [2][Hp][Wp][3] float32: the image, then its mirror */
+} spg_prenet_member;
+/* spg_prenet for members of different image sizes, scales and angles in one call (a batch of images of different sizes,
+ * each with its own items): member i's pair equals the one spg_prenet gives for that image and item alone.  Every member
+ * is validated before the first launch (spg_prenet's rules per member; SPG_E_INVALID names the first bad one as
+ * "member i").  Asynchronous on `stream`; `members` may be reused as soon as the call returns.  The scratch grid of
+ * rotated members grows on demand to the total of Hp * Wp * 3 bytes of the rotated members of one launch (up to a few
+ * hundred members). */
+int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, const spg_prenet_member *members,
+                      int32_t n_members, void *stream);
 
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */

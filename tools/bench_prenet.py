@@ -13,7 +13,13 @@ Per setting it prints
     input_stage="host" against "device".
 and the card's name and power limit.
 
-usage: python tools/bench_prenet.py [--iters 50] [--out profiles/prenet/bench_prenet.json]"""
+The ragged setting (--only ragged, or all) builds the inputs of a batch as dropin.predict_batch does: the 16 COCO-shaped
+images of tools/bench_predict_batch.py at boxsize 640, grouped by network input size (dropin.plan_items), each member
+written into its slot of its size's batch tensor, under [1] x [0] and [0.5, 1, 1.5, 2] x [0, 30, -30].  It compares one
+spg_prenet call per member against one spg_prenet_ragged call per input size: call time from CUDA events, kernel time
+from torch.profiler in a separate pass, launches per batch, and the bytes-over-3.35 TB/s floor as a share of the kernels.
+
+usage: python tools/bench_prenet.py [--iters 50] [--only all|single|ragged] [--out profiles/prenet/bench_prenet.json]"""
 import argparse
 import itertools
 import json
@@ -26,8 +32,10 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 HBM_BPS = 3.35e12
+RAGGED_SETTINGS = [([1.0], [0.0]), ([0.5, 1.0, 1.5, 2.0], [0.0, 30.0, -30.0])]
 SETTINGS = [([1.0], [0.0]), ([1.0], [0.0, 30.0, -30.0]), ([0.5, 1.0, 1.5, 2.0], [0.0]), ([0.5, 1.0, 1.5, 2.0], [0.0, 30.0, -30.0])]
 MODEL_PARAMS = dict(boxsize=640, stride=4, max_downsample=64, padValue=128)
 
@@ -67,9 +75,89 @@ def stand_in_model(x):
     return [[y.expand(2, 50, y.shape[2], y.shape[3]).contiguous()]]
 
 
+def timed(fn, iters, g):
+    """(ms per call from CUDA events, {kernel: ms per call} from torch.profiler, launches per call) of fn()."""
+    import torch
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(iters):
+        fn()
+    end.record()
+    end.synchronize()
+    call_ms = start.elapsed_time(end) / iters
+    launches = g._lib.spg_launch_count(g._h)
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+    launches = (g._lib.spg_launch_count(g._h) - launches) / iters
+    kernels = {}
+    for ev in prof.key_averages():
+        if "prenet" in ev.key:
+            us = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+            kernels[ev.key.split("(")[0]] = us / 1e3 / iters
+    return call_ms, kernels, launches
+
+
+def ragged(iters, name, power):
+    """The ragged setting: per-member spg_prenet calls against one spg_prenet_ragged call per network input size."""
+    import torch
+
+    from bench_predict_batch import SHAPES
+    from improved_body_parts_b200 import dropin, skeleton
+    from improved_body_parts_b200.grouping import Grouper
+    rng = np.random.default_rng(2029)  # the first 16 images of tools/bench_predict_batch.py
+    images = [rng.integers(0, 256, size=SHAPES[int(rng.integers(len(SHAPES)))] + (3,), dtype=np.uint8) for _ in range(16)]
+    dev_imgs = [torch.from_numpy(im).cuda() for im in images]
+    g = Grouper(max_batch=16, device=0)
+    results = []
+    for scale_search, angles in RAGGED_SETTINGS:
+        params = dict(skeleton.default_params(), scale_search=scale_search, rotation_search=angles)
+        plan, buckets = dropin.plan_items([im.shape[:2] for im in images], params, MODEL_PARAMS)
+        xs = {key: torch.empty((2 * len(m), key[0], key[1], 3), dtype=torch.float32, device="cuda") for key, m in buckets.items()}
+        nbytes = 0
+        for (Hp, Wp), members in buckets.items():
+            for i, t in members:
+                # the pair written, the source read once; a rotated member's uint8 grid written and read
+                nbytes += 2 * Hp * Wp * 3 * 4 + images[i].size + (2 * Hp * Wp * 3 if plan[i][t][2] != 0 else 0)
+
+        def per_member():
+            for key, members in buckets.items():
+                for j, (i, t) in enumerate(members):
+                    g.prenet(dev_imgs[i], [plan[i][t][0]], [plan[i][t][2]], max_downsample=64, pad_value=128,
+                             out=[xs[key][2 * j:2 * j + 2]])
+
+        def one_per_size():
+            for key, members in buckets.items():
+                g.prenet_ragged([(dev_imgs[i], plan[i][t][0], plan[i][t][2]) for i, t in members], max_downsample=64,
+                                pad_value=128, out=[xs[key][2 * j:2 * j + 2] for j in range(len(members))])
+
+        r = dict(setting="ragged", scale_search=scale_search, rotation_search=angles, images=16,
+                 members=sum(len(m) for m in buckets.values()), input_sizes=len(buckets), bytes=nbytes,
+                 hbm_floor_ms=nbytes / HBM_BPS * 1e3, device=name, power_limit=power)
+        for label, fn in (("per_member", per_member), ("ragged", one_per_size)):
+            call_ms, kernels, launches = timed(fn, iters, g)
+            kern_ms = sum(kernels.values())
+            r[label] = dict(call_ms=call_ms, kernel_ms=kern_ms, kernels=kernels, launches=launches,
+                            share_of_hbm=r["hbm_floor_ms"] / kern_ms)
+            print(f"ragged {scale_search} x {angles}: {r['members']} members in {len(buckets)} input sizes, {label}: "
+                  f"call {call_ms:.3f} ms, kernels {kern_ms:.4f} ms ({launches:g} launches; "
+                  + ", ".join(f"{k} {v:.4f}" for k, v in kernels.items())
+                  + f"), floor {r['hbm_floor_ms']:.4f} ms = {r['hbm_floor_ms'] / kern_ms:.2f} of HBM")
+        sys.stdout.flush()
+        results.append(r)
+        del xs
+    g.close()
+    return results
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--only", default="all", choices=("all", "single", "ragged"))
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "prenet", "bench_prenet.json"),
                     help="JSON results (default under profiles/, which git ignores)")
     args = ap.parse_args()
@@ -85,9 +173,9 @@ def main():
     image = rng.integers(0, 256, (480, 640, 3), dtype=np.uint8)
     dev_img = torch.from_numpy(image).cuda()
     params = dict(skeleton.default_params())
-    results = []
+    results = ragged(args.iters, name, power) if args.only in ("all", "ragged") else []
     g = Grouper(max_batch=1, device=0)
-    for scale_search, angles in SETTINGS:
+    for scale_search, angles in SETTINGS if args.only in ("all", "single") else []:
         multiplier = [x * 640 / 480 for x in scale_search]
         items = g.prenet(dev_img, multiplier, angles, max_downsample=64, pad_value=128)
         outs = [p for p, _, _ in items]
