@@ -23,7 +23,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import wire
+from . import sharding, wire
 from .grouping import Grouper, GroupingError, clamp_scale, input_geometry
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
@@ -639,19 +639,43 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
     ``forward_batch > 1`` runs ``predict_batch`` on each group of ``batch`` images instead of ``predict`` per image, for
     any ``scale_search`` and ``rotation_search`` at stride 4 (see there for when its maps equal ``predict``'s).  A
     non-zero status raises ``GroupingError``.  ``image_name(coco, image_id)`` gives the file name (default: ``coco.imgs[image_id]['file_name']``, evaluate.py:546-547).  ``process()``
-    is not called, so the reference's ``batch_time`` meter is not updated."""
-    import os
+    is not called, so the reference's ``batch_time`` meter is not updated.
 
-    import cv2
+    In an initialised ``torch.distributed`` world of N > 1 processes (one per GPU) this is rank 0's call, and the other
+    ranks run ``serve_predict_many``: the images are sharded over the ranks in contiguous blocks
+    (``sharding.shard_range``), each rank runs its block exactly as above, and rank 0 returns the same dict a single
+    process returns.  A block that raises on any rank raises ``GroupingError`` here, naming the rank and the image."""
     assert (not set(validation_ids).difference(set(coco.getImgIds())))
     if int(batch) < 1:
         raise ValueError("batch must be >= 1")
     fb = _forward_batch(forward_batch)
+    names = [image_name(coco, iid) if image_name is not None else coco.imgs[iid]["file_name"] for iid in validation_ids]
+    rank, world = sharding._world()
+    if world == 1:
+        return _predict_block(images_directory, list(zip(validation_ids, names)), params, model, model_params,
+                              heat_layers, paf_layers, int(batch), fb)
+    if rank != 0:
+        raise RuntimeError(f"predict_many runs on rank 0; rank {rank} of {world} calls serve_predict_many")
+    import os
+    return _predict_sharded(dict(images_directory=os.path.abspath(images_directory), ids=list(validation_ids),
+                                 names=names, params=params, model_params=model_params, heat_layers=heat_layers,
+                                 paf_layers=paf_layers, batch=int(batch), forward_batch=fb), model)
+
+
+def _predict_block(images_directory, named_ids, params, model, model_params, heat_layers, paf_layers, batch: int,
+                   fb: int, at: Optional[list] = None) -> dict:
+    """The body of ``predict_many`` over ``named_ids`` = ``[(image_id, file name)]``: ``{image_id: people}`` in that
+    order.  ``at`` (a list) is kept holding the ids of the image or grouping batch being worked on, for error reports."""
+    import os
+
+    import cv2
+    at = [] if at is None else at
     keypoints = {}
     pending = []  # (image_id, (heatmap, paf) -- or the image itself for predict_batch, oriImg.shape[0])
 
     def flush():
         if pending:
+            at[:] = [iid for iid, _, _ in pending]  # the batch's ragged calls fail as one
             maps = [m for _, m, _ in pending]
             if fb > 1:
                 maps = predict_batch(maps, dict(params), model, dict(model_params), forward_batch=fb)
@@ -660,8 +684,8 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
                 keypoints[iid] = kp
             pending.clear()
 
-    for image_id in validation_ids:
-        name = image_name(coco, image_id) if image_name is not None else coco.imgs[image_id]["file_name"]
+    for image_id, name in named_ids:
+        at[:] = [image_id]
         path = os.path.join(images_directory, name)
         ori = cv2.imread(path)  # B,G,R order (evaluate.py:502)
         if fb > 1:
@@ -669,10 +693,69 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
         else:
             pending.append((image_id, predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path),
                             ori.shape[0]))
-        if len(pending) >= int(batch):
+        if len(pending) >= batch:
             flush()
     flush()
     return keypoints
+
+
+def _run_job(job: dict, model, rank: int, world: int):
+    """This rank's block of ``job``: its ``{image_id: people}``, or, if the block raised, the text that says where and
+    why (sent in place of the dict, so that the gather completes on every rank)."""
+    lo, hi = sharding.shard_range(len(job["ids"]), rank, world)
+    at: list = []
+    try:
+        return _predict_block(job["images_directory"], list(zip(job["ids"][lo:hi], job["names"][lo:hi])), job["params"],
+                              model, job["model_params"], job["heat_layers"], job["paf_layers"], job["batch"],
+                              job["forward_batch"], at)
+    except Exception as e:  # noqa: BLE001 -- any failure of the block is reported to rank 0, which raises it
+        where = f"image {at[0]}" if len(at) == 1 else f"images {at}"
+        return f"{where}: {type(e).__name__}: {e}"
+
+
+def _predict_sharded(job: dict, model) -> dict:
+    """Rank 0 of ``predict_many`` in a world of N > 1: broadcast the job, run block 0, gather every rank's dict."""
+    import torch.distributed as dist
+    rank, world = sharding._world()
+    dist.broadcast_object_list([job], src=0)
+    mine = _run_job(job, model, rank, world)
+    blocks: List[object] = [None] * world
+    dist.gather_object(mine, blocks, dst=0)
+    failed = [f"rank {r}, {b}" for r, b in enumerate(blocks) if isinstance(b, str)]
+    if failed:
+        raise GroupingError("predict_many failed on " + "; ".join(failed))
+    keypoints = {}
+    for b in blocks:  # rank order is image order: the blocks are contiguous
+        keypoints.update(b)
+    return keypoints
+
+
+def serve_predict_many(model) -> None:
+    """Ranks other than 0 of a ``torch.distributed`` world: run this rank's block of every ``predict_many`` call of
+    rank 0 with the network ``model`` on this rank's device (``configure(device=local_rank)``), send rank 0 its
+    ``{image_id: people}`` (or the text of the exception its block raised), and return at the empty job that
+    ``end_serving`` on rank 0 broadcasts."""
+    import torch.distributed as dist
+    rank, world = sharding._world()
+    if rank == 0:
+        raise RuntimeError("serve_predict_many runs on the ranks other than 0")
+    while True:
+        job = [None]
+        dist.broadcast_object_list(job, src=0)
+        if not job[0]:
+            return
+        dist.gather_object(_run_job(job[0], model, rank, world), None, dst=0)
+
+
+def end_serving() -> None:
+    """Rank 0: broadcast the empty job that makes ``serve_predict_many`` return on the other ranks (call it once rank 0
+    is done with ``predict_many``, also when it raised).  Nothing to do in a world of one process."""
+    import torch.distributed as dist
+    rank, world = sharding._world()
+    if world > 1:
+        if rank != 0:
+            raise RuntimeError("end_serving runs on rank 0")
+        dist.broadcast_object_list([None], src=0)
 
 
 def keypoints(subset, candidate):
@@ -729,7 +812,10 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     groups ``batch`` images per call; it uses the module's ``posenet`` and ``get_image_name`` and leaves the module's
     ``batch_time`` meter alone.  ``forward_batch > 1`` (with ``device_predict`` and ``batch > 1``) makes that
     ``predict_many`` run the network on up to ``forward_batch`` items (images, or with a multi-scale or rotation search
-    their scaled and rotated copies) of the same input size at once (``predict_batch``)."""
+    their scaled and rotated copies) of the same input size at once (``predict_batch``).  In an initialised
+    ``torch.distributed`` world of N > 1 processes, one per GPU, each with ``configure(device=local_rank)``, that
+    ``predict_many`` shards the images over the ranks: rank 0 calls it (``evaluate.validation()``), the other ranks
+    run ``serve_predict_many`` until rank 0 calls ``end_serving``."""
     if int(batch) > 1 and not device_predict:
         raise ValueError("batch > 1 needs device_predict=True: the batched grouping takes the maps predict() leaves on the device")
     fb = _forward_batch(forward_batch)

@@ -3,6 +3,7 @@
 
     python tools/run_evaluate_b200.py --reference /path/to/Improved-Body-Parts [--config utils/config] [--check] [--batch N]
                                       [--forward-batch M]
+    torchrun --nproc-per-node G tools/run_evaluate_b200.py --reference ... --batch N [--forward-batch M] --gpus G
 
 What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is never modified:
 
@@ -25,6 +26,12 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
 ``prepare()`` returns the module; building ``evaluate.posenet`` (``:626-641``: checkpoint + apex amp) and calling
 ``evaluate.validation(...)`` is then exactly what ``evaluate.__main__`` does.  With ``--check`` the launcher runs one
 synthetic image through ``evaluate``'s own call sequence (``:509-511``) on the GPU and prints what it found.
+
+With ``--gpus G`` (``prepare(..., gpus=G)``), every one of the G processes torchrun starts joins the process group, is
+pinned to its ``LOCAL_RANK`` device and installs the ``predict_many`` that shards the images over the ranks.  Each rank
+then builds ``evaluate.posenet`` on its device and calls ``validate(evaluate, ...)``: rank 0 runs
+``evaluate.validation()`` unchanged, the other ranks serve their blocks of its ``predict_many``.  ``--check`` runs on
+every rank, on that rank's device.
 """
 from __future__ import annotations
 
@@ -62,9 +69,42 @@ def _stub_missing() -> list:
     return stubbed
 
 
+def gpus_error(gpus: int, batch: int):
+    """Why ``--gpus gpus`` cannot run here, or None: it needs ``batch > 1`` (the sharded path is the batched
+    ``predict_many``) and a ``torchrun --nproc-per-node gpus`` environment."""
+    if batch < 2:
+        return "--gpus needs --batch > 1"
+    if "LOCAL_RANK" not in os.environ or os.environ.get("WORLD_SIZE") != str(gpus):
+        return f"--gpus {gpus} runs under torchrun --nproc-per-node {gpus} (WORLD_SIZE={os.environ.get('WORLD_SIZE')})"
+    return None
+
+
+def init_ranks() -> int:
+    """One process per GPU under torchrun: pin this process to ``LOCAL_RANK`` and join the process group (NCCL for CUDA
+    tensors, gloo for the CPU objects ``predict_many`` broadcasts and gathers); returns the local rank."""
+    import torch
+    import torch.distributed as dist
+    local = int(os.environ["LOCAL_RANK"])
+    torch.cuda.set_device(local)
+    if not dist.is_initialized():
+        dist.init_process_group(backend="cuda:nccl,cpu:gloo")
+    return local
+
+
 def prepare(reference_root: str, config_path: str = None, device: int = None, install: bool = True,
-            replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1):
-    """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites."""
+            replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1, gpus: int = None):
+    """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites.
+
+    ``gpus=G`` (under ``torchrun --nproc-per-node G``, with ``batch > 1``) joins the process group, pins this rank to
+    its ``LOCAL_RANK`` device and installs the ``predict_many`` that shards the images over the G ranks; run
+    ``validate`` on every rank."""
+    if gpus is not None:
+        err = gpus_error(int(gpus), int(batch))
+        if err:
+            raise ValueError(err)
+        if device is not None:
+            raise ValueError("gpus= takes each rank's device from LOCAL_RANK: pass no device")
+        device = init_ranks()
     reference_root = os.path.abspath(reference_root)
     if not os.path.isfile(os.path.join(reference_root, "evaluate.py")):
         raise FileNotFoundError(f"no evaluate.py under {reference_root}")
@@ -104,6 +144,21 @@ def prepare(reference_root: str, config_path: str = None, device: int = None, in
     return evaluate
 
 
+def validate(evaluate, **kwargs):
+    """``evaluate.validation(evaluate.posenet, **kwargs)`` on rank 0, which returns its result; on every other rank,
+    ``dropin.serve_predict_many(evaluate.posenet)``, which runs that rank's share of ``predict_many`` and returns None.
+    Each rank builds ``evaluate.posenet`` on its own device first, as ``evaluate.__main__`` does (``:626-641``).  In a
+    single process this is ``evaluate.validation(...)``."""
+    from improved_body_parts_b200 import dropin, sharding
+    if sharding._world()[0] != 0:
+        dropin.serve_predict_many(evaluate.posenet)
+        return None
+    try:
+        return evaluate.validation(evaluate.posenet, **kwargs)
+    finally:
+        dropin.end_serving()  # the other ranks return, also when validation raised
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reference", default=os.environ.get("SPG_REFERENCE_ROOT"), required="SPG_REFERENCE_ROOT" not in os.environ,
@@ -115,6 +170,8 @@ def main() -> None:
                     help="images per grouping call in predict_many (> 1 implies the device predict; default 1)")
     ap.add_argument("--forward-batch", type=int, default=1,
                     help="images per network forward pass in predict_many (> 1 needs --batch > 1; default 1)")
+    ap.add_argument("--gpus", type=int, default=None,
+                    help="under torchrun --nproc-per-node G: shard predict_many's images over the G GPUs (needs --batch > 1)")
     a = ap.parse_args()
     if a.batch < 1:
         ap.error("--batch must be >= 1")
@@ -122,8 +179,17 @@ def main() -> None:
         ap.error("--forward-batch must be >= 1")
     if a.forward_batch > 1 and a.batch < 2:
         ap.error("--forward-batch > 1 needs --batch > 1")
-    ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch)
-    print(f"evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
+    if a.gpus is not None:
+        if a.gpus < 1:
+            ap.error("--gpus must be >= 1")
+        if a.device is not None:
+            ap.error("--gpus takes each rank's device from LOCAL_RANK: drop --device")
+        err = gpus_error(a.gpus, a.batch)
+        if err:
+            ap.error(err)
+    ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch, gpus=a.gpus)
+    rank = f"rank {os.environ['RANK']}: " if a.gpus is not None else ""
+    print(f"{rank}evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
           f"find_peaks -> {ev.find_peaks.__module__}.{ev.find_peaks.__name__}")
     if a.check:
         import numpy as np
@@ -133,8 +199,11 @@ def main() -> None:
         peaks = ev.find_peaks(hw, ev.params)                                   # evaluate.py:509
         conns, special = ev.find_connections(peaks, pw, hw.shape[0], ev.params)  # :510
         subset, candidate = ev.find_people(conns, special, peaks, ev.params)    # :511
-        print(f"check: {sum(len(p) for p in peaks)} peaks, {sum(len(c) for c in conns if len(c))} connections, "
+        print(f"{rank}check: {sum(len(p) for p in peaks)} peaks, {sum(len(c) for c in conns if len(c))} connections, "
               f"{len(subset)} persons")
+    if a.gpus is not None:
+        import torch.distributed as dist
+        dist.destroy_process_group()
 
 
 if __name__ == "__main__":
