@@ -76,6 +76,11 @@ constexpr uint32_t kStRowOverflow = 1u << 2;
 constexpr uint32_t kStSampleIndex = 1u << 3;
 constexpr uint32_t kStAssert = 1u << 4;
 constexpr uint32_t kStWireOverflow = 1u << 5;
+constexpr uint32_t kStNonfinite = 1u << 6;
+constexpr uint32_t kStNanPriority = 1u << 7;
+// Scorer-internal, never published: a candidate of the limb has a NaN priority.  publish_limb turns it into
+// kStNanPriority when the limb has another candidate to be sorted against.
+constexpr uint32_t kStNanPrioCand = 1u << 31;
 
 struct Params {
     double thre1, thre2, connect_ration, len_rate, connection_tole, min_mean_score;

@@ -115,11 +115,11 @@ __global__ void __launch_bounds__(kUbScoreThreads) ub_score_kernel(UbArgs u, Sco
     const size_t slot = (size_t)k * capP + i;
     const int64_t out = WRITE ? u.row_off[slot] : 0;
     int nc = 0;
-    bool bad = false;
+    uint32_t flags = 0;
     for (int j = 0; j < nB; j++) {
         double score, prio;
         const bool ok = score_pair_exact<T, 1, TA>(plane, H, W, sa, g, i, j, ain && inside_map(g.bx[j], g.by[j], H, W), thre2,
-                                                   score, prio, bad);
+                                                   score, prio, flags);
         if (ok) {
             if (WRITE) {
                 const int64_t o = out + nc;
@@ -133,7 +133,9 @@ __global__ void __launch_bounds__(kUbScoreThreads) ub_score_kernel(UbArgs u, Sco
         }
     }
     if (!WRITE) u.row_count[slot] = nc;
-    if (bad) atomicOr(ws.status, kStSampleIndex);
+    // a NaN priority is judged per limb, by ub_match_kernel, once the limb's candidate count is known
+    flags &= ~kStNanPrioCand;
+    if (flags) atomicOr(ws.status, flags);
 }
 
 // Greedy acceptance of limb k's candidates in priority order (:263-270), one thread per limb.
@@ -149,6 +151,12 @@ __global__ void ub_match_kernel(UbArgs u) {
     if (nA == 0 || nB == 0) {  // special_k (:272-274)
         ws.conn_count[k] = -1;
         return;
+    }
+    // a NaN priority among two or more candidates: the reference's sort order (:259) is not reproduced
+    if (c1 - c0 > 1) {
+        bool nan_prio = false;
+        for (int64_t c = c0; c < c1; c++) nan_prio |= isnan(ws.cand_prio[c]);
+        if (nan_prio) atomicOr(ws.status, kStNanPriority);
     }
     unsigned char *usedA = u.used + (size_t)k * 2 * capP, *usedB = usedA + capP;
     const int lim = min(nA, nB);

@@ -131,17 +131,25 @@ struct PairGeom {  // one limb's end-point lists in shared memory
     const double *rcp;  // rcp[d] = RN(1/d), d = 1 .. mid_num-1
 };
 
-// Phase B: the reference's evaluation of one pair (evaluate.py:224-255).  Returns true if it is a candidate.
+// Phase B: the reference's evaluation of one pair (evaluate.py:224-255).  Returns true if it is a candidate.  `flags`
+// collects what the reference would raise for -- kStNonfinite (a non-finite pair length: round() at :226 raises),
+// kStSampleIndex (a sample outside the map: :235 raises) -- and kStNanPrioCand for a candidate with a NaN priority.
 // kExactBatch: samples of the exact evaluation whose index computations and loads are in flight together (register budget)
 // T: the type the plane is STORED in; TA: the type the reference's arithmetic runs in (TA = double with T = float is
 // SPG_F32_AS_F64: float64 maps whose values are exact float32 numbers, the single-scale output of predict()).
 template <typename T, int kExactBatch = 1, typename TA = T>
 __device__ __forceinline__ bool score_pair_exact(const T *__restrict__ plane, int H, int W, const ScoreArgs &a,
                                                  const PairGeom &g, int i, int j, bool interior, TA thre2,
-                                                 double &score, double &prio, bool &bad) {
+                                                 double &score, double &prio, uint32_t &flags) {
     const double ax = g.ax[i], ay = g.ay[i], bx = g.bx[j], by = g.by[j];
     const double vx = __dsub_rn(bx, ax), vy = __dsub_rn(by, ay);                            // :224
     const double n2 = __dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy));
+    // a NaN or infinite end point (or a length past DBL_MAX): int(round(norm + 1)) at :226 raises before the norm == 0
+    // test.  Returning here also keeps a NaN position away from every index computation below.
+    if (!isfinite(n2)) {
+        flags |= kStNonfinite;
+        return false;
+    }
     if (n2 == 0.0) return false;                             // norm == 0 (:228-230); sqrt(x) == 0 iff x == 0
     // norm = sqrt(n2) (:225) is only materialised when a decision needs it:
     //  - m = min(round(norm + 1), mid_num) (:226): n2 >= mid_num^2 implies norm >= mid_num, hence m = mid_num;
@@ -233,7 +241,7 @@ __device__ __forceinline__ bool score_pair_exact(const T *__restrict__ plane, in
             if (yi < 0) yi += H;  // numpy index semantics: negatives wrap once
             if (xi < 0) xi += W;
             if (yi < 0 || yi >= H || xi < 0 || xi >= W) {  // the reference would raise IndexError
-                bad = true;
+                flags |= kStSampleIndex;
                 return false;
             }
             const TA v = (TA)plane[(size_t)yi * W + xi];
@@ -258,6 +266,7 @@ __device__ __forceinline__ bool score_pair_exact(const T *__restrict__ plane, in
     const double need = __dmul_rn(a.connect_ration, (double)m);
     const bool crit1 = a.crit1_strict ? (double)above > need : (double)above >= need;       // :246 (demo_image.py:288: `>`)
     const bool crit2 = score > 0.0;                                                         // :251
+    if (crit1 && crit2 && isnan(prio)) flags |= kStNanPrioCand;
     return crit1 && crit2;
 }
 
@@ -276,10 +285,13 @@ __device__ __forceinline__ void store_candidate(const Workspace &ws, size_t out_
     }
 }
 
-// Publishes limb `slot` of image n: candidate count (-1 = special_k), survivors of the screen, status bits.
+// Publishes limb `slot` of image n: candidate count (-1 = special_k), survivors of the screen, status bits (`flags` as
+// score_pair_exact collects them: a NaN priority matters only when the limb has another candidate to sort it against).
 __device__ __forceinline__ void publish_limb(const Workspace &ws, int n, size_t slot, int ncand, int nsurv, uint32_t flags) {
     ws.cand_count[slot] = min(ncand, ws.capC);
     if (ws.surv_count) ws.surv_count[slot] = nsurv;
+    if ((flags & kStNanPrioCand) && ncand > 1) flags |= kStNanPriority;
+    flags &= ~kStNanPrioCand;
     if (ncand > ws.capC) flags |= kStCandOverflow;
     if (flags) atomicOr(&ws.status[n], flags);
 }
@@ -475,9 +487,9 @@ __device__ __forceinline__ void limb_score_plane(const ScoreArgs &a, const Works
         const int i = nB > 1 ? (int)__umulhi((uint32_t)p, magic) : p;
         const int j = p - i * nB;
         double score, prio;
-        bool bad = false;
-        const bool ok = score_pair_exact<T, 1, TA>(plane, H, W, a, g, i, j, s_ain[i] && s_bin[j], thre2_exact, score, prio, bad);
-        if (bad) atomicOr(&s_flags, kStSampleIndex);
+        uint32_t flags = 0;
+        const bool ok = score_pair_exact<T, 1, TA>(plane, H, W, a, g, i, j, s_ain[i] && s_bin[j], thre2_exact, score, prio, flags);
+        if (flags) atomicOr(&s_flags, flags);
         if (ok) {
             const int pos = atomicAdd(&s_count, 1);  // warp-aggregated by ptxas (REDUX + one ATOMS)
             if (pos < ws.capC) store_candidate<TA>(ws, out_base, pos, i, j, score, prio);

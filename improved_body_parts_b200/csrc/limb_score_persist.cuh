@@ -331,9 +331,9 @@ __global__ void __launch_bounds__(kPersistThreads, 1) limb_score_persist_kernel(
             const int jj = p - i * nB;
             PairGeom g{ps.ax, ps.ay, ps.bx, ps.by, ps.as, ps.bs, s_rcp};
             double score, prio;
-            bool bad = false;
-            const bool ok = score_pair_exact<T, 10, TA>(plane, H, W, a, g, i, jj, ps.ain[i] && ps.bin[jj], thre2_exact, score, prio, bad);
-            if (bad) atomicOr(&ms.flags, kStSampleIndex);
+            uint32_t flags = 0;
+            const bool ok = score_pair_exact<T, 10, TA>(plane, H, W, a, g, i, jj, ps.ain[i] && ps.bin[jj], thre2_exact, score, prio, flags);
+            if (flags) atomicOr(&ms.flags, flags);
             if (ok) {
                 const size_t out_base = ((size_t)h.n * L + h.k) * ws.capC;
                 const int pos = atomicAdd(&ms.ncand, 1);

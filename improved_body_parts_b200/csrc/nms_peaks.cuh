@@ -14,6 +14,8 @@
 // nms_peaks_banded.cuh): the 8-neighbour test, the peak finisher, the scanners' pass 1 and their role constants.
 #pragma once
 
+#include <cfloat>
+
 #include "common.cuh"
 
 namespace spg {
@@ -29,8 +31,11 @@ struct NmsArgs {
 constexpr int kNmsThreads = 256;
 constexpr int kNmsBufs = 3;  // band ring: two bands in flight while one is scanned
 
+// The peak rule of util.py:182 + evaluate.py:193: np.nonzero(heat * keep).  A non-finite pixel is always a peak (NaN * 0,
+// inf * 0 and -inf * 0 are all NaN, never 0); a finite one needs keep = 1 -- v >= thre, no value in its clipped 3x3
+// window greater than v or NaN (torch's max-pool propagates NaN) -- and v != 0 (-0.0 * 1 is a zero).
 __device__ __forceinline__ bool nms_is_peak(const float *buf, int lo, int H, int W, int y, int x, float v, float thr) {
-    // keep = (hmax == heat) & (heat >= thre); np.nonzero(heat * keep) drops exact zeros
+    if (!isfinite(v)) return true;
     if (!(v >= thr) || v == 0.0f) return false;
 #pragma unroll
     for (int dy = -1; dy <= 1; dy++) {
@@ -111,10 +116,10 @@ __device__ __forceinline__ void nms_test_group(const float *rows, int y, int x0,
 #pragma unroll
     for (int e = 0; e < 4; e++) {
         const float v = C[e + 1];
-        // keep = (hmax == heat) & (heat >= thre) (util.py:182); np.nonzero(heat * keep) drops exact zeros.
-        // "all neighbours <= v" (not fmax) so that a NaN neighbour vetoes the peak like torch's max-pool
-        const bool pk = (v >= thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
-                        (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v);
+        // nms_is_peak's rule.  "all neighbours <= v" (not fmax) so that a NaN neighbour vetoes a finite peak like torch's
+        // max-pool; a non-finite v is a peak whatever its neighbours
+        const bool pk = !isfinite(v) | ((v >= thr) & (v != 0.0f) & (U[e] <= v) & (U[e + 1] <= v) & (U[e + 2] <= v) &
+                                        (C[e] <= v) & (C[e + 2] <= v) & (D[e] <= v) & (D[e + 1] <= v) & (D[e + 2] <= v));
         if (pk) {
             const int pos = atomicAdd(cnt, 1);
             if (pos < capP) list[pos] = (uint32_t)(y * W + x0 + e);
@@ -168,6 +173,15 @@ constexpr int kNmsPLists = 2 * kNmsPFinishers;
 constexpr int kNmsPScanners = kNmsPThreads / 32 - 1 - kNmsPFinishers;  // 28
 constexpr int kNmsPMaxIter = 5;  // 32-lane passes of pass 1 over a scanner's share of a plane or band
 
+// Pass 1's vote on one float4 group: true if the group may hold a peak -- a value that reaches thre1, or a non-finite
+// one (a peak whatever its value).  fmaxf drops NaN and -inf never reaches thre1, so the max alone would miss both; the
+// sum of magnitudes is NaN or inf when any value is (or when finite values overflow: a harmless extra vote, pass 2
+// decides).
+__device__ __forceinline__ bool nms_group_vote(float4 c4, float thr) {
+    const float mag = fabsf(c4.x) + fabsf(c4.y) + fabsf(c4.z) + fabsf(c4.w);
+    return (fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= thr) | !(mag <= FLT_MAX);
+}
+
 // Pass 1 of a persistent scanner: the float4 groups g = g0 + it * g_step + lane (it < ITER, g < g_end) of `data` that
 // reach thre1 are queued in `wq`, warp-aggregated, in group order.  First only the votes (one load, three max, one
 // compare, one ballot per 128 elements -- the common case is an empty mask), then the queue from the masks.  Returns the
@@ -180,8 +194,7 @@ __device__ __forceinline__ int nms_queue_groups(const float *data, int g0, int g
         const int g = g0 + it * g_step + lane;
         bool act = false;
         if (g < g_end) {
-            const float4 c4 = *reinterpret_cast<const float4 *>(data + 4 * (size_t)g);
-            act = fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= thr;
+            act = nms_group_vote(*reinterpret_cast<const float4 *>(data + 4 * (size_t)g), thr);
         }
         am[it] = __ballot_sync(0xffffffffu, act);
     }
@@ -293,8 +306,7 @@ __device__ __forceinline__ void nms_peaks_plane(const NmsArgs &a, int n_local, i
                 const int g = g0 + lane;
                 bool act = false;
                 if (g < g_hi) {
-                    const float4 c4 = *reinterpret_cast<const float4 *>(buf + (size_t)(y0 - lo) * W + 4 * (size_t)g);
-                    act = fmaxf(fmaxf(c4.x, c4.y), fmaxf(c4.z, c4.w)) >= a.thr;
+                    act = nms_group_vote(*reinterpret_cast<const float4 *>(buf + (size_t)(y0 - lo) * W + 4 * (size_t)g), a.thr);
                 }
                 const uint32_t am = __ballot_sync(0xffffffffu, act);
                 if (act) wq[nq + __popc(am & ((1u << lane) - 1u))] = (uint16_t)g;

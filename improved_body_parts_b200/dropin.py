@@ -24,7 +24,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import sharding, wire
-from .grouping import Grouper, GroupingError, clamp_scale, input_geometry
+from .grouping import ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -105,9 +105,12 @@ def _params(params):
 
 
 def _check_status(status: int) -> None:
+    status = int(status)
     if status:
-        raise GroupingError(f"grouping capacity exceeded or invalid sample index (status {status:#x}); "
-                            f"capacities: {CAP_PEAKS} peaks/part, {CAP_CANDS} candidates/limb, {CAP_ROWS} person rows")
+        why = [text for bit, text in ST_MEANING.items() if status & bit]
+        raise GroupingError(f"grouping failed (status {status:#x}): " + ("; ".join(why) if why else
+                            f"capacity exceeded; capacities: {CAP_PEAKS} peaks/part, {CAP_CANDS} candidates/limb, "
+                            f"{CAP_ROWS} person rows"))
 
 
 #: status bits of an image that went past the handle's capacities (SPG_ST_PEAK_OVERFLOW | SPG_ST_CAND_OVERFLOW |

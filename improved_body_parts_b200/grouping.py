@@ -22,6 +22,16 @@ LIB_PATH = os.path.join(_HERE, "libspgroup.so")
 ABI_VERSION = 2
 
 ST_PEAK_OVERFLOW, ST_CAND_OVERFLOW, ST_ROW_OVERFLOW, ST_SAMPLE_INDEX, ST_ASSERT, ST_WIRE_OVERFLOW = 1, 2, 4, 8, 16, 32
+ST_NONFINITE, ST_NAN_PRIORITY = 64, 128
+#: what the reference does where a status bit is set (the bits of the conditions it would raise for, and the one whose
+#: outputs it computes in an order that is not reproduced)
+ST_MEANING = {ST_SAMPLE_INDEX: "SAMPLE_INDEX: a line sample index outside the map (the reference raises IndexError, "
+                               "evaluate.py:235)",
+              ST_ASSERT: "ASSERT: a keypoint shared by two persons (the reference raises at evaluate.py:437-439)",
+              ST_NONFINITE: "NONFINITE: a limb pair with a non-finite length (the reference raises ValueError, "
+                            "evaluate.py:226)",
+              ST_NAN_PRIORITY: "NAN_PRIORITY: a NaN candidate priority among others (the reference's sort order at "
+                               "evaluate.py:259 is undefined)"}
 F32, F64, F32_AS_F64, F16 = 0, 1, 2, 3
 
 

@@ -47,7 +47,13 @@ enum {
     SPG_ST_SAMPLE_INDEX = 1u << 3,   /* a line sample fell outside the map: the reference would  */
                                      /* raise IndexError at evaluate.py:235                      */
     SPG_ST_ASSERT = 1u << 4,         /* the reference would raise at evaluate.py:437-439         */
-    SPG_ST_WIRE_OVERFLOW = 1u << 5   /* more persons than the wire record holds (rows beyond are dropped) */
+    SPG_ST_WIRE_OVERFLOW = 1u << 5,  /* more persons than the wire record holds (rows beyond are dropped) */
+    SPG_ST_NONFINITE = 1u << 6,      /* a limb pair has a non-finite length (an end point with a NaN or infinite  */
+                                     /* coordinate, from a non-finite map value inside its refinement box): the   */
+                                     /* reference would raise ValueError / OverflowError at evaluate.py:226       */
+    SPG_ST_NAN_PRIORITY = 1u << 7    /* a limb with two or more candidates has one with a NaN priority (a border */
+                                     /* peak with a NaN score, or +inf + -inf): the reference's sort at           */
+                                     /* evaluate.py:259 orders unordered keys, which is not reproduced            */
 };
 
 /* dtype of the body-part planes.  predict() accumulates them in float64 (evaluate.py:86,161); with a single scale
@@ -146,8 +152,8 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n_imag
  * image itself, bit-identical to the reference as the bounded path is: peaks -> connections -> people of `image` (its
  * maps, size and image_extent) on `stream`.  The host sizes each stage's tables from the previous stage's counts, so the
  * call synchronises `stream` three times; the tables belong to the handle, grow on demand and live until spg_destroy.
- * The tier's status word carries SPG_ST_SAMPLE_INDEX and SPG_ST_ASSERT as the bounded path sets them, never a capacity
- * bit.  Its own limits -- at most 65535 peaks per part ((i, j) of a connection are packed in 16 bits each), 32767
+ * The tier's status word carries SPG_ST_SAMPLE_INDEX, SPG_ST_ASSERT, SPG_ST_NONFINITE and SPG_ST_NAN_PRIORITY as the
+ * bounded path sets them, never a capacity bit.  Its own limits -- at most 65535 peaks per part ((i, j) of a connection are packed in 16 bits each), 32767
  * accepted connections per image (the person table has one row per connection) and 2^31 - 1 candidates -- and a failed
  * allocation make the call return an error, never undefined output.  Maps: 2 <= height, width <= 32767; the handle's
  * max_h / max_w do not apply. */

@@ -69,6 +69,11 @@ def resize_cubic(src: np.ndarray, dsize: Optional[Tuple[int, int]] = None, fx: f
     else:
         W, H = int(dsize[0]), int(dsize[1])
         sx, sy = 1.0 / (W / w), 1.0 / (H / h)  # inv_scale = dst/src; scale = 1/inv_scale (two roundings, as OpenCV)
+    if (W, H) == (w, h):
+        # resize.cpp: `if (dsize == ssize) { src.copyTo(dst); return; }` -- not the [0, 1, 0, 0] taps, which would turn
+        # an infinite neighbour into NaN (inf * 0)
+        out = a.copy()
+        return out[:, :, 0] if squeeze else out
     ix, ax = _axis_table(W, w, sx)
     iy, ay = _axis_table(H, h, sy)
     # horizontal pass on every source row, float32, taps summed left to right

@@ -47,6 +47,8 @@
 #define SPGO_ERR_CAPACITY (-1)   /* an output capacity was exceeded                      */
 #define SPGO_ERR_INDEX    (-2)   /* the reference would raise IndexError (sample index)  */
 #define SPGO_ERR_ASSERT   (-3)   /* the reference would raise in find_people :437-439    */
+#define SPGO_ERR_NONFINITE (-4)  /* a pair's length is not finite: round() raises at :226  */
+#define SPGO_ERR_NAN_PRIORITY (-5) /* a NaN priority among >= 2 candidates: the order sorted() gives at :259 is not reproduced */
 
 typedef struct spgo_params {
     double thre1, thre2, connect_ration, len_rate, connection_tole, min_mean_score;
@@ -114,10 +116,12 @@ int spgo_find_peaks(const float *heat, int K, int H, int W, int64_t cs, int64_t 
         for (int y = 0; y < H; y++) {
             for (int x = 0; x < W; x++) {
                 const float v = m[(int64_t)y * rs + x];
-                /* util.py:182: keep = (hmax == heat) * (heat >= thre); np.nonzero(heat*keep) at :193 */
-                if (!(v >= thr) || v == 0.0f) continue;
+                /* util.py:182: keep = (hmax == heat) * (heat >= thre); np.nonzero(heat*keep) at :193.  A non-finite
+                 * pixel is always a peak (NaN*0, inf*0, -inf*0 are NaN); a finite one needs keep = 1 and v != 0, and
+                 * keep = 1 needs v >= thre and no neighbour greater or NaN (torch's max-pool propagates NaN). */
                 int is_max = 1;
-                for (int dy = -1; dy <= 1 && is_max; dy++) {
+                if (isfinite(v) && (!(v >= thr) || v == 0.0f)) continue;
+                for (int dy = -1; dy <= 1 && is_max && isfinite(v); dy++) {
                     const int yy = y + dy;
                     if (yy < 0 || yy >= H) continue;
                     for (int dx = -1; dx <= 1; dx++) {
@@ -237,6 +241,7 @@ int spgo_find_connections(const double *px, const double *py, const float *pscor
                 const double bx = px[off[b] + j], by = py[off[b] + j];
                 const double vx = bx - ax, vy = by - ay;           /* :224 */
                 const double norm = sqrt(vx * vx + vy * vy);       /* :225 */
+                if (!isfinite(norm)) { rc = SPGO_ERR_NONFINITE; break; } /* int(round(norm + 1)) raises at :226 */
                 if (norm == 0.0) { cov(COV_NORM0); continue; }      /* :228-230 */
                 long mn = (long)rint(norm + 1.0);                   /* :226 round() half-even */
                 if (mn > p->mid_num) mn = p->mid_num;
@@ -294,6 +299,9 @@ int spgo_find_connections(const double *px, const double *py, const float *pscor
         }
         if (rc) break;
         if (cand_count) cand_count[k] = nc;
+        for (int c = 0; c < nc && nc > 1; c++)
+            if (isnan(cands[c].prio)) rc = SPGO_ERR_NAN_PRIORITY;
+        if (rc) break;
         sort_cands(cands, tmp, nc);
         memset(usedA, 0, (size_t)nA);
         memset(usedB, 0, (size_t)nB);

@@ -21,7 +21,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libspg_oracle.so")
 
-ERR_CAPACITY, ERR_INDEX, ERR_ASSERT = -1, -2, -3
+ERR_CAPACITY, ERR_INDEX, ERR_ASSERT, ERR_NONFINITE, ERR_NAN_PRIORITY = -1, -2, -3, -4, -5
 
 
 class _Params(C.Structure):

@@ -25,8 +25,8 @@ def _feq(a, b, tol) -> bool:
     b = np.asarray(b, np.float64)
     if a.shape != b.shape:
         return False
-    if tol == 0:
-        return bool(np.array_equal(a, b))
+    if tol == 0:  # bit-exact values; NaN (maps with non-finite values) compared by position
+        return bool(np.array_equal(a, b, equal_nan=True))
     return bool(np.all(np.abs(a - b) <= tol))
 
 

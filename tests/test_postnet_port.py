@@ -106,3 +106,31 @@ def test_three_instruction_division_of_the_multi_scale_kernel_is_exact():
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     assert mod.check(3, binades=(127,), sample=300) == 0
+
+
+@pytest.mark.parametrize("shape,kw", CASES)
+def test_resize_on_nonfinite_maps_equals_opencv_generic_path(no_ipp, shape, kw):
+    """NaN, +inf and -inf in the source (a network output the reference does not scrub): the port and cv2 (IPP off)
+    agree on where NaN lands (inf * a tap weight of either sign, inf - inf), on every infinity, and to rounding on the
+    finite values."""
+    rng = np.random.default_rng(8)
+    src = rng.random(shape, dtype=np.float32)
+    flat = src.reshape(-1)
+    pos = rng.choice(flat.size, size=max(3, flat.size // 200), replace=False)
+    flat[pos] = np.array([np.nan, np.inf, -np.inf], np.float32)[np.arange(pos.size) % 3]
+    ref, got = _cv(src, kw), _port(src, kw)
+    assert ref.shape == got.shape
+    assert np.array_equal(np.isnan(ref), np.isnan(got))
+    assert np.array_equal(np.isposinf(ref), np.isposinf(got)) and np.array_equal(np.isneginf(ref), np.isneginf(got))
+    fin = np.isfinite(ref)
+    assert np.isnan(got).any() and np.isinf(got).any() and fin.any()
+    assert np.abs(ref[fin] - got[fin]).max() <= 5e-7
+
+
+def test_same_size_resize_is_a_copy_as_in_opencv(no_ipp):
+    """cv2.resize to the source's own size copies the source (resize.cpp's dsize == ssize shortcut): an infinity stays
+    one pixel, where the [0, 1, 0, 0] taps would make NaN of its neighbours (inf * 0)."""
+    src = np.random.default_rng(9).random((9, 11, 3), dtype=np.float32)
+    src[4, 5, 0], src[2, 3, 1], src[6, 6, 2] = np.inf, -np.inf, np.nan
+    ref, got = cv2.resize(src, (11, 9), interpolation=cv2.INTER_CUBIC), _port(src, dict(dsize=(11, 9)))
+    assert np.array_equal(ref, src, equal_nan=True) and np.array_equal(got.view(np.uint32), src.view(np.uint32))
