@@ -723,11 +723,27 @@ static_assert(kPostR_R1 * kPostTW <= kPostF_RS * (kPostF_CS + kPostF_C1), "pass 
 // value (y, x) is val(g[(y - y0) * pitch + (x - x0) * CS]); taps outside the grid read 0 (BORDER_CONSTANT) and are never
 // loaded.  Every product and sum is rounded to float32, left to right.  Shared by the inverse warp of the maps
 // (postnet_rot_kernel) and the forward warp of the input image (prenet.cuh).
+// (xs, ys) -> the top-left tap (sx, sy) and the 1/32 px fractions (ax, ay) of warpAffine's INTER_TAB_SIZE table; shared
+// with the uint8 tap combine of the training-sample warp (targets.cuh)
+struct WarpTap {
+    int sx, sy, ax, ay;
+};
+__device__ __forceinline__ WarpTap warp_tap(int xs, int ys) {
+    const int xf = xs >> 5, yf = ys >> 5;
+    return {clampi(xf >> 5, -32768, 32767), clampi(yf >> 5, -32768, 32767), xf & 31, yf & 31};  // saturate_cast<short>
+}
+// warpAffine's fixed-point source coordinates (X0 + adelta, Y0 + bdelta, the +16 rounding term included) of destination
+// pixel (x, y) under the inverted matrix m (rounded ties-to-even like cvRound)
+__device__ __forceinline__ void warp_coords(const double m[6], int x, int y, int &xs, int &ys) {
+    const double xd = (double)x, yd = (double)y;
+    xs = __double2int_rn(__dmul_rn(__dmul_rn(m[0], xd), 1024.0)) + __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], yd), m[2]), 1024.0)) + 16;
+    ys = __double2int_rn(__dmul_rn(__dmul_rn(m[3], xd), 1024.0)) + __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], yd), m[5]), 1024.0)) + 16;
+}
 template <int CS, typename T, typename Val>
 __device__ __forceinline__ float warp_linear(int xs, int ys, int w, int h, const T *g, int pitch, int x0, int y0, const Val &val) {
-    const int xf = xs >> 5, yf = ys >> 5;
-    const int sx = clampi(xf >> 5, -32768, 32767), sy = clampi(yf >> 5, -32768, 32767);  // saturate_cast<short>
-    const float fx = __fmul_rn((float)(xf & 31), 0.03125f), fy = __fmul_rn((float)(yf & 31), 0.03125f);
+    const WarpTap t = warp_tap(xs, ys);
+    const int sx = t.sx, sy = t.sy;
+    const float fx = __fmul_rn((float)t.ax, 0.03125f), fy = __fmul_rn((float)t.ay, 0.03125f);
     const float gx = __fsub_rn(1.0f, fx), gy = __fsub_rn(1.0f, fy);
     const bool x0in = sx >= 0 && sx < w, x1in = sx + 1 >= 0 && sx + 1 < w;
     const bool y0in = sy >= 0 && sy < h, y1in = sy + 1 >= 0 && sy + 1 < h;

@@ -147,11 +147,8 @@ __global__ void __launch_bounds__(kPreThreads) prenet_kernel(const __grid_consta
     float f[3];
     if (ROT) {
         // warpAffine's adelta / bdelta and X0 / Y0 (rounded ties-to-even like cvRound), as postnet_rot_kernel
-        const double xd = (double)x, yd = (double)y;
-        const int xs = __double2int_rn(__dmul_rn(__dmul_rn(a.rot[0], xd), 1024.0)) +
-                       __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.rot[1], yd), a.rot[2]), 1024.0)) + 16;
-        const int ys = __double2int_rn(__dmul_rn(__dmul_rn(a.rot[3], xd), 1024.0)) +
-                       __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.rot[4], yd), a.rot[5]), 1024.0)) + 16;
+        int xs, ys;
+        warp_coords(a.rot, x, y, xs, ys);
 #pragma unroll
         for (int ch = 0; ch < 3; ch++)
             f[ch] = warp_linear<3>(xs, ys, a.Wp, a.Hp, a.grid + ch, 3 * a.Wp, 0, 0, [&](unsigned char v) { return lut[v]; });

@@ -30,6 +30,7 @@
 #include "nms_peaks_banded.cuh"
 #include "postnet.cuh"
 #include "prenet.cuh"
+#include "targets.cuh"
 
 using namespace spg;
 
@@ -38,7 +39,7 @@ static_assert(sizeof(spg_params) == sizeof(spg::Params), "spg_params layout");
 static thread_local std::string g_create_error;
 
 // the stage numbers of spg_stage_kernel (include/spgroup.h)
-enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageCount };
+enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageTargets, kStageCount };
 
 // device scratch that grows on demand (grow) and lives until spg_destroy
 struct Scratch {
@@ -67,7 +68,7 @@ struct spg_handle {
     bool ub_valid = false;
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
-    const char *stage_kernel[kStageCount] = {"", "", "", "", "", ""};
+    const char *stage_kernel[kStageCount] = {"", "", "", "", "", "", ""};
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
@@ -140,6 +141,27 @@ int launch(spg_handle *h, int stage, const char *name, void (*kern)(P...), dim3 
     h->stage_kernel[stage] = name;
     h->launches++;
     SPG_CUDA(h, cudaGetLastError());
+    return SPG_OK;
+}
+
+// The training-sample launches (spg_targets_warp / spg_targets_maps): every sample has the same CTA count
+// `per_sample`; launches of up to `per_launch` samples back to back, each with its member table as the parameter.
+template <class R, class M>
+int targets_launch(spg_handle *h, const char *name, void (*kern)(R), R &r, const std::vector<M> &ms, int per_launch,
+                   long long per_sample, cudaStream_t st) {
+    if (ms.empty()) return SPG_OK;
+    if (per_sample > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "a sample's %lld CTAs are above grid.x's 2^31 - 1", per_sample);
+    per_launch = (int)std::min<long long>(per_launch, 0x7fffffffLL / per_sample);
+    DeviceGuard guard(h->device);
+    for (size_t i0 = 0; i0 < ms.size(); i0 += (size_t)per_launch) {
+        r.n = (int)std::min(ms.size() - i0, (size_t)per_launch);
+        for (int k = 0; k < r.n; k++) {
+            r.img[k] = ms[i0 + k];
+            r.img[k].first_cta = (int)(k * per_sample);
+        }
+        int rc;
+        if ((rc = launch(h, kStageTargets, name, kern, dim3((unsigned)(per_sample * r.n)), kTgtThreads, 0, st, r))) return rc;
+    }
     return SPG_OK;
 }
 
@@ -1323,6 +1345,99 @@ int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_
     if (ms.empty()) return SPG_OK;
     DeviceGuard guard(h->device);
     return prenet_launch(h, ms, rotated, static_cast<cudaStream_t>(stream));
+}
+
+// ---- training samples --------------------------------------------------------------------------
+namespace {
+
+// the parameters every sample of a call shares, checked and resolved
+int targets_common(spg_handle *h, const spg_target_params *p, TgtCommon &c) {
+    if (!p) return fail(h, SPG_E_INVALID, "params is NULL");
+    if (p->stride < 1 || p->out_h < 1 || p->out_w < 1 || p->out_h > 32767 || p->out_w > 32767)
+        return fail(h, SPG_E_INVALID, "stride %d or output %dx%d outside [1, 32767]", p->stride, p->out_h, p->out_w);
+    if (p->out_h % p->stride || p->out_w % p->stride)
+        return fail(h, SPG_E_INVALID, "stride %d does not divide the output %dx%d", p->stride, p->out_h, p->out_w);
+    if (p->gaussian_size < 0 || p->gaussian_size > 32767) return fail(h, SPG_E_INVALID, "gaussian_size %d outside [0, 32767]", p->gaussian_size);
+    if (!std::isfinite(p->sigma) || !(p->sigma > 0) || !std::isfinite(p->paf_sigma) || !(p->paf_sigma > 0))
+        return fail(h, SPG_E_INVALID, "sigma and paf_sigma must be finite and positive");
+    if (!std::isfinite(p->limb_gaussian_thre) || !std::isfinite(p->paf_thre))
+        return fail(h, SPG_E_INVALID, "limb_gaussian_thre and paf_thre must be finite");
+    const int border[5] = {p->border_image[0], p->border_image[1], p->border_image[2], p->border_mask_miss, p->border_mask_all};
+    for (int k = 0; k < 5; k++)
+        if (border[k] < 0 || border[k] > 255) return fail(h, SPG_E_INVALID, "border value %d outside [0, 255]", border[k]);
+    if (p->reserved != 0) return fail(h, SPG_E_INVALID, "reserved must be 0");
+    c = TgtCommon{};
+    c.stride = p->stride;
+    c.out_h = p->out_h;
+    c.out_w = p->out_w;
+    c.map_h = p->out_h / p->stride;
+    c.map_w = p->out_w / p->stride;
+    c.half = p->gaussian_size / 2;
+    for (int k = 0; k < 5; k++) c.border[k] = border[k];
+    c.kp_ds2 = (float)(2.0 * p->sigma * p->sigma);          // np.array([2 * sigma * sigma]).astype(np.float32)
+    c.paf_thre = (float)p->paf_thre;                        // float32 coordinate - paf_thre stays float32
+    c.paf_ds2 = 2.0 * (p->paf_sigma * p->paf_sigma);        // 2 * sigma ** 2
+    c.limb_thre = p->limb_gaussian_thre;
+    for (int i = 0; i < 256; i++) c.lut[i] = (float)i / 255.0f;  // np.float32(u8) / 255.: a float32 division
+    return SPG_OK;
+}
+
+}  // namespace
+
+int spg_targets_warp(spg_handle *h, const spg_target_params *params, const spg_target_sample *samples, int32_t n, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    TgtWarpRagged r{};
+    if ((rc = targets_common(h, params, r.c))) return rc;
+    if (n < 0 || (n > 0 && !samples)) return fail(h, SPG_E_INVALID, "samples is NULL or n_samples negative");
+    const long long img_px = (long long)r.c.out_h * r.c.out_w, map_px = (long long)r.c.map_h * r.c.map_w;
+    std::vector<TgtWarpMember> ms((size_t)n);
+    for (int i = 0; i < n; i++) {  // validate every sample before the first launch
+        const spg_target_sample &s = samples[i];
+        if (s.height < 1 || s.width < 1 || s.height > 32767 || s.width > 32767)
+            return fail(h, SPG_E_INVALID, "sample %d: source %dx%d outside [1, 32767]", i, s.height, s.width);
+        if (!s.image || !s.mask_miss || !s.mask_all || !s.image_out || !s.mask_miss_out || !s.mask_all_out)
+            return fail(h, SPG_E_INVALID, "sample %d: a source or output pointer is NULL", i);
+        if (s.image_row_stride < 3LL * s.width || s.mask_row_stride < s.width)
+            return fail(h, SPG_E_INVALID, "sample %d: a row stride is below the row's bytes", i);
+        for (int k = 0; k < 6; k++)
+            if (!std::isfinite(s.matrix[k])) return fail(h, SPG_E_INVALID, "sample %d: matrix entry %d is not finite", i, k);
+        TgtWarpMember &a = ms[i];
+        a.src = s.image; a.miss = s.mask_miss; a.all = s.mask_all;
+        a.src_stride = s.image_row_stride; a.mask_stride = s.mask_row_stride;
+        a.img_out = s.image_out; a.miss_out = s.mask_miss_out; a.all_out = s.mask_all_out;
+        invert_affine(s.matrix, a.rot);
+        a.h = s.height; a.w = s.width;
+        a.img_ctas = (int)((img_px + kTgtThreads - 1) / kTgtThreads);
+    }
+    const long long per_sample = (img_px + kTgtThreads - 1) / kTgtThreads + (map_px + kTgtThreads - 1) / kTgtThreads;
+    return targets_launch(h, "targets_warp_kernel", targets_warp_kernel, r, ms, kTgtWarpMax, per_sample, static_cast<cudaStream_t>(stream));
+}
+
+int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_target_joints *samples, int32_t n, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    TgtMapsRagged r{};
+    if ((rc = targets_common(h, params, r.c))) return rc;
+    if (n < 0 || (n > 0 && !samples)) return fail(h, SPG_E_INVALID, "samples is NULL or n_samples negative");
+    r.K = h->ws.K;
+    r.L = h->ws.L;
+    for (int k = 0; k < 2 * r.L; k++) r.limbs[k] = h->ws.limbs[k];
+    const long long map_px = (long long)r.c.map_h * r.c.map_w;
+    const int tiles = (int)((map_px + kTgtThreads - 1) / kTgtThreads);
+    const long long channels = r.L + r.K + 2;
+    std::vector<TgtMapsMember> ms((size_t)n);
+    for (int i = 0; i < n; i++) {  // validate every sample before the first launch
+        const spg_target_joints &s = samples[i];
+        if (s.n_persons < 0 || (long long)s.n_persons * r.K > 0x7fffffffLL - kTgtThreads)
+            return fail(h, SPG_E_INVALID, "sample %d: n_persons %d outside [0, 2^31 / n_parts)", i, s.n_persons);
+        if (s.reserved != 0) return fail(h, SPG_E_INVALID, "sample %d: reserved must be 0", i);
+        if ((s.n_persons > 0 && !s.joints) || !s.mask_all || !s.labels)
+            return fail(h, SPG_E_INVALID, "sample %d: joints, mask_all or labels is NULL", i);
+        ms[i] = TgtMapsMember{s.joints, s.mask_all, s.labels, s.n_persons, tiles, 0};
+    }
+    return targets_launch(h, "targets_maps_kernel", targets_maps_kernel, r, ms, kTgtMapsMax, channels * tiles,
+                          static_cast<cudaStream_t>(stream));
 }
 
 // ---- stages ------------------------------------------------------------------------------------

@@ -92,6 +92,20 @@ PRENET_MEMBER = np.dtype([("image", np.uint64), ("row_stride", np.int64), ("heig
                           ("out", np.uint64)], align=True)
 
 
+#: ``spg_target_params``, ``spg_target_sample`` and ``spg_target_joints`` (include/spgroup.h) as numpy records: a batch of
+#: training samples fills one record per sample
+TARGET_PARAMS = np.dtype([("stride", np.int32), ("gaussian_size", np.int32), ("out_h", np.int32), ("out_w", np.int32),
+                          ("sigma", np.float64), ("paf_sigma", np.float64), ("limb_gaussian_thre", np.float64),
+                          ("paf_thre", np.float64), ("border_image", np.int32, (3,)), ("border_mask_miss", np.int32),
+                          ("border_mask_all", np.int32), ("reserved", np.int32)], align=True)
+TARGET_SAMPLE = np.dtype([("image", np.uint64), ("mask_miss", np.uint64), ("mask_all", np.uint64),
+                          ("image_row_stride", np.int64), ("mask_row_stride", np.int64), ("height", np.int32),
+                          ("width", np.int32), ("matrix", np.float64, (6,)), ("image_out", np.uint64),
+                          ("mask_miss_out", np.uint64), ("mask_all_out", np.uint64)], align=True)
+TARGET_JOINTS = np.dtype([("joints", np.uint64), ("n_persons", np.int32), ("reserved", np.int32), ("mask_all", np.uint64),
+                          ("labels", np.uint64)], align=True)
+
+
 class _ImageMaps(C.Structure):
     _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
                 ("paf_chan_stride", C.c_int64), ("height", C.c_int32), ("width", C.c_int32), ("image_extent", C.c_double)]
@@ -130,6 +144,9 @@ _PROTOTYPES = {
                                         _ptr]),
     "spg_prenet": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _P(_PrenetItem), _i32, _ptr]),
     "spg_prenet_ragged": (_int, [_ptr, _i32, _i32, _ptr, _i32, _ptr]),  # members: a PRENET_MEMBER array
+    # params: a TARGET_PARAMS record; samples: a TARGET_SAMPLE / TARGET_JOINTS array
+    "spg_targets_warp": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
+    "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -852,6 +869,27 @@ class Grouper:
                 not o[(0,) * (len(shape) - 4)].is_contiguous():
             raise GroupingError(f"{name} must be a float32 {form}")
         return o
+
+    # -- training samples (targets.py builds the records) ----------------------------------------------------------
+    def targets_warp(self, params: np.ndarray, samples: np.ndarray, stream=None) -> None:
+        """``spg_targets_warp``: ``params`` one ``TARGET_PARAMS`` record, ``samples`` a ``TARGET_SAMPLE`` array of device
+        addresses on the handle's device.  Asynchronous on ``stream``."""
+        p, s = self._records(params, TARGET_PARAMS), self._records(samples, TARGET_SAMPLE)
+        _check(self._lib.spg_targets_warp(self._h, p.ctypes.data, s.ctypes.data, len(s), self._stream_ptr(stream)),
+               "spg_targets_warp", self._h)
+
+    def targets_maps(self, params: np.ndarray, samples: np.ndarray, stream=None) -> None:
+        """``spg_targets_maps``: ``samples`` a ``TARGET_JOINTS`` array; the limb table is the handle's."""
+        p, s = self._records(params, TARGET_PARAMS), self._records(samples, TARGET_JOINTS)
+        _check(self._lib.spg_targets_maps(self._h, p.ctypes.data, s.ctypes.data, len(s), self._stream_ptr(stream)),
+               "spg_targets_maps", self._h)
+
+    @staticmethod
+    def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:
+        a = np.ascontiguousarray(a).reshape(-1)
+        if a.dtype != dtype:
+            raise GroupingError(f"records of dtype {dtype} expected")
+        return a
 
     # -- stages -------------------------------------------------------------------------------------
     def nms_peaks(self, heat, params=None, stream=None) -> None:

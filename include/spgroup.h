@@ -304,6 +304,56 @@ typedef struct spg_prenet_member {
 int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, const spg_prenet_member *members,
                       int32_t n_members, void *stream);
 
+/* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
+ * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
+ * reference's CanonicalConfig / TransformationParams: */
+typedef struct spg_target_params {
+    int32_t stride;             /* config.stride: the map is the warped image / stride (must divide out_h and out_w) */
+    int32_t gaussian_size;      /* Heatmapper.gaussian_size: a keypoint window is round(x / stride) +- gaussian_size // 2 */
+    int32_t out_h, out_w;       /* warped image rows / columns: warpAffine's dsize (config.height, config.width) is */
+                                /* (columns, rows), so out_h = config.width and out_w = config.height                 */
+    double sigma;               /* transform_params.sigma: keypoint Gaussian */
+    double paf_sigma;           /* transform_params.paf_sigma: body-part Gaussian */
+    double limb_gaussian_thre;  /* body-part values <= this become 0.01 */
+    double paf_thre;            /* transform_params.paf_thre: the body-part box's margin in image pixels */
+    int32_t border_image[3];    /* warpAffine's borderValue for the image: (124, 127, 127) */
+    int32_t border_mask_miss;   /* 255 */
+    int32_t border_mask_all;    /* 0 */
+    int32_t reserved;           /* 0 */
+} spg_target_params;
+/* One sample of spg_targets_warp: device sources and outputs. */
+typedef struct spg_target_sample {
+    const uint8_t *image;       /* [height][width][3] uint8 (BGR as read), rows image_row_stride bytes apart */
+    const uint8_t *mask_miss;   /* [height][width] uint8, rows mask_row_stride bytes apart */
+    const uint8_t *mask_all;    /* [height][width] uint8, rows mask_row_stride bytes apart */
+    int64_t image_row_stride, mask_row_stride;
+    int32_t height, width;
+    double matrix[6];           /* the row-major 2x3 matrix AugmentSelection.affine returns (source -> output) */
+    float *image_out;           /* [out_h][out_w][3] float32 */
+    float *mask_miss_out;       /* [out_h / stride][out_w / stride] float32 */
+    float *mask_all_out;        /* [out_h / stride][out_w / stride] float32 */
+} spg_target_sample;
+/* Per sample: cv2.warpAffine(image, matrix, (out_w, out_h), INTER_LINEAR, BORDER_CONSTANT, border_image) / 255. as
+ * float32, and each mask through the same warp (its own border value), cv2.resize(..., INTER_AREA) by the integer factor
+ * stride and / 255.  The warp and the area resize follow OpenCV's uint8 algorithms bit for bit; the full-size warped masks
+ * are never stored.  Every sample is validated before the first launch (SPG_E_INVALID names the first bad one).
+ * Asynchronous on `stream` (never synchronises); `samples` may be reused as soon as the call returns. */
+int spg_targets_warp(spg_handle *h, const spg_target_params *params, const spg_target_sample *samples, int32_t n_samples,
+                     void *stream);
+/* One sample of spg_targets_maps. */
+typedef struct spg_target_joints {
+    const float *joints;        /* [n_persons][n_parts][3] float32 device (x, y, v) in output pixels; v < 2 is visible */
+    int32_t n_persons;          /* any count >= 0 */
+    int32_t reserved;           /* 0 */
+    const float *mask_all;      /* [out_h / stride][out_w / stride] float32 device: spg_targets_warp's mask_all_out */
+    float *labels;              /* [n_limbs + n_parts + 2][out_h / stride][out_w / stride] float32 */
+} spg_target_joints;
+/* Per sample, Heatmapper.create_heatmaps: body-part channels 0..L-1 (the handle's limb table), keypoint channels
+ * L..L+K-1, cv2.erode(mask_all, ones(3, 3)) in channel L+K and the max of the keypoint channels in channel L+K+1, clipped
+ * to [0, 1].  Each value is written once.  Validation, asynchrony and reuse of `samples` as spg_targets_warp. */
+int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_target_joints *samples, int32_t n_samples,
+                     void *stream);
+
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
 int spg_nms_peaks(spg_handle *h, const float *heat_dev, int64_t image_stride, int64_t chan_stride,
@@ -388,7 +438,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage, 5 pre-network stage);
+ * 4 post-network stage, 5 pre-network stage, 6 training samples);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 
