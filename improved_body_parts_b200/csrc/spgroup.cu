@@ -144,23 +144,27 @@ int launch(spg_handle *h, int stage, const char *name, void (*kern)(P...), dim3 
     return SPG_OK;
 }
 
-// The training-sample launches (spg_targets_warp / spg_targets_maps): every sample has the same CTA count
-// `per_sample`; launches of up to `per_launch` samples back to back, each with its member table as the parameter.
+// The training-sample launches (spg_targets_warp / spg_targets_maps / spg_targets_tint): sample i takes ctas[i] CTAs;
+// launches of up to `per_launch` samples and 2^31 - 1 CTAs back to back, each with its member table as the parameter.
+// With one CTA count for every sample, a launch holds min(per_launch, (2^31 - 1) / count) samples.
 template <class R, class M>
 int targets_launch(spg_handle *h, const char *name, void (*kern)(R), R &r, const std::vector<M> &ms, int per_launch,
-                   long long per_sample, cudaStream_t st) {
+                   const std::vector<long long> &ctas, cudaStream_t st) {
     if (ms.empty()) return SPG_OK;
-    if (per_sample > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "a sample's %lld CTAs are above grid.x's 2^31 - 1", per_sample);
-    per_launch = (int)std::min<long long>(per_launch, 0x7fffffffLL / per_sample);
+    for (long long c : ctas)
+        if (c > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "a sample's %lld CTAs are above grid.x's 2^31 - 1", c);
     DeviceGuard guard(h->device);
-    for (size_t i0 = 0; i0 < ms.size(); i0 += (size_t)per_launch) {
-        r.n = (int)std::min(ms.size() - i0, (size_t)per_launch);
-        for (int k = 0; k < r.n; k++) {
-            r.img[k] = ms[i0 + k];
-            r.img[k].first_cta = (int)(k * per_sample);
+    for (size_t i = 0; i < ms.size();) {
+        long long total = 0;
+        r.n = 0;
+        while (i < ms.size() && r.n < per_launch && total + ctas[i] <= 0x7fffffffLL) {
+            r.img[r.n] = ms[i];
+            r.img[r.n].first_cta = (int)total;
+            total += ctas[i++];
+            r.n++;
         }
         int rc;
-        if ((rc = launch(h, kStageTargets, name, kern, dim3((unsigned)(per_sample * r.n)), kTgtThreads, 0, st, r))) return rc;
+        if ((rc = launch(h, kStageTargets, name, kern, dim3((unsigned)total), kTgtThreads, 0, st, r))) return rc;
     }
     return SPG_OK;
 }
@@ -1411,7 +1415,8 @@ int spg_targets_warp(spg_handle *h, const spg_target_params *params, const spg_t
         a.img_ctas = (int)((img_px + kTgtThreads - 1) / kTgtThreads);
     }
     const long long per_sample = (img_px + kTgtThreads - 1) / kTgtThreads + (map_px + kTgtThreads - 1) / kTgtThreads;
-    return targets_launch(h, "targets_warp_kernel", targets_warp_kernel, r, ms, kTgtWarpMax, per_sample, static_cast<cudaStream_t>(stream));
+    return targets_launch(h, "targets_warp_kernel", targets_warp_kernel, r, ms, kTgtWarpMax, std::vector<long long>((size_t)n, per_sample),
+                          static_cast<cudaStream_t>(stream));
 }
 
 int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_target_joints *samples, int32_t n, void *stream) {
@@ -1436,8 +1441,31 @@ int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_t
             return fail(h, SPG_E_INVALID, "sample %d: joints, mask_all or labels is NULL", i);
         ms[i] = TgtMapsMember{s.joints, s.mask_all, s.labels, s.n_persons, tiles, 0};
     }
-    return targets_launch(h, "targets_maps_kernel", targets_maps_kernel, r, ms, kTgtMapsMax, channels * tiles,
+    return targets_launch(h, "targets_maps_kernel", targets_maps_kernel, r, ms, kTgtMapsMax, std::vector<long long>((size_t)n, channels * tiles),
                           static_cast<cudaStream_t>(stream));
+}
+
+int spg_targets_tint(spg_handle *h, const spg_target_tint *samples, int32_t n, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    if (n < 0 || (n > 0 && !samples)) return fail(h, SPG_E_INVALID, "samples is NULL or n_samples negative");
+    TgtTintRagged r{};
+    std::vector<TgtTintMember> ms((size_t)n);
+    std::vector<long long> ctas((size_t)n);
+    for (int i = 0; i < n; i++) {  // validate every sample before the first launch
+        const spg_target_tint &s = samples[i];
+        if (s.height < 1 || s.width < 1 || s.height > 32767 || s.width > 32767)
+            return fail(h, SPG_E_INVALID, "sample %d: source %dx%d outside [1, 32767]", i, s.height, s.width);
+        if (!s.image) return fail(h, SPG_E_INVALID, "sample %d: image is NULL", i);
+        if (s.row_stride < 3LL * s.width) return fail(h, SPG_E_INVALID, "sample %d: row_stride %lld is below the row's bytes", i, (long long)s.row_stride);
+        if (s.hue < 0 || s.hue > 20 || s.saturation < 0 || s.saturation > 80 || s.value < 0 || s.value > 60)
+            return fail(h, SPG_E_INVALID, "sample %d: draws (%d, %d, %d) outside [0, 20] x [0, 80] x [0, 60]", i, s.hue, s.saturation, s.value);
+        if (s.row_block < 1) return fail(h, SPG_E_INVALID, "sample %d: row_block %d below 1", i, s.row_block);
+        const int groups = (s.width + kTintPix - 1) / kTintPix;
+        ms[i] = TgtTintMember{s.image, s.row_stride, s.height, s.width, s.hue - 10, s.saturation - 20, s.value - 20,
+                              s.width - s.width % s.row_block, groups, 0};
+        ctas[i] = ((long long)s.height * groups + kTgtThreads - 1) / kTgtThreads;
+    }
+    return targets_launch(h, "targets_tint_kernel", targets_tint_kernel, r, ms, kTgtTintMax, ctas, static_cast<cudaStream_t>(stream));
 }
 
 // ---- stages ------------------------------------------------------------------------------------

@@ -25,7 +25,9 @@
 // into shared memory in person order; every thread then runs its pixel over the list.  Windows are clipped in double
 // before any conversion to int, so coordinates up to +-FLT_MAX give empty windows and no overflow.
 //
-// Both launches are ragged like prenet.cuh: a member table (one sample each) travels as a __grid_constant__ kernel
+// targets_tint_kernel (below the warp): the colour distortion, in place on the uint8 sources before the warp.
+//
+// The launches are ragged like prenet.cuh: a member table (one sample each) travels as a __grid_constant__ kernel
 // parameter and a CTA finds its member by binary search over first_cta (post_ragged_image).
 #pragma once
 
@@ -113,6 +115,135 @@ __global__ void __launch_bounds__(kTgtThreads) targets_warp_kernel(const __grid_
     const float area = (float)(c.stride * c.stride);  // the quotient is correctly rounded; rint then ties to even
     a.miss_out[p] = c.lut[__float2int_rn(__fdiv_rn((float)s_miss, area))];
     a.all_out[p] = c.lut[__float2int_rn(__fdiv_rn((float)s_all, area))];
+}
+
+// ---- colour distortion -----------------------------------------------------------------------------------------------
+// targets_tint_kernel: Transformer.distort_color (py_data_transformer.py:97-110) in place on uint8 BGR sources, before
+// targets_warp_kernel reads them.  A separate pass rather than part of the warp's tap reads: the warp stays as it is
+// (untinted samples cannot move, its border value stays untinted as in the reference), and the pass costs one read and
+// one write of the tinted sources.  Per pixel:
+//   cv2.cvtColor(COLOR_BGR2HSV), uint8: integer arithmetic on the 2^12 fixed-point tables sdiv / hdiv (shared memory,
+//     computed per CTA: no quotient is a tie, so the integer rounding below is cvRound's);
+//   the draws minus (10, 20, 20) added, clamped to [0, 179], [0, 255], [0, 255];
+//   cv2.cvtColor(COLOR_HSV2BGR), uint8: float32 with the two fused multiply-adds OpenCV's vector code has (the build has
+//     -fmad=false, so only the written __fmaf_rn fuse), then x * 255 truncated -- or rounded to nearest even in the last
+//     width % row_block columns of every row, which OpenCV's scalar tail handles (DESIGN.md §4).
+// A thread owns kTintPix consecutive pixels of one row: 16-byte accesses when the group's address is 16-byte aligned,
+// 4-byte when 4-byte aligned, bytes otherwise (a row's last group, odd pitches).
+constexpr int kTintPix = 16;
+constexpr int kTintWords = kTintPix * 3 / 4;
+
+struct TgtTintMember {
+    unsigned char *image;    // [h][w][3], rows row_stride bytes apart; tinted in place
+    long long row_stride;
+    int h, w;
+    int dh, ds, dv;          // the draws minus 10, 20, 20
+    int tail;                // first rounded column: w - w % row_block
+    int groups;              // kTintPix-pixel groups per row
+    int first_cta;
+};
+constexpr int kTgtTintMax = (int)((kTgtParamBytes - 16) / sizeof(TgtTintMember));
+struct TgtTintRagged {
+    int n;
+    TgtTintMember img[kTgtTintMax];   // first_cta increasing
+};
+static_assert(sizeof(TgtTintRagged) <= kTgtParamBytes, "a launch's parameters fit the kernel-parameter limit");
+
+// the HSV -> BGR table entry k of [V, V(1-S), V(1-S hh), V(1-S(1-hh))] without dynamic indexing into registers
+__device__ __forceinline__ float tint_pick(int k, float t0, float t1, float t2, float t3) {
+    return k == 0 ? t0 : (k == 1 ? t1 : (k == 2 ? t2 : t3));
+}
+
+// one pixel (b, g, r) in place
+__device__ __forceinline__ void tint_pixel(const int *sdiv, const int *hdiv, const TgtTintMember &a, bool round, int &b, int &g, int &r) {
+    int v = max(max(b, g), r);
+    const int diff = v - min(min(b, g), r);
+    int s = (diff * sdiv[v] + (1 << 11)) >> 12;
+    const int vr = -(int)(v == r), vg = -(int)(v == g);
+    int h = (vr & (g - b)) + (~vr & ((vg & (b - r + 2 * diff)) + (~vg & (r - g + 4 * diff))));
+    h = (h * hdiv[diff] + (1 << 11)) >> 12;
+    h += h < 0 ? 180 : 0;
+    h = min(max(h + a.dh, 0), 179);
+    s = min(max(s + a.ds, 0), 255);
+    v = min(max(v + a.dv, 0), 255);
+    const float S = __fmul_rn((float)s, 1.f / 255.f), V = __fmul_rn((float)v, 1.f / 255.f);
+    float hh = __fmul_rn((float)h, 6.f / 180.f);
+    if (hh >= 6.f) hh = __fsub_rn(hh, 6.f);
+    const float fl = floorf(hh);
+    const int sector = (int)fl;  // 0..5
+    hh = __fsub_rn(hh, fl);
+    // S == 0 needs no case of its own: every entry is then exactly V
+    const float t0 = V, t1 = __fmul_rn(V, __fsub_rn(1.f, S)), t2 = __fmul_rn(V, __fmaf_rn(-S, hh, 1.f)),
+                t3 = __fmul_rn(V, __fmaf_rn(-S, __fsub_rn(1.f, hh), 1.f));
+    // cv2's sector table {1,3,0},{1,0,2},{3,0,1},{0,2,1},{0,1,3},{2,1,0}, one 2-bit entry per sector and channel
+    const int sh = 2 * sector;
+    const float fb = __fmul_rn(tint_pick((0x835 >> sh) & 3, t0, t1, t2, t3), 255.f);
+    const float fg = __fmul_rn(tint_pick((0x583 >> sh) & 3, t0, t1, t2, t3), 255.f);
+    const float fr = __fmul_rn(tint_pick((0x358 >> sh) & 3, t0, t1, t2, t3), 255.f);
+    b = min(max(round ? __float2int_rn(fb) : __float2int_rz(fb), 0), 255);
+    g = min(max(round ? __float2int_rn(fg) : __float2int_rz(fg), 0), 255);
+    r = min(max(round ? __float2int_rn(fr) : __float2int_rz(fr), 0), 255);
+}
+
+__global__ void __launch_bounds__(kTgtThreads) targets_tint_kernel(const __grid_constant__ TgtTintRagged r) {
+    __shared__ int sdiv[256], hdiv[256];
+    for (int i = threadIdx.x; i < 256; i += kTgtThreads) {  // round((255 << 12) / i), round((180 << 12) / (6 i))
+        sdiv[i] = i ? (2 * (255 << 12) + i) / (2 * i) : 0;
+        hdiv[i] = i ? (2 * (180 << 12) + 6 * i) / (12 * i) : 0;
+    }
+    __syncthreads();
+    const TgtTintMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const long long q = (long long)((int)blockIdx.x - a.first_cta) * kTgtThreads + threadIdx.x;
+    if (q >= (long long)a.h * a.groups) return;
+    const int y = (int)(q / a.groups), x0 = (int)(q - (long long)y * a.groups) * kTintPix;
+    const int np = min(kTintPix, a.w - x0);
+    unsigned char *p = a.image + (long long)y * a.row_stride + (long long)x0 * 3;
+    const unsigned long long addr = (unsigned long long)p;
+    unsigned int wd[kTintWords];
+    const bool full = np == kTintPix, v16 = full && (addr & 15) == 0, v4 = full && (addr & 3) == 0;
+    if (v16) {
+#pragma unroll
+        for (int k = 0; k < kTintWords / 4; k++) {
+            const uint4 u = reinterpret_cast<const uint4 *>(p)[k];
+            wd[4 * k] = u.x; wd[4 * k + 1] = u.y; wd[4 * k + 2] = u.z; wd[4 * k + 3] = u.w;
+        }
+    } else if (v4) {
+#pragma unroll
+        for (int k = 0; k < kTintWords; k++) wd[k] = reinterpret_cast<const unsigned int *>(p)[k];
+    } else {
+#pragma unroll
+        for (int k = 0; k < kTintWords; k++) {
+            unsigned int u = 0;
+#pragma unroll
+            for (int j = 0; j < 4; j++) u |= (4 * k + j < 3 * np ? (unsigned int)p[4 * k + j] : 0u) << (8 * j);
+            wd[k] = u;
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < kTintPix; i++) {
+        if (i >= np) continue;
+        int c[3];
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++) c[ch] = (wd[(3 * i + ch) >> 2] >> (8 * ((3 * i + ch) & 3))) & 255;
+        tint_pixel(sdiv, hdiv, a, x0 + i >= a.tail, c[0], c[1], c[2]);
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++) {
+            const int k = (3 * i + ch) >> 2, sft = 8 * ((3 * i + ch) & 3);
+            wd[k] = (wd[k] & ~(255u << sft)) | ((unsigned int)c[ch] << sft);
+        }
+    }
+    if (v16) {
+#pragma unroll
+        for (int k = 0; k < kTintWords / 4; k++)
+            reinterpret_cast<uint4 *>(p)[k] = make_uint4(wd[4 * k], wd[4 * k + 1], wd[4 * k + 2], wd[4 * k + 3]);
+    } else if (v4) {
+#pragma unroll
+        for (int k = 0; k < kTintWords; k++) reinterpret_cast<unsigned int *>(p)[k] = wd[k];
+    } else {
+#pragma unroll
+        for (int k = 0; k < 3 * kTintPix; k++)
+            if (k < 3 * np) p[k] = (unsigned char)(wd[k >> 2] >> (8 * (k & 3)));
+    }
 }
 
 // ---- ground-truth maps ---------------------------------------------------------------------------------------------

@@ -104,6 +104,10 @@ TARGET_SAMPLE = np.dtype([("image", np.uint64), ("mask_miss", np.uint64), ("mask
                           ("mask_miss_out", np.uint64), ("mask_all_out", np.uint64)], align=True)
 TARGET_JOINTS = np.dtype([("joints", np.uint64), ("n_persons", np.int32), ("reserved", np.int32), ("mask_all", np.uint64),
                           ("labels", np.uint64)], align=True)
+#: ``spg_target_tint``: one source to tint in place, the reference's three draws and cv2's HSV->BGR row block
+TARGET_TINT = np.dtype([("image", np.uint64), ("row_stride", np.int64), ("height", np.int32), ("width", np.int32),
+                        ("hue", np.int32), ("saturation", np.int32), ("value", np.int32), ("row_block", np.int32)],
+                       align=True)
 
 
 class _ImageMaps(C.Structure):
@@ -147,6 +151,7 @@ _PROTOTYPES = {
     # params: a TARGET_PARAMS record; samples: a TARGET_SAMPLE / TARGET_JOINTS array
     "spg_targets_warp": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
+    "spg_targets_tint": (_int, [_ptr, _ptr, _i32, _ptr]),  # samples: a TARGET_TINT array
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -883,6 +888,12 @@ class Grouper:
         p, s = self._records(params, TARGET_PARAMS), self._records(samples, TARGET_JOINTS)
         _check(self._lib.spg_targets_maps(self._h, p.ctypes.data, s.ctypes.data, len(s), self._stream_ptr(stream)),
                "spg_targets_maps", self._h)
+
+    def targets_tint(self, records: np.ndarray, stream=None) -> None:
+        """``spg_targets_tint``: ``records`` a ``TARGET_TINT`` array; each source is tinted in place on the device."""
+        s = self._records(records, TARGET_TINT)
+        _check(self._lib.spg_targets_tint(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)), "spg_targets_tint",
+               self._h)
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

@@ -14,8 +14,10 @@ two CUDA kernels (csrc/targets.cuh) through ``spg_targets_warp`` / ``spg_targets
 - ``make_batch`` builds a whole batch of samples of any source sizes in one call and returns ``gen()``'s three outputs
   stacked, on the device, without a host synchronisation.
 
-Colour distortion (``tint``: an HSV round trip with ``np.random`` draws) is not done here: apply the reference's
-``Transformer.distort_color`` to the uint8 image first and pass a selection with ``tint=False``.
+Colour distortion (``Transformer.distort_color``: an HSV round trip with three ``np.random`` draws) runs on the device
+too, through ``spg_targets_tint``, when asked for: ``make_batch(..., tint=True)`` and ``Transformer(config, tint=True)``.
+It equals cv2's result bit for bit given the row block of cv2's HSV->BGR vector loop (``TargetConfig.tint_row_block``,
+``cv2_row_block()``; DESIGN.md §4).  Without ``tint=True`` a selection with ``tint`` set is refused, as before.
 """
 from __future__ import annotations
 
@@ -58,6 +60,10 @@ class TargetConfig:
 
     def __init__(self, width: int = 512, height: int = 512, stride: int = 4):
         self.width, self.height, self.stride = int(width), int(height), int(stride)
+        #: cv2's HSV->BGR row block on the host whose results you want to match: the last ``width % tint_row_block``
+        #: pixels of every row are rounded, the others truncated (32 where OpenCV dispatches to AVX-512;
+        #: ``cv2_row_block()`` measures it)
+        self.tint_row_block = 32
         self.num_parts = NUM_PARTS
         self.limbs_conn = list(LIMBS)
         self.leftParts = [PART_NAMES.index(p) for p in _LEFT]
@@ -176,6 +182,47 @@ def _check_joints(i: int, joints: np.ndarray) -> None:
         raise ValueError(f"sample {i}: a visible joint (v < 2) has a non-finite coordinate")
 
 
+def cv2_row_block(max_width: int = 4096) -> int:
+    """The row block of the installed cv2's uint8 ``COLOR_HSV2BGR``, measured: for ``TargetConfig.tint_row_block``.
+
+    cv2 truncates ``x * 255`` in its vector loop and rounds it in the scalar tail, the last ``width % block`` pixels of
+    every row.  The probe is two rows of HSV ``(0, 1, 1)``, whose blue ``V (1 - S) * 255 ~ 0.996`` comes back 1 where
+    rounded and 0 where truncated; the block is the narrowest width at which no pixel comes back rounded.  Needs cv2
+    (the product path never imports it)."""
+    import cv2
+    for w in range(1, max_width + 1):
+        out = cv2.cvtColor(np.full((2, w, 3), (0, 1, 1), np.uint8), cv2.COLOR_HSV2BGR)[:, :, 0]
+        rounded = (out == 1).sum(axis=1)
+        if rounded[0] != rounded[1]:
+            raise RuntimeError(f"cv2's HSV->BGR rounded {rounded.tolist()} pixels in two equal rows of width {w}")
+        if rounded[0] == 0:
+            return w
+    raise RuntimeError(f"cv2's HSV->BGR rounded every pixel of rows up to {max_width} wide: no vector loop to match")
+
+
+def tint_records(images: Sequence[Tuple[int, int, int, int]], draws: Sequence[Tuple[int, int, int]],
+                 row_block: int = 32) -> np.ndarray:
+    """The ``TARGET_TINT`` records of ``images`` (per source ``(device pointer, row stride in bytes, height, width)``)
+    with ``draws`` (per source ``(hue, saturation, value)`` as drawn: 0..20, 0..80, 0..60)."""
+    recs = np.zeros(len(images), grouping.TARGET_TINT)
+    for i, ((ptr, pitch, h, w), d) in enumerate(zip(images, draws)):
+        recs[i] = (ptr, pitch, h, w, d[0], d[1], d[2], row_block)
+    return recs
+
+
+def draw_tint() -> Tuple[int, int, int]:
+    """``distort_color``'s draws from ``np.random`` in its order: hue, saturation, value."""
+    return int(np.random.randint(20 + 1)), int(np.random.randint(80 + 1)), int(np.random.randint(60 + 1))
+
+
+def _row_block(config) -> int:
+    """``config.tint_row_block`` (the reference's own config has none: 32)."""
+    b = int(getattr(config, "tint_row_block", 32))
+    if b < 1:
+        raise ValueError(f"tint_row_block must be >= 1, got {b}")
+    return b
+
+
 class _Device:
     """One handle per (device, limb table): the training-sample calls use the handle's limb table only."""
     _handles = {}
@@ -190,7 +237,7 @@ class _Device:
 
 
 def make_batch(samples: Sequence, augs: Sequence[Optional[AugmentSelection]], config=None, *, device: int = 0,
-               stream=None):
+               stream=None, tint: bool = False):
     """``gen()``'s three outputs for a batch of samples, stacked, on ``cuda:device``.
 
     ``samples``: per sample ``(img, mask_miss, mask_all, meta)`` as ``gen`` reads them -- a uint8 HxWx3 source of any
@@ -198,24 +245,33 @@ def make_batch(samples: Sequence, augs: Sequence[Optional[AugmentSelection]], co
     sample an ``AugmentSelection`` (``None``: ``AugmentSelection.random``).  Returns ``(images [N, H, W, 3],
     mask_miss [N, 1, h, w], labels [N, 50, h, w])`` float32 CUDA tensors.  One host-to-device copy for all sources and
     one for all joints, one launch per chunk of each kernel, no host synchronisation; ``meta`` is not modified.
-    Malformed input raises ``ValueError`` before anything is launched."""
+    Malformed input raises ``ValueError`` before anything is launched.
+
+    ``tint=True`` applies ``distort_color`` to the samples whose selection has ``tint`` set: each draws its three offsets
+    from ``np.random`` in sample order once the whole batch has passed validation, and one ``spg_targets_tint`` launch
+    tints their sources in the device staging buffer before the warp, with ``config.tint_row_block``.  A seeded
+    ``random`` and ``np.random`` thus give what a sequential ``gen()`` loop gives.  ``tint=False`` refuses such a
+    selection."""
     import torch
     config = TargetConfig() if config is None else config
     samples, augs = list(samples), list(augs)
     if len(augs) != len(samples):
         raise ValueError("one augmentation per sample expected")
     params = target_params(config)
+    row_block = _row_block(config) if tint else 0
     n = len(samples)
     out_h, out_w, s = int(params["out_h"][0]), int(params["out_w"][0]), config.stride
     mh, mw = out_h // s, out_w // s
     # host geometry and the two staging buffers: sources (image, mask_miss, mask_all back to back) and joints
-    geo, src_off, jnt_off = [], [0], [0]
+    geo, src_off, jnt_off, tinted = [], [0], [0], []
     for i, ((img, mask_miss, mask_all, meta), aug) in enumerate(zip(samples, augs)):
         _check_sample(i, img, mask_miss, mask_all, meta)
         aug = AugmentSelection.random(config.transform_params) if aug is None else aug
-        if aug.tint:
+        if aug.tint and not tint:
             raise ValueError(f"sample {i}: tint is not applied here; run the reference's Transformer.distort_color on "
                              "the uint8 image first and pass a selection with tint=False")
+        if aug.tint:
+            tinted.append(i)
         M, _ = aug.affine(meta['objpos'][0], meta['scale_provided'][0], config)
         joints = transform_joints(meta['joints'], M, aug.flip, config).astype(np.float32)
         _check_joints(i, joints)
@@ -223,6 +279,7 @@ def make_batch(samples: Sequence, augs: Sequence[Optional[AugmentSelection]], co
         h, w = np.asarray(img).shape[:2]
         src_off.append(src_off[-1] + h * w * 5)
         jnt_off.append(jnt_off[-1] + joints.size)
+    draws = [draw_tint() for _ in tinted]  # after validation: a refused batch consumes no draws
     dev = torch.device("cuda", device)
     g = _Device.grouper(config, device)
     src_host = torch.empty(src_off[-1], dtype=torch.uint8, pin_memory=True)
@@ -251,16 +308,40 @@ def make_batch(samples: Sequence, augs: Sequence[Optional[AugmentSelection]], co
         ws[i] = (base, base + h * w * 3, base + h * w * 4, w * 3, w, h, w, geo[i][0].reshape(6),
                  images[i].data_ptr(), miss[i].data_ptr(), all_[i].data_ptr())
         wj[i] = (jnt.data_ptr() + 4 * jnt_off[i], geo[i][1].shape[0], 0, all_[i].data_ptr(), labels[i].data_ptr())
+    if tinted:  # in place in the staging buffer, ahead of the warp on the same stream
+        shapes = [np.asarray(samples[i][0]).shape[:2] for i in tinted]
+        g.targets_tint(tint_records([(src.data_ptr() + src_off[i], 3 * w, h, w) for i, (h, w) in zip(tinted, shapes)],
+                                    draws, row_block), stream=st)
     g.targets_warp(params, ws, stream=st)
     g.targets_maps(params, wj, stream=st)  # src, jnt and all_ were allocated on st: their reuse is ordered after this
     return images, miss, labels
 
 
 class Transformer:
-    """The reference's ``Transformer``: ``transform`` warps one sample on the device and returns host arrays."""
+    """The reference's ``Transformer``: ``transform`` warps one sample on the device and returns host arrays.  With
+    ``tint=True`` it also applies ``distort_color`` when the selection asks for it, so that
+    ``py_data_iterator.Transformer = targets.Transformer`` covers the whole of the reference's ``transform``."""
 
-    def __init__(self, config, device: int = 0):
-        self.config, self.device = config, device
+    def __init__(self, config, device: int = 0, tint: bool = False):
+        self.config, self.device, self.tint = config, device, tint
+
+    @staticmethod
+    def distort_color(img, *, row_block: int = 32, device: Optional[int] = None) -> np.ndarray:
+        """The reference's ``distort_color(img)``: uint8 ``[H, W, 3]`` BGR in, the tinted uint8 image out, on the host.
+        Draws hue, saturation and value from ``np.random`` as the reference does; the HSV round trip runs on the
+        device (``cuda:device``, the current device when ``None``) with cv2's HSV->BGR ``row_block``."""
+        import torch
+        a = np.asarray(img)
+        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
+            raise ValueError(f"the source must be a uint8 HxWx3 array, got {a.dtype} {a.shape}")
+        if row_block < 1:
+            raise ValueError(f"row_block must be >= 1, got {row_block}")
+        device = torch.cuda.current_device() if device is None else int(device)
+        d = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", device))
+        h, w = a.shape[:2]
+        _Device.grouper(TargetConfig(), device).targets_tint(tint_records([(d.data_ptr(), 3 * w, h, w)], [draw_tint()],
+                                                                          row_block))
+        return d.cpu().numpy()
 
     def transform(self, img, mask_miss, mask_all, meta, aug=None):
         """``(img [H, W, 3], mask_miss [h, w], mask_all [h, w], meta)`` float32 in [0, 1], with ``meta['joints']``
@@ -268,10 +349,11 @@ class Transformer:
         import torch
         aug = AugmentSelection.random(self.config.transform_params) if aug is None else aug
         _check_sample(0, img, mask_miss, mask_all, meta)
-        if aug.tint:
+        if aug.tint and not self.tint:
             raise ValueError("tint is not applied here; run the reference's Transformer.distort_color on the uint8 "
                              "image first and pass a selection with tint=False")
         params = target_params(self.config)
+        row_block = _row_block(self.config) if aug.tint else 0
         M, _ = aug.affine(meta['objpos'][0], meta['scale_provided'][0], self.config)
         dev = torch.device("cuda", self.device)
         out_h, out_w, s = int(params["out_h"][0]), int(params["out_w"][0]), self.config.stride
@@ -279,10 +361,13 @@ class Transformer:
         out = [torch.empty(shape, dtype=torch.float32, device=dev) for shape in
                ((out_h, out_w, 3), (out_h // s, out_w // s), (out_h // s, out_w // s))]
         h, w = src[1].shape
+        g = _Device.grouper(self.config, self.device)
+        if aug.tint:  # the reference tints before it warps; np.random is drawn as its distort_color draws
+            g.targets_tint(tint_records([(src[0].data_ptr(), 3 * w, h, w)], [draw_tint()], row_block))
         rec = np.zeros(1, grouping.TARGET_SAMPLE)
         rec[0] = (src[0].data_ptr(), src[1].data_ptr(), src[2].data_ptr(), w * 3, w, h, w, M.reshape(6),
                   out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr())
-        _Device.grouper(self.config, self.device).targets_warp(params, rec)
+        g.targets_warp(params, rec)
         meta['joints'] = transform_joints(meta['joints'], M, aug.flip, self.config)
         return out[0].cpu().numpy(), out[1].cpu().numpy(), out[2].cpu().numpy(), meta
 

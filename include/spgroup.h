@@ -353,6 +353,20 @@ typedef struct spg_target_joints {
  * to [0, 1].  Each value is written once.  Validation, asynchrony and reuse of `samples` as spg_targets_warp. */
 int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_target_joints *samples, int32_t n_samples,
                      void *stream);
+/* One sample of spg_targets_tint: a uint8 BGR source tinted in place, and the reference's three draws. */
+typedef struct spg_target_tint {
+    uint8_t *image;             /* [height][width][3] uint8 device, rows row_stride bytes apart */
+    int64_t row_stride;         /* >= 3 * width */
+    int32_t height, width;
+    int32_t hue, saturation, value;  /* np.random.randint(21), randint(81), randint(61): applied as -10, -20, -20 */
+    int32_t row_block;          /* >= 1: OpenCV's HSV->BGR vector block (32 with AVX-512): the last width % row_block */
+                                /* pixels of every row are rounded to nearest, the others truncated                  */
+} spg_target_tint;
+/* Per sample, Transformer.distort_color (py_data_transformer.py:97-110) in place: cv2.cvtColor(COLOR_BGR2HSV), the
+ * draws minus (10, 20, 20) added and clamped to [0, 179] / [0, 255] / [0, 255], cv2.cvtColor(COLOR_HSV2BGR), bit for bit
+ * with OpenCV's uint8 algorithms.  Run it on the sources before spg_targets_warp reads them.  Validation (draws in range,
+ * row_stride, NULL image, row_block), asynchrony and reuse of `samples` as spg_targets_warp. */
+int spg_targets_tint(spg_handle *h, const spg_target_tint *samples, int32_t n_samples, void *stream);
 
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */

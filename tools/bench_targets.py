@@ -4,7 +4,12 @@ Prints one JSON line.  256 seeded samples at the default 512 x 512 config (128 x
 persons, random augmentations (tint off).  Kernel times are CUDA events around many launches of one kernel on the whole
 batch; a kernel's algorithmic bytes are what it must write plus the source bytes it must read, over its time, as a share
 of the H100 SXM's 3.35 TB/s.  The CPU rate is the single-process numpy port (tests/targets_port.py) on the same samples,
-or the reference's own classes when --reference points at them.  Usage:
+or the reference's own classes when --reference points at them.
+
+Colour distortion: targets_tint_kernel's time over many launches tinting every source of the batch in place (6
+algorithmic bytes per source pixel), make_batch(tint=True) samples/s with no sample tinted and with tint drawn at the
+reference's tint_prob 0.2 (the two alternated, median of --iters each), and the CPU rate of distort_color on the same
+sources (the reference's with --reference, else its cv2 calls restated).  Usage:
     python tools/bench_targets.py [--samples 256] [--iters 20] [--cpu-samples 16] [--reference DIR]
 """
 from __future__ import annotations
@@ -120,6 +125,28 @@ def main():
     t_maps = timed(lambda: g.targets_maps(params, wj))
     warp_bytes = n * (H * W * 3 * 4 + 2 * m * m * 4) + src_bytes
     maps_bytes = n * (50 * m * m * 4 + m * m * 4) + sum(j.numel() * 4 for j in joints)
+    # colour distortion: every source of the batch tinted in place, repeatedly (6 bytes per pixel: read and write BGR)
+    drng = np.random.default_rng(1)
+    tint_recs = targets.tint_records([(s[0].data_ptr(), 3 * s[0].shape[1], s[0].shape[0], s[0].shape[1]) for s in srcs],
+                                     [tuple(int(v) for v in drng.integers(0, (21, 81, 61))) for _ in srcs],
+                                     cfg.tint_row_block)
+    t_tint = timed(lambda: g.targets_tint(tint_recs))
+    tint_px = sum(s[0].shape[0] * s[0].shape[1] for s in srcs)
+    # make_batch at the reference's tint_prob 0.2 and at 0, alternated so that both see the same host and device state
+    trng = np.random.default_rng(2)
+    augs_tint = []
+    for aug in augs:
+        t = targets.AugmentSelection(aug.flip, bool(trng.random() < cfg.transform_params.tint_prob), aug.degree, aug.crop,
+                                     aug.scale)
+        augs_tint.append(t)
+    rates = {0.0: [], 0.2: []}
+    for _ in range(a.iters):
+        for prob, aa in ((0.0, augs), (0.2, augs_tint)):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = targets.make_batch(samples, aa, cfg, tint=True)
+            torch.cuda.synchronize()
+            rates[prob].append(n / (time.perf_counter() - t0))
     # CPU: the numpy port (or the reference's classes) on the first samples, one process
     k = min(a.cpu_samples, n)
     t0 = time.perf_counter()
@@ -142,6 +169,25 @@ def main():
             tp.label_maps(jt, pma, skeleton.LIMBS, 4, 9, 7, 0.015, 4, 14)
         cpu_what = "numpy port"
     cpu_rate = k / (time.perf_counter() - t0)
+    # CPU colour distortion: the reference's Transformer.distort_color (or its cv2 calls restated, without --reference)
+    # on the same sources, one process
+    try:
+        import cv2  # noqa: F401
+        if a.reference:
+            distort, dc_what = tr.Transformer.distort_color, "reference distort_color"
+        else:
+            def distort(img):
+                hsv = cv2.cvtColor(img, cv2.COLOR_BGR2HSV).astype(np.int16)
+                for ch, (hi, off, top) in enumerate(((20, 10, 179), (80, 20, 255), (60, 20, 255))):
+                    hsv[:, :, ch] = np.maximum(np.minimum(hsv[:, :, ch] - off + np.random.randint(hi + 1), top), 0)
+                return cv2.cvtColor(hsv.astype(np.uint8), cv2.COLOR_HSV2BGR)
+            dc_what = "distort_color's cv2 calls"
+        t0 = time.perf_counter()
+        for s in samples[:k]:
+            distort(s[0])
+        dc_rate = round(k / (time.perf_counter() - t0), 1)
+    except ImportError as e:
+        dc_rate, dc_what = None, f"not measured ({e})"
     del out
     print(json.dumps({
         "gpu": name, "power_limit": power, "samples": n, "config": f"{W}x{H}, stride {cfg.stride}",
@@ -149,7 +195,12 @@ def main():
         "targets_warp_kernel_ms": round(t_warp * 1e3, 3), "targets_maps_kernel_ms": round(t_maps * 1e3, 3),
         "kernel_samples_per_s": round(n / (t_warp + t_maps), 1),
         "warp_hbm_share": round(warp_bytes / t_warp / HBM, 3), "maps_hbm_share": round(maps_bytes / t_maps / HBM, 3),
-        "cpu_samples_per_s": round(cpu_rate, 2), "cpu": cpu_what, "cpu_samples": k}))
+        "cpu_samples_per_s": round(cpu_rate, 2), "cpu": cpu_what, "cpu_samples": k,
+        "targets_tint_kernel_ms": round(t_tint * 1e3, 3), "tint_hbm_share": round(6 * tint_px / t_tint / HBM, 3),
+        "make_batch_samples_per_s_tint_prob_0": round(float(np.median(rates[0.0])), 1),
+        "make_batch_samples_per_s_tint_prob_0.2": round(float(np.median(rates[0.2])), 1),
+        "tinted_samples_at_0.2": sum(t.tint for t in augs_tint),
+        "cpu_distort_color_per_s": dc_rate, "cpu_distort_color": dc_what}))
 
 
 if __name__ == "__main__":
