@@ -177,6 +177,26 @@ __device__ __forceinline__ void mbar_wait_sleep(uint64_t *bar, uint32_t parity, 
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Ragged launches: one launch covers many members (images, items or samples) whose descriptors travel in a table passed
+// as a __grid_constant__ kernel parameter, so a call returns with nothing of the caller's left to copy.  grid.x walks the
+// members' CTAs back to back; member k starts at img[k].first_cta (increasing).  A table fits the kernel-parameter limit
+// (CUDA 12.1 and later) together with the launch's other arguments.
+// ---------------------------------------------------------------------------------------------
+constexpr int kParamBytes = 32764;
+
+// the member whose CTAs hold CTA `cta`: the last one whose first CTA is <= cta
+template <class R>
+__device__ __forceinline__ const auto &ragged_member(const R &r, int cta) {
+    int lo = 0, hi = r.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (r.img[mid].first_cta <= cta) lo = mid;
+        else hi = mid - 1;
+    }
+    return r.img[lo];
+}
+
 // numpy's pairwise summation order for 8 <= n <= 128 (and the plain loop for n < 8): what both
 // `score_box.sum()` (f32) and `(score_box * grid).sum()` (f64) use in utils/util.py:206-211.
 template <typename T>

@@ -29,7 +29,7 @@
 
 #include <cuda_fp16.h>
 
-#include "common.cuh"
+#include "interp.cuh"
 
 namespace spg {
 
@@ -49,60 +49,45 @@ struct PostScale {              // one entry of the scale loop (evaluate.py:90)
     double sx2, sy2;            // source step per destination pixel of the resize to the image
 };
 
+// What every image of a launch shares.
 struct PostArgs {
-    PostScale sc[kPostMaxScales];  // the scales summed inside ONE launch, in the order of the scale loop (stride 4 fuses up to
-                                   // kPostMaxScales; the generic and the rotated kernel take one)
-    int n_fused;                // entries of `sc` in this launch; scale_index is the index of sc[0] in the whole loop
-    int H, W;                   // image size = output size
+    int scale_index, n_scales;  // accumulate over the scale loop (:160-161)
+    int n_fused;                // items (scales) summed inside ONE launch (stride 4 fuses up to kPostMaxScales; the generic
+                                // and the rotated kernel take one); scale_index is the index of the first in the whole loop
     int n_out;                  // output channels handled: K keypoint + L body-part
     int K;                      // first K outputs are keypoint channels
     short src_chan[kMaxNetChannels];   // network channel of output c (keypoints: heat_chan0 + c; body parts: paf_chan0 + k)
     short flip_chan[kMaxNetChannels];  // network channel of the mirrored output that is averaged into output c
-    float *heat;                // [N][K][H][W] float32 (what find_peaks reads after its cast, evaluate.py:173)
-    void *paf;                  // [N][L][H][W] float32 (single scale: the float64 values are exact float32) or float64
-    double *heat_acc;           // [N][K][H][W] float64 scratch, only for n_scales > 1
     int paf_is_f64;
-    int scale_index, n_scales;  // accumulate over the scale loop (:160-161)
     int nan_scrub;              // demo_image.py:179-180: NaN -> 0 after the accumulation
-    int tile_w, tile_h, tiles_x, tiles_y;
     int chan_chunk;             // stride-4 kernel: channels one CTA walks over (grid.y = ceil(n_out / chan_chunk))
     double sx1, sy1;            // source step per destination pixel of the x stride resize (the second resize's: sc[t])
-    double rot[6];              // postnet_rot_kernel: the inverse of the item's warp matrix (x4 grid of the output -> of the input)
 };
 
-// interpolateCubic (imgproc/src/resize.cpp), float32, exactly oracle/postnet_port.py::cubic_coeffs
-__device__ __forceinline__ void cubic_coeffs(float x, float c[4]) {
-    const float A = -0.75f;
-    const float x1 = __fadd_rn(x, 1.0f);
-    c[0] = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, x1), __fmul_rn(5.0f, A)), x1), __fmul_rn(8.0f, A)), x1), __fmul_rn(4.0f, A));
-    const float a2 = __fadd_rn(A, 2.0f), a3 = __fadd_rn(A, 3.0f);
-    c[1] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(a2, x), a3), x), x), 1.0f);
-    const float y = __fsub_rn(1.0f, x);
-    c[2] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(a2, y), a3), y), y), 1.0f);
-    c[3] = __fsub_rn(__fsub_rn(__fsub_rn(1.0f, c[0]), c[1]), c[2]);
-}
-
-// destination index d of an axis -> first tap (s - 1, unclamped) and the four weights
-__device__ __forceinline__ int axis_entry(int d, double scale, float c[4]) {
-    const float f = (float)__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5);  // fx = (float)((dx+0.5)*scale_x - 0.5)
-    const float fl = floorf(f);
-    cubic_coeffs(__fsub_rn(f, fl), c);
-    return (int)fl - 1;
-}
+// One image of a launch and the launch's items of it.  The per-launch kernels take one for all grid.z = N images of one
+// size (pointers to slot 0; slot n is n planes further), the ragged kernels a table of them.
+struct PostImage {
+    PostScale sc[kPostMaxScales];  // the items of the launch, in the order of the scale loop (a.n_fused of them)
+    int H, W;                   // image size = output size
+    float *heat;                // [K][H][W] float32 (what find_peaks reads after its cast, evaluate.py:173)
+    void *paf;                  // [L][H][W] float32 (single scale: the float64 values are exact float32) or float64
+    double *heat_acc;           // [K][H][W] float64 scratch of sums that outlive a launch, or nullptr
+    int tile_w, tile_h, tiles_x, tiles_y;
+    int first_cta;              // ragged launches: the first CTA (blockIdx.x) of the image's tiles
+    double rot[6];              // rotated items: the inverse of the warp matrix (x4 grid of the output -> of the input)
+};
 
 __device__ __forceinline__ float tap4(float a0, float a1, float a2, float a3, const float *c) {
     // taps summed left to right, every product and sum rounded to float32
     return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a0, c[0]), __fmul_rn(a1, c[1])), __fmul_rn(a2, c[2])), __fmul_rn(a3, c[3]));
 }
 
-__device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
-
 struct AxisTab {  // per destination index of a tile: first tap (absolute source index, unclamped) + weights
     int s;
     float c[4];
 };
 
-__global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs a) {
+__global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs a, PostImage im) {
     __shared__ AxisTab t2x[kPostTW], t2y[kPostTH], t1x[kPostC1], t1y[kPostR1];
     __shared__ float s0[kPostRS * kPostCS];     // source tile, flip-averaged
     __shared__ float s1[kPostRS * kPostC1];     // after the horizontal x stride pass
@@ -112,11 +97,11 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
 
     const int tid = threadIdx.x;
     const int tile = blockIdx.x, c = blockIdx.y, n = blockIdx.z;
-    const int ty = tile / a.tiles_x, tx = tile - ty * a.tiles_x;
-    const int ox0 = tx * a.tile_w, oy0 = ty * a.tile_h;
-    const int tw = min(a.tile_w, a.W - ox0), th = min(a.tile_h, a.H - oy0);
-    const PostScale &S = a.sc[0];
-    const bool identity = S.crop_h == a.H && S.crop_w == a.W;  // second resize with scale 1: weights (0, 1, 0, 0)
+    const int ty = tile / im.tiles_x, tx = tile - ty * im.tiles_x;
+    const int ox0 = tx * im.tile_w, oy0 = ty * im.tile_h;
+    const int tw = min(im.tile_w, im.W - ox0), th = min(im.tile_h, im.H - oy0);
+    const PostScale &S = im.sc[0];
+    const bool identity = S.crop_h == im.H && S.crop_w == im.W;  // second resize with scale 1: weights (0, 1, 0, 0)
 
     // ---- tables of the second resize for this tile's output columns / rows
     if (tid < tw) t2x[tid].s = axis_entry(ox0 + tid, S.sx2, t2x[tid].c);
@@ -191,7 +176,7 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
     }
     // ---- pass 4 + epilogue: vertical pass, / n in float32, float64 accumulation over the scale loop (:160-161)
     const float nf = (float)a.n_scales;
-    const size_t plane = (size_t)a.H * a.W;
+    const size_t plane = (size_t)im.H * im.W;
     const bool is_heat = c < a.K;
     const size_t pbase = is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane;
     const bool first = a.scale_index == 0, last = a.scale_index == a.n_scales - 1;
@@ -206,19 +191,19 @@ __global__ void __launch_bounds__(kPostThreads) postnet_generic_kernel(PostArgs 
             v = tap4(col[clampi(t.s, 0, S.crop_h - 1) * kPostTW], col[clampi(t.s + 1, 0, S.crop_h - 1) * kPostTW],
                      col[clampi(t.s + 2, 0, S.crop_h - 1) * kPostTW], col[clampi(t.s + 3, 0, S.crop_h - 1) * kPostTW], t.c);
         }
-        const size_t o = pbase + (size_t)(oy0 + y) * a.W + (ox0 + x);
+        const size_t o = pbase + (size_t)(oy0 + y) * im.W + (ox0 + x);
         const float part = __fdiv_rn(v, nf);  // float32 array / Python int -> float32
         if (a.n_scales == 1) {  // avg = 0.0 + part: exact, the float64 value is the float32 one
             const float r = (a.nan_scrub && part != part) ? 0.0f : part;
-            if (is_heat) a.heat[o] = r;
-            else if (a.paf_is_f64) static_cast<double *>(a.paf)[o] = (double)r;
-            else static_cast<float *>(a.paf)[o] = r;
+            if (is_heat) im.heat[o] = r;
+            else if (a.paf_is_f64) static_cast<double *>(im.paf)[o] = (double)r;
+            else static_cast<float *>(im.paf)[o] = r;
         } else {
-            double *acc = is_heat ? a.heat_acc : static_cast<double *>(a.paf);
+            double *acc = is_heat ? im.heat_acc : static_cast<double *>(im.paf);
             double s = __dadd_rn(first ? 0.0 : acc[o], (double)part);
             if (a.nan_scrub && s != s) s = 0.0;  // demo_image.py:179-180 scrubs after every scale
             acc[o] = s;
-            if (is_heat && last) a.heat[o] = (float)s;  // find_peaks: heatmap_avg.astype(np.float32)
+            if (is_heat && last) im.heat[o] = (float)s;  // find_peaks: heatmap_avg.astype(np.float32)
         }
     }
 }
@@ -466,39 +451,6 @@ __device__ __forceinline__ void post_resize2_h(const PostTabs &T, const float *s
     }
 }
 
-// One image of a ragged launch (postnet_ragged_kernel, postnet_x4_ident_ragged_kernel): one scale, its output planes
-// [K][H][W] / [L][H][W], its own tiling, and the first CTA (blockIdx.x) of its tiles in the launch.  The helpers and
-// kernel bodies below read an image's fields from `im`: the per-launch kernels pass their PostArgs (the same field
-// names), the ragged kernels their image's PostImage.
-struct PostImage {
-    PostScale sc[1];
-    int H, W;
-    float *heat;
-    void *paf;
-    int tile_w, tile_h, tiles_x, tiles_y;
-    int first_cta;
-};
-
-// One image of a multi-item ragged launch (postnet_items_ragged_kernel, postnet_rot_ragged_kernel): the image's items in
-// this launch's group (a.n_fused of them; the rotated kernel takes one), its own float64 keypoint sums and, for a rotated
-// item, its own inverse warp matrix (the rotation centre depends on the image's padded size).
-struct PostItemsImage {
-    PostScale sc[kPostMaxScales];
-    int H, W;
-    float *heat;
-    void *paf;
-    double *heat_acc;           // [K][H][W] float64 scratch of sums that outlive a launch, or nullptr
-    int tile_w, tile_h, tiles_x, tiles_y;
-    int first_cta;
-    double rot[6];
-};
-
-// The float64 keypoint sums that outlive a launch: the launch's scratch (slot n of it) for the per-launch and the
-// single-item ragged kernels, the image's own for the multi-item ragged kernels.
-__device__ __forceinline__ double *post_heat_acc(const PostArgs &a, const PostArgs &) { return a.heat_acc; }
-__device__ __forceinline__ double *post_heat_acc(const PostArgs &a, const PostImage &) { return a.heat_acc; }
-__device__ __forceinline__ double *post_heat_acc(const PostArgs &, const PostItemsImage &im) { return im.heat_acc; }
-
 // Where channel c of image n goes: one base pointer per dtype (32-bit offsets from it per thread; the dtype branches are
 // block-uniform), and whether the values stored are float32.
 struct PostOut {
@@ -507,24 +459,23 @@ struct PostOut {
     double *d;
     bool store_f;
 };
-template <class I>
-__device__ __forceinline__ PostOut post_out(const PostArgs &a, const I &im, int n, int c, int ox0, int oy0, bool more_follow) {
+__device__ __forceinline__ PostOut post_out(const PostArgs &a, const PostImage &im, int n, int c, int ox0, int oy0, bool more_follow) {
     const size_t plane = (size_t)im.H * im.W;
     const bool is_heat = c < a.K;
     PostOut o;
     o.pbase = (is_heat ? ((size_t)n * a.K + c) * plane : ((size_t)n * (a.n_out - a.K) + (c - a.K)) * plane) + (size_t)oy0 * im.W + ox0;
     o.f = is_heat ? im.heat + o.pbase : static_cast<float *>(im.paf) + o.pbase;
-    o.d = (is_heat ? post_heat_acc(a, im) : static_cast<double *>(im.paf)) + (is_heat && post_heat_acc(a, im) == nullptr ? 0 : o.pbase);
+    o.d = (is_heat ? im.heat_acc : static_cast<double *>(im.paf)) + (is_heat && im.heat_acc == nullptr ? 0 : o.pbase);
     o.store_f = is_heat ? !more_follow : !a.paf_is_f64;
     return o;
 }
 
 // continuing a scale loop longer than one launch: the float64 sums so far
-template <bool SINGLE, class I>
-__device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, const I &im,
+template <bool SINGLE>
+__device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostArgs &a, const PostImage &im,
                                               int c, size_t pbase, int tw, int th, int lane, int warp) {
     if (!SINGLE && a.scale_index > 0) {
-        const double *prev = c < a.K ? post_heat_acc(a, im) : static_cast<const double *>(im.paf);
+        const double *prev = c < a.K ? im.heat_acc : static_cast<const double *>(im.paf);
 #pragma unroll
         for (int ky = 0; ky < kPostKY; ky++)
 #pragma unroll
@@ -538,9 +489,9 @@ __device__ __forceinline__ void post_load_acc(double (&acc)[SINGLE ? 1 : kPostKY
 // Pass 4 and epilogue: vertical pass of the second resize (s3; with an identity second resize the crop itself, s2),
 // / n in float32, float64 sum over the scale loop (:160-161) in registers.  SINGLE: the maps are stored from here.
 // (c_org, y_org) is the crop position of element 0 of s2.
-template <bool SINGLE, bool IDENT, class I>
+template <bool SINGLE, bool IDENT>
 __device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostTabs &T,
-                                               const float *s2, const float *s3, bool identity, const PostArgs &a, const I &im,
+                                               const float *s2, const float *s3, bool identity, const PostArgs &a, const PostImage &im,
                                                const PostOut &out,
                                                int ox0, int oy0, int tw, int th, int c_org, int y_org, bool zero_start,
                                                float nf, float nf_rcp, bool nf_small, int lane, int warp) {
@@ -596,8 +547,8 @@ __device__ __forceinline__ void post_resize2_v(double (&acc)[SINGLE ? 1 : kPostK
 }
 
 // the averaged maps, written once: keypoint maps as float32 (find_peaks' cast, :173), body parts float64 / float32
-template <bool SINGLE, class I>
-__device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const I &im,
+template <bool SINGLE>
+__device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : kPostKY][SINGLE ? 1 : kPostKX], const PostImage &im,
                                                const PostOut &out, int tw, int th, int lane, int warp) {
     if (!SINGLE) {
 #pragma unroll
@@ -621,8 +572,8 @@ __device__ __forceinline__ void post_store_acc(const double (&acc)[SINGLE ? 1 : 
 // IDENT: every fused scale's second resize is the identity (crop == image: weights (0,1,0,0)) -- passes 3 and 4 fall away.
 // F16: the network output is float16.
 // One CTA: tile `tile` of image `im` (slot n of its output planes), channel chunk `chunk`.
-template <bool SINGLE, bool IDENT, bool F16, class I>
-__device__ __forceinline__ void postnet_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
+template <bool SINGLE, bool IDENT, bool F16>
+__device__ __forceinline__ void postnet_tile(const PostArgs &a, const PostImage &im, int tile, int chunk, int n) {
     constexpr int kTabs = SINGLE ? 1 : kPostMaxScales;
     extern __shared__ __align__(16) unsigned char post_smem[];
     PostTabs *TT = reinterpret_cast<PostTabs *>(post_smem);
@@ -690,8 +641,8 @@ __device__ __forceinline__ void postnet_tile(const PostArgs &a, const I &im, int
 }
 
 template <bool SINGLE, bool IDENT, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a) {
-    postnet_tile<SINGLE, IDENT, F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_kernel(PostArgs a, PostImage im) {
+    postnet_tile<SINGLE, IDENT, F16>(a, im, blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -718,45 +669,9 @@ constexpr size_t postR_smem_bytes() {
 }
 static_assert(kPostR_R1 * kPostTW <= kPostF_RS * (kPostF_CS + kPostF_C1), "pass 3's output fits where the source tile was");
 
-// One destination pixel of warpAffine's INTER_LINEAR (imgproc/src/imgwarp.cpp) on a w x h grid: (xs, ys) are its source
-// coordinates in OpenCV's fixed point, X0 + adelta and Y0 + bdelta (1/1024 px, the +16 rounding term included).  The grid's
-// value (y, x) is val(g[(y - y0) * pitch + (x - x0) * CS]); taps outside the grid read 0 (BORDER_CONSTANT) and are never
-// loaded.  Every product and sum is rounded to float32, left to right.  Shared by the inverse warp of the maps
-// (postnet_rot_kernel) and the forward warp of the input image (prenet.cuh).
-// (xs, ys) -> the top-left tap (sx, sy) and the 1/32 px fractions (ax, ay) of warpAffine's INTER_TAB_SIZE table; shared
-// with the uint8 tap combine of the training-sample warp (targets.cuh)
-struct WarpTap {
-    int sx, sy, ax, ay;
-};
-__device__ __forceinline__ WarpTap warp_tap(int xs, int ys) {
-    const int xf = xs >> 5, yf = ys >> 5;
-    return {clampi(xf >> 5, -32768, 32767), clampi(yf >> 5, -32768, 32767), xf & 31, yf & 31};  // saturate_cast<short>
-}
-// warpAffine's fixed-point source coordinates (X0 + adelta, Y0 + bdelta, the +16 rounding term included) of destination
-// pixel (x, y) under the inverted matrix m (rounded ties-to-even like cvRound)
-__device__ __forceinline__ void warp_coords(const double m[6], int x, int y, int &xs, int &ys) {
-    const double xd = (double)x, yd = (double)y;
-    xs = __double2int_rn(__dmul_rn(__dmul_rn(m[0], xd), 1024.0)) + __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], yd), m[2]), 1024.0)) + 16;
-    ys = __double2int_rn(__dmul_rn(__dmul_rn(m[3], xd), 1024.0)) + __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], yd), m[5]), 1024.0)) + 16;
-}
-template <int CS, typename T, typename Val>
-__device__ __forceinline__ float warp_linear(int xs, int ys, int w, int h, const T *g, int pitch, int x0, int y0, const Val &val) {
-    const WarpTap t = warp_tap(xs, ys);
-    const int sx = t.sx, sy = t.sy;
-    const float fx = __fmul_rn((float)t.ax, 0.03125f), fy = __fmul_rn((float)t.ay, 0.03125f);
-    const float gx = __fsub_rn(1.0f, fx), gy = __fsub_rn(1.0f, fy);
-    const bool x0in = sx >= 0 && sx < w, x1in = sx + 1 >= 0 && sx + 1 < w;
-    const bool y0in = sy >= 0 && sy < h, y1in = sy + 1 >= 0 && sy + 1 < h;
-    const T *u = g + (sy - y0) * pitch + (sx - x0) * CS;
-    const float t00 = (y0in && x0in) ? val(u[0]) : 0.0f, t01 = (y0in && x1in) ? val(u[CS]) : 0.0f;
-    const float t10 = (y1in && x0in) ? val(u[pitch]) : 0.0f, t11 = (y1in && x1in) ? val(u[pitch + CS]) : 0.0f;
-    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t00, __fmul_rn(gy, gx)), __fmul_rn(t01, __fmul_rn(gy, fx))),
-                               __fmul_rn(t10, __fmul_rn(fy, gx))), __fmul_rn(t11, __fmul_rn(fy, fx)));
-}
-
 // One CTA: tile `tile` of the rotated item of image `im` (slot n of its output planes), channel chunk `chunk`.
-template <bool SINGLE, bool F16, class I>
-__device__ __forceinline__ void postnet_rot_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
+template <bool SINGLE, bool F16>
+__device__ __forceinline__ void postnet_rot_tile(const PostArgs &a, const PostImage &im, int tile, int chunk, int n) {
     extern __shared__ __align__(16) unsigned char post_smem[];
     PostTabs &T = *reinterpret_cast<PostTabs *>(post_smem);
     float *s0 = reinterpret_cast<float *>(post_smem + sizeof(PostTabs));  // source tile, flip-averaged [RS][kPostF_CS]
@@ -842,8 +757,8 @@ __device__ __forceinline__ void postnet_rot_tile(const PostArgs &a, const I &im,
 }
 
 template <bool SINGLE, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a) {
-    postnet_rot_tile<SINGLE, F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_kernel(PostArgs a, PostImage im) {
+    postnet_rot_tile<SINGLE, F16>(a, im, blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -862,8 +777,8 @@ constexpr int kPostI_S0 = kPostI_CS;                // row stride of the source 
 constexpr int kPostI_LD = (kPostI_RS * kPostI_CS + kPostThreads - 1) / kPostThreads;  // source elements per thread
 
 // One CTA: tile `tile` of image `im` (slot n of its output planes), channel chunk `chunk`.
-template <bool F16, class I>
-__device__ __forceinline__ void postnet_x4_ident_tile(const PostArgs &a, const I &im, int tile, int chunk, int n) {
+template <bool F16>
+__device__ __forceinline__ void postnet_x4_ident_tile(const PostArgs &a, const PostImage &im, int tile, int chunk, int n) {
     __shared__ float s0[2][kPostI_RS * kPostI_S0];                  // source tile, flip-averaged
     __shared__ __align__(16) float s1[2][kPostI_RS * kPostI_TW];   // after the horizontal pass
     __shared__ int s_o1x[kPostI_Q + 1][5], s_o1y[kPostI_P][5];
@@ -1046,73 +961,49 @@ __device__ __forceinline__ void postnet_x4_ident_tile(const PostArgs &a, const I
 }
 
 template <bool F16>
-__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostArgs a) {
-    postnet_x4_ident_tile<F16>(a, a, blockIdx.x, blockIdx.y, blockIdx.z);
+__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_kernel(PostArgs a, PostImage im) {
+    postnet_x4_ident_tile<F16>(a, im, blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Ragged batches: one single-scale, unrotated, stride-4 item per image, images of different sizes in one launch (what
-// predict() runs per image, for a batch of images).  grid.x walks the images' tiles back to back, grid.y the channel
-// chunks (one chunk size per launch).  Each CTA runs the per-launch kernel's body on its image's geometry, so every image
-// gets exactly the maps a launch of its own gives it.  The host puts identity items (crop == image) and the others in
-// separate launches, largest image first.
-// Images per launch; the descriptors travel as a kernel parameter (PostArgs + 64 x 136 B, inside the 32 764 bytes CUDA
-// 12.1 allows), so a call returns with nothing of the caller's left to copy.
-constexpr int kPostRaggedMaxImages = 64;
-struct PostRagged {
+// Ragged batches (predict() for a batch of images of different sizes, with one item or several items -- the
+// multi-scale and rotation search -- each): every image has the same items (one product(multiplier, rotate_angle)), so
+// a launch covers one group of items -- up to kPostMaxScales fused unrotated items, or one item when any is rotated --
+// for many images.  grid.x walks the images' tiles back to back, grid.y the channel chunks (one chunk size per launch).
+// The float64 sums of the items in one launch stay in registers (postnet_tile); sums that outlive a launch go through
+// each image's own keypoint scratch (PostImage::heat_acc) and its float64 body-part planes.  Each CTA runs the
+// per-launch kernel's body on its image's geometry: every image gets exactly the maps spg_postnet_rotated gives it
+// alone.  Images per launch: as many descriptors as fit next to PostArgs in the kernel parameters.
+constexpr int kPostTableImages = (int)((kParamBytes - sizeof(PostArgs) - 8) / sizeof(PostImage));
+struct PostTable {
     int n;                                  // images of this launch
-    PostImage img[kPostRaggedMaxImages];    // first_cta increasing
+    PostImage img[kPostTableImages];        // first_cta increasing
 };
-
-// the image whose tiles hold CTA `cta`: the last one whose first CTA is <= cta
-template <class R>
-__device__ __forceinline__ const auto &post_ragged_image(const R &r, int cta) {
-    int lo = 0, hi = r.n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (r.img[mid].first_cta <= cta) lo = mid;
-        else hi = mid - 1;
-    }
-    return r.img[lo];
-}
+static_assert(sizeof(PostArgs) + sizeof(PostTable) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
 
 template <bool F16>
-__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_ragged_kernel(PostArgs a, const __grid_constant__ PostRagged r) {
-    const PostImage &im = post_ragged_image(r, blockIdx.x);
+__global__ void __launch_bounds__(kPostThreads, 4) postnet_x4_ident_ragged_kernel(PostArgs a, const __grid_constant__ PostTable r) {
+    const PostImage &im = ragged_member(r, blockIdx.x);
     postnet_x4_ident_tile<F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 
+// The four-phase body as two kernels, one item per image and fused items, so that spg_stage_kernel's names (the kernels'
+// own) tell the two schedules apart.
 template <bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_ragged_kernel(PostArgs a, const __grid_constant__ PostRagged r) {
-    const PostImage &im = post_ragged_image(r, blockIdx.x);
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_ragged_kernel(PostArgs a, const __grid_constant__ PostTable r) {
+    const PostImage &im = ragged_member(r, blockIdx.x);
     postnet_tile<true, false, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Ragged batches of multi-item images (predict()'s multi-scale and rotation search for a batch of images): every image
-// has the same items (one product(multiplier, rotate_angle)), so a launch covers one group of items -- up to
-// kPostMaxScales fused unrotated items, or one item when any is rotated -- for many images of different sizes.  The
-// float64 sums of the items in one launch stay in registers (postnet_tile); sums that outlive a launch go through each
-// image's own keypoint scratch (PostItemsImage::heat_acc) and its float64 body-part planes.  Each CTA runs the per-launch
-// kernel's body on its image's geometry: every image gets exactly the maps spg_postnet_rotated gives it alone.
-// Images per launch: as many descriptors as fit next to PostArgs in the 32 764 bytes of kernel parameters.
-constexpr int kPostParamBytes = 32764;
-constexpr int kPostItemsMaxImages = (int)((kPostParamBytes - sizeof(PostArgs) - 8) / sizeof(PostItemsImage));
-struct PostItemsRagged {
-    int n;                                      // images of this launch
-    PostItemsImage img[kPostItemsMaxImages];    // first_cta increasing
-};
-static_assert(sizeof(PostArgs) + sizeof(PostItemsRagged) <= kPostParamBytes, "a launch's parameters fit the kernel-parameter limit");
-
 template <bool IDENT, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_items_ragged_kernel(PostArgs a, const __grid_constant__ PostItemsRagged r) {
-    const PostItemsImage &im = post_ragged_image(r, blockIdx.x);
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_items_ragged_kernel(PostArgs a, const __grid_constant__ PostTable r) {
+    const PostImage &im = ragged_member(r, blockIdx.x);
     postnet_tile<false, IDENT, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 
 template <bool SINGLE, bool F16>
-__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_ragged_kernel(PostArgs a, const __grid_constant__ PostItemsRagged r) {
-    const PostItemsImage &im = post_ragged_image(r, blockIdx.x);
+__global__ void __launch_bounds__(kPostThreads, 2) postnet_rot_ragged_kernel(PostArgs a, const __grid_constant__ PostTable r) {
+    const PostImage &im = ragged_member(r, blockIdx.x);
     postnet_rot_tile<SINGLE, F16>(a, im, blockIdx.x - im.first_cta, blockIdx.y, 0);
 }
 

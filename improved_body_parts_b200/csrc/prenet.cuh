@@ -21,13 +21,13 @@
 // The stage is ragged: a launch covers many members -- one (scale, angle) item of one source image each -- whose
 // sources and padded sizes may all differ.  Each member has a descriptor (PreMember) in a table that travels as the
 // kernel parameter; grid.x walks each member's CTAs (one per kPreThreads pixels of one padded row) back to back, and a
-// CTA finds its member by binary search over the table's first_cta (post_ragged_image).  A CTA belongs to one member.
+// CTA finds its member by binary search over the table's first_cta (ragged_member).  A CTA belongs to one member.
 // Unrotated members are one launch of prenet_kernel<false>: a thread computes one padded pixel straight from the source
 // and stores it to the image and to the mirror.  Rotated members first write their padded uint8 images to the handle's
 // scratch grid (prenet_resize_kernel); prenet_kernel<true> then warps from the grid.  Every output float is stored once.
 #pragma once
 
-#include "postnet.cuh"
+#include "interp.cuh"
 
 namespace spg {
 
@@ -52,19 +52,16 @@ struct PreMember {
     int first_cta;                 // the member's first grid.x position in its launch
 };
 
-// Members per launch: as many descriptors as fit in the 32 764 bytes of kernel parameters, so a call returns with nothing
-// of the caller's left to copy.
-constexpr int kPreParamBytes = 32764;
-constexpr int kPreMaxMembers = (int)((kPreParamBytes - 8) / sizeof(PreMember));
+constexpr int kPreMaxMembers = (int)((kParamBytes - 8) / sizeof(PreMember));
 struct PreRagged {
     int n;                                // members of this launch
     PreMember img[kPreMaxMembers];        // first_cta increasing
 };
-static_assert(sizeof(PreRagged) <= kPreParamBytes, "a launch's parameters fit the kernel-parameter limit");
+static_assert(sizeof(PreRagged) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
 
 // the member of CTA blockIdx.x and the pixel (y, x) of its padded image this thread computes
 __device__ __forceinline__ const PreMember &prenet_member(const PreRagged &r, int &y, int &x) {
-    const PreMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const PreMember &a = ragged_member(r, (int)blockIdx.x);
     const int cta = (int)blockIdx.x - a.first_cta;
     y = cta / a.tiles_x;
     x = (cta - y * a.tiles_x) * kPreThreads + (int)threadIdx.x;

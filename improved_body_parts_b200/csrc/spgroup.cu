@@ -144,27 +144,57 @@ int launch(spg_handle *h, int stage, const char *name, void (*kern)(P...), dim3 
     return SPG_OK;
 }
 
-// The training-sample launches (spg_targets_warp / spg_targets_maps / spg_targets_tint): sample i takes ctas[i] CTAs;
-// launches of up to `per_launch` samples and 2^31 - 1 CTAs back to back, each with its member table as the parameter.
-// With one CTA count for every sample, a launch holds min(per_launch, (2^31 - 1) / count) samples.
-template <class R, class M>
-int targets_launch(spg_handle *h, const char *name, void (*kern)(R), R &r, const std::vector<M> &ms, int per_launch,
-                   const std::vector<long long> &ctas, cudaStream_t st) {
-    if (ms.empty()) return SPG_OK;
-    for (long long c : ctas)
-        if (c > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "a sample's %lld CTAs are above grid.x's 2^31 - 1", c);
-    DeviceGuard guard(h->device);
-    for (size_t i = 0; i < ms.size();) {
-        long long total = 0;
-        r.n = 0;
-        while (i < ms.size() && r.n < per_launch && total + ctas[i] <= 0x7fffffffLL) {
-            r.img[r.n] = ms[i];
-            r.img[r.n].first_cta = (int)total;
-            total += ctas[i++];
-            r.n++;
+// Every ragged launch's table boundaries: given each member's CTA count, consecutive ranges of at most `capacity`
+// members (the kernel's table) and at most 2^31 - 1 CTAs (grid.x), and each member's first CTA inside its range.  Fails
+// only when one member alone has more CTAs than grid.x holds; it is named as `what` and ids[i] (nullptr: its position).
+struct RaggedRange {
+    size_t begin, end;  // members [begin, end)
+    unsigned ctas;      // grid.x
+};
+int deal_ragged(spg_handle *h, const std::vector<long long> &ctas, size_t capacity, const char *what, const int *ids,
+                std::vector<RaggedRange> &ranges, std::vector<int> &first_cta) {
+    ranges.clear();
+    first_cta.assign(ctas.size(), 0);
+    long long total = 0;
+    for (size_t i = 0; i < ctas.size(); i++) {
+        if (ctas[i] > 0x7fffffffLL)
+            return fail(h, SPG_E_INVALID, "%s %d: its %lld CTAs are above grid.x's 2^31 - 1", what, ids ? ids[i] : (int)i, ctas[i]);
+        if (ranges.empty() || ranges.back().end - ranges.back().begin == capacity || total + ctas[i] > 0x7fffffffLL) {
+            ranges.push_back(RaggedRange{i, i, 0});
+            total = 0;
         }
-        int rc;
-        if ((rc = launch(h, kStageTargets, name, kern, dim3((unsigned)total), kTgtThreads, 0, st, r))) return rc;
+        first_cta[i] = (int)total;
+        total += ctas[i];
+        ranges.back().end = i + 1;
+        ranges.back().ctas = (unsigned)total;
+    }
+    return SPG_OK;
+}
+
+// range g of the members into the table r, each at its first CTA
+template <class Table, class M>
+void fill_table(Table &r, const std::vector<M> &ms, const std::vector<int> &first_cta, const RaggedRange &g) {
+    r.n = (int)(g.end - g.begin);
+    for (int k = 0; k < r.n; k++) {
+        r.img[k] = ms[g.begin + k];
+        r.img[k].first_cta = first_cta[g.begin + k];
+    }
+}
+
+// The training-sample launches (spg_targets_warp / spg_targets_maps / spg_targets_tint): sample i takes ctas[i] CTAs,
+// each launch has its member table as the parameter.
+template <class R, class M>
+int launch_samples(spg_handle *h, const char *name, void (*kern)(R), R &r, const std::vector<M> &ms, const std::vector<long long> &ctas,
+                   cudaStream_t st) {
+    if (ms.empty()) return SPG_OK;
+    std::vector<RaggedRange> ranges;
+    std::vector<int> first;
+    int rc;
+    if ((rc = deal_ragged(h, ctas, sizeof(r.img) / sizeof(r.img[0]), "sample", nullptr, ranges, first))) return rc;
+    DeviceGuard guard(h->device);
+    for (const RaggedRange &g : ranges) {
+        fill_table(r, ms, first, g);
+        if ((rc = launch(h, kStageTargets, name, kern, dim3(g.ctas), kTgtThreads, 0, st, r))) return rc;
     }
     return SPG_OK;
 }
@@ -388,32 +418,6 @@ int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, 
     return launch(h, kStageScore, k.item_name[pl.kind], k.item[pl.kind], grid, kScoreThreads, pl.smem, st, a);
 }
 
-// Images of a ragged call, as many per launch as the descriptor struct holds (it travels as the kernel parameter).
-// place(r, k, x) puts image k of the launch's descriptors r at grid.x position x and returns its CTA count; grid.y is
-// grid_y.  The caller keeps a launch inside the grid limits (the validation of its images).
-template <typename Args, typename Ragged, typename Image, typename Place>
-int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), Place place, int grid_y, int block,
-                  size_t smem, cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
-    constexpr size_t cap = sizeof(Ragged::img) / sizeof(Image);
-    for (size_t i0 = 0; i0 < imgs.size(); i0 += cap) {
-        const size_t cnt = std::min(cap, imgs.size() - i0);
-        Ragged r{};
-        std::copy(imgs.begin() + i0, imgs.begin() + i0 + cnt, r.img);
-        int x = 0;
-        for (size_t k = 0; k < cnt; k++) x += place(r, (int)k, x);
-        int rc;
-        if ((rc = launch(h, stage, name, kern, dim3((unsigned)x, (unsigned)grid_y), block, smem, st, a, r))) return rc;
-    }
-    return SPG_OK;
-}
-
-// ... with `per_image` CTAs each
-template <typename Args, typename Ragged, typename Image>
-int launch_ragged(spg_handle *h, int stage, const char *name, void (*kern)(Args, Ragged), int per_image, int block, size_t smem,
-                  cudaStream_t st, const Args &a, const std::vector<Image> &imgs) {
-    return launch_ragged(h, stage, name, kern, [per_image](Ragged &, int, int) { return per_image; }, 1, block, smem, st, a, imgs);
-}
-
 int launch_match(spg_handle *h, int base, int n, cudaStream_t st) {
     if (n == 0) return SPG_OK;
     MatchArgs a{};
@@ -595,6 +599,9 @@ int spg_create(const spg_config *cfg, spg_handle **out) {
     for (size_t g = 0; g < J; g++) ws.out_from_part[g] = (int16_t)cfg->out_from_part[g];
     if (rc == SPG_OK && cudaMemset(ws.status, 0, sizeof(uint32_t) * N) != cudaSuccess) rc = SPG_E_CUDA;
     if (rc == SPG_OK && cudaMemset(ws.peak_count, 0, sizeof(int32_t) * N * K) != cudaSuccess) rc = SPG_E_CUDA;
+    // a fetch after the peaks stage alone downloads the connection counts too: none until a stage writes them
+    if (rc == SPG_OK && cudaMemset(ws.cand_count, 0, sizeof(int32_t) * N * L) != cudaSuccess) rc = SPG_E_CUDA;
+    if (rc == SPG_OK && cudaMemset(ws.conn_count, 0, sizeof(int32_t) * N * L) != cudaSuccess) rc = SPG_E_CUDA;
     if (rc == SPG_OK && cudaMemset(h->score_queue, 0, sizeof(unsigned int) * 4) != cudaSuccess) rc = SPG_E_CUDA;
     for (int s = 0; s < 2 && rc == SPG_OK; s++)
         if (cudaStreamCreateWithFlags(&h->streams[s], cudaStreamNonBlocking) != cudaSuccess) rc = SPG_E_CUDA;
@@ -791,15 +798,8 @@ static int post_chan_chunk(const spg_handle *h, int n_out, long long tiles, int 
     return (n_out + n_chunks - 1) / n_chunks;
 }
 
-// the tiles_x x tiles_y output tiles of tile_w x tile_h that cover an H x W image; returns their number
-static long long post_tiles(int H, int W, int tile_w, int tile_h, int &tiles_x, int &tiles_y) {
-    tiles_x = (W + tile_w - 1) / tile_w;
-    tiles_y = (H + tile_h - 1) / tile_h;
-    return (long long)tiles_x * tiles_y;
-}
-
-static int postnet_grid(spg_handle *h, PostArgs &a, int n, int ctas_per_sm, dim3 *grid) {
-    const long long tiles = post_tiles(a.H, a.W, a.tile_w, a.tile_h, a.tiles_x, a.tiles_y);
+static int postnet_grid(spg_handle *h, PostArgs &a, const PostImage &im, int n, int ctas_per_sm, dim3 *grid) {
+    const long long tiles = (long long)im.tiles_x * im.tiles_y;
     if (tiles > 0x7fffffffLL || n > 65535) return fail(h, SPG_E_INVALID, "postnet grid too large");
     a.chan_chunk = post_chan_chunk(h, a.n_out, tiles * n, ctas_per_sm);
     *grid = dim3((unsigned)tiles, (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk), (unsigned)n);
@@ -872,35 +872,32 @@ static int post_common(spg_handle *h, int stride, int n_scales, int paf_chan0, i
     return SPG_OK;
 }
 
-// The kernel families of the post-network stage (PostPlan::family), each with its kernels by template flags
-// [single][ident][f16] (nullptr: not instantiated), its single-scale ragged kernels by [f16] and its multi-item ragged
-// kernels by the same flags as its per-launch kernels, under the names spg_stage_kernel reports.
+// The kernel families of the post-network stage (PostPlan::family), each with its per-launch and its ragged kernels by
+// template flags [single][ident][f16] (nullptr: not instantiated), under the names spg_stage_kernel reports (the ragged
+// ones by [single]).
 enum : int { kPostIdent, kPostFourPhase, kPostRotated, kPostGeneric };
 struct PostKernels {
     const char *name;
-    void (*fn[2][2][2])(PostArgs);
-    const char *ragged_name;
-    void (*ragged[2])(PostArgs, PostRagged);
-    const char *items_name;
-    void (*items[2][2][2])(PostArgs, PostItemsRagged);
+    void (*fn[2][2][2])(PostArgs, PostImage);
+    const char *ragged_name[2];
+    void (*ragged[2][2][2])(PostArgs, PostTable);
 };
 static const PostKernels kPostKernels[4] = {
     {"postnet_x4_ident_kernel", {{}, {{}, {postnet_x4_ident_kernel<false>, postnet_x4_ident_kernel<true>}}},
-     "postnet_x4_ident_ragged_kernel", {postnet_x4_ident_ragged_kernel<false>, postnet_x4_ident_ragged_kernel<true>}, "", {}},
+     {"", "postnet_x4_ident_ragged_kernel"}, {{}, {{}, {postnet_x4_ident_ragged_kernel<false>, postnet_x4_ident_ragged_kernel<true>}}}},
     {"postnet_kernel",
      {{{postnet_kernel<false, false, false>, postnet_kernel<false, false, true>}, {postnet_kernel<false, true, false>, postnet_kernel<false, true, true>}},
       {{postnet_kernel<true, false, false>, postnet_kernel<true, false, true>}, {}}},
-     "postnet_ragged_kernel", {postnet_ragged_kernel<false>, postnet_ragged_kernel<true>},
-     "postnet_items_ragged_kernel",
+     {"postnet_items_ragged_kernel", "postnet_ragged_kernel"},
      {{{postnet_items_ragged_kernel<false, false>, postnet_items_ragged_kernel<false, true>},
-       {postnet_items_ragged_kernel<true, false>, postnet_items_ragged_kernel<true, true>}}}},
+       {postnet_items_ragged_kernel<true, false>, postnet_items_ragged_kernel<true, true>}},
+      {{postnet_ragged_kernel<false>, postnet_ragged_kernel<true>}, {}}}},
     {"postnet_rot_kernel",
      {{{postnet_rot_kernel<false, false>, postnet_rot_kernel<false, true>}, {}}, {{postnet_rot_kernel<true, false>, postnet_rot_kernel<true, true>}, {}}},
-     "", {},
-     "postnet_rot_ragged_kernel",
+     {"postnet_rot_ragged_kernel", "postnet_rot_ragged_kernel"},
      {{{postnet_rot_ragged_kernel<false, false>, postnet_rot_ragged_kernel<false, true>}, {}},
       {{postnet_rot_ragged_kernel<true, false>, postnet_rot_ragged_kernel<true, true>}, {}}}},
-    {"postnet_generic_kernel", {{{postnet_generic_kernel}}}, "", {}, "", {}},
+    {"postnet_generic_kernel", {{{postnet_generic_kernel}}}, {}, {}},
 };
 
 struct PostPlan {
@@ -911,10 +908,12 @@ struct PostPlan {
     size_t smem;              // dynamic shared memory
 };
 
-// The schedule of one launch over the n_fused scales sc of an H x W image; rot: the inverse warp matrix of a rotated item.
+// The schedule of one launch over the n_fused items of image im (im.sc, im.H x im.W; a rotated item: im.rot).
 // `single`: one scale in the whole scale loop; `item` names the item in the error.
-static int plan_post(spg_handle *h, const PostScale *sc, int n_fused, bool single, int stride, int H, int W, const double *rot,
-                     int item, PostPlan *pl) {
+static int plan_post(spg_handle *h, const PostImage &im, int n_fused, bool single, int stride, bool rotated, int item, PostPlan *pl) {
+    const PostScale *sc = im.sc;
+    const int H = im.H, W = im.W;
+    const double *rot = rotated ? im.rot : nullptr;
     const double s1 = 1.0 / (double)stride;  // PostArgs::sx1 (post_common)
     if (stride != 4) {
         *pl = PostPlan{kPostGeneric, false, false, false, post_tile_dim(sc[0].sx2, s1, kPostC1, kPostCS, kPostTW, 7.0),
@@ -962,6 +961,20 @@ static int plan_post(spg_handle *h, const PostScale *sc, int n_fused, bool singl
     return SPG_OK;
 }
 
+// Completes image im's descriptor for one group of n_fused items, whose scales, size, output planes and float64 sums the
+// caller has set: the inverse of a rotated item's warp matrix (rot: the forward matrix, nullptr: not rotated) and the
+// tiling plan_post picks for the image alone.
+static int post_image(spg_handle *h, PostImage &im, int n_fused, bool single, int stride, const double *rot, int item, PostPlan *pl) {
+    if (rot) invert_affine(rot, im.rot);
+    int rc;
+    if ((rc = plan_post(h, im, n_fused, single, stride, rot != nullptr, item, pl))) return rc;
+    im.tile_w = pl->tile_w;
+    im.tile_h = pl->tile_h;
+    im.tiles_x = (im.W + im.tile_w - 1) / im.tile_w;
+    im.tiles_y = (im.H + im.tile_h - 1) / im.tile_h;
+    return SPG_OK;
+}
+
 int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_postnet_rotation *rot, int32_t n, int32_t H, int32_t W,
                         float *heat_out, void *paf_out, int32_t paf_dtype, void *stream) {
     if (!h) return SPG_E_INVALID;
@@ -993,7 +1006,6 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
         if ((rc = grow(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double)))) return rc;
     }
-    a.H = H; a.W = W; a.heat = heat_out; a.paf = paf_out; a.heat_acc = static_cast<double *>(h->heat_acc.p);
     for (int t = 0; t < d->n_scales; t++) {
         const spg_postnet_scale &sc = d->scales[t];
         snprintf(what, sizeof what, "scale %d", t);
@@ -1006,19 +1018,19 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     for (int t0 = 0; t0 < d->n_scales; t0 += group) {
         a.n_fused = std::min(group, d->n_scales - t0);
         a.scale_index = t0;
+        PostImage im{};
         for (int t = 0; t < a.n_fused; t++) {
             const spg_postnet_scale &sc = d->scales[t0 + t];
-            a.sc[t] = post_scale(sc.net_out, sc.dtype, sc.image_stride, sc.pair_stride, sc.chan_stride, sc.h, sc.w, sc.crop_h, sc.crop_w, H, W);
+            im.sc[t] = post_scale(sc.net_out, sc.dtype, sc.image_stride, sc.pair_stride, sc.chan_stride, sc.h, sc.w, sc.crop_h, sc.crop_w, H, W);
         }
-        const bool rotated = any_rot && rot[t0].apply;
-        if (rotated) invert_affine(rot[t0].matrix, a.rot);
+        im.H = H; im.W = W; im.heat = heat_out; im.paf = paf_out; im.heat_acc = static_cast<double *>(h->heat_acc.p);
         PostPlan pl;
         dim3 grid;
-        if ((rc = plan_post(h, a.sc, a.n_fused, d->n_scales == 1, d->stride, H, W, rotated ? a.rot : nullptr, t0, &pl))) return rc;
-        a.tile_w = pl.tile_w; a.tile_h = pl.tile_h;
-        if ((rc = postnet_grid(h, a, n, pl.ctas_per_sm, &grid))) return rc;
+        if ((rc = post_image(h, im, a.n_fused, d->n_scales == 1, d->stride, any_rot && rot[t0].apply ? rot[t0].matrix : nullptr, t0, &pl)) ||
+            (rc = postnet_grid(h, a, im, n, pl.ctas_per_sm, &grid)))
+            return rc;
         const PostKernels &k = kPostKernels[pl.family];
-        if ((rc = launch(h, kStagePostnet, k.name, k.fn[pl.single][pl.ident][pl.f16], grid, kPostThreads, pl.smem, st, a))) return rc;
+        if ((rc = launch(h, kStagePostnet, k.name, k.fn[pl.single][pl.ident][pl.f16], grid, kPostThreads, pl.smem, st, a, im))) return rc;
     }
     return SPG_OK;
 }
@@ -1026,9 +1038,8 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
 // Ragged batches, over items[n][n_items] and rot (NULL, or one entry per item): spg_postnet_rotated's schedule for every
 // image at once.  The items go in groups -- kPostMaxScales fused unrotated items, or one item per group when any is
 // rotated -- and within a group each image goes in the family and tile plan_post picks for it alone.  A group's images
-// are bucketed by kernel, identity family first, and each bucket's images go largest first, as many per launch as its
-// kernel's descriptor struct holds, with one channel chunk for all its launches.  One unrotated item per image takes
-// the single-scale ragged kernels.
+// are bucketed by kernel, identity family first, and each bucket's images go largest first into its launches' tables
+// (deal_ragged), with one channel chunk for all its launches.
 static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg_postnet_image *items,
                           const spg_postnet_rotation *rot, int32_t n, int32_t n_items, int32_t paf_dtype, void *stream) {
     if (!h) return SPG_E_INVALID;
@@ -1087,10 +1098,12 @@ static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg
     // the schedule of every launch, planned (and checked) before the first one: per item group, one launch list per kernel
     struct Bucket {
         int t0, n_fused;
-        bool single_scale;  // one unrotated item per image: the single-scale ragged kernels
         PostPlan plan;
         long long tiles;
-        std::vector<PostItemsImage> imgs;
+        std::vector<std::pair<int, PostImage>> imgs;  // (image, its descriptor)
+        std::vector<PostImage> ms;                    // the descriptors in launch order, dealt into ranges
+        std::vector<RaggedRange> ranges;
+        std::vector<int> first_cta;
     };
     std::vector<Bucket> buckets;
     const int per_group = any_rot ? 1 : kPostMaxScales;
@@ -1104,11 +1117,10 @@ static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg
     for (int t0 = 0; t0 < n_items; t0 += per_group) {
         const int nf = std::min(per_group, n_items - t0);
         const bool rotated = any_rot && rot[t0].apply;
-        const bool single_scale = n_items == 1 && !rotated;
         const size_t first = buckets.size();
         for (int i = 0; i < n; i++) {
             const spg_postnet_image &im = items[(size_t)i * n_items];
-            PostItemsImage d{};
+            PostImage d{};
             for (int t = 0; t < nf; t++) {
                 const spg_postnet_image &it = items[(size_t)i * n_items + t0 + t];
                 d.sc[t] = post_scale(it.net_out, cm->net_dtype, 0, it.pair_stride, it.chan_stride, it.h, it.w, it.crop_h, it.crop_w,
@@ -1116,57 +1128,49 @@ static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg
             }
             d.H = im.height; d.W = im.width; d.heat = im.heat_out; d.paf = im.paf_out;
             d.heat_acc = acc ? acc + acc_off[i] : nullptr;
-            if (rotated) invert_affine(rot[(size_t)i * n_items + t0].matrix, d.rot);
             PostPlan pl;
-            if ((rc = plan_post(h, d.sc, nf, n_items == 1, 4, d.H, d.W, rotated ? d.rot : nullptr, t0, &pl)))
+            if ((rc = post_image(h, d, nf, n_items == 1, 4, rotated ? rot[(size_t)i * n_items + t0].matrix : nullptr, t0, &pl)))
                 return fail(h, rc, "%s: %s", name(i, t0), std::string(h->err).c_str());
-            d.tile_w = pl.tile_w; d.tile_h = pl.tile_h;
-            const long long tl = post_tiles(d.H, d.W, d.tile_w, d.tile_h, d.tiles_x, d.tiles_y);
-            if (tl * (single_scale ? kPostRaggedMaxImages : kPostItemsMaxImages) > 0x7fffffffLL)
-                return fail(h, SPG_E_INVALID, "image %d: %dx%d tiles are too many for one launch", i, d.tiles_x, d.tiles_y);
             size_t b = first;
             while (b < buckets.size() && !(buckets[b].plan.family == pl.family && buckets[b].plan.single == pl.single &&
                                            buckets[b].plan.ident == pl.ident))
                 b++;
-            if (b == buckets.size()) buckets.push_back(Bucket{t0, nf, single_scale, pl, 0, {}});
-            buckets[b].imgs.push_back(d);
-            buckets[b].tiles += tl;
+            if (b == buckets.size()) buckets.push_back(Bucket{t0, nf, pl, 0, {}, {}, {}, {}});
+            buckets[b].imgs.emplace_back(i, d);
+            buckets[b].tiles += (long long)d.tiles_x * d.tiles_y;
         }
         // identity family first; the buckets of fused or rotated items are of one family each and keep their order
         std::stable_sort(buckets.begin() + first, buckets.end(), [](const Bucket &x, const Bucket &y) {
             return x.plan.family < y.plan.family;
         });
     }
-    auto place = [](auto &r, int k, int x) {
-        r.img[k].first_cta = x;
-        r.n = k + 1;
-        return r.img[k].tiles_x * r.img[k].tiles_y;
-    };
+    // each bucket's images largest first, dealt into its launches' tables
     for (Bucket &b : buckets) {
-        std::stable_sort(b.imgs.begin(), b.imgs.end(), [](const PostItemsImage &x, const PostItemsImage &y) {
-            return (int64_t)x.H * x.W > (int64_t)y.H * y.W;
+        std::stable_sort(b.imgs.begin(), b.imgs.end(), [](const std::pair<int, PostImage> &x, const std::pair<int, PostImage> &y) {
+            return (int64_t)x.second.H * x.second.W > (int64_t)y.second.H * y.second.W;
         });
+        std::vector<int> ids;
+        std::vector<long long> ctas;
+        for (const auto &e : b.imgs) {
+            ids.push_back(e.first);
+            b.ms.push_back(e.second);
+            ctas.push_back((long long)e.second.tiles_x * e.second.tiles_y);
+        }
+        if ((rc = deal_ragged(h, ctas, kPostTableImages, "image", ids.data(), b.ranges, b.first_cta))) return rc;
+    }
+    PostTable r{};
+    for (const Bucket &b : buckets) {
         const PostKernels &k = kPostKernels[b.plan.family];
         a.n_fused = b.n_fused;
         a.scale_index = b.t0;
         a.chan_chunk = post_chan_chunk(h, a.n_out, b.tiles, b.plan.ctas_per_sm);
-        const int chunks = (a.n_out + a.chan_chunk - 1) / a.chan_chunk;
-        if (b.single_scale) {
-            std::vector<PostImage> imgs(b.imgs.size());
-            for (size_t j = 0; j < imgs.size(); j++) {
-                const PostItemsImage &d = b.imgs[j];
-                PostImage &s = imgs[j];
-                s.sc[0] = d.sc[0];
-                s.H = d.H; s.W = d.W; s.heat = d.heat; s.paf = d.paf;
-                s.tile_w = d.tile_w; s.tile_h = d.tile_h; s.tiles_x = d.tiles_x; s.tiles_y = d.tiles_y;
-            }
-            rc = launch_ragged(h, kStagePostnet, k.ragged_name, k.ragged[b.plan.f16], place, chunks, kPostThreads, b.plan.smem, st, a,
-                               imgs);
-        } else {
-            rc = launch_ragged(h, kStagePostnet, k.items_name, k.items[b.plan.single][b.plan.ident][b.plan.f16], place, chunks,
-                               kPostThreads, b.plan.smem, st, a, b.imgs);
+        const unsigned chunks = (unsigned)((a.n_out + a.chan_chunk - 1) / a.chan_chunk);
+        for (const RaggedRange &g : b.ranges) {
+            fill_table(r, b.ms, b.first_cta, g);
+            if ((rc = launch(h, kStagePostnet, k.ragged_name[b.plan.single], k.ragged[b.plan.single][b.plan.ident][b.plan.f16],
+                             dim3(g.ctas, chunks), kPostThreads, b.plan.smem, st, a, r)))
+                return rc;
         }
-        if (rc) return rc;
     }
     return SPG_OK;
 }
@@ -1217,60 +1221,53 @@ int prenet_member(spg_handle *h, const char *what, int index, int height, int wi
     return SPG_OK;
 }
 
-// The launches of validated members.  Unrotated members go in chunks of one prenet_kernel<false> launch; rotated ones in
-// chunks of a prenet_resize_kernel launch, which writes each member's padded uint8 image to its own part of the
-// handle's scratch grid (grown to the largest chunk's total), and a prenet_kernel<true> launch that warps from it.  A
-// chunk holds as many members as one launch's table; every chunk is planned and checked before the first launch.
-int prenet_launch(spg_handle *h, std::vector<PreMember> &ms, const std::vector<char> &rotated, cudaStream_t st) {
-    struct Chunk {
-        bool rot;
-        std::vector<int> members;
-    };
-    std::vector<Chunk> chunks;
-    std::vector<size_t> grid_at(ms.size());  // rotated members: the offset of the member's image in the scratch grid
+// The launches of validated members: the unrotated ones in prenet_kernel<false> launches, then the rotated ones, each
+// launch of them a prenet_resize_kernel, which writes every member's padded uint8 image to its own part of the handle's
+// scratch grid (grown to the largest launch's total), and a prenet_kernel<true> that warps from it.  Every launch is
+// planned and checked before the first.
+int prenet_launch(spg_handle *h, const std::vector<PreMember> &ms, const std::vector<char> &rotated, cudaStream_t st) {
+    struct Group {
+        std::vector<PreMember> ms;
+        std::vector<RaggedRange> ranges;
+        std::vector<int> first_cta;
+    } groups[2];
     size_t grid_need = 0;
+    int rc;
     for (int rot = 0; rot < 2; rot++) {
-        size_t grid_bytes = 0;
-        long long ctas = 0;
+        Group &gr = groups[rot];
+        std::vector<int> ids;
+        std::vector<long long> ctas;
         for (int i = 0; i < (int)ms.size(); i++) {
             if (rotated[i] != rot) continue;
-            PreMember &a = ms[i];
-            if (chunks.empty() || chunks.back().rot != (rot != 0) || chunks.back().members.size() == (size_t)kPreMaxMembers) {
-                chunks.push_back(Chunk{rot != 0, {}});
-                grid_bytes = 0;
-                ctas = 0;
-            }
-            a.first_cta = (int)ctas;
-            ctas += (long long)a.tiles_x * a.Hp;
-            if (ctas > 0x7fffffffLL)
-                return fail(h, SPG_E_INVALID, "member %d: the %lld CTAs of its launch are above grid.x's 2^31 - 1", i, ctas);
-            if (rot) {
-                grid_at[i] = grid_bytes;
-                grid_bytes += (size_t)a.Hp * a.Wp * 3;
-                grid_need = std::max(grid_need, grid_bytes);
-            }
-            chunks.back().members.push_back(i);
+            ids.push_back(i);
+            gr.ms.push_back(ms[i]);
+            ctas.push_back((long long)ms[i].tiles_x * ms[i].Hp);
+        }
+        if ((rc = deal_ragged(h, ctas, kPreMaxMembers, "member", ids.data(), gr.ranges, gr.first_cta))) return rc;
+        for (const RaggedRange &g : gr.ranges) {
+            size_t bytes = 0;
+            for (size_t k = g.begin; rot && k < g.end; k++) bytes += (size_t)gr.ms[k].Hp * gr.ms[k].Wp * 3;
+            grid_need = std::max(grid_need, bytes);
         }
     }
-    if (chunks.empty()) return SPG_OK;
-    int rc;
     if ((rc = grow(h, h->pre_grid, grid_need))) return rc;
-    for (const Chunk &c : chunks) {
-        PreRagged r{};
-        r.n = (int)c.members.size();
-        int x = 0;
-        for (int k = 0; k < r.n; k++) {
-            r.img[k] = ms[c.members[k]];
-            if (c.rot) r.img[k].grid = static_cast<unsigned char *>(h->pre_grid.p) + grid_at[c.members[k]];
-            x = r.img[k].first_cta + r.img[k].tiles_x * r.img[k].Hp;
-        }
-        const dim3 grid((unsigned)x);
-        if (c.rot) {
-            if ((rc = launch(h, kStagePrenet, "prenet_resize_kernel", prenet_resize_kernel, grid, kPreThreads, 0, st, r)) ||
-                (rc = launch(h, kStagePrenet, "prenet_kernel<true>", prenet_kernel<true>, grid, kPreThreads, 0, st, r)))
+    PreRagged r{};
+    for (int rot = 0; rot < 2; rot++) {
+        for (const RaggedRange &g : groups[rot].ranges) {
+            fill_table(r, groups[rot].ms, groups[rot].first_cta, g);
+            const dim3 grid(g.ctas);
+            if (rot) {
+                size_t at = 0;  // the range's padded images back to back in the scratch grid
+                for (int k = 0; k < r.n; k++) {
+                    r.img[k].grid = static_cast<unsigned char *>(h->pre_grid.p) + at;
+                    at += (size_t)r.img[k].Hp * r.img[k].Wp * 3;
+                }
+                if ((rc = launch(h, kStagePrenet, "prenet_resize_kernel", prenet_resize_kernel, grid, kPreThreads, 0, st, r)) ||
+                    (rc = launch(h, kStagePrenet, "prenet_kernel<true>", prenet_kernel<true>, grid, kPreThreads, 0, st, r)))
+                    return rc;
+            } else if ((rc = launch(h, kStagePrenet, "prenet_kernel<false>", prenet_kernel<false>, grid, kPreThreads, 0, st, r))) {
                 return rc;
-        } else if ((rc = launch(h, kStagePrenet, "prenet_kernel<false>", prenet_kernel<false>, grid, kPreThreads, 0, st, r))) {
-            return rc;
+            }
         }
     }
     return SPG_OK;
@@ -1415,7 +1412,7 @@ int spg_targets_warp(spg_handle *h, const spg_target_params *params, const spg_t
         a.img_ctas = (int)((img_px + kTgtThreads - 1) / kTgtThreads);
     }
     const long long per_sample = (img_px + kTgtThreads - 1) / kTgtThreads + (map_px + kTgtThreads - 1) / kTgtThreads;
-    return targets_launch(h, "targets_warp_kernel", targets_warp_kernel, r, ms, kTgtWarpMax, std::vector<long long>((size_t)n, per_sample),
+    return launch_samples(h, "targets_warp_kernel", targets_warp_kernel, r, ms, std::vector<long long>((size_t)n, per_sample),
                           static_cast<cudaStream_t>(stream));
 }
 
@@ -1441,7 +1438,7 @@ int spg_targets_maps(spg_handle *h, const spg_target_params *params, const spg_t
             return fail(h, SPG_E_INVALID, "sample %d: joints, mask_all or labels is NULL", i);
         ms[i] = TgtMapsMember{s.joints, s.mask_all, s.labels, s.n_persons, tiles, 0};
     }
-    return targets_launch(h, "targets_maps_kernel", targets_maps_kernel, r, ms, kTgtMapsMax, std::vector<long long>((size_t)n, channels * tiles),
+    return launch_samples(h, "targets_maps_kernel", targets_maps_kernel, r, ms, std::vector<long long>((size_t)n, channels * tiles),
                           static_cast<cudaStream_t>(stream));
 }
 
@@ -1465,7 +1462,7 @@ int spg_targets_tint(spg_handle *h, const spg_target_tint *samples, int32_t n, v
                               s.width - s.width % s.row_block, groups, 0};
         ctas[i] = ((long long)s.height * groups + kTgtThreads - 1) / kTgtThreads;
     }
-    return targets_launch(h, "targets_tint_kernel", targets_tint_kernel, r, ms, kTgtTintMax, ctas, static_cast<cudaStream_t>(stream));
+    return launch_samples(h, "targets_tint_kernel", targets_tint_kernel, r, ms, ctas, static_cast<cudaStream_t>(stream));
 }
 
 // ---- stages ------------------------------------------------------------------------------------
@@ -1596,14 +1593,26 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SPG_CUDA(h, cudaMemsetAsync(ws.status, 0, sizeof(uint32_t) * (size_t)n, st));
     if (n == 0) return SPG_OK;
-    if ((rc = launch_ragged(h, kStageNms, "nms_peaks_ragged_kernel", nms_peaks_ragged_kernel, ws.K, kNmsThreads, nms_smem, st,
-                            nms_args(h, p), nms)))
+    // `per` CTAs (its parts or limbs) per image; the kernels find an image at blockIdx.x / per
+    auto per_image = [&](int stage, const char *name, auto kern, auto &r, int per, int block, size_t smem, const auto &args,
+                         const auto &imgs) {
+        std::vector<RaggedRange> ranges;
+        std::vector<int> first;
+        int rc2 = deal_ragged(h, std::vector<long long>(imgs.size(), per), sizeof(r.img) / sizeof(r.img[0]), "image", nullptr, ranges, first);
+        for (size_t j = 0; rc2 == SPG_OK && j < ranges.size(); j++) {
+            std::copy(imgs.begin() + ranges[j].begin, imgs.begin() + ranges[j].end, r.img);
+            rc2 = launch(h, stage, name, kern, dim3(ranges[j].ctas), block, smem, st, args, r);
+        }
+        return rc2;
+    };
+    NmsRagged nr{};
+    ScoreRagged sr{};
+    if ((rc = per_image(kStageNms, "nms_peaks_ragged_kernel", nms_peaks_ragged_kernel, nr, ws.K, kNmsThreads, nms_smem, nms_args(h, p), nms)))
         return rc;
     h->cand_dtype = dtype;
     const ScoreArgs sa = score_args(h, p);
-    if ((rc = launch_ragged(h, kStageScore, k.ragged_name[1], k.ragged[1], ws.L, kScoreThreads, staged_smem, st, sa, staged)) ||
-        (rc = launch_ragged(h, kStageScore, k.ragged_name[0], k.ragged[0], ws.L, kScoreThreads, score_smem_bytes(0, ws.capP), st, sa,
-                            sampled)) ||
+    if ((rc = per_image(kStageScore, k.ragged_name[1], k.ragged[1], sr, ws.L, kScoreThreads, staged_smem, sa, staged)) ||
+        (rc = per_image(kStageScore, k.ragged_name[0], k.ragged[0], sr, ws.L, kScoreThreads, score_smem_bytes(0, ws.capP), sa, sampled)) ||
         (rc = launch_people(h, 0, n, p, st)))
         return rc;
     h->stage = 4;

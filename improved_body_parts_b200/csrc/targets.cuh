@@ -28,10 +28,10 @@
 // targets_tint_kernel (below the warp): the colour distortion, in place on the uint8 sources before the warp.
 //
 // The launches are ragged like prenet.cuh: a member table (one sample each) travels as a __grid_constant__ kernel
-// parameter and a CTA finds its member by binary search over first_cta (post_ragged_image).
+// parameter and a CTA finds its member by binary search over first_cta (ragged_member).
 #pragma once
 
-#include "postnet.cuh"
+#include "interp.cuh"
 
 namespace spg {
 
@@ -62,14 +62,13 @@ struct TgtWarpMember {
     int img_ctas;                            // CTAs of the image part; the mask part follows
     int first_cta;
 };
-constexpr int kTgtParamBytes = 32764;
-constexpr int kTgtWarpMax = (int)((kTgtParamBytes - sizeof(TgtCommon) - 8) / sizeof(TgtWarpMember));
+constexpr int kTgtWarpMax = (int)((kParamBytes - sizeof(TgtCommon) - 8) / sizeof(TgtWarpMember));
 struct TgtWarpRagged {
     TgtCommon c;
     int n;
     TgtWarpMember img[kTgtWarpMax];   // first_cta increasing
 };
-static_assert(sizeof(TgtWarpRagged) <= kTgtParamBytes, "a launch's parameters fit the kernel-parameter limit");
+static_assert(sizeof(TgtWarpRagged) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
 
 // one channel of warpAffine's uint8 INTER_LINEAR at tap t: int sum of the four taps with weights summing to 2^15
 __device__ __forceinline__ int warp_u8(const WarpTap &t, const unsigned char *g, long long pitch, int cs, int w, int h, int border) {
@@ -84,7 +83,7 @@ __device__ __forceinline__ int warp_u8(const WarpTap &t, const unsigned char *g,
 }
 
 __global__ void __launch_bounds__(kTgtThreads) targets_warp_kernel(const __grid_constant__ TgtWarpRagged r) {
-    const TgtWarpMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const TgtWarpMember &a = ragged_member(r, (int)blockIdx.x);
     const TgtCommon &c = r.c;
     const int cta = (int)blockIdx.x - a.first_cta;
     if (cta < a.img_ctas) {  // one output pixel of the image per thread
@@ -142,12 +141,12 @@ struct TgtTintMember {
     int groups;              // kTintPix-pixel groups per row
     int first_cta;
 };
-constexpr int kTgtTintMax = (int)((kTgtParamBytes - 16) / sizeof(TgtTintMember));
+constexpr int kTgtTintMax = (int)((kParamBytes - 16) / sizeof(TgtTintMember));
 struct TgtTintRagged {
     int n;
     TgtTintMember img[kTgtTintMax];   // first_cta increasing
 };
-static_assert(sizeof(TgtTintRagged) <= kTgtParamBytes, "a launch's parameters fit the kernel-parameter limit");
+static_assert(sizeof(TgtTintRagged) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
 
 // the HSV -> BGR table entry k of [V, V(1-S), V(1-S hh), V(1-S(1-hh))] without dynamic indexing into registers
 __device__ __forceinline__ float tint_pick(int k, float t0, float t1, float t2, float t3) {
@@ -192,7 +191,7 @@ __global__ void __launch_bounds__(kTgtThreads) targets_tint_kernel(const __grid_
         hdiv[i] = i ? (2 * (180 << 12) + 6 * i) / (12 * i) : 0;
     }
     __syncthreads();
-    const TgtTintMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const TgtTintMember &a = ragged_member(r, (int)blockIdx.x);
     const long long q = (long long)((int)blockIdx.x - a.first_cta) * kTgtThreads + threadIdx.x;
     if (q >= (long long)a.h * a.groups) return;
     const int y = (int)(q / a.groups), x0 = (int)(q - (long long)y * a.groups) * kTintPix;
@@ -255,7 +254,7 @@ struct TgtMapsMember {
     int tiles;                // CTAs per channel: ceil(map_h * map_w / kTgtThreads)
     int first_cta;
 };
-constexpr int kTgtMapsMax = (int)((kTgtParamBytes - sizeof(TgtCommon) - sizeof(int16_t) * kMaxLimbs * 2 - 32) / sizeof(TgtMapsMember));
+constexpr int kTgtMapsMax = (int)((kParamBytes - sizeof(TgtCommon) - sizeof(int16_t) * kMaxLimbs * 2 - 32) / sizeof(TgtMapsMember));
 struct TgtMapsRagged {
     TgtCommon c;
     int K, L;
@@ -263,7 +262,7 @@ struct TgtMapsRagged {
     int n;
     TgtMapsMember img[kTgtMapsMax];   // first_cta increasing
 };
-static_assert(sizeof(TgtMapsRagged) <= kTgtParamBytes, "a launch's parameters fit the kernel-parameter limit");
+static_assert(sizeof(TgtMapsRagged) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
 
 // a window [x0, x1) x [y0, y1) of the map and what the pixels inside it need
 struct TgtItem {
@@ -328,7 +327,7 @@ __device__ __forceinline__ float tgt_kp_axis(const TgtCommon &c, int i, float x)
 __global__ void __launch_bounds__(kTgtThreads) targets_maps_kernel(const __grid_constant__ TgtMapsRagged r) {
     __shared__ TgtItem list[kTgtThreads];
     __shared__ int warp_count[kTgtWarps];
-    const TgtMapsMember &a = post_ragged_image(r, (int)blockIdx.x);
+    const TgtMapsMember &a = ragged_member(r, (int)blockIdx.x);
     const TgtCommon &c = r.c;
     const int K = r.K, L = r.L;
     const int cta = (int)blockIdx.x - a.first_cta;

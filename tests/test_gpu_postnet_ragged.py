@@ -107,18 +107,23 @@ def test_pairs_read_in_place_from_a_shared_batch_output(env):
                           t.float32, False)
 
 
+POST_TABLE_IMAGES = 82  # kPostTableImages in csrc/postnet.cuh: image descriptors per launch
+
+
 @pytest.mark.parametrize("identity", [True, False])
-def test_more_images_than_one_launch_holds(env, identity):
+def test_more_images_than_one_table_holds(env, identity):
     t = env.torch
     rng = np.random.default_rng(5 if identity else 6)
+    n = 2 * POST_TABLE_IMAGES + 22
     spec = [(int(rng.integers(8, 70)), int(rng.integers(8, 90)), 1.0 if identity else float(rng.choice([0.6, 1.4])))
-            for _ in range(150)]
+            for _ in range(n)]
     imgs = _images(env, spec, t.float16, seed=900)
-    before = env.g.launch_count
-    got = env.g.postnet_ragged(imgs)
-    assert env.g.launch_count - before == 3  # 64 + 64 + 22 images
-    assert env.g.postnet_kernel() == ("postnet_x4_ident_ragged_kernel" if identity else "postnet_ragged_kernel")
-    _check_against_single(env, imgs, got, t.float32, False)
+    with env.grouping.Grouper(max_batch=n, max_h=1024, max_w=1024) as g:
+        before = g.launch_count
+        got = g.postnet_ragged(imgs)
+        assert g.launch_count - before == 3  # two full tables and 22 images
+        assert g.postnet_kernel() == ("postnet_x4_ident_ragged_kernel" if identity else "postnet_ragged_kernel")
+        _check_against_single(env, imgs, got, t.float32, False)
 
 
 def test_outputs_stay_inside_their_planes(env):

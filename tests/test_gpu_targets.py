@@ -137,3 +137,57 @@ def test_round_trip_skeletons_to_labels_to_grouping(cuda_device):
             want = expected[n][p][list(skeleton.COCO_FROM_PART)]
             best = min(range(3), key=lambda q: np.abs(found[q] - want).max())
             assert np.abs(found[best] - want).max() <= 1.0, (n, p, found[best], want)
+
+
+# members per launch of the training-sample kernels: kTgtWarpMax, kTgtMapsMax, kTgtTintMax in csrc/targets.cuh
+WARP_TABLE, MAPS_TABLE, TINT_TABLE = 247, 784, 682
+
+
+def test_more_samples_than_one_table_holds(cuda_device):
+    """800 tiny samples through targets_tint, targets_warp and targets_maps, one call each: every kernel's launches split
+    at its table's capacity, and every sample equals a call of its own."""
+    import torch
+    n, h, w, P = 800, 6, 7, 2
+    cfg = targets.TargetConfig(8, 8)
+    params = targets.target_params(cfg)
+    g = targets._Device.grouper(cfg, 0)
+    rng = np.random.default_rng(23)
+    src = torch.from_numpy(rng.integers(0, 256, (n, h, w, 3), dtype=np.uint8)).to(cuda_device)
+    masks = torch.from_numpy(rng.integers(0, 256, (2, n, h, w), dtype=np.uint8)).to(cuda_device)
+    joints = np.zeros((n, P, 18, 3), np.float32)
+    joints[..., 0:2] = rng.uniform(-2, 10, (n, P, 18, 2))
+    joints[..., 2] = rng.choice([0, 1, 2], (n, P, 18))
+    joints = torch.from_numpy(joints).to(cuda_device)
+    n_persons = rng.integers(0, P + 1, n)
+    mats = np.zeros((n, 2, 3))
+    for i in range(n):
+        a, s = rng.uniform(-np.pi, np.pi), rng.uniform(0.7, 1.4)
+        mats[i] = [[s * np.cos(a), -s * np.sin(a), rng.uniform(-2, 6)], [s * np.sin(a), s * np.cos(a), rng.uniform(-2, 6)]]
+    draws = [(int(rng.integers(0, 21)), int(rng.integers(0, 81)), int(rng.integers(0, 61))) for _ in range(n)]
+
+    def outputs():
+        return (torch.full((n, 8, 8, 3), -1.0, device=cuda_device), torch.full((2, n, 2, 2), -1.0, device=cuda_device),
+                torch.full((n, 50, 2, 2), -1.0, device=cuda_device))
+
+    def run(idx, img, out):
+        g.targets_tint(targets.tint_records([(img[i].data_ptr(), 3 * w, h, w) for i in idx], [draws[i] for i in idx]))
+        ws = np.zeros(len(idx), grouping.TARGET_SAMPLE)
+        wj = np.zeros(len(idx), grouping.TARGET_JOINTS)
+        for k, i in enumerate(idx):
+            ws[k] = (img[i].data_ptr(), masks[0, i].data_ptr(), masks[1, i].data_ptr(), 3 * w, w, h, w, mats[i].reshape(6),
+                     out[0][i].data_ptr(), out[1][0, i].data_ptr(), out[1][1, i].data_ptr())
+            wj[k] = (joints[i].data_ptr(), n_persons[i], 0, out[1][1, i].data_ptr(), out[2][i].data_ptr())
+        g.targets_warp(params, ws)
+        g.targets_maps(params, wj)
+
+    batch_src, alone_src = src.clone(), src.clone()
+    batch, alone = outputs(), outputs()
+    before = g.launch_count
+    run(range(n), batch_src, batch)
+    ranges = [-(-n // c) for c in (TINT_TABLE, WARP_TABLE, MAPS_TABLE)]
+    assert ranges == [2, 4, 2] and g.launch_count - before == sum(ranges)
+    for i in range(n):
+        run([i], alone_src, alone)
+    assert torch.equal(batch_src, alone_src) and not torch.equal(batch_src, src)
+    for b, a in zip(batch, alone):
+        assert (b >= 0).all() and torch.equal(b.view(torch.int32), a.view(torch.int32))
