@@ -24,6 +24,7 @@
 #include "limb_match.cuh"
 #include "limb_score.cuh"
 #include "limb_score_persist.cuh"
+#include "loss.cuh"
 #include "match_assemble.cuh"
 #include "nms_peaks.cuh"
 #include "nms_peaks_persist.cuh"
@@ -39,7 +40,7 @@ static_assert(sizeof(spg_params) == sizeof(spg::Params), "spg_params layout");
 static thread_local std::string g_create_error;
 
 // the stage numbers of spg_stage_kernel (include/spgroup.h)
-enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageTargets, kStageCount };
+enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageTargets, kStageLoss, kStageCount };
 
 // device scratch that grows on demand (grow) and lives until spg_destroy
 struct Scratch {
@@ -61,6 +62,7 @@ struct spg_handle {
     unsigned long long armed_value = 0;
     Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
     Scratch pre_grid;  // prenet: the padded uint8 images of a launch's rotated members
+    Scratch loss_partial;  // spg_loss_forward: the ticket (first 256 bytes), then the float64 partial sums of the CTAs
     // the capacity-free tier (spg_group_unbounded): fixed-size words, tables sized by the peak counts, the candidate list
     // with the sort's scratch, the person table and outputs; `ub_ws` describes the last call's results
     Scratch ub_small, ub_peaks, ub_cands, ub_people;
@@ -68,7 +70,7 @@ struct spg_handle {
     bool ub_valid = false;
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
-    const char *stage_kernel[kStageCount] = {"", "", "", "", "", "", ""};
+    const char *stage_kernel[kStageCount] = {"", "", "", "", "", "", "", ""};
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)
@@ -98,12 +100,16 @@ int fail(spg_handle *h, int code, const char *fmt, ...) {
         if (e_ != cudaSuccess) return fail((h), SPG_E_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); \
     } while (0)
 
+// a workspace array, zero-filled: the downloads copy whole capacity-sized arrays, so the slots no stage has written yet
+// (past a count, or before the first call) hold zeros rather than whatever the memory held before
 template <typename T>
 int dalloc(spg_handle *h, T **p, size_t count) {
     void *q = nullptr;
-    SPG_CUDA(h, cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
+    const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
+    SPG_CUDA(h, cudaMalloc(&q, bytes));
     h->allocs.push_back(q);
     *p = static_cast<T *>(q);
+    SPG_CUDA(h, cudaMemset(q, 0, bytes));
     return SPG_OK;
 }
 
@@ -597,12 +603,8 @@ int spg_create(const spg_config *cfg, spg_handle **out) {
     A(dalloc(h, &h->score_queue, 4));
     for (size_t i = 0; i < L * 2; i++) ws.limbs[i] = (int16_t)cfg->limbs[i];
     for (size_t g = 0; g < J; g++) ws.out_from_part[g] = (int16_t)cfg->out_from_part[g];
-    if (rc == SPG_OK && cudaMemset(ws.status, 0, sizeof(uint32_t) * N) != cudaSuccess) rc = SPG_E_CUDA;
-    if (rc == SPG_OK && cudaMemset(ws.peak_count, 0, sizeof(int32_t) * N * K) != cudaSuccess) rc = SPG_E_CUDA;
-    // a fetch after the peaks stage alone downloads the connection counts too: none until a stage writes them
-    if (rc == SPG_OK && cudaMemset(ws.cand_count, 0, sizeof(int32_t) * N * L) != cudaSuccess) rc = SPG_E_CUDA;
-    if (rc == SPG_OK && cudaMemset(ws.conn_count, 0, sizeof(int32_t) * N * L) != cudaSuccess) rc = SPG_E_CUDA;
-    if (rc == SPG_OK && cudaMemset(h->score_queue, 0, sizeof(unsigned int) * 4) != cudaSuccess) rc = SPG_E_CUDA;
+    // every array starts zeroed (dalloc): no status, peaks, candidates or connections until a stage writes them, and
+    // score_queue's item queues at 0
     for (int s = 0; s < 2 && rc == SPG_OK; s++)
         if (cudaStreamCreateWithFlags(&h->streams[s], cudaStreamNonBlocking) != cudaSuccess) rc = SPG_E_CUDA;
     if (rc != SPG_OK) {
@@ -619,7 +621,7 @@ void spg_destroy(spg_handle *h) {
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
     for (void *p : h->allocs) cudaFree(p);
-    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid, &h->ub_small, &h->ub_peaks, &h->ub_cands, &h->ub_people})
+    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid, &h->loss_partial, &h->ub_small, &h->ub_peaks, &h->ub_cands, &h->ub_people})
         if (s->p) cudaFree(s->p);
     if (h->done_counter) cudaFree(h->done_counter);
     for (auto &s : h->streams)
@@ -1463,6 +1465,130 @@ int spg_targets_tint(spg_handle *h, const spg_target_tint *samples, int32_t n, v
         ctas[i] = ((long long)s.height * groups + kTgtThreads - 1) / kTgtThreads;
     }
     return launch_samples(h, "targets_tint_kernel", targets_tint_kernel, r, ms, ctas, static_cast<cudaStream_t>(stream));
+}
+
+// ---- training loss -----------------------------------------------------------------------------
+namespace {
+
+// the loss kernels per prediction dtype, with the names spg_stage_kernel reports
+struct LossKernels {
+    int dtype;
+    size_t esz;
+    void (*fwd)(LossArgs), (*bwd)(LossArgs);
+    const char *fwd_name, *bwd_name;
+};
+const LossKernels kLossKernels[] = {
+    {SPG_F32, 4, loss_forward_kernel<float>, loss_backward_kernel<float>, "loss_forward_kernel<float>", "loss_backward_kernel<float>"},
+    {SPG_BF16, 2, loss_forward_kernel<__nv_bfloat16>, loss_backward_kernel<__nv_bfloat16>, "loss_forward_kernel<bf16>",
+     "loss_backward_kernel<bf16>"},
+    {SPG_F16, 2, loss_forward_kernel<__half>, loss_backward_kernel<__half>, "loss_forward_kernel<f16>", "loss_backward_kernel<f16>"},
+};
+
+bool aligned(const void *p, size_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// everything a loss launch needs, validated: the kernels, the arguments, the grid and the dynamic shared memory
+int loss_setup(spg_handle *h, const spg_loss_params *p, const float *mask, const float *labels, const spg_loss_pred *preds,
+               int32_t dtype, bool backward, const LossKernels *&kern, LossArgs &a, long long &ctas, size_t &smem) {
+    if (!p) return fail(h, SPG_E_INVALID, "params is NULL");
+    if (p->mode != SPG_LOSS_FOCAL && p->mode != SPG_LOSS_L2) return fail(h, SPG_E_INVALID, "mode %d is not SPG_LOSS_FOCAL or SPG_LOSS_L2", p->mode);
+    if (p->nstack < 1 || p->nstack > kLossMaxStacks) return fail(h, SPG_E_INVALID, "nstack %d outside [1, %d]", p->nstack, kLossMaxStacks);
+    if (p->batch < 1 || p->channels < (p->mode == SPG_LOSS_FOCAL ? 2 : 1))
+        return fail(h, SPG_E_INVALID, "targets: batch %d or channels %d too small", p->batch, p->channels);
+    if (p->height < kLossBand || p->width < kLossBand || p->height % kLossBand || p->width % kLossBand || p->height > 32767 || p->width > 32767)
+        return fail(h, SPG_E_INVALID, "targets: map %dx%d is not a multiple of %d in [%d, 32767]", p->height, p->width, kLossBand, kLossBand);
+    if (p->mode == SPG_LOSS_FOCAL && (p->heat_start < 0 || p->heat_start > p->bkg_start || p->bkg_start > p->channels))
+        return fail(h, SPG_E_INVALID, "heat_start %d / bkg_start %d outside 0 <= heat_start <= bkg_start <= %d", p->heat_start, p->bkg_start, p->channels);
+    if (!labels || !aligned(labels, 16)) return fail(h, SPG_E_INVALID, "labels is NULL or not 16-byte aligned");
+    if (!mask || !aligned(mask, 16)) return fail(h, SPG_E_INVALID, "mask_miss is NULL or not 16-byte aligned");
+    kern = nullptr;
+    for (const LossKernels &k : kLossKernels)
+        if (k.dtype == dtype) kern = &k;
+    if (!kern) return fail(h, SPG_E_INVALID, "pred_dtype %d is not SPG_F32, SPG_BF16 or SPG_F16", dtype);
+    if (!preds) return fail(h, SPG_E_INVALID, "preds is NULL");
+    smem = loss_smem_bytes(p->width);
+    if (smem > h->smem_optin)
+        return fail(h, SPG_E_INVALID, "targets: map width %d needs %zu B of shared memory (limit %zu)", p->width, smem, h->smem_optin);
+    const int bands = p->height / kLossBand;
+    ctas = (long long)p->batch * p->channels * bands;
+    if (ctas > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "targets: %lld CTAs are above grid.x's 2^31 - 1", ctas);
+    a = LossArgs{};
+    a.labels = labels;
+    a.mask = mask;
+    a.focal = p->mode == SPG_LOSS_FOCAL;
+    a.nstack = p->nstack;
+    a.B = p->batch; a.C = p->channels; a.H = p->height; a.W = p->width;
+    a.heat_start = a.focal ? p->heat_start : 0;
+    a.bkg_start = a.focal ? p->bkg_start : 0;
+    a.bands = bands;
+    a.w_bkg = (float)p->multi_task_weight;
+    a.w_heat = (float)p->keypoint_task_weight;
+    for (int k = 0; k < p->nstack; k++) a.nw[k] = (float)p->nstack_weight[k];
+    for (int j = 0; j < kLossScales; j++) a.sw[j] = (float)p->scale_weight[j];
+    // CUDA torch divides by a host scalar b as a multiply by 1.0f / (float)b
+    a.inv_batch = 1.0f / (float)p->batch_divisor;
+    a.inv_sw = 1.0f / (float)p->scale_weight_sum;
+    a.inv_nw = 1.0f / (float)p->nstack_weight_sum;
+    const size_t vb = kLossVec * kern->esz;
+    for (int k = 0; k < p->nstack; k++)
+        for (int j = 0; j < kLossScales; j++) {
+            const spg_loss_pred &q = preds[k * kLossScales + j];
+            const int i = k * kLossScales + j;
+            if (!q.data || (backward && !q.grad))
+                return fail(h, SPG_E_INVALID, "prediction %d (stack %d, scale %d): %s is NULL", i, k, j, q.data ? "grad" : "data");
+            if (q.batch_stride < 0 || q.chan_stride < 0 || q.row_stride < 0 ||
+                (backward && (q.grad_batch_stride < 0 || q.grad_chan_stride < 0 || q.grad_row_stride < 0)))
+                return fail(h, SPG_E_INVALID, "prediction %d (stack %d, scale %d): negative stride", i, k, j);
+            if (!aligned(q.data, kern->esz) || (backward && !aligned(q.grad, kern->esz)))
+                return fail(h, SPG_E_INVALID, "prediction %d (stack %d, scale %d): not aligned to its dtype", i, k, j);
+            const long long v = kLossVec;
+            bool vec = (p->width >> j) % kLossVec == 0 && aligned(q.data, vb) && q.batch_stride % v == 0 && q.chan_stride % v == 0 &&
+                       q.row_stride % v == 0;
+            if (backward)
+                vec = vec && aligned(q.grad, vb) && q.grad_batch_stride % v == 0 && q.grad_chan_stride % v == 0 && q.grad_row_stride % v == 0;
+            a.pred[i] = LossPred{q.data, backward ? q.grad : nullptr, q.batch_stride, q.chan_stride, q.row_stride,
+                                 q.grad_batch_stride, q.grad_chan_stride, q.grad_row_stride, (int)vec};
+        }
+    return SPG_OK;
+}
+
+}  // namespace
+
+int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
+                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    const LossKernels *kern;
+    LossArgs a;
+    long long ctas;
+    size_t smem;
+    int rc;
+    if ((rc = loss_setup(h, params, mask_miss, labels, preds, pred_dtype, false, kern, a, ctas, smem))) return rc;
+    if (!stack_sums || !loss) return fail(h, SPG_E_INVALID, "stack_sums or loss is NULL");
+    DeviceGuard guard(h->device);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t need = 256 + sizeof(double) * kLossScales * a.nstack * (size_t)ctas;
+    const bool fresh = h->loss_partial.bytes < need;
+    if ((rc = grow(h, h->loss_partial, need))) return rc;
+    if (fresh) SPG_CUDA(h, cudaMemsetAsync(h->loss_partial.p, 0, 256, st));  // the ticket starts at 0; each launch leaves it so
+    a.ticket = static_cast<unsigned int *>(h->loss_partial.p);
+    a.partial = reinterpret_cast<double *>(static_cast<unsigned char *>(h->loss_partial.p) + 256);
+    a.sums = stack_sums;
+    a.loss = loss;
+    return launch(h, kStageLoss, kern->fwd_name, kern->fwd, dim3((unsigned)ctas), kLossThreads, smem, st, a);
+}
+
+int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
+                      const spg_loss_pred *preds, int32_t pred_dtype, const float *grad_output, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    const LossKernels *kern;
+    LossArgs a;
+    long long ctas;
+    size_t smem;
+    int rc;
+    if ((rc = loss_setup(h, params, mask_miss, labels, preds, pred_dtype, true, kern, a, ctas, smem))) return rc;
+    if (!grad_output) return fail(h, SPG_E_INVALID, "grad_output is NULL");
+    a.grad_output = grad_output;
+    DeviceGuard guard(h->device);
+    return launch(h, kStageLoss, kern->bwd_name, kern->bwd, dim3((unsigned)ctas), kLossThreads, smem, static_cast<cudaStream_t>(stream), a);
 }
 
 // ---- stages ------------------------------------------------------------------------------------

@@ -32,7 +32,7 @@ ST_MEANING = {ST_SAMPLE_INDEX: "SAMPLE_INDEX: a line sample index outside the ma
                             "evaluate.py:226)",
               ST_NAN_PRIORITY: "NAN_PRIORITY: a NaN candidate priority among others (the reference's sort order at "
                                "evaluate.py:259 is undefined)"}
-F32, F64, F32_AS_F64, F16 = 0, 1, 2, 3
+F32, F64, F32_AS_F64, F16, BF16 = 0, 1, 2, 3, 4
 
 
 class GroupingError(RuntimeError):
@@ -109,6 +109,19 @@ TARGET_TINT = np.dtype([("image", np.uint64), ("row_stride", np.int64), ("height
                         ("hue", np.int32), ("saturation", np.int32), ("value", np.int32), ("row_block", np.int32)],
                        align=True)
 
+#: ``spg_loss_params`` and ``spg_loss_pred`` (include/spgroup.h): the training loss's shared record and one record per
+#: prediction tensor (``pred_tuple[k][j]`` at ``k * 5 + j``)
+LOSS_FOCAL, LOSS_L2 = 0, 1
+LOSS_PARAMS = np.dtype([("mode", np.int32), ("nstack", np.int32), ("batch", np.int32), ("channels", np.int32),
+                        ("height", np.int32), ("width", np.int32), ("heat_start", np.int32), ("bkg_start", np.int32),
+                        ("multi_task_weight", np.float64), ("keypoint_task_weight", np.float64),
+                        ("nstack_weight", np.float64, (8,)), ("scale_weight", np.float64, (5,)),
+                        ("batch_divisor", np.float64), ("scale_weight_sum", np.float64),
+                        ("nstack_weight_sum", np.float64)], align=True)
+LOSS_PRED = np.dtype([("data", np.uint64), ("grad", np.uint64), ("batch_stride", np.int64), ("chan_stride", np.int64),
+                      ("row_stride", np.int64), ("grad_batch_stride", np.int64), ("grad_chan_stride", np.int64),
+                      ("grad_row_stride", np.int64)], align=True)
+
 
 class _ImageMaps(C.Structure):
     _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
@@ -152,6 +165,9 @@ _PROTOTYPES = {
     "spg_targets_warp": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_tint": (_int, [_ptr, _ptr, _i32, _ptr]),  # samples: a TARGET_TINT array
+    # params: a LOSS_PARAMS record; preds: a LOSS_PRED array
+    "spg_loss_forward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr]),
+    "spg_loss_backward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -894,6 +910,26 @@ class Grouper:
         s = self._records(records, TARGET_TINT)
         _check(self._lib.spg_targets_tint(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)), "spg_targets_tint",
                self._h)
+
+    # -- training loss (loss.py builds the records) ---------------------------------------------------------------
+    def loss_forward(self, params: np.ndarray, mask_miss: int, labels: int, preds: np.ndarray, dtype: int,
+                     stack_sums: int, loss: int, stream=None) -> None:
+        """``spg_loss_forward``: ``params`` one ``LOSS_PARAMS`` record, ``preds`` a ``LOSS_PRED`` array; the tensors are
+        device addresses on the handle's device.  Asynchronous on ``stream``."""
+        p, r = self._records(params, LOSS_PARAMS), self._records(preds, LOSS_PRED)
+        _check(self._lib.spg_loss_forward(self._h, p.ctypes.data, mask_miss, labels, r.ctypes.data, dtype, stack_sums, loss,
+                                          self._stream_ptr(stream)), "spg_loss_forward", self._h)
+
+    def loss_backward(self, params: np.ndarray, mask_miss: int, labels: int, preds: np.ndarray, dtype: int,
+                      grad_output: int, stream=None) -> None:
+        """``spg_loss_backward``: every ``preds[i]["grad"]`` written from the float32 device scalar at ``grad_output``."""
+        p, r = self._records(params, LOSS_PARAMS), self._records(preds, LOSS_PRED)
+        _check(self._lib.spg_loss_backward(self._h, p.ctypes.data, mask_miss, labels, r.ctypes.data, dtype, grad_output,
+                                           self._stream_ptr(stream)), "spg_loss_backward", self._h)
+
+    def loss_kernel(self) -> str:
+        """Name of the kernel the last loss call launched."""
+        return (self._lib.spg_stage_kernel(self._h, 7) or b"").decode()
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

@@ -235,6 +235,14 @@ class _Device:
             cls._handles[key] = grouping.Grouper(limbs, config.num_parts, max_batch=1, max_h=16, max_w=16, device=device)
         return cls._handles[key]
 
+    @classmethod
+    def for_device(cls, device: int) -> grouping.Grouper:
+        """A handle on ``device`` for the calls that use no limb table (the loss): a cached one, else the default's."""
+        for (d, _, _), g in cls._handles.items():
+            if d == int(device):
+                return g
+        return cls.grouper(TargetConfig(), device)
+
 
 def make_batch(samples: Sequence, augs: Sequence[Optional[AugmentSelection]], config=None, *, device: int = 0,
                stream=None, tint: bool = False):

@@ -59,8 +59,9 @@ enum {
 /* dtype of the body-part planes.  predict() accumulates them in float64 (evaluate.py:86,161); with a single scale
  * (the reference's default, utils/config:26) every float64 value is exactly a float32 one, so the planes can be STORED
  * as float32 and evaluated with the float64 arithmetic the reference applies: SPG_F32_AS_F64 -- half the HBM traffic,
- * bit-identical results to SPG_F64 planes holding the same values.  SPG_F16 is accepted for network outputs only. */
-enum { SPG_F32 = 0, SPG_F64 = 1, SPG_F32_AS_F64 = 2, SPG_F16 = 3 };
+ * bit-identical results to SPG_F64 planes holding the same values.  SPG_F16 is accepted for network outputs and loss
+ * predictions only, SPG_BF16 for loss predictions only. */
+enum { SPG_F32 = 0, SPG_F64 = 1, SPG_F32_AS_F64 = 2, SPG_F16 = 3, SPG_BF16 = 4 };
 
 typedef struct spg_handle spg_handle;
 
@@ -368,6 +369,51 @@ typedef struct spg_target_tint {
  * row_stride, NULL image, row_block), asynchrony and reuse of `samples` as spg_targets_warp. */
 int spg_targets_tint(spg_handle *h, const spg_target_tint *samples, int32_t n_samples, void *stream);
 
+/* ---- training loss: the reference's MultiTaskLoss (models/loss_model.py:22-81, 133-161) and MultiTaskLossParallel's
+ * L2 (models/loss_model_parallel.py:19-75, 120-139) over nstack x 5 prediction tensors ------------------------------ */
+enum {
+    SPG_LOSS_FOCAL = 0,  /* MultiTaskLoss: focal L2 (gamma 1, alpha = beta = 0), mask thresholded at 0.5 and weighted */
+    SPG_LOSS_L2 = 1      /* MultiTaskLossParallel: plain L2 with the interpolated mask; no batch division            */
+};
+typedef struct spg_loss_params {
+    int32_t mode;                /* SPG_LOSS_FOCAL | SPG_LOSS_L2 */
+    int32_t nstack;              /* 1..8 */
+    int32_t batch, channels, height, width;  /* of the targets: labels [B][C][H][W], mask_miss [B][1][H][W]; H and W */
+                                 /* multiples of 16; scale j of every stack is (H >> j) x (W >> j)                   */
+    int32_t heat_start, bkg_start;  /* focal: channels heat_start..bkg_start-1 take keypoint_task_weight */
+    double multi_task_weight;    /* focal: channel C - 2's mask weight */
+    double keypoint_task_weight; /* focal */
+    double nstack_weight[8];     /* [nstack] */
+    double scale_weight[5];
+    double batch_divisor;        /* focal: opt.batch_size; l2: 1 */
+    double scale_weight_sum;     /* sum(scale_weight) as Python sums it */
+    double nstack_weight_sum;    /* sum(nstack_weight) */
+} spg_loss_params;
+/* One prediction tensor, pred_tuple[k][j] at index k * 5 + j: [B][>= C][H >> j][W >> j] with unit column stride.  The
+ * loss reads channels 0..C-1.  Strides are in elements.  grad is written by spg_loss_backward only, with its own strides,
+ * in the same dtype. */
+typedef struct spg_loss_pred {
+    const void *data;
+    void *grad;
+    int64_t batch_stride, chan_stride, row_stride;
+    int64_t grad_batch_stride, grad_chan_stride, grad_row_stride;
+} spg_loss_pred;
+/* The loss of the predictions `preds` (nstack * 5 records, `pred_dtype` SPG_F32 | SPG_BF16 | SPG_F16, all the same)
+ * against labels (float32 [B][C][H][W]) and mask_miss (float32 [B][1][H][W]), both contiguous and 16-byte aligned:
+ * stack_sums [5][nstack] float32 device (the per-stack sums the reference prints, float64 accumulation rounded once) and
+ * *loss float32 device (combined from those sums in the reference's order of float32 operations).  A low-precision
+ * prediction is the reference applied to its float32 value.  Every argument is validated before the first launch
+ * (SPG_E_INVALID names the bad one); asynchronous on `stream`; `params` and `preds` may be reused on return.  The
+ * handle's partial-sum buffer grows on demand (a call with no larger shape than an earlier one allocates nothing); calls
+ * on one handle must not run concurrently on different streams. */
+int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
+                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, void *stream);
+/* Every prediction's gradient of (*grad_output, a float32 device scalar) x loss, written once into preds[i].grad in the
+ * prediction's dtype (the float32 gradient rounded once).  Recomputed from the inputs: independent of any forward call.
+ * Validation, asynchrony and reuse as spg_loss_forward; allocates nothing. */
+int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
+                      const spg_loss_pred *preds, int32_t pred_dtype, const float *grad_output, void *stream);
+
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
 int spg_nms_peaks(spg_handle *h, const float *heat_dev, int64_t image_stride, int64_t chan_stride,
@@ -452,7 +498,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage, 5 pre-network stage, 6 training samples);
+ * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 
