@@ -53,6 +53,7 @@ struct spg_handle {
     int device = 0;
     int sm_count = 0;
     size_t smem_optin = 0;
+    std::vector<std::pair<const void *, size_t>> smem_rooms;  // smem_room's cache: kernel -> dynamic shared memory it may take
     Workspace ws{};
     std::vector<void *> allocs;
     Scratch in_heat, in_paf;  // staging for spg_group_host
@@ -148,6 +149,22 @@ int launch(spg_handle *h, int stage, const char *name, void (*kern)(P...), dim3 
     h->launches++;
     SPG_CUDA(h, cudaGetLastError());
     return SPG_OK;
+}
+
+// The dynamic shared memory a launch of `kern` may ask for: the opt-in limit less the kernel's static __shared__ arrays,
+// because a block needs dynamic + static <= opt-in (cudaFuncSetAttribute refuses a larger dynamic size).  Every plan that
+// sizes dynamic shared memory by the shape or the capacities compares against this, not against smem_optin.  Queried
+// once per kernel and handle; if the query fails, the opt-in limit is returned and the launch reports the CUDA error.
+template <typename... P>
+size_t smem_room(spg_handle *h, void (*kern)(P...)) {
+    const void *key = reinterpret_cast<const void *>(kern);
+    for (const auto &r : h->smem_rooms)
+        if (r.first == key) return r.second;
+    cudaFuncAttributes fa{};
+    if (cudaFuncGetAttributes(&fa, kern) != cudaSuccess) return h->smem_optin;
+    const size_t room = fa.sharedSizeBytes < h->smem_optin ? h->smem_optin - fa.sharedSizeBytes : 0;
+    h->smem_rooms.emplace_back(key, room);
+    return room;
 }
 
 // Every ragged launch's table boundaries: given each member's CTA count, consecutive ranges of at most `capacity`
@@ -280,14 +297,14 @@ struct NmsPlan {
     NmsBanding bg;
 };
 
-// `image` >= 0 names the image of a ragged call in the error
-int plan_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_stride, int H, int W, bool persistent, int image,
-             NmsPlan *pl) {
+// `image` >= 0 names the image of a ragged call in the error; `radius` picks the persistent kernel's instantiation
+int plan_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_stride, int H, int W, bool persistent, int radius,
+             int image, NmsPlan *pl) {
     const int capP = h->ws.capP;
     *pl = NmsPlan{};
     pl->use_bulk = (W % 4 == 0) && (img_stride % 4 == 0) && (chan_stride % 4 == 0) && ((reinterpret_cast<uintptr_t>(heat) & 15) == 0);
     const bool persist = persistent && h->persist && pl->use_bulk;
-    if (persist && nms_persist_smem_bytes(H, W, capP) <= h->smem_optin && (size_t)H * W / 4 < 65536 &&
+    if (persist && nms_persist_smem_bytes(H, W, capP) <= smem_room(h, kNmsPersistKernels[radius]) && (size_t)H * W / 4 < 65536 &&
         (size_t)H * W * sizeof(float) < (1u << 20) &&
         ((size_t)H * W / 4 + kNmsPScanners - 1) / kNmsPScanners <= (size_t)32 * kNmsPMaxIter) {
         // one resident CTA per SM: loader, 28 scanners, 3 finishers over a ring of 3 plane slots
@@ -295,7 +312,9 @@ int plan_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_
         pl->smem = nms_persist_smem_bytes(H, W, capP);
         return SPG_OK;
     }
-    if (persist) pl->bg = nms_banding(H, W, capP, h->smem_optin - 1024);
+    // The bands are sized 1 KB below the opt-in limit, which covers the kernel's static barriers.  The room alone would
+    // change the slot count of some planes that fit either way, so it only caps that budget.
+    if (persist) pl->bg = nms_banding(H, W, capP, std::min(h->smem_optin - 1024, smem_room(h, nms_peaks_banded_kernel)));
     if (pl->bg.slots >= kNmsBTeams) {
         // planes that do not fit three times: the same roles over a ring of ~17 KB band slots, four scanner teams
         pl->kind = NmsPlan::kBanded;
@@ -307,11 +326,12 @@ int plan_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t chan_
     pl->kind = NmsPlan::kBands;
     pl->band_rows = std::max(4, std::min(H, 4096 / W));
     pl->smem = nms_smem_bytes(pl->band_rows, H, W, capP);
-    if (pl->smem <= h->smem_optin) return SPG_OK;
+    const size_t room = std::min(smem_room(h, nms_peaks_kernel), smem_room(h, nms_peaks_ragged_kernel));  // either launches the plan
+    if (pl->smem <= room) return SPG_OK;
     if (image < 0)
-        return fail(h, SPG_E_INVALID, "map width %d needs %zu B of shared memory per band (limit %zu)", W, pl->smem, h->smem_optin);
+        return fail(h, SPG_E_INVALID, "map width %d needs %zu B of shared memory per band (limit %zu)", W, pl->smem, room);
     return fail(h, SPG_E_INVALID, "image %d: map width %d needs %zu B of shared memory per band (limit %zu)", image, W, pl->smem,
-                h->smem_optin);
+                room);
 }
 
 struct ScorePlan {
@@ -319,16 +339,22 @@ struct ScorePlan {
     size_t smem;
 };
 
-ScorePlan plan_score(const spg_handle *h, const ScoreKernels &k, const void *paf, int64_t img_stride, int64_t chan_stride, int H,
-                     int W, bool persistent) {
+// the room of a kind of limb-scoring kernel: the plan must fit its per-plane and its ragged launch alike
+size_t score_room(spg_handle *h, const ScoreKernels &k, int kind) {
+    return std::min(smem_room(h, k.item[kind]), smem_room(h, k.ragged[kind]));
+}
+
+ScorePlan plan_score(spg_handle *h, const ScoreKernels &k, const void *paf, int64_t img_stride, int64_t chan_stride, int H, int W,
+                     bool persistent) {
     const int capP = h->ws.capP;
     const size_t plane_bytes = (size_t)H * W * k.esz;
     const bool aligned = (plane_bytes % 16 == 0) && ((img_stride * k.esz) % 16 == 0) && ((chan_stride * k.esz) % 16 == 0) &&
                          ((reinterpret_cast<uintptr_t>(paf) & 15) == 0) && plane_bytes < (1u << 20);
-    if (persistent && h->persist && k.persist && aligned && capP <= kPersistMaxCapP && persist_smem_bytes(plane_bytes, capP) <= h->smem_optin)
+    if (persistent && h->persist && k.persist && aligned && capP <= kPersistMaxCapP &&
+        persist_smem_bytes(plane_bytes, capP) <= smem_room(h, k.persist))
         return {ScorePlan::kPersist, persist_smem_bytes(plane_bytes, capP)};  // one resident CTA per SM walking a ring of 3 plane slots (loader / screeners / scorers)
     const size_t staged = score_smem_bytes(plane_bytes, capP);
-    if (aligned && staged <= h->smem_optin) return {ScorePlan::kStaged, staged};
+    if (aligned && staged <= score_room(h, k, ScorePlan::kStaged)) return {ScorePlan::kStaged, staged};
     return {ScorePlan::kSampled, score_smem_bytes(0, capP)};  // plane larger than shared memory (or unaligned): sample through L2
 }
 
@@ -376,7 +402,7 @@ int launch_nms(spg_handle *h, const float *heat, int64_t img_stride, int64_t cha
     if (n == 0) return SPG_OK;
     NmsPlan pl;
     int rc;
-    if ((rc = plan_nms(h, heat, img_stride, chan_stride, H, W, true, -1, &pl))) return rc;
+    if ((rc = plan_nms(h, heat, img_stride, chan_stride, H, W, true, p->offset_radius, -1, &pl))) return rc;
     NmsArgs a = nms_args(h, p);
     a.heat = heat;
     a.img_stride = img_stride;
@@ -442,7 +468,8 @@ int launch_assemble(spg_handle *h, int base, int n, const spg_params *p, cudaStr
     h->armed_flag = nullptr;  // one shot
     a.use_bulk = ((size_t)h->ws.L * h->ws.capP * sizeof(uint32_t)) % 16 == 0;  // bulk copies move multiples of 16 bytes
     const size_t smem = assemble_smem_bytes(h->ws.K, h->ws.capP, h->ws.capR) + assemble_conn_bytes(h->ws.L, h->ws.capP);
-    if (smem > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need %zu B of shared memory in assemble (limit %zu)", smem, h->smem_optin);
+    const size_t room = smem_room(h, assemble_kernel);
+    if (smem > room) return fail(h, SPG_E_INVALID, "capacities need %zu B of shared memory in assemble (limit %zu)", smem, room);
     return launch(h, kStageAssemble, "assemble_kernel", assemble_kernel, n, kAssembleThreads, smem, st, a);
 }
 
@@ -451,7 +478,7 @@ int launch_match_assemble(spg_handle *h, int base, int n, const spg_params *p, c
     AssembleArgs a = assemble_args(h, base, n, p);
     a.use_bulk = ((size_t)h->ws.K * h->ws.capP * sizeof(float)) % 16 == 0;  // bulk copies move multiples of 16 bytes
     const size_t smem = match_assemble_smem_bytes(h->ws.K, h->ws.L, h->ws.capP, h->ws.capR, h->ma_warps);
-    if (smem > h->smem_optin) {  // very large capacities: the two stand-alone kernels need less shared memory
+    if (smem > smem_room(h, match_assemble_kernel)) {  // very large capacities: the two stand-alone kernels need less shared memory
         int rc;
         if ((rc = launch_match(h, base, n, st))) return rc;
         return launch_assemble(h, base, n, p, st);  // consumes the armed signal itself
@@ -607,6 +634,11 @@ int spg_create(const spg_config *cfg, spg_handle **out) {
     // score_queue's item queues at 0
     for (int s = 0; s < 2 && rc == SPG_OK; s++)
         if (cudaStreamCreateWithFlags(&h->streams[s], cudaStreamNonBlocking) != cudaSuccess) rc = SPG_E_CUDA;
+    // every limb-scoring plan falls back to the sampled kernels, whose shared memory depends on the capacities alone
+    for (const ScoreKernels &k : kScoreKernels)
+        if (rc == SPG_OK && score_smem_bytes(0, ws.capP) > score_room(h, k, ScorePlan::kSampled))
+            rc = fail(h, SPG_E_INVALID, "max_peaks_per_part %d needs %zu B of shared memory in limb scoring (limit %zu)", ws.capP,
+                      score_smem_bytes(0, ws.capP), score_room(h, k, ScorePlan::kSampled));
     if (rc != SPG_OK) {
         g_create_error = h->err.empty() ? "device allocation failed" : h->err;
         spg_destroy(h);
@@ -1505,9 +1537,10 @@ int loss_setup(spg_handle *h, const spg_loss_params *p, const float *mask, const
         if (k.dtype == dtype) kern = &k;
     if (!kern) return fail(h, SPG_E_INVALID, "pred_dtype %d is not SPG_F32, SPG_BF16 or SPG_F16", dtype);
     if (!preds) return fail(h, SPG_E_INVALID, "preds is NULL");
+    // the forward kernel's room bounds both directions, so that forward and backward admit the same widths
     smem = loss_smem_bytes(p->width);
-    if (smem > h->smem_optin)
-        return fail(h, SPG_E_INVALID, "targets: map width %d needs %zu B of shared memory (limit %zu)", p->width, smem, h->smem_optin);
+    const size_t room = smem_room(h, kern->fwd);
+    if (smem > room) return fail(h, SPG_E_INVALID, "targets: map width %d needs %zu B of shared memory (limit %zu)", p->width, smem, room);
     const int bands = p->height / kLossBand;
     ctas = (long long)p->batch * p->channels * bands;
     if (ctas > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "targets: %lld CTAs are above grid.x's 2^31 - 1", ctas);
@@ -1561,9 +1594,9 @@ int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *
     long long ctas;
     size_t smem;
     int rc;
+    DeviceGuard guard(h->device);  // loss_setup reads the kernels' attributes on the handle's device
     if ((rc = loss_setup(h, params, mask_miss, labels, preds, pred_dtype, false, kern, a, ctas, smem))) return rc;
     if (!stack_sums || !loss) return fail(h, SPG_E_INVALID, "stack_sums or loss is NULL");
-    DeviceGuard guard(h->device);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t need = 256 + sizeof(double) * kLossScales * a.nstack * (size_t)ctas;
     const bool fresh = h->loss_partial.bytes < need;
@@ -1584,10 +1617,10 @@ int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float 
     long long ctas;
     size_t smem;
     int rc;
+    DeviceGuard guard(h->device);  // loss_setup reads the kernels' attributes on the handle's device
     if ((rc = loss_setup(h, params, mask_miss, labels, preds, pred_dtype, true, kern, a, ctas, smem))) return rc;
     if (!grad_output) return fail(h, SPG_E_INVALID, "grad_output is NULL");
     a.grad_output = grad_output;
-    DeviceGuard guard(h->device);
     return launch(h, kStageLoss, kern->bwd_name, kern->bwd, dim3((unsigned)ctas), kLossThreads, smem, static_cast<cudaStream_t>(stream), a);
 }
 
@@ -1678,6 +1711,7 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
     const Workspace &ws = h->ws;
     const ScoreKernels &k = kScoreKernels[dtype];
     const int max_h = std::min(h->cfg.max_h, 32767), max_w = std::min(h->cfg.max_w, 32767);
+    DeviceGuard guard(h->device);  // the plans read the kernels' attributes on the handle's device
     // validate every image before the first launch
     std::vector<int> order((size_t)n);
     NmsPlan np;
@@ -1686,10 +1720,9 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
         if (!im.heat || !im.paf) return fail(h, SPG_E_INVALID, "image %d: heat/paf is NULL", i);
         if (im.height < 2 || im.width < 2 || im.height > max_h || im.width > max_w)
             return fail(h, SPG_E_INVALID, "image %d: map %dx%d outside [2, %dx%d]", i, im.height, im.width, max_h, max_w);
-        if ((rc = plan_nms(h, im.heat, 0, im.heat_chan_stride, im.height, im.width, false, i, &np))) return rc;
+        if ((rc = plan_nms(h, im.heat, 0, im.heat_chan_stride, im.height, im.width, false, 0, i, &np))) return rc;
         order[i] = i;
     }
-    if (score_smem_bytes(0, ws.capP) > h->smem_optin) return fail(h, SPG_E_INVALID, "capacities need too much shared memory in limb scoring");
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
         return (int64_t)images[x].height * images[x].width > (int64_t)images[y].height * images[y].width;
     });
@@ -1700,7 +1733,7 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
     for (int i : order) {
         const spg_image_maps &im = images[i];
         const int H = im.height, W = im.width;
-        plan_nms(h, im.heat, 0, im.heat_chan_stride, H, W, false, i, &np);  // succeeded in the validation above
+        plan_nms(h, im.heat, 0, im.heat_chan_stride, H, W, false, 0, i, &np);  // succeeded in the validation above
         NmsImage d{};
         d.heat = im.heat; d.chan_stride = im.heat_chan_stride; d.H = H; d.W = W; d.band_rows = np.band_rows; d.use_bulk = np.use_bulk; d.slot = i;
         nms_smem = std::max(nms_smem, np.smem);
@@ -1715,7 +1748,6 @@ int spg_group_ragged(spg_handle *h, const spg_image_maps *images, int32_t n, int
             sampled.push_back(s);
         }
     }
-    DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SPG_CUDA(h, cudaMemsetAsync(ws.status, 0, sizeof(uint32_t) * (size_t)n, st));
     if (n == 0) return SPG_OK;

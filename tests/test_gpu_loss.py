@@ -125,17 +125,17 @@ def _clone(leaves, pred_tuple, dtype=None):
     return out, new
 
 
-def _port(pred_tuple, mask, labels, opt, focal):
+def _port(pred_tuple, mask, labels, opt, focal, cfg=CFG):
     from oracle import loss_port
     return loss_port.port_loss(pred_tuple, mask, labels, nstack=opt.nstack, scale_weight=opt.scale_weight,
                                nstack_weight=opt.nstack_weight, batch_size=opt.batch_size, focal=focal,
-                               heat_start=CFG.heat_start, bkg_start=CFG.bkg_start, multi_task_weight=opt.multi_task_weight,
-                               keypoint_task_weight=opt.keypoint_task_weight, offset_start=CFG.offset_start)
+                               heat_start=cfg.heat_start, bkg_start=cfg.bkg_start, multi_task_weight=opt.multi_task_weight,
+                               keypoint_task_weight=opt.keypoint_task_weight, offset_start=cfg.offset_start)
 
 
-def _criterion(opt, focal):
+def _criterion(opt, focal, cfg=CFG):
     from improved_body_parts_b200.loss import MultiTaskLoss, MultiTaskLossParallel
-    return (MultiTaskLoss if focal else MultiTaskLossParallel)(opt, CFG)
+    return (MultiTaskLoss if focal else MultiTaskLossParallel)(opt, cfg)
 
 
 def _ulps(a: float, b: float) -> int:
@@ -143,14 +143,14 @@ def _ulps(a: float, b: float) -> int:
     return abs(int(fa) - int(fb))
 
 
-def _check_case(dev, pred_tuple, leaves, mask, labels, opt, focal, go, exact_sums=False):
+def _check_case(dev, pred_tuple, leaves, mask, labels, opt, focal, go, exact_sums=False, cfg=CFG):
     import torch
-    crit = _criterion(opt, focal)
+    crit = _criterion(opt, focal, cfg)
     loss = crit(pred_tuple, (mask, labels))
     loss.backward(torch.tensor(go, device=dev))
     sums = crit.last_stack_losses.cpu()
     pt, pleaves = _clone(leaves, pred_tuple)
-    r = _port(pt, mask, labels, opt, focal)
+    r = _port(pt, mask, labels, opt, focal, cfg)
     r.loss.backward(torch.tensor(go, device=dev))
     for i, (a, b) in enumerate(zip(leaves, pleaves)):
         assert _same(a.grad, b.grad), f"gradient of leaf {i} differs"
