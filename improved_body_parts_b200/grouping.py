@@ -122,6 +122,20 @@ LOSS_PRED = np.dtype([("data", np.uint64), ("grad", np.uint64), ("batch_stride",
                       ("row_stride", np.int64), ("grad_batch_stride", np.int64), ("grad_chan_stride", np.int64),
                       ("grad_row_stride", np.int64)], align=True)
 
+#: ``spg_coco_params``, ``spg_coco_data`` and ``spg_coco_eval`` (include/spgroup.h): keypoint evaluation's tables, its
+#: packed ground truths and detections, and evaluate()'s results; every array field is a device address
+COCO_IGNORE, COCO_CROWD = 1, 2
+COCO_PARAMS = np.dtype([("iou_thrs", np.uint64), ("rec_thrs", np.uint64), ("area_rng", np.uint64), ("max_dets", np.uint64),
+                        ("kpt_vars", np.uint64), ("n_iou", np.int32), ("n_rec", np.int32), ("n_area", np.int32),
+                        ("n_max_dets", np.int32), ("n_kpt", np.int32)], align=True)
+COCO_DATA = np.dtype([("n_images", np.int32), ("n_cats", np.int32), ("n_gt", np.int32), ("n_dt", np.int32),
+                      ("n_kept", np.int32), ("n_ious", np.int32)] +
+                     [(f, np.uint64) for f in ("gt_start", "dt_start", "kept_start", "iou_start", "dt_unit", "gt_kpts",
+                                               "gt_bbox", "gt_area", "gt_id", "gt_flags", "dt_kpts", "dt_area", "dt_score",
+                                               "dt_id")], align=True)
+COCO_EVAL = np.dtype([(f, np.uint64) for f in ("ious", "dt_order", "dt_rank", "cat_order", "gt_order", "gt_ignore",
+                                               "gt_matches", "dt_matches", "dt_ignore")], align=True)
+
 
 class _ImageMaps(C.Structure):
     _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
@@ -168,6 +182,9 @@ _PROTOTYPES = {
     # params: a LOSS_PARAMS record; preds: a LOSS_PRED array
     "spg_loss_forward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr]),
     "spg_loss_backward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr]),
+    # params / data / eval: a COCO_PARAMS / COCO_DATA / COCO_EVAL record
+    "spg_coco_evaluate": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr]),
+    "spg_coco_accumulate": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -930,6 +947,25 @@ class Grouper:
     def loss_kernel(self) -> str:
         """Name of the kernel the last loss call launched."""
         return (self._lib.spg_stage_kernel(self._h, 7) or b"").decode()
+
+    # -- keypoint evaluation (cocoeval.py builds the records) ------------------------------------------------------
+    def coco_evaluate(self, params: np.ndarray, data: np.ndarray, ev: np.ndarray, stream=None) -> None:
+        """``spg_coco_evaluate``: one ``COCO_PARAMS``, ``COCO_DATA`` and ``COCO_EVAL`` record each, holding device
+        addresses on the handle's device.  Asynchronous on ``stream``."""
+        p, d, e = self._records(params, COCO_PARAMS), self._records(data, COCO_DATA), self._records(ev, COCO_EVAL)
+        _check(self._lib.spg_coco_evaluate(self._h, p.ctypes.data, d.ctypes.data, e.ctypes.data, self._stream_ptr(stream)),
+               "spg_coco_evaluate", self._h)
+
+    def coco_accumulate(self, params: np.ndarray, data: np.ndarray, ev: np.ndarray, precision: int, recall: int,
+                        scores: int, stream=None) -> None:
+        """``spg_coco_accumulate`` into the float64 device arrays at ``precision``, ``recall`` and ``scores``."""
+        p, d, e = self._records(params, COCO_PARAMS), self._records(data, COCO_DATA), self._records(ev, COCO_EVAL)
+        _check(self._lib.spg_coco_accumulate(self._h, p.ctypes.data, d.ctypes.data, e.ctypes.data, precision, recall,
+                                             scores, self._stream_ptr(stream)), "spg_coco_accumulate", self._h)
+
+    def coco_kernel(self) -> str:
+        """Name of the kernel the last keypoint-evaluation call launched."""
+        return (self._lib.spg_stage_kernel(self._h, 8) or b"").decode()
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

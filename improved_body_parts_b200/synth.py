@@ -202,3 +202,83 @@ def make_network_output(seed: int, h: int, w: int, persons: int, *, body_scale: 
     out[1, 30:48] = heat[np.argsort(FLIP_HEAT_ORD[:NUM_PARTS])][..., ::-1]
     out[1] += (rng.random((50, h, w), dtype=np.float32) - 0.5) * np.float32(noise)
     return out
+
+
+def coco_keypoint_set(seed: int, n_images: int, *, first_id: int = 1, categories: int = 1):
+    """A seeded ground truth and result list shaped like ``person_keypoints_val2017`` and ``format_results``' output,
+    for keypoint evaluation: ``(dataset, results)``.
+
+    Per image 0-12 persons of every COCO area range, some of them with no labelled keypoint and about one image in
+    eight with a crowd region (``iscrowd`` 1, no keypoints); 0-25 detections per image, most of them noisy copies of a
+    person (points ``format_results`` writes as ``(0, 0, 0)`` where a joint is missing), the rest false positives, with
+    scores that sometimes tie.  Ground-truth points are integers with visibility 0-2, as in the COCO files.
+    ``categories`` > 1: category c (1-based) of the same images is the set of seed ``seed + 100 (c - 1)``, its
+    annotation ids offset by ``c x 10^6``."""
+    if categories > 1:
+        dataset, results = coco_keypoint_set(seed, n_images, first_id=first_id)
+        ids = [i["id"] for i in dataset["images"]]
+        for c in range(2, categories + 1):
+            d2, r2 = coco_keypoint_set(seed + 100 * (c - 1), n_images, first_id=first_id)
+            remap = dict(zip([i["id"] for i in d2["images"]], ids))
+            for a in d2["annotations"]:
+                a.update(image_id=remap[a["image_id"]], category_id=c, id=a["id"] + c * 10 ** 6)
+            for r in r2:
+                r.update(image_id=remap[r["image_id"]], category_id=c)
+            dataset["annotations"] += d2["annotations"]
+            results += r2
+        dataset["categories"] = [{"id": c, "name": f"person{c}", "supercategory": "person"}
+                                 for c in range(1, categories + 1)]
+        return dataset, results
+    rng = np.random.default_rng(seed)
+    images, anns, results = [], [], []
+    tmpl = np.concatenate([_TEMPLATE[:1], _TEMPLATE[2:]])[:17]  # 17 points, the neck dropped
+    ann_id = first_id
+    for n in range(n_images):
+        img_id = first_id + 7 * n + int(rng.integers(0, 7))
+        W, H = int(rng.integers(320, 641)), int(rng.integers(240, 481))
+        images.append({"id": img_id, "file_name": f"{img_id:012d}.jpg", "width": W, "height": H})
+        persons, has_boxless = [], False
+        for _ in range(int(rng.integers(0, 13)) if rng.random() < 0.9 else 0):
+            scale = float(np.exp(rng.uniform(np.log(0.3), np.log(8.0))))
+            cx, cy = rng.uniform(0, W), rng.uniform(0, H)
+            pts = np.stack([cx + tmpl[:, 0] * scale, cy + tmpl[:, 1] * scale], 1) + rng.normal(0, 0.5, (17, 2))
+            # at most one keypoint-less ground truth (a person or the crowd region) per image: two of them around one
+            # detection give it OKS that differ only by the rounding of far points' terms, a near-tie no test can pin
+            boxless = rng.random() < 0.1 and not has_boxless
+            has_boxless |= boxless
+            vis = np.zeros(17, int) if boxless else rng.choice([0, 1, 2], size=17, p=[0.25, 0.15, 0.6])
+            kp = np.zeros((17, 3), np.int64)
+            kp[vis > 0, 0:2] = np.rint(pts[vis > 0]).astype(np.int64)
+            kp[:, 2] = vis
+            x0, y0 = pts.min(0) - scale
+            bw, bh = pts.max(0) - pts.min(0) + 2 * scale
+            area = float(bw * bh * rng.uniform(0.4, 0.7))
+            anns.append({"id": ann_id, "image_id": img_id, "category_id": 1, "iscrowd": 0,
+                         "num_keypoints": int((vis > 0).sum()), "keypoints": kp.reshape(-1).tolist(),
+                         "bbox": [float(x0), float(y0), float(bw), float(bh)], "area": area})
+            ann_id += 1
+            persons.append((pts, scale))
+        if rng.random() < 0.125 and not has_boxless:
+            bw, bh = rng.uniform(30, 200), rng.uniform(30, 200)
+            anns.append({"id": ann_id, "image_id": img_id, "category_id": 1, "iscrowd": 1, "num_keypoints": 0,
+                         "keypoints": [0] * 51, "bbox": [float(rng.uniform(0, W - bw)), float(rng.uniform(0, H - bh)),
+                                                         float(bw), float(bh)], "area": float(bw * bh * 0.6)})
+            ann_id += 1
+        n_det = int(rng.integers(0, 26)) if persons or rng.random() < 0.3 else 0
+        for _ in range(n_det):
+            if persons and rng.random() < 0.75:
+                pts, scale = persons[int(rng.integers(0, len(persons)))]
+                xy = pts + rng.normal(0, rng.uniform(0.1, 1.5) * scale, (17, 2))
+            else:
+                scale = float(np.exp(rng.uniform(np.log(0.3), np.log(8.0))))
+                xy = np.stack([rng.uniform(0, W) + tmpl[:, 0] * scale, rng.uniform(0, H) + tmpl[:, 1] * scale], 1)
+            miss = rng.random(17) < 0.15
+            xy[miss] = 0.0
+            kp = np.concatenate([xy, (~miss)[:, None].astype(np.float64)], 1)
+            score = float(np.round(rng.uniform(0.05, 1.0), 2 if rng.random() < 0.3 else 12))
+            results.append({"image_id": img_id, "category_id": 1,
+                            "keypoints": [v if j % 3 != 2 else int(v) for j, v in enumerate(kp.reshape(-1).tolist())],
+                            "score": score})
+    dataset = {"images": images, "annotations": anns,
+               "categories": [{"id": 1, "name": "person", "supercategory": "person"}]}
+    return dataset, results

@@ -414,6 +414,62 @@ int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *
 int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
                       const spg_loss_pred *preds, int32_t pred_dtype, const float *grad_output, void *stream);
 
+/* ---- keypoint evaluation: pycocotools' COCOeval(iouType='keypoints') evaluate() and accumulate() (evaluate.py:617-619)
+ * on packed device arrays.  A unit is one (category, image) pair, u = category * n_images + image, in the sorted order
+ * of params.catIds and params.imgIds.  Every array below is a device array; counts are element counts. -------------- */
+typedef struct spg_coco_params {
+    const double *iou_thrs;  /* [n_iou]: params.iouThrs */
+    const double *rec_thrs;  /* [n_rec]: params.recThrs */
+    const double *area_rng;  /* [n_area][2]: params.areaRng */
+    const int32_t *max_dets; /* [n_max_dets]: params.maxDets, ascending (evaluate() sorts them); a detection counts */
+                             /* for max_dets[m] below that rank and below its unit's kept count                   */
+    const double *kpt_vars;  /* [n_kpt]: (params.kpt_oks_sigmas * 2) ** 2 as numpy computes it */
+    int32_t n_iou, n_rec, n_area, n_max_dets, n_kpt;  /* n_kpt 1..128 */
+} spg_coco_params;
+typedef struct spg_coco_data {
+    int32_t n_images, n_cats;
+    int32_t n_gt, n_dt;   /* ground truths and detections, each grouped by unit, in annotation order within a unit */
+    int32_t n_kept;       /* sum over units of min(detections, max_dets[n_max_dets - 1]) */
+    int32_t n_ious;       /* sum over units of min(detections, max_dets[n_max_dets - 1]) x ground truths */
+    const int32_t *gt_start, *dt_start, *kept_start, *iou_start;  /* [n_units + 1]: each unit's first entry */
+    const int32_t *dt_unit;  /* [n_dt] */
+    const double *gt_kpts;   /* [n_gt][n_kpt][3] */
+    const double *gt_bbox;   /* [n_gt][4] */
+    const double *gt_area;   /* [n_gt] */
+    const int64_t *gt_id;    /* [n_gt] */
+    const uint8_t *gt_flags; /* [n_gt]: SPG_COCO_IGNORE | SPG_COCO_CROWD */
+    const double *dt_kpts;   /* [n_dt][n_kpt][3] */
+    const double *dt_area, *dt_score;  /* [n_dt] */
+    const int64_t *dt_id;    /* [n_dt] */
+} spg_coco_data;
+enum {
+    SPG_COCO_IGNORE = 1, /* _prepare's gt['ignore']: iscrowd or num_keypoints == 0 */
+    SPG_COCO_CROWD = 2   /* int(gt['iscrowd']) != 0 */
+};
+/* evaluate()'s results, which accumulate() reads. */
+typedef struct spg_coco_eval {
+    double *ious;          /* [n_ious]: per unit its [kept][gts] OKS matrix (computeOks), rows in score order */
+    int32_t *dt_order;     /* [n_dt]: per unit, its detections' indices sorted by descending score (stable) */
+    int32_t *dt_rank;      /* [n_dt]: each detection's position in its unit's dt_order */
+    int32_t *cat_order;    /* [n_dt]: per category, its detections in image order stably sorted by descending score */
+    int32_t *gt_order;     /* [n_area][n_gt]: per unit, its ground truths' indices in evaluateImg's order */
+    uint8_t *gt_ignore;    /* [n_area][n_gt]: evalImgs' gtIgnore, in gt_order */
+    int64_t *gt_matches;   /* [n_area][n_iou][n_gt]: gtMatches (the matched detection's id, or 0), in gt_order */
+    int64_t *dt_matches;   /* [n_area][n_iou][n_kept]: dtMatches (the matched ground truth's id, or 0), in dt_order */
+    uint8_t *dt_ignore;    /* [n_area][n_iou][n_kept]: dtIgnore */
+} spg_coco_eval;
+/* computeOks and evaluateImg for every unit, area range and threshold.  Sorts use NaN-last keys with -0.0 == 0.0 and
+ * keep ties in input order, as numpy's mergesort.  Every count and product of counts must fit in int32; arguments are
+ * validated before the first launch.  Asynchronous on `stream`; the handle's sort scratch grows on demand, so calls on
+ * one handle must not run concurrently on different streams. */
+int spg_coco_evaluate(spg_handle *h, const spg_coco_params *params, const spg_coco_data *data, const spg_coco_eval *eval,
+                      void *stream);
+/* accumulate() from spg_coco_evaluate's results with the same params and data: precision and scores
+ * [n_iou][n_rec][n_cats][n_area][n_max_dets] and recall [n_iou][n_cats][n_area][n_max_dets], float64; -1 where a
+ * (category, area range) has no ground truth that is not ignored.  Asynchronous; the scratch grows on demand. */
+int spg_coco_accumulate(spg_handle *h, const spg_coco_params *params, const spg_coco_data *data, const spg_coco_eval *eval,
+                        double *precision, double *recall, double *scores, void *stream);
+
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
 int spg_nms_peaks(spg_handle *h, const float *heat_dev, int64_t image_stride, int64_t chan_stride,
@@ -498,7 +554,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss);
+ * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 

@@ -21,7 +21,10 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
 4. fills the globals ``evaluate.__main__`` would set (``:643-646``): ``params, model_params`` from the reference's own
    ``utils/config`` through ``skeleton.read_reference_ini`` (``utils/config_reader.py:7`` hard-codes the author's path),
    ``show_eval_speed``;
-5. optionally replaces ``format_results`` (``:563-582``) by ``wire.format_results`` (same file contents).
+5. optionally replaces ``format_results`` (``:563-582``) by ``wire.format_results`` (same file contents);
+6. with ``--device-cocoeval`` (``prepare(..., device_cocoeval=True)``) binds ``evaluate.COCOeval`` to
+   ``cocoeval.COCOeval``, which scores the results on the GPU (``:617-620``), and ``evaluate.COCO`` to
+   ``cocoeval.COCO`` where pycocotools is missing, so that ``validation()`` produces its metric without pycocotools.
 
 ``prepare()`` returns the module; building ``evaluate.posenet`` (``:626-641``: checkpoint + apex amp) and calling
 ``evaluate.validation(...)`` is then exactly what ``evaluate.__main__`` does.  With ``--check`` the launcher runs one
@@ -92,12 +95,14 @@ def init_ranks() -> int:
 
 
 def prepare(reference_root: str, config_path: str = None, device: int = None, install: bool = True,
-            replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1, gpus: int = None):
+            replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1, gpus: int = None,
+            device_cocoeval: bool = False):
     """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites.
 
     ``gpus=G`` (under ``torchrun --nproc-per-node G``, with ``batch > 1``) joins the process group, pins this rank to
     its ``LOCAL_RANK`` device and installs the ``predict_many`` that shards the images over the G ranks; run
-    ``validate`` on every rank."""
+    ``validate`` on every rank.  ``device_cocoeval=True`` puts the GPU keypoint evaluation behind ``evaluate.COCOeval``
+    (and the minimal loader behind ``evaluate.COCO`` when pycocotools was stubbed)."""
     if gpus is not None:
         err = gpus_error(int(gpus), int(batch))
         if err:
@@ -140,6 +145,11 @@ def prepare(reference_root: str, config_path: str = None, device: int = None, in
     evaluate.show_eval_speed = False
     if replace_format_results:
         evaluate.format_results = wire.format_results
+    if device_cocoeval:
+        from improved_body_parts_b200 import cocoeval
+        evaluate.COCOeval = cocoeval.COCOeval
+        if "pycocotools.coco" in stubbed:
+            evaluate.COCO = cocoeval.COCO
     evaluate.__spg_stubbed__ = stubbed
     return evaluate
 
@@ -170,6 +180,8 @@ def main() -> None:
                     help="images per grouping call in predict_many (> 1 implies the device predict; default 1)")
     ap.add_argument("--forward-batch", type=int, default=1,
                     help="images per network forward pass in predict_many (> 1 needs --batch > 1; default 1)")
+    ap.add_argument("--device-cocoeval", action="store_true",
+                    help="score validation() with the GPU COCOeval (and the minimal COCO loader without pycocotools)")
     ap.add_argument("--gpus", type=int, default=None,
                     help="under torchrun --nproc-per-node G: shard predict_many's images over the G GPUs (needs --batch > 1)")
     a = ap.parse_args()
@@ -187,7 +199,8 @@ def main() -> None:
         err = gpus_error(a.gpus, a.batch)
         if err:
             ap.error(err)
-    ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch, gpus=a.gpus)
+    ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch, gpus=a.gpus,
+                 device_cocoeval=a.device_cocoeval)
     rank = f"rank {os.environ['RANK']}: " if a.gpus is not None else ""
     print(f"{rank}evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
           f"find_peaks -> {ev.find_peaks.__module__}.{ev.find_peaks.__name__}")

@@ -40,3 +40,11 @@ g3.group_device(torch.from_numpy(heat3).to(dev), torch.from_numpy(paf3).to(dev),
 k3 = g3.stage_kernels()
 torch.cuda.synchronize()
 print("persons", r.n_persons.tolist(), "status", r.status.tolist(), "kernels", k1, g.stage_kernels(), "postnet", tuple(h1.shape), tuple(p3.shape), tuple(hi.shape), "large planes", k3)
+# keypoint evaluation: the sorts, OKS, matcher and accumulation kernels on a 37-image val2017-shaped set with three
+# categories (the accumulation's CTAs of different categories share a launch)
+from improved_body_parts_b200 import cocoeval
+ds, res = synth.coco_keypoint_set(1037, 37, categories=3)
+gt = cocoeval.COCO(); gt.dataset = ds; gt.createIndex()
+ce = cocoeval.COCOeval(gt, gt.loadRes(res)); ce.evaluate(); ce.accumulate()
+torch.cuda.synchronize()
+print("cocoeval", ce.eval["counts"], float(ce.eval["precision"].max()))
