@@ -24,13 +24,14 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import sharding, wire
-from .grouping import ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry
+from .grouping import JPEG_OK, JPEG_RECORD, ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
 _device = 0
 _variant = "evaluate"
 _input_stage = "host"
+_decode = "host"
 _groupers: Dict[int, Grouper] = {}  # the max_batch=1 handle of the per-image calls, per device
 _ragged: Dict[int, Grouper] = {}  # the handle of the batched calls (group_many / predict_many), per device
 CAP_PEAKS, CAP_CANDS, CAP_ROWS = 128, 4096, 128
@@ -50,14 +51,24 @@ def _forward_batch(n) -> int:
 
 
 def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optional[int] = None,
-              variant: Optional[str] = None, input_stage: Optional[str] = None) -> None:
+              variant: Optional[str] = None, input_stage: Optional[str] = None, decode: Optional[str] = None) -> None:
     """Select the limb table (default: the Canonical ``limbs_conn``, config/config.py:94), the CUDA device, the
     behavioural variant: ``"evaluate"`` (evaluate.py, the default) or ``"demo"`` (demo_image.py's inlined copy, which
-    differs at :288, :414-415 and :533 -- SURVEY.md 3.2), and where ``predict`` builds the network's input:
-    ``"host"`` (cv2, the default) or ``"device"`` (``spg_prenet``)."""
-    global _limbs, _device, _variant, _input_stage
-    if input_stage is not None:
-        _input_stage = _stage(input_stage)
+    differs at :288, :414-415 and :533 -- SURVEY.md 3.2), where ``predict`` builds the network's input:
+    ``"host"`` (cv2, the default) or ``"device"`` (``spg_prenet``), and how ``predict_many`` reads the image files:
+    ``"host"`` (``cv2.imread``, the default) or ``"device"`` (``imread_many``: each group of ``batch`` files decoded on
+    the GPU in one call), which needs the device input stage.  The combination is checked after the call's changes:
+    with ``decode="device"`` in effect, ``configure(input_stage="host")`` raises ``ValueError`` unless it also passes
+    ``decode="host"``."""
+    global _limbs, _device, _variant, _input_stage, _decode
+    stage = _input_stage if input_stage is None else _stage(input_stage)
+    dec = _decode if decode is None else decode
+    if dec not in ("host", "device"):
+        raise ValueError("decode must be 'host' or 'device'")
+    if dec == "device" and stage != "device":
+        raise ValueError("decode='device' needs input_stage='device': the network input is built from the decoded CUDA "
+                         "image")
+    _input_stage, _decode = stage, dec
     if limbs is not None:
         _limbs = tuple((int(a), int(b)) for a, b in limbs)
     if device is not None:
@@ -257,6 +268,64 @@ def _upload_images(images) -> list:
         for i, a in host_imgs.items():
             out[i] = packed[at[i]:at[i] + a.size].view(a.shape)
     return out
+
+
+def imread_many(paths) -> Tuple[list, int]:
+    """``cv2.imread(path)`` of every path as a ``[H, W, 3]`` uint8 CUDA tensor on the current device, in order, and the
+    number of files that were read on the host.
+
+    The files are read and parsed (``spg_jpeg_parse``); the ones the device decoder takes -- baseline and
+    extended-sequential Huffman JPEGs, grey or YCbCr 4:4:4 / 4:2:2 / 4:4:0 / 4:2:0 -- go up together through one pinned
+    buffer and one copy and are decoded in one ``spg_jpeg_decode_ragged`` call, bit-identical to ``cv2.imread``.  Every
+    other file (progressive, another format, anything the parser or the decoder finds malformed) is read with
+    ``cv2.imread`` and uploaded: those are the host fallbacks.  A file cv2 cannot read, a missing or unreadable path
+    included, gives ``None``, as ``cv2.imread`` does."""
+    import cv2
+    import torch
+    dev = torch.device("cuda", _device)
+    datas = []
+    for p in paths:
+        try:
+            with open(p, "rb") as f:
+                datas.append(f.read())
+        except OSError:  # missing or unreadable: cv2.imread below gives None for it
+            datas.append(None)
+    todo = [i for i, d in enumerate(datas) if d is not None]
+    recs = {i: jpeg_parse(datas[i]) for i in todo}
+    todo = [i for i in todo if recs[i]["status"] == JPEG_OK]
+    out = [None] * len(datas)
+    if todo:
+        nbytes = sum(len(datas[i]) for i in todo)
+        host = _pinned("jpeg", nbytes, torch.uint8)
+        staged, at, off = host.numpy(), [], 0
+        for i in todo:
+            staged[off:off + len(datas[i])] = np.frombuffer(datas[i], np.uint8)
+            at.append(off)
+            off += len(datas[i])
+        files = host.to(dev, non_blocking=True)
+        _copied("jpeg")
+        sizes = [int(recs[i]["height"]) * int(recs[i]["width"]) * 3 for i in todo]
+        images = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
+        status = torch.empty(len(todo), dtype=torch.int32, device=dev)
+        arr = np.zeros(len(todo), JPEG_RECORD)
+        o = 0
+        for k, i in enumerate(todo):
+            arr[k] = recs[i]
+            arr[k]["data"], arr[k]["out"] = files.data_ptr() + at[k], images.data_ptr() + o
+            arr[k]["decode_status"] = status.data_ptr() + 4 * k
+            out[i] = images[o:o + sizes[k]].view(int(recs[i]["height"]), int(recs[i]["width"]), 3)
+            o += sizes[k]
+        _grouper().jpeg_decode(arr)
+        for k, st in enumerate(status.cpu().tolist()):  # synchronises the decode
+            if st != JPEG_OK:
+                out[todo[k]] = None
+    host_reads = 0
+    for i, p in enumerate(paths):
+        if out[i] is None:
+            host_reads += 1
+            img = cv2.imread(p)
+            out[i] = None if img is None else torch.from_numpy(img).to(dev)
+    return out, host_reads
 
 
 def predict(image, params, model, model_params, heat_layers=None, paf_layers=None, input_image_path=None,
@@ -668,11 +737,13 @@ def predict_many(coco, images_directory, validation_ids, params, model, model_pa
 def _predict_block(images_directory, named_ids, params, model, model_params, heat_layers, paf_layers, batch: int,
                    fb: int, at: Optional[list] = None) -> dict:
     """The body of ``predict_many`` over ``named_ids`` = ``[(image_id, file name)]``: ``{image_id: people}`` in that
-    order.  ``at`` (a list) is kept holding the ids of the image or grouping batch being worked on, for error reports."""
+    order.  ``at`` (a list) is kept holding the ids of the image or grouping batch being worked on, for error reports.
+    With ``configure(decode="device")`` each group of ``batch`` files is read with one ``imread_many`` call."""
     import os
 
     import cv2
     at = [] if at is None else at
+    named_ids = list(named_ids)
     keypoints = {}
     pending = []  # (image_id, (heatmap, paf) -- or the image itself for predict_batch, oriImg.shape[0])
 
@@ -687,17 +758,23 @@ def _predict_block(images_directory, named_ids, params, model, model_params, hea
                 keypoints[iid] = kp
             pending.clear()
 
-    for image_id, name in named_ids:
-        at[:] = [image_id]
-        path = os.path.join(images_directory, name)
-        ori = cv2.imread(path)  # B,G,R order (evaluate.py:502)
-        if fb > 1:
-            pending.append((image_id, ori, ori.shape[0]))
-        else:
-            pending.append((image_id, predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers, path),
-                            ori.shape[0]))
-        if len(pending) >= batch:
-            flush()
+    for g0 in range(0, len(named_ids), batch):
+        group = named_ids[g0:g0 + batch]
+        paths = [os.path.join(images_directory, name) for _, name in group]
+        decoded = None
+        if _decode == "device":
+            at[:] = [iid for iid, _ in group]
+            decoded = imread_many(paths)[0]
+        for k, (image_id, _) in enumerate(group):
+            at[:] = [image_id]
+            ori = decoded[k] if decoded is not None else cv2.imread(paths[k])  # B,G,R order (evaluate.py:502)
+            if fb > 1:
+                pending.append((image_id, ori, int(ori.shape[0])))
+            else:
+                pending.append((image_id, predict(ori, dict(params), model, dict(model_params), heat_layers + 2, paf_layers,
+                                                  paths[k]), int(ori.shape[0])))
+            if len(pending) >= batch:
+                flush()
     flush()
     return keypoints
 
@@ -804,7 +881,7 @@ def keypoint_heatmap_nms(heat, kernel: int = 3, thre: float = 0.1):
 
 
 def install(evaluate_module, device_predict: bool = False, device_input: bool = False, batch: int = 1,
-            forward_batch: int = 1) -> None:
+            forward_batch: int = 1, device_decode: bool = False) -> None:
     """Rebind ``find_peaks / find_connections / find_people`` of an imported reference ``evaluate`` module.
 
     ``limbSeq`` is taken from the module (evaluate.py:54) so alternative skeletons keep working.  With
@@ -815,7 +892,9 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     groups ``batch`` images per call; it uses the module's ``posenet`` and ``get_image_name`` and leaves the module's
     ``batch_time`` meter alone.  ``forward_batch > 1`` (with ``device_predict`` and ``batch > 1``) makes that
     ``predict_many`` run the network on up to ``forward_batch`` items (images, or with a multi-scale or rotation search
-    their scaled and rotated copies) of the same input size at once (``predict_batch``).  In an initialised
+    their scaled and rotated copies) of the same input size at once (``predict_batch``).  ``device_decode`` (with
+    ``device_input`` and ``batch > 1``) makes that ``predict_many`` decode each group of ``batch`` JPEG files on the GPU
+    (``imread_many``) instead of ``cv2.imread`` per file.  In an initialised
     ``torch.distributed`` world of N > 1 processes, one per GPU, each with ``configure(device=local_rank)``, that
     ``predict_many`` shards the images over the ranks: rank 0 calls it (``evaluate.validation()``), the other ranks
     run ``serve_predict_many`` until rank 0 calls ``end_serving``."""
@@ -824,7 +903,11 @@ def install(evaluate_module, device_predict: bool = False, device_input: bool = 
     fb = _forward_batch(forward_batch)
     if fb > 1 and (not device_predict or int(batch) < 2):
         raise ValueError("forward_batch > 1 needs device_predict=True and batch > 1: it batches predict_many's forward passes")
-    configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host")
+    if device_decode and (not (device_predict and device_input) or int(batch) < 2):
+        raise ValueError("device_decode needs device_predict=True, device_input=True and batch > 1: it replaces the "
+                         "cv2.imread of predict_many, whose images feed the device input stage")
+    configure(limbs=getattr(evaluate_module, "limbSeq", _limbs), input_stage="device" if device_input else "host",
+              decode="device" if device_decode else "host")
     evaluate_module.find_peaks = find_peaks
     evaluate_module.find_connections = find_connections
     evaluate_module.find_people = find_people

@@ -136,6 +136,27 @@ COCO_DATA = np.dtype([("n_images", np.int32), ("n_cats", np.int32), ("n_gt", np.
 COCO_EVAL = np.dtype([(f, np.uint64) for f in ("ious", "dt_order", "dt_rank", "cat_order", "gt_order", "gt_ignore",
                                                "gt_matches", "dt_matches", "dt_ignore")], align=True)
 
+#: ``spg_jpeg_huff`` and ``spg_jpeg_record`` (include/spgroup.h): one parsed JPEG file; ``spg_jpeg_parse`` fills it and
+#: the caller sets ``data``, ``out`` and ``decode_status`` (device addresses) for ``spg_jpeg_decode_ragged``
+JPEG_OK, JPEG_CORRUPT, JPEG_RANGE = 0, 11, 12
+JPEG_HUFF = np.dtype([("lookup", np.uint16, (512,)), ("maxcode", np.int32, (18,)), ("valoff", np.int32, (18,)),
+                      ("symbols", np.uint8, (256,))], align=True)
+JPEG_RECORD = np.dtype([(f, np.int32) for f in ("status", "orientation", "height", "width", "frame_height", "frame_width",
+                                                "n_components", "h_samp", "v_samp", "mcus_x", "mcus_y", "blocks_per_mcu",
+                                                "restart_interval", "n_intervals")] +
+                       [("scan_offset", np.int64), ("scan_length", np.int64), ("quant", np.uint16, (3, 64)),
+                        ("dc", JPEG_HUFF, (3,)), ("ac", JPEG_HUFF, (3,)), ("data", np.uint64), ("out", np.uint64),
+                        ("decode_status", np.uint64)], align=True)
+
+
+def jpeg_parse(data) -> np.ndarray:
+    """``spg_jpeg_parse`` of one file's bytes (host only): a ``JPEG_RECORD`` whose ``status`` is ``JPEG_OK`` or the
+    reason the file is left to cv2."""
+    buf = np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, np.uint8)
+    rec = np.zeros(1, JPEG_RECORD)
+    _check(load_library().spg_jpeg_parse(buf.ctypes.data if buf.size else None, buf.size, rec.ctypes.data), "spg_jpeg_parse")
+    return rec[0]
+
 
 class _ImageMaps(C.Structure):
     _fields_ = [("heat", C.c_void_p), ("paf", C.c_void_p), ("heat_chan_stride", C.c_int64),
@@ -185,6 +206,9 @@ _PROTOTYPES = {
     # params / data / eval: a COCO_PARAMS / COCO_DATA / COCO_EVAL record
     "spg_coco_evaluate": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr]),
     "spg_coco_accumulate": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr]),
+    # record: a JPEG_RECORD; records: a JPEG_RECORD array
+    "spg_jpeg_parse": (_int, [_ptr, _i64, _ptr]),
+    "spg_jpeg_decode_ragged": (_int, [_ptr, _ptr, _i32, _ptr]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -966,6 +990,20 @@ class Grouper:
     def coco_kernel(self) -> str:
         """Name of the kernel the last keypoint-evaluation call launched."""
         return (self._lib.spg_stage_kernel(self._h, 8) or b"").decode()
+
+    # -- JPEG decoding (dropin.imread_many builds the records) ------------------------------------------------------
+    def jpeg_decode(self, records: np.ndarray, stream=None) -> None:
+        """``spg_jpeg_decode_ragged``: ``records`` a ``JPEG_RECORD`` array of files parsed with status ``JPEG_OK``, each
+        with the device addresses of its bytes, its ``[height, width, 3]`` uint8 output and its int32 decode status.
+        Asynchronous on ``stream``; read the statuses after it (``JPEG_CORRUPT`` / ``JPEG_RANGE``: leave the file to
+        cv2)."""
+        s = self._records(records, JPEG_RECORD)
+        _check(self._lib.spg_jpeg_decode_ragged(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)),
+               "spg_jpeg_decode_ragged", self._h)
+
+    def jpeg_kernel(self) -> str:
+        """Name of the kernel the last JPEG decode launched."""
+        return (self._lib.spg_stage_kernel(self._h, 9) or b"").decode()
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

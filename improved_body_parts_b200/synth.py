@@ -282,3 +282,16 @@ def coco_keypoint_set(seed: int, n_images: int, *, first_id: int = 1, categories
     dataset = {"images": images, "annotations": anns,
                "categories": [{"id": 1, "name": "person", "supercategory": "person"}]}
     return dataset, results
+
+
+def photo(seed: int, h: int, w: int, grey: bool = False) -> np.ndarray:
+    """A seeded photo-like uint8 BGR (or grey) image: smooth noise at several scales plus fine grain, so that a JPEG of it
+    has the size and coefficient statistics of a camera picture rather than of white noise."""
+    import cv2
+    rng = np.random.default_rng(seed)
+    out = np.zeros((h, w, 3), np.float32)
+    for s, amp in ((64, 45.0), (16, 30.0), (4, 18.0), (1, 8.0)):
+        n = rng.standard_normal((h // s + 2, w // s + 2, 3)).astype(np.float32)
+        out += cv2.resize(n, (w, h), interpolation=cv2.INTER_CUBIC) * amp
+    img = np.clip(out + 128, 0, 255).astype(np.uint8)
+    return cv2.cvtColor(img, cv2.COLOR_BGR2GRAY) if grey else img

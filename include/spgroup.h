@@ -470,6 +470,67 @@ int spg_coco_evaluate(spg_handle *h, const spg_coco_params *params, const spg_co
 int spg_coco_accumulate(spg_handle *h, const spg_coco_params *params, const spg_coco_data *data, const spg_coco_eval *eval,
                         double *precision, double *recall, double *scores, void *stream);
 
+/* ---- JPEG decoding: what cv2.imread(path) returns for the validation images (evaluate.py:502), on the device ---------
+ * Baseline and extended-sequential Huffman files (SOF0 / SOF1) with 8-bit samples, 8- or 16-bit quantisation tables, one
+ * component (returned as BGR, as IMREAD_COLOR does) or three YCbCr components in one interleaved scan with luma sampling
+ * 1x1, 2x1, 1x2 or 2x2 and 1x1 chroma, with or without restart intervals, any APPn / COM segments, and the EXIF
+ * orientation OpenCV applies.  The output equals OpenCV 4.x with libjpeg-turbo's default decode (islow IDCT, fancy
+ * upsampling) bit for bit.  Every other file is refused with a reason, for the caller to read with cv2. */
+enum {
+    SPG_JPEG_OK = 0,
+    SPG_JPEG_NOT_JPEG = 1,   /* no SOI marker */
+    SPG_JPEG_TRUNCATED = 2,  /* a segment or the entropy-coded data runs past the end of the buffer, or no EOI */
+    SPG_JPEG_PROCESS = 3,    /* progressive, lossless, arithmetic-coded or hierarchical */
+    SPG_JPEG_PRECISION = 4,  /* samples other than 8-bit */
+    SPG_JPEG_COLOR = 5,      /* not 1 or 3 components, or 3 that libjpeg treats as RGB (Adobe transform 0, ids 'R','G','B') */
+    SPG_JPEG_SAMPLING = 6,   /* sampling other than luma 1x1 / 2x1 / 1x2 / 2x2 with 1x1 chroma */
+    SPG_JPEG_SCAN = 7,       /* more than one scan, a scan without every component in frame order, or Ss/Se/Ah/Al */
+    SPG_JPEG_TABLES = 8,     /* a missing or invalid quantisation or Huffman table */
+    SPG_JPEG_MALFORMED = 9,  /* a length, count or marker libjpeg rejects or treats as corrupt */
+    SPG_JPEG_EXIF = 10,      /* an EXIF block whose orientation cannot be read the way OpenCV reads it */
+    SPG_JPEG_CORRUPT = 11,   /* decoder: a bad Huffman code, a coefficient index past 63, too few bits or blocks */
+    SPG_JPEG_RANGE = 12      /* decoder: a block outside the range where libjpeg-turbo's SIMD and C islow IDCTs agree */
+};
+/* A decoding table of one Huffman table. */
+typedef struct spg_jpeg_huff {
+    uint16_t lookup[512];    /* the next 9 bits -> (code length << 8) | symbol; 0: the code is longer than 9 bits */
+    int32_t maxcode[18];     /* [l]: the largest code of length l (1..16), -1 when there is none */
+    int32_t valoff[18];      /* [l]: symbols[code + valoff[l]] is the symbol of a code of length l */
+    uint8_t symbols[256];
+} spg_jpeg_huff;
+/* One parsed file.  spg_jpeg_parse fills everything down to `ac`; the caller sets the last three fields for
+ * spg_jpeg_decode_ragged. */
+typedef struct spg_jpeg_record {
+    int32_t status;          /* SPG_JPEG_OK, or why the file is refused (the fields below are then unspecified) */
+    int32_t orientation;     /* EXIF orientation 1..8 (1 when absent) */
+    int32_t height, width;   /* the decoded image: after the orientation */
+    int32_t frame_height, frame_width;  /* as coded (SOF) */
+    int32_t n_components;    /* 1 or 3 */
+    int32_t h_samp, v_samp;  /* luma sampling factors; chroma is 1x1 (1 and 1 for one component) */
+    int32_t mcus_x, mcus_y;  /* MCU columns and rows */
+    int32_t blocks_per_mcu;  /* h_samp * v_samp + 2, or 1 */
+    int32_t restart_interval;  /* MCUs per restart interval; 0: none */
+    int32_t n_intervals;     /* ceil(mcus_x * mcus_y / restart_interval), or 1 */
+    int64_t scan_offset;     /* the entropy-coded data: its first byte in the file */
+    int64_t scan_length;     /* its bytes, up to the 0xFF that starts EOI (restart markers and stuffing included) */
+    uint16_t quant[3][64];   /* per component, natural (row-major) order */
+    spg_jpeg_huff dc[3], ac[3];  /* per component */
+    const uint8_t *data;     /* device: the file's bytes (at least scan_offset + scan_length of them) */
+    uint8_t *out;            /* device: [height][width][3] uint8 BGR */
+    int32_t *decode_status;  /* device: set to SPG_JPEG_OK, SPG_JPEG_CORRUPT or SPG_JPEG_RANGE by the decode */
+} spg_jpeg_record;
+/* Host only (no device, no handle): parse `size` bytes at `data` into *record.  Every length and count is checked
+ * against the buffer; nothing outside it is read.  Returns SPG_OK with record->status saying whether the file can be
+ * decoded on the device, or SPG_E_INVALID for a NULL record, a negative size or NULL data with a positive size. */
+int spg_jpeg_parse(const uint8_t *data, int64_t size, spg_jpeg_record *record);
+/* Decode n files parsed with status SPG_JPEG_OK into their `out` images, every image of the call in each launch.  Each
+ * record's decode_status gets SPG_JPEG_OK, or SPG_JPEG_CORRUPT / SPG_JPEG_RANGE for an image whose data the device
+ * path cannot reproduce cv2 on: its `out` is then unspecified and the file is for cv2.  Records are validated before
+ * the first launch (SPG_E_INVALID names the first bad one).  Asynchronous on `stream`; `records` may be reused on
+ * return.  The handle's scratch (the unstuffed data, coefficients and planes) grows on demand, so calls on one handle
+ * must not run concurrently on different streams. */
+int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_t n, void *stream);
+
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
 int spg_nms_peaks(spg_handle *h, const float *heat_dev, int64_t image_stride, int64_t chan_stride,
@@ -554,7 +615,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation);
+ * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation, 9 JPEG decode);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 

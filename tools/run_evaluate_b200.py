@@ -2,7 +2,7 @@
 """Run the reference's ``evaluate.py`` UNCHANGED with its grouping stage on the H100 path.
 
     python tools/run_evaluate_b200.py --reference /path/to/Improved-Body-Parts [--config utils/config] [--check] [--batch N]
-                                      [--forward-batch M]
+                                      [--forward-batch M] [--device-decode]
     torchrun --nproc-per-node G tools/run_evaluate_b200.py --reference ... --batch N [--forward-batch M] --gpus G
 
 What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is never modified:
@@ -17,7 +17,9 @@ What it does (SURVEY.md §8b, INTEGRATION.md §1) -- the reference checkout is n
    replaces ``predict`` by the device one and ``predict_many`` (``:550-560``) by ``dropin.predict_many``, which groups
    N images per call; ``--forward-batch M`` (M > 1, with N > 1) also runs the network on up to M images of the same
    input size at once (``dropin.predict_batch``; with several scales or a rotation search in ``utils/config``, up to M
-   items: the images' scaled and rotated copies);
+   items: the images' scaled and rotated copies); ``--device-decode`` (with N > 1) also decodes each group of N JPEG
+   files on the GPU (``dropin.imread_many``) in place of ``cv2.imread`` (``:502``), and builds the network input on the
+   GPU as well (``device_input=True``), which the decoded images feed;
 4. fills the globals ``evaluate.__main__`` would set (``:643-646``): ``params, model_params`` from the reference's own
    ``utils/config`` through ``skeleton.read_reference_ini`` (``utils/config_reader.py:7`` hard-codes the author's path),
    ``show_eval_speed``;
@@ -96,13 +98,16 @@ def init_ranks() -> int:
 
 def prepare(reference_root: str, config_path: str = None, device: int = None, install: bool = True,
             replace_format_results: bool = False, batch: int = 1, forward_batch: int = 1, gpus: int = None,
-            device_cocoeval: bool = False):
+            device_cocoeval: bool = False, device_decode: bool = False):
     """Import the reference's ``evaluate`` module (unchanged) and put the H100 grouping path behind its call sites.
 
     ``gpus=G`` (under ``torchrun --nproc-per-node G``, with ``batch > 1``) joins the process group, pins this rank to
     its ``LOCAL_RANK`` device and installs the ``predict_many`` that shards the images over the G ranks; run
     ``validate`` on every rank.  ``device_cocoeval=True`` puts the GPU keypoint evaluation behind ``evaluate.COCOeval``
-    (and the minimal loader behind ``evaluate.COCO`` when pycocotools was stubbed)."""
+    (and the minimal loader behind ``evaluate.COCO`` when pycocotools was stubbed).  ``device_decode=True`` (with
+    ``batch > 1``) decodes ``predict_many``'s JPEG files on the GPU, with the device input stage."""
+    if device_decode and batch < 2:
+        raise ValueError("device_decode needs batch > 1: only the batched predict_many reads the image files")
     if gpus is not None:
         err = gpus_error(int(gpus), int(batch))
         if err:
@@ -137,6 +142,8 @@ def prepare(reference_root: str, config_path: str = None, device: int = None, in
             dropin.configure(device=device)
         if batch > 1:  # the batched grouping takes the maps the device predict() leaves on the GPU
             extra = dict(forward_batch=forward_batch) if forward_batch > 1 else {}
+            if device_decode:
+                extra.update(device_input=True, device_decode=True)
             dropin.install(evaluate, device_predict=True, batch=batch, **extra)
         else:
             dropin.install(evaluate)
@@ -182,6 +189,8 @@ def main() -> None:
                     help="images per network forward pass in predict_many (> 1 needs --batch > 1; default 1)")
     ap.add_argument("--device-cocoeval", action="store_true",
                     help="score validation() with the GPU COCOeval (and the minimal COCO loader without pycocotools)")
+    ap.add_argument("--device-decode", action="store_true",
+                    help="decode predict_many's JPEG files on the GPU, with the device input stage (needs --batch > 1)")
     ap.add_argument("--gpus", type=int, default=None,
                     help="under torchrun --nproc-per-node G: shard predict_many's images over the G GPUs (needs --batch > 1)")
     a = ap.parse_args()
@@ -191,6 +200,8 @@ def main() -> None:
         ap.error("--forward-batch must be >= 1")
     if a.forward_batch > 1 and a.batch < 2:
         ap.error("--forward-batch > 1 needs --batch > 1")
+    if a.device_decode and a.batch < 2:
+        ap.error("--device-decode needs --batch > 1")
     if a.gpus is not None:
         if a.gpus < 1:
             ap.error("--gpus must be >= 1")
@@ -200,7 +211,7 @@ def main() -> None:
         if err:
             ap.error(err)
     ev = prepare(a.reference, a.config, a.device, batch=a.batch, forward_batch=a.forward_batch, gpus=a.gpus,
-                 device_cocoeval=a.device_cocoeval)
+                 device_cocoeval=a.device_cocoeval, device_decode=a.device_decode)
     rank = f"rank {os.environ['RANK']}: " if a.gpus is not None else ""
     print(f"{rank}evaluate imported from {ev.__file__}; stubbed: {ev.__spg_stubbed__}; limbs: {len(ev.limbSeq)}; "
           f"find_peaks -> {ev.find_peaks.__module__}.{ev.find_peaks.__name__}")
