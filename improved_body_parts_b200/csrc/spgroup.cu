@@ -84,6 +84,7 @@ struct spg_handle {
     int fuse_ma = 1;      // whole-path calls run the fused match+assemble kernel (SPG_FUSE_MA=0: the two kernels back to back)
     int cand_dtype = SPG_F32;  // dtype of the planes the current candidates were scored on
     int stage = 0;  // 0 none, 1 peaks, 2 candidates, 3 connections, 4 people
+    bool frames_reserved = false;  // spg_reserve_frame was called: captured calls reset the scorer's queue
     std::string err;
 };
 
@@ -139,6 +140,27 @@ int grow(spg_handle *h, Scratch &s, size_t bytes) {
     SPG_CUDA(h, cudaMalloc(&s.p, bytes));
     s.bytes = bytes;
     return SPG_OK;
+}
+
+// whether `st` is capturing a CUDA graph
+int stream_capturing(spg_handle *h, cudaStream_t st, bool *capturing) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    SPG_CUDA(h, cudaStreamIsCapturing(st, &cs));
+    *capturing = cs == cudaStreamCaptureStatusActive;
+    return SPG_OK;
+}
+
+// grow() for a call on `st`: while `st` captures, an allocation would invalidate the capture, so a buffer below `bytes`
+// is SPG_E_CAPTURE instead (`what` names the buffer); the caller has enqueued nothing yet
+int grow_on(spg_handle *h, Scratch &s, size_t bytes, cudaStream_t st, const char *what) {
+    if (s.bytes >= bytes) return SPG_OK;
+    bool capturing = false;
+    int rc;
+    if ((rc = stream_capturing(h, st, &capturing))) return rc;
+    if (capturing)
+        return fail(h, SPG_E_CAPTURE, "%s need %zu B of scratch, %zu B are reserved, and the stream is capturing a graph: reserve "
+                    "the frame first (spg_reserve_frame)", what, bytes, s.bytes);
+    return grow(h, s, bytes);
 }
 
 // Every kernel launch on a handle goes through here: it raises the kernel's dynamic shared memory limit to `smem`,
@@ -448,6 +470,13 @@ int launch_score(spg_handle *h, const void *paf, int dtype, int64_t img_stride, 
         // The kernel leaves its queue at 0 for the next launch on the same stream.  spg_group_host's chunks run on the
         // handle's two streams and may overlap, so the second stream has a queue of its own.
         unsigned int *queue = h->score_queue + (st == h->streams[1] ? 2 : 0);
+        // On a handle prepared for capture (spg_reserve_frame), a captured call also zeroes it with a memset node, so
+        // that every replay of the graph starts from 0 whatever ran on the handle between replays.  Other handles never
+        // ask the stream.
+        bool capturing = false;
+        int rc;
+        if (h->frames_reserved && (rc = stream_capturing(h, st, &capturing))) return rc;
+        if (capturing) SPG_CUDA(h, cudaMemsetAsync(queue, 0, 2 * sizeof(unsigned int), st));
         return launch(h, kStageScore, k.persist_name, k.persist, std::min(grid, h->sm_count), kPersistThreads, pl.smem, st, a, grid,
                       queue);
     }
@@ -1042,7 +1071,8 @@ int spg_postnet_rotated(spg_handle *h, const spg_postnet_desc *d, const spg_post
     DeviceGuard guard(h->device);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (d->n_scales > 1 && (d->stride != 4 || d->n_scales > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
-        if ((rc = grow(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double)))) return rc;
+        if ((rc = grow_on(h, h->heat_acc, (size_t)h->cfg.max_batch * ws.K * H * W * sizeof(double), st, "the float64 keypoint sums")))
+            return rc;
     }
     for (int t = 0; t < d->n_scales; t++) {
         const spg_postnet_scale &sc = d->scales[t];
@@ -1149,7 +1179,7 @@ static int postnet_ragged(spg_handle *h, const spg_postnet_common *cm, const spg
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     double *acc = nullptr;
     if (n_items > 1 && (n_items > kPostMaxScales || any_rot)) {  // float64 keypoint sums that outlive a launch
-        if ((rc = grow(h, h->heat_acc, acc_total * sizeof(double)))) return rc;
+        if ((rc = grow_on(h, h->heat_acc, acc_total * sizeof(double), st, "the float64 keypoint sums"))) return rc;
         acc = static_cast<double *>(h->heat_acc.p);
     }
     for (int t0 = 0; t0 < n_items; t0 += per_group) {
@@ -1288,7 +1318,7 @@ int prenet_launch(spg_handle *h, const std::vector<PreMember> &ms, const std::ve
             grid_need = std::max(grid_need, bytes);
         }
     }
-    if ((rc = grow(h, h->pre_grid, grid_need))) return rc;
+    if ((rc = grow_on(h, h->pre_grid, grid_need, st, "the rotated items' padded images"))) return rc;
     PreRagged r{};
     for (int rot = 0; rot < 2; rot++) {
         for (const RaggedRange &g : groups[rot].ranges) {
@@ -1384,6 +1414,38 @@ int spg_prenet(spg_handle *h, const uint8_t *image, int64_t image_stride, int64_
     if (ms.empty()) return SPG_OK;
     DeviceGuard guard(h->device);
     return prenet_launch(h, ms, rotated, static_cast<cudaStream_t>(stream));
+}
+
+int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_downsample, const spg_prenet_item *items,
+                      int32_t n_items, int32_t stride, int32_t *moved) {
+    if (!h) return SPG_E_INVALID;
+    if (moved) *moved = 0;
+    int rc;
+    if ((rc = check_prenet_common(h, max_downsample, 0))) return rc;
+    if (n_items < 1 || !items) return fail(h, SPG_E_INVALID, "items is NULL or n_items %d below 1", n_items);
+    if (stride < 1 || stride > 16) return fail(h, SPG_E_INVALID, "stride outside [1,16]");
+    if ((rc = check_dims(h, 1, height, width))) return rc;
+    // spg_prenet's scratch grid: the padded images of the rotated items, which one launch holds at most
+    size_t grid = 0;
+    bool any_rot = false;
+    for (int t = 0; t < n_items; t++) {
+        const spg_prenet_item &it = items[t];
+        PreMember a;
+        float out;  // the geometry does not read the output
+        if ((rc = prenet_member(h, "item", t, height, width, max_downsample, 0, it.scale, it.rotate, it.reserved, it.matrix, &out, a)))
+            return rc;
+        if (it.rotate) grid += (size_t)a.Hp * a.Wp * 3;
+        any_rot = any_rot || it.rotate;
+    }
+    // spg_postnet_rotated's float64 keypoint sums, when they outlive a launch
+    size_t acc = 0;
+    if (n_items > 1 && (stride != 4 || n_items > kPostMaxScales || any_rot))
+        acc = (size_t)h->cfg.max_batch * h->ws.K * height * width * sizeof(double);
+    if (moved) *moved = grid > h->pre_grid.bytes || acc > h->heat_acc.bytes;  // set before a failed growth too
+    h->frames_reserved = true;
+    DeviceGuard guard(h->device);
+    if ((rc = grow(h, h->pre_grid, grid))) return rc;
+    return grow(h, h->heat_acc, acc);
 }
 
 // ---- training samples --------------------------------------------------------------------------

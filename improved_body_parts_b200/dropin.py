@@ -19,12 +19,13 @@ There is no CPU path: without the CUDA library / an sm_90 GPU these functions ra
 from __future__ import annotations
 
 import dataclasses
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import sharding, wire
-from .grouping import JPEG_OK, JPEG_RECORD, ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse
+from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse,
+                       prenet_item)
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -83,9 +84,10 @@ def configure(limbs: Optional[Sequence[Tuple[int, int]]] = None, device: Optiona
     _ragged.clear()
 
 
-def _new_grouper(max_batch: int) -> Grouper:
+def _new_grouper(max_batch: int, device: Optional[int] = None) -> Grouper:
     return Grouper(_limbs, NUM_PARTS, COCO_FROM_PART, max_batch=max_batch, max_h=MAX_DIM, max_w=MAX_DIM,
-                   max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS, device=_device)
+                   max_peaks_per_part=CAP_PEAKS, max_cands_per_limb=CAP_CANDS, max_person_rows=CAP_ROWS,
+                   device=_device if device is None else device)
 
 
 def _grouper() -> Grouper:
@@ -478,6 +480,237 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
     maps = g.postnet_ragged_items([(e, tuple(int(v) for v in img.shape[:2])) for e, img in zip(entries, images)],
                                   nan_scrub=_variant == "demo")
     return [(DeviceMaps(heat, False), DeviceMaps(paf, paf.dtype == torch.float32)) for heat, paf in maps]
+
+
+class FrameResult(NamedTuple):
+    """``FrameStream.result(ticket, detail=True)``: the people, the frame's wire record (``include/spgroup.h``; only the
+    header and the first ``n_persons`` rows are the frame's) and copies of its averaged maps."""
+    people: list
+    record: np.ndarray
+    heat: "DeviceMaps"
+    paf: "DeviceMaps"
+
+
+class _Frame:
+    """One slot's buffers for one frame shape and input kind, and the graph captured over them."""
+
+    def __init__(self, fs: "FrameStream", H: int, W: int, cuda_input: bool):
+        import itertools
+
+        import torch
+        dev = torch.device("cuda", fs.device)
+        mp, md = fs.model_params, int(fs.model_params["max_downsample"])
+        self.H, self.W, self.graph = H, W, None
+        self.multiplier = [x * mp["boxsize"] / H for x in fs.params["scale_search"]]
+        items = [prenet_item(H, W, m, a, md) for m, a in itertools.product(self.multiplier, fs.params["rotation_search"])]
+        self.scales = [scale for scale, _, _, _ in items]
+        self.crops = [geo[:2] for _, geo, _, _ in items]
+        self.reverses = [reverse for _, _, _, reverse in items]
+        self.pairs = [torch.empty((2, geo[2], geo[3], 3), dtype=torch.float32, device=dev) for _, geo, _, _ in items]
+        if fs.input_stage == "device":
+            self.image = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
+            self.host = None if cuda_input else torch.empty((H, W, 3), dtype=torch.uint8, pin_memory=True)
+        else:
+            self.host = [torch.empty(p.shape, dtype=torch.float32, pin_memory=True) for p in self.pairs]
+        self.as_f64 = len(items) == 1  # float32 storage of the float64 values for a single item, as predict() returns
+        self.heat = torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev)
+        self.paf = torch.empty((1, len(fs.limbs), H, W), dtype=torch.float32 if self.as_f64 else torch.float64, device=dev)
+        self.rec = torch.zeros(fs._g.wire_record_bytes(), dtype=torch.uint8, device=dev)
+        self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
+
+
+class FrameStream:
+    """Frames posed one at a time at the GPU's rate: ``predict`` + ``group`` per frame, replayed from a CUDA graph.
+
+    ``submit(frame)`` takes a ``[H, W, 3]`` uint8 BGR frame (numpy, or a CUDA tensor on the stream's device) and returns a
+    ticket; ``result(ticket)`` returns ``process()``'s value for that frame (evaluate.py:523-543), the
+    ``[([17 x (x, y)], score)]`` of ``predict_many``: equal, value for value and type for type, to ``keypoints`` of
+    ``group`` on the maps ``predict`` gives for the frame.
+
+    The first frame of a shape in a slot runs call by call -- it is the shape's warm-up (the network's lazy set-up,
+    cuDNN's choices) -- and the slot then captures one CUDA graph over its buffers for that shape: the upload from the
+    slot's pinned buffer (``input_stage="device"``: the uint8 frame, then ``spg_prenet`` for every item of
+    ``scale_search x rotation_search``; ``"host"``: the pairs cv2 built on the host), the forward pass of every item,
+    ``spg_postnet_rotated``, ``spg_group_batch`` writing the frame's wire record and the record's copy into the slot's
+    pinned host buffer.  Every later frame of that shape in that slot is one graph launch.  A CUDA frame is copied into
+    the slot's device image ahead of a graph of its own, which starts at ``spg_prenet``.  The graphs share one memory
+    pool: they replay one at a time on the stream's own CUDA stream, and nothing allocated inside a capture outlives it.
+
+    ``slots`` frames are in flight at most.  Each slot owns its inputs, maps and record until its frame is finished, so
+    the host stages frame k+1 while frame k's graph runs; a submit to a slot whose frame is unread finishes that frame
+    and keeps its result for ``result``.  A record with a capacity bit in its status (a crowded frame) is regrouped on
+    the capacity-free tier from the slot's maps, as ``group`` does; any other status bit raises ``GroupingError`` from
+    ``result``.  The variant (``configure(variant=...)``), the limb table and the default device are those in effect at
+    construction.  The network's output is ``model(x)[-1][0]``, as for ``predict``; the model must be capture-safe after
+    its first call at a shape (no host synchronisation, no host-to-device copy).  A stride other than 4 raises
+    ``ValueError``, a capture that fails raises ``GroupingError``: there is no call-by-call fallback."""
+
+    def __init__(self, model, params, model_params, *, slots: int = 2, input_stage: str = "device",
+                 device: Optional[int] = None):
+        if int(model_params["stride"]) != 4:
+            raise ValueError(f"FrameStream needs stride 4 (model_params['stride'] is {model_params['stride']}): the "
+                             "ragged and rotated post-network kernels it records are stride-4 kernels")
+        if int(slots) < 1:
+            raise ValueError("slots must be >= 1")
+        import torch
+        self.model, self.params, self.model_params = model, dict(params), dict(model_params)
+        self.input_stage = _stage(input_stage)
+        self.device = _device if device is None else int(device)
+        self.limbs = _limbs
+        self._gp = _group_params(params)
+        self._nan_scrub = _variant == "demo"
+        self._g = _new_grouper(1, self.device)     # the graphs' handle
+        self._tier = _new_grouper(1, self.device)  # the capacity-free tier's, used while later graphs run
+        self._stream = torch.cuda.Stream(device=self.device)
+        self._tier_stream = torch.cuda.Stream(device=self.device)
+        self._pool = None
+        self._frames: List[Dict[tuple, _Frame]] = [{} for _ in range(int(slots))]
+        self._busy: List[Optional[tuple]] = [None] * int(slots)  # per slot (ticket, frame, done event)
+        self._done: Dict[int, object] = {}  # finished tickets: (people, record) or the exception to raise
+        self._next = 0
+        self.captures = 0  # graphs captured so far (a frame shape's first sight in a slot, or after a buffer moved)
+
+    def close(self) -> None:
+        for frames in self._frames:
+            frames.clear()
+        self._g.close()
+        self._tier.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def submit(self, frame) -> int:
+        """Stage ``frame`` in the next slot and launch its graph (the shape's first frame in the slot: its calls, then the
+        capture).  Returns the frame's ticket."""
+        import torch
+        cuda = isinstance(frame, torch.Tensor) and frame.is_cuda
+        if cuda:
+            if self.input_stage == "host":
+                raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
+            if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or frame.device.index != self.device:
+                raise ValueError(f"a CUDA frame is a [H, W, 3] uint8 tensor on cuda:{self.device}")
+        else:
+            frame = np.ascontiguousarray(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
+            if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
+                raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
+        H, W = int(frame.shape[0]), int(frame.shape[1])
+        ticket = self._next
+        slot = ticket % len(self._frames)
+        if self._busy[slot] is not None:
+            self._finish(slot)
+        f = self._frames[slot].get((H, W, cuda))
+        if f is None:
+            f = self._frames[slot][(H, W, cuda)] = _Frame(self, H, W, cuda)
+            if self._g.reserve_frame(H, W, f.multiplier, self.params["rotation_search"],
+                                     max_downsample=int(self.model_params["max_downsample"])):
+                for frames in self._frames:  # a scratch buffer moved: the graphs recorded its old address
+                    for other in frames.values():
+                        other.graph = None
+        if cuda:
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(self._stream):
+                f.image.copy_(frame, non_blocking=True)
+            frame.record_stream(self._stream)
+        elif self.input_stage == "device":
+            f.host.numpy()[...] = frame
+        else:
+            for t, angle in enumerate(a for _ in f.multiplier for a in self.params["rotation_search"]):
+                _host_pair(frame, f.scales[t], angle, self.model_params, out=f.host[t].numpy())
+        eager = f.graph is None
+        with torch.cuda.stream(self._stream):
+            if eager:
+                self._path(f)
+            else:
+                f.graph.replay()
+            done = torch.cuda.Event()
+            done.record(self._stream)
+        if eager:
+            self._capture(f)
+        self._busy[slot] = (ticket, f, done)
+        self._next += 1
+        return ticket
+
+    def result(self, ticket: int, *, detail: bool = False):
+        """``process()``'s value for the frame of ``ticket`` (waits for it); each ticket is read once.  ``detail=True``
+        returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame to still
+        hold its slot: read it before ``slots`` later submits."""
+        frame = None
+        for slot, busy in enumerate(self._busy):
+            if busy is not None and busy[0] == ticket:
+                frame = busy[1]
+                self._finish(slot)
+                break
+        if ticket not in self._done:
+            raise ValueError(f"ticket {ticket} is not a submitted frame whose result is unread")
+        if detail and frame is None:
+            raise ValueError(f"ticket {ticket}: its slot holds a later frame; read detail=True before {len(self._busy)} "
+                             "later submits")
+        out = self._done.pop(ticket)
+        if isinstance(out, Exception):
+            raise out
+        people, record = out
+        if not detail:
+            return people
+        return FrameResult(people, record, DeviceMaps(frame.heat.clone(), False), DeviceMaps(frame.paf.clone(), frame.as_f64))
+
+    def _path(self, f: _Frame) -> None:
+        """One frame's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
+        import torch
+        md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
+        if self.input_stage == "device":
+            if f.host is not None:
+                f.image.copy_(f.host, non_blocking=True)
+            self._g.prenet(f.image, f.multiplier, self.params["rotation_search"], max_downsample=md, pad_value=pv,
+                           out=f.pairs)
+        else:
+            for pair, host in zip(f.pairs, f.host):
+                pair.copy_(host, non_blocking=True)
+        with torch.no_grad():
+            outs = [_network_output(self.model, pair)[None].contiguous() for pair in f.pairs]
+        self._g.postnet(outs, f.crops, (f.H, f.W), stride=4, nan_scrub=self._nan_scrub, rotations=f.reverses,
+                        heat_out=f.heat, paf_out=f.paf)
+        self._g.set_wire_output(f.rec.data_ptr())
+        try:
+            self._g.group_device(f.heat, f.paf, f.H, self._gp, paf_as_f64=f.as_f64)
+        finally:
+            self._g.set_wire_output(None)
+        f.rec_host.copy_(f.rec, non_blocking=True)
+
+    def _capture(self, f: _Frame) -> None:
+        import torch
+        graph = torch.cuda.CUDAGraph()
+        try:
+            with torch.cuda.graph(graph, pool=self._pool, stream=self._stream):
+                self._path(f)
+        except Exception as e:
+            raise GroupingError(f"capturing the path of a {f.H}x{f.W} frame failed (a model that synchronises with the "
+                                f"host or copies from it in its forward cannot be captured): {type(e).__name__}: {e}") from e
+        if self._pool is None:
+            self._pool = graph.pool()
+        f.graph = graph
+        self.captures += 1
+
+    def _finish(self, slot: int) -> None:
+        """Wait for the slot's frame and keep its result (or the error it raises) under its ticket; frees the slot."""
+        ticket, f, done = self._busy[slot]
+        self._busy[slot] = None
+        done.synchronize()
+        record = f.rec_host.numpy().copy()
+        rec = wire.as_records(record, self._g.J, self._g.capR)[0]
+        try:
+            if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
+                r = self._tier.group_unbounded(f.heat, f.paf, f.H, self._gp, paf_as_f64=f.as_f64, stream=self._tier_stream)
+                _check_status(r.status[0])
+                people = _people_of_result(r)
+            else:
+                _check_status(rec["status"])
+                people = wire.people_of(rec)
+            self._done[ticket] = (people, record)
+        except GroupingError as e:
+            self._done[ticket] = e
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:

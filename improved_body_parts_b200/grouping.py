@@ -33,6 +33,8 @@ ST_MEANING = {ST_SAMPLE_INDEX: "SAMPLE_INDEX: a line sample index outside the ma
               ST_NAN_PRIORITY: "NAN_PRIORITY: a NaN candidate priority among others (the reference's sort order at "
                                "evaluate.py:259 is undefined)"}
 F32, F64, F32_AS_F64, F16, BF16 = 0, 1, 2, 3, 4
+#: return code of a call that would have had to grow a scratch buffer while its stream captures a CUDA graph
+E_CAPTURE = -5
 
 
 class GroupingError(RuntimeError):
@@ -196,6 +198,7 @@ _PROTOTYPES = {
                                         _ptr]),
     "spg_prenet": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _P(_PrenetItem), _i32, _ptr]),
     "spg_prenet_ragged": (_int, [_ptr, _i32, _i32, _ptr, _i32, _ptr]),  # members: a PRENET_MEMBER array
+    "spg_reserve_frame": (_int, [_ptr, _i32, _i32, _i32, _P(_PrenetItem), _i32, _i32, _P(C.c_int32)]),
     # params: a TARGET_PARAMS record; samples: a TARGET_SAMPLE / TARGET_JOINTS array
     "spg_targets_warp": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
@@ -297,6 +300,11 @@ def prenet_item(h: int, w: int, scale: float, angle: float, max_downsample: int)
         centre = (geo[2] / 2, geo[3] / 2)
         forward, reverse = cv2.getRotationMatrix2D(centre, angle, 1), cv2.getRotationMatrix2D(centre, -angle, 1)
     return scale, geo, forward, reverse
+
+
+def _matrix6(m) -> C.Array:
+    """A 2x3 matrix (``None``: zeros) as the ``double[6]`` of a C record."""
+    return (C.c_double * 6)(*(np.asarray(m, np.float64).reshape(6).tolist() if m is not None else [0.0] * 6))
 
 
 def _vp(a: Optional[np.ndarray]):
@@ -878,8 +886,7 @@ class Grouper:
             scale, (H1, W1, Hp, Wp), forward, reverse = prenet_item(h, w, scale, angle, md)
             o = self._prenet_out(None if out is None else out[t] if batched else out[t][None], (N, 2, Hp, Wp, 3),
                                  f"out[{t}]", f"[N,2,{Hp},{Wp},3] CUDA tensor with contiguous images")
-            m = (C.c_double * 6)(*(np.asarray(forward, np.float64).reshape(6).tolist() if forward is not None else [0.0] * 6))
-            items[t] = _PrenetItem(scale, int(forward is not None), 0, m, o.data_ptr(), o.stride(0))
+            items[t] = _PrenetItem(scale, int(forward is not None), 0, _matrix6(forward), o.data_ptr(), o.stride(0))
             results.append((o if batched else o[0], (H1, W1), reverse))
         rc = self._lib.spg_prenet(self._h, img.data_ptr(), img.stride(0), img.stride(1), N, h, w, md, pv, items, len(pairs),
                                   self._stream_ptr(stream))
@@ -920,6 +927,23 @@ class Grouper:
         rc = self._lib.spg_prenet_ragged(self._h, md, pv, arr.ctypes.data, len(members), self._stream_ptr(stream))
         _check(rc, "spg_prenet_ragged", self._h)
         return results
+
+    def reserve_frame(self, height: int, width: int, scales, angles, *, max_downsample: int, stride: int = 4) -> bool:
+        """``spg_reserve_frame``: grow, outside any capture, every scratch buffer that one ``height x width`` frame needs
+        through ``prenet(image, scales, angles, max_downsample=...)`` and ``postnet`` at ``stride``, so that those calls
+        can be recorded into a CUDA graph.  Returns whether a buffer moved: graphs captured earlier from this handle's
+        calls then hold its old address and must be captured again."""
+        import itertools
+        md = int(max_downsample)
+        pairs = list(itertools.product(scales, angles))
+        items = (_PrenetItem * max(len(pairs), 1))()
+        for t, (scale, angle) in enumerate(pairs):
+            scale, _, forward, _ = prenet_item(int(height), int(width), scale, angle, md)
+            items[t] = _PrenetItem(scale, int(forward is not None), 0, _matrix6(forward), None, 0)
+        moved = C.c_int32(0)
+        _check(self._lib.spg_reserve_frame(self._h, int(height), int(width), md, items, len(pairs), int(stride), C.byref(moved)),
+               "spg_reserve_frame", self._h)
+        return bool(moved.value)
 
     def _prenet_out(self, o, shape, name, form):
         """A pre-network output of ``shape`` on the handle's device: ``o`` checked (the leading pair contiguous), or a new

@@ -36,7 +36,9 @@ enum {
     SPG_E_INVALID = -1,   /* bad argument (shape, capacity, alignment, null pointer) */
     SPG_E_CUDA = -2,      /* a CUDA runtime call failed; see spg_last_error          */
     SPG_E_NO_DEVICE = -3, /* no CUDA device / not an sm_90 part                      */
-    SPG_E_STATE = -4      /* stage called before the stage that feeds it             */
+    SPG_E_STATE = -4,     /* stage called before the stage that feeds it             */
+    SPG_E_CAPTURE = -5    /* the call would have to grow a scratch buffer while its stream is capturing a */
+                          /* CUDA graph: reserve it first (spg_reserve_frame); nothing was enqueued      */
 };
 
 /* per-image status bits (spg_download_status) */
@@ -304,6 +306,24 @@ typedef struct spg_prenet_member {
  * hundred members). */
 int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, const spg_prenet_member *members,
                       int32_t n_members, void *stream);
+
+/* ---- frames recorded into a CUDA graph ---------------------------------------------------------------------------
+ * spg_prenet, spg_postnet / spg_postnet_rotated and spg_group_batch (with or without spg_set_wire_output) can be
+ * recorded on a stream that is capturing a CUDA graph: they neither synchronise nor read device data back, and every
+ * choice they make (kernel, tiling, shared memory) depends on their arguments alone.  A call made while its stream
+ * captures never allocates: if it would have to grow one of the handle's scratch buffers it returns SPG_E_CAPTURE before
+ * enqueueing anything, and the capture, the stream and the handle stay usable.  The persistent limb scorer's item queue
+ * is zeroed by a memset node ahead of its kernel in a captured call on a handle that spg_reserve_frame prepared, so
+ * every replay starts from the same state.
+ *
+ * spg_reserve_frame grows, outside any capture, every scratch buffer one frame needs: an image of height x width
+ * through spg_prenet with `items` (their scale, rotate, reserved and matrix fields; out is not read) and
+ * max_downsample, then through spg_postnet_rotated with one scale per item at `stride` and a rotation wherever the item
+ * has rotate = 1.  The handle's max_batch sizes the post-network sums as spg_postnet_rotated does.  *moved (may be NULL)
+ * is set to 1 when a buffer had to be reallocated, which invalidates graphs captured earlier from this handle's calls
+ * (they hold the old address), else to 0.  Synchronous; must not be called while any stream of the device captures. */
+int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_downsample, const spg_prenet_item *items,
+                      int32_t n_items, int32_t stride, int32_t *moved);
 
 /* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
