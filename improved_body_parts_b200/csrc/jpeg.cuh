@@ -32,9 +32,13 @@
 // and C IDCTs agree sets SPG_JPEG_RANGE (DESIGN.md §4).  The launches are ragged like prenet.cuh: the member table travels
 // as a __grid_constant__ parameter and a CTA finds its image by binary search over first_cta (ragged_member).
 //
-// The kernels are compiled in their own translation unit, jpeg.cu, which spgroup.cu calls through jpeg_launch: in
-// spgroup.cu's module their presence changed how nvcc optimised match_assemble_kernel, and in their own every kernel that
-// existed before them keeps its SASS.  This header is what the two share.
+// The frame form (spg_jpeg_decode_frame: one frame, recorded into a CUDA graph and replayed for every frame of one format)
+// runs the same count to write kernels with grids sized for a capacity in scan bytes; they read the frame's segment
+// address and length from its device record at run time, and the CTAs past the frame's work return (jpeg_kernels.cuh).
+//
+// The kernels are compiled in translation units of their own, jpeg.cu and jpeg_frame.cu, which spgroup.cu calls through
+// jpeg_launch: in spgroup.cu's module their presence changed how nvcc optimised match_assemble_kernel, and in their own
+// every kernel that existed before them keeps its SASS.  This header is what they share.
 #pragma once
 
 #include "../../include/spgroup.h"
@@ -58,7 +62,7 @@ struct JpegSub {
     int entry_pos, entry_uk, exit_pos, exit_uk, n, base;
 };
 
-// One image of a call.
+// One image of a call (of spg_jpeg_decode_frame: seg is unused, seg_len, n_chunks and n_subs are the capacity's).
 struct JpegMember {
     const spg_jpeg_record *rec;     // device copy of the record (tables)
     const unsigned char *seg;       // the entropy-coded segment
@@ -84,12 +88,20 @@ struct JpegRagged {
     JpegMember img[kJpegTableMax];  // first_cta increasing
 };
 
-// The decoder's kernels, in launch order, and their block sizes.
-enum JpegKernel : int { kJpegCount, kJpegPrefix, kJpegPack, kJpegInterval, kJpegSync, kJpegFixup, kJpegWrite, kJpegDc, kJpegIdct, kJpegColor, kJpegKernels };
+// The decoder's kernels, in launch order, and their block sizes; then the frame form's count to write kernels, which read
+// the segment's address and length from the device record (spg_jpeg_decode_frame; the DC, IDCT and colour kernels are
+// the ragged ones).
+enum JpegKernel : int { kJpegCount, kJpegPrefix, kJpegPack, kJpegInterval, kJpegSync, kJpegFixup, kJpegWrite, kJpegDc, kJpegIdct, kJpegColor,
+                        kJpegCountFrame, kJpegPrefixFrame, kJpegPackFrame, kJpegIntervalFrame, kJpegSyncFrame, kJpegFixupFrame,
+                        kJpegWriteFrame, kJpegKernels };
 constexpr int kJpegBlock[kJpegKernels] = {kJpegPackThreads, kJpegPackThreads, kJpegPackThreads, kJpegThreads, kJpegSubThreads, kJpegThreads,
-                                          kJpegSubThreads, kJpegThreads, kJpegThreads, kJpegThreads};
+                                          kJpegSubThreads, kJpegThreads, kJpegThreads, kJpegThreads,
+                                          kJpegPackThreads, kJpegPackThreads, kJpegPackThreads, kJpegThreads, kJpegSubThreads, kJpegThreads,
+                                          kJpegSubThreads};
 extern const char *const kJpegKernelName[kJpegKernels];
-// one launch of kernel k over `grid` CTAs with member table r on stream st (jpeg.cu); returns cudaGetLastError()
+// one launch of kernel k over `grid` CTAs with member table r on stream st (jpeg.cu; the frame form's kernels through
+// jpeg_frame_launch, jpeg_frame.cu); returns cudaGetLastError()
 cudaError_t jpeg_launch(JpegKernel k, unsigned grid, cudaStream_t st, const JpegRagged &r);
+cudaError_t jpeg_frame_launch(JpegKernel k, unsigned grid, cudaStream_t st, const JpegRagged &r);
 
 }  // namespace spg

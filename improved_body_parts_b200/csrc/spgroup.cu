@@ -2158,12 +2158,13 @@ struct Carver {
     }
 };
 
+// `what` given: a call on `st`, which grows nothing while `st` captures (grow_on)
 template <typename F>
-int carve(spg_handle *h, Scratch &s, F &&layout) {
+int carve(spg_handle *h, Scratch &s, F &&layout, cudaStream_t st = nullptr, const char *what = nullptr) {
     Carver m;
     layout(m);
     int rc;
-    if ((rc = grow(h, s, m.bytes))) return rc;
+    if ((rc = what ? grow_on(h, s, m.bytes, st, what) : grow(h, s, m.bytes))) return rc;
     Carver c;
     c.base = static_cast<unsigned char *>(s.p);
     layout(c);
@@ -2631,6 +2632,79 @@ void jpeg_parse(const uint8_t *d, long long n, spg_jpeg_record *r) {
 // the largest entropy-coded segment a decode takes: bit positions are int
 constexpr long long kJpegMaxSegment = (1ll << 28) - 1;
 
+// A record's checks before any launch: the fields the kernels size their work by (`what` names it in the message).
+int jpeg_check(spg_handle *h, const spg_jpeg_record &r, const char *what) {
+    if (r.status != SPG_JPEG_OK) return fail(h, SPG_E_INVALID, "%s: status %d is not SPG_JPEG_OK", what, r.status);
+    if (!r.data || !r.out || !r.decode_status) return fail(h, SPG_E_INVALID, "%s: data, out or decode_status is NULL", what);
+    const bool grey = r.n_components == 1;
+    if (!(grey || r.n_components == 3) || r.h_samp < 1 || r.h_samp > 2 || r.v_samp < 1 || r.v_samp > 2 ||
+        (grey && (r.h_samp != 1 || r.v_samp != 1)) || r.blocks_per_mcu != r.h_samp * r.v_samp + (grey ? 0 : 2))
+        return fail(h, SPG_E_INVALID, "%s: components or sampling", what);
+    if (r.frame_height < 1 || r.frame_width < 1 || r.orientation < 1 || r.orientation > 8 ||
+        r.mcus_x != (r.frame_width + 8 * r.h_samp - 1) / (8 * r.h_samp) ||
+        r.mcus_y != (r.frame_height + 8 * r.v_samp - 1) / (8 * r.v_samp) ||
+        r.height != (r.orientation >= 5 ? r.frame_width : r.frame_height) ||
+        r.width != (r.orientation >= 5 ? r.frame_height : r.frame_width))
+        return fail(h, SPG_E_INVALID, "%s: geometry", what);
+    const long long mcus = (long long)r.mcus_x * r.mcus_y;
+    if (r.restart_interval < 0 || r.n_intervals != (r.restart_interval ? (mcus + r.restart_interval - 1) / r.restart_interval : 1))
+        return fail(h, SPG_E_INVALID, "%s: restart interval", what);
+    if (r.scan_offset < 0 || r.scan_length < 0 || r.scan_length > kJpegMaxSegment)
+        return fail(h, SPG_E_INVALID, "%s: scan length %lld outside [0, 2^28)", what, (long long)r.scan_length);
+    if (mcus * r.blocks_per_mcu > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "%s: more than 2^31 - 1 blocks", what);
+    return SPG_OK;
+}
+
+// One image's member and its arrays in the decode's scratch, for `scan_bytes` of entropy-coded data: its chunk counts,
+// interval starts, subsequence states, unstuffed stream and component planes (rec and coef are the caller's).
+JpegMember jpeg_member(Carver &c, const spg_jpeg_record &r, long long scan_bytes) {
+    JpegMember m{};
+    m.seg = r.data + r.scan_offset;
+    m.seg_len = (int)scan_bytes;
+    m.n_chunks = (int)std::max<long long>(1, (scan_bytes + kJpegChunk - 1) / kJpegChunk);
+    m.chunk_counts = c.take<int>(2 * (size_t)m.n_chunks);
+    m.starts = c.take<int>((size_t)r.n_intervals + 1);
+    m.n_subs = r.restart_interval ? 0 : (int)std::max<long long>(1, (8 * scan_bytes + kJpegSubBits - 1) / kJpegSubBits);
+    m.subs = c.take<JpegSub>((size_t)m.n_subs);
+    m.packed = c.take<unsigned char>((size_t)scan_bytes);
+    m.frame_h = r.frame_height;
+    m.frame_w = r.frame_width;
+    m.out_h = r.height;
+    m.out_w = r.width;
+    m.orientation = r.orientation;
+    m.n_comp = r.n_components;
+    m.hs = r.h_samp;
+    m.vs = r.v_samp;
+    m.mcus_x = r.mcus_x;
+    m.mcus_y = r.mcus_y;
+    m.bpm = r.blocks_per_mcu;
+    m.restart = r.restart_interval;
+    m.n_intervals = r.n_intervals;
+    m.total_blocks = r.mcus_x * r.mcus_y * r.blocks_per_mcu;
+    m.out = r.out;
+    m.status = r.decode_status;
+    for (int k = 0; k < r.n_components; k++) {
+        const int hk = k == 0 ? r.h_samp : 1, vk = k == 0 ? r.v_samp : 1;
+        m.plane_w[k] = r.mcus_x * hk * 8;
+        m.plane[k] = c.take<unsigned char>((size_t)m.plane_w[k] * r.mcus_y * vk * 8);
+    }
+    return m;
+}
+
+// spg_jpeg_reserve_frame / spg_jpeg_decode_frame's arguments
+int jpeg_check_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes) {
+    if (!format) return fail(h, SPG_E_INVALID, "format is NULL");
+    if (max_scan_bytes < 1 || max_scan_bytes > kJpegMaxSegment)
+        return fail(h, SPG_E_INVALID, "max_scan_bytes %lld outside [1, 2^28)", (long long)max_scan_bytes);
+    return jpeg_check(h, *format, "format");
+}
+
+// the frame form's scratch: the member for max_scan_bytes, then its coefficients
+void jpeg_frame_layout(Carver &c, const spg_jpeg_record &format, int64_t max_scan_bytes, JpegMember &m) {
+    m = jpeg_member(c, format, max_scan_bytes);
+    m.coef = c.take<short>((size_t)m.total_blocks * 64);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2654,25 +2728,10 @@ int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_
     if (n == 0) return SPG_OK;
     // every record validated before the first launch: the fields the kernels size their work by
     for (int i = 0; i < n; i++) {
-        const spg_jpeg_record &r = records[i];
-        if (r.status != SPG_JPEG_OK) return fail(h, SPG_E_INVALID, "record %d: status %d is not SPG_JPEG_OK", i, r.status);
-        if (!r.data || !r.out || !r.decode_status) return fail(h, SPG_E_INVALID, "record %d: data, out or decode_status is NULL", i);
-        const bool grey = r.n_components == 1;
-        if (!(grey || r.n_components == 3) || r.h_samp < 1 || r.h_samp > 2 || r.v_samp < 1 || r.v_samp > 2 ||
-            (grey && (r.h_samp != 1 || r.v_samp != 1)) || r.blocks_per_mcu != r.h_samp * r.v_samp + (grey ? 0 : 2))
-            return fail(h, SPG_E_INVALID, "record %d: components or sampling", i);
-        if (r.frame_height < 1 || r.frame_width < 1 || r.orientation < 1 || r.orientation > 8 ||
-            r.mcus_x != (r.frame_width + 8 * r.h_samp - 1) / (8 * r.h_samp) ||
-            r.mcus_y != (r.frame_height + 8 * r.v_samp - 1) / (8 * r.v_samp) ||
-            r.height != (r.orientation >= 5 ? r.frame_width : r.frame_height) ||
-            r.width != (r.orientation >= 5 ? r.frame_height : r.frame_width))
-            return fail(h, SPG_E_INVALID, "record %d: geometry", i);
-        const long long mcus = (long long)r.mcus_x * r.mcus_y;
-        if (r.restart_interval < 0 || r.n_intervals != (r.restart_interval ? (mcus + r.restart_interval - 1) / r.restart_interval : 1))
-            return fail(h, SPG_E_INVALID, "record %d: restart interval", i);
-        if (r.scan_offset < 0 || r.scan_length < 0 || r.scan_length > kJpegMaxSegment)
-            return fail(h, SPG_E_INVALID, "record %d: scan length %lld outside [0, 2^28)", i, (long long)r.scan_length);
-        if (mcus * r.blocks_per_mcu > 0x7fffffffLL) return fail(h, SPG_E_INVALID, "record %d: more than 2^31 - 1 blocks", i);
+        char what[32];
+        snprintf(what, sizeof what, "record %d", i);
+        int rc;
+        if ((rc = jpeg_check(h, records[i], what))) return rc;
     }
     DeviceGuard guard(h->device);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2685,40 +2744,9 @@ int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_
         recs = c.take<spg_jpeg_record>((size_t)n);
         coef_count = 0;
         for (int i = 0; i < n; i++) {
-            const spg_jpeg_record &r = records[i];
-            JpegMember &m = ms[i];
-            m = JpegMember{};
-            m.rec = recs + i;
-            m.seg = r.data + r.scan_offset;
-            m.seg_len = (int)r.scan_length;
-            m.n_chunks = (int)std::max<long long>(1, (r.scan_length + kJpegChunk - 1) / kJpegChunk);
-            m.chunk_counts = c.take<int>(2 * (size_t)m.n_chunks);
-            m.starts = c.take<int>((size_t)r.n_intervals + 1);
-            m.n_subs = r.restart_interval ? 0 : (int)std::max<long long>(1, (8 * r.scan_length + kJpegSubBits - 1) / kJpegSubBits);
-            m.subs = c.take<JpegSub>((size_t)m.n_subs);
-            m.packed = c.take<unsigned char>((size_t)r.scan_length);
-            m.frame_h = r.frame_height;
-            m.frame_w = r.frame_width;
-            m.out_h = r.height;
-            m.out_w = r.width;
-            m.orientation = r.orientation;
-            m.n_comp = r.n_components;
-            m.hs = r.h_samp;
-            m.vs = r.v_samp;
-            m.mcus_x = r.mcus_x;
-            m.mcus_y = r.mcus_y;
-            m.bpm = r.blocks_per_mcu;
-            m.restart = r.restart_interval;
-            m.n_intervals = r.n_intervals;
-            m.total_blocks = r.mcus_x * r.mcus_y * r.blocks_per_mcu;
-            m.out = r.out;
-            m.status = r.decode_status;
-            for (int k = 0; k < r.n_components; k++) {
-                const int hk = k == 0 ? r.h_samp : 1, vk = k == 0 ? r.v_samp : 1;
-                m.plane_w[k] = r.mcus_x * hk * 8;
-                m.plane[k] = c.take<unsigned char>((size_t)m.plane_w[k] * r.mcus_y * vk * 8);
-            }
-            coef_count += (size_t)m.total_blocks * 64;
+            ms[i] = jpeg_member(c, records[i], records[i].scan_length);
+            ms[i].rec = recs + i;
+            coef_count += (size_t)ms[i].total_blocks * 64;
         }
         coef_base = c.take<short>(coef_count);
         size_t o = 0;
@@ -2770,6 +2798,55 @@ int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_
         (rc = run(kJpegIdct, [](const JpegMember &m) { return ((long long)m.total_blocks + kJpegThreads - 1) / kJpegThreads; }, all)) ||
         (rc = run(kJpegColor, [](const JpegMember &m) { return ((long long)m.out_h * m.out_w + kJpegThreads - 1) / kJpegThreads; }, all)))
         return rc;
+    return SPG_OK;
+}
+
+int spg_jpeg_reserve_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes, int32_t *moved) {
+    if (!h) return SPG_E_INVALID;
+    if (moved) *moved = 0;
+    int rc;
+    if ((rc = jpeg_check_frame(h, format, max_scan_bytes))) return rc;
+    Carver c;
+    JpegMember m;
+    jpeg_frame_layout(c, *format, max_scan_bytes, m);
+    if (moved) *moved = c.bytes > h->jpeg.bytes;  // set before a failed growth too
+    DeviceGuard guard(h->device);
+    return grow(h, h->jpeg, c.bytes);
+}
+
+int spg_jpeg_decode_frame(spg_handle *h, const spg_jpeg_record *device_record, const spg_jpeg_record *format,
+                          int64_t max_scan_bytes, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    int rc;
+    if ((rc = jpeg_check_frame(h, format, max_scan_bytes))) return rc;
+    if (!device_record) return fail(h, SPG_E_INVALID, "device_record is NULL");
+    DeviceGuard guard(h->device);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    JpegRagged table{};
+    table.n = 1;
+    JpegMember &m = table.img[0];
+    if ((rc = carve(h, h->jpeg, [&](Carver &c) { jpeg_frame_layout(c, *format, max_scan_bytes, m); }, st,
+                    "the JPEG frame decode's unstuffed stream, coefficients and planes")))
+        return rc;
+    m.rec = device_record;
+    m.first_cta = 0;
+    SPG_CUDA(h, cudaMemsetAsync(m.coef, 0, (size_t)m.total_blocks * 64 * sizeof(short), st));
+    // the grids cover the capacity (the member's seg_len, n_chunks and n_subs); the kernels read the frame's own length
+    const long long subs = ((long long)m.n_subs + kJpegSubThreads - 1) / kJpegSubThreads;
+    std::vector<std::pair<JpegKernel, long long>> runs = {{kJpegCountFrame, m.n_chunks}, {kJpegPrefixFrame, 1}, {kJpegPackFrame, m.n_chunks}};
+    if (m.restart)
+        runs.push_back({kJpegIntervalFrame, ((long long)m.n_intervals + kJpegThreads - 1) / kJpegThreads});
+    else
+        runs.insert(runs.end(), {{kJpegSyncFrame, subs}, {kJpegFixupFrame, 1}, {kJpegWriteFrame, subs}});
+    runs.insert(runs.end(), {{kJpegDc, m.n_comp},
+                             {kJpegIdct, ((long long)m.total_blocks + kJpegThreads - 1) / kJpegThreads},
+                             {kJpegColor, ((long long)m.out_h * m.out_w + kJpegThreads - 1) / kJpegThreads}});
+    for (const auto &[k, ctas] : runs) {
+        const cudaError_t e = jpeg_launch(k, (unsigned)ctas, st, table);
+        h->stage_kernel[kStageJpeg] = kJpegKernelName[k];
+        h->launches++;
+        if (e != cudaSuccess) return fail(h, SPG_E_CUDA, "%s launch failed: %s", kJpegKernelName[k], cudaGetErrorString(e));
+    }
     return SPG_OK;
 }
 

@@ -484,11 +484,26 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
 
 class FrameResult(NamedTuple):
     """``FrameStream.result(ticket, detail=True)``: the people, the frame's wire record (``include/spgroup.h``; only the
-    header and the first ``n_persons`` rows are the frame's) and copies of its averaged maps."""
+    header and the first ``n_persons`` rows are the frame's), copies of its averaged maps and, for a frame submitted as
+    JPEG bytes, the ``[H, W, 3]`` uint8 BGR image it was decoded to (on the device or by ``cv2.imdecode``), else None."""
     people: list
     record: np.ndarray
     heat: "DeviceMaps"
     paf: "DeviceMaps"
+    image: Optional[np.ndarray] = None
+
+
+#: the fields of a parsed JPEG that a frame graph's launches depend on: the format a graph serves
+JPEG_FORMAT = ("frame_height", "frame_width", "n_components", "h_samp", "v_samp", "restart_interval", "orientation")
+
+
+def _imdecode(data: np.ndarray) -> np.ndarray:
+    """``cv2.imdecode(data, IMREAD_COLOR)``; ``ValueError`` for bytes cv2 cannot decode either."""
+    import cv2
+    img = cv2.imdecode(data, cv2.IMREAD_COLOR)
+    if img is None:
+        raise ValueError("the frame's bytes are not an image cv2.imdecode can decode")
+    return img
 
 
 class _Frame:
@@ -517,6 +532,26 @@ class _Frame:
         self.paf = torch.empty((1, len(fs.limbs), H, W), dtype=torch.float32 if self.as_f64 else torch.float64, device=dev)
         self.rec = torch.zeros(fs._g.wire_record_bytes(), dtype=torch.uint8, device=dev)
         self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
+        self.format = None  # JPEG frames: the format's JPEG_RECORD (set_capacity)
+
+    def set_capacity(self, rec, capacity: int) -> None:
+        """Make this a JPEG frame's slot of ``capacity`` bytes for the format of ``rec``: the frame's bytes and parsed
+        record go up from pinned buffers, and ``spg_jpeg_decode_frame`` decodes them into ``image``."""
+        import torch
+        dev = self.image.device
+        if self.format is None:
+            self.record_host = torch.empty(JPEG_RECORD.itemsize, dtype=torch.uint8, pin_memory=True)
+            self.record = torch.empty(JPEG_RECORD.itemsize, dtype=torch.uint8, device=dev)
+            self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.status_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+            self.format = np.zeros(1, JPEG_RECORD)
+            self.format[0] = rec
+        self.capacity, self.nbytes = int(capacity), 0
+        self.bytes_host = torch.empty(self.capacity, dtype=torch.uint8, pin_memory=True)
+        self.bytes = torch.empty(self.capacity, dtype=torch.uint8, device=dev)
+        f = self.format
+        f["data"], f["out"], f["decode_status"] = self.bytes.data_ptr(), self.image.data_ptr(), self.status.data_ptr()
+        self.graph = None
 
 
 class FrameStream:
@@ -535,6 +570,21 @@ class FrameStream:
     pinned host buffer.  Every later frame of that shape in that slot is one graph launch.  A CUDA frame is copied into
     the slot's device image ahead of a graph of its own, which starts at ``spg_prenet``.  The graphs share one memory
     pool: they replay one at a time on the stream's own CUDA stream, and nothing allocated inside a capture outlives it.
+
+    ``submit`` also takes a JPEG file's bytes (``bytes``, ``bytearray`` or ``memoryview``), parsed on the host with
+    ``spg_jpeg_parse``.  A file the device decoder takes (baseline or extended-sequential Huffman, grey or YCbCr 4:4:4 /
+    4:2:2 / 4:4:0 / 4:2:0) is staged with its parsed record in the slot's pinned buffers, and the slot's graph for its
+    format -- frame height and width, component count, luma sampling, restart interval and EXIF orientation -- starts
+    with their copies and ``spg_jpeg_decode_frame`` into the slot's device image, bit-identical to ``cv2.imdecode``;
+    the scan's offset and length, the tables and the segments in front of the scan are read on the device from the
+    frame's record, so they may change from frame to frame.  A slot reserves a capacity in bytes per format (the next
+    power of two of the file's size, at least 64 KiB); a longer file grows it, which captures that graph again.  A file
+    the parser refuses (progressive, arithmetic-coded, other samplings and so on) is decoded with ``cv2.imdecode`` at
+    submit and posed as a decoded frame; one the device decoder flags (corrupt data, or blocks outside the range where
+    libjpeg-turbo's IDCTs agree) is posed again from the slot's bytes the same way when its result is read, so a JPEG
+    frame's result is always the one for ``cv2.imdecode(bytes, IMREAD_COLOR)``.  ``host_decodes`` counts the JPEG frames
+    ``cv2.imdecode`` decoded; with ``input_stage="host"`` that is every JPEG frame, decoded at submit.  Bytes cv2 cannot
+    decode either raise ``ValueError``.
 
     ``slots`` frames are in flight at most.  Each slot owns its inputs, maps and record until its frame is finished, so
     the host stages frame k+1 while frame k's graph runs; a submit to a slot whose frame is unread finishes that frame
@@ -569,6 +619,7 @@ class FrameStream:
         self._done: Dict[int, object] = {}  # finished tickets: (people, record) or the exception to raise
         self._next = 0
         self.captures = 0  # graphs captured so far (a frame shape's first sight in a slot, or after a buffer moved)
+        self.host_decodes = 0  # JPEG frames decoded with cv2.imdecode
 
     def close(self) -> None:
         for frames in self._frames:
@@ -584,32 +635,64 @@ class FrameStream:
 
     def submit(self, frame) -> int:
         """Stage ``frame`` in the next slot and launch its graph (the shape's first frame in the slot: its calls, then the
-        capture).  Returns the frame's ticket."""
+        capture).  ``frame`` is a ``[H, W, 3]`` uint8 BGR image (numpy, or a CUDA tensor on the stream's device) or a
+        JPEG file's bytes.  Returns the frame's ticket."""
         import torch
+        decoded = rec = None
+        if isinstance(frame, (bytes, bytearray, memoryview)):
+            data = np.frombuffer(frame, np.uint8)
+            if data.size == 0:
+                raise ValueError("a JPEG frame's bytes are empty")
+            rec = jpeg_parse(data) if self.input_stage == "device" else None
+            if rec is None or rec["status"] != JPEG_OK:
+                frame = decoded = _imdecode(data)
+                self.host_decodes += 1
+                rec = None
         cuda = isinstance(frame, torch.Tensor) and frame.is_cuda
         if cuda:
             if self.input_stage == "host":
                 raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
             if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or frame.device.index != self.device:
                 raise ValueError(f"a CUDA frame is a [H, W, 3] uint8 tensor on cuda:{self.device}")
-        else:
+        elif rec is None:
             frame = np.ascontiguousarray(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
             if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
                 raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
-        H, W = int(frame.shape[0]), int(frame.shape[1])
         ticket = self._next
         slot = ticket % len(self._frames)
         if self._busy[slot] is not None:
             self._finish(slot)
-        f = self._frames[slot].get((H, W, cuda))
+        f, done = self._launch(slot, frame if rec is None else data, rec)
+        self._busy[slot] = (ticket, f, done, decoded)
+        self._next += 1
+        return ticket
+
+    def _launch(self, slot: int, frame, rec=None):
+        """Stage ``frame`` (an image, or JPEG bytes parsed into ``rec``) in ``slot`` and run its graph, or its calls and
+        then the capture; returns the slot's frame and the event of the launch's end."""
+        import torch
+        cuda = rec is None and isinstance(frame, torch.Tensor)
+        if rec is None:
+            H, W, kind = int(frame.shape[0]), int(frame.shape[1]), cuda
+        else:  # a graph per format: it starts with the decode into the slot's device image
+            H, W, kind = int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)
+        f = self._frames[slot].get((H, W, kind))
         if f is None:
-            f = self._frames[slot][(H, W, cuda)] = _Frame(self, H, W, cuda)
+            f = self._frames[slot][(H, W, kind)] = _Frame(self, H, W, cuda or rec is not None)
             if self._g.reserve_frame(H, W, f.multiplier, self.params["rotation_search"],
                                      max_downsample=int(self.model_params["max_downsample"])):
-                for frames in self._frames:  # a scratch buffer moved: the graphs recorded its old address
-                    for other in frames.values():
-                        other.graph = None
-        if cuda:
+                self._invalidate()
+        if rec is not None:
+            if f.format is None or frame.size > f.capacity:
+                f.set_capacity(rec, max(1 << 16, 1 << (frame.size - 1).bit_length()))
+                if self._g.jpeg_reserve_frame(f.format, f.capacity):
+                    self._invalidate()
+            f.bytes_host.numpy()[:frame.size] = frame
+            f.nbytes = frame.size
+            for k in ("data", "out", "decode_status"):  # the slot's device addresses, as the format's
+                rec[k] = f.format[0][k]
+            f.record_host.numpy()[:] = np.frombuffer(rec.tobytes(), np.uint8)
+        elif cuda:
             self._stream.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(self._stream):
                 f.image.copy_(frame, non_blocking=True)
@@ -629,19 +712,22 @@ class FrameStream:
             done.record(self._stream)
         if eager:
             self._capture(f)
-        self._busy[slot] = (ticket, f, done)
-        self._next += 1
-        return ticket
+        return f, done
+
+    def _invalidate(self) -> None:
+        """A scratch buffer moved: every graph recorded its old address."""
+        for frames in self._frames:
+            for other in frames.values():
+                other.graph = None
 
     def result(self, ticket: int, *, detail: bool = False):
         """``process()``'s value for the frame of ``ticket`` (waits for it); each ticket is read once.  ``detail=True``
         returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame to still
         hold its slot: read it before ``slots`` later submits."""
-        frame = None
+        frame = decoded = None
         for slot, busy in enumerate(self._busy):
             if busy is not None and busy[0] == ticket:
-                frame = busy[1]
-                self._finish(slot)
+                frame, decoded = self._finish(slot)
                 break
         if ticket not in self._done:
             raise ValueError(f"ticket {ticket} is not a submitted frame whose result is unread")
@@ -654,7 +740,10 @@ class FrameStream:
         people, record = out
         if not detail:
             return people
-        return FrameResult(people, record, DeviceMaps(frame.heat.clone(), False), DeviceMaps(frame.paf.clone(), frame.as_f64))
+        if decoded is None and frame.format is not None:
+            decoded = frame.image.cpu().numpy()
+        return FrameResult(people, record, DeviceMaps(frame.heat.clone(), False), DeviceMaps(frame.paf.clone(), frame.as_f64),
+                           decoded)
 
     def _path(self, f: _Frame) -> None:
         """One frame's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
@@ -663,6 +752,11 @@ class FrameStream:
         if self.input_stage == "device":
             if f.host is not None:
                 f.image.copy_(f.host, non_blocking=True)
+            if f.format is not None:
+                f.bytes.copy_(f.bytes_host, non_blocking=True)
+                f.record.copy_(f.record_host, non_blocking=True)
+                self._g.jpeg_decode_frame(f.record.data_ptr(), f.format, f.capacity)
+                f.status_host.copy_(f.status, non_blocking=True)
             self._g.prenet(f.image, f.multiplier, self.params["rotation_search"], max_downsample=md, pad_value=pv,
                            out=f.pairs)
         else:
@@ -693,11 +787,18 @@ class FrameStream:
         f.graph = graph
         self.captures += 1
 
-    def _finish(self, slot: int) -> None:
-        """Wait for the slot's frame and keep its result (or the error it raises) under its ticket; frees the slot."""
-        ticket, f, done = self._busy[slot]
+    def _finish(self, slot: int):
+        """Wait for the slot's frame and keep its result (or the error it raises) under its ticket; frees the slot.  A
+        JPEG frame the device decoder flagged is posed again from the slot's bytes, decoded with cv2.  Returns the
+        slot's frame that holds the result's maps, and the cv2-decoded image of a JPEG frame (else None)."""
+        ticket, f, done, decoded = self._busy[slot]
         self._busy[slot] = None
         done.synchronize()
+        if f.format is not None and int(f.status_host[0]) != JPEG_OK:
+            decoded = _imdecode(f.bytes_host[:f.nbytes].numpy())
+            self.host_decodes += 1
+            f, done = self._launch(slot, decoded)
+            done.synchronize()
         record = f.rec_host.numpy().copy()
         rec = wire.as_records(record, self._g.J, self._g.capR)[0]
         try:
@@ -711,6 +812,7 @@ class FrameStream:
             self._done[ticket] = (people, record)
         except GroupingError as e:
             self._done[ticket] = e
+        return f, decoded
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:

@@ -19,7 +19,7 @@ from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libspgroup.so")
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 ST_PEAK_OVERFLOW, ST_CAND_OVERFLOW, ST_ROW_OVERFLOW, ST_SAMPLE_INDEX, ST_ASSERT, ST_WIRE_OVERFLOW = 1, 2, 4, 8, 16, 32
 ST_NONFINITE, ST_NAN_PRIORITY = 64, 128
@@ -212,6 +212,8 @@ _PROTOTYPES = {
     # record: a JPEG_RECORD; records: a JPEG_RECORD array
     "spg_jpeg_parse": (_int, [_ptr, _i64, _ptr]),
     "spg_jpeg_decode_ragged": (_int, [_ptr, _ptr, _i32, _ptr]),
+    "spg_jpeg_decode_frame": (_int, [_ptr, _ptr, _ptr, _i64, _ptr]),  # device_record: a device JPEG_RECORD
+    "spg_jpeg_reserve_frame": (_int, [_ptr, _ptr, _i64, _P(C.c_int32)]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -1024,6 +1026,24 @@ class Grouper:
         s = self._records(records, JPEG_RECORD)
         _check(self._lib.spg_jpeg_decode_ragged(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)),
                "spg_jpeg_decode_ragged", self._h)
+
+    def jpeg_reserve_frame(self, format: np.ndarray, max_scan_bytes: int) -> bool:
+        """``spg_jpeg_reserve_frame``: grow, outside any capture, the scratch that ``jpeg_decode_frame`` needs for the
+        frames of ``format`` (a ``JPEG_RECORD``) with up to ``max_scan_bytes`` of entropy-coded data.  Returns whether
+        the buffer moved: graphs that recorded this handle's JPEG frame decodes must then be captured again."""
+        f = self._records(format, JPEG_RECORD)
+        moved = C.c_int32(0)
+        _check(self._lib.spg_jpeg_reserve_frame(self._h, f.ctypes.data, int(max_scan_bytes), C.byref(moved)),
+               "spg_jpeg_reserve_frame", self._h)
+        return bool(moved.value)
+
+    def jpeg_decode_frame(self, device_record: int, format: np.ndarray, max_scan_bytes: int, stream=None) -> None:
+        """``spg_jpeg_decode_frame``: decode the frame whose parsed ``JPEG_RECORD`` is at the device address
+        ``device_record`` into ``format``'s ``out`` (its ``decode_status`` gets the frame's status); ``format`` holds
+        the frame's format.  Can be recorded into a CUDA graph once ``jpeg_reserve_frame`` has reserved the scratch."""
+        f = self._records(format, JPEG_RECORD)
+        _check(self._lib.spg_jpeg_decode_frame(self._h, int(device_record), f.ctypes.data, int(max_scan_bytes),
+                                               self._stream_ptr(stream)), "spg_jpeg_decode_frame", self._h)
 
     def jpeg_kernel(self) -> str:
         """Name of the kernel the last JPEG decode launched."""

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define SPG_ABI_VERSION 2
+#define SPG_ABI_VERSION 3
 
 enum {
     SPG_OK = 0,
@@ -321,7 +321,11 @@ int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, 
  * max_downsample, then through spg_postnet_rotated with one scale per item at `stride` and a rotation wherever the item
  * has rotate = 1.  The handle's max_batch sizes the post-network sums as spg_postnet_rotated does.  *moved (may be NULL)
  * is set to 1 when a buffer had to be reallocated, which invalidates graphs captured earlier from this handle's calls
- * (they hold the old address), else to 0.  Synchronous; must not be called while any stream of the device captures. */
+ * (they hold the old address), else to 0.  Synchronous; must not be called while any stream of the device captures.
+ *
+ * spg_jpeg_decode_frame (below) is the JPEG decode of one frame in a form that can be recorded: its graph serves every
+ * frame of one format, and spg_jpeg_reserve_frame grows its scratch for a format and a capacity ahead of the capture,
+ * with *moved as here. */
 int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_downsample, const spg_prenet_item *items,
                       int32_t n_items, int32_t stride, int32_t *moved);
 
@@ -550,6 +554,23 @@ int spg_jpeg_parse(const uint8_t *data, int64_t size, spg_jpeg_record *record);
  * return.  The handle's scratch (the unstuffed data, coefficients and planes) grows on demand, so calls on one handle
  * must not run concurrently on different streams. */
 int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_t n, void *stream);
+/* The decode of one frame, which can be recorded into a CUDA graph (see "frames recorded into a CUDA graph") and replayed
+ * for every frame of one format.  The format is what the recorded launches depend on: frame height and width, component
+ * count, luma sampling, restart interval and EXIF orientation, taken from the host record `format` (validated as
+ * spg_jpeg_decode_ragged validates a record; its `out` and `decode_status` are the frame's output and status).  The rest
+ * is read on the device when the launches run, from `device_record` (a device copy of the frame's parsed record): the
+ * bytes at `data`, the scan's offset and length, the quantisation and Huffman tables.  The grids cover max_scan_bytes of
+ * entropy-coded data, 1 .. 2^28 - 1; a frame whose scan_length exceeds it gets SPG_JPEG_CORRUPT, and no byte past a
+ * frame's own data is read, whatever an earlier, longer frame left in the buffers.  The frame's image and status are
+ * those spg_jpeg_decode_ragged gives.  Asynchronous on `stream`; never synchronises or allocates while `stream`
+ * captures: a scratch buffer too small then returns SPG_E_CAPTURE with nothing enqueued.  The calls of one handle share
+ * its scratch, so they must run in stream order. */
+int spg_jpeg_decode_frame(spg_handle *h, const spg_jpeg_record *device_record, const spg_jpeg_record *format,
+                          int64_t max_scan_bytes, void *stream);
+/* Grow, outside any capture, the scratch spg_jpeg_decode_frame needs for `format` and max_scan_bytes; *moved (may be
+ * NULL) as for spg_reserve_frame: 1 when the buffer was reallocated, which invalidates graphs that recorded this handle's
+ * JPEG frame decodes.  Synchronous; must not be called while any stream of the device captures. */
+int spg_jpeg_reserve_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes, int32_t *moved);
 
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */
