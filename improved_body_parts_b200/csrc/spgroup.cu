@@ -1448,6 +1448,46 @@ int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_
     return grow(h, h->heat_acc, acc);
 }
 
+int spg_reserve_frames(spg_handle *h, int32_t max_downsample, const spg_prenet_member *members, int32_t n_images,
+                       int32_t n_items, int32_t *moved) {
+    if (!h) return SPG_E_INVALID;
+    if (moved) *moved = 0;
+    int rc;
+    if ((rc = check_prenet_common(h, max_downsample, 0))) return rc;
+    if (!members || n_images < 1 || n_items < 1)
+        return fail(h, SPG_E_INVALID, "members is NULL, or n_images %d or n_items %d below 1", n_images, n_items);
+    // spg_postnet_ragged_items and spg_group_ragged hold the batch in the handle's max_batch-sized workspace
+    if ((rc = check_batch(h, n_images))) return rc;
+    // spg_prenet_ragged's scratch grid: at most every rotated member's padded image in one launch; then
+    // spg_postnet_ragged_items' float64 keypoint sums, when they outlive a launch
+    size_t grid = 0, acc = 0;
+    bool any_rot = false;
+    for (int i = 0; i < n_images; i++) {
+        const spg_prenet_member &im = members[(size_t)i * n_items];
+        if ((rc = check_dims(h, 1, im.height, im.width))) return fail(h, rc, "image %d: %s", i, std::string(h->err).c_str());
+        for (int t = 0; t < n_items; t++) {
+            const int k = i * n_items + t;
+            const spg_prenet_member &m = members[k];
+            if (m.height != im.height || m.width != im.width)
+                return fail(h, SPG_E_INVALID, "member %d: its image size differs from its image's first member", k);
+            PreMember a;
+            float out;  // the geometry does not read the output
+            if ((rc = prenet_member(h, "member", k, m.height, m.width, max_downsample, 0, m.scale, m.rotate, m.reserved, m.matrix,
+                                    &out, a)))
+                return rc;
+            if (m.rotate) grid += (size_t)a.Hp * a.Wp * 3;
+            any_rot = any_rot || m.rotate;
+        }
+        acc += (size_t)h->ws.K * im.height * im.width * sizeof(double);
+    }
+    if (!(n_items > 1 && (n_items > kPostMaxScales || any_rot))) acc = 0;
+    if (moved) *moved = grid > h->pre_grid.bytes || acc > h->heat_acc.bytes;  // set before a failed growth too
+    h->frames_reserved = true;
+    DeviceGuard guard(h->device);
+    if ((rc = grow(h, h->pre_grid, grid))) return rc;
+    return grow(h, h->heat_acc, acc);
+}
+
 // ---- training samples --------------------------------------------------------------------------
 namespace {
 
@@ -2691,18 +2731,85 @@ JpegMember jpeg_member(Carver &c, const spg_jpeg_record &r, long long scan_bytes
     return m;
 }
 
-// spg_jpeg_reserve_frame / spg_jpeg_decode_frame's arguments
-int jpeg_check_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes) {
-    if (!format) return fail(h, SPG_E_INVALID, "format is NULL");
-    if (max_scan_bytes < 1 || max_scan_bytes > kJpegMaxSegment)
-        return fail(h, SPG_E_INVALID, "max_scan_bytes %lld outside [1, 2^28)", (long long)max_scan_bytes);
-    return jpeg_check(h, *format, "format");
+// spg_jpeg_reserve_frames / spg_jpeg_decode_frames' arguments
+int jpeg_check_frames(spg_handle *h, const spg_jpeg_record *formats, const int64_t *capacities, int32_t n) {
+    if (n < 1 || !formats || !capacities) return fail(h, SPG_E_INVALID, "formats or capacities is NULL or n %d below 1", n);
+    for (int i = 0; i < n; i++) {
+        char what[32];
+        snprintf(what, sizeof what, "format %d", i);
+        if (capacities[i] < 1 || capacities[i] > kJpegMaxSegment)
+            return fail(h, SPG_E_INVALID, "%s: capacity %lld outside [1, 2^28)", what, (long long)capacities[i]);
+        int rc;
+        if ((rc = jpeg_check(h, formats[i], what))) return rc;
+    }
+    return SPG_OK;
 }
 
-// the frame form's scratch: the member for max_scan_bytes, then its coefficients
-void jpeg_frame_layout(Carver &c, const spg_jpeg_record &format, int64_t max_scan_bytes, JpegMember &m) {
-    m = jpeg_member(c, format, max_scan_bytes);
-    m.coef = c.take<short>((size_t)m.total_blocks * 64);
+// the frame form's scratch: each member for its capacity, then every member's coefficients back to back (one memset);
+// *coef_count is their total
+void jpeg_frames_layout(Carver &c, const spg_jpeg_record *formats, const int64_t *capacities, int n, JpegMember *ms,
+                        size_t *coef_count) {
+    *coef_count = 0;
+    for (int i = 0; i < n; i++) {
+        ms[i] = jpeg_member(c, formats[i], capacities[i]);
+        *coef_count += (size_t)ms[i].total_blocks * 64;
+    }
+    short *coef = c.take<short>(*coef_count);
+    for (int i = 0; i < n; i++) {
+        ms[i].coef = coef;
+        if (coef) coef += (size_t)ms[i].total_blocks * 64;
+    }
+}
+
+// One ragged launch of JPEG kernel k over the members `sel` selects, each taking ctas_of(m) CTAs (through jpeg_launch:
+// the kernels are in jpeg.cu's and jpeg_frame.cu's translation units).
+template <class Ctas, class Sel>
+int jpeg_run(spg_handle *h, JpegKernel k, const std::vector<JpegMember> &ms, Ctas &&ctas_of, Sel &&sel, cudaStream_t st) {
+    std::vector<JpegMember> sub;
+    std::vector<long long> ctas;
+    for (const JpegMember &m : ms)
+        if (sel(m)) {
+            sub.push_back(m);
+            ctas.push_back(ctas_of(m));
+        }
+    if (sub.empty()) return SPG_OK;
+    std::vector<RaggedRange> ranges;
+    std::vector<int> first;
+    int rc;
+    if ((rc = deal_ragged(h, ctas, kJpegTableMax, "image", nullptr, ranges, first))) return rc;
+    JpegRagged table{};
+    for (const RaggedRange &g : ranges) {
+        fill_table(table, sub, first, g);
+        const cudaError_t e = jpeg_launch(k, g.ctas, st, table);
+        h->stage_kernel[kStageJpeg] = kJpegKernelName[k];
+        h->launches++;
+        if (e != cudaSuccess) return fail(h, SPG_E_CUDA, "%s launch failed: %s", kJpegKernelName[k], cudaGetErrorString(e));
+    }
+    return SPG_OK;
+}
+
+// Every launch of a decode, in order: the count to write kernels of the ragged form, or of the frame form (`frame`), then
+// the DC, IDCT and colour kernels.  Interval members and subsequence members go in one call.
+int jpeg_decode_launches(spg_handle *h, const std::vector<JpegMember> &ms, bool frame, cudaStream_t st) {
+    const int f = frame ? kJpegCountFrame - kJpegCount : 0;
+    auto run = [&](int k, auto &&ctas_of, auto &&sel) { return jpeg_run(h, (JpegKernel)k, ms, ctas_of, sel, st); };
+    auto all = [](const JpegMember &) { return true; };
+    auto with_rst = [](const JpegMember &m) { return m.restart > 0; };
+    auto without_rst = [](const JpegMember &m) { return m.restart == 0; };
+    auto chunks = [](const JpegMember &m) { return (long long)m.n_chunks; };
+    auto subs = [](const JpegMember &m) { return (long long)(m.n_subs + kJpegSubThreads - 1) / kJpegSubThreads; };
+    auto one = [](const JpegMember &) { return 1ll; };
+    int rc;
+    if ((rc = run(kJpegCount + f, chunks, all)) || (rc = run(kJpegPrefix + f, one, all)) || (rc = run(kJpegPack + f, chunks, all)) ||
+        (rc = run(kJpegInterval + f, [](const JpegMember &m) { return (long long)(m.n_intervals + kJpegThreads - 1) / kJpegThreads; },
+                  with_rst)) ||
+        (rc = run(kJpegSync + f, subs, without_rst)) || (rc = run(kJpegFixup + f, one, without_rst)) ||
+        (rc = run(kJpegWrite + f, subs, without_rst)) ||
+        (rc = run(kJpegDc, [](const JpegMember &m) { return (long long)m.n_comp; }, all)) ||
+        (rc = run(kJpegIdct, [](const JpegMember &m) { return ((long long)m.total_blocks + kJpegThreads - 1) / kJpegThreads; }, all)) ||
+        (rc = run(kJpegColor, [](const JpegMember &m) { return ((long long)m.out_h * m.out_w + kJpegThreads - 1) / kJpegThreads; }, all)))
+        return rc;
+    return SPG_OK;
 }
 
 }  // namespace
@@ -2758,96 +2865,51 @@ int spg_jpeg_decode_ragged(spg_handle *h, const spg_jpeg_record *records, int32_
     if (rc) return rc;
     SPG_CUDA(h, cudaMemcpyAsync(recs, records, sizeof(spg_jpeg_record) * n, cudaMemcpyHostToDevice, st));
     SPG_CUDA(h, cudaMemsetAsync(coef_base, 0, coef_count * sizeof(short), st));
-    // one ragged launch of kernel k over the members `sel` selects, each taking ctas_of(m) CTAs (through jpeg_launch:
-    // the kernels are in jpeg.cu's translation unit)
-    auto run = [&](JpegKernel k, auto &&ctas_of, auto &&sel) -> int {
-        std::vector<JpegMember> sub;
-        std::vector<long long> ctas;
-        for (int i = 0; i < n; i++)
-            if (sel(ms[i])) {
-                sub.push_back(ms[i]);
-                ctas.push_back(ctas_of(ms[i]));
-            }
-        if (sub.empty()) return SPG_OK;
-        std::vector<RaggedRange> ranges;
-        std::vector<int> first;
-        int rc2;
-        if ((rc2 = deal_ragged(h, ctas, kJpegTableMax, "image", nullptr, ranges, first))) return rc2;
-        JpegRagged table{};
-        for (const RaggedRange &g : ranges) {
-            fill_table(table, sub, first, g);
-            const cudaError_t e = jpeg_launch(k, g.ctas, st, table);
-            h->stage_kernel[kStageJpeg] = kJpegKernelName[k];
-            h->launches++;
-            if (e != cudaSuccess) return fail(h, SPG_E_CUDA, "%s launch failed: %s", kJpegKernelName[k], cudaGetErrorString(e));
-        }
-        return SPG_OK;
-    };
-    auto all = [](const JpegMember &) { return true; };
-    auto with_rst = [](const JpegMember &m) { return m.restart > 0; };
-    auto without_rst = [](const JpegMember &m) { return m.restart == 0; };
-    auto chunks = [](const JpegMember &m) { return (long long)m.n_chunks; };
-    auto subs = [](const JpegMember &m) { return (long long)(m.n_subs + kJpegSubThreads - 1) / kJpegSubThreads; };
-    auto one = [](const JpegMember &) { return 1ll; };
-    if ((rc = run(kJpegCount, chunks, all)) || (rc = run(kJpegPrefix, one, all)) || (rc = run(kJpegPack, chunks, all)) ||
-        (rc = run(kJpegInterval, [](const JpegMember &m) { return (long long)(m.n_intervals + kJpegThreads - 1) / kJpegThreads; },
-                  with_rst)) ||
-        (rc = run(kJpegSync, subs, without_rst)) || (rc = run(kJpegFixup, one, without_rst)) ||
-        (rc = run(kJpegWrite, subs, without_rst)) ||
-        (rc = run(kJpegDc, [](const JpegMember &m) { return (long long)m.n_comp; }, all)) ||
-        (rc = run(kJpegIdct, [](const JpegMember &m) { return ((long long)m.total_blocks + kJpegThreads - 1) / kJpegThreads; }, all)) ||
-        (rc = run(kJpegColor, [](const JpegMember &m) { return ((long long)m.out_h * m.out_w + kJpegThreads - 1) / kJpegThreads; }, all)))
-        return rc;
-    return SPG_OK;
+    return jpeg_decode_launches(h, ms, false, st);
 }
 
-int spg_jpeg_reserve_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes, int32_t *moved) {
+int spg_jpeg_reserve_frames(spg_handle *h, const spg_jpeg_record *formats, const int64_t *capacities, int32_t n,
+                            int32_t *moved) {
     if (!h) return SPG_E_INVALID;
     if (moved) *moved = 0;
     int rc;
-    if ((rc = jpeg_check_frame(h, format, max_scan_bytes))) return rc;
+    if ((rc = jpeg_check_frames(h, formats, capacities, n))) return rc;
     Carver c;
-    JpegMember m;
-    jpeg_frame_layout(c, *format, max_scan_bytes, m);
+    std::vector<JpegMember> ms((size_t)n);
+    size_t coef_count;
+    jpeg_frames_layout(c, formats, capacities, n, ms.data(), &coef_count);
     if (moved) *moved = c.bytes > h->jpeg.bytes;  // set before a failed growth too
     DeviceGuard guard(h->device);
     return grow(h, h->jpeg, c.bytes);
 }
 
-int spg_jpeg_decode_frame(spg_handle *h, const spg_jpeg_record *device_record, const spg_jpeg_record *format,
-                          int64_t max_scan_bytes, void *stream) {
+int spg_jpeg_reserve_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes, int32_t *moved) {
+    return spg_jpeg_reserve_frames(h, format, &max_scan_bytes, 1, moved);
+}
+
+int spg_jpeg_decode_frames(spg_handle *h, const spg_jpeg_record *device_records, const spg_jpeg_record *formats,
+                           const int64_t *capacities, int32_t n, void *stream) {
     if (!h) return SPG_E_INVALID;
     int rc;
-    if ((rc = jpeg_check_frame(h, format, max_scan_bytes))) return rc;
-    if (!device_record) return fail(h, SPG_E_INVALID, "device_record is NULL");
+    if ((rc = jpeg_check_frames(h, formats, capacities, n))) return rc;
+    if (!device_records) return fail(h, SPG_E_INVALID, "device_records is NULL");
     DeviceGuard guard(h->device);
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    JpegRagged table{};
-    table.n = 1;
-    JpegMember &m = table.img[0];
-    if ((rc = carve(h, h->jpeg, [&](Carver &c) { jpeg_frame_layout(c, *format, max_scan_bytes, m); }, st,
-                    "the JPEG frame decode's unstuffed stream, coefficients and planes")))
+    std::vector<JpegMember> ms((size_t)n);
+    size_t coef_count = 0;
+    if ((rc = carve(h, h->jpeg, [&](Carver &c) { jpeg_frames_layout(c, formats, capacities, n, ms.data(), &coef_count); }, st,
+                    "the JPEG frame decode's unstuffed streams, coefficients and planes")))
         return rc;
-    m.rec = device_record;
-    m.first_cta = 0;
-    SPG_CUDA(h, cudaMemsetAsync(m.coef, 0, (size_t)m.total_blocks * 64 * sizeof(short), st));
-    // the grids cover the capacity (the member's seg_len, n_chunks and n_subs); the kernels read the frame's own length
-    const long long subs = ((long long)m.n_subs + kJpegSubThreads - 1) / kJpegSubThreads;
-    std::vector<std::pair<JpegKernel, long long>> runs = {{kJpegCountFrame, m.n_chunks}, {kJpegPrefixFrame, 1}, {kJpegPackFrame, m.n_chunks}};
-    if (m.restart)
-        runs.push_back({kJpegIntervalFrame, ((long long)m.n_intervals + kJpegThreads - 1) / kJpegThreads});
-    else
-        runs.insert(runs.end(), {{kJpegSyncFrame, subs}, {kJpegFixupFrame, 1}, {kJpegWriteFrame, subs}});
-    runs.insert(runs.end(), {{kJpegDc, m.n_comp},
-                             {kJpegIdct, ((long long)m.total_blocks + kJpegThreads - 1) / kJpegThreads},
-                             {kJpegColor, ((long long)m.out_h * m.out_w + kJpegThreads - 1) / kJpegThreads}});
-    for (const auto &[k, ctas] : runs) {
-        const cudaError_t e = jpeg_launch(k, (unsigned)ctas, st, table);
-        h->stage_kernel[kStageJpeg] = kJpegKernelName[k];
-        h->launches++;
-        if (e != cudaSuccess) return fail(h, SPG_E_CUDA, "%s launch failed: %s", kJpegKernelName[k], cudaGetErrorString(e));
-    }
-    return SPG_OK;
+    for (int i = 0; i < n; i++) ms[i].rec = device_records + i;
+    SPG_CUDA(h, cudaMemsetAsync(ms[0].coef, 0, coef_count * sizeof(short), st));
+    // the grids cover each member's capacity (its seg_len, n_chunks and n_subs); the kernels read the frame's own length,
+    // and a member's CTAs past it return at once
+    return jpeg_decode_launches(h, ms, true, st);
+}
+
+int spg_jpeg_decode_frame(spg_handle *h, const spg_jpeg_record *device_record, const spg_jpeg_record *format,
+                          int64_t max_scan_bytes, void *stream) {
+    return spg_jpeg_decode_frames(h, device_record, format, &max_scan_bytes, 1, stream);
 }
 
 }  // extern "C"

@@ -554,6 +554,56 @@ class _Frame:
         self.graph = None
 
 
+def _align(n: int) -> int:
+    return -(-int(n) // 256) * 256
+
+
+class _Tick:
+    """One slot's buffers for one tick key, and the graph captured over them.  ``kinds``: per frame ``(H, W, kind)``,
+    kind False for a host image, True for a CUDA image, a ``JPEG_FORMAT`` tuple for JPEG bytes; ``caps``: per frame
+    its capacity in bytes (0 for an image); ``recs``: per frame its parsed JPEG record or None."""
+
+    def __init__(self, fs: "FrameStream", kinds: tuple, caps: list, recs: list):
+        import torch
+        dev = torch.device("cuda", fs.device)
+        self.kinds, self.caps, self.graph = kinds, list(caps), None
+        self.held: List[int] = []  # tickets of finished frames whose maps FrameStream._held still refers to
+        self.plan, self.buckets = plan_items([k[:2] for k in kinds], fs.params, fs.model_params)
+        self.jpeg = [j for j, k in enumerate(kinds) if isinstance(k[2], tuple)]
+        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames
+        self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
+        for j, (H, W, kind) in enumerate(kinds):
+            if kind is not True:
+                self.at[j] = off
+                off = _align(off + (self.caps[j] if j in self.jpeg else H * W * 3))
+        self.up_host = torch.empty(off, dtype=torch.uint8, pin_memory=True)
+        self.up = torch.empty(off, dtype=torch.uint8, device=dev)
+        self.nbytes = [0] * len(kinds)
+        self.images = [self.up[self.at[j]:self.at[j] + H * W * 3].view(H, W, 3) if kind is False else
+                       torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for j, (H, W, kind) in enumerate(kinds)]
+        self.status = torch.zeros(max(len(self.jpeg), 1), dtype=torch.int32, device=dev)
+        self.status_host = torch.zeros(self.status.shape, dtype=torch.int32, pin_memory=True)
+        self.formats = np.zeros(len(self.jpeg), JPEG_RECORD)
+        for jj, j in enumerate(self.jpeg):
+            self.formats[jj] = recs[j]
+            self.formats[jj]["data"] = self.up.data_ptr() + self.at[j]
+            self.formats[jj]["out"] = self.images[j].data_ptr()
+            self.formats[jj]["decode_status"] = self.status.data_ptr() + 4 * jj
+        self.inputs = {size: torch.empty((2 * len(members),) + size + (3,), dtype=torch.float32, device=dev)
+                       for size, members in self.buckets.items()}
+        self.n_items = len(self.plan[0])
+        self.as_f64 = self.n_items == 1  # as predict() returns
+        self.heat = [torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev) for H, W, _ in kinds]
+        self.paf = [torch.empty((1, len(fs.limbs), H, W), dtype=torch.float32 if self.as_f64 else torch.float64, device=dev)
+                    for H, W, _ in kinds]
+        self.rec = torch.zeros((len(kinds), fs._g.wire_record_bytes()), dtype=torch.uint8, device=dev)
+        self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
+
+    def members(self):
+        """Per frame, per item: ``(H, W, multiplier, angle)``, what ``Grouper.reserve_frames`` takes."""
+        return [(H, W, item[0], item[2]) for (H, W, _), items in zip(self.kinds, self.plan) for item in items]
+
+
 class FrameStream:
     """Frames posed one at a time at the GPU's rate: ``predict`` + ``group`` per frame, replayed from a CUDA graph.
 
@@ -620,12 +670,23 @@ class FrameStream:
         self._next = 0
         self.captures = 0  # graphs captured so far (a frame shape's first sight in a slot, or after a buffer moved)
         self.host_decodes = 0  # JPEG frames decoded with cv2.imdecode
+        # submit_many: the ticks' handle (its max_batch grows to the largest tick), each slot's _Tick per tick key, the
+        # next tick's slot, and the maps of finished tick frames whose result is unread
+        self._gm: Optional[Grouper] = None
+        self._ticks: List[Dict[tuple, "_Tick"]] = [{} for _ in range(int(slots))]
+        self._tick_next = 0
+        self._held: Dict[int, tuple] = {}
 
     def close(self) -> None:
         for frames in self._frames:
             frames.clear()
+        for ticks in self._ticks:
+            ticks.clear()
+        self._held.clear()
         self._g.close()
         self._tier.close()
+        if self._gm is not None:
+            self._gm.close()
 
     def __enter__(self):
         return self
@@ -637,6 +698,20 @@ class FrameStream:
         """Stage ``frame`` in the next slot and launch its graph (the shape's first frame in the slot: its calls, then the
         capture).  ``frame`` is a ``[H, W, 3]`` uint8 BGR image (numpy, or a CUDA tensor on the stream's device) or a
         JPEG file's bytes.  Returns the frame's ticket."""
+        frame, rec, decoded = self._frame_of(frame)
+        ticket = self._next
+        slot = ticket % len(self._frames)
+        if self._busy[slot] is not None:
+            self._finish(slot)
+        f, done = self._launch(slot, frame, rec)
+        self._busy[slot] = (ticket, f, done, decoded)
+        self._next += 1
+        return ticket
+
+    def _frame_of(self, frame):
+        """A submitted frame checked: ``(frame, rec, decoded)`` -- a JPEG file the parser takes as its bytes (uint8
+        array) and parsed record, any other JPEG file as cv2's image of it (also ``decoded``; counted in
+        ``host_decodes``), an image as a contiguous uint8 array or the CUDA tensor it is, with ``rec`` None."""
         import torch
         decoded = rec = None
         if isinstance(frame, (bytes, bytearray, memoryview)):
@@ -648,24 +723,19 @@ class FrameStream:
                 frame = decoded = _imdecode(data)
                 self.host_decodes += 1
                 rec = None
+            else:
+                return data, rec, None
         cuda = isinstance(frame, torch.Tensor) and frame.is_cuda
         if cuda:
             if self.input_stage == "host":
                 raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
             if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or frame.device.index != self.device:
                 raise ValueError(f"a CUDA frame is a [H, W, 3] uint8 tensor on cuda:{self.device}")
-        elif rec is None:
+        else:
             frame = np.ascontiguousarray(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
             if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
                 raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
-        ticket = self._next
-        slot = ticket % len(self._frames)
-        if self._busy[slot] is not None:
-            self._finish(slot)
-        f, done = self._launch(slot, frame if rec is None else data, rec)
-        self._busy[slot] = (ticket, f, done, decoded)
-        self._next += 1
-        return ticket
+        return frame, rec, decoded
 
     def _launch(self, slot: int, frame, rec=None):
         """Stage ``frame`` (an image, or JPEG bytes parsed into ``rec``) in ``slot`` and run its graph, or its calls and
@@ -714,6 +784,181 @@ class FrameStream:
             self._capture(f)
         return f, done
 
+    def submit_many(self, frames) -> List[int]:
+        """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
+        CUDA graph, and return one ticket per frame, each read with ``result``.
+
+        ``frames`` may mix every kind ``submit`` takes (numpy or CUDA ``[H, W, 3]`` uint8 BGR images, JPEG bytes) and
+        every shape; it needs ``input_stage="device"``.  A tick holds one slot.  The slot keeps one graph per tick key:
+        each frame's shape and kind (host image, CUDA image, or JPEG format) in order, and each JPEG frame's capacity.
+        The key's first tick runs call by call as its warm-up and is then captured (``captures``).  The graph holds one
+        pinned upload of the tick's host frames, JPEG bytes and parsed records; ``spg_jpeg_decode_frames`` for every
+        JPEG frame; ``spg_prenet_ragged`` for every item of every frame into one input tensor per network input size;
+        one forward pass per input size; ``spg_postnet_ragged_items`` reading each item's pair out of its forward in
+        place; ``spg_group_ragged`` writing the K wire records; and one copy of the records and JPEG statuses to pinned
+        host memory.  A JPEG file longer than its frame's capacity grows it, which captures that key again.  Ticks
+        take the slots in turn on a counter of their own; ``submit`` takes the slot of its ticket modulo ``slots``.  So
+        when the two are mixed, a call can land on a slot whose tick or frame is unread: it then waits for that work
+        and keeps its results, as ``submit`` does for its own slots.  If the launch or its capture raises, no ticket is
+        issued.
+
+        The fallbacks are ``submit``'s, per frame: a file the parser refuses is decoded by ``cv2.imdecode`` here and
+        joins the tick as an image; a file the device decoder flags is posed again alone, through ``submit``'s path,
+        from the slot's bytes when its tickets are read; a record with a capacity bit is regrouped on the capacity-free
+        tier from the frame's maps.  ``host_decodes`` counts the cv2 decodes.  ``result(ticket, detail=True)`` returns
+        the frame's record, maps and (for JPEG bytes) image while the tick's slot holds it.
+
+        Every kernel treats each frame on its own, so with a network whose output for a sample does not depend on its
+        batch each ticket's result equals ``submit``'s for the same frame, value for value and type for type.  The tick
+        runs each input size's items as one batch: cuDNN may pick other algorithms for a larger batch, and the maps
+        can then differ in the last bits."""
+        import torch
+        if self.input_stage != "device":
+            raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
+                             "spg_prenet_ragged")
+        staged = [self._frame_of(f) for f in frames]
+        if not staged:
+            raise ValueError("submit_many needs at least one frame")
+        kinds = tuple((int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)) if rec is not None
+                      else (int(frame.shape[0]), int(frame.shape[1]), isinstance(frame, torch.Tensor))
+                      for frame, rec, _ in staged)
+        slot = self._tick_next % len(self._ticks)
+        if self._busy[slot] is not None:
+            self._finish(slot)
+        tk, done = self._launch_tick(slot, kinds, staged)
+        tickets = list(range(self._next, self._next + len(staged)))  # issued once the tick runs
+        self._next += len(staged)
+        self._tick_next += 1
+        self._busy[slot] = (tickets, tk, done, [d for _, _, d in staged])
+        return tickets
+
+    def _launch_tick(self, slot: int, kinds: tuple, staged: list):
+        """Stage a tick's frames in the slot's ``_Tick`` for ``kinds`` (made on the key's first sight, made again when a
+        JPEG frame outgrows its capacity) and run its graph, or reserve its scratch, run its calls and capture them;
+        returns the ``_Tick`` and the event of the launch's end."""
+        import torch
+        if self._gm is None or self._gm.max_batch < len(kinds):
+            self._stream.synchronize()  # the old handle's scratch may be in use
+            if self._gm is not None:
+                self._gm.close()
+            self._gm = _new_grouper(len(kinds), self.device)
+            self._invalidate_ticks()
+        tk = self._ticks[slot].get(kinds)
+        sizes = [frame.size if rec is not None else 0 for frame, rec, _ in staged]
+        if tk is None or any(s > c for s, c in zip(sizes, tk.caps)):
+            caps = [max(1 << 16, 1 << (s - 1).bit_length()) if s else 0 for s in sizes]
+            if tk is not None:
+                caps = [max(a, b) for a, b in zip(caps, tk.caps)]
+            if tk is not None:
+                self._drop_held(tk)
+            tk = self._ticks[slot][kinds] = _Tick(self, kinds, caps, [rec for _, rec, _ in staged])
+        if tk.graph is None:
+            # Before every call-by-call run, not only on a key's first sight: a key whose graph was dropped (a buffer
+            # moved, or the handle was replaced for a larger tick) would otherwise grow a buffer in its eager run and
+            # free the address that graphs captured since then replay.
+            moved = self._gm.reserve_frames(tk.members(), tk.n_items,
+                                            max_downsample=int(self.model_params["max_downsample"]))
+            if tk.jpeg and self._gm.jpeg_reserve_frames(tk.formats, [tk.caps[j] for j in tk.jpeg]):
+                moved = True
+            if moved:
+                self._invalidate_ticks()
+        self._drop_held(tk)  # the maps of the key's earlier tick are overwritten
+        host = tk.up_host.numpy()
+        for j, ((frame, rec, _), (H, W, kind)) in enumerate(zip(staged, kinds)):
+            if rec is not None:
+                jj = tk.jpeg.index(j)
+                host[tk.at[j]:tk.at[j] + frame.size] = frame
+                tk.nbytes[j] = frame.size
+                for k in ("data", "out", "decode_status"):  # the tick's device addresses, as the format's
+                    rec[k] = tk.formats[jj][k]
+                host[jj * JPEG_RECORD.itemsize:(jj + 1) * JPEG_RECORD.itemsize] = np.frombuffer(rec.tobytes(), np.uint8)
+            elif kind:
+                self._stream.wait_stream(torch.cuda.current_stream(self.device))
+                with torch.cuda.stream(self._stream):
+                    tk.images[j].copy_(frame, non_blocking=True)
+                frame.record_stream(self._stream)
+            else:
+                host[tk.at[j]:tk.at[j] + frame.size] = frame.reshape(-1)
+        eager = tk.graph is None
+        with torch.cuda.stream(self._stream):
+            if eager:
+                self._tick_path(tk)
+            else:
+                tk.graph.replay()
+            done = torch.cuda.Event()
+            done.record(self._stream)
+        if eager:
+            self._capture(tk, self._tick_path)
+        return tk, done
+
+    def _tick_path(self, tk: _Tick) -> None:
+        """One tick's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
+        import torch
+        g = self._gm
+        md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
+        tk.up.copy_(tk.up_host, non_blocking=True)
+        if tk.jpeg:
+            g.jpeg_decode_frames(tk.up.data_ptr(), tk.formats, [tk.caps[j] for j in tk.jpeg])
+            tk.status_host.copy_(tk.status, non_blocking=True)
+        members, outs = [], []
+        for size, ms in tk.buckets.items():
+            for k, (i, t) in enumerate(ms):
+                members.append((tk.images[i], tk.plan[i][t][0], tk.plan[i][t][2]))
+                outs.append(tk.inputs[size][2 * k:2 * k + 2])
+        built = iter(g.prenet_ragged(members, max_downsample=md, pad_value=pv, out=outs))
+        entries = [[None] * tk.n_items for _ in tk.kinds]
+        with torch.no_grad():
+            for size, ms in tk.buckets.items():
+                out = _network_output(self.model, tk.inputs[size]).contiguous()
+                for k, (i, t) in enumerate(ms):
+                    _, crop, reverse = next(built)
+                    entries[i][t] = (out[2 * k:2 * k + 2], crop, reverse)
+        maps = list(zip(tk.heat, tk.paf))
+        g.postnet_ragged_items([(e, (H, W)) for e, (H, W, _) in zip(entries, tk.kinds)], outs=maps,
+                               nan_scrub=self._nan_scrub)
+        g.set_wire_output(tk.rec.data_ptr())
+        try:
+            g.group_ragged(maps, [H for H, _, _ in tk.kinds], self._gp, paf_as_f64=tk.as_f64)
+        finally:
+            g.set_wire_output(None)
+        tk.rec_host.copy_(tk.rec, non_blocking=True)
+
+    def _finish_tick(self, slot: int):
+        """``_finish`` for a slot that holds a tick: every frame's result kept under its ticket, with its maps for
+        ``result(detail=True)``.  A JPEG frame the device decoder flagged is posed again alone from the slot's bytes,
+        decoded with cv2, through ``submit``'s path."""
+        tickets, tk, done, decoded = self._busy[slot]
+        self._busy[slot] = None
+        done.synchronize()
+        records = tk.rec_host.numpy().copy()
+        for j, ticket in enumerate(tickets):
+            record, heat, paf, H, as_f64, image = records[j], tk.heat[j], tk.paf[j], tk.kinds[j][0], tk.as_f64, decoded[j]
+            if j in tk.jpeg and int(tk.status_host[tk.jpeg.index(j)]) != JPEG_OK:
+                image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + tk.nbytes[j]].numpy())
+                self.host_decodes += 1
+                f, d = self._launch(slot, image)
+                d.synchronize()
+                record, heat, paf, H, as_f64 = f.rec_host.numpy().copy(), f.heat.clone(), f.paf.clone(), f.H, f.as_f64
+            self._keep(ticket, record, heat, paf, H, as_f64)
+            if image is None and j in tk.jpeg:
+                image = tk.images[j]  # decoded on the device: copied to the host if detail asks for it
+            self._held[ticket] = (heat, paf, as_f64, image)
+            tk.held.append(ticket)
+        return None, None
+
+    def _drop_held(self, tk: _Tick) -> None:
+        """Forget the maps of ``tk``'s finished frames whose result is unread: its buffers are about to be overwritten
+        or dropped.  Their people stay readable; ``detail=True`` then raises as for a slot that holds a later frame."""
+        for ticket in tk.held:
+            self._held.pop(ticket, None)
+        tk.held.clear()
+
+    def _invalidate_ticks(self) -> None:
+        """A scratch buffer of the ticks' handle moved, or the handle was replaced: every tick graph recorded it."""
+        for ticks in self._ticks:
+            for tk in ticks.values():
+                tk.graph = None
+
     def _invalidate(self) -> None:
         """A scratch buffer moved: every graph recorded its old address."""
         for frames in self._frames:
@@ -726,11 +971,14 @@ class FrameStream:
         hold its slot: read it before ``slots`` later submits."""
         frame = decoded = None
         for slot, busy in enumerate(self._busy):
-            if busy is not None and busy[0] == ticket:
+            if busy is not None and (busy[0] == ticket or (isinstance(busy[0], list) and ticket in busy[0])):
                 frame, decoded = self._finish(slot)
                 break
         if ticket not in self._done:
             raise ValueError(f"ticket {ticket} is not a submitted frame whose result is unread")
+        held = self._held.pop(ticket, None)  # a frame of a tick: its maps, while its tick's buffers hold them
+        if held is not None:
+            frame = held
         if detail and frame is None:
             raise ValueError(f"ticket {ticket}: its slot holds a later frame; read detail=True before {len(self._busy)} "
                              "later submits")
@@ -740,6 +988,11 @@ class FrameStream:
         people, record = out
         if not detail:
             return people
+        if frame is held:
+            heat, paf, as_f64, image = held
+            if image is not None and not isinstance(image, np.ndarray):
+                image = image.cpu().numpy()
+            return FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
         if decoded is None and frame.format is not None:
             decoded = frame.image.cpu().numpy()
         return FrameResult(people, record, DeviceMaps(frame.heat.clone(), False), DeviceMaps(frame.paf.clone(), frame.as_f64),
@@ -773,14 +1026,16 @@ class FrameStream:
             self._g.set_wire_output(None)
         f.rec_host.copy_(f.rec, non_blocking=True)
 
-    def _capture(self, f: _Frame) -> None:
+    def _capture(self, f, path=None) -> None:
+        """Capture ``path(f)`` (default: ``_path``, a ``_Frame``'s) into ``f.graph``."""
         import torch
         graph = torch.cuda.CUDAGraph()
         try:
             with torch.cuda.graph(graph, pool=self._pool, stream=self._stream):
-                self._path(f)
+                (path or self._path)(f)
         except Exception as e:
-            raise GroupingError(f"capturing the path of a {f.H}x{f.W} frame failed (a model that synchronises with the "
+            what = f"a {f.H}x{f.W} frame" if path is None else f"a tick of {len(f.kinds)} frames"
+            raise GroupingError(f"capturing the path of {what} failed (a model that synchronises with the "
                                 f"host or copies from it in its forward cannot be captured): {type(e).__name__}: {e}") from e
         if self._pool is None:
             self._pool = graph.pool()
@@ -791,6 +1046,8 @@ class FrameStream:
         """Wait for the slot's frame and keep its result (or the error it raises) under its ticket; frees the slot.  A
         JPEG frame the device decoder flagged is posed again from the slot's bytes, decoded with cv2.  Returns the
         slot's frame that holds the result's maps, and the cv2-decoded image of a JPEG frame (else None)."""
+        if isinstance(self._busy[slot][0], list):
+            return self._finish_tick(slot)
         ticket, f, done, decoded = self._busy[slot]
         self._busy[slot] = None
         done.synchronize()
@@ -799,11 +1056,16 @@ class FrameStream:
             self.host_decodes += 1
             f, done = self._launch(slot, decoded)
             done.synchronize()
-        record = f.rec_host.numpy().copy()
+        self._keep(ticket, f.rec_host.numpy().copy(), f.heat, f.paf, f.H, f.as_f64)
+        return f, decoded
+
+    def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool) -> None:
+        """Keep the people of one frame's wire record (or the error they raise) under its ticket.  A record with a
+        capacity bit is regrouped on the capacity-free tier from the frame's maps."""
         rec = wire.as_records(record, self._g.J, self._g.capR)[0]
         try:
             if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
-                r = self._tier.group_unbounded(f.heat, f.paf, f.H, self._gp, paf_as_f64=f.as_f64, stream=self._tier_stream)
+                r = self._tier.group_unbounded(heat, paf, H, self._gp, paf_as_f64=as_f64, stream=self._tier_stream)
                 _check_status(r.status[0])
                 people = _people_of_result(r)
             else:
@@ -812,7 +1074,6 @@ class FrameStream:
             self._done[ticket] = (people, record)
         except GroupingError as e:
             self._done[ticket] = e
-        return f, decoded
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:

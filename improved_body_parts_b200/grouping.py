@@ -199,6 +199,7 @@ _PROTOTYPES = {
     "spg_prenet": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _P(_PrenetItem), _i32, _ptr]),
     "spg_prenet_ragged": (_int, [_ptr, _i32, _i32, _ptr, _i32, _ptr]),  # members: a PRENET_MEMBER array
     "spg_reserve_frame": (_int, [_ptr, _i32, _i32, _i32, _P(_PrenetItem), _i32, _i32, _P(C.c_int32)]),
+    "spg_reserve_frames": (_int, [_ptr, _i32, _ptr, _i32, _i32, _P(C.c_int32)]),  # members: a PRENET_MEMBER array
     # params: a TARGET_PARAMS record; samples: a TARGET_SAMPLE / TARGET_JOINTS array
     "spg_targets_warp": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
@@ -214,6 +215,9 @@ _PROTOTYPES = {
     "spg_jpeg_decode_ragged": (_int, [_ptr, _ptr, _i32, _ptr]),
     "spg_jpeg_decode_frame": (_int, [_ptr, _ptr, _ptr, _i64, _ptr]),  # device_record: a device JPEG_RECORD
     "spg_jpeg_reserve_frame": (_int, [_ptr, _ptr, _i64, _P(C.c_int32)]),
+    # device_records: a device JPEG_RECORD array; formats: a JPEG_RECORD array; capacities: an int64 array
+    "spg_jpeg_decode_frames": (_int, [_ptr, _ptr, _ptr, _ptr, _i32, _ptr]),
+    "spg_jpeg_reserve_frames": (_int, [_ptr, _ptr, _ptr, _i32, _P(C.c_int32)]),
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -947,6 +951,27 @@ class Grouper:
                "spg_reserve_frame", self._h)
         return bool(moved.value)
 
+    def reserve_frames(self, members, n_items: int, *, max_downsample: int) -> bool:
+        """``spg_reserve_frames``: grow, outside any capture, every scratch buffer that one tick of frames needs through
+        ``prenet_ragged``, ``postnet_ragged_items`` and ``group_ragged``, so that those calls can be recorded into a CUDA
+        graph.  ``members``: per image, per item of ``product(multiplier, rotate_angle)`` (``n_items`` each), the
+        ``(height, width, scale, angle)`` of that item of that image.  Returns whether a buffer moved, as
+        ``reserve_frame``."""
+        md = int(max_downsample)
+        members = list(members)
+        arr = np.zeros(max(len(members), 1), PRENET_MEMBER)
+        for i, (h, w, scale, angle) in enumerate(members):
+            scale, _, forward, _ = prenet_item(int(h), int(w), scale, angle, md)
+            arr[i] = (0, 0, int(h), int(w), scale, int(forward is not None), 0,
+                      np.zeros(6) if forward is None else np.asarray(forward, np.float64).reshape(6), 0)
+        n_items = int(n_items)
+        if n_items < 1 or len(members) % n_items:
+            raise GroupingError(f"{len(members)} members are not whole images of {n_items} items")
+        moved = C.c_int32(0)
+        _check(self._lib.spg_reserve_frames(self._h, md, arr.ctypes.data, len(members) // n_items, n_items, C.byref(moved)),
+               "spg_reserve_frames", self._h)
+        return bool(moved.value)
+
     def _prenet_out(self, o, shape, name, form):
         """A pre-network output of ``shape`` on the handle's device: ``o`` checked (the leading pair contiguous), or a new
         tensor for ``None``."""
@@ -1044,6 +1069,30 @@ class Grouper:
         f = self._records(format, JPEG_RECORD)
         _check(self._lib.spg_jpeg_decode_frame(self._h, int(device_record), f.ctypes.data, int(max_scan_bytes),
                                                self._stream_ptr(stream)), "spg_jpeg_decode_frame", self._h)
+
+    def jpeg_reserve_frames(self, formats: np.ndarray, capacities) -> bool:
+        """``spg_jpeg_reserve_frames``: ``jpeg_reserve_frame`` for the ``n`` frames of one ``jpeg_decode_frames`` call,
+        each with its format (``formats``, a ``JPEG_RECORD`` array) and capacity in scan bytes."""
+        f = self._records(formats, JPEG_RECORD)
+        caps = np.ascontiguousarray(capacities, np.int64).reshape(-1)
+        if len(caps) != len(f):
+            raise GroupingError(f"{len(f)} formats but {len(caps)} capacities")
+        moved = C.c_int32(0)
+        _check(self._lib.spg_jpeg_reserve_frames(self._h, f.ctypes.data, caps.ctypes.data, len(f), C.byref(moved)),
+               "spg_jpeg_reserve_frames", self._h)
+        return bool(moved.value)
+
+    def jpeg_decode_frames(self, device_records: int, formats: np.ndarray, capacities, stream=None) -> None:
+        """``spg_jpeg_decode_frames``: ``jpeg_decode_frame`` for ``n`` frames in each launch -- frame i's parsed
+        ``JPEG_RECORD`` at device address ``device_records + i * JPEG_RECORD.itemsize``, its format ``formats[i]`` and
+        its capacity ``capacities[i]``.  Can be recorded into a CUDA graph once ``jpeg_reserve_frames`` has reserved
+        the scratch."""
+        f = self._records(formats, JPEG_RECORD)
+        caps = np.ascontiguousarray(capacities, np.int64).reshape(-1)
+        if len(caps) != len(f):
+            raise GroupingError(f"{len(f)} formats but {len(caps)} capacities")
+        _check(self._lib.spg_jpeg_decode_frames(self._h, int(device_records), f.ctypes.data, caps.ctypes.data, len(f),
+                                                self._stream_ptr(stream)), "spg_jpeg_decode_frames", self._h)
 
     def jpeg_kernel(self) -> str:
         """Name of the kernel the last JPEG decode launched."""

@@ -328,6 +328,17 @@ int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, 
  * with *moved as here. */
 int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_downsample, const spg_prenet_item *items,
                       int32_t n_items, int32_t stride, int32_t *moved);
+/* Several frames in one graph (a tick): spg_prenet_ragged, spg_postnet_ragged_items and spg_group_ragged (with or without
+ * spg_set_wire_output) can be recorded as the calls above can.  They neither synchronise nor copy from the host: their
+ * member tables travel as kernel parameters.  spg_group_ragged allocates nothing (its workspace is the handle's,
+ * max_batch images); the other two grow a scratch buffer only through the rule above.  spg_reserve_frames grows, outside
+ * any capture, what one tick needs: members [n_images][n_items] in product(multiplier, rotate_angle) order, as
+ * spg_prenet_ragged takes them (every member of image i reads an image of its height x width; image, out and row_stride
+ * are not read), then spg_postnet_ragged_items over those images with n_items items (rotated where the member is) and
+ * spg_group_ragged over n_images <= max_batch images.  *moved as for spg_reserve_frame.  Synchronous; must not be called
+ * while any stream of the device captures. */
+int spg_reserve_frames(spg_handle *h, int32_t max_downsample, const spg_prenet_member *members, int32_t n_images,
+                       int32_t n_items, int32_t *moved);
 
 /* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
@@ -571,6 +582,19 @@ int spg_jpeg_decode_frame(spg_handle *h, const spg_jpeg_record *device_record, c
  * NULL) as for spg_reserve_frame: 1 when the buffer was reallocated, which invalidates graphs that recorded this handle's
  * JPEG frame decodes.  Synchronous; must not be called while any stream of the device captures. */
 int spg_jpeg_reserve_frame(spg_handle *h, const spg_jpeg_record *format, int64_t max_scan_bytes, int32_t *moved);
+/* spg_jpeg_decode_frame for n frames in each launch (spg_jpeg_decode_frame is this call with n = 1): member i has its own
+ * format formats[i] (host), its own capacity capacities[i] in scan bytes (host) and its own device record
+ * device_records[i] (a device array of n records).  Interval and subsequence members mix in one call.  Each member's
+ * grids cover its capacity; its CTAs past its own chunk or subsequence count return at once; a member whose scan_length
+ * exceeds its capacity gets SPG_JPEG_CORRUPT and no byte past a member's own data is read.  Each member's image and
+ * status equal those spg_jpeg_decode_ragged gives.  Asynchronous, capture rules and stream order as
+ * spg_jpeg_decode_frame. */
+int spg_jpeg_decode_frames(spg_handle *h, const spg_jpeg_record *device_records, const spg_jpeg_record *formats,
+                           const int64_t *capacities, int32_t n, void *stream);
+/* Grow, outside any capture, the scratch spg_jpeg_decode_frames needs for these n formats and capacities; *moved as for
+ * spg_jpeg_reserve_frame (which is this call with n = 1). */
+int spg_jpeg_reserve_frames(spg_handle *h, const spg_jpeg_record *formats, const int64_t *capacities, int32_t n,
+                            int32_t *moved);
 
 /* ---- stage entry points (stage-wise parity; each consumes the previous stage's device state) ---- */
 /* find_peaks: evaluate.py:169-203 = util.keypoint_heatmap_nms (utils/util.py:177-183) + util.refine_centroid (:186-211) */

@@ -1,0 +1,104 @@
+"""CPU: ``FrameStream.submit_many`` before it touches a device -- the C declarations of the tick calls, their refusal
+without a handle, ``submit_many``'s argument checks, the tick key it forms and the routing of refused JPEG files to
+``cv2.imdecode`` (the device path stubbed)."""
+import ctypes
+import os
+import re
+
+import numpy as np
+import pytest
+
+from improved_body_parts_b200 import dropin, grouping
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "spgroup.h")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "jpeg")
+cv2 = pytest.importorskip("cv2")
+
+
+@pytest.fixture(scope="module")
+def lib():
+    import __graft_entry__ as ge
+
+    ge.build()
+    return grouping.load_library()
+
+
+def _golden(name):
+    with open(os.path.join(GOLDEN, name + ".jpg"), "rb") as f:
+        return f.read()
+
+
+@pytest.mark.parametrize("name,params", [
+    ("spg_jpeg_decode_frames", ["spg_handle *h", "const spg_jpeg_record *device_records", "const spg_jpeg_record *formats",
+                                "const int64_t *capacities", "int32_t n", "void *stream"]),
+    ("spg_jpeg_reserve_frames", ["spg_handle *h", "const spg_jpeg_record *formats", "const int64_t *capacities",
+                                 "int32_t n", "int32_t *moved"]),
+    ("spg_reserve_frames", ["spg_handle *h", "int32_t max_downsample", "const spg_prenet_member *members",
+                            "int32_t n_images", "int32_t n_items", "int32_t *moved"])])
+def test_tick_calls_are_declared_and_bound(name, params):
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    m = re.search(rf"int\s+{name}\s*\(([^)]*)\)\s*;", src)
+    assert m, f"{name} is not declared"
+    assert [" ".join(p.split()) for p in m.group(1).split(",")] == params
+    restype, argtypes = grouping._PROTOTYPES[name]
+    assert restype is ctypes.c_int and len(argtypes) == len(params)
+
+
+def test_tick_calls_without_a_handle_are_invalid(lib):
+    fmt = np.zeros(1, grouping.JPEG_RECORD)
+    fmt[0] = grouping.jpeg_parse(_golden("samp_420"))
+    caps = np.array([1 << 16], np.int64)
+    moved = ctypes.c_int32(7)
+    assert lib.spg_jpeg_reserve_frames(None, fmt.ctypes.data, caps.ctypes.data, 1, ctypes.byref(moved)) == -1
+    assert lib.spg_jpeg_decode_frames(None, None, fmt.ctypes.data, caps.ctypes.data, 1, None) == -1
+    members = np.zeros(1, grouping.PRENET_MEMBER)
+    assert lib.spg_reserve_frames(None, 32, members.ctypes.data, 1, 1, ctypes.byref(moved)) == -1
+
+
+def _stream(input_stage="device", slots=2):
+    """A FrameStream without a device: _launch_tick records the tick key and the staged frames instead of running."""
+    fs = object.__new__(dropin.FrameStream)
+    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._tick_next = input_stage, 0, 0, 0, 0
+    fs._frames, fs._busy, fs._ticks, fs.launched = [{}] * slots, [None] * slots, [{}] * slots, []
+
+    def launch_tick(slot, kinds, staged):
+        fs.launched.append((slot, kinds, staged))
+        return None, None
+
+    fs._launch_tick = launch_tick
+    fs._finish = lambda slot: None
+    return fs
+
+
+def test_submit_many_arguments(lib):
+    with pytest.raises(ValueError, match="at least one"):
+        _stream().submit_many([])
+    with pytest.raises(ValueError, match="input_stage"):
+        _stream("host").submit_many([np.zeros((8, 8, 3), np.uint8)])
+    fs = _stream()
+    with pytest.raises(ValueError, match="uint8 BGR"):  # one bad frame refuses the whole tick before it is staged
+        fs.submit_many([np.zeros((8, 8, 3), np.uint8), np.zeros((4, 4), np.uint8)])
+    with pytest.raises(ValueError, match="empty"):
+        fs.submit_many([b""])
+    assert fs.launched == [] and fs._next == 0
+
+
+def test_tick_key_and_tickets(lib):
+    fs = _stream()
+    jpeg = _golden("samp_420")
+    rec = grouping.jpeg_parse(jpeg)
+    img = np.zeros((30, 40, 3), np.uint8)
+    prog = _golden("progressive")
+    tickets = fs.submit_many([img, jpeg, prog])
+    assert tickets == [0, 1, 2]
+    slot, kinds, staged = fs.launched[-1]
+    decoded = cv2.imdecode(np.frombuffer(prog, np.uint8), cv2.IMREAD_COLOR)
+    assert slot == 0
+    assert kinds == ((30, 40, False), (int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in dropin.JPEG_FORMAT)),
+                     decoded.shape[:2] + (False,))
+    assert staged[1][1] is not None and staged[1][0].tobytes() == jpeg  # the parser's file goes up as bytes
+    assert staged[2][1] is None and np.array_equal(staged[2][0], decoded)  # the refused one as cv2's image
+    assert fs.host_decodes == 1
+    assert fs._busy[0][0] == tickets
+    assert fs.submit_many([img]) == [3] and fs.launched[-1][0] == 1  # the next tick takes the next slot
