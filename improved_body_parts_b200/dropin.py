@@ -506,54 +506,6 @@ def _imdecode(data: np.ndarray) -> np.ndarray:
     return img
 
 
-class _Frame:
-    """One slot's buffers for one frame shape and input kind, and the graph captured over them."""
-
-    def __init__(self, fs: "FrameStream", H: int, W: int, cuda_input: bool):
-        import itertools
-
-        import torch
-        dev = torch.device("cuda", fs.device)
-        mp, md = fs.model_params, int(fs.model_params["max_downsample"])
-        self.H, self.W, self.graph = H, W, None
-        self.multiplier = [x * mp["boxsize"] / H for x in fs.params["scale_search"]]
-        items = [prenet_item(H, W, m, a, md) for m, a in itertools.product(self.multiplier, fs.params["rotation_search"])]
-        self.scales = [scale for scale, _, _, _ in items]
-        self.crops = [geo[:2] for _, geo, _, _ in items]
-        self.reverses = [reverse for _, _, _, reverse in items]
-        self.pairs = [torch.empty((2, geo[2], geo[3], 3), dtype=torch.float32, device=dev) for _, geo, _, _ in items]
-        if fs.input_stage == "device":
-            self.image = torch.empty((H, W, 3), dtype=torch.uint8, device=dev)
-            self.host = None if cuda_input else torch.empty((H, W, 3), dtype=torch.uint8, pin_memory=True)
-        else:
-            self.host = [torch.empty(p.shape, dtype=torch.float32, pin_memory=True) for p in self.pairs]
-        self.as_f64 = len(items) == 1  # float32 storage of the float64 values for a single item, as predict() returns
-        self.heat = torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev)
-        self.paf = torch.empty((1, len(fs.limbs), H, W), dtype=torch.float32 if self.as_f64 else torch.float64, device=dev)
-        self.rec = torch.zeros(fs._g.wire_record_bytes(), dtype=torch.uint8, device=dev)
-        self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
-        self.format = None  # JPEG frames: the format's JPEG_RECORD (set_capacity)
-
-    def set_capacity(self, rec, capacity: int) -> None:
-        """Make this a JPEG frame's slot of ``capacity`` bytes for the format of ``rec``: the frame's bytes and parsed
-        record go up from pinned buffers, and ``spg_jpeg_decode_frame`` decodes them into ``image``."""
-        import torch
-        dev = self.image.device
-        if self.format is None:
-            self.record_host = torch.empty(JPEG_RECORD.itemsize, dtype=torch.uint8, pin_memory=True)
-            self.record = torch.empty(JPEG_RECORD.itemsize, dtype=torch.uint8, device=dev)
-            self.status = torch.zeros(1, dtype=torch.int32, device=dev)
-            self.status_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-            self.format = np.zeros(1, JPEG_RECORD)
-            self.format[0] = rec
-        self.capacity, self.nbytes = int(capacity), 0
-        self.bytes_host = torch.empty(self.capacity, dtype=torch.uint8, pin_memory=True)
-        self.bytes = torch.empty(self.capacity, dtype=torch.uint8, device=dev)
-        f = self.format
-        f["data"], f["out"], f["decode_status"] = self.bytes.data_ptr(), self.image.data_ptr(), self.status.data_ptr()
-        self.graph = None
-
-
 def _align(n: int) -> int:
     return -(-int(n) // 256) * 256
 
@@ -566,21 +518,29 @@ class _Tick:
     def __init__(self, fs: "FrameStream", kinds: tuple, caps: list, recs: list):
         import torch
         dev = torch.device("cuda", fs.device)
+        host_stage = fs.input_stage == "host"
         self.kinds, self.caps, self.graph = kinds, list(caps), None
         self.held: List[int] = []  # tickets of finished frames whose maps FrameStream._held still refers to
         self.plan, self.buckets = plan_items([k[:2] for k in kinds], fs.params, fs.model_params)
+        md = int(fs.model_params["max_downsample"])
+        # per frame, per item: the crop and reverse rotation the post-network stage takes, as spg_prenet builds the item
+        self.built = [[(geo[:2], reverse) for _, geo, _, reverse in
+                       (prenet_item(H, W, item[0], item[2], md) for item in items)]
+                      for (H, W, _), items in zip(kinds, self.plan)]
         self.jpeg = [j for j, k in enumerate(kinds) if isinstance(k[2], tuple)]
-        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames
+        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames (with
+        # input_stage="host" the pairs cv2 built go up instead)
         self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
         for j, (H, W, kind) in enumerate(kinds):
-            if kind is not True:
+            if kind is not True and not host_stage:
                 self.at[j] = off
                 off = _align(off + (self.caps[j] if j in self.jpeg else H * W * 3))
         self.up_host = torch.empty(off, dtype=torch.uint8, pin_memory=True)
         self.up = torch.empty(off, dtype=torch.uint8, device=dev)
         self.nbytes = [0] * len(kinds)
-        self.images = [self.up[self.at[j]:self.at[j] + H * W * 3].view(H, W, 3) if kind is False else
-                       torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for j, (H, W, kind) in enumerate(kinds)]
+        self.images = None if host_stage else [
+            self.up[self.at[j]:self.at[j] + H * W * 3].view(H, W, 3) if kind is False else
+            torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for j, (H, W, kind) in enumerate(kinds)]
         self.status = torch.zeros(max(len(self.jpeg), 1), dtype=torch.int32, device=dev)
         self.status_host = torch.zeros(self.status.shape, dtype=torch.int32, pin_memory=True)
         self.formats = np.zeros(len(self.jpeg), JPEG_RECORD)
@@ -591,6 +551,8 @@ class _Tick:
             self.formats[jj]["decode_status"] = self.status.data_ptr() + 4 * jj
         self.inputs = {size: torch.empty((2 * len(members),) + size + (3,), dtype=torch.float32, device=dev)
                        for size, members in self.buckets.items()}
+        self.pairs = {size: torch.empty(x.shape, dtype=torch.float32, pin_memory=True)
+                      for size, x in self.inputs.items()} if host_stage else None
         self.n_items = len(self.plan[0])
         self.as_f64 = self.n_items == 1  # as predict() returns
         self.heat = [torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev) for H, W, _ in kinds]
@@ -605,45 +567,56 @@ class _Tick:
 
 
 class FrameStream:
-    """Frames posed one at a time at the GPU's rate: ``predict`` + ``group`` per frame, replayed from a CUDA graph.
+    """Frames posed at the GPU's rate: ``predict`` + ``group`` per frame, replayed from a CUDA graph per tick of frames.
 
-    ``submit(frame)`` takes a ``[H, W, 3]`` uint8 BGR frame (numpy, or a CUDA tensor on the stream's device) and returns a
-    ticket; ``result(ticket)`` returns ``process()``'s value for that frame (evaluate.py:523-543), the
+    ``submit(frame)`` takes a ``[H, W, 3]`` uint8 BGR frame (numpy, or a CUDA tensor on the stream's device) or a JPEG
+    file's bytes and returns a ticket; ``submit_many(frames)`` takes a tick of several and returns one ticket each.
+    ``result(ticket)`` returns ``process()``'s value for that frame (evaluate.py:523-543), the
     ``[([17 x (x, y)], score)]`` of ``predict_many``: equal, value for value and type for type, to ``keypoints`` of
-    ``group`` on the maps ``predict`` gives for the frame.
+    ``group`` on the maps ``predict`` gives for the frame.  ``submit`` poses a tick of one frame and ``submit_many`` a
+    tick of several, through the same calls.
 
-    The first frame of a shape in a slot runs call by call -- it is the shape's warm-up (the network's lazy set-up,
-    cuDNN's choices) -- and the slot then captures one CUDA graph over its buffers for that shape: the upload from the
-    slot's pinned buffer (``input_stage="device"``: the uint8 frame, then ``spg_prenet`` for every item of
-    ``scale_search x rotation_search``; ``"host"``: the pairs cv2 built on the host), the forward pass of every item,
-    ``spg_postnet_rotated``, ``spg_group_batch`` writing the frame's wire record and the record's copy into the slot's
-    pinned host buffer.  Every later frame of that shape in that slot is one graph launch.  A CUDA frame is copied into
-    the slot's device image ahead of a graph of its own, which starts at ``spg_prenet``.  The graphs share one memory
-    pool: they replay one at a time on the stream's own CUDA stream, and nothing allocated inside a capture outlives it.
+    A tick holds one slot.  The slot keeps one CUDA graph per **tick key**: each frame's shape and kind (host image,
+    CUDA image, or JPEG format) in order.  The key's first tick in a slot runs call by call -- it is the key's warm-up
+    (the network's lazy set-up, cuDNN's choices) -- and the slot then captures the graph over its buffers for that key;
+    every later tick of that key in that slot is one graph launch.  The graph holds one upload from the slot's pinned
+    buffer of the tick's host frames, JPEG bytes and parsed records; ``spg_jpeg_decode_frames`` for every JPEG frame;
+    ``spg_prenet_ragged`` for every item of ``scale_search x rotation_search`` of every frame, into one input tensor per
+    network input size (``input_stage="host"``: the upload of the pairs cv2 built on the host instead); the forward
+    passes; ``spg_postnet_ragged_items``; ``spg_group_ragged`` writing each frame's wire record; and one copy of the
+    records and JPEG statuses into pinned host memory.  A CUDA frame is copied into the slot's device image ahead of the
+    graph.  The graphs share one memory pool: they replay one at a time on the stream's own CUDA stream, and nothing
+    allocated inside a capture outlives it.
 
-    ``submit`` also takes a JPEG file's bytes (``bytes``, ``bytearray`` or ``memoryview``), parsed on the host with
-    ``spg_jpeg_parse``.  A file the device decoder takes (baseline or extended-sequential Huffman, grey or YCbCr 4:4:4 /
-    4:2:2 / 4:4:0 / 4:2:0) is staged with its parsed record in the slot's pinned buffers, and the slot's graph for its
-    format -- frame height and width, component count, luma sampling, restart interval and EXIF orientation -- starts
-    with their copies and ``spg_jpeg_decode_frame`` into the slot's device image, bit-identical to ``cv2.imdecode``;
-    the scan's offset and length, the tables and the segments in front of the scan are read on the device from the
-    frame's record, so they may change from frame to frame.  A slot reserves a capacity in bytes per format (the next
-    power of two of the file's size, at least 64 KiB); a longer file grows it, which captures that graph again.  A file
-    the parser refuses (progressive, arithmetic-coded, other samplings and so on) is decoded with ``cv2.imdecode`` at
-    submit and posed as a decoded frame; one the device decoder flags (corrupt data, or blocks outside the range where
-    libjpeg-turbo's IDCTs agree) is posed again from the slot's bytes the same way when its result is read, so a JPEG
-    frame's result is always the one for ``cv2.imdecode(bytes, IMREAD_COLOR)``.  ``host_decodes`` counts the JPEG frames
-    ``cv2.imdecode`` decoded; with ``input_stage="host"`` that is every JPEG frame, decoded at submit.  Bytes cv2 cannot
-    decode either raise ``ValueError``.
+    A tick of one frame forwards each item alone, as ``predict`` does, so ``submit`` equals ``predict`` + ``group``
+    with any network.  A larger tick forwards each input size's items at once: every kernel treats each frame on its
+    own, so with a network whose output for a sample does not depend on its batch each ticket equals ``submit``'s
+    result for the frame; cuDNN may pick other algorithms for a larger batch, and the maps can then differ in the last
+    bits.
 
-    ``slots`` frames are in flight at most.  Each slot owns its inputs, maps and record until its frame is finished, so
-    the host stages frame k+1 while frame k's graph runs; a submit to a slot whose frame is unread finishes that frame
-    and keeps its result for ``result``.  A record with a capacity bit in its status (a crowded frame) is regrouped on
-    the capacity-free tier from the slot's maps, as ``group`` does; any other status bit raises ``GroupingError`` from
-    ``result``.  The variant (``configure(variant=...)``), the limb table and the default device are those in effect at
-    construction.  The network's output is ``model(x)[-1][0]``, as for ``predict``; the model must be capture-safe after
-    its first call at a shape (no host synchronisation, no host-to-device copy).  A stride other than 4 raises
-    ``ValueError``, a capture that fails raises ``GroupingError``: there is no call-by-call fallback."""
+    JPEG bytes (``bytes``, ``bytearray`` or ``memoryview``) are parsed on the host with ``spg_jpeg_parse``.  A file the
+    device decoder takes (baseline or extended-sequential Huffman, grey or YCbCr 4:4:4 / 4:2:2 / 4:4:0 / 4:2:0) is
+    decoded inside the graph, bit-identical to ``cv2.imdecode``; its kind is its format -- frame height and width,
+    component count, luma sampling, restart interval and EXIF orientation -- and the scan's offset and length, the
+    tables and the segments in front of the scan are read on the device from the frame's record, so they may change
+    from frame to frame.  A slot reserves a capacity in bytes per JPEG frame of a key (the next power of two of the
+    file's size, at least 64 KiB); a longer file grows it, which captures that key again.  A file the parser refuses
+    (progressive, arithmetic-coded, other samplings and so on) is decoded with ``cv2.imdecode`` at submit and posed as
+    a decoded frame; one the device decoder flags (corrupt data, or blocks outside the range where libjpeg-turbo's
+    IDCTs agree) is decoded with cv2 from the slot's bytes when its result is read and posed again as a one-frame tick
+    in the same slot, so a JPEG frame's result is always the one for ``cv2.imdecode(bytes, IMREAD_COLOR)``.
+    ``host_decodes`` counts the JPEG frames ``cv2.imdecode`` decoded; with ``input_stage="host"`` that is every JPEG
+    frame, decoded at submit.  Bytes cv2 cannot decode either raise ``ValueError``.
+
+    ``slots`` ticks are in flight at most; each call to ``submit`` or ``submit_many`` takes the next slot in turn.  A
+    slot owns its inputs, maps and records until its tick is finished, so the host stages tick k+1 while tick k's graph
+    runs; a call to a slot whose tick is unread finishes that tick and keeps its results for ``result``.  A record with
+    a capacity bit in its status (a crowded frame) is regrouped on the capacity-free tier from the frame's maps, as
+    ``group`` does; any other status bit raises ``GroupingError`` from ``result``.  The variant
+    (``configure(variant=...)``), the limb table and the default device are those in effect at construction.  The
+    network's output is ``model(x)[-1][0]``, as for ``predict``; the model must be capture-safe after its first call at
+    a shape (no host synchronisation, no host-to-device copy).  A stride other than 4 raises ``ValueError``, a capture
+    that fails raises ``GroupingError``: there is no call-by-call fallback."""
 
     def __init__(self, model, params, model_params, *, slots: int = 2, input_stage: str = "device",
                  device: Optional[int] = None):
@@ -659,34 +632,26 @@ class FrameStream:
         self.limbs = _limbs
         self._gp = _group_params(params)
         self._nan_scrub = _variant == "demo"
-        self._g = _new_grouper(1, self.device)     # the graphs' handle
+        self._g = _new_grouper(1, self.device)     # the graphs' handle; its max_batch grows to the largest tick
         self._tier = _new_grouper(1, self.device)  # the capacity-free tier's, used while later graphs run
         self._stream = torch.cuda.Stream(device=self.device)
         self._tier_stream = torch.cuda.Stream(device=self.device)
         self._pool = None
-        self._frames: List[Dict[tuple, _Frame]] = [{} for _ in range(int(slots))]
-        self._busy: List[Optional[tuple]] = [None] * int(slots)  # per slot (ticket, frame, done event)
+        self._ticks: List[Dict[tuple, _Tick]] = [{} for _ in range(int(slots))]  # per slot, its _Tick per tick key
+        self._busy: List[Optional[tuple]] = [None] * int(slots)  # per slot (tickets, _Tick, done event, cv2 images)
         self._done: Dict[int, object] = {}  # finished tickets: (people, record) or the exception to raise
-        self._next = 0
-        self.captures = 0  # graphs captured so far (a frame shape's first sight in a slot, or after a buffer moved)
+        self._held: Dict[int, tuple] = {}  # finished tickets' maps, while their tick's buffers hold them
+        self._next = 0  # the next ticket
+        self._calls = 0  # ticks launched: the next one takes slot _calls % slots
+        self.captures = 0  # graphs captured so far (a tick key's first sight in a slot, or after a buffer moved)
         self.host_decodes = 0  # JPEG frames decoded with cv2.imdecode
-        # submit_many: the ticks' handle (its max_batch grows to the largest tick), each slot's _Tick per tick key, the
-        # next tick's slot, and the maps of finished tick frames whose result is unread
-        self._gm: Optional[Grouper] = None
-        self._ticks: List[Dict[tuple, "_Tick"]] = [{} for _ in range(int(slots))]
-        self._tick_next = 0
-        self._held: Dict[int, tuple] = {}
 
     def close(self) -> None:
-        for frames in self._frames:
-            frames.clear()
         for ticks in self._ticks:
             ticks.clear()
         self._held.clear()
         self._g.close()
         self._tier.close()
-        if self._gm is not None:
-            self._gm.close()
 
     def __enter__(self):
         return self
@@ -695,18 +660,25 @@ class FrameStream:
         self.close()
 
     def submit(self, frame) -> int:
-        """Stage ``frame`` in the next slot and launch its graph (the shape's first frame in the slot: its calls, then the
-        capture).  ``frame`` is a ``[H, W, 3]`` uint8 BGR image (numpy, or a CUDA tensor on the stream's device) or a
-        JPEG file's bytes.  Returns the frame's ticket."""
-        frame, rec, decoded = self._frame_of(frame)
-        ticket = self._next
-        slot = ticket % len(self._frames)
-        if self._busy[slot] is not None:
-            self._finish(slot)
-        f, done = self._launch(slot, frame, rec)
-        self._busy[slot] = (ticket, f, done, decoded)
-        self._next += 1
-        return ticket
+        """Pose ``frame`` as a tick of one frame in the next slot and return its ticket.  ``frame`` is a ``[H, W, 3]``
+        uint8 BGR image (numpy, or a CUDA tensor on the stream's device) or a JPEG file's bytes.  ``submit(f)`` and
+        ``submit_many([f])`` form the same tick key, so in one slot they share one graph."""
+        return self._submit([self._frame_of(frame)])[0]
+
+    def submit_many(self, frames) -> List[int]:
+        """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
+        CUDA graph in the next slot, and return one ticket per frame, each read with ``result``.
+
+        ``frames`` may mix every kind ``submit`` takes and every shape; it needs ``input_stage="device"``.  A frame
+        ``submit`` would refuse refuses the whole tick before anything is staged; if the launch or its capture raises,
+        no ticket is issued."""
+        if self.input_stage != "device":
+            raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
+                             "spg_prenet_ragged")
+        staged = [self._frame_of(f) for f in frames]
+        if not staged:
+            raise ValueError("submit_many needs at least one frame")
+        return self._submit(staged)
 
     def _frame_of(self, frame):
         """A submitted frame checked: ``(frame, rec, decoded)`` -- a JPEG file the parser takes as its bytes (uint8
@@ -737,131 +709,50 @@ class FrameStream:
                 raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
         return frame, rec, decoded
 
-    def _launch(self, slot: int, frame, rec=None):
-        """Stage ``frame`` (an image, or JPEG bytes parsed into ``rec``) in ``slot`` and run its graph, or its calls and
-        then the capture; returns the slot's frame and the event of the launch's end."""
+    def _submit(self, staged: list) -> List[int]:
+        """Launch a tick of checked frames (``_frame_of``) in the next slot; returns its tickets."""
         import torch
-        cuda = rec is None and isinstance(frame, torch.Tensor)
-        if rec is None:
-            H, W, kind = int(frame.shape[0]), int(frame.shape[1]), cuda
-        else:  # a graph per format: it starts with the decode into the slot's device image
-            H, W, kind = int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)
-        f = self._frames[slot].get((H, W, kind))
-        if f is None:
-            f = self._frames[slot][(H, W, kind)] = _Frame(self, H, W, cuda or rec is not None)
-            if self._g.reserve_frame(H, W, f.multiplier, self.params["rotation_search"],
-                                     max_downsample=int(self.model_params["max_downsample"])):
-                self._invalidate()
-        if rec is not None:
-            if f.format is None or frame.size > f.capacity:
-                f.set_capacity(rec, max(1 << 16, 1 << (frame.size - 1).bit_length()))
-                if self._g.jpeg_reserve_frame(f.format, f.capacity):
-                    self._invalidate()
-            f.bytes_host.numpy()[:frame.size] = frame
-            f.nbytes = frame.size
-            for k in ("data", "out", "decode_status"):  # the slot's device addresses, as the format's
-                rec[k] = f.format[0][k]
-            f.record_host.numpy()[:] = np.frombuffer(rec.tobytes(), np.uint8)
-        elif cuda:
-            self._stream.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(self._stream):
-                f.image.copy_(frame, non_blocking=True)
-            frame.record_stream(self._stream)
-        elif self.input_stage == "device":
-            f.host.numpy()[...] = frame
-        else:
-            for t, angle in enumerate(a for _ in f.multiplier for a in self.params["rotation_search"]):
-                _host_pair(frame, f.scales[t], angle, self.model_params, out=f.host[t].numpy())
-        eager = f.graph is None
-        with torch.cuda.stream(self._stream):
-            if eager:
-                self._path(f)
-            else:
-                f.graph.replay()
-            done = torch.cuda.Event()
-            done.record(self._stream)
-        if eager:
-            self._capture(f)
-        return f, done
-
-    def submit_many(self, frames) -> List[int]:
-        """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
-        CUDA graph, and return one ticket per frame, each read with ``result``.
-
-        ``frames`` may mix every kind ``submit`` takes (numpy or CUDA ``[H, W, 3]`` uint8 BGR images, JPEG bytes) and
-        every shape; it needs ``input_stage="device"``.  A tick holds one slot.  The slot keeps one graph per tick key:
-        each frame's shape and kind (host image, CUDA image, or JPEG format) in order, and each JPEG frame's capacity.
-        The key's first tick runs call by call as its warm-up and is then captured (``captures``).  The graph holds one
-        pinned upload of the tick's host frames, JPEG bytes and parsed records; ``spg_jpeg_decode_frames`` for every
-        JPEG frame; ``spg_prenet_ragged`` for every item of every frame into one input tensor per network input size;
-        one forward pass per input size; ``spg_postnet_ragged_items`` reading each item's pair out of its forward in
-        place; ``spg_group_ragged`` writing the K wire records; and one copy of the records and JPEG statuses to pinned
-        host memory.  A JPEG file longer than its frame's capacity grows it, which captures that key again.  Ticks
-        take the slots in turn on a counter of their own; ``submit`` takes the slot of its ticket modulo ``slots``.  So
-        when the two are mixed, a call can land on a slot whose tick or frame is unread: it then waits for that work
-        and keeps its results, as ``submit`` does for its own slots.  If the launch or its capture raises, no ticket is
-        issued.
-
-        The fallbacks are ``submit``'s, per frame: a file the parser refuses is decoded by ``cv2.imdecode`` here and
-        joins the tick as an image; a file the device decoder flags is posed again alone, through ``submit``'s path,
-        from the slot's bytes when its tickets are read; a record with a capacity bit is regrouped on the capacity-free
-        tier from the frame's maps.  ``host_decodes`` counts the cv2 decodes.  ``result(ticket, detail=True)`` returns
-        the frame's record, maps and (for JPEG bytes) image while the tick's slot holds it.
-
-        Every kernel treats each frame on its own, so with a network whose output for a sample does not depend on its
-        batch each ticket's result equals ``submit``'s for the same frame, value for value and type for type.  The tick
-        runs each input size's items as one batch: cuDNN may pick other algorithms for a larger batch, and the maps
-        can then differ in the last bits."""
-        import torch
-        if self.input_stage != "device":
-            raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
-                             "spg_prenet_ragged")
-        staged = [self._frame_of(f) for f in frames]
-        if not staged:
-            raise ValueError("submit_many needs at least one frame")
         kinds = tuple((int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)) if rec is not None
                       else (int(frame.shape[0]), int(frame.shape[1]), isinstance(frame, torch.Tensor))
                       for frame, rec, _ in staged)
-        slot = self._tick_next % len(self._ticks)
+        slot = self._calls % len(self._busy)
         if self._busy[slot] is not None:
             self._finish(slot)
-        tk, done = self._launch_tick(slot, kinds, staged)
+        tk, done = self._launch(slot, kinds, staged)
         tickets = list(range(self._next, self._next + len(staged)))  # issued once the tick runs
         self._next += len(staged)
-        self._tick_next += 1
+        self._calls += 1
         self._busy[slot] = (tickets, tk, done, [d for _, _, d in staged])
         return tickets
 
-    def _launch_tick(self, slot: int, kinds: tuple, staged: list):
+    def _launch(self, slot: int, kinds: tuple, staged: list):
         """Stage a tick's frames in the slot's ``_Tick`` for ``kinds`` (made on the key's first sight, made again when a
         JPEG frame outgrows its capacity) and run its graph, or reserve its scratch, run its calls and capture them;
         returns the ``_Tick`` and the event of the launch's end."""
         import torch
-        if self._gm is None or self._gm.max_batch < len(kinds):
+        if self._g.max_batch < len(kinds):
             self._stream.synchronize()  # the old handle's scratch may be in use
-            if self._gm is not None:
-                self._gm.close()
-            self._gm = _new_grouper(len(kinds), self.device)
-            self._invalidate_ticks()
+            self._g.close()
+            self._g = _new_grouper(len(kinds), self.device)
+            self._invalidate()
         tk = self._ticks[slot].get(kinds)
         sizes = [frame.size if rec is not None else 0 for frame, rec, _ in staged]
         if tk is None or any(s > c for s, c in zip(sizes, tk.caps)):
             caps = [max(1 << 16, 1 << (s - 1).bit_length()) if s else 0 for s in sizes]
             if tk is not None:
                 caps = [max(a, b) for a, b in zip(caps, tk.caps)]
-            if tk is not None:
                 self._drop_held(tk)
             tk = self._ticks[slot][kinds] = _Tick(self, kinds, caps, [rec for _, rec, _ in staged])
         if tk.graph is None:
             # Before every call-by-call run, not only on a key's first sight: a key whose graph was dropped (a buffer
             # moved, or the handle was replaced for a larger tick) would otherwise grow a buffer in its eager run and
             # free the address that graphs captured since then replay.
-            moved = self._gm.reserve_frames(tk.members(), tk.n_items,
-                                            max_downsample=int(self.model_params["max_downsample"]))
-            if tk.jpeg and self._gm.jpeg_reserve_frames(tk.formats, [tk.caps[j] for j in tk.jpeg]):
+            moved = self._g.reserve_frames(tk.members(), tk.n_items,
+                                           max_downsample=int(self.model_params["max_downsample"]))
+            if tk.jpeg and self._g.jpeg_reserve_frames(tk.formats, [tk.caps[j] for j in tk.jpeg]):
                 moved = True
             if moved:
-                self._invalidate_ticks()
+                self._invalidate()
         self._drop_held(tk)  # the maps of the key's earlier tick are overwritten
         host = tk.up_host.numpy()
         for j, ((frame, rec, _), (H, W, kind)) in enumerate(zip(staged, kinds)):
@@ -877,42 +768,54 @@ class FrameStream:
                 with torch.cuda.stream(self._stream):
                     tk.images[j].copy_(frame, non_blocking=True)
                 frame.record_stream(self._stream)
-            else:
+            elif tk.pairs is None:
                 host[tk.at[j]:tk.at[j] + frame.size] = frame.reshape(-1)
+        if tk.pairs is not None:  # input_stage="host": each item's pair built by cv2 into the pinned copy of its input
+            for size, ms in tk.buckets.items():
+                for k, (i, t) in enumerate(ms):
+                    _host_pair(staged[i][0], tk.plan[i][t][1], tk.plan[i][t][2], self.model_params,
+                               out=tk.pairs[size][2 * k:2 * k + 2].numpy())
         eager = tk.graph is None
         with torch.cuda.stream(self._stream):
             if eager:
-                self._tick_path(tk)
+                self._path(tk)
             else:
                 tk.graph.replay()
             done = torch.cuda.Event()
             done.record(self._stream)
         if eager:
-            self._capture(tk, self._tick_path)
+            self._capture(tk)
         return tk, done
 
-    def _tick_path(self, tk: _Tick) -> None:
+    def _path(self, tk: _Tick) -> None:
         """One tick's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
         import torch
-        g = self._gm
+        g = self._g
         md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
-        tk.up.copy_(tk.up_host, non_blocking=True)
-        if tk.jpeg:
-            g.jpeg_decode_frames(tk.up.data_ptr(), tk.formats, [tk.caps[j] for j in tk.jpeg])
-            tk.status_host.copy_(tk.status, non_blocking=True)
-        members, outs = [], []
-        for size, ms in tk.buckets.items():
-            for k, (i, t) in enumerate(ms):
-                members.append((tk.images[i], tk.plan[i][t][0], tk.plan[i][t][2]))
-                outs.append(tk.inputs[size][2 * k:2 * k + 2])
-        built = iter(g.prenet_ragged(members, max_downsample=md, pad_value=pv, out=outs))
+        if tk.pairs is None:
+            tk.up.copy_(tk.up_host, non_blocking=True)
+            if tk.jpeg:
+                g.jpeg_decode_frames(tk.up.data_ptr(), tk.formats, [tk.caps[j] for j in tk.jpeg])
+                tk.status_host.copy_(tk.status, non_blocking=True)
+            members, outs = [], []
+            for size, ms in tk.buckets.items():
+                for k, (i, t) in enumerate(ms):
+                    members.append((tk.images[i], tk.plan[i][t][0], tk.plan[i][t][2]))
+                    outs.append(tk.inputs[size][2 * k:2 * k + 2])
+            g.prenet_ragged(members, max_downsample=md, pad_value=pv, out=outs)
+        else:
+            for size, x in tk.inputs.items():
+                x.copy_(tk.pairs[size], non_blocking=True)
+        # A tick of one frame forwards each item alone, as predict does, so that submit equals predict + group with any
+        # network; a larger tick forwards each input size's items at once.
         entries = [[None] * tk.n_items for _ in tk.kinds]
         with torch.no_grad():
             for size, ms in tk.buckets.items():
-                out = _network_output(self.model, tk.inputs[size]).contiguous()
-                for k, (i, t) in enumerate(ms):
-                    _, crop, reverse = next(built)
-                    entries[i][t] = (out[2 * k:2 * k + 2], crop, reverse)
+                step = 1 if len(tk.kinds) == 1 else len(ms)
+                for c in range(0, len(ms), step):
+                    out = _network_output(self.model, tk.inputs[size][2 * c:2 * (c + step)]).contiguous()
+                    for k, (i, t) in enumerate(ms[c:c + step]):
+                        entries[i][t] = (out[2 * k:2 * k + 2],) + tk.built[i][t]
         maps = list(zip(tk.heat, tk.paf))
         g.postnet_ragged_items([(e, (H, W)) for e, (H, W, _) in zip(entries, tk.kinds)], outs=maps,
                                nan_scrub=self._nan_scrub)
@@ -923,63 +826,69 @@ class FrameStream:
             g.set_wire_output(None)
         tk.rec_host.copy_(tk.rec, non_blocking=True)
 
-    def _finish_tick(self, slot: int):
-        """``_finish`` for a slot that holds a tick: every frame's result kept under its ticket, with its maps for
-        ``result(detail=True)``.  A JPEG frame the device decoder flagged is posed again alone from the slot's bytes,
-        decoded with cv2, through ``submit``'s path."""
+    def _capture(self, tk: _Tick) -> None:
+        """Capture ``_path(tk)`` into ``tk.graph``."""
+        import torch
+        graph = torch.cuda.CUDAGraph()
+        try:
+            with torch.cuda.graph(graph, pool=self._pool, stream=self._stream):
+                self._path(tk)
+        except Exception as e:
+            raise GroupingError(f"capturing the path of a tick of {len(tk.kinds)} frame(s) failed (a model that "
+                                "synchronises with the host or copies from it in its forward cannot be captured): "
+                                f"{type(e).__name__}: {e}") from e
+        if self._pool is None:
+            self._pool = graph.pool()
+        tk.graph = graph
+        self.captures += 1
+
+    def _finish(self, slot: int) -> None:
+        """Wait for the slot's tick and keep every frame's result (or the error it raises) under its ticket, with its
+        maps for ``result(detail=True)``; frees the slot.  A JPEG frame the device decoder flagged is decoded with cv2
+        from the slot's bytes and posed again as a one-frame tick in the same slot."""
         tickets, tk, done, decoded = self._busy[slot]
         self._busy[slot] = None
         done.synchronize()
         records = tk.rec_host.numpy().copy()
         for j, ticket in enumerate(tickets):
-            record, heat, paf, H, as_f64, image = records[j], tk.heat[j], tk.paf[j], tk.kinds[j][0], tk.as_f64, decoded[j]
+            record, heat, paf, image = records[j], tk.heat[j], tk.paf[j], decoded[j]
             if j in tk.jpeg and int(tk.status_host[tk.jpeg.index(j)]) != JPEG_OK:
                 image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + tk.nbytes[j]].numpy())
                 self.host_decodes += 1
-                f, d = self._launch(slot, image)
+                again, d = self._launch(slot, ((image.shape[0], image.shape[1], False),), [(image, None, image)])
                 d.synchronize()
-                record, heat, paf, H, as_f64 = f.rec_host.numpy().copy(), f.heat.clone(), f.paf.clone(), f.H, f.as_f64
-            self._keep(ticket, record, heat, paf, H, as_f64)
-            if image is None and j in tk.jpeg:
+                record, heat, paf = again.rec_host[0].numpy().copy(), again.heat[0].clone(), again.paf[0].clone()
+            elif j in tk.jpeg:
                 image = tk.images[j]  # decoded on the device: copied to the host if detail asks for it
-            self._held[ticket] = (heat, paf, as_f64, image)
+            self._keep(ticket, record, heat, paf, tk.kinds[j][0], tk.as_f64)
+            self._held[ticket] = (heat, paf, tk.as_f64, image)
             tk.held.append(ticket)
-        return None, None
 
     def _drop_held(self, tk: _Tick) -> None:
         """Forget the maps of ``tk``'s finished frames whose result is unread: its buffers are about to be overwritten
-        or dropped.  Their people stay readable; ``detail=True`` then raises as for a slot that holds a later frame."""
+        or dropped.  Their people stay readable; ``detail=True`` then raises."""
         for ticket in tk.held:
             self._held.pop(ticket, None)
         tk.held.clear()
 
-    def _invalidate_ticks(self) -> None:
-        """A scratch buffer of the ticks' handle moved, or the handle was replaced: every tick graph recorded it."""
+    def _invalidate(self) -> None:
+        """A scratch buffer of the graphs' handle moved, or the handle was replaced: every graph recorded it."""
         for ticks in self._ticks:
             for tk in ticks.values():
                 tk.graph = None
 
-    def _invalidate(self) -> None:
-        """A scratch buffer moved: every graph recorded its old address."""
-        for frames in self._frames:
-            for other in frames.values():
-                other.graph = None
-
     def result(self, ticket: int, *, detail: bool = False):
         """``process()``'s value for the frame of ``ticket`` (waits for it); each ticket is read once.  ``detail=True``
-        returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame to still
-        hold its slot: read it before ``slots`` later submits."""
-        frame = decoded = None
+        returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame's buffers
+        to still hold them: read it before ``slots`` later calls to ``submit`` or ``submit_many``."""
         for slot, busy in enumerate(self._busy):
-            if busy is not None and (busy[0] == ticket or (isinstance(busy[0], list) and ticket in busy[0])):
-                frame, decoded = self._finish(slot)
+            if busy is not None and ticket in busy[0]:
+                self._finish(slot)
                 break
         if ticket not in self._done:
             raise ValueError(f"ticket {ticket} is not a submitted frame whose result is unread")
-        held = self._held.pop(ticket, None)  # a frame of a tick: its maps, while its tick's buffers hold them
-        if held is not None:
-            frame = held
-        if detail and frame is None:
+        held = self._held.pop(ticket, None)
+        if detail and held is None:
             raise ValueError(f"ticket {ticket}: its slot holds a later frame; read detail=True before {len(self._busy)} "
                              "later submits")
         out = self._done.pop(ticket)
@@ -988,76 +897,10 @@ class FrameStream:
         people, record = out
         if not detail:
             return people
-        if frame is held:
-            heat, paf, as_f64, image = held
-            if image is not None and not isinstance(image, np.ndarray):
-                image = image.cpu().numpy()
-            return FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
-        if decoded is None and frame.format is not None:
-            decoded = frame.image.cpu().numpy()
-        return FrameResult(people, record, DeviceMaps(frame.heat.clone(), False), DeviceMaps(frame.paf.clone(), frame.as_f64),
-                           decoded)
-
-    def _path(self, f: _Frame) -> None:
-        """One frame's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
-        import torch
-        md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
-        if self.input_stage == "device":
-            if f.host is not None:
-                f.image.copy_(f.host, non_blocking=True)
-            if f.format is not None:
-                f.bytes.copy_(f.bytes_host, non_blocking=True)
-                f.record.copy_(f.record_host, non_blocking=True)
-                self._g.jpeg_decode_frame(f.record.data_ptr(), f.format, f.capacity)
-                f.status_host.copy_(f.status, non_blocking=True)
-            self._g.prenet(f.image, f.multiplier, self.params["rotation_search"], max_downsample=md, pad_value=pv,
-                           out=f.pairs)
-        else:
-            for pair, host in zip(f.pairs, f.host):
-                pair.copy_(host, non_blocking=True)
-        with torch.no_grad():
-            outs = [_network_output(self.model, pair)[None].contiguous() for pair in f.pairs]
-        self._g.postnet(outs, f.crops, (f.H, f.W), stride=4, nan_scrub=self._nan_scrub, rotations=f.reverses,
-                        heat_out=f.heat, paf_out=f.paf)
-        self._g.set_wire_output(f.rec.data_ptr())
-        try:
-            self._g.group_device(f.heat, f.paf, f.H, self._gp, paf_as_f64=f.as_f64)
-        finally:
-            self._g.set_wire_output(None)
-        f.rec_host.copy_(f.rec, non_blocking=True)
-
-    def _capture(self, f, path=None) -> None:
-        """Capture ``path(f)`` (default: ``_path``, a ``_Frame``'s) into ``f.graph``."""
-        import torch
-        graph = torch.cuda.CUDAGraph()
-        try:
-            with torch.cuda.graph(graph, pool=self._pool, stream=self._stream):
-                (path or self._path)(f)
-        except Exception as e:
-            what = f"a {f.H}x{f.W} frame" if path is None else f"a tick of {len(f.kinds)} frames"
-            raise GroupingError(f"capturing the path of {what} failed (a model that synchronises with the "
-                                f"host or copies from it in its forward cannot be captured): {type(e).__name__}: {e}") from e
-        if self._pool is None:
-            self._pool = graph.pool()
-        f.graph = graph
-        self.captures += 1
-
-    def _finish(self, slot: int):
-        """Wait for the slot's frame and keep its result (or the error it raises) under its ticket; frees the slot.  A
-        JPEG frame the device decoder flagged is posed again from the slot's bytes, decoded with cv2.  Returns the
-        slot's frame that holds the result's maps, and the cv2-decoded image of a JPEG frame (else None)."""
-        if isinstance(self._busy[slot][0], list):
-            return self._finish_tick(slot)
-        ticket, f, done, decoded = self._busy[slot]
-        self._busy[slot] = None
-        done.synchronize()
-        if f.format is not None and int(f.status_host[0]) != JPEG_OK:
-            decoded = _imdecode(f.bytes_host[:f.nbytes].numpy())
-            self.host_decodes += 1
-            f, done = self._launch(slot, decoded)
-            done.synchronize()
-        self._keep(ticket, f.rec_host.numpy().copy(), f.heat, f.paf, f.H, f.as_f64)
-        return f, decoded
+        heat, paf, as_f64, image = held
+        if image is not None and not isinstance(image, np.ndarray):
+            image = image.cpu().numpy()
+        return FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
 
     def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool) -> None:
         """Keep the people of one frame's wire record (or the error they raise) under its ticket.  A record with a

@@ -55,13 +55,15 @@ def test_frame_decode_without_a_handle_is_invalid(lib):
 
 
 def _stream(input_stage="device"):
-    """A FrameStream without a device: only what submit reads before it stages a frame, and _launch recording its
-    arguments instead of running the slot."""
+    """A FrameStream without a device: only what submit reads before it stages a frame, and _launch recording the
+    tick's one frame and its parsed record instead of running the slot."""
     fs = object.__new__(dropin.FrameStream)
-    fs.input_stage, fs.device, fs.host_decodes, fs._next = input_stage, 0, 0, 0
-    fs._frames, fs._busy, fs.launched = [{}], [None], []
+    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._calls = input_stage, 0, 0, 0, 0
+    fs._busy, fs.launched = [None], []
 
-    def launch(slot, frame, rec=None):
+    def launch(slot, kinds, staged):
+        assert len(kinds) == 1  # submit poses a tick of one frame
+        (frame, rec, _), = staged
         fs.launched.append((frame, rec))
         return None, None
 
@@ -104,7 +106,7 @@ def test_the_format_key_of_the_goldens(lib):
     assert keys["exif1_II"] == keys["exif_9_ignored"]
 
 
-def test_refused_files_go_to_cv2(lib):
+def test_refused_files_go_to_cv2_in_a_one_frame_tick(lib):
     fs = _stream()
     prog = cv2.imencode(".jpg", np.full((16, 24, 3), 90, np.uint8), [cv2.IMWRITE_JPEG_PROGRESSIVE, 1])[1].tobytes()
     refused = [_golden("progressive"), _golden("samp_411"), _golden("fill_before_stuffing"), prog]
@@ -121,7 +123,7 @@ def test_refused_files_go_to_cv2(lib):
     assert fs.host_decodes == len(refused)
 
 
-def test_host_input_stage_decodes_jpeg_with_cv2(lib):
+def test_host_input_stage_decodes_jpeg_with_cv2_in_a_one_frame_tick(lib):
     fs = _stream("host")
     data = _golden("samp_420")
     fs.submit(data)

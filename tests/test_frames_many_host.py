@@ -1,6 +1,6 @@
 """CPU: ``FrameStream.submit_many`` before it touches a device -- the C declarations of the tick calls, their refusal
-without a handle, ``submit_many``'s argument checks, the tick key it forms and the routing of refused JPEG files to
-``cv2.imdecode`` (the device path stubbed)."""
+without a handle, ``submit_many``'s argument checks, the tick key it forms, ``submit`` as a tick of one frame and the
+routing of refused JPEG files to ``cv2.imdecode`` (the device path stubbed)."""
 import ctypes
 import os
 import re
@@ -57,16 +57,17 @@ def test_tick_calls_without_a_handle_are_invalid(lib):
 
 
 def _stream(input_stage="device", slots=2):
-    """A FrameStream without a device: _launch_tick records the tick key and the staged frames instead of running."""
+    """A FrameStream without a device: _launch records the slot, the tick key and the staged frames instead of
+    running."""
     fs = object.__new__(dropin.FrameStream)
-    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._tick_next = input_stage, 0, 0, 0, 0
-    fs._frames, fs._busy, fs._ticks, fs.launched = [{}] * slots, [None] * slots, [{}] * slots, []
+    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._calls = input_stage, 0, 0, 0, 0
+    fs._busy, fs.launched = [None] * slots, []
 
-    def launch_tick(slot, kinds, staged):
+    def launch(slot, kinds, staged):
         fs.launched.append((slot, kinds, staged))
         return None, None
 
-    fs._launch_tick = launch_tick
+    fs._launch = launch
     fs._finish = lambda slot: None
     return fs
 
@@ -84,7 +85,7 @@ def test_submit_many_arguments(lib):
     assert fs.launched == [] and fs._next == 0
 
 
-def test_tick_key_and_tickets(lib):
+def test_tick_key_tickets_and_slots_through_the_one_launcher(lib):
     fs = _stream()
     jpeg = _golden("samp_420")
     rec = grouping.jpeg_parse(jpeg)
@@ -102,3 +103,15 @@ def test_tick_key_and_tickets(lib):
     assert fs.host_decodes == 1
     assert fs._busy[0][0] == tickets
     assert fs.submit_many([img]) == [3] and fs.launched[-1][0] == 1  # the next tick takes the next slot
+
+
+def test_submit_is_a_tick_of_one_frame(lib):
+    fs = _stream()
+    img = np.zeros((30, 40, 3), np.uint8)
+    jpeg = _golden("samp_420")
+    assert fs.submit(img) == 0 and fs.submit_many([img]) == [1]
+    assert fs.submit_many([jpeg]) == [2] and fs.submit(jpeg) == 3
+    assert [slot for slot, _, _ in fs.launched] == [0, 1, 0, 1]  # one counter: each call takes the next slot
+    assert fs.launched[0][1] == fs.launched[1][1] == ((30, 40, False),)  # the same key
+    assert fs.launched[2][1] == fs.launched[3][1] and len(fs.launched[3][1]) == 1
+    assert fs._busy[1][0] == [3]

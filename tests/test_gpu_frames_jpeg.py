@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import make_jpeg_golden as mjg
-from test_gpu_frames import MODEL_PARAMS, StandIn, _live, _typed
+from frames_reference import MODEL_PARAMS, StandIn, _live, _typed
 
 pytestmark = pytest.mark.gpu
 cv2 = pytest.importorskip("cv2")

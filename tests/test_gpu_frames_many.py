@@ -1,9 +1,11 @@
 """GPU: ``dropin.FrameStream.submit_many`` -- a tick of frames through one CUDA graph (``spg_jpeg_decode_frames``,
 ``spg_prenet_ragged``, one forward per input size, ``spg_postnet_ragged_items``, ``spg_group_ragged``) -- against
-``submit`` of the same frames on a stream of its own: people by value and type, wire records and maps equal.  Then the
-C calls under it: the ragged calls recorded after ``spg_reserve_frames`` equal the same calls made one by one, refuse to
-grow inside a capture, and ``spg_jpeg_decode_frames`` equals ``spg_jpeg_decode_ragged`` and ``cv2.imdecode``.  The network
-is test_gpu_frames.py's stand-in, whose output for a sample does not depend on its batch."""
+``dropin.predict`` + ``dropin.group`` of each frame (of ``cv2.imdecode``'s image for JPEG bytes): people by value and
+type, wire records, maps and decoded images equal.  ``submit`` and a one-frame ``submit_many`` share one graph.  Then
+the C calls under it: the ragged calls recorded after ``spg_reserve_frames`` equal the same calls made one by one,
+refuse to grow inside a capture, and ``spg_jpeg_decode_frames`` equals ``spg_jpeg_decode_ragged`` and ``cv2.imdecode``.
+The reference and the stand-in network, whose output for a sample does not depend on its batch, are
+frames_reference.py's."""
 import glob
 import os
 import types
@@ -12,7 +14,7 @@ import numpy as np
 import pytest
 
 import make_jpeg_golden as mjg
-from test_gpu_frames import MODEL_PARAMS, StandIn, _live, _typed
+from frames_reference import MODEL_PARAMS, StandIn, _live, _reference, _typed
 
 pytestmark = pytest.mark.gpu
 cv2 = pytest.importorskip("cv2")
@@ -78,22 +80,28 @@ def _assert_same(env, got, want, what):
         assert got.image is not None and np.array_equal(got.image, want.image), f"{what}: image"
 
 
+def _want(env, frame, params, model, model_params=MODEL_PARAMS):
+    """The reference's FrameResult for ``frame``: predict + group of the frame (of cv2.imdecode's image for JPEG
+    bytes)."""
+    image = _decode(frame) if isinstance(frame, bytes) else None
+    heat, paf, people, record = _reference(env, frame if image is None else image, params, model,
+                                           model_params=model_params)
+    return env.dropin.FrameResult(people, record, heat, paf, image)
+
+
 def _compare(env, ticks, params, model=None, slots=2, model_params=MODEL_PARAMS):
-    """Every tick through submit_many, every frame through submit on another stream: equal results.  Returns the tick
-    stream and the number of persons seen."""
+    """Every tick through submit_many, every frame through the reference: equal results.  Returns the tick stream and
+    the number of persons seen."""
     model = model or StandIn(env.torch, env.synth)
-    d = env.dropin
-    fs = d.FrameStream(model, params, model_params, slots=slots)
+    fs = env.dropin.FrameStream(model, params, model_params, slots=slots)
     persons = 0
-    with d.FrameStream(model, params, model_params, slots=slots) as ref:
-        for n, frames in enumerate(ticks):
-            tickets = fs.submit_many(frames)
-            assert len(tickets) == len(frames) and len(set(tickets)) == len(frames)
-            for j, (tk, frame) in enumerate(zip(tickets, frames)):
-                got = fs.result(tk, detail=True)
-                want = ref.result(ref.submit(frame), detail=True)
-                _assert_same(env, got, want, f"tick {n} frame {j}")
-                persons += len(got.people)
+    for n, frames in enumerate(ticks):
+        tickets = fs.submit_many(frames)
+        assert len(tickets) == len(frames) and len(set(tickets)) == len(frames)
+        for j, (tk, frame) in enumerate(zip(tickets, frames)):
+            got = fs.result(tk, detail=True)
+            _assert_same(env, got, _want(env, frame, params, model, model_params), f"tick {n} frame {j}")
+            persons += len(got.people)
     return fs, persons
 
 
@@ -192,12 +200,11 @@ def test_slot_reuse_with_unread_tickets(env):
     model = StandIn(env.torch, env.synth)
     d = env.dropin
     ticks = [_frames(env, 3, SHAPES, 20 + n) for n in range(5)]
-    with d.FrameStream(model, params, MODEL_PARAMS, slots=2) as fs, \
-            d.FrameStream(model, params, MODEL_PARAMS, slots=2) as ref:
+    with d.FrameStream(model, params, MODEL_PARAMS, slots=2) as fs:
         tickets = [fs.submit_many(tick) for tick in ticks]  # every slot reused with its tickets unread
         for tick, tks in zip(ticks, tickets):
             for frame, tk in zip(tick, tks):
-                assert _typed(fs.result(tk)) == _typed(ref.result(ref.submit(frame)))
+                assert _typed(fs.result(tk)) == _typed(_want(env, frame, params, model).people)
         last = fs.submit_many(ticks[0])
         fs.submit_many(ticks[1])
         fs.submit_many(ticks[2])  # the slot of `last` now holds a later tick
@@ -216,6 +223,22 @@ def test_a_longer_jpeg_member_captures_again(env):
         assert fs.captures == 2 and fs.host_decodes == 0
     finally:
         fs.close()
+
+
+@pytest.mark.parametrize("search", ["1 item", "3 angles"])
+def test_submit_and_a_one_frame_tick_share_a_graph(env, search):
+    """submit(a) and submit_many([a]) form one tick key: in one slot they share one graph, and with a rotation search
+    (three items of one input size) the one-frame tick forwards each item alone, as predict and submit do."""
+    params = _params(env, search)
+    model = StandIn(env.torch, env.synth)
+    a = mjg.content(30, 120, 160)
+    want = _want(env, a, params, model)
+    with env.dropin.FrameStream(model, params, MODEL_PARAMS, slots=1) as fs:
+        got = [fs.result(fs.submit(a), detail=True), fs.result(fs.submit_many([a])[0], detail=True),
+               fs.result(fs.submit(a), detail=True)]
+        assert fs.captures == 1
+    for n, g in enumerate(got):
+        _assert_same(env, g, want, f"call {n}")
 
 
 def test_submit_many_arguments(env):

@@ -3,9 +3,9 @@
 ``dropin.predict`` + ``dropin.group`` per frame, alternated round by round in the same run.
 
 Workload: --frames seeded random uint8 frames, shapes drawn from a fixed table of COCO val2017 sizes, at the reference's
-settings (boxsize 640, max_downsample 64, scale_search [1], rotation_search [0], stride 4); the network is imhn.IMHN at
-the reference's random initialisation, bf16 autocast, channels-last (``imhn.Runner`` without a graph of its own: the
-frame graph records its forward).  Modes:
+settings (boxsize 640, max_downsample 64, stride 4; scale_search [1] and rotation_search [0] unless --scale-search and
+--rotation-search say otherwise); the network is imhn.IMHN at the reference's random initialisation, bf16 autocast,
+channels-last (``imhn.Runner`` without a graph of its own: the frame graph records its forward).  Modes:
   * per_call:  predict + group + keypoints per frame, each frame finished before the next;
   * stream:    submit then result per frame (slots=2): the latency of one frame from submit to result;
   * pipelined: frame k+1 submitted before frame k's result is read (slots=2): the stream's frame rate.
@@ -15,7 +15,8 @@ first call to the result, and, in a separate pass under torch.profiler, the kern
 memset excluded; listed apart).  The people of every mode are compared with per_call's.  The card's name and power
 limit are read in the same run.
 
-usage: python tools/bench_frames.py [--frames 48] [--rounds 3] [--out profiles/frames.json]"""
+usage: python tools/bench_frames.py [--frames 48] [--rounds 3] [--scale-search 1] [--rotation-search 0]
+                                   [--out profiles/frames.json]"""
 import argparse
 import json
 import os
@@ -47,6 +48,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=48)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--scale-search", type=float, nargs="+", default=[1.0])
+    ap.add_argument("--rotation-search", type=float, nargs="+", default=[0.0])
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "frames.json"))
     a = ap.parse_args()
     import torch
@@ -59,7 +62,7 @@ def main():
     rng = np.random.default_rng(2031)
     frames = [rng.integers(0, 256, size=SHAPES[int(rng.integers(len(SHAPES)))] + (3,), dtype=np.uint8)
               for _ in range(a.frames)]
-    params = dict(skeleton.default_params(), scale_search=[1.0], rotation_search=[0.0])
+    params = dict(skeleton.default_params(), scale_search=a.scale_search, rotation_search=a.rotation_search)
     runner = imhn.Runner(imhn.IMHN().init_like_reference_(0), device="cuda:0", use_graph=False)
 
     def model(x):
@@ -123,9 +126,10 @@ def main():
                     k += ev.device_time_total / 1e3
         kern[m] = (k, c)
     name, pl = card()
-    res = {"card": name, "power_limit": pl, "frames": a.frames, "rounds": a.rounds, "captures": fs.captures, "modes": {}}
-    print(f"{name}, power limit {pl}; {a.frames} frames, IMHN bf16, boxsize 640, scale_search [1], rotation_search [0]; "
-          f"{fs.captures} graphs captured")
+    res = {"card": name, "power_limit": pl, "frames": a.frames, "rounds": a.rounds, "scale_search": a.scale_search,
+           "rotation_search": a.rotation_search, "captures": fs.captures, "modes": {}}
+    print(f"{name}, power limit {pl}; {a.frames} frames, IMHN bf16, boxsize 640, scale_search {a.scale_search}, "
+          f"rotation_search {a.rotation_search}; {fs.captures} graphs captured")
     for m in modes:
         ts = sorted(times[m])
         med = ts[len(ts) // 2]
