@@ -24,8 +24,8 @@ from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 import numpy as np
 
 from . import sharding, wire
-from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse,
-                       prenet_item)
+from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, YUV_I420, YUV_MEMBER, YUV_NV12, YUV_YUYV, Grouper, GroupingError,
+                       clamp_scale, input_geometry, jpeg_parse, prenet_item)
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -485,7 +485,8 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
 class FrameResult(NamedTuple):
     """``FrameStream.result(ticket, detail=True)``: the people, the frame's wire record (``include/spgroup.h``; only the
     header and the first ``n_persons`` rows are the frame's), copies of its averaged maps and, for a frame submitted as
-    JPEG bytes, the ``[H, W, 3]`` uint8 BGR image it was decoded to (on the device or by ``cv2.imdecode``), else None."""
+    JPEG bytes or a ``YUVFrame``, the ``[H, W, 3]`` uint8 BGR image it was decoded or converted to (on the device, or by
+    ``cv2.imdecode`` / ``cv2.cvtColor``), else None."""
     people: list
     record: np.ndarray
     heat: "DeviceMaps"
@@ -506,14 +507,97 @@ def _imdecode(data: np.ndarray) -> np.ndarray:
     return img
 
 
+#: cv2.cvtColor's code and spg_yuv_to_bgr's format of each YUV layout FrameStream takes
+_YUV = {"nv12": ("COLOR_YUV2BGR_NV12", YUV_NV12), "i420": ("COLOR_YUV2BGR_I420", YUV_I420),
+        "yuyv": ("COLOR_YUV2BGR_YUYV", YUV_YUYV)}
+
+
+def _yuv_layout(fmt: str, H: int, W: int) -> List[Tuple[int, Tuple[int, int]]]:
+    """Per plane of an H x W frame in ``fmt``: its offset in the packed planes and its shape."""
+    shapes = {"nv12": [(H, W), (H // 2, W)], "i420": [(H, W), (H // 2, W // 2), (H // 2, W // 2)],
+              "yuyv": [(H, 2 * W)]}[fmt]
+    offsets = np.cumsum([0] + [h * w for h, w in shapes]).tolist()
+    return list(zip(offsets, shapes))
+
+
+def _yuv_bytes(fmt: str, H: int, W: int) -> int:
+    """The packed planes' bytes: 1.5 per pixel for NV12 and I420, 2 for YUYV."""
+    return H * W * 3 // 2 if fmt != "yuyv" else 2 * H * W
+
+
+class YUVFrame:
+    """A camera or video frame in YUV, for ``FrameStream.submit`` and ``submit_many``.
+
+    ``format`` is ``"nv12"`` (NVDEC and GPU video readers), ``"i420"`` (FFmpeg / PyAV ``yuv420p``, software
+    pipelines) or ``"yuyv"`` (V4L2 / UVC webcams), and ``planes`` a tuple of 2-D uint8 arrays, all numpy or all CUDA
+    tensors on one device: NV12 Y ``[H, W]`` and interleaved UV ``[H/2, W]``; I420 Y ``[H, W]``, U and V
+    ``[H/2, W/2]``; YUYV the packed ``[H, 2W]``.  A plane's rows may be pitched -- stride ``(pitch, 1)`` with ``pitch``
+    at least its row's bytes -- so the views of a decoder's surface can be passed as they are.  H and W must be even
+    (W for YUYV), as ``cv2.cvtColor`` requires.  The frame is posed as ``cv2.cvtColor(frame, COLOR_YUV2BGR_*)``, OpenCV's
+    BT.601 limited-range conversion."""
+
+    __slots__ = ("format", "planes", "height", "width", "device")
+
+    def __init__(self, format: str, planes):
+        import torch
+        if format not in _YUV:
+            raise ValueError(f"a YUV frame's format is one of {tuple(_YUV)}, not {format!r}")
+        planes = tuple(p.numpy() if isinstance(p, torch.Tensor) and not p.is_cuda else p for p in planes)
+        n = len(_yuv_layout(format, 2, 2))
+        if len(planes) != n:
+            raise ValueError(f"a {format} frame has {n} plane(s), not {len(planes)}")
+        cuda = [isinstance(p, torch.Tensor) for p in planes]
+        if any(cuda) and (not all(cuda) or len({p.device for p in planes}) != 1):
+            raise ValueError("a YUV frame's planes are all numpy arrays or all CUDA tensors on one device")
+        for k, p in enumerate(planes):
+            if not (isinstance(p, np.ndarray) or cuda[k]) or p.dtype != (torch.uint8 if cuda[k] else np.uint8) or p.ndim != 2:
+                raise ValueError(f"plane {k} of a YUV frame is a 2-D uint8 array")
+            if p.shape[0] < 1 or p.shape[1] < 1:
+                raise ValueError("a YUV frame is empty")
+            row, col = p.stride() if cuda[k] else p.strides  # bytes and elements agree for uint8
+            if col != 1 or (p.shape[0] > 1 and row < p.shape[1]):
+                raise ValueError(f"plane {k} of a YUV frame needs rows of contiguous bytes, stride (pitch, 1) with pitch "
+                                 f">= its {p.shape[1]} bytes per row (it has {(row, col)})")
+        H, W = int(planes[0].shape[0]), int(planes[0].shape[1]) // (2 if format == "yuyv" else 1)
+        if W % 2 or (format != "yuyv" and H % 2):
+            raise ValueError(f"a {format} frame needs an even {'width' if format == 'yuyv' else 'height and width'} "
+                             f"(cv2.cvtColor refuses {H}x{W})")
+        want = [shape for _, shape in _yuv_layout(format, H, W)]
+        got = [tuple(int(d) for d in p.shape) for p in planes]
+        if got != want:
+            raise ValueError(f"the planes of a {H}x{W} {format} frame are {want}, not {got}")
+        self.format, self.planes, self.height, self.width = format, planes, H, W
+        self.device = planes[0].device.index if cuda[0] else None
+
+    def to_bgr(self) -> np.ndarray:
+        """``cv2.cvtColor`` of a host frame, on cv2's single-array layout (``[H*3/2, W]`` or ``[H, W, 2]``)."""
+        import cv2
+        if self.device is not None:
+            raise ValueError("to_bgr converts a host frame: its planes are CUDA tensors")
+        if self.format == "yuyv":
+            src = np.ascontiguousarray(self.planes[0]).reshape(self.height, self.width, 2)
+        else:
+            src = np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in self.planes])
+            src = src.reshape(self.height * 3 // 2, self.width)
+        return cv2.cvtColor(src, getattr(cv2, _YUV[self.format][0]))
+
+
+@dataclasses.dataclass(frozen=True)
+class _YUVKind:
+    """The tick-key kind of a ``YUVFrame``: its layout and whether its planes are CUDA tensors."""
+    format: str
+    cuda: bool
+
+
 def _align(n: int) -> int:
     return -(-int(n) // 256) * 256
 
 
 class _Tick:
     """One slot's buffers for one tick key, and the graph captured over them.  ``kinds``: per frame ``(H, W, kind)``,
-    kind False for a host image, True for a CUDA image, a ``JPEG_FORMAT`` tuple for JPEG bytes; ``caps``: per frame
-    its capacity in bytes (0 for an image); ``recs``: per frame its parsed JPEG record or None."""
+    kind False for a host image, True for a CUDA image, a ``JPEG_FORMAT`` tuple for JPEG bytes, a ``_YUVKind`` for a
+    ``YUVFrame``; ``caps``: per frame its capacity in bytes (0 for the others); ``recs``: per frame its parsed JPEG
+    record or None."""
 
     def __init__(self, fs: "FrameStream", kinds: tuple, caps: list, recs: list):
         import torch
@@ -528,13 +612,24 @@ class _Tick:
                        (prenet_item(H, W, item[0], item[2], md) for item in items)]
                       for (H, W, _), items in zip(kinds, self.plan)]
         self.jpeg = [j for j, k in enumerate(kinds) if isinstance(k[2], tuple)]
-        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames (with
-        # input_stage="host" the pairs cv2 built go up instead)
+        self.yuv = [j for j, k in enumerate(kinds) if isinstance(k[2], _YUVKind)]
+        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames and host
+        # YUV frames' packed planes (with input_stage="host" the pairs cv2 built go up instead); a CUDA YUV frame's
+        # planes are copied into packed planes of their own
         self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
+        self.yuv_dev = {}
         for j, (H, W, kind) in enumerate(kinds):
-            if kind is not True and not host_stage:
-                self.at[j] = off
-                off = _align(off + (self.caps[j] if j in self.jpeg else H * W * 3))
+            if isinstance(kind, _YUVKind):
+                size = _yuv_bytes(kind.format, H, W)
+                if kind.cuda:
+                    self.yuv_dev[j] = torch.empty(size, dtype=torch.uint8, device=dev)
+                    continue
+            elif kind is True or host_stage:
+                continue
+            else:
+                size = self.caps[j] if j in self.jpeg else H * W * 3
+            self.at[j] = off
+            off = _align(off + size)
         self.up_host = torch.empty(off, dtype=torch.uint8, pin_memory=True)
         self.up = torch.empty(off, dtype=torch.uint8, device=dev)
         self.nbytes = [0] * len(kinds)
@@ -549,6 +644,15 @@ class _Tick:
             self.formats[jj]["data"] = self.up.data_ptr() + self.at[j]
             self.formats[jj]["out"] = self.images[j].data_ptr()
             self.formats[jj]["decode_status"] = self.status.data_ptr() + 4 * jj
+        self.yuv_members = np.zeros(len(self.yuv), YUV_MEMBER)  # every address is the slot's own
+        for jj, j in enumerate(self.yuv):
+            H, W, kind = kinds[j]
+            base = self.yuv_dev[j].data_ptr() if kind.cuda else self.up.data_ptr() + self.at[j]
+            m = self.yuv_members[jj]
+            m["format"], m["height"], m["width"] = _YUV[kind.format][1], H, W
+            for k, (o, (_, w)) in enumerate(_yuv_layout(kind.format, H, W)):
+                m["planes"][k], m["pitches"][k] = base + o, w
+            m["out"], m["out_pitch"] = self.images[j].data_ptr(), 3 * W
         self.inputs = {size: torch.empty((2 * len(members),) + size + (3,), dtype=torch.float32, device=dev)
                        for size, members in self.buckets.items()}
         self.pairs = {size: torch.empty(x.shape, dtype=torch.float32, pin_memory=True)
@@ -569,24 +673,26 @@ class _Tick:
 class FrameStream:
     """Frames posed at the GPU's rate: ``predict`` + ``group`` per frame, replayed from a CUDA graph per tick of frames.
 
-    ``submit(frame)`` takes a ``[H, W, 3]`` uint8 BGR frame (numpy, or a CUDA tensor on the stream's device) or a JPEG
-    file's bytes and returns a ticket; ``submit_many(frames)`` takes a tick of several and returns one ticket each.
-    ``result(ticket)`` returns ``process()``'s value for that frame (evaluate.py:523-543), the
+    ``submit(frame)`` takes a ``[H, W, 3]`` uint8 BGR frame (numpy, or a CUDA tensor on the stream's device), a JPEG
+    file's bytes or a ``YUVFrame`` and returns a ticket; ``submit_many(frames)`` takes a tick of several and returns
+    one ticket each.  ``result(ticket)`` returns ``process()``'s value for that frame (evaluate.py:523-543), the
     ``[([17 x (x, y)], score)]`` of ``predict_many``: equal, value for value and type for type, to ``keypoints`` of
     ``group`` on the maps ``predict`` gives for the frame.  ``submit`` poses a tick of one frame and ``submit_many`` a
     tick of several, through the same calls.
 
     A tick holds one slot.  The slot keeps one CUDA graph per **tick key**: each frame's shape and kind (host image,
-    CUDA image, or JPEG format) in order.  The key's first tick in a slot runs call by call -- it is the key's warm-up
-    (the network's lazy set-up, cuDNN's choices) -- and the slot then captures the graph over its buffers for that key;
-    every later tick of that key in that slot is one graph launch.  The graph holds one upload from the slot's pinned
-    buffer of the tick's host frames, JPEG bytes and parsed records; ``spg_jpeg_decode_frames`` for every JPEG frame;
+    CUDA image, JPEG format, or YUV layout on the host or on the device) in order.  The key's first tick in a slot runs
+    call by call -- it is the key's warm-up (the network's lazy set-up, cuDNN's choices) -- and the slot then captures
+    the graph over its buffers for that key; every later tick of that key in that slot is one graph launch.  The graph
+    holds one upload from the slot's pinned buffer of the tick's host frames, host YUV planes, JPEG bytes and parsed
+    records; ``spg_jpeg_decode_frames`` for every JPEG frame; one ``spg_yuv_to_bgr`` for every YUV frame;
     ``spg_prenet_ragged`` for every item of ``scale_search x rotation_search`` of every frame, into one input tensor per
     network input size (``input_stage="host"``: the upload of the pairs cv2 built on the host instead); the forward
     passes; ``spg_postnet_ragged_items``; ``spg_group_ragged`` writing each frame's wire record; and one copy of the
-    records and JPEG statuses into pinned host memory.  A CUDA frame is copied into the slot's device image ahead of the
-    graph.  The graphs share one memory pool: they replay one at a time on the stream's own CUDA stream, and nothing
-    allocated inside a capture outlives it.
+    records and JPEG statuses into pinned host memory.  A CUDA frame is copied into the slot's device image, and a CUDA
+    YUV frame's planes into the slot's packed planes, ahead of the graph, so a graph never holds a caller's address.
+    The graphs share one memory pool: they replay one at a time on the stream's own CUDA stream, and nothing allocated
+    inside a capture outlives it.
 
     A tick of one frame forwards each item alone, as ``predict`` does, so ``submit`` equals ``predict`` + ``group``
     with any network.  A larger tick forwards each input size's items at once: every kernel treats each frame on its
@@ -607,6 +713,11 @@ class FrameStream:
     in the same slot, so a JPEG frame's result is always the one for ``cv2.imdecode(bytes, IMREAD_COLOR)``.
     ``host_decodes`` counts the JPEG frames ``cv2.imdecode`` decoded; with ``input_stage="host"`` that is every JPEG
     frame, decoded at submit.  Bytes cv2 cannot decode either raise ``ValueError``.
+
+    A ``YUVFrame`` (NV12, I420 or YUYV planes, numpy or CUDA, rows possibly pitched) is converted inside the graph into
+    the slot's device image, bit-identical to ``cv2.cvtColor(frame, COLOR_YUV2BGR_*)``: a host frame goes up packed at
+    1.5 (NV12, I420) or 2 (YUYV) bytes per pixel.  With ``input_stage="host"`` a host YUV frame is converted with
+    ``cv2.cvtColor`` at submit and posed as an image.  Either way its result is the one for cv2's image.
 
     ``slots`` ticks are in flight at most; each call to ``submit`` or ``submit_many`` takes the next slot in turn.  A
     slot owns its inputs, maps and records until its tick is finished, so the host stages tick k+1 while tick k's graph
@@ -661,8 +772,8 @@ class FrameStream:
 
     def submit(self, frame) -> int:
         """Pose ``frame`` as a tick of one frame in the next slot and return its ticket.  ``frame`` is a ``[H, W, 3]``
-        uint8 BGR image (numpy, or a CUDA tensor on the stream's device) or a JPEG file's bytes.  ``submit(f)`` and
-        ``submit_many([f])`` form the same tick key, so in one slot they share one graph."""
+        uint8 BGR image (numpy, or a CUDA tensor on the stream's device), a JPEG file's bytes or a ``YUVFrame``.
+        ``submit(f)`` and ``submit_many([f])`` form the same tick key, so in one slot they share one graph."""
         return self._submit([self._frame_of(frame)])[0]
 
     def submit_many(self, frames) -> List[int]:
@@ -683,9 +794,18 @@ class FrameStream:
     def _frame_of(self, frame):
         """A submitted frame checked: ``(frame, rec, decoded)`` -- a JPEG file the parser takes as its bytes (uint8
         array) and parsed record, any other JPEG file as cv2's image of it (also ``decoded``; counted in
-        ``host_decodes``), an image as a contiguous uint8 array or the CUDA tensor it is, with ``rec`` None."""
+        ``host_decodes``), a ``YUVFrame`` as it is (``input_stage="host"``: as cv2's image of it, also ``decoded``), an
+        image as a contiguous uint8 array or the CUDA tensor it is, with ``rec`` None."""
         import torch
         decoded = rec = None
+        if isinstance(frame, YUVFrame):
+            if frame.device is not None and self.input_stage == "host":
+                raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
+            if frame.device is not None and frame.device != self.device:
+                raise ValueError(f"a CUDA YUV frame's planes are on cuda:{self.device}, not cuda:{frame.device}")
+            if self.input_stage == "device":
+                return frame, None, None
+            frame = decoded = frame.to_bgr()
         if isinstance(frame, (bytes, bytearray, memoryview)):
             data = np.frombuffer(frame, np.uint8)
             if data.size == 0:
@@ -713,6 +833,8 @@ class FrameStream:
         """Launch a tick of checked frames (``_frame_of``) in the next slot; returns its tickets."""
         import torch
         kinds = tuple((int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)) if rec is not None
+                      else (frame.height, frame.width, _YUVKind(frame.format, frame.device is not None))
+                      if isinstance(frame, YUVFrame)
                       else (int(frame.shape[0]), int(frame.shape[1]), isinstance(frame, torch.Tensor))
                       for frame, rec, _ in staged)
         slot = self._calls % len(self._busy)
@@ -763,6 +885,18 @@ class FrameStream:
                 for k in ("data", "out", "decode_status"):  # the tick's device addresses, as the format's
                     rec[k] = tk.formats[jj][k]
                 host[jj * JPEG_RECORD.itemsize:(jj + 1) * JPEG_RECORD.itemsize] = np.frombuffer(rec.tobytes(), np.uint8)
+            elif isinstance(kind, _YUVKind):  # the planes packed, in the upload or in the slot's device planes
+                layout = _yuv_layout(kind.format, H, W)
+                if kind.cuda:
+                    self._stream.wait_stream(torch.cuda.current_stream(self.device))
+                    with torch.cuda.stream(self._stream):
+                        for p, (o, (h, w)) in zip(frame.planes, layout):
+                            tk.yuv_dev[j][o:o + h * w].view(h, w).copy_(p, non_blocking=True)
+                    for p in frame.planes:
+                        p.record_stream(self._stream)
+                else:
+                    for p, (o, (h, w)) in zip(frame.planes, layout):
+                        host[tk.at[j] + o:tk.at[j] + o + h * w].reshape(h, w)[:] = p
             elif kind:
                 self._stream.wait_stream(torch.cuda.current_stream(self.device))
                 with torch.cuda.stream(self._stream):
@@ -797,6 +931,8 @@ class FrameStream:
             if tk.jpeg:
                 g.jpeg_decode_frames(tk.up.data_ptr(), tk.formats, [tk.caps[j] for j in tk.jpeg])
                 tk.status_host.copy_(tk.status, non_blocking=True)
+            if tk.yuv:
+                g.yuv_to_bgr(tk.yuv_members)
             members, outs = [], []
             for size, ms in tk.buckets.items():
                 for k, (i, t) in enumerate(ms):
@@ -858,8 +994,8 @@ class FrameStream:
                 again, d = self._launch(slot, ((image.shape[0], image.shape[1], False),), [(image, None, image)])
                 d.synchronize()
                 record, heat, paf = again.rec_host[0].numpy().copy(), again.heat[0].clone(), again.paf[0].clone()
-            elif j in tk.jpeg:
-                image = tk.images[j]  # decoded on the device: copied to the host if detail asks for it
+            elif j in tk.jpeg or j in tk.yuv:
+                image = tk.images[j]  # decoded or converted on the device: copied to the host if detail asks for it
             self._keep(ticket, record, heat, paf, tk.kinds[j][0], tk.as_f64)
             self._held[ticket] = (heat, paf, tk.as_f64, image)
             tk.held.append(ticket)

@@ -150,6 +150,13 @@ JPEG_RECORD = np.dtype([(f, np.int32) for f in ("status", "orientation", "height
                         ("dc", JPEG_HUFF, (3,)), ("ac", JPEG_HUFF, (3,)), ("data", np.uint64), ("out", np.uint64),
                         ("decode_status", np.uint64)], align=True)
 
+#: ``spg_yuv_member`` (include/spgroup.h): one YUV frame of ``spg_yuv_to_bgr`` -- its format (``YUV_NV12``,
+#: ``YUV_I420``, ``YUV_YUYV``), size, up to three device planes with their row pitches in bytes, and its device BGR output
+YUV_NV12, YUV_I420, YUV_YUYV = 1, 2, 3
+YUV_MEMBER = np.dtype([("format", np.int32), ("height", np.int32), ("width", np.int32), ("reserved", np.int32),
+                       ("planes", np.uint64, (3,)), ("pitches", np.int64, (3,)), ("out", np.uint64),
+                       ("out_pitch", np.int64)], align=True)
+
 
 def jpeg_parse(data) -> np.ndarray:
     """``spg_jpeg_parse`` of one file's bytes (host only): a ``JPEG_RECORD`` whose ``status`` is ``JPEG_OK`` or the
@@ -218,6 +225,7 @@ _PROTOTYPES = {
     # device_records: a device JPEG_RECORD array; formats: a JPEG_RECORD array; capacities: an int64 array
     "spg_jpeg_decode_frames": (_int, [_ptr, _ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_jpeg_reserve_frames": (_int, [_ptr, _ptr, _ptr, _i32, _P(C.c_int32)]),
+    "spg_yuv_to_bgr": (_int, [_ptr, _ptr, _i32, _ptr]),  # members: a YUV_MEMBER array
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -1097,6 +1105,14 @@ class Grouper:
     def jpeg_kernel(self) -> str:
         """Name of the kernel the last JPEG decode launched."""
         return (self._lib.spg_stage_kernel(self._h, 9) or b"").decode()
+
+    # -- YUV frames (dropin.FrameStream builds the records) -------------------------------------------------------
+    def yuv_to_bgr(self, members: np.ndarray, stream=None) -> None:
+        """``spg_yuv_to_bgr``: ``members`` a ``YUV_MEMBER`` array; each frame's planes are converted into its BGR
+        output as ``cv2.cvtColor`` converts them.  Asynchronous on ``stream``; can be recorded into a CUDA graph."""
+        s = self._records(members, YUV_MEMBER)
+        _check(self._lib.spg_yuv_to_bgr(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)), "spg_yuv_to_bgr",
+               self._h)
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

@@ -325,7 +325,7 @@ int spg_prenet_ragged(spg_handle *h, int32_t max_downsample, int32_t pad_value, 
  *
  * spg_jpeg_decode_frame (below) is the JPEG decode of one frame in a form that can be recorded: its graph serves every
  * frame of one format, and spg_jpeg_reserve_frame grows its scratch for a format and a capacity ahead of the capture,
- * with *moved as here. */
+ * with *moved as here.  spg_yuv_to_bgr (below) can be recorded as it is: it has no scratch to reserve. */
 int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_downsample, const spg_prenet_item *items,
                       int32_t n_items, int32_t stride, int32_t *moved);
 /* Several frames in one graph (a tick): spg_prenet_ragged, spg_postnet_ragged_items and spg_group_ragged (with or without
@@ -339,6 +339,32 @@ int spg_reserve_frame(spg_handle *h, int32_t height, int32_t width, int32_t max_
  * while any stream of the device captures. */
 int spg_reserve_frames(spg_handle *h, int32_t max_downsample, const spg_prenet_member *members, int32_t n_images,
                        int32_t n_items, int32_t *moved);
+
+/* ---- YUV frames: cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420 / _YUYV) ----------------------------------------- */
+enum {
+    SPG_YUV_NV12 = 1,  /* planes[0] Y [height][width], planes[1] interleaved U, V [height / 2][width] */
+    SPG_YUV_I420 = 2,  /* planes[0] Y [height][width], planes[1] U and planes[2] V [height / 2][width / 2] */
+    SPG_YUV_YUYV = 3   /* planes[0] Y0 U Y1 V [height][2 * width] (packed 4:2:2) */
+};
+/* One frame of spg_yuv_to_bgr: its planes (device memory, rows pitches[k] bytes apart; the planes a format does not use
+ * are not read) and its [height][width][3] uint8 BGR output (device, rows out_pitch bytes apart). */
+typedef struct spg_yuv_member {
+    int32_t format;             /* SPG_YUV_NV12, SPG_YUV_I420 or SPG_YUV_YUYV */
+    int32_t height, width;      /* even for NV12 and I420; width even for YUYV (cv2 refuses the others) */
+    int32_t reserved;           /* 0 */
+    const uint8_t *planes[3];
+    int64_t pitches[3];         /* >= each plane's row bytes */
+    uint8_t *out;
+    int64_t out_pitch;          /* >= 3 * width */
+} spg_yuv_member;
+/* Per member, OpenCV's integer BT.601 limited-range conversion, bit for bit with cv2.cvtColor: with y = max(0, Y - 16)
+ * * 1220542 and r = 1 << 19, B = (y + r + 2116026 (U - 128)) >> 20, G = (y + r - 409993 (U - 128) - 852492 (V - 128))
+ * >> 20 and R = (y + r + 1673527 (V - 128)) >> 20, each saturated to [0, 255]; a 2x2 block (4:2:0) or a 2x1 pair (4:2:2)
+ * shares its U and V.  Every member is validated before the first launch (SPG_E_INVALID names the first bad one as
+ * "member i").  Asynchronous on `stream`; `members` may be reused as soon as the call returns.  The call allocates
+ * nothing and never synchronises, and its launches depend on the members alone, so it can be recorded into a CUDA graph
+ * (see "frames recorded into a CUDA graph") and replayed with new contents in the same planes. */
+int spg_yuv_to_bgr(spg_handle *h, const spg_yuv_member *members, int32_t n, void *stream);
 
 /* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
