@@ -2,6 +2,7 @@
 per rule, and against pycocotools itself where it is installed."""
 import contextlib
 import copy
+import functools
 import io
 import math
 
@@ -16,7 +17,7 @@ T = 10  # thresholds
 
 
 def _run(name):
-    ds, res, setup = cases.CASES[name]()
+    ds, res, setup = (cases.CASES | cases.CROWD_CASES)[name]()
     c = cocoeval.COCO()
     c.dataset = copy.deepcopy(ds)
     c.createIndex()
@@ -148,11 +149,9 @@ def test_every_case_runs():
         assert _run(name).stats.shape == (10,)
 
 
-@pytest.mark.parametrize("seed, n", [(1, 37), (2, 200)])
-def test_port_matches_pycocotools(seed, n):
+def _against_pycocotools(ds, res, setup=None):
     pc = pytest.importorskip("pycocotools.cocoeval")
     from pycocotools.coco import COCO
-    ds, res = synth.coco_keypoint_set(seed, n)
     gt = COCO()
     gt.dataset = copy.deepcopy(ds)
     gt.createIndex()
@@ -161,6 +160,8 @@ def test_port_matches_pycocotools(seed, n):
     mine = port.COCOevalPort(gt, dt)
     with contextlib.redirect_stdout(io.StringIO()):
         for e in (ref, mine):
+            if setup:
+                setup(e.params)
             e.evaluate()
             e.accumulate()
             e.summarize()
@@ -177,6 +178,24 @@ def test_port_matches_pycocotools(seed, n):
     assert np.array_equal(ref.stats, mine.stats)
 
 
+@pytest.mark.parametrize("seed, n", [(1, 37), (2, 200)])
+def test_port_matches_pycocotools(seed, n):
+    _against_pycocotools(*synth.coco_keypoint_set(seed, n))
+
+
+_CROWD_SETS = {"crowded_images": cases.crowded_images, "two_categories": cases.two_categories,
+               **cases.CROWD_CASES,
+               **{f"keypoints_{k}": functools.partial(cases.keypoint_count, k) for k in cases.SIGMA_COUNTS},
+               **{f"{name}_{where}": functools.partial(cases.param_set, name, where)
+                  for name in cases.PARAM_SETS for where in ("seeded", "crowded")}}
+
+
+@pytest.mark.parametrize("name", sorted(_CROWD_SETS))
+def test_port_matches_pycocotools_past_one_warp(name):
+    """The crowded sets, the step-edge cases and the user-set parameters of tests/test_gpu_cocoeval_crowd.py."""
+    _against_pycocotools(*_CROWD_SETS[name]())
+
+
 def test_categories_are_accumulated_on_their_own():
     e = _run("categories")
     assert e.params.catIds == [1, 2, 3] and e.eval['counts'][2] == 3
@@ -189,3 +208,81 @@ def test_categories_are_accumulated_on_their_own():
     assert s.params.catIds == [1, 3] and s.eval['counts'][2] == 2
     assert np.array_equal(s.eval['precision'][:, :, 1], e.eval['precision'][:, :, 2])
     assert [x['category_id'] for x in s.evalImgs if x] == [1] * 6 + [3] * 6
+
+
+# -- past one warp of ground truths: the device matcher's 32-ground-truth steps ----------------------------------------
+
+def test_ties_across_steps_go_to_the_later_ground_truth():
+    e = _run("dup_across_steps")
+    assert set(np.unique(e.ious[1, 1]).tolist()) == {0.0, 1.0}
+    x = _img(e, 1)
+    assert x['gtIds'] == list(range(1, 71))
+    # positions (5, 37), (31, 32), (0, 64): the later one first, then the earlier one; ids are positions + 1
+    assert (x['dtMatches'] == np.array([38, 6, 33, 32, 65, 1])).all()
+    m = x['gtMatches']
+    assert (m[:, [37, 5, 32, 31, 64, 0]] == np.arange(1, 7)).all() and np.count_nonzero(m) == 6 * T
+
+
+def test_an_earlier_step_maximum_holds_against_a_smaller_later_one():
+    e = _run("earlier_max")
+    m = e.ious[1, 1]
+    assert m[0, 3] == 1.0 and m[0, 36] == 16 / 17 and np.count_nonzero(m[0]) == 2
+    x = _img(e, 1)
+    assert (x['dtMatches'][:, 0] == 4).all(), "OKS 1.0 at position 3 is kept against 16/17 at position 36"
+    assert x['dtMatches'][:, 1].tolist() == [37] * 9 + [0], "16/17 at position 36 matches up to threshold 0.9"
+
+
+def test_nan_oks_at_the_edges_of_a_step():
+    e = _run("nan_steps")
+    for img, q in ((1, 31), (2, 32), (3, 63)):
+        m = e.ious[img, 1]
+        assert np.isnan(m[:, q]).all() and np.isnan(m).sum() == 2
+        assert m[0, 10] == 1.0 and m[0, q + 8] == 16 / 17
+        x = _img(e, img)
+        ids = x['gtIds']
+        assert ids == list(range(72 * (img - 1) + 1, 72 * img + 1))
+        # the NaN at q replaces OKS 1.0 at position 10; from there every ground truth is taken up to the 16/17
+        assert (x['dtMatches'][:, 0] == ids[q + 8]).all(), q
+        # the next detection: 16/17 taken, so OKS 0.0 carries the match on to the last free ground truth
+        assert (x['dtMatches'][:, 1] == ids[71 if q + 8 < 71 else 70]).all(), q
+        assert not x['dtIgnore'].any()
+
+
+def test_a_matched_ground_truth_past_32_is_skipped():
+    e = _run("taken_past_32")
+    x = _img(e, 1)
+    assert (x['dtMatches'][:, 0] == 36).all()
+    assert x['dtMatches'][:, 1].tolist() == [39] * 9 + [0], "position 35 is taken: on to 16/17 at position 38"
+    assert (x['dtMatches'][:, 2] == 0).all()
+    assert (x['gtMatches'][:, 35] == 1).all()
+
+
+def test_a_crowd_region_past_32_takes_several_detections():
+    e = _run("crowd_past_32")
+    assert [g['id'] for g in e._gts[1, 1]].index(100) == 34, "the crowd is in the second step of annotation order"
+    x = _img(e, 1)
+    assert x['gtIds'] == list(range(1, 37)) + [100] and x['gtIgnore'].tolist() == [0] * 36 + [1]
+    assert (x['dtMatches'] == np.array([8, 100, 100, 100, 0])).all()
+    assert (x['dtIgnore'] == np.array([False, True, True, True, False])).all()
+    assert (x['gtMatches'][:, 36] == 4).all(), "the crowd keeps the last detection's id"
+    assert (e.eval['recall'][:, 0, 0, 0] == 1 / 36).all()
+
+
+def test_the_scan_breaks_at_an_ignored_ground_truth_past_32():
+    e = _run("break_past_32")
+    ids = [g['id'] for g in e._gts[1, 1]]
+    assert [ids.index(i) for i in (101, 102, 103)] == [33, 38, 42], "annotation indices past the first step"
+    x = _img(e, 1)
+    assert x['gtIds'] == list(range(1, 41)) + [101, 102, 103]
+    assert x['gtIgnore'].tolist() == [0] * 40 + [1] * 3
+    assert e.ious[1, 1][0].tolist().count(1.0) == 2, "ground truths 21 and 101 tie at OKS 1.0"
+    assert (x['dtMatches'] == np.array([21, 102, 0, 101])).all()
+    assert (x['dtIgnore'] == np.array([False, True, False, True])).all()
+
+
+def test_iou_thresholds_zero_and_one():
+    e = _run("iou_thr_edges")
+    x = _img(e, 1)
+    assert e.params.iouThrs.tolist() == [0.0, 0.5, 1.0]
+    assert x['dtMatches'].tolist() == [[13, 26, 40, 39], [13, 26, 0, 0], [13, 0, 0, 0]]
+    assert e.eval['recall'][:, 0, 0, 0].tolist() == [4 / 40, 2 / 40, 1 / 40]
