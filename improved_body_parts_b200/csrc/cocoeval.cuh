@@ -1,7 +1,7 @@
 // cocoeval.cuh -- pycocotools' COCOeval for iouType='keypoints' (the metric evaluate.py:617-621 reports) on the device:
 // computeOks, evaluateImg and accumulate over every (category, image) unit at once.
 //
-// Inputs are the packed arrays of spg_coco_data (include/spgroup.h); spgroup.cu sorts the detections with CUB's stable
+// Inputs are the packed arrays of spg_coco_data (include/spgroup.h); cocoeval.cu sorts the detections with CUB's stable
 // radix sort on coco_score_key, which orders like numpy's mergesort of -score (NaN last, -0.0 == 0.0, ties in input
 // order).  Then:
 //   coco_oks_kernel:        one thread per OKS matrix entry (ragged over units).  The 17 terms are summed in numpy's

@@ -68,6 +68,7 @@ constexpr int kMaxCapPeaks = 128;    // peaks per (image, part); two 64-bit "use
 constexpr int kMaxCapRows = 128;     // subset rows per image; four 32-bit alive masks in assemble
 constexpr int kMaxRefineRadius = 4;  // (2r+1)^2 <= 81 <= numpy's 128-element pairwise block
 constexpr int kMaxOutJoints = 32;
+constexpr int kMAMatchWarps = 7;   // matcher warps of match_assemble_kernel by default; the launch may use 1..15 (blockDim.x = 32 * (1 + matchers))
 
 // status bits, identical to SPG_ST_* in include/spgroup.h
 constexpr uint32_t kStPeakOverflow = 1u << 0;

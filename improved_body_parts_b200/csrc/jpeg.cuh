@@ -36,9 +36,8 @@
 // runs the same count to write kernels with grids sized for a capacity in scan bytes; they read the frame's segment
 // address and length from its device record at run time, and the CTAs past the frame's work return (jpeg_kernels.cuh).
 //
-// The kernels are compiled in translation units of their own, jpeg.cu and jpeg_frame.cu, which spgroup.cu calls through
-// jpeg_launch: in spgroup.cu's module their presence changed how nvcc optimised match_assemble_kernel, and in their own
-// every kernel that existed before them keeps its SASS.  This header is what they share.
+// jpeg.cu compiles the kernels and holds the host code; jpeg_frame.cu compiles the frame form's kernels with the frame
+// macros, in a module of their own, and exports them as kJpegFrameKernels.  This header is what the two share.
 #pragma once
 
 #include "../../include/spgroup.h"
@@ -98,10 +97,7 @@ constexpr int kJpegBlock[kJpegKernels] = {kJpegPackThreads, kJpegPackThreads, kJ
                                           kJpegSubThreads, kJpegThreads, kJpegThreads, kJpegThreads,
                                           kJpegPackThreads, kJpegPackThreads, kJpegPackThreads, kJpegThreads, kJpegSubThreads, kJpegThreads,
                                           kJpegSubThreads};
-extern const char *const kJpegKernelName[kJpegKernels];
-// one launch of kernel k over `grid` CTAs with member table r on stream st (jpeg.cu; the frame form's kernels through
-// jpeg_frame_launch, jpeg_frame.cu); returns cudaGetLastError()
-cudaError_t jpeg_launch(JpegKernel k, unsigned grid, cudaStream_t st, const JpegRagged &r);
-cudaError_t jpeg_frame_launch(JpegKernel k, unsigned grid, cudaStream_t st, const JpegRagged &r);
+// the frame form's kernels, kJpegCountFrame to kJpegWriteFrame (jpeg_frame.cu)
+extern void (*const kJpegFrameKernels[kJpegKernels - kJpegCountFrame])(JpegRagged);
 
 }  // namespace spg

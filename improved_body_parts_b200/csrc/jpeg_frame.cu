@@ -1,5 +1,5 @@
-// jpeg_frame.cu -- the frame form of the JPEG decoder's count to write kernels (spg_jpeg_decode_frame; jpeg_kernels.cuh
-// holds their source) and their launch, a translation unit of its own so that jpeg.cu's kernels keep their code.
+// jpeg_frame.cu -- the frame form of the JPEG decoder's count to write kernels (spg_jpeg_decode_frames; jpeg_kernels.cuh
+// holds their source), compiled with the frame macros in a unit of their own; jpeg.cu launches them by kJpegFrameKernels.
 #include "jpeg.cuh"
 
 namespace spg {
@@ -34,12 +34,8 @@ __device__ __forceinline__ JpegMember jpeg_framed(const JpegMember &cap) {
 
 namespace spg {
 
-cudaError_t jpeg_frame_launch(JpegKernel k, unsigned grid, cudaStream_t st, const JpegRagged &r) {
-    void (*const kern[kJpegKernels - kJpegCountFrame])(JpegRagged) = {
-        jpeg_count_frame_kernel, jpeg_prefix_frame_kernel, jpeg_pack_frame_kernel, jpeg_interval_frame_kernel,
-        jpeg_sync_frame_kernel,  jpeg_fixup_frame_kernel,  jpeg_write_frame_kernel};
-    kern[k - kJpegCountFrame]<<<grid, kJpegBlock[k], 0, st>>>(r);
-    return cudaGetLastError();
-}
+void (*const kJpegFrameKernels[kJpegKernels - kJpegCountFrame])(JpegRagged) = {
+    jpeg_count_frame_kernel, jpeg_prefix_frame_kernel, jpeg_pack_frame_kernel, jpeg_interval_frame_kernel,
+    jpeg_sync_frame_kernel,  jpeg_fixup_frame_kernel,  jpeg_write_frame_kernel};
 
 }  // namespace spg

@@ -16,7 +16,6 @@
 
 namespace spg {
 
-constexpr int kMAMatchWarps = 7;   // default; the launch may use 1..15 (blockDim.x = 32 * (1 + matchers))
 constexpr int kMAThreads = 32 * (1 + kMAMatchWarps);
 constexpr int kMAMaxThreads = 512;
 

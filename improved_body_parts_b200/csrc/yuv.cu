@@ -1,4 +1,6 @@
-// yuv.cu -- yuv_to_bgr_kernel (spg_yuv_to_bgr; yuv.cuh describes it) and its launch, a translation unit of its own.
+// yuv.cu -- spg_yuv_to_bgr and its kernel, yuv_to_bgr_kernel (yuv.cuh describes it).
+#include "runtime.cuh"
+
 #include "yuv.cuh"
 
 namespace spg {
@@ -49,9 +51,64 @@ __global__ void __launch_bounds__(kYuvThreads) yuv_to_bgr_kernel(const __grid_co
     }
 }
 
-cudaError_t yuv_launch(unsigned grid, cudaStream_t st, const YuvRagged &r) {
-    yuv_to_bgr_kernel<<<grid, kYuvThreads, 0, st>>>(r);
-    return cudaGetLastError();
+}  // namespace spg
+
+using namespace spg;
+
+extern "C" {
+
+int spg_yuv_to_bgr(spg_handle *h, const spg_yuv_member *members, int32_t n, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    if (n < 0 || (n > 0 && !members)) return fail(h, SPG_E_INVALID, "members is NULL or n negative");
+    std::vector<YuvMember> ms((size_t)n);
+    std::vector<long long> ctas((size_t)n);
+    for (int i = 0; i < n; i++) {  // validate every member before the first launch
+        const spg_yuv_member &s = members[i];
+        const int H = s.height, W = s.width, f = s.format;
+        if (f != SPG_YUV_NV12 && f != SPG_YUV_I420 && f != SPG_YUV_YUYV)
+            return fail(h, SPG_E_INVALID, "member %d: format %d is not SPG_YUV_NV12, SPG_YUV_I420 or SPG_YUV_YUYV", i, f);
+        if (s.reserved != 0) return fail(h, SPG_E_INVALID, "member %d: reserved must be 0", i);
+        if (H < 1 || W < 1 || H > 32767 || W > 32767) return fail(h, SPG_E_INVALID, "member %d: frame %dx%d outside [1, 32767]", i, H, W);
+        if (W % 2 != 0 || (f != SPG_YUV_YUYV && H % 2 != 0))
+            return fail(h, SPG_E_INVALID, "member %d: a %s frame needs an even %s (got %dx%d)", i, f == SPG_YUV_YUYV ? "YUYV" : "4:2:0",
+                        f == SPG_YUV_YUYV ? "width" : "height and width", H, W);
+        const int n_planes = f == SPG_YUV_NV12 ? 2 : (f == SPG_YUV_I420 ? 3 : 1);
+        const long long row[3] = {f == SPG_YUV_YUYV ? 2LL * W : W, f == SPG_YUV_NV12 ? W : W / 2, W / 2};
+        YuvMember m{};
+        for (int k = 0; k < n_planes; k++) {
+            if (!s.planes[k]) return fail(h, SPG_E_INVALID, "member %d: plane %d is NULL", i, k);
+            if (s.pitches[k] < row[k])
+                return fail(h, SPG_E_INVALID, "member %d: plane %d's pitch %lld is below its row's %lld bytes", i, k,
+                            (long long)s.pitches[k], row[k]);
+            m.plane[k] = s.planes[k];
+            m.pitch[k] = s.pitches[k];
+        }
+        if (!s.out) return fail(h, SPG_E_INVALID, "member %d: out is NULL", i);
+        if (s.out_pitch < 3LL * W)
+            return fail(h, SPG_E_INVALID, "member %d: out_pitch %lld is below the row's %lld bytes", i, (long long)s.out_pitch, 3LL * W);
+        m.out = s.out;
+        m.out_pitch = s.out_pitch;
+        m.format = f;
+        m.h = H;
+        m.w = W;
+        m.units = W / 2;
+        ms[i] = m;
+        ctas[i] = ((long long)(f == SPG_YUV_YUYV ? H : H / 2) * m.units + kYuvThreads - 1) / kYuvThreads;
+    }
+    if (ms.empty()) return SPG_OK;
+    std::vector<RaggedRange> ranges;
+    std::vector<int> first;
+    int rc;
+    if ((rc = deal_ragged(h, ctas, kYuvTableMax, "member", nullptr, ranges, first))) return rc;
+    DeviceGuard guard(h->device);
+    YuvRagged table{};
+    for (const RaggedRange &g : ranges) {
+        fill_table(table, ms, first, g);
+        if ((rc = launch(h, kStageYuv, "yuv_to_bgr_kernel", yuv_to_bgr_kernel, dim3(g.ctas), kYuvThreads, 0,
+                         static_cast<cudaStream_t>(stream), table)))
+            return rc;
+    }
+    return SPG_OK;
 }
 
-}  // namespace spg
+}  // extern "C"

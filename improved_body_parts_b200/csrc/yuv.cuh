@@ -2,9 +2,6 @@
 // with OpenCV's integer BT.601 limited-range formula, bit for bit.  One ragged launch per call: the member table travels
 // as a __grid_constant__ parameter and a CTA finds its frame by binary search over first_cta (ragged_member).  A thread
 // converts one 2x2 block of a 4:2:0 frame, or one 2x1 pair of a 4:2:2 frame, which share one U and one V.
-//
-// The kernel is compiled in a translation unit of its own, yuv.cu, which spgroup.cu calls through yuv_launch, so that
-// every kernel of spgroup.cu's module keeps its code (as jpeg.cuh explains for the JPEG decoder).
 #pragma once
 
 #include "../../include/spgroup.h"
@@ -31,8 +28,5 @@ struct YuvRagged {
     YuvMember img[kYuvTableMax];  // first_cta increasing
 };
 static_assert(sizeof(YuvRagged) <= kParamBytes, "a launch's parameters fit the kernel-parameter limit");
-
-// one launch of yuv_to_bgr_kernel over `grid` CTAs with member table r on stream st (yuv.cu); returns cudaGetLastError()
-cudaError_t yuv_launch(unsigned grid, cudaStream_t st, const YuvRagged &r);
 
 }  // namespace spg

@@ -160,11 +160,31 @@ def test_environment_is_read_only_in_spg_create():
     assert b"SPG_DEBUG" not in blob
     for name in (b"SPG_PERSIST", b"SPG_NO_SCREEN", b"SPG_EXACT_WARPS"):
         assert name in blob
-    src = open(os.path.join(ROOT, "improved_body_parts_b200", "csrc", "spgroup.cu")).read()
+    csrc = os.path.join(ROOT, "improved_body_parts_b200", "csrc")
+    src = open(os.path.join(csrc, "spgroup.cu")).read()
     body = src.split("int spg_create(")[1].split("\nvoid spg_destroy")[0]
-    outside = src.replace(body, "")
     assert body.count("getenv(") >= 3
-    assert "getenv(" not in outside
-    for name in os.listdir(os.path.join(ROOT, "improved_body_parts_b200", "csrc")):
-        if name.endswith(".cuh"):
-            assert "getenv(" not in open(os.path.join(ROOT, "improved_body_parts_b200", "csrc", name)).read(), name
+    for name in os.listdir(csrc):
+        if name.endswith((".cu", ".cuh")):
+            txt = open(os.path.join(csrc, name)).read()
+            assert "getenv(" not in (txt.replace(body, "") if name == "spgroup.cu" else txt), name
+
+
+def test_every_handle_launch_goes_through_launch():
+    """launch() (runtime.cuh) is the one place a kernel is launched on a handle: it records the stage's kernel, counts the
+    launch and turns a launch error into the call's error.  The only other launches are the three handle-less wire
+    entry points' kernels in spgroup.cu."""
+    csrc = os.path.join(ROOT, "improved_body_parts_b200", "csrc")
+    runtime = open(os.path.join(csrc, "runtime.cuh")).read()
+    body = runtime.split("\nint launch(")[1].split("\n}\n")[0]
+    assert body.count("<<<") == 1
+    wire = ("int spg_wire_signal(", "int spg_wire_signal_many(", "int spg_wire_wait(")
+    spgroup = open(os.path.join(csrc, "spgroup.cu")).read()
+    for entry in wire:
+        fn = spgroup.split(entry)[1].split("\n}\n")[0]
+        assert fn.count("<<<") == 1, entry
+        spgroup = spgroup.replace(fn, "")
+    for name in os.listdir(csrc):
+        if name.endswith((".cu", ".cuh")):
+            txt = {"runtime.cuh": runtime.replace(body, ""), "spgroup.cu": spgroup}.get(name)
+            assert "<<<" not in (txt if txt is not None else open(os.path.join(csrc, name)).read()), name
