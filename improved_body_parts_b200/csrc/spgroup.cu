@@ -4,7 +4,7 @@
 // Each stage is a translation unit of its own, its kernels with its host code, so that each CUDA module holds one
 // stage's kernels and an edit to one stage cannot change another's code: group.cu (the grouping pass and its
 // capacity-free tier), postnet.cu (the post- and pre-network stages), train.cu (training samples and loss), cocoeval.cu,
-// jpeg.cu with jpeg_frame.cu, and yuv.cu.  No torch, no CPU implementation: if the device or a launch fails the call
+// jpeg.cu with jpeg_frame.cu, yuv.cu and track.cu.  No torch, no CPU implementation: if the device or a launch fails the call
 // fails.
 #include "runtime.cuh"
 

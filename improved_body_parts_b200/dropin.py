@@ -24,8 +24,8 @@ from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 import numpy as np
 
 from . import sharding, wire
-from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, YUV_I420, YUV_MEMBER, YUV_NV12, YUV_YUYV, Grouper, GroupingError,
-                       clamp_scale, input_geometry, jpeg_parse, prenet_item)
+from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, TRACK_FRAME, TRACK_TABLE, YUV_I420, YUV_MEMBER, YUV_NV12, YUV_YUYV,
+                       Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse, prenet_item)
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -589,6 +589,29 @@ class _YUVKind:
     cuda: bool
 
 
+@dataclasses.dataclass(frozen=True)
+class TrackParams:
+    """``FrameStream``'s tracking: ``streams`` tables of tracks (one per camera or video, frames name theirs with
+    ``submit(..., stream=s)``), the OKS at or above which a person may continue a track, and the frames of its stream a
+    track outlives unmatched (``include/spgroup.h`` "tracking" has the rules)."""
+    streams: int = 1
+    oks_threshold: float = 0.5
+    max_age: int = 30
+
+    def __post_init__(self):
+        for name in ("streams", "max_age"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError(f"TrackParams.{name} is an int, not {v!r}")
+        if not 1 <= self.streams < 1 << 31:
+            raise ValueError(f"TrackParams.streams must be in [1, 2^31), not {self.streams}")
+        if not 0 <= self.max_age < 1 << 31:
+            raise ValueError(f"TrackParams.max_age must be in [0, 2^31), not {self.max_age}")
+        t = self.oks_threshold
+        if isinstance(t, bool) or not isinstance(t, (int, float, np.integer, np.floating)) or not 0.0 <= float(t) <= 1.0:
+            raise ValueError(f"TrackParams.oks_threshold must be a number in [0, 1], not {t!r}")
+
+
 def _align(n: int) -> int:
     return -(-int(n) // 256) * 256
 
@@ -617,6 +640,9 @@ class _Tick:
         # YUV frames' packed planes (with input_stage="host" the pairs cv2 built go up instead); a CUDA YUV frame's
         # planes are copied into packed planes of their own
         self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
+        self.streams_at = None  # with tracking: the frames' stream indices (int32) in the upload
+        if fs._track is not None:
+            self.streams_at, off = off, _align(off + 4 * len(kinds))
         self.yuv_dev = {}
         for j, (H, W, kind) in enumerate(kinds):
             if isinstance(kind, _YUVKind):
@@ -664,6 +690,16 @@ class _Tick:
                     for H, W, _ in kinds]
         self.rec = torch.zeros((len(kinds), fs._g.wire_record_bytes()), dtype=torch.uint8, device=dev)
         self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
+        self.track = None
+        if fs._track is not None:  # per frame its people's ids, and its spg_track_frames member
+            self.ids = torch.empty((len(kinds), fs._g.capR), dtype=torch.int64, device=dev)
+            self.ids_host = torch.empty(self.ids.shape, dtype=torch.int64, pin_memory=True)
+            self.track = np.zeros(len(kinds), TRACK_FRAME)
+            for j in range(len(kinds)):
+                self.track[j]["record"] = self.rec[j].data_ptr()
+                self.track[j]["stream"] = self.up.data_ptr() + self.streams_at + 4 * j
+                self.track[j]["jpeg_status"] = self.status.data_ptr() + 4 * self.jpeg.index(j) if j in self.jpeg else 0
+                self.track[j]["ids"] = self.ids[j].data_ptr()
 
     def members(self):
         """Per frame, per item: ``(H, W, multiplier, angle)``, what ``Grouper.reserve_frames`` takes."""
@@ -727,15 +763,28 @@ class FrameStream:
     (``configure(variant=...)``), the limb table and the default device are those in effect at construction.  The
     network's output is ``model(x)[-1][0]``, as for ``predict``; the model must be capture-safe after its first call at
     a shape (no host synchronisation, no host-to-device copy).  A stride other than 4 raises ``ValueError``, a capture
-    that fails raises ``GroupingError``: there is no call-by-call fallback."""
+    that fails raises ``GroupingError``: there is no call-by-call fallback.
+
+    ``track=TrackParams(...)`` follows people across frames: each frame belongs to a stream (``submit(frame,
+    stream=s)``, ``submit_many(frames, streams=[...])``; stream 0 by default), and ``spg_track_frames``, recorded into
+    the graph after the grouping, matches the frame's people to its stream's tracks by OKS and gives each an id
+    (``result(ticket, ids=True)``).  Every graph replays on the stream's one CUDA stream in submit order, so a stream's
+    frames are tracked in submit order, also across slots in flight; the stream indices travel in the tick's upload, so
+    frames of any streams share a graph.  A frame whose record has a status bit (a crowded frame, whose people come from
+    the capacity-free tier, or a grouping error) or whose JPEG decode was flagged is unobserved: its stream's tracks age
+    and its people get id -1, also after the flagged frame is posed again."""
+
+    _track: Optional[TrackParams] = None  # the tracking parameters, or None
 
     def __init__(self, model, params, model_params, *, slots: int = 2, input_stage: str = "device",
-                 device: Optional[int] = None):
+                 device: Optional[int] = None, track: Optional[TrackParams] = None):
         if int(model_params["stride"]) != 4:
             raise ValueError(f"FrameStream needs stride 4 (model_params['stride'] is {model_params['stride']}): the "
                              "ragged and rotated post-network kernels it records are stride-4 kernels")
         if int(slots) < 1:
             raise ValueError("slots must be >= 1")
+        if track is not None and not isinstance(track, TrackParams):
+            raise ValueError(f"track is a TrackParams or None, not {track!r}")
         import torch
         self.model, self.params, self.model_params = model, dict(params), dict(model_params)
         self.input_stage = _stage(input_stage)
@@ -756,6 +805,9 @@ class FrameStream:
         self._calls = 0  # ticks launched: the next one takes slot _calls % slots
         self.captures = 0  # graphs captured so far (a tick key's first sight in a slot, or after a buffer moved)
         self.host_decodes = 0  # JPEG frames decoded with cv2.imdecode
+        self._track = track
+        if track is not None:  # every stream's table of tracks, empty
+            self._tables = torch.zeros((track.streams, TRACK_TABLE.itemsize), dtype=torch.uint8, device=self.device)
 
     def close(self) -> None:
         for ticks in self._ticks:
@@ -770,26 +822,49 @@ class FrameStream:
     def __exit__(self, *exc):
         self.close()
 
-    def submit(self, frame) -> int:
+    def submit(self, frame, *, stream: int = 0) -> int:
         """Pose ``frame`` as a tick of one frame in the next slot and return its ticket.  ``frame`` is a ``[H, W, 3]``
         uint8 BGR image (numpy, or a CUDA tensor on the stream's device), a JPEG file's bytes or a ``YUVFrame``.
-        ``submit(f)`` and ``submit_many([f])`` form the same tick key, so in one slot they share one graph."""
-        return self._submit([self._frame_of(frame)])[0]
+        ``submit(f)`` and ``submit_many([f])`` form the same tick key, so in one slot they share one graph.  ``stream``:
+        the frame's stream with tracking (``TrackParams.streams``); without, only 0."""
+        streams = self._streams_of([stream])
+        return self._submit([self._frame_of(frame)], streams)[0]
 
-    def submit_many(self, frames) -> List[int]:
+    def submit_many(self, frames, *, streams=None) -> List[int]:
         """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
         CUDA graph in the next slot, and return one ticket per frame, each read with ``result``.
 
         ``frames`` may mix every kind ``submit`` takes and every shape; it needs ``input_stage="device"``.  A frame
         ``submit`` would refuse refuses the whole tick before anything is staged; if the launch or its capture raises,
-        no ticket is issued."""
+        no ticket is issued.  ``streams``: with tracking, None (every frame is stream 0's: the next K frames of one
+        video) or one stream per frame (one per camera, say); without, None."""
         if self.input_stage != "device":
             raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
                              "spg_prenet_ragged")
+        frames = list(frames)
+        if streams is not None:
+            streams = list(streams)
+            if len(streams) != len(frames):
+                raise ValueError(f"{len(frames)} frames but {len(streams)} streams")
+        streams = self._streams_of([0] * len(frames) if streams is None else streams)
         staged = [self._frame_of(f) for f in frames]
         if not staged:
             raise ValueError("submit_many needs at least one frame")
-        return self._submit(staged)
+        return self._submit(staged, streams)
+
+    def _streams_of(self, streams) -> Optional[List[int]]:
+        """The frames' stream indices checked: None without tracking (where only stream 0 exists)."""
+        out = []
+        for s in streams:
+            if isinstance(s, bool) or not isinstance(s, (int, np.integer)):
+                raise ValueError(f"a stream index is an int, not {s!r}")
+            if self._track is None:
+                if s != 0:
+                    raise ValueError(f"stream {s}: streams other than 0 need tracking (FrameStream(track=TrackParams(...)))")
+            elif not 0 <= s < self._track.streams:
+                raise ValueError(f"stream {s} is outside [0, {self._track.streams})")
+            out.append(int(s))
+        return None if self._track is None else out
 
     def _frame_of(self, frame):
         """A submitted frame checked: ``(frame, rec, decoded)`` -- a JPEG file the parser takes as its bytes (uint8
@@ -829,8 +904,9 @@ class FrameStream:
                 raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
         return frame, rec, decoded
 
-    def _submit(self, staged: list) -> List[int]:
-        """Launch a tick of checked frames (``_frame_of``) in the next slot; returns its tickets."""
+    def _submit(self, staged: list, streams: Optional[List[int]] = None) -> List[int]:
+        """Launch a tick of checked frames (``_frame_of``) in the next slot, with their stream indices when tracking;
+        returns its tickets."""
         import torch
         kinds = tuple((int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)) if rec is not None
                       else (frame.height, frame.width, _YUVKind(frame.format, frame.device is not None))
@@ -840,17 +916,18 @@ class FrameStream:
         slot = self._calls % len(self._busy)
         if self._busy[slot] is not None:
             self._finish(slot)
-        tk, done = self._launch(slot, kinds, staged)
+        tk, done = self._launch(slot, kinds, staged) if streams is None else self._launch(slot, kinds, staged, streams)
         tickets = list(range(self._next, self._next + len(staged)))  # issued once the tick runs
         self._next += len(staged)
         self._calls += 1
         self._busy[slot] = (tickets, tk, done, [d for _, _, d in staged])
         return tickets
 
-    def _launch(self, slot: int, kinds: tuple, staged: list):
-        """Stage a tick's frames in the slot's ``_Tick`` for ``kinds`` (made on the key's first sight, made again when a
-        JPEG frame outgrows its capacity) and run its graph, or reserve its scratch, run its calls and capture them;
-        returns the ``_Tick`` and the event of the launch's end."""
+    def _launch(self, slot: int, kinds: tuple, staged: list, streams: Optional[List[int]] = None):
+        """Stage a tick's frames (and with tracking their stream indices, -1 to skip a frame) in the slot's ``_Tick``
+        for ``kinds`` (made on the key's first sight, made again when a JPEG frame outgrows its capacity) and run its
+        graph, or reserve its scratch, run its calls and capture them; returns the ``_Tick`` and the event of the
+        launch's end."""
         import torch
         if self._g.max_batch < len(kinds):
             self._stream.synchronize()  # the old handle's scratch may be in use
@@ -877,6 +954,8 @@ class FrameStream:
                 self._invalidate()
         self._drop_held(tk)  # the maps of the key's earlier tick are overwritten
         host = tk.up_host.numpy()
+        if tk.track is not None:
+            host[tk.streams_at:tk.streams_at + 4 * len(kinds)] = np.asarray(streams, np.int32).view(np.uint8)
         for j, ((frame, rec, _), (H, W, kind)) in enumerate(zip(staged, kinds)):
             if rec is not None:
                 jj = tk.jpeg.index(j)
@@ -926,8 +1005,9 @@ class FrameStream:
         import torch
         g = self._g
         md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
-        if tk.pairs is None:
+        if tk.pairs is None or tk.track is not None:
             tk.up.copy_(tk.up_host, non_blocking=True)
+        if tk.pairs is None:
             if tk.jpeg:
                 g.jpeg_decode_frames(tk.up.data_ptr(), tk.formats, [tk.caps[j] for j in tk.jpeg])
                 tk.status_host.copy_(tk.status, non_blocking=True)
@@ -960,6 +1040,10 @@ class FrameStream:
             g.group_ragged(maps, [H for H, _, _ in tk.kinds], self._gp, paf_as_f64=tk.as_f64)
         finally:
             g.set_wire_output(None)
+        if tk.track is not None:
+            t = self._track
+            g.track_frames(tk.track, self._tables.data_ptr(), t.streams, t.oks_threshold, t.max_age)
+            tk.ids_host.copy_(tk.ids, non_blocking=True)
         tk.rec_host.copy_(tk.rec, non_blocking=True)
 
     def _capture(self, tk: _Tick) -> None:
@@ -986,17 +1070,22 @@ class FrameStream:
         self._busy[slot] = None
         done.synchronize()
         records = tk.rec_host.numpy().copy()
+        ids = tk.ids_host.numpy().copy() if tk.track is not None else None
         for j, ticket in enumerate(tickets):
             record, heat, paf, image = records[j], tk.heat[j], tk.paf[j], decoded[j]
+            frame_ids = None if ids is None else ids[j]
             if j in tk.jpeg and int(tk.status_host[tk.jpeg.index(j)]) != JPEG_OK:
                 image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + tk.nbytes[j]].numpy())
                 self.host_decodes += 1
-                again, d = self._launch(slot, ((image.shape[0], image.shape[1], False),), [(image, None, image)])
+                key, frame = ((image.shape[0], image.shape[1], False),), [(image, None, image)]
+                # the tick tracked the frame as unobserved: posing it again tracks nothing, and its people get -1
+                again, d = self._launch(slot, key, frame) if ids is None else self._launch(slot, key, frame, [-1])
                 d.synchronize()
                 record, heat, paf = again.rec_host[0].numpy().copy(), again.heat[0].clone(), again.paf[0].clone()
+                frame_ids = None
             elif j in tk.jpeg or j in tk.yuv:
                 image = tk.images[j]  # decoded or converted on the device: copied to the host if detail asks for it
-            self._keep(ticket, record, heat, paf, tk.kinds[j][0], tk.as_f64)
+            self._keep(ticket, record, heat, paf, tk.kinds[j][0], tk.as_f64, frame_ids)
             self._held[ticket] = (heat, paf, tk.as_f64, image)
             tk.held.append(ticket)
 
@@ -1013,10 +1102,14 @@ class FrameStream:
             for tk in ticks.values():
                 tk.graph = None
 
-    def result(self, ticket: int, *, detail: bool = False):
+    def result(self, ticket: int, *, detail: bool = False, ids: bool = False):
         """``process()``'s value for the frame of ``ticket`` (waits for it); each ticket is read once.  ``detail=True``
         returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame's buffers
-        to still hold them: read it before ``slots`` later calls to ``submit`` or ``submit_many``."""
+        to still hold them: read it before ``slots`` later calls to ``submit`` or ``submit_many``.  ``ids=True`` (with
+        tracking) returns ``(value, ids)``: per person its track's id within the frame's stream, -1 for the people of an
+        unobserved frame."""
+        if ids and self._track is None:
+            raise ValueError("ids=True needs tracking (FrameStream(track=TrackParams(...)))")
         for slot, busy in enumerate(self._busy):
             if busy is not None and ticket in busy[0]:
                 self._finish(slot)
@@ -1030,17 +1123,19 @@ class FrameStream:
         out = self._done.pop(ticket)
         if isinstance(out, Exception):
             raise out
-        people, record = out
-        if not detail:
-            return people
-        heat, paf, as_f64, image = held
-        if image is not None and not isinstance(image, np.ndarray):
-            image = image.cpu().numpy()
-        return FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
+        people, record, person_ids = out
+        value = people
+        if detail:
+            heat, paf, as_f64, image = held
+            if image is not None and not isinstance(image, np.ndarray):
+                image = image.cpu().numpy()
+            value = FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
+        return (value, person_ids) if ids else value
 
-    def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool) -> None:
-        """Keep the people of one frame's wire record (or the error they raise) under its ticket.  A record with a
-        capacity bit is regrouped on the capacity-free tier from the frame's maps."""
+    def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool, ids=None) -> None:
+        """Keep the people of one frame's wire record (or the error they raise) under its ticket, with their ids: with
+        tracking, ``ids`` the frame's ids output, or None for -1 each.  A record with a capacity bit is regrouped on the
+        capacity-free tier from the frame's maps."""
         rec = wire.as_records(record, self._g.J, self._g.capR)[0]
         try:
             if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
@@ -1050,7 +1145,10 @@ class FrameStream:
             else:
                 _check_status(rec["status"])
                 people = wire.people_of(rec)
-            self._done[ticket] = (people, record)
+            person_ids = None
+            if self._track is not None:
+                person_ids = [-1] * len(people) if ids is None or rec["status"] else [int(v) for v in ids[:len(people)]]
+            self._done[ticket] = (people, record, person_ids)
         except GroupingError as e:
             self._done[ticket] = e
 

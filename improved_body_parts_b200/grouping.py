@@ -157,6 +157,16 @@ YUV_MEMBER = np.dtype([("format", np.int32), ("height", np.int32), ("width", np.
                        ("planes", np.uint64, (3,)), ("pitches", np.int64, (3,)), ("out", np.uint64),
                        ("out_pitch", np.int64)], align=True)
 
+#: ``spg_track_table`` and ``spg_track_frame`` (include/spgroup.h): a stream's tracks (caller-owned device memory; all
+#: zeros is an empty table) and one frame of ``spg_track_frames`` -- the device addresses of its wire record, its stream
+#: index (int32; -1 skips the frame), its JPEG decode status (0: none), its ids output (int64 per row) and, optionally,
+#: its OKS matrix output ([TRACK_SLOTS][rows] float64; 0: none)
+TRACK_SLOTS = 128
+TRACK = np.dtype([("id", np.int64), ("age", np.int32), ("live", np.int32), ("xy", np.float64, (17, 2)),
+                  ("present", np.uint64)], align=True)
+TRACK_TABLE = np.dtype([("next_id", np.int64), ("reserved", np.int64), ("tracks", TRACK, (TRACK_SLOTS,))], align=True)
+TRACK_FRAME = np.dtype([(f, np.uint64) for f in ("record", "stream", "jpeg_status", "ids", "oks")], align=True)
+
 
 def jpeg_parse(data) -> np.ndarray:
     """``spg_jpeg_parse`` of one file's bytes (host only): a ``JPEG_RECORD`` whose ``status`` is ``JPEG_OK`` or the
@@ -226,6 +236,7 @@ _PROTOTYPES = {
     "spg_jpeg_decode_frames": (_int, [_ptr, _ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_jpeg_reserve_frames": (_int, [_ptr, _ptr, _ptr, _i32, _P(C.c_int32)]),
     "spg_yuv_to_bgr": (_int, [_ptr, _ptr, _i32, _ptr]),  # members: a YUV_MEMBER array
+    "spg_track_frames": (_int, [_ptr, _ptr, _i32, _ptr, _i32, _f64, _i32, _ptr]),  # frames: a TRACK_FRAME array
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -1113,6 +1124,16 @@ class Grouper:
         s = self._records(members, YUV_MEMBER)
         _check(self._lib.spg_yuv_to_bgr(self._h, s.ctypes.data, len(s), self._stream_ptr(stream)), "spg_yuv_to_bgr",
                self._h)
+
+    # -- tracking (dropin.FrameStream builds the frames) -----------------------------------------------------------
+    def track_frames(self, frames: np.ndarray, tables: int, n_tables: int, oks_threshold: float, max_age: int,
+                     stream=None) -> None:
+        """``spg_track_frames``: ``frames`` a ``TRACK_FRAME`` array, ``tables`` the device address of ``n_tables``
+        ``TRACK_TABLE`` records.  Each frame's people are matched to its stream's tracks, in order, and get their ids.
+        Asynchronous on ``stream``; can be recorded into a CUDA graph."""
+        f = self._records(frames, TRACK_FRAME)
+        _check(self._lib.spg_track_frames(self._h, f.ctypes.data, len(f), int(tables), int(n_tables), float(oks_threshold),
+                                          int(max_age), self._stream_ptr(stream)), "spg_track_frames", self._h)
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

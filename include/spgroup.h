@@ -366,6 +366,54 @@ typedef struct spg_yuv_member {
  * (see "frames recorded into a CUDA graph") and replayed with new contents in the same planes. */
 int spg_yuv_to_bgr(spg_handle *h, const spg_yuv_member *members, int32_t n, void *stream);
 
+/* ---- tracking people across a stream's frames: OKS association of each frame's people with the stream's tracks ------
+ * A stream (one camera or one video) keeps a table of at most SPG_TRACK_SLOTS tracks in caller-owned device memory; a
+ * zero-filled table is empty, with its id counter at 0.  A track holds its id, its age (frames of its stream since it
+ * was last matched) and its last pose, 17 COCO joints as a wire record row stores them. */
+#define SPG_TRACK_SLOTS 128
+typedef struct spg_track {
+    int64_t id;
+    int32_t age;
+    int32_t live;               /* 0: the slot is free */
+    double xy[17][2];
+    uint64_t present;           /* bit g: joint g was found (as a wire record row's mask) */
+} spg_track;
+typedef struct spg_track_table {
+    int64_t next_id;            /* the id the stream's next track takes: ids are unique within a stream */
+    int64_t reserved;
+    spg_track tracks[SPG_TRACK_SLOTS];
+} spg_track_table;
+/* One frame of spg_track_frames; every address is device memory, read or written when the launch runs. */
+typedef struct spg_track_frame {
+    const void *record;         /* the frame's wire record, spg_wire_record_bytes(h) bytes (the handle's wire rows) */
+    const int32_t *stream;      /* the frame's table index in [0, n_tables), or -1: the frame is skipped */
+    const int32_t *jpeg_status; /* NULL, or the frame's decode_status: a value other than SPG_JPEG_OK makes the */
+                                /* frame unobserved                                                            */
+    int64_t *ids;               /* [wire rows]: the first n_persons get the id of each row's person, or -1 */
+    double *oks;                /* NULL, or [SPG_TRACK_SLOTS][wire rows]: OKS of each live track (by slot) with */
+                                /* each person of an observed frame, as matched; other entries are not written */
+} spg_track_frame;
+/* Per frame, in order (several frames of one stream in one call are taken in call order):
+ *   1. the OKS of each live track with each of the record's first n_persons persons: COCO's keypoint sigmas
+ *      (cocoeval.py's kpt_oks_sigmas), the track's pose as ground truth; T = its joints present with finite x and y,
+ *      area = max((xmax - xmin) * (ymax - ymin), 1) over T; per joint of T present and finite in the person
+ *      e = (dx^2 + dy^2) / (2 sigma)^2 / area / 2 in float64 in that order, OKS = sum of exp(-e) in joint order / |T|
+ *      (0 when T is empty); a joint of T the person lacks counts in |T| and adds nothing;
+ *   2. greedy matching over the pairs with OKS >= oks_threshold: highest OKS first, ties to the lower track id, then to
+ *      the lower person row, a pair taken when both members are free;
+ *   3. a matched track takes the person's pose and age 0; the person gets the track's id;
+ *   4. every other live track ages by 1 and is dropped when its age exceeds max_age;
+ *   5. in row order, each unmatched person starts a track with the stream's next id in the lowest free slot, or, in a
+ *      full table, in place of the track of largest age (ties: smallest id).
+ * A frame whose record has a status bit, or whose jpeg_status is not SPG_JPEG_OK, is unobserved: only step 4 runs and
+ * its persons get -1.  A skipped frame (stream -1) changes no table; its persons get -1.  The handle must have 17 output
+ * joints; oks_threshold is finite and max_age >= 0.  One CTA per stream of the call, from the first frame of it.
+ * Asynchronous on `stream`; allocates nothing and never synchronises, and its launches depend on n alone, so it can be
+ * recorded into a CUDA graph and replayed with new records, stream indices and statuses at the same addresses.  Frames
+ * may be reused as soon as the call returns. */
+int spg_track_frames(spg_handle *h, const spg_track_frame *frames, int32_t n, spg_track_table *tables, int32_t n_tables,
+                     double oks_threshold, int32_t max_age, void *stream);
+
 /* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
  * reference's CanonicalConfig / TransformationParams: */
@@ -706,7 +754,8 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 /* number of kernel launches issued by this handle since creation (bench.py's gpu_launches) */
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
- * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation, 9 JPEG decode);
+ * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation, 9 JPEG decode,
+ * 10 YUV conversion, 11 tracking);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 
