@@ -19,6 +19,7 @@ There is no CPU path: without the CUDA library / an sm_90 GPU these functions ra
 from __future__ import annotations
 
 import dataclasses
+import functools
 from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
@@ -171,6 +172,17 @@ def _people_of_result(r) -> list:
     return out
 
 
+def _people_of_record(rec, regroup) -> list:
+    """``process()``'s return value from one image's wire record, which holds at most capR persons: with a capacity bit
+    the image's people come from ``regroup()``, its one-image ``GroupResult`` on the capacity-free tier."""
+    if _over_capacity(rec["status"]):
+        r = regroup()
+        _check_status(r.status[0])
+        return _people_of_result(r)
+    _check_status(rec["status"])
+    return wire.people_of(rec)
+
+
 def _maps_to_device(hwc: np.ndarray, channels: int, dtype):
     """``[H, W, C]`` host maps (what predict() returns) -> ``[1, channels, H, W]`` device planes of torch ``dtype``.
 
@@ -250,25 +262,30 @@ def _copied(slot: str) -> None:
     _staging[slot] = (_staging[slot][0], ev)
 
 
+def _pack(slot: str, arrays) -> list:
+    """The uint8 host ``arrays`` packed into ``slot``'s pinned buffer and sent up with one asynchronous copy into one
+    device buffer: per array its flat view of that buffer."""
+    import torch
+    arrays = [a.reshape(-1) for a in arrays]
+    host = _pinned(slot, sum(a.size for a in arrays), torch.uint8)
+    staged, bounds = host.numpy(), np.cumsum([0] + [a.size for a in arrays]).tolist()
+    for a, o in zip(arrays, bounds):
+        staged[o:o + a.size] = a
+    packed = host.to(f"cuda:{_device}", non_blocking=True)
+    _copied(slot)
+    return [packed[o0:o1] for o0, o1 in zip(bounds, bounds[1:])]
+
+
 def _upload_images(images) -> list:
     """The ``[H, W, 3]`` uint8 CUDA image of every entry of ``images``: CUDA tensors as they are (on the current device),
     host images packed into one pinned buffer and sent up with one asynchronous copy into one device buffer, of which
     each gets a view."""
     import torch
-    dev = f"cuda:{_device}"
-    out = [img.to(dev) if isinstance(img, torch.Tensor) else None for img in images]
+    out = [img.to(f"cuda:{_device}") if isinstance(img, torch.Tensor) else None for img in images]
     host_imgs = {i: np.ascontiguousarray(img, np.uint8) for i, img in enumerate(images) if out[i] is None}
     if host_imgs:
-        host = _pinned("image", sum(a.size for a in host_imgs.values()), torch.uint8)
-        staged, at, off = host.numpy(), {}, 0
-        for i, a in host_imgs.items():
-            staged[off:off + a.size] = a.reshape(-1)
-            at[i] = off
-            off += a.size
-        packed = host.to(dev, non_blocking=True)
-        _copied("image")
-        for i, a in host_imgs.items():
-            out[i] = packed[at[i]:at[i] + a.size].view(a.shape)
+        for (i, a), v in zip(host_imgs.items(), _pack("image", host_imgs.values())):
+            out[i] = v.view(a.shape)
     return out
 
 
@@ -297,15 +314,7 @@ def imread_many(paths) -> Tuple[list, int]:
     todo = [i for i in todo if recs[i]["status"] == JPEG_OK]
     out = [None] * len(datas)
     if todo:
-        nbytes = sum(len(datas[i]) for i in todo)
-        host = _pinned("jpeg", nbytes, torch.uint8)
-        staged, at, off = host.numpy(), [], 0
-        for i in todo:
-            staged[off:off + len(datas[i])] = np.frombuffer(datas[i], np.uint8)
-            at.append(off)
-            off += len(datas[i])
-        files = host.to(dev, non_blocking=True)
-        _copied("jpeg")
+        files = _pack("jpeg", [np.frombuffer(datas[i], np.uint8) for i in todo])
         sizes = [int(recs[i]["height"]) * int(recs[i]["width"]) * 3 for i in todo]
         images = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
         status = torch.empty(len(todo), dtype=torch.int32, device=dev)
@@ -313,7 +322,7 @@ def imread_many(paths) -> Tuple[list, int]:
         o = 0
         for k, i in enumerate(todo):
             arr[k] = recs[i]
-            arr[k]["data"], arr[k]["out"] = files.data_ptr() + at[k], images.data_ptr() + o
+            arr[k]["data"], arr[k]["out"] = files[k].data_ptr(), images.data_ptr() + o
             arr[k]["decode_status"] = status.data_ptr() + 4 * k
             out[i] = images[o:o + sizes[k]].view(int(recs[i]["height"]), int(recs[i]["width"]), 3)
             o += sizes[k]
@@ -394,6 +403,24 @@ def _host_pair(image: np.ndarray, scale: float, angle: float, model_params, out:
     return out, image_to_test.shape[:2], reverse
 
 
+def _host_pairs(images, plan, members, model_params, out) -> list:
+    """The cv2 pair of every member ``(image index, item index)`` of one network input size (``plan_items``), written
+    into the pinned ``[2 * len(members), Hp, Wp, 3]`` float32 tensor ``out``; per member ``(crop, reverse)``."""
+    return [_host_pair(images[i], plan[i][t][1], plan[i][t][2], model_params, out=out[2 * j:2 * j + 2].numpy())[1:]
+            for j, (i, t) in enumerate(members)]
+
+
+def _forward_bucket(model, x, members, built, step: int, entries) -> None:
+    """Forward one input size's tensor ``x`` (the pairs of ``members``) ``step`` members at a time, and set each member's
+    ``entries[i][t]`` to ``(output pair, crop, reverse)`` (``built``: per member its crop and reverse)."""
+    import torch
+    with torch.no_grad():
+        for c in range(0, len(members), step):
+            out = _network_output(model, x[2 * c:2 * (c + step)]).contiguous()
+            for k, (i, t) in enumerate(members[c:c + step]):
+                entries[i][t] = (out[2 * k:2 * k + 2],) + built[c + k]
+
+
 def _network_output(model, x):
     """The network's maps for the input batch ``x`` (evaluate.py:124-126): the last stack's finest scale, float32 unless
     the network answers in float16."""
@@ -458,24 +485,15 @@ def predict_batch(images, params, model, model_params, *, forward_batch: int, in
         k = len(members)
         x = torch.empty((2 * k, Hp, Wp, 3), dtype=torch.float32, device=dev)
         if stage == "host":
-            built = []  # per member (crop, rotate_matrix_reverse)
             host = _pinned("pairs", x.numel(), torch.float32).view(x.shape)
-            for j, (i, t) in enumerate(members):
-                _, scale, angle = plan[i][t][:3]
-                built.append(_host_pair(images[i], scale, angle, model_params, out=host[2 * j:2 * j + 2].numpy())[1:])
+            built = _host_pairs(images, plan, members, model_params, host)
             x.copy_(host, non_blocking=True)
             _copied("pairs")
         else:
             pairs = g.prenet_ragged([(uploaded[i], plan[i][t][0], plan[i][t][2]) for i, t in members], max_downsample=md,
                                     pad_value=pv, out=[x[2 * j:2 * j + 2] for j in range(k)])
             built = [(crop, reverse) for _, crop, reverse in pairs]
-        for c0 in range(0, k, fb):
-            c1 = min(k, c0 + fb)
-            with torch.no_grad():
-                out = _network_output(model, x[2 * c0:2 * c1]).contiguous()
-            for j in range(c0, c1):
-                i, t = members[j]
-                entries[i][t] = (out[2 * (j - c0):2 * (j - c0) + 2],) + built[j]
+        _forward_bucket(model, x, members, built, fb, entries)
         del x
     maps = g.postnet_ragged_items([(e, tuple(int(v) for v in img.shape[:2])) for e, img in zip(entries, images)],
                                   nan_scrub=_variant == "demo")
@@ -583,13 +601,6 @@ class YUVFrame:
 
 
 @dataclasses.dataclass(frozen=True)
-class _YUVKind:
-    """The tick-key kind of a ``YUVFrame``: its layout and whether its planes are CUDA tensors."""
-    format: str
-    cuda: bool
-
-
-@dataclasses.dataclass(frozen=True)
 class TrackParams:
     """``FrameStream``'s tracking: ``streams`` tables of tracks (one per camera or video, frames name theirs with
     ``submit(..., stream=s)``), the OKS at or above which a person may continue a track, and the frames of its stream a
@@ -612,56 +623,120 @@ class TrackParams:
             raise ValueError(f"TrackParams.oks_threshold must be a number in [0, 1], not {t!r}")
 
 
+class _Key(NamedTuple):
+    """A frame's part of a tick key: its size, its source -- a host or CUDA BGR image (``"image"``, ``"cuda"``), JPEG
+    bytes the device decodes (``"jpeg"``), a ``YUVFrame`` with host or CUDA planes (``"yuv"``, ``"yuv_cuda"``) -- and its
+    ``JPEG_FORMAT`` values or YUV layout (None for an image)."""
+    height: int
+    width: int
+    source: str
+    format: object = None
+
+
+class _Frame(NamedTuple):
+    """A frame ``_admit`` took: its key, what is staged (a contiguous host or a CUDA image, JPEG bytes as uint8, the
+    ``YUVFrame``), its parsed JPEG record, and the image cv2 decoded or converted it to at submit, if it did."""
+    key: _Key
+    data: object
+    rec: Optional[np.ndarray] = None
+    decoded: Optional[np.ndarray] = None
+
+
+def _admit(frames, streams, *, input_stage: str, device: int, n_streams: Optional[int]):
+    """A tick's frames and stream indices checked before anything is staged: per frame its ``_Frame``, the stream
+    indices as ints, and how many frames ``cv2.imdecode`` decoded.  ``n_streams``: ``TrackParams.streams``, or None
+    without tracking (only stream 0 exists).  A JPEG file the parser refuses, and with ``input_stage="host"`` every
+    JPEG or YUV frame, is staged as cv2's image of it."""
+    import torch
+    checked = []
+    for s in streams:
+        if isinstance(s, bool) or not isinstance(s, (int, np.integer)):
+            raise ValueError(f"a stream index is an int, not {s!r}")
+        if n_streams is None:
+            if s != 0:
+                raise ValueError(f"stream {s}: streams other than 0 need tracking (FrameStream(track=TrackParams(...)))")
+        elif not 0 <= s < n_streams:
+            raise ValueError(f"stream {s} is outside [0, {n_streams})")
+        checked.append(int(s))
+    out, decodes = [], 0
+    for frame in frames:
+        decoded = None
+        yuv = isinstance(frame, YUVFrame)
+        cuda = frame.device is not None if yuv else isinstance(frame, torch.Tensor) and frame.is_cuda
+        if cuda and input_stage == "host":
+            raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
+        if yuv:
+            if cuda and frame.device != device:
+                raise ValueError(f"a CUDA YUV frame's planes are on cuda:{device}, not cuda:{frame.device}")
+            if input_stage == "device":
+                out.append(_Frame(_Key(frame.height, frame.width, "yuv_cuda" if cuda else "yuv", frame.format), frame))
+                continue
+            frame = decoded = frame.to_bgr()
+        elif isinstance(frame, (bytes, bytearray, memoryview)):
+            data = np.frombuffer(frame, np.uint8)
+            if data.size == 0:
+                raise ValueError("a JPEG frame's bytes are empty")
+            rec = jpeg_parse(data) if input_stage == "device" else None
+            if rec is not None and rec["status"] == JPEG_OK:
+                fmt = tuple(int(rec[k]) for k in JPEG_FORMAT)
+                out.append(_Frame(_Key(int(rec["height"]), int(rec["width"]), "jpeg", fmt), data, rec))
+                continue
+            frame = decoded = _imdecode(data)
+            decodes += 1
+        if cuda:
+            if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or frame.device.index != device:
+                raise ValueError(f"a CUDA frame is a [H, W, 3] uint8 tensor on cuda:{device}")
+            source = "cuda"
+        else:
+            frame = np.ascontiguousarray(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
+            if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
+                raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
+            source = "image"
+        out.append(_Frame(_Key(int(frame.shape[0]), int(frame.shape[1]), source), frame, None, decoded))
+    return out, checked, decodes
+
+
 def _align(n: int) -> int:
     return -(-int(n) // 256) * 256
 
 
 class _Tick:
-    """One slot's buffers for one tick key, and the graph captured over them.  ``kinds``: per frame ``(H, W, kind)``,
-    kind False for a host image, True for a CUDA image, a ``JPEG_FORMAT`` tuple for JPEG bytes, a ``_YUVKind`` for a
-    ``YUVFrame``; ``caps``: per frame its capacity in bytes (0 for the others); ``recs``: per frame its parsed JPEG
-    record or None."""
+    """One slot's buffers for one tick key, and the graph captured over them.  ``keys``: per frame its ``_Key``;
+    ``caps``: per frame its capacity in bytes (0 for the others); ``recs``: per frame its parsed JPEG record or None."""
 
-    def __init__(self, fs: "FrameStream", kinds: tuple, caps: list, recs: list):
+    def __init__(self, fs: "FrameStream", keys: tuple, caps: list, recs: list):
         import torch
         dev = torch.device("cuda", fs.device)
         host_stage = fs.input_stage == "host"
-        self.kinds, self.caps, self.graph = kinds, list(caps), None
+        self.keys, self.caps, self.graph = keys, list(caps), None
+        self.stream, self.model_params = fs._stream, fs.model_params
         self.held: List[int] = []  # tickets of finished frames whose maps FrameStream._held still refers to
-        self.plan, self.buckets = plan_items([k[:2] for k in kinds], fs.params, fs.model_params)
+        self.plan, self.buckets = plan_items([k[:2] for k in keys], fs.params, fs.model_params)
         md = int(fs.model_params["max_downsample"])
         # per frame, per item: the crop and reverse rotation the post-network stage takes, as spg_prenet builds the item
         self.built = [[(geo[:2], reverse) for _, geo, _, reverse in
-                       (prenet_item(H, W, item[0], item[2], md) for item in items)]
-                      for (H, W, _), items in zip(kinds, self.plan)]
-        self.jpeg = [j for j, k in enumerate(kinds) if isinstance(k[2], tuple)]
-        self.yuv = [j for j, k in enumerate(kinds) if isinstance(k[2], _YUVKind)]
-        # the one upload: the JPEG frames' records, then their bytes (a capacity each), then the host frames and host
-        # YUV frames' packed planes (with input_stage="host" the pairs cv2 built go up instead); a CUDA YUV frame's
-        # planes are copied into packed planes of their own
+                       (prenet_item(k.height, k.width, item[0], item[2], md) for item in items)]
+                      for k, items in zip(keys, self.plan)]
+        self.jpeg = [j for j, k in enumerate(keys) if k.source == "jpeg"]
+        self.yuv = [j for j, k in enumerate(keys) if k.source in ("yuv", "yuv_cuda")]
+        # the one upload: the JPEG frames' records, with tracking the frames' stream indices (int32), then per frame its
+        # bytes: a JPEG frame's capacity, a host image (with input_stage="host" the pairs cv2 built go up instead) or a
+        # host YUV frame's packed planes.  A CUDA YUV frame's planes are copied into packed planes of their own.
         self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
-        self.streams_at = None  # with tracking: the frames' stream indices (int32) in the upload
+        self.streams_at = None
         if fs._track is not None:
-            self.streams_at, off = off, _align(off + 4 * len(kinds))
-        self.yuv_dev = {}
-        for j, (H, W, kind) in enumerate(kinds):
-            if isinstance(kind, _YUVKind):
-                size = _yuv_bytes(kind.format, H, W)
-                if kind.cuda:
-                    self.yuv_dev[j] = torch.empty(size, dtype=torch.uint8, device=dev)
-                    continue
-            elif kind is True or host_stage:
-                continue
-            else:
-                size = self.caps[j] if j in self.jpeg else H * W * 3
-            self.at[j] = off
-            off = _align(off + size)
+            self.streams_at, off = off, _align(off + 4 * len(keys))
+        for j, (H, W, source, fmt) in enumerate(keys):
+            size = {"jpeg": self.caps[j], "yuv": _yuv_bytes(fmt, H, W), "image": None if host_stage else H * W * 3}
+            if size.get(source) is not None:
+                self.at[j], off = off, _align(off + size[source])
+        self.yuv_dev = {j: torch.empty(_yuv_bytes(fmt, H, W), dtype=torch.uint8, device=dev)
+                        for j, (H, W, source, fmt) in enumerate(keys) if source == "yuv_cuda"}
         self.up_host = torch.empty(off, dtype=torch.uint8, pin_memory=True)
         self.up = torch.empty(off, dtype=torch.uint8, device=dev)
-        self.nbytes = [0] * len(kinds)
         self.images = None if host_stage else [
-            self.up[self.at[j]:self.at[j] + H * W * 3].view(H, W, 3) if kind is False else
-            torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for j, (H, W, kind) in enumerate(kinds)]
+            self.up[self.at[j]:self.at[j] + H * W * 3].view(H, W, 3) if source == "image" else
+            torch.empty((H, W, 3), dtype=torch.uint8, device=dev) for j, (H, W, source, _) in enumerate(keys)]
         self.status = torch.zeros(max(len(self.jpeg), 1), dtype=torch.int32, device=dev)
         self.status_host = torch.zeros(self.status.shape, dtype=torch.int32, pin_memory=True)
         self.formats = np.zeros(len(self.jpeg), JPEG_RECORD)
@@ -672,11 +747,11 @@ class _Tick:
             self.formats[jj]["decode_status"] = self.status.data_ptr() + 4 * jj
         self.yuv_members = np.zeros(len(self.yuv), YUV_MEMBER)  # every address is the slot's own
         for jj, j in enumerate(self.yuv):
-            H, W, kind = kinds[j]
-            base = self.yuv_dev[j].data_ptr() if kind.cuda else self.up.data_ptr() + self.at[j]
+            H, W, source, fmt = keys[j]
+            base = self.yuv_dev[j].data_ptr() if source == "yuv_cuda" else self.up.data_ptr() + self.at[j]
             m = self.yuv_members[jj]
-            m["format"], m["height"], m["width"] = _YUV[kind.format][1], H, W
-            for k, (o, (_, w)) in enumerate(_yuv_layout(kind.format, H, W)):
+            m["format"], m["height"], m["width"] = _YUV[fmt][1], H, W
+            for k, (o, (_, w)) in enumerate(_yuv_layout(fmt, H, W)):
                 m["planes"][k], m["pitches"][k] = base + o, w
             m["out"], m["out_pitch"] = self.images[j].data_ptr(), 3 * W
         self.inputs = {size: torch.empty((2 * len(members),) + size + (3,), dtype=torch.float32, device=dev)
@@ -685,25 +760,58 @@ class _Tick:
                       for size, x in self.inputs.items()} if host_stage else None
         self.n_items = len(self.plan[0])
         self.as_f64 = self.n_items == 1  # as predict() returns
-        self.heat = [torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev) for H, W, _ in kinds]
+        self.heat = [torch.empty((1, NUM_PARTS, H, W), dtype=torch.float32, device=dev) for H, W, _, _ in keys]
         self.paf = [torch.empty((1, len(fs.limbs), H, W), dtype=torch.float32 if self.as_f64 else torch.float64, device=dev)
-                    for H, W, _ in kinds]
-        self.rec = torch.zeros((len(kinds), fs._g.wire_record_bytes()), dtype=torch.uint8, device=dev)
+                    for H, W, _, _ in keys]
+        self.rec = torch.zeros((len(keys), fs._g.wire_record_bytes()), dtype=torch.uint8, device=dev)
         self.rec_host = torch.empty(self.rec.shape, dtype=torch.uint8, pin_memory=True)
         self.track = None
         if fs._track is not None:  # per frame its people's ids, and its spg_track_frames member
-            self.ids = torch.empty((len(kinds), fs._g.capR), dtype=torch.int64, device=dev)
+            self.ids = torch.empty((len(keys), fs._g.capR), dtype=torch.int64, device=dev)
             self.ids_host = torch.empty(self.ids.shape, dtype=torch.int64, pin_memory=True)
-            self.track = np.zeros(len(kinds), TRACK_FRAME)
-            for j in range(len(kinds)):
+            self.track = np.zeros(len(keys), TRACK_FRAME)
+            for j in range(len(keys)):
                 self.track[j]["record"] = self.rec[j].data_ptr()
                 self.track[j]["stream"] = self.up.data_ptr() + self.streams_at + 4 * j
                 self.track[j]["jpeg_status"] = self.status.data_ptr() + 4 * self.jpeg.index(j) if j in self.jpeg else 0
                 self.track[j]["ids"] = self.ids[j].data_ptr()
 
-    def members(self):
-        """Per frame, per item: ``(H, W, multiplier, angle)``, what ``Grouper.reserve_frames`` takes."""
-        return [(H, W, item[0], item[2]) for (H, W, _), items in zip(self.kinds, self.plan) for item in items]
+    def stage(self, frames: List[_Frame], streams: List[int]) -> None:
+        """Write a tick's frames into this slot's buffers: the upload's host side (with tracking the stream indices, -1
+        skipping a frame), CUDA images and planes copied on the stream ahead of the graph, and with input_stage="host"
+        each item's pair built by cv2 into the pinned copy of its input."""
+        import torch
+        host, copies = self.up_host.numpy(), []  # copies: (slot's device buffer, caller's CUDA tensor)
+        if self.track is not None:
+            host[self.streams_at:self.streams_at + 4 * len(frames)] = np.asarray(streams, np.int32).view(np.uint8)
+        for j, (key, data, rec, _) in enumerate(frames):
+            at = self.at.get(j)
+            if key.source == "jpeg":
+                jj = self.jpeg.index(j)
+                host[at:at + data.size] = data
+                for k in ("data", "out", "decode_status"):  # the tick's device addresses, as the format's
+                    rec[k] = self.formats[jj][k]
+                host[jj * JPEG_RECORD.itemsize:(jj + 1) * JPEG_RECORD.itemsize] = np.frombuffer(rec.tobytes(), np.uint8)
+            elif key.source in ("yuv", "yuv_cuda"):
+                for p, (o, (h, w)) in zip(data.planes, _yuv_layout(key.format, key.height, key.width)):
+                    if key.source == "yuv":
+                        host[at + o:at + o + h * w].reshape(h, w)[:] = p
+                    else:
+                        copies.append((self.yuv_dev[j][o:o + h * w].view(h, w), p))
+            elif key.source == "cuda":
+                copies.append((self.images[j], data))
+            elif self.pairs is None:
+                host[at:at + data.size] = data.reshape(-1)
+        if copies:
+            self.stream.wait_stream(torch.cuda.current_stream(self.stream.device))
+            with torch.cuda.stream(self.stream):
+                for dst, src in copies:
+                    dst.copy_(src, non_blocking=True)
+            for _, src in copies:
+                src.record_stream(self.stream)
+        if self.pairs is not None:
+            for size, ms in self.buckets.items():
+                _host_pairs([f.data for f in frames], self.plan, ms, self.model_params, self.pairs[size])
 
 
 class FrameStream:
@@ -716,10 +824,11 @@ class FrameStream:
     ``group`` on the maps ``predict`` gives for the frame.  ``submit`` poses a tick of one frame and ``submit_many`` a
     tick of several, through the same calls.
 
-    A tick holds one slot.  The slot keeps one CUDA graph per **tick key**: each frame's shape and kind (host image,
-    CUDA image, JPEG format, or YUV layout on the host or on the device) in order.  The key's first tick in a slot runs
-    call by call -- it is the key's warm-up (the network's lazy set-up, cuDNN's choices) -- and the slot then captures
-    the graph over its buffers for that key; every later tick of that key in that slot is one graph launch.  The graph
+    A tick holds one slot.  The slot keeps one CUDA graph per **tick key**: each frame's shape and source (host image,
+    CUDA image, JPEG bytes of one format, or YUV planes of one layout on the host or on the device) in order.  The
+    key's first tick in a slot runs call by call -- it is the key's warm-up (the network's lazy set-up, cuDNN's
+    choices) -- and the slot then captures the graph over its buffers for that key; every later tick of that key in
+    that slot is one graph launch.  The graph
     holds one upload from the slot's pinned buffer of the tick's host frames, host YUV planes, JPEG bytes and parsed
     records; ``spg_jpeg_decode_frames`` for every JPEG frame; one ``spg_yuv_to_bgr`` for every YUV frame;
     ``spg_prenet_ragged`` for every item of ``scale_search x rotation_search`` of every frame, into one input tensor per
@@ -738,7 +847,7 @@ class FrameStream:
 
     JPEG bytes (``bytes``, ``bytearray`` or ``memoryview``) are parsed on the host with ``spg_jpeg_parse``.  A file the
     device decoder takes (baseline or extended-sequential Huffman, grey or YCbCr 4:4:4 / 4:2:2 / 4:4:0 / 4:2:0) is
-    decoded inside the graph, bit-identical to ``cv2.imdecode``; its kind is its format -- frame height and width,
+    decoded inside the graph, bit-identical to ``cv2.imdecode``; its key holds its format -- frame height and width,
     component count, luma sampling, restart interval and EXIF orientation -- and the scan's offset and length, the
     tables and the segments in front of the scan are read on the device from the frame's record, so they may change
     from frame to frame.  A slot reserves a capacity in bytes per JPEG frame of a key (the next power of two of the
@@ -798,7 +907,7 @@ class FrameStream:
         self._tier_stream = torch.cuda.Stream(device=self.device)
         self._pool = None
         self._ticks: List[Dict[tuple, _Tick]] = [{} for _ in range(int(slots))]  # per slot, its _Tick per tick key
-        self._busy: List[Optional[tuple]] = [None] * int(slots)  # per slot (tickets, _Tick, done event, cv2 images)
+        self._busy: List[Optional[tuple]] = [None] * int(slots)  # per slot (tickets, _Tick, done event, _Frames)
         self._done: Dict[int, object] = {}  # finished tickets: (people, record) or the exception to raise
         self._held: Dict[int, tuple] = {}  # finished tickets' maps, while their tick's buffers hold them
         self._next = 0  # the next ticket
@@ -827,8 +936,7 @@ class FrameStream:
         uint8 BGR image (numpy, or a CUDA tensor on the stream's device), a JPEG file's bytes or a ``YUVFrame``.
         ``submit(f)`` and ``submit_many([f])`` form the same tick key, so in one slot they share one graph.  ``stream``:
         the frame's stream with tracking (``TrackParams.streams``); without, only 0."""
-        streams = self._streams_of([stream])
-        return self._submit([self._frame_of(frame)], streams)[0]
+        return self._submit([frame], [stream])[0]
 
     def submit_many(self, frames, *, streams=None) -> List[int]:
         """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
@@ -842,152 +950,59 @@ class FrameStream:
             raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
                              "spg_prenet_ragged")
         frames = list(frames)
-        if streams is not None:
-            streams = list(streams)
-            if len(streams) != len(frames):
-                raise ValueError(f"{len(frames)} frames but {len(streams)} streams")
-        streams = self._streams_of([0] * len(frames) if streams is None else streams)
-        staged = [self._frame_of(f) for f in frames]
-        if not staged:
+        streams = [0] * len(frames) if streams is None else list(streams)
+        if len(streams) != len(frames):
+            raise ValueError(f"{len(frames)} frames but {len(streams)} streams")
+        if not frames:
             raise ValueError("submit_many needs at least one frame")
-        return self._submit(staged, streams)
+        return self._submit(frames, streams)
 
-    def _streams_of(self, streams) -> Optional[List[int]]:
-        """The frames' stream indices checked: None without tracking (where only stream 0 exists)."""
-        out = []
-        for s in streams:
-            if isinstance(s, bool) or not isinstance(s, (int, np.integer)):
-                raise ValueError(f"a stream index is an int, not {s!r}")
-            if self._track is None:
-                if s != 0:
-                    raise ValueError(f"stream {s}: streams other than 0 need tracking (FrameStream(track=TrackParams(...)))")
-            elif not 0 <= s < self._track.streams:
-                raise ValueError(f"stream {s} is outside [0, {self._track.streams})")
-            out.append(int(s))
-        return None if self._track is None else out
-
-    def _frame_of(self, frame):
-        """A submitted frame checked: ``(frame, rec, decoded)`` -- a JPEG file the parser takes as its bytes (uint8
-        array) and parsed record, any other JPEG file as cv2's image of it (also ``decoded``; counted in
-        ``host_decodes``), a ``YUVFrame`` as it is (``input_stage="host"``: as cv2's image of it, also ``decoded``), an
-        image as a contiguous uint8 array or the CUDA tensor it is, with ``rec`` None."""
-        import torch
-        decoded = rec = None
-        if isinstance(frame, YUVFrame):
-            if frame.device is not None and self.input_stage == "host":
-                raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
-            if frame.device is not None and frame.device != self.device:
-                raise ValueError(f"a CUDA YUV frame's planes are on cuda:{self.device}, not cuda:{frame.device}")
-            if self.input_stage == "device":
-                return frame, None, None
-            frame = decoded = frame.to_bgr()
-        if isinstance(frame, (bytes, bytearray, memoryview)):
-            data = np.frombuffer(frame, np.uint8)
-            if data.size == 0:
-                raise ValueError("a JPEG frame's bytes are empty")
-            rec = jpeg_parse(data) if self.input_stage == "device" else None
-            if rec is None or rec["status"] != JPEG_OK:
-                frame = decoded = _imdecode(data)
-                self.host_decodes += 1
-                rec = None
-            else:
-                return data, rec, None
-        cuda = isinstance(frame, torch.Tensor) and frame.is_cuda
-        if cuda:
-            if self.input_stage == "host":
-                raise ValueError("input_stage='host' builds the network input with cv2: pass host frames")
-            if frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3 or frame.device.index != self.device:
-                raise ValueError(f"a CUDA frame is a [H, W, 3] uint8 tensor on cuda:{self.device}")
-        else:
-            frame = np.ascontiguousarray(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
-            if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
-                raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
-        return frame, rec, decoded
-
-    def _submit(self, staged: list, streams: Optional[List[int]] = None) -> List[int]:
-        """Launch a tick of checked frames (``_frame_of``) in the next slot, with their stream indices when tracking;
-        returns its tickets."""
-        import torch
-        kinds = tuple((int(rec["height"]), int(rec["width"]), tuple(int(rec[k]) for k in JPEG_FORMAT)) if rec is not None
-                      else (frame.height, frame.width, _YUVKind(frame.format, frame.device is not None))
-                      if isinstance(frame, YUVFrame)
-                      else (int(frame.shape[0]), int(frame.shape[1]), isinstance(frame, torch.Tensor))
-                      for frame, rec, _ in staged)
+    def _submit(self, frames: list, streams: list) -> List[int]:
+        """Admit a tick's frames and stream indices (``_admit``), launch it in the next slot and return its tickets."""
+        frames, streams, decodes = _admit(frames, streams, input_stage=self.input_stage, device=self.device,
+                                          n_streams=None if self._track is None else self._track.streams)
+        self.host_decodes += decodes
         slot = self._calls % len(self._busy)
         if self._busy[slot] is not None:
             self._finish(slot)
-        tk, done = self._launch(slot, kinds, staged) if streams is None else self._launch(slot, kinds, staged, streams)
-        tickets = list(range(self._next, self._next + len(staged)))  # issued once the tick runs
-        self._next += len(staged)
+        tk, done = self._launch(slot, frames, streams)
+        tickets = list(range(self._next, self._next + len(frames)))  # issued once the tick runs
+        self._next += len(frames)
         self._calls += 1
-        self._busy[slot] = (tickets, tk, done, [d for _, _, d in staged])
+        self._busy[slot] = (tickets, tk, done, frames)
         return tickets
 
-    def _launch(self, slot: int, kinds: tuple, staged: list, streams: Optional[List[int]] = None):
-        """Stage a tick's frames (and with tracking their stream indices, -1 to skip a frame) in the slot's ``_Tick``
-        for ``kinds`` (made on the key's first sight, made again when a JPEG frame outgrows its capacity) and run its
-        graph, or reserve its scratch, run its calls and capture them; returns the ``_Tick`` and the event of the
-        launch's end."""
+    def _launch(self, slot: int, frames: List[_Frame], streams: List[int]):
+        """Stage a tick's frames and stream indices (``_Tick.stage``) in the slot's ``_Tick`` for their keys (made on the
+        key's first sight, made again when a JPEG frame outgrows its capacity) and run its graph, or reserve its
+        scratch, run its calls and capture them; returns the ``_Tick`` and the event of the launch's end."""
         import torch
-        if self._g.max_batch < len(kinds):
+        keys = tuple(f.key for f in frames)
+        if self._g.max_batch < len(keys):
             self._stream.synchronize()  # the old handle's scratch may be in use
             self._g.close()
-            self._g = _new_grouper(len(kinds), self.device)
+            self._g = _new_grouper(len(keys), self.device)
             self._invalidate()
-        tk = self._ticks[slot].get(kinds)
-        sizes = [frame.size if rec is not None else 0 for frame, rec, _ in staged]
+        tk = self._ticks[slot].get(keys)
+        sizes = [f.data.size if f.key.source == "jpeg" else 0 for f in frames]
         if tk is None or any(s > c for s, c in zip(sizes, tk.caps)):
             caps = [max(1 << 16, 1 << (s - 1).bit_length()) if s else 0 for s in sizes]
             if tk is not None:
                 caps = [max(a, b) for a, b in zip(caps, tk.caps)]
                 self._drop_held(tk)
-            tk = self._ticks[slot][kinds] = _Tick(self, kinds, caps, [rec for _, rec, _ in staged])
+            tk = self._ticks[slot][keys] = _Tick(self, keys, caps, [f.rec for f in frames])
         if tk.graph is None:
             # Before every call-by-call run, not only on a key's first sight: a key whose graph was dropped (a buffer
             # moved, or the handle was replaced for a larger tick) would otherwise grow a buffer in its eager run and
             # free the address that graphs captured since then replay.
-            moved = self._g.reserve_frames(tk.members(), tk.n_items,
-                                           max_downsample=int(self.model_params["max_downsample"]))
+            members = [(k.height, k.width, item[0], item[2]) for k, items in zip(tk.keys, tk.plan) for item in items]
+            moved = self._g.reserve_frames(members, tk.n_items, max_downsample=int(self.model_params["max_downsample"]))
             if tk.jpeg and self._g.jpeg_reserve_frames(tk.formats, [tk.caps[j] for j in tk.jpeg]):
                 moved = True
             if moved:
                 self._invalidate()
         self._drop_held(tk)  # the maps of the key's earlier tick are overwritten
-        host = tk.up_host.numpy()
-        if tk.track is not None:
-            host[tk.streams_at:tk.streams_at + 4 * len(kinds)] = np.asarray(streams, np.int32).view(np.uint8)
-        for j, ((frame, rec, _), (H, W, kind)) in enumerate(zip(staged, kinds)):
-            if rec is not None:
-                jj = tk.jpeg.index(j)
-                host[tk.at[j]:tk.at[j] + frame.size] = frame
-                tk.nbytes[j] = frame.size
-                for k in ("data", "out", "decode_status"):  # the tick's device addresses, as the format's
-                    rec[k] = tk.formats[jj][k]
-                host[jj * JPEG_RECORD.itemsize:(jj + 1) * JPEG_RECORD.itemsize] = np.frombuffer(rec.tobytes(), np.uint8)
-            elif isinstance(kind, _YUVKind):  # the planes packed, in the upload or in the slot's device planes
-                layout = _yuv_layout(kind.format, H, W)
-                if kind.cuda:
-                    self._stream.wait_stream(torch.cuda.current_stream(self.device))
-                    with torch.cuda.stream(self._stream):
-                        for p, (o, (h, w)) in zip(frame.planes, layout):
-                            tk.yuv_dev[j][o:o + h * w].view(h, w).copy_(p, non_blocking=True)
-                    for p in frame.planes:
-                        p.record_stream(self._stream)
-                else:
-                    for p, (o, (h, w)) in zip(frame.planes, layout):
-                        host[tk.at[j] + o:tk.at[j] + o + h * w].reshape(h, w)[:] = p
-            elif kind:
-                self._stream.wait_stream(torch.cuda.current_stream(self.device))
-                with torch.cuda.stream(self._stream):
-                    tk.images[j].copy_(frame, non_blocking=True)
-                frame.record_stream(self._stream)
-            elif tk.pairs is None:
-                host[tk.at[j]:tk.at[j] + frame.size] = frame.reshape(-1)
-        if tk.pairs is not None:  # input_stage="host": each item's pair built by cv2 into the pinned copy of its input
-            for size, ms in tk.buckets.items():
-                for k, (i, t) in enumerate(ms):
-                    _host_pair(staged[i][0], tk.plan[i][t][1], tk.plan[i][t][2], self.model_params,
-                               out=tk.pairs[size][2 * k:2 * k + 2].numpy())
+        tk.stage(frames, streams)
         eager = tk.graph is None
         with torch.cuda.stream(self._stream):
             if eager:
@@ -1002,7 +1017,6 @@ class FrameStream:
 
     def _path(self, tk: _Tick) -> None:
         """One tick's work on the current stream: run as it is for the warm-up, recorded by ``_capture``."""
-        import torch
         g = self._g
         md, pv = int(self.model_params["max_downsample"]), int(self.model_params["padValue"])
         if tk.pairs is None or tk.track is not None:
@@ -1024,20 +1038,15 @@ class FrameStream:
                 x.copy_(tk.pairs[size], non_blocking=True)
         # A tick of one frame forwards each item alone, as predict does, so that submit equals predict + group with any
         # network; a larger tick forwards each input size's items at once.
-        entries = [[None] * tk.n_items for _ in tk.kinds]
-        with torch.no_grad():
-            for size, ms in tk.buckets.items():
-                step = 1 if len(tk.kinds) == 1 else len(ms)
-                for c in range(0, len(ms), step):
-                    out = _network_output(self.model, tk.inputs[size][2 * c:2 * (c + step)]).contiguous()
-                    for k, (i, t) in enumerate(ms[c:c + step]):
-                        entries[i][t] = (out[2 * k:2 * k + 2],) + tk.built[i][t]
+        entries = [[None] * tk.n_items for _ in tk.keys]
+        for size, ms in tk.buckets.items():
+            _forward_bucket(self.model, tk.inputs[size], ms, [tk.built[i][t] for i, t in ms],
+                            1 if len(tk.keys) == 1 else len(ms), entries)
         maps = list(zip(tk.heat, tk.paf))
-        g.postnet_ragged_items([(e, (H, W)) for e, (H, W, _) in zip(entries, tk.kinds)], outs=maps,
-                               nan_scrub=self._nan_scrub)
+        g.postnet_ragged_items([(e, k[:2]) for e, k in zip(entries, tk.keys)], outs=maps, nan_scrub=self._nan_scrub)
         g.set_wire_output(tk.rec.data_ptr())
         try:
-            g.group_ragged(maps, [H for H, _, _ in tk.kinds], self._gp, paf_as_f64=tk.as_f64)
+            g.group_ragged(maps, [k.height for k in tk.keys], self._gp, paf_as_f64=tk.as_f64)
         finally:
             g.set_wire_output(None)
         if tk.track is not None:
@@ -1054,7 +1063,7 @@ class FrameStream:
             with torch.cuda.graph(graph, pool=self._pool, stream=self._stream):
                 self._path(tk)
         except Exception as e:
-            raise GroupingError(f"capturing the path of a tick of {len(tk.kinds)} frame(s) failed (a model that "
+            raise GroupingError(f"capturing the path of a tick of {len(tk.keys)} frame(s) failed (a model that "
                                 "synchronises with the host or copies from it in its forward cannot be captured): "
                                 f"{type(e).__name__}: {e}") from e
         if self._pool is None:
@@ -1066,26 +1075,26 @@ class FrameStream:
         """Wait for the slot's tick and keep every frame's result (or the error it raises) under its ticket, with its
         maps for ``result(detail=True)``; frees the slot.  A JPEG frame the device decoder flagged is decoded with cv2
         from the slot's bytes and posed again as a one-frame tick in the same slot."""
-        tickets, tk, done, decoded = self._busy[slot]
+        tickets, tk, done, frames = self._busy[slot]
         self._busy[slot] = None
         done.synchronize()
         records = tk.rec_host.numpy().copy()
         ids = tk.ids_host.numpy().copy() if tk.track is not None else None
         for j, ticket in enumerate(tickets):
-            record, heat, paf, image = records[j], tk.heat[j], tk.paf[j], decoded[j]
+            record, heat, paf, image = records[j], tk.heat[j], tk.paf[j], frames[j].decoded
             frame_ids = None if ids is None else ids[j]
             if j in tk.jpeg and int(tk.status_host[tk.jpeg.index(j)]) != JPEG_OK:
-                image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + tk.nbytes[j]].numpy())
+                image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + frames[j].data.size].numpy())
                 self.host_decodes += 1
-                key, frame = ((image.shape[0], image.shape[1], False),), [(image, None, image)]
+                frame = _Frame(_Key(image.shape[0], image.shape[1], "image"), image, None, image)
                 # the tick tracked the frame as unobserved: posing it again tracks nothing, and its people get -1
-                again, d = self._launch(slot, key, frame) if ids is None else self._launch(slot, key, frame, [-1])
+                again, d = self._launch(slot, [frame], [-1])
                 d.synchronize()
                 record, heat, paf = again.rec_host[0].numpy().copy(), again.heat[0].clone(), again.paf[0].clone()
                 frame_ids = None
             elif j in tk.jpeg or j in tk.yuv:
                 image = tk.images[j]  # decoded or converted on the device: copied to the host if detail asks for it
-            self._keep(ticket, record, heat, paf, tk.kinds[j][0], tk.as_f64, frame_ids)
+            self._keep(ticket, record, heat, paf, tk.keys[j].height, tk.as_f64, frame_ids)
             self._held[ticket] = (heat, paf, tk.as_f64, image)
             tk.held.append(ticket)
 
@@ -1138,13 +1147,8 @@ class FrameStream:
         capacity-free tier from the frame's maps."""
         rec = wire.as_records(record, self._g.J, self._g.capR)[0]
         try:
-            if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
-                r = self._tier.group_unbounded(heat, paf, H, self._gp, paf_as_f64=as_f64, stream=self._tier_stream)
-                _check_status(r.status[0])
-                people = _people_of_result(r)
-            else:
-                _check_status(rec["status"])
-                people = wire.people_of(rec)
+            people = _people_of_record(rec, lambda: self._tier.group_unbounded(heat, paf, H, self._gp, paf_as_f64=as_f64,
+                                                                              stream=self._tier_stream))
             person_ids = None
             if self._track is not None:
                 person_ids = [-1] * len(people) if ids is None or rec["status"] else [int(v) for v in ids[:len(people)]]
@@ -1361,16 +1365,8 @@ def _people_of_batch(maps, extents, params) -> list:
     ``process()``'s return value (evaluate.py:523-543)."""
     extents = list(extents)
     g, n, buf, regroup = _group_ragged(maps, extents, params, records=True)
-    out = []
-    for i, rec in enumerate(wire.as_records(buf[:n].cpu().numpy(), g.J, g.capR)):
-        if _over_capacity(rec["status"]):  # the record holds at most capR persons: the tier's arrays hold them all
-            ri = regroup(i)
-            _check_status(ri.status[0])
-            out.append(_people_of_result(ri))
-            continue
-        _check_status(rec["status"])
-        out.append(wire.people_of(rec))
-    return out
+    return [_people_of_record(rec, functools.partial(regroup, i))
+            for i, rec in enumerate(wire.as_records(buf[:n].cpu().numpy(), g.J, g.capR))]
 
 
 def predict_many(coco, images_directory, validation_ids, params, model, model_params, heat_layers, paf_layers,

@@ -1,11 +1,12 @@
 """CPU: JPEG frames in ``dropin.FrameStream`` before they touch a device -- the C declarations of the frame decode,
-``submit``'s argument checks, the format key the host parser gives for the goldens, and the routing of the files the
-parser refuses to ``cv2.imdecode`` (the device path stubbed)."""
+the checks ``_admit`` makes for ``submit``, the tick key the host parser gives the goldens, and the routing of the files
+the parser refuses to ``cv2.imdecode`` (the device path stubbed)."""
 import ctypes
 import json
 import os
 import re
 
+import frames_stub
 import numpy as np
 import pytest
 
@@ -54,22 +55,8 @@ def test_frame_decode_without_a_handle_is_invalid(lib):
     assert lib.spg_jpeg_decode_frame(None, None, None, 1 << 16, None) == -1
 
 
-def _stream(input_stage="device"):
-    """A FrameStream without a device: only what submit reads before it stages a frame, and _launch recording the
-    tick's one frame and its parsed record instead of running the slot."""
-    fs = object.__new__(dropin.FrameStream)
-    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._calls = input_stage, 0, 0, 0, 0
-    fs._busy, fs.launched = [None], []
-
-    def launch(slot, kinds, staged):
-        assert len(kinds) == 1  # submit poses a tick of one frame
-        (frame, rec, _), = staged
-        fs.launched.append((frame, rec))
-        return None, None
-
-    fs._launch = launch
-    fs._finish = lambda slot: None
-    return fs
+def _admit(frames, input_stage="device"):
+    return dropin._admit(frames, [0] * len(frames), input_stage=input_stage, device=0, n_streams=None)
 
 
 @pytest.mark.parametrize("frame,match", [(b"", "empty"), (bytearray(), "empty"), (12, "uint8 BGR"),
@@ -77,7 +64,11 @@ def _stream(input_stage="device"):
                                          (b"not a jpeg", "imdecode")])
 def test_submit_arguments(lib, frame, match):
     with pytest.raises(ValueError, match=match):
-        _stream().submit(frame)
+        _admit([frame])
+    fs = frames_stub.stream()
+    with pytest.raises(ValueError, match=match):
+        fs.submit(frame)
+    assert fs.launched == [] and fs.host_decodes == 0
 
 
 def test_the_format_key_of_the_goldens(lib):
@@ -92,6 +83,8 @@ def test_the_format_key_of_the_goldens(lib):
         h, w = (key["frame_width"], key["frame_height"]) if key["orientation"] >= 5 else \
             (key["frame_height"], key["frame_width"])
         assert [h, w, 3] == case["cv2_shape"] == [int(rec["height"]), int(rec["width"]), 3], name
+        (f,), _, _ = _admit([_golden(name)])
+        assert f.key == (h, w, "jpeg", tuple(key.values())), name
         keys[name] = key
     assert keys["grey"]["n_components"] == 1 and (keys["grey"]["h_samp"], keys["grey"]["v_samp"]) == (1, 1)
     for name, hv in (("samp_444", (1, 1)), ("samp_422", (2, 1)), ("samp_440", (1, 2)), ("samp_420", (2, 2))):
@@ -106,27 +99,34 @@ def test_the_format_key_of_the_goldens(lib):
     assert keys["exif1_II"] == keys["exif_9_ignored"]
 
 
-def test_refused_files_go_to_cv2_in_a_one_frame_tick(lib):
-    fs = _stream()
+def test_admit_routes_refused_files_to_cv2(lib):
     prog = cv2.imencode(".jpg", np.full((16, 24, 3), 90, np.uint8), [cv2.IMWRITE_JPEG_PROGRESSIVE, 1])[1].tobytes()
     refused = [_golden("progressive"), _golden("samp_411"), _golden("fill_before_stuffing"), prog]
-    for k, data in enumerate(refused):
+    parsed = [_golden("samp_420"), memoryview(_golden("rst3")), bytearray(_golden("exif6_MM"))]
+    for data in refused:
+        (f,), _, decodes = _admit([data])
+        want = cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR)
+        assert decodes == 1 and f.rec is None and f.key == want.shape[:2] + ("image", None)  # keyed as a cv2 image
+        assert np.array_equal(f.data, want) and f.decoded is f.data
+    for data in parsed:
+        (f,), _, decodes = _admit([data])
+        assert decodes == 0 and f.rec is not None and int(f.rec["status"]) == grouping.JPEG_OK
+        assert f.key.source == "jpeg" and f.decoded is None
+        assert f.data.dtype == np.uint8 and f.data.tobytes() == bytes(data)
+    fs = frames_stub.stream()
+    for k, data in enumerate(refused + parsed):
         fs.submit(data)
-        frame, rec = fs.launched[-1]
-        assert rec is None and np.array_equal(frame, cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR))
-        assert fs.host_decodes == k + 1
-    for data in (_golden("samp_420"), memoryview(_golden("rst3")), bytearray(_golden("exif6_MM"))):
-        fs.submit(data)
-        frame, rec = fs.launched[-1]
-        assert rec is not None and int(rec["status"]) == grouping.JPEG_OK
-        assert frame.dtype == np.uint8 and frame.tobytes() == bytes(data)
-    assert fs.host_decodes == len(refused)
+        _, frames, _ = fs.launched[-1]
+        assert len(frames) == 1  # submit poses a tick of one frame
+        assert fs.host_decodes == min(k + 1, len(refused))
 
 
-def test_host_input_stage_decodes_jpeg_with_cv2_in_a_one_frame_tick(lib):
-    fs = _stream("host")
+def test_admit_decodes_jpeg_with_cv2_at_the_host_input_stage(lib):
     data = _golden("samp_420")
+    (f,), _, decodes = _admit([data], "host")
+    want = cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR)
+    assert decodes == 1 and f.rec is None and f.key == want.shape[:2] + ("image", None)
+    assert np.array_equal(f.data, want)
+    fs = frames_stub.stream("host")
     fs.submit(data)
-    frame, rec = fs.launched[-1]
-    assert rec is None and np.array_equal(frame, cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR))
-    assert fs.host_decodes == 1
+    assert len(fs.launched[-1][1]) == 1 and fs.host_decodes == 1

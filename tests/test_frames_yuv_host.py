@@ -1,11 +1,12 @@
 """CPU: YUV frames before they touch a device -- ``spg_yuv_to_bgr``'s declaration and member record against the real
-header, its refusal without a handle, ``dropin.YUVFrame``'s checks, and the tick key ``FrameStream`` forms for YUV
-frames (the launcher stubbed)."""
+header, its refusal without a handle, ``dropin.YUVFrame``'s checks, and the tick key ``_admit`` forms for YUV
+frames."""
 import ctypes
 import os
 import re
 import subprocess
 
+import frames_stub
 import numpy as np
 import pytest
 
@@ -131,74 +132,74 @@ def test_frame_checks():
         dropin.YUVFrame("yuyv", (np.lib.stride_tricks.as_strided(np.zeros(64, np.uint8), (4, 8), (4, 1)),))
 
 
-def _stream(input_stage="device", slots=2):
-    """A FrameStream without a device: _launch records the slot, the tick key and the staged frames instead of
-    running."""
-    fs = object.__new__(dropin.FrameStream)
-    fs.input_stage, fs.device, fs.host_decodes, fs._next, fs._calls = input_stage, 0, 0, 0, 0
-    fs._busy, fs.launched = [None] * slots, []
-
-    def launch(slot, kinds, staged):
-        fs.launched.append((slot, kinds, staged))
-        return None, None
-
-    fs._launch = launch
-    fs._finish = lambda slot: None
-    return fs
+def _admit(frames, input_stage="device"):
+    return dropin._admit(frames, [0] * len(frames), input_stage=input_stage, device=0, n_streams=None)
 
 
 def _cuda_frame(fmt, H, W, device=0):
-    """A YUVFrame whose planes claim to be CUDA tensors on ``device`` (built without a device: the kind is all the tick
-    key reads)."""
+    """A YUVFrame whose planes claim to be CUDA tensors on ``device`` (built without a device: its device is all the
+    tick key reads)."""
     f = dropin.YUVFrame(fmt, _planes(fmt, H, W))
     f.device = device
     return f
 
 
-def test_tick_key_of_yuv_frames(lib):
-    fs = _stream()
+def test_admit_keys_yuv_frames(lib):
     with open(os.path.join(GOLDEN, "samp_420.jpg"), "rb") as fh:
         jpeg = fh.read()
     rec = grouping.jpeg_parse(jpeg)
     host = dropin.YUVFrame("nv12", _planes("nv12", 6, 10))
     cuda = _cuda_frame("nv12", 6, 10)
     img = np.zeros((6, 10, 3), np.uint8)
-    assert fs.submit_many([host, cuda, img, jpeg, dropin.YUVFrame("yuyv", _planes("yuyv", 5, 10))]) == [0, 1, 2, 3, 4]
-    _, kinds, staged = fs.launched[-1]
-    assert [k[:2] for k in kinds] == [(6, 10), (6, 10), (6, 10), (int(rec["height"]), int(rec["width"])), (5, 10)]
-    k_host, k_cuda, k_img, k_jpeg, k_yuyv = (k[2] for k in kinds)
-    assert k_host != k_cuda  # host and CUDA planes: two kinds
-    assert k_host == dropin._YUVKind("nv12", False) and k_cuda == dropin._YUVKind("nv12", True)
-    assert k_yuyv == dropin._YUVKind("yuyv", False)
-    # neither is taken for a JPEG frame (a tuple), an image (a bool) or each other's format
-    assert isinstance(k_jpeg, tuple)
-    for k in (k_host, k_cuda, k_yuyv):
-        assert not isinstance(k, (tuple, bool)) and k not in (True, False) and k != k_jpeg
-    assert staged[0][0] is host and staged[0][1] is None and staged[1][0] is cuda
+    frames, _, decodes = _admit([host, cuda, img, jpeg, dropin.YUVFrame("yuyv", _planes("yuyv", 5, 10))])
+    keys = tuple(f.key for f in frames)
+    assert [k[:2] for k in keys] == [(6, 10), (6, 10), (6, 10), (int(rec["height"]), int(rec["width"])), (5, 10)]
+    k_host, k_cuda, k_img, k_jpeg, k_yuyv = keys
+    assert k_host != k_cuda  # host and CUDA planes: two keys
+    assert k_host == (6, 10, "yuv", "nv12") and k_cuda == (6, 10, "yuv_cuda", "nv12")
+    assert k_yuyv == (5, 10, "yuv", "yuyv")
+    # neither is taken for a JPEG frame, an image or each other's format
+    assert k_jpeg.source == "jpeg" and k_img == (6, 10, "image", None)
+    for k in (k_host, k_cuda):
+        assert k not in (k_img, k_jpeg)
+    assert frames[0].data is host and frames[0].rec is None and frames[1].data is cuda and decodes == 0
     # the same frames again form the same key; another format or another side forms another
-    fs.submit_many([dropin.YUVFrame("nv12", _planes("nv12", 6, 10, seed=1)), _cuda_frame("nv12", 6, 10), img, jpeg,
-                    dropin.YUVFrame("yuyv", _planes("yuyv", 5, 10, seed=2))])
-    assert fs.launched[-1][1] == kinds
-    fs.submit(dropin.YUVFrame("i420", _planes("i420", 6, 10)))
-    assert fs.launched[-1][1] == ((6, 10, dropin._YUVKind("i420", False)),)
-    assert len({fs.launched[-1][1], ((6, 10, k_host),), ((6, 10, k_cuda),)}) == 3
+    again, _, _ = _admit([dropin.YUVFrame("nv12", _planes("nv12", 6, 10, seed=1)), _cuda_frame("nv12", 6, 10), img, jpeg,
+                          dropin.YUVFrame("yuyv", _planes("yuyv", 5, 10, seed=2))])
+    assert tuple(f.key for f in again) == keys
+    (i420,), _, _ = _admit([dropin.YUVFrame("i420", _planes("i420", 6, 10))])
+    assert i420.key == (6, 10, "yuv", "i420")
+    assert len({(i420.key,), (k_host,), (k_cuda,)}) == 3
+    # every layout, on the host and on the device
+    for fmt in yp.FORMATS:
+        got, _, _ = _admit([dropin.YUVFrame(fmt, _planes(fmt, 6, 10)), _cuda_frame(fmt, 6, 10)])
+        assert [f.key for f in got] == [(6, 10, "yuv", fmt), (6, 10, "yuv_cuda", fmt)]
+    # submit and submit_many pose the same key
+    fs = frames_stub.stream()
+    fs.submit(host)
+    fs.submit_many([host])
+    assert frames_stub.keys(fs.launched[0][1]) == frames_stub.keys(fs.launched[1][1]) == ((6, 10, "yuv", "nv12"),)
 
 
 def test_yuv_frames_on_another_device_or_host_stage(lib):
     with pytest.raises(ValueError, match="cuda:0"):
-        _stream().submit(_cuda_frame("nv12", 6, 10, device=1))
+        _admit([_cuda_frame("nv12", 6, 10, device=1)])
     with pytest.raises(ValueError, match="host frames"):
-        _stream("host").submit(_cuda_frame("nv12", 6, 10))
-    assert _stream().launched == []
+        _admit([_cuda_frame("nv12", 6, 10)], "host")
+    fs = frames_stub.stream()
+    with pytest.raises(ValueError, match="cuda:0"):
+        fs.submit(_cuda_frame("nv12", 6, 10, device=1))
+    assert fs.launched == []
 
 
 @pytest.mark.parametrize("fmt", yp.FORMATS)
-def test_host_input_stage_converts_with_cv2(lib, fmt):
-    fs = _stream("host")
+def test_admit_converts_yuv_with_cv2_at_the_host_input_stage(lib, fmt):
     planes = _planes(fmt, 6, 10)
-    assert fs.submit(dropin.YUVFrame(fmt, planes)) == 0
-    _, kinds, staged = fs.launched[-1]
+    (f,), _, decodes = _admit([dropin.YUVFrame(fmt, planes)], "host")
     want = cv2.cvtColor(yp.cv2_layout(fmt, planes), yp.cv2_code(fmt))
-    assert kinds == ((6, 10, False),)  # posed as an image
-    assert np.array_equal(staged[0][0], want) and staged[0][2] is staged[0][0]  # and kept for detail's image
-    assert fs.host_decodes == 0  # which counts JPEG frames only
+    assert f.key == (6, 10, "image", None)  # posed as an image
+    assert np.array_equal(f.data, want) and f.decoded is f.data  # and kept for detail's image
+    assert decodes == 0  # which counts JPEG frames only
+    fs = frames_stub.stream("host")
+    assert fs.submit(dropin.YUVFrame(fmt, planes)) == 0 and fs.host_decodes == 0
+    assert frames_stub.keys(fs.launched[-1][1]) == ((6, 10, "image", None),)
