@@ -13,15 +13,15 @@
 //   l2:    term = (d d) m
 // and its gradient, autograd's chain in float32: gA = G m; pa = (gA factor) (2 d); pb = (gA (d d)) sign(u), negated
 // when st = s; grad = pa + pb (l2: grad = gA (2 d)).  G of (scale j, stack k) is autograd's chain outermost first,
-// ((((g / B) / sum_sw) sw_j) / sum_nw) nw_k, where CUDA torch divides by a host scalar as a multiply by its float32
-// reciprocal.  Built with -fmad=false like the rest of the library: no contraction can move a bit.
+// ((((g / B) / sum_sw) sw_j) / sum_nw) nw_k, where CUDA torch divides by a host scalar b as a multiply by
+// (float)(1.0 / b).  Built with -fmad=false like the rest of the library: no contraction can move a bit.
 //
 // One CTA per (sample, channel, band of kLossBand scale-0 rows): it stages the band's labels and mask in shared memory,
 // builds both pyramids there (scale j's band is kLossBand >> j rows), then streams the band's pixels of all nstack x 5
 // prediction tensors: thread t owns the groups of kLossVec consecutive elements t, t + kLossThreads, ... of a band, read
 // with one vector access when the tensor's rows allow it, so the order of a thread's sum never depends on alignment.
 //   loss_forward_kernel:  per (scale, stack) a float64 sum of the float32 terms per thread, reduced over the CTA in a
-//     fixed order into one partial per CTA; the last CTA to finish (a ticket the handle owns, reset by that CTA) adds the
+//     fixed order into one partial per CTA; the last CTA to finish (a ticket the caller owns, reset by that CTA) adds the
 //     partials in a fixed order, rounds each sum to float32 and combines them into the loss in the reference's order of
 //     float32 operations.  Nothing depends on the SM count: the bits repeat from run to run and from card to card.
 //   loss_backward_kernel: every prediction's gradient written once, recomputed from the inputs and *grad_output (a
@@ -56,8 +56,8 @@ struct LossArgs {
     const float *mask;              // [B][1][H][W]
     float *sums;                    // forward: [5][nstack]
     float *loss;                    // forward: the scalar
-    double *partial;                // forward: [5 * nstack][gridDim.x]
-    unsigned int *ticket;           // forward: CTAs done; 0 between launches
+    double *partial;                // forward: [5 * nstack][gridDim.x], the call's own
+    unsigned int *ticket;           // forward: CTAs done, the call's own; 0 on entry, left 0 by the last CTA
     const float *grad_output;       // backward
     int focal, nstack, B, C, H, W, heat_start, bkg_start, bands;
     float w_bkg, w_heat;            // channel C - 2; channels heat_start..bkg_start-1

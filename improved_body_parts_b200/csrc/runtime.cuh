@@ -43,7 +43,6 @@ struct spg_handle {
     unsigned long long armed_value = 0;
     spg::Scratch heat_acc;  // postnet: float64 accumulator of the keypoint maps over the scale loop
     spg::Scratch pre_grid;  // prenet: the padded uint8 images of a launch's rotated members
-    spg::Scratch loss_partial;  // spg_loss_forward: the ticket (first 256 bytes), then the float64 partial sums of the CTAs
     spg::Scratch coco_sort, coco_acc;  // spg_coco_evaluate: sort keys and CUB scratch; spg_coco_accumulate: the curves
     spg::Scratch jpeg;  // spg_jpeg_decode_ragged: records, unstuffed streams, subsequence states, coefficients, planes
     // the capacity-free tier (spg_group_unbounded): fixed-size words, tables sized by the peak counts, the candidate list

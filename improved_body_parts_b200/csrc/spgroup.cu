@@ -239,7 +239,7 @@ void spg_destroy(spg_handle *h) {
     DeviceGuard guard(h->device);
     cudaDeviceSynchronize();
     for (void *p : h->allocs) cudaFree(p);
-    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid, &h->loss_partial, &h->coco_sort, &h->coco_acc, &h->jpeg, &h->ub_small, &h->ub_peaks, &h->ub_cands, &h->ub_people})
+    for (Scratch *s : {&h->in_heat, &h->in_paf, &h->heat_acc, &h->pre_grid, &h->coco_sort, &h->coco_acc, &h->jpeg, &h->ub_small, &h->ub_peaks, &h->ub_cands, &h->ub_people})
         if (s->p) cudaFree(s->p);
     if (h->done_counter) cudaFree(h->done_counter);
     for (auto &s : h->streams)

@@ -208,10 +208,11 @@ int loss_setup(spg_handle *h, const spg_loss_params *p, const float *mask, const
     a.w_heat = (float)p->keypoint_task_weight;
     for (int k = 0; k < p->nstack; k++) a.nw[k] = (float)p->nstack_weight[k];
     for (int j = 0; j < kLossScales; j++) a.sw[j] = (float)p->scale_weight[j];
-    // CUDA torch divides by a host scalar b as a multiply by 1.0f / (float)b
-    a.inv_batch = 1.0f / (float)p->batch_divisor;
-    a.inv_sw = 1.0f / (float)p->scale_weight_sum;
-    a.inv_nw = 1.0f / (float)p->nstack_weight_sum;
+    // CUDA torch divides a float32 tensor by a host scalar b as a multiply by its reciprocal taken in float64 and
+    // rounded to float32, (float)(1.0 / b): not 1.0f / (float)b, which differs for b = 3.9 or 4.9
+    a.inv_batch = (float)(1.0 / p->batch_divisor);
+    a.inv_sw = (float)(1.0 / p->scale_weight_sum);
+    a.inv_nw = (float)(1.0 / p->nstack_weight_sum);
     const size_t vb = kLossVec * kern->esz;
     for (int k = 0; k < p->nstack; k++)
         for (int j = 0; j < kLossScales; j++) {
@@ -237,8 +238,16 @@ int loss_setup(spg_handle *h, const spg_loss_params *p, const float *mask, const
 
 }  // namespace
 
+int64_t spg_loss_workspace_bytes(const spg_loss_params *p) {
+    if (!p || p->nstack < 1 || p->nstack > kLossMaxStacks || p->batch < 1 || p->channels < 1 || p->height < kLossBand ||
+        p->height % kLossBand)
+        return -1;
+    return (int64_t)sizeof(double) * kLossScales * p->nstack * p->batch * p->channels * (p->height / kLossBand);
+}
+
 int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
-                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, void *stream) {
+                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, uint32_t *ticket,
+                     double *partials, void *stream) {
     if (!h) return SPG_E_INVALID;
     const LossKernels *kern;
     LossArgs a;
@@ -248,16 +257,13 @@ int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *
     DeviceGuard guard(h->device);  // loss_setup reads the kernels' attributes on the handle's device
     if ((rc = loss_setup(h, params, mask_miss, labels, preds, pred_dtype, false, kern, a, ctas, smem))) return rc;
     if (!stack_sums || !loss) return fail(h, SPG_E_INVALID, "stack_sums or loss is NULL");
-    const cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t need = 256 + sizeof(double) * kLossScales * a.nstack * (size_t)ctas;
-    const bool fresh = h->loss_partial.bytes < need;
-    if ((rc = grow(h, h->loss_partial, need))) return rc;
-    if (fresh) SPG_CUDA(h, cudaMemsetAsync(h->loss_partial.p, 0, 256, st));  // the ticket starts at 0; each launch leaves it so
-    a.ticket = static_cast<unsigned int *>(h->loss_partial.p);
-    a.partial = reinterpret_cast<double *>(static_cast<unsigned char *>(h->loss_partial.p) + 256);
+    if (!ticket || !aligned(ticket, sizeof(uint32_t))) return fail(h, SPG_E_INVALID, "ticket is NULL or not 4-byte aligned");
+    if (!partials || !aligned(partials, sizeof(double))) return fail(h, SPG_E_INVALID, "partials is NULL or not 8-byte aligned");
+    a.ticket = ticket;
+    a.partial = partials;
     a.sums = stack_sums;
     a.loss = loss;
-    return launch(h, kStageLoss, kern->fwd_name, kern->fwd, dim3((unsigned)ctas), kLossThreads, smem, st, a);
+    return launch(h, kStageLoss, kern->fwd_name, kern->fwd, dim3((unsigned)ctas), kLossThreads, smem, static_cast<cudaStream_t>(stream), a);
 }
 
 int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,

@@ -222,7 +222,8 @@ _PROTOTYPES = {
     "spg_targets_maps": (_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
     "spg_targets_tint": (_int, [_ptr, _ptr, _i32, _ptr]),  # samples: a TARGET_TINT array
     # params: a LOSS_PARAMS record; preds: a LOSS_PRED array
-    "spg_loss_forward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr]),
+    "spg_loss_workspace_bytes": (_i64, [_ptr]),
+    "spg_loss_forward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr]),
     "spg_loss_backward": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr]),
     # params / data / eval: a COCO_PARAMS / COCO_DATA / COCO_EVAL record
     "spg_coco_evaluate": (_int, [_ptr, _ptr, _ptr, _ptr, _ptr]),
@@ -1023,13 +1024,21 @@ class Grouper:
                self._h)
 
     # -- training loss (loss.py builds the records) ---------------------------------------------------------------
+    def loss_workspace_bytes(self, params: np.ndarray) -> int:
+        """``spg_loss_workspace_bytes``: the bytes of float64 partial sums one ``loss_forward`` of ``params`` needs."""
+        n = self._lib.spg_loss_workspace_bytes(self._records(params, LOSS_PARAMS).ctypes.data)
+        if n < 0:
+            raise GroupingError("spg_loss_workspace_bytes: the loss parameters are out of range")
+        return int(n)
+
     def loss_forward(self, params: np.ndarray, mask_miss: int, labels: int, preds: np.ndarray, dtype: int,
-                     stack_sums: int, loss: int, stream=None) -> None:
+                     stack_sums: int, loss: int, ticket: int, partials: int, stream=None) -> None:
         """``spg_loss_forward``: ``params`` one ``LOSS_PARAMS`` record, ``preds`` a ``LOSS_PRED`` array; the tensors are
-        device addresses on the handle's device.  Asynchronous on ``stream``."""
+        device addresses on the handle's device, ``ticket`` a zeroed uint32 and ``partials`` ``loss_workspace_bytes``
+        bytes, both the call's own.  Asynchronous on ``stream``."""
         p, r = self._records(params, LOSS_PARAMS), self._records(preds, LOSS_PRED)
         _check(self._lib.spg_loss_forward(self._h, p.ctypes.data, mask_miss, labels, r.ctypes.data, dtype, stack_sums, loss,
-                                          self._stream_ptr(stream)), "spg_loss_forward", self._h)
+                                          ticket, partials, self._stream_ptr(stream)), "spg_loss_forward", self._h)
 
     def loss_backward(self, params: np.ndarray, mask_miss: int, labels: int, preds: np.ndarray, dtype: int,
                       grad_output: int, stream=None) -> None:

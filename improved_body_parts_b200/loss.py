@@ -20,7 +20,8 @@ tensors per scale for the backward.  Here both directions are one CUDA kernel ea
   the copy); any batch, channel and row strides are read in place.
 
 Malformed shapes, dtypes and devices raise ``ValueError``.  The handle is the per-device one ``targets`` caches; there
-is no CPU path.
+is no CPU path.  Each forward takes its own ticket and partial sums from torch's allocator on the current stream, so
+losses may run concurrently on different streams and a forward captured in a CUDA graph needs no warm-up call.
 """
 from __future__ import annotations
 
@@ -106,8 +107,12 @@ class _FusedLoss(torch.autograd.Function):
         g = targets._Device.for_device(dev.index)
         sums = torch.empty((SCALES, int(params["nstack"][0])), dtype=torch.float32, device=dev)
         loss = torch.empty((), dtype=torch.float32, device=dev)
+        # the call's own ticket and partial sums, from torch's allocator on the current stream (the graph's pool while
+        # capturing): no buffer is shared with another call, another stream or a captured graph
+        ticket = torch.zeros((), dtype=torch.int32, device=dev)
+        partials = torch.empty(g.loss_workspace_bytes(params) // 8, dtype=torch.float64, device=dev)
         g.loss_forward(params, mask_miss.data_ptr(), labels.data_ptr(), _records(preds), _DTYPES[preds[0].dtype],
-                       sums.data_ptr(), loss.data_ptr())
+                       sums.data_ptr(), loss.data_ptr(), ticket.data_ptr(), partials.data_ptr())
         ctx.params = params
         ctx.save_for_backward(mask_miss, labels, *preds)
         ctx.mark_non_differentiable(sums)

@@ -507,19 +507,25 @@ typedef struct spg_loss_pred {
     int64_t batch_stride, chan_stride, row_stride;
     int64_t grad_batch_stride, grad_chan_stride, grad_row_stride;
 } spg_loss_pred;
+/* Bytes of float64 partial sums spg_loss_forward needs for `params`: 8 x 5 x nstack x batch x channels x height / 16
+ * (one per (scale, stack) and CTA); -1 when params is NULL or its nstack, batch, channels or height is out of range. */
+int64_t spg_loss_workspace_bytes(const spg_loss_params *params);
 /* The loss of the predictions `preds` (nstack * 5 records, `pred_dtype` SPG_F32 | SPG_BF16 | SPG_F16, all the same)
  * against labels (float32 [B][C][H][W]) and mask_miss (float32 [B][1][H][W]), both contiguous and 16-byte aligned:
  * stack_sums [5][nstack] float32 device (the per-stack sums the reference prints, float64 accumulation rounded once) and
  * *loss float32 device (combined from those sums in the reference's order of float32 operations).  A low-precision
- * prediction is the reference applied to its float32 value.  Every argument is validated before the first launch
- * (SPG_E_INVALID names the bad one); asynchronous on `stream`; `params` and `preds` may be reused on return.  The
- * handle's partial-sum buffer grows on demand (a call with no larger shape than an earlier one allocates nothing); calls
- * on one handle must not run concurrently on different streams. */
+ * prediction is the reference applied to its float32 value.  The call's workspace is the caller's: `ticket` one uint32
+ * device word that is 0 when the call starts (the call leaves it 0 again, so calls in order on one stream may share it)
+ * and `partials` spg_loss_workspace_bytes(params) device bytes, 8-byte aligned, needing no initial value.  Calls with
+ * workspaces of their own may run concurrently on different streams, and a call captured in a CUDA graph keeps
+ * pointing at the workspace it was given.  Every argument is validated before the first launch (SPG_E_INVALID names the
+ * bad one); asynchronous on `stream`; allocates nothing; `params` and `preds` may be reused on return. */
 int spg_loss_forward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
-                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, void *stream);
+                     const spg_loss_pred *preds, int32_t pred_dtype, float *stack_sums, float *loss, uint32_t *ticket,
+                     double *partials, void *stream);
 /* Every prediction's gradient of (*grad_output, a float32 device scalar) x loss, written once into preds[i].grad in the
  * prediction's dtype (the float32 gradient rounded once).  Recomputed from the inputs: independent of any forward call.
- * Validation, asynchrony and reuse as spg_loss_forward; allocates nothing. */
+ * Validation, asynchrony and reuse as spg_loss_forward; needs no workspace and allocates nothing. */
 int spg_loss_backward(spg_handle *h, const spg_loss_params *params, const float *mask_miss, const float *labels,
                       const spg_loss_pred *preds, int32_t pred_dtype, const float *grad_output, void *stream);
 

@@ -5,7 +5,7 @@ alpha = beta = 0) and ``models/loss_model_parallel.py:MultiTaskLossParallel`` (p
 in the same order so that it carries whichever device's arithmetic its tensors are on: on CPU it equals the reference
 class bit for bit (tests/golden/loss/), on CUDA it is what the reference computes on the GPU it trains on.  Gradients
 come from autograd.  ``port_loss`` also returns the elementwise terms, so that a test can form exact per-(scale, stack)
-sums.
+sums, and ``combine`` is its last step alone, to be applied to another implementation's per-stack sums.
 """
 from __future__ import annotations
 
@@ -30,16 +30,25 @@ def scale_targets(mask_miss, labels, size, focal: bool):
     return gt, m
 
 
-def _stack_combine(per_stack, nstack_weight):
-    weighted = [per_stack[k] * nstack_weight[k] for k in range(len(nstack_weight))]
-    return sum(weighted) / sum(nstack_weight)
+def combine(stack_sums, nstack_weight, scale_weight, batch_size=1, focal=True):
+    """The reference's loss from its per-stack sums (``stack_sums[j][k]``, one 0-dim or ``[nstack]`` tensor per scale, or
+    a ``[5, nstack]`` tensor): the stacks weighted and summed per scale, the scales weighted and summed, each sum with
+    Python's ``sum()`` and each division by a Python number, in that order.  ``focal``: divided by ``batch_size``."""
+    per_scale = []
+    for j in range(5):
+        weighted = [stack_sums[j][k] * nstack_weight[k] for k in range(len(nstack_weight))]
+        per_scale.append(sum(weighted) / sum(nstack_weight) * scale_weight[j])
+    loss = sum(per_scale) / sum(scale_weight)
+    if focal:
+        loss = loss / batch_size
+    return loss
 
 
 def port_loss(pred_tuple, mask_miss, labels, *, nstack, scale_weight, nstack_weight, batch_size=1, focal=True,
               heat_start=0, bkg_start=0, multi_task_weight=0.1, keypoint_task_weight=1, offset_start=None):
     """The reference's loss of ``pred_tuple[k][j]`` (k < nstack, j < 5) against ``(mask_miss, labels)``.  ``focal``:
     MultiTaskLoss (divided by ``batch_size``); else MultiTaskLossParallel (channels ``:offset_start``, no division)."""
-    per_scale, sums, terms = [], [], []
+    per_stack_sums, sums, terms = [], [], []
     for j in range(5):
         s = torch.cat([pred_tuple[k][j][None, ...] for k in range(nstack)], dim=0)
         if not focal:
@@ -55,10 +64,7 @@ def port_loss(pred_tuple, mask_miss, labels, *, nstack, scale_weight, nstack_wei
         else:
             out = (s - gt) ** 2 * m
         per_stack = out.sum(dim=(1, 2, 3, 4))
+        per_stack_sums.append(per_stack)
         sums.append(per_stack.detach())
         terms.append(out.detach())
-        per_scale.append(_stack_combine(per_stack, nstack_weight) * scale_weight[j])
-    loss = sum(per_scale) / sum(scale_weight)
-    if focal:
-        loss = loss / batch_size
-    return PortResult(loss, sums, terms)
+    return PortResult(combine(per_stack_sums, nstack_weight, scale_weight, batch_size, focal), sums, terms)

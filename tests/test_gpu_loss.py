@@ -43,7 +43,7 @@ def _synthetic_targets(B, H, W, seed, dev):
     idx = rng.choice(labels.size, labels.size // 10, replace=False)
     labels.flat[idx] = sp[rng.integers(0, 3, idx.size)]
     mask = rng.integers(0, 256, (B, 1, H, W)).astype(np.float32) / np.float32(255)
-    mask[:, 0, :32, :32] = (np.add.outer(np.arange(32), np.arange(32)) % 2).astype(np.float32)
+    mask[:, 0, :32, :32] = (np.add.outer(np.arange(32), np.arange(32)) % 2).astype(np.float32)[:H, :W]
     mask[:, 0, 40:56, :] = np.float32(128) / np.float32(255)
     return torch.from_numpy(mask).to(dev), torch.from_numpy(labels).to(dev)
 
@@ -257,7 +257,7 @@ def test_forward_and_backward_capture_in_a_cuda_graph(cuda_device):
     crit = _criterion(opt, True)
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):  # the warm-up call: the handle and its partial-sum buffer exist before the capture
+    with torch.cuda.stream(side):  # the eager bits to compare with (test_gpu_loss_space.py captures without this call)
         loss = crit(pt, (mask, labels))
         loss.backward()
         eager = [L.grad.clone() for L in leaves]

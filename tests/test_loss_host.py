@@ -98,3 +98,31 @@ def test_loss_records_match_the_header(tmp_path):
     src = open(os.path.join(ROOT, "include", "spgroup.h")).read()
     assert "SPG_BF16 = 4" in src and grouping.BF16 == 4
     assert "SPG_LOSS_FOCAL = 0" in src and "SPG_LOSS_L2 = 1" in src and (grouping.LOSS_FOCAL, grouping.LOSS_L2) == (0, 1)
+
+
+def test_the_case_table_covers_every_axis():
+    """tests/loss_cases.py, which tests/test_gpu_loss_space.py runs: every stack count, weight, channel layout, target
+    shape and divisor the loss admits and has edges at."""
+    import sys
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from loss_cases import CASES, device_bytes
+    assert len({c.name for c in CASES}) == len(CASES)
+    assert {c.nstack for c in CASES} == set(range(1, 9))
+    assert any(c.nstack >= 5 and c.focal for c in CASES) and any(c.nstack >= 7 and not c.focal for c in CASES)
+    assert {0.0, 0.1, 0.3, 2.5} <= {w for c in CASES for w in c.nstack_weight}
+    assert any(0.0 in c.scale_weight for c in CASES)
+    assert {2, 3, 12, 50, 57} <= {c.C for c in CASES}
+    focal = [c for c in CASES if c.focal]
+    assert any(c.heat[0] == c.heat[1] for c in focal)                       # empty keypoint range
+    assert any(c.heat[0] == c.heat[1] == c.C for c in focal)                # empty, bkg_start == C
+    assert any(c.heat[0] <= c.C - 2 < c.heat[1] and c.heat[0] > 0 and c.heat[1] < c.C for c in focal)  # covers C - 2
+    assert any(c.heat[0] == 0 < c.heat[1] for c in focal)                   # starts at 0
+    assert any(0 < c.heat[0] < c.heat[1] == c.C for c in focal)             # ends at C
+    assert all(0 <= c.heat[0] <= c.heat[1] <= c.C for c in focal)
+    assert all(c.extra == 3 for c in CASES if not c.focal) and any(not c.focal for c in CASES)
+    shapes = {(c.H, c.W, c.B) for c in CASES}
+    assert {(16, 16), (16, 256), (256, 16), (48, 80), (112, 208)} <= {(h, w) for h, w, _ in shapes}
+    assert {(128, 128, 16), (256, 384, 2), (512, 512, 1)} <= shapes
+    assert any(c.batch_size != c.B for c in focal)
+    assert any(c.C % 2 for c in CASES)
+    assert all(device_bytes(c) < 2 ** 31 for c in CASES), [(c.name, device_bytes(c)) for c in CASES]
