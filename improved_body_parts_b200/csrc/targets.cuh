@@ -7,8 +7,9 @@
 // through the same warp (their own border values) and cv2.resize(..., INTER_AREA) by the integer factor `stride`, then the
 // table.  OpenCV's uint8 warp is fixed point: the coordinates of warp_linear (warp_coords / warp_tap), then short weights
 // 32 * (32 - ay)(32 - ax) ... summing to 2^15, the four taps combined in int (taps outside the source read the border
-// value) and (sum + 2^14) >> 15.  INTER_AREA by an integer factor is rint(box sum / stride^2), ties to even.  A mask
-// pixel is the box of stride x stride warped pixels it consumes, so the full-size masks are never written.
+// value) and (sum + 2^14) >> 15.  INTER_AREA by an integer factor is OpenCV's fast-area arithmetic (area_u8): (box sum
+// + 2) >> 2 at stride 2, else rint(float32(box sum) * float32(1 / stride^2)), ties to even.  A mask pixel is the box of
+// stride x stride warped pixels it consumes, so the full-size masks are never written.
 //
 // targets_maps_kernel: per sample the [L + K + 2][h][w] float32 target, every value written once by one thread:
 //   body-part channels 0..L-1: the reference's distances() Gaussian of every visible limb (both ends v < 2) whose box
@@ -82,6 +83,15 @@ __device__ __forceinline__ int warp_u8(const WarpTap &t, const unsigned char *g,
     return (acc + (1 << 14)) >> 15;
 }
 
+// cv2.resize(INTER_AREA)'s uint8 value of a box sum s by the integer factor f (f^2 <= 2^24): the 2 x 2 path's
+// (s + 2) >> 2 (ties up), else the generic fast-area path's saturate_cast<uchar>(s * (1.f / f^2)) -- an int sum, a float32
+// reciprocal and product, rounded ties to even.  The product is not always the correctly rounded quotient (f = 22, 34, ...).
+__device__ __forceinline__ int area_u8(int s, int f) {
+    if (f == 2) return (s + 2) >> 2;
+    const int v = __float2int_rn(__fmul_rn(__int2float_rn(s), __fdiv_rn(1.0f, (float)(f * f))));
+    return min(max(v, 0), 255);
+}
+
 __global__ void __launch_bounds__(kTgtThreads) targets_warp_kernel(const __grid_constant__ TgtWarpRagged r) {
     const TgtWarpMember &a = ragged_member(r, (int)blockIdx.x);
     const TgtCommon &c = r.c;
@@ -111,9 +121,8 @@ __global__ void __launch_bounds__(kTgtThreads) targets_warp_kernel(const __grid_
             s_miss += warp_u8(t, a.miss, a.mask_stride, 1, a.w, a.h, c.border[3]);
             s_all += warp_u8(t, a.all, a.mask_stride, 1, a.w, a.h, c.border[4]);
         }
-    const float area = (float)(c.stride * c.stride);  // the quotient is correctly rounded; rint then ties to even
-    a.miss_out[p] = c.lut[__float2int_rn(__fdiv_rn((float)s_miss, area))];
-    a.all_out[p] = c.lut[__float2int_rn(__fdiv_rn((float)s_all, area))];
+    a.miss_out[p] = c.lut[area_u8(s_miss, c.stride)];
+    a.all_out[p] = c.lut[area_u8(s_all, c.stride)];
 }
 
 // ---- colour distortion -----------------------------------------------------------------------------------------------
@@ -271,8 +280,10 @@ struct TgtItem {
     double ax, ay, den;       // limbs: x1, y1, norm2 + 1e-6
 };
 
-// [lo, hi) clipped to [0, n) in double (no int overflow for any finite input): false when empty
+// [lo, hi) clipped to [0, n) in double (no int overflow for any finite input): false when empty.  A NaN bound (a NaN
+// joint coordinate) is empty too, as +-inf ones are: fmax / fmin would replace it by the map's edge.
 __device__ __forceinline__ bool tgt_clip(double lo, double hi, int n, int &a, int &b) {
+    if (isnan(lo) || isnan(hi)) return false;
     lo = fmax(lo, 0.0);
     hi = fmin(hi, (double)n);
     if (!(lo < hi)) return false;

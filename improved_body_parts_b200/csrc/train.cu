@@ -43,6 +43,9 @@ int targets_common(spg_handle *h, const spg_target_params *p, TgtCommon &c) {
         return fail(h, SPG_E_INVALID, "stride %d or output %dx%d outside [1, 32767]", p->stride, p->out_h, p->out_w);
     if (p->out_h % p->stride || p->out_w % p->stride)
         return fail(h, SPG_E_INVALID, "stride %d does not divide the output %dx%d", p->stride, p->out_h, p->out_w);
+    // a mask pixel's box sum of up to 255 * stride^2 bytes is an int, as in OpenCV's area resize
+    if (255LL * p->stride * p->stride > 0x7fffffffLL)
+        return fail(h, SPG_E_INVALID, "stride %d: a mask box sum of 255 * stride^2 overflows int (stride <= 2901)", p->stride);
     if (p->gaussian_size < 0 || p->gaussian_size > 32767) return fail(h, SPG_E_INVALID, "gaussian_size %d outside [0, 32767]", p->gaussian_size);
     if (!std::isfinite(p->sigma) || !(p->sigma > 0) || !std::isfinite(p->paf_sigma) || !(p->paf_sigma > 0))
         return fail(h, SPG_E_INVALID, "sigma and paf_sigma must be finite and positive");

@@ -418,7 +418,8 @@ int spg_track_frames(spg_handle *h, const spg_track_frame *frames, int32_t n, sp
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
  * reference's CanonicalConfig / TransformationParams: */
 typedef struct spg_target_params {
-    int32_t stride;             /* config.stride: the map is the warped image / stride (must divide out_h and out_w) */
+    int32_t stride;             /* config.stride: the map is the warped image / stride (must divide out_h and out_w; */
+                                /* at most 2901, so that a mask box sum of 255 * stride^2 fits an int)              */
     int32_t gaussian_size;      /* Heatmapper.gaussian_size: a keypoint window is round(x / stride) +- gaussian_size // 2 */
     int32_t out_h, out_w;       /* warped image rows / columns: warpAffine's dsize (config.height, config.width) is */
                                 /* (columns, rows), so out_h = config.width and out_w = config.height                 */
@@ -445,14 +446,22 @@ typedef struct spg_target_sample {
 } spg_target_sample;
 /* Per sample: cv2.warpAffine(image, matrix, (out_w, out_h), INTER_LINEAR, BORDER_CONSTANT, border_image) / 255. as
  * float32, and each mask through the same warp (its own border value), cv2.resize(..., INTER_AREA) by the integer factor
- * stride and / 255.  The warp and the area resize follow OpenCV's uint8 algorithms bit for bit; the full-size warped masks
- * are never stored.  Every sample is validated before the first launch (SPG_E_INVALID names the first bad one).
+ * stride and / 255.  The warp follows OpenCV's uint8 fixed-point algorithm bit for bit; the area resize follows its
+ * fast-area arithmetic on the int box sum s: (s + 2) >> 2 at stride 2, else saturate_cast<uchar>(s * (1.f / stride^2)),
+ * a float32 product rounded ties to even (not always the correctly rounded s / stride^2: strides 22, 34, 44, ...).  The
+ * full-size warped masks are never stored.  Every sample is validated before the first launch (SPG_E_INVALID names the first bad one).
  * Asynchronous on `stream` (never synchronises); `samples` may be reused as soon as the call returns. */
 int spg_targets_warp(spg_handle *h, const spg_target_params *params, const spg_target_sample *samples, int32_t n_samples,
                      void *stream);
 /* One sample of spg_targets_maps. */
 typedef struct spg_target_joints {
     const float *joints;        /* [n_persons][n_parts][3] float32 device (x, y, v) in output pixels; v < 2 is visible */
+                                /* (v NaN is not); a visible joint may have any coordinates: one that is NaN or     */
+                                /* +-inf, or so large that its window misses the map, draws no keypoint, and a limb */
+                                /* with a NaN end draws nothing.  A limb with an infinite end, or whose length      */
+                                /* overflows float32, draws the reference's expressions' values (NaN or 1.0 in its  */
+                                /* box, as the numpy port computes them).  targets.py refuses non-finite visible    */
+                                /* joints, as the reference's int(round(x)) does.                                   */
     int32_t n_persons;          /* any count >= 0 */
     int32_t reserved;           /* 0 */
     const float *mask_all;      /* [out_h / stride][out_w / stride] float32 device: spg_targets_warp's mask_all_out */

@@ -48,10 +48,16 @@ def warp_affine_u8(src: np.ndarray, M: np.ndarray, dsize, border) -> np.ndarray:
 
 def resize_area_int(a: np.ndarray, f: int) -> np.ndarray:
     """``cv2.resize(a, (w // f, h // f), INTER_AREA)`` of uint8 ``a [h, w]`` by the integer factor ``f`` dividing both
-    sides: ``rint(box sum / f^2)``, ties to even."""
+    sides, as OpenCV's fast-area code computes it from the box sum ``s``: ``(s + 2) >> 2`` at ``f = 2`` (ties up), else
+    ``saturate_cast<uchar>(s * (1.f / f^2))`` -- the sum converted to float32, times the float32 reciprocal, rounded ties
+    to even.  The product is not always the correctly rounded ``s / f^2`` (``f = 22, 34, 44, ...``); at ``f = 1`` cv2
+    copies, which the product also gives."""
     h, w = a.shape
     s = a.reshape(h // f, f, w // f, f).astype(np.int64).sum(axis=(1, 3))
-    return np.rint(s / (f * f)).astype(np.uint8)
+    if f == 2:
+        return ((s + 2) >> 2).astype(np.uint8)
+    inv = np.float32(1) / np.float32(f * f)
+    return np.clip(np.rint(s.astype(np.float32) * inv), 0, 255).astype(np.uint8)
 
 
 def erode3(m: np.ndarray) -> np.ndarray:
@@ -66,13 +72,17 @@ def lut() -> np.ndarray:
     return np.arange(256, dtype=np.uint8).astype(np.float32) / 255.
 
 
-def warp_sample(img, mask_miss, mask_all, M, out_hw, stride):
-    """The float32 ``(img [H, W, 3], mask_miss [h, w], mask_all [h, w])`` of one sample; ``out_hw = (rows, cols)``."""
+BORDERS = ((124, 127, 127), 255, 0)  # the reference's borderValue for the image, mask_miss and mask_all
+
+
+def warp_sample(img, mask_miss, mask_all, M, out_hw, stride, borders=BORDERS):
+    """The float32 ``(img [H, W, 3], mask_miss [h, w], mask_all [h, w])`` of one sample; ``out_hw = (rows, cols)``,
+    ``borders = (image (B, G, R), mask_miss, mask_all)``."""
     H, W = out_hw
     t = lut()
-    im = warp_affine_u8(img, M, (W, H), (124, 127, 127))
-    mm = resize_area_int(warp_affine_u8(mask_miss, M, (W, H), 255), stride)
-    ma = resize_area_int(warp_affine_u8(mask_all, M, (W, H), 0), stride)
+    im = warp_affine_u8(img, M, (W, H), borders[0])
+    mm = resize_area_int(warp_affine_u8(mask_miss, M, (W, H), borders[1]), stride)
+    ma = resize_area_int(warp_affine_u8(mask_all, M, (W, H), borders[2]), stride)
     return t[im], t[mm], t[ma]
 
 
@@ -85,7 +95,8 @@ def _kp_exp(arg: np.ndarray, exp: str) -> np.ndarray:
 
 
 def _window(lo: float, hi: float, n: int):
-    """[lo, hi) clipped to the map: (a, b) or None when empty (Python slicing of the reference's window)."""
+    """[lo, hi) clipped to the map: (a, b) or None when empty (Python slicing of the reference's window); None too when
+    a bound is NaN."""
     a, b = max(lo, 0), min(hi, n)
     return (int(a), int(b)) if a < b else None
 
@@ -131,8 +142,11 @@ def label_maps(joints: np.ndarray, mask_all: np.ndarray, limbs, stride: int, sig
             dx, dy = x2 - x1, y2 - y1
             if dx * dx + dy * dy == 0:
                 continue
-            lx, hx = float(np.rint((min(x1, x2) - pt) / fs)), float(np.rint((max(x1, x2) + pt) / fs))
-            ly, hy = float(np.rint((min(y1, y2) - pt) / fs)), float(np.rint((max(y1, y2) + pt) / fs))
+            # the reference's (x1, x2) if x1 < x2 else (x2, x1), not min / max: with a NaN end both put the NaN in the box
+            mnx, mxx = (x1, x2) if x1 < x2 else (x2, x1)
+            mny, mxy = (y1, y2) if y1 < y2 else (y2, y1)
+            lx, hx = float(np.rint((mnx - pt) / fs)), float(np.rint((mxx + pt) / fs))
+            ly, hy = float(np.rint((mny - pt) / fs)), float(np.rint((mxy + pt) / fs))
             wx, wy = _window(lx, hx + 1, w), _window(ly, hy + 1, h)
             if wx is None or wy is None:
                 continue
@@ -154,11 +168,13 @@ def label_maps(joints: np.ndarray, mask_all: np.ndarray, limbs, stride: int, sig
     return np.clip(out, 0., 1.)
 
 
-# ---- golden cases (tests/golden/targets/, made by tests/golden/make_targets_golden.py) ----------------------------------
-def golden_paths():
+# ---- golden cases (tests/golden/targets/ and targets_space/, made by tests/golden/make_targets_golden.py) ---------------
+def golden_paths(kind: str = "targets"):
+    """The cases of ``tests/golden/<kind>/``: ``targets`` (the default configuration at 256 and 512) or
+    ``targets_space`` (other strides, sizes, Gaussian parameters and limb tables)."""
     import glob
     import os
-    d = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "targets")
+    d = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", kind)
     return sorted(p for p in glob.glob(os.path.join(d, "*.npz")) if not p.endswith("augment_draws.npz"))
 
 
@@ -174,10 +190,32 @@ def load_case(path: str) -> dict:
     return z
 
 
-def port_case(z: dict, exp: str = "rounded"):
-    """``(image, mask_miss, mask_all, labels)`` of a golden case by the port, from the case's M and joints."""
+def case_params(z: dict) -> dict:
+    """The configuration a golden case was made with: the reference's defaults unless the case records its own."""
     from improved_body_parts_b200 import skeleton
-    s, n = 4, z["size"]
-    im, mm, ma = warp_sample(z["img"], z["mask_miss_src"], z["mask_all_src"], z["M"], (n, n), s)
-    labels = label_maps(z["joints"].astype(np.float32), ma, skeleton.LIMBS, s, 9, 7, 0.015, 4, 14, exp=exp)
+    return dict(stride=int(z.get("stride", 4)), sigma=float(z.get("sigma", 9)), paf_sigma=float(z.get("paf_sigma", 7)),
+                limb_thre=float(z.get("limb_gaussian_thre", 0.015)), paf_thre=float(z.get("paf_thre", 4)),
+                gsize=int(z.get("gaussian_size", 14)), limbs=[tuple(int(v) for v in l) for l in z.get("limbs", skeleton.LIMBS)])
+
+
+def target_config(z: dict):
+    """A ``targets.TargetConfig`` with a golden case's size, stride, transform parameters and limb table."""
+    from improved_body_parts_b200 import targets
+    c = case_params(z)
+    cfg = targets.TargetConfig(z["size"], z["size"], c["stride"])
+    t = cfg.transform_params
+    t.sigma, t.paf_sigma, t.limb_gaussian_thre, t.paf_thre = c["sigma"], c["paf_sigma"], c["limb_thre"], c["paf_thre"]
+    t.keypoint_gaussian_thre = float(z.get("keypoint_gaussian_thre", 0.015))
+    cfg.limbs_conn = c["limbs"]
+    cfg.derive()
+    return cfg
+
+
+def port_case(z: dict, exp: str = "rounded"):
+    """``(image, mask_miss, mask_all, labels)`` of a golden case by the port, from the case's M, joints and
+    configuration."""
+    c, n = case_params(z), z["size"]
+    im, mm, ma = warp_sample(z["img"], z["mask_miss_src"], z["mask_all_src"], z["M"], (n, n), c["stride"])
+    labels = label_maps(z["joints"].astype(np.float32), ma, c["limbs"], c["stride"], c["sigma"], c["paf_sigma"],
+                        c["limb_thre"], c["paf_thre"], c["gsize"], exp=exp)
     return im, mm, ma, labels

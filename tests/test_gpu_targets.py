@@ -11,6 +11,7 @@ from improved_body_parts_b200 import grouping, skeleton, targets
 
 pytestmark = pytest.mark.gpu
 CASES = tp.golden_paths()
+SPACE = tp.golden_paths("targets_space")
 
 
 def _ulp(a, b):
@@ -18,13 +19,15 @@ def _ulp(a, b):
 
 
 def _kernels(cuda_device, z):
-    """image, mask_miss, mask_all, labels of a golden case from the kernels, with the case's M and joints."""
+    """image, mask_miss, mask_all, labels of a golden case from the kernels, with the case's M, joints, stride,
+    parameters and limb table."""
     import torch
-    cfg = targets.TargetConfig(z["size"], z["size"])
+    cfg = tp.target_config(z)
     params = targets.target_params(cfg)
-    n, m = z["size"], z["size"] // 4
+    n, m = z["size"], z["size"] // cfg.stride
     src = [torch.from_numpy(np.ascontiguousarray(a)).to(cuda_device) for a in (z["img"], z["mask_miss_src"], z["mask_all_src"])]
-    out = [torch.empty(s, dtype=torch.float32, device=cuda_device) for s in ((n, n, 3), (m, m), (m, m), (50, m, m))]
+    out = [torch.empty(s, dtype=torch.float32, device=cuda_device)
+           for s in ((n, n, 3), (m, m), (m, m), (cfg.num_layers, m, m))]
     h, w = z["img"].shape[:2]
     ws = np.zeros(1, grouping.TARGET_SAMPLE)
     ws[0] = (src[0].data_ptr(), src[1].data_ptr(), src[2].data_ptr(), 3 * w, w, h, w, z["M"].reshape(6), out[0].data_ptr(),
@@ -39,20 +42,43 @@ def _kernels(cuda_device, z):
     return [t.cpu().numpy() for t in out]
 
 
-@pytest.mark.parametrize("path", CASES, ids=lambda p: os.path.basename(p)[:-4])
+def _hold_the_golden_contract(z, im, mm, ma, lab):
+    """The reference's own output: image, masks and channel L+K exact, body parts within 1 ULP, keypoints and channel
+    L+K+1 within 5 ULP with the same zeros."""
+    L, ref = len(tp.case_params(z)["limbs"]), z["labels"]
+    assert lab.shape == ref.shape
+    assert np.array_equal(im, z["image"]) and np.array_equal(mm, z["mask_miss"]) and np.array_equal(ma, z["mask_all"])
+    assert np.array_equal(lab[L + 18], ref[L + 18])
+    assert _ulp(lab[:L], ref[:L]).max(initial=0) <= 1
+    for c in list(range(L, L + 18)) + [L + 19]:
+        assert np.array_equal(lab[c] == 0, ref[c] == 0) and _ulp(lab[c], ref[c]).max() <= 5, c
+
+
+@pytest.mark.parametrize("path", CASES + SPACE, ids=lambda p: os.path.basename(p)[:-4])
 def test_kernels_equal_the_port_and_hold_the_golden_contract(cuda_device, path):
     z = tp.load_case(path)
     im, mm, ma, lab = _kernels(cuda_device, z)
     pim, pmm, pma, plab = tp.port_case(z, "rounded")
     assert np.array_equal(im, pim) and np.array_equal(mm, pmm) and np.array_equal(ma, pma)
-    for c in range(50):
+    for c in range(len(plab)):
         assert np.array_equal(lab[c].view(np.int32), plab[c].view(np.int32)), f"channel {c}"
-    # against the reference's own output
-    assert np.array_equal(im, z["image"]) and np.array_equal(mm, z["mask_miss"]) and np.array_equal(ma, z["mask_all"])
-    assert np.array_equal(lab[48], z["labels"][48])
-    assert _ulp(lab[:30], z["labels"][:30]).max() <= 1
-    for c in list(range(30, 48)) + [49]:
-        assert np.array_equal(lab[c] == 0, z["labels"][c] == 0) and _ulp(lab[c], z["labels"][c]).max() <= 5, c
+    _hold_the_golden_contract(z, im, mm, ma, lab)
+
+
+@pytest.mark.parametrize("path", [p for p in SPACE if os.path.basename(p).startswith(("s2_", "s8_"))],
+                         ids=lambda p: os.path.basename(p)[:-4])
+def test_make_batch_holds_the_golden_contract_at_strides_2_and_8(cuda_device, path):
+    """make_batch from the golden's source, meta and augmentation with a config of its stride and parameters."""
+    z = tp.load_case(path)
+    cfg = tp.target_config(z)
+    aug = targets.AugmentSelection(bool(z["aug_flip"]), False, float(z["aug_degree"]), tuple(int(v) for v in z["aug_crop"]),
+                                   float(z["aug_scale"]))
+    meta = {"objpos": [list(z["objpos"])], "scale_provided": [float(z["scale_provided"])], "joints": z["joints_src"]}
+    images, miss, labels = targets.make_batch([(z["img"], z["mask_miss_src"], z["mask_all_src"], meta)], [aug], cfg)
+    im, mm, lab = images[0].cpu().numpy(), miss[0, 0].cpu().numpy(), labels[0].cpu().numpy()
+    L = len(cfg.limbs_conn)
+    _hold_the_golden_contract(z, im, mm, z["mask_all"], lab)
+    assert np.array_equal(lab[L + 18], tp.erode3(z["mask_all"]))
 
 
 def _ragged_batch(seed, n=64, size=256):

@@ -7,22 +7,19 @@ import subprocess
 import numpy as np
 import pytest
 
+import targets_cases as tc
 import targets_port as tp
-from improved_body_parts_b200 import grouping, targets
+from improved_body_parts_b200 import grouping, skeleton, targets
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = tp.golden_paths()
+SPACE = tp.golden_paths("targets_space")
 
 
-def _config(size):
-    c = targets.TargetConfig(size, size)
-    return c
-
-
-@pytest.mark.parametrize("path", CASES, ids=lambda p: os.path.basename(p)[:-4])
+@pytest.mark.parametrize("path", CASES + SPACE, ids=lambda p: os.path.basename(p)[:-4])
 def test_affine_and_joints_equal_the_goldens(path):
     z = tp.load_case(path)
-    cfg = _config(z["size"])
+    cfg = tp.target_config(z)
     aug = targets.AugmentSelection(bool(z["aug_flip"]), False, float(z["aug_degree"]), tuple(int(v) for v in z["aug_crop"]),
                                    float(z["aug_scale"]))
     M, _ = aug.affine(list(z["objpos"]), float(z["scale_provided"]), cfg)
@@ -43,6 +40,70 @@ def test_seeded_random_draws_equal_the_reference():
 
 def test_gaussian_size_default():
     assert targets.gaussian_size(targets.TargetConfig()) == 14
+
+
+@pytest.mark.parametrize("path", SPACE, ids=lambda p: os.path.basename(p)[:-4])
+def test_target_params_equal_the_goldens_configuration(path):
+    """target_params of a TargetConfig carrying a golden's stride, transform parameters and limb table: the
+    reference's gaussian_size, shapes and the values the kernels take."""
+    z = tp.load_case(path)
+    c = tp.case_params(z)
+    cfg = tp.target_config(z)
+    assert targets.gaussian_size(cfg) == c["gsize"]
+    assert cfg.num_layers == z["labels"].shape[0] and cfg.mask_shape == z["mask_miss"].shape
+    p = targets.target_params(cfg)[0]
+    assert (int(p["stride"]), int(p["gaussian_size"]), int(p["out_h"]), int(p["out_w"])) == \
+        (c["stride"], c["gsize"], z["size"], z["size"])
+    assert (p["sigma"], p["paf_sigma"], p["limb_gaussian_thre"], p["paf_thre"]) == \
+        (c["sigma"], c["paf_sigma"], c["limb_thre"], c["paf_thre"])
+
+
+def test_case_table_covers_every_axis():
+    """tests/targets_cases.py against the axes spg_targets_warp / spg_targets_maps admit."""
+    cases = tc.CASES
+    assert len({c.name for c in cases}) == len(cases)
+    assert {c.stride for c in cases} >= {1, 2, 3, 4, 5, 6, 8}
+    maps = [c.map_hw for c in cases]
+    assert any(h == w > 1 for h, w in maps) and any(h != w for h, w in maps) and (1, 1) in maps
+    for c in cases:
+        assert c.out_hw[0] % c.stride == 0 and c.out_hw[1] % c.stride == 0
+        assert len(c.sources) == len(c.persons) and all(0 <= a < c.K and 0 <= b < c.K for a, b in c.limbs)
+        assert 1 <= len(c.limbs) <= 64 and c.K <= 32
+    g = [(c.gaussian_size, c.map_hw) for c in cases]
+    assert any(s == 0 for s, _ in g) and any(s % 2 for s, _ in g) and any(s // 2 >= max(hw) for s, hw in g)
+    assert any(c.borders != tc.DEFAULT_BORDERS for c in cases)
+    assert any(c.pad[0] > 0 for c in cases) and any(c.pad[1] > 0 for c in cases)
+    assert any(c.pad[0] % 4 for c in cases)  # an image pitch that is no multiple of 4
+    tables = {(len(c.limbs), c.K) for c in cases}
+    assert {(1, 18), (24, 18), (64, 18), (64, 32), (1, 32)} <= tables
+    assert any(tuple(c.limbs) == tuple(skeleton.LIMBS) for c in cases)
+    assert any(a == b for c in cases for a, b in c.limbs)  # a self-limb
+    assert any(len(set(c.limbs)) < len(c.limbs) for c in cases)  # a repeated limb
+    assert len({(c.sigma, c.paf_sigma, c.limb_thre, c.paf_thre) for c in cases}) >= 6
+    assert any(c.paf_thre != int(c.paf_thre) for c in cases)
+    # joints: ties, +-FLT_MAX, +-inf, NaN (visible), v exactly 2 and v NaN; 0 persons and > 256 persons x parts
+    allj = []
+    for c in cases:
+        for (_, _, _, M, j) in tc.inputs(c):
+            assert M.shape == (2, 3) and np.isfinite(M).all() and j.dtype == np.float32 and j.shape[1:] == (c.K, 3)
+            if len(j) > 1:  # person 0 on x / stride ties (person 1 holds the special values)
+                vis = j[0, :, 2] < 2
+                x = j[0, vis, 0] / np.float32(c.stride)
+                assert vis.any() and np.array_equal(x - np.floor(x), np.full(x.shape, 0.5, np.float32)), c.name
+            allj.append(j.reshape(-1, 3))
+    a = np.concatenate(allj)
+    vis = a[:, 2] < 2
+    xy = a[vis, :2]
+    fmax = np.float32(tc.FLT_MAX)
+    assert (xy == fmax).any() and (xy == -fmax).any() and np.isposinf(xy).any() and np.isneginf(xy).any()
+    assert np.isnan(xy[:, 0]).any() and np.isnan(xy[:, 1]).any()
+    assert (a[:, 2] == 2).any() and np.isnan(a[:, 2]).any()
+    for c in cases:  # every case has a visible limb with one NaN end and the other end on the map
+        a, b = tc.nan_limb(c)
+        j = [d[4] for d in tc.inputs(c) if len(d[4]) >= 3]
+        assert j and np.isnan(j[0][-1, a, 0]) and np.isfinite(j[0][-1, b, :2]).all() and (j[0][-1, [a, b], 2] < 2).all()
+    counts = [p for c in cases for p in c.persons]
+    assert 0 in counts and any(p * c.K > 256 for c in cases for p in c.persons)
 
 
 def _sample(h=40, w=50, P=2):
