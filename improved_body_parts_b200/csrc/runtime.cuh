@@ -18,7 +18,7 @@
 namespace spg {
 
 // the stage numbers of spg_stage_kernel (include/spgroup.h)
-enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageTargets, kStageLoss, kStageCoco, kStageJpeg, kStageYuv, kStageTrack, kStageCount };
+enum : int { kStageNms, kStageScore, kStageMatch, kStageAssemble, kStagePostnet, kStagePrenet, kStageTargets, kStageLoss, kStageCoco, kStageJpeg, kStageYuv, kStageTrack, kStageSmooth, kStageCount };
 
 // device scratch that grows on demand (grow) and lives until spg_destroy
 struct Scratch {
@@ -52,7 +52,7 @@ struct spg_handle {
     bool ub_valid = false;
     cudaStream_t streams[2] = {nullptr, nullptr};
     int64_t launches = 0;
-    const char *stage_kernel[spg::kStageCount] = {"", "", "", "", "", "", "", "", "", "", "", ""};
+    const char *stage_kernel[spg::kStageCount] = {"", "", "", "", "", "", "", "", "", "", "", "", ""};
     // tuning / A-B switches, read from the environment ONCE in spg_create (never per launch); none changes a result
     int persist = 1;      // persistent warp-specialised nms_peaks / limb_score when they apply (SPG_PERSIST=0 turns them off)
     int screen = 1;       // limb_score phase A on (SPG_NO_SCREEN=1 turns it off: every pair is evaluated exactly)

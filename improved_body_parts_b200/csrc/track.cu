@@ -1,8 +1,11 @@
-// track.cu -- spg_track_frames and its kernel, track_kernel (track.cuh describes it).
+// track.cu -- spg_track_frames and its kernel, track_kernel (track.cuh describes it), and spg_smooth_frames and its
+// kernel, smooth_kernel (smooth.cuh), which reads the ids tracking wrote.
 #include "runtime.cuh"
 
+#include "smooth.cuh"
 #include "track.cuh"
 
+#include <climits>
 #include <cmath>
 
 namespace spg {
@@ -216,6 +219,185 @@ track_kernel(const __grid_constant__ TrackRagged r, spg_track_table *tables, int
     if (tid == 0) tb->next_id = s_next;
 }
 
+// the double nearest 2 pi
+constexpr double kTwoPi = 6.283185307179586;
+
+__global__ void __launch_bounds__(kSmoothThreads, 1)
+smooth_kernel(const __grid_constant__ SmoothRagged r, spg_smooth_table *tables, int n_tables, double min_cutoff, double beta,
+              double d_cutoff, int rows) {
+    extern __shared__ double s_scale[];  // [rows]; then s_slot [rows] and s_used [rows]
+    int *s_slot = reinterpret_cast<int *>(s_scale + rows);  // per row: its slot, -1 raw, -2 a claim to make
+    unsigned *s_used = reinterpret_cast<unsigned *>(s_slot + rows);  // per row: its used joints
+    __shared__ long long s_id[kSmoothSlots], s_last[kSmoothSlots];
+    __shared__ int s_live[kSmoothSlots], s_owner[kSmoothSlots];
+    __shared__ unsigned s_mask[kSmoothSlots];
+    constexpr int kWarps = kSmoothThreads / 32;
+    constexpr double kInf = __builtin_huge_val();
+    const int k = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int s = *r.img[k].stream;
+    if (s < 0 || s >= n_tables) {  // skipped: no table changes, the rows are passed through raw
+        const SmoothFrame &f = r.img[k];
+        const int np = min(max(*reinterpret_cast<const int *>(f.record), 0), rows);
+        const double *row0 = reinterpret_cast<const double *>(f.record + 8);
+        for (int q = tid; q < np * 2 * kSmoothJoints; q += kSmoothThreads) {
+            const int p = q / (2 * kSmoothJoints);
+            f.xy[q] = row0[(size_t)p * kRowWords + q - p * 2 * kSmoothJoints];
+        }
+        return;
+    }
+    for (int j = 0; j < k; j++)
+        if (*r.img[j].stream == s) return;  // the stream's frames run in the CTA of its first frame
+    spg_smooth_table *tb = tables + s;
+    if (tid < kSmoothSlots) {
+        s_id[tid] = tb->slots[tid].id;
+        s_last[tid] = tb->slots[tid].last;
+        s_live[tid] = tb->slots[tid].live != 0;
+        s_mask[tid] = tb->slots[tid].mask;
+    }
+    long long tick = tb->clock;
+    for (int j = k; j < r.n; j++) {
+        if (*r.img[j].stream != s) continue;
+        const SmoothFrame &f = r.img[j];
+        const int np = min(max(*reinterpret_cast<const int *>(f.record), 0), rows);
+        const double *row0 = reinterpret_cast<const double *>(f.record + 8);
+        const double t = *f.time;
+        tick++;  // 1. the clock advances
+        if (tid < kSmoothSlots) s_owner[tid] = INT_MAX;
+        __syncthreads();
+        // 2. per person (one warp each): its used joints, its scale and the live slot holding its id
+        for (int p = warp; p < np; p += kWarps) {
+            const double *pr = row0 + (size_t)p * kRowWords;
+            const unsigned long long pm = reinterpret_cast<const unsigned long long *>(pr)[kRowWords - 1];
+            double x = 0.0, y = 0.0;
+            if (lane < kSmoothJoints) x = pr[2 * lane], y = pr[2 * lane + 1];
+            const bool used = lane < kSmoothJoints && ((pm >> lane) & 1) && isfinite(x) && isfinite(y);
+            const unsigned um = __ballot_sync(0xffffffffu, used);
+            double x0 = used ? x : kInf, x1 = used ? x : -kInf, y0 = used ? y : kInf, y1 = used ? y : -kInf;
+            for (int o = 16; o > 0; o >>= 1) {
+                x0 = fmin(x0, __shfl_xor_sync(0xffffffffu, x0, o));
+                x1 = fmax(x1, __shfl_xor_sync(0xffffffffu, x1, o));
+                y0 = fmin(y0, __shfl_xor_sync(0xffffffffu, y0, o));
+                y1 = fmax(y1, __shfl_xor_sync(0xffffffffu, y1, o));
+            }
+            double sc = 1.0;
+            if (um) {
+                sc = ((x1 - x0) + (y1 - y0)) / 2.0;
+                sc = sc > 1.0 ? sc : 1.0;
+            }
+            const long long pid = f.ids[p];
+            int slot = -1;
+            if (pid >= 0) {
+                slot = -2;
+                for (int b = 0; b < kSmoothSlots; b += 32) {
+                    const unsigned m = __ballot_sync(0xffffffffu, s_live[b + lane] && s_id[b + lane] == pid);
+                    if (m) {
+                        slot = b + __ffs(m) - 1;
+                        break;
+                    }
+                }
+            }
+            if (lane == 0) {
+                s_scale[p] = sc;
+                s_slot[p] = slot;
+                s_used[p] = um;
+                if (slot >= 0) atomicMin(&s_owner[slot], p);
+            }
+        }
+        __syncthreads();
+        // a repeated id: the slot belongs to its first row, the others are passed through raw; 4. used slots' last
+        for (int p = tid; p < np; p += kSmoothThreads) {
+            const int slot = s_slot[p];
+            if (slot < 0) continue;
+            if (s_owner[slot] != p) s_slot[p] = -1;
+            else s_last[slot] = tick;
+        }
+        __syncthreads();
+        // 3. in row order, each person without a slot claims one: the lowest free slot, else the least recently used
+        // slot this frame has not used (ties: the lowest index), reset
+        if (warp == 0) {
+            for (int b = 0; b < np; b += 32) {
+                unsigned need = __ballot_sync(0xffffffffu, b + lane < np && s_slot[b + lane] == -2);
+                while (need) {
+                    const int p = b + __ffs(need) - 1;
+                    need &= need - 1;
+                    const long long pid = f.ids[p];
+                    int slot = -1;
+                    bool taken = false;  // an earlier row of this frame claimed a slot for the same id
+                    for (int c = 0; c < kSmoothSlots && !taken; c += 32)
+                        taken = __ballot_sync(0xffffffffu, s_live[c + lane] && s_id[c + lane] == pid) != 0;
+                    for (int c = 0; c < kSmoothSlots && !taken && slot < 0; c += 32) {
+                        const unsigned open = __ballot_sync(0xffffffffu, !s_live[c + lane]);
+                        if (open) slot = c + __ffs(open) - 1;
+                    }
+                    if (!taken && slot < 0) {
+                        long long v = LLONG_MAX;
+                        int at = -1;
+                        for (int c = lane; c < kSmoothSlots; c += 32)
+                            if (s_last[c] < tick && (at < 0 || s_last[c] < v)) v = s_last[c], at = c;
+                        for (int o = 16; o > 0; o >>= 1) {
+                            const long long ov = __shfl_xor_sync(0xffffffffu, v, o);
+                            const int oa = __shfl_xor_sync(0xffffffffu, at, o);
+                            if (oa >= 0 && (at < 0 || ov < v || (ov == v && oa < at))) v = ov, at = oa;
+                        }
+                        slot = at;
+                    }
+                    if (slot >= 0) {
+                        double *st = &tb->slots[slot].joint[0][0];
+                        for (int w = lane; w < 5 * kSmoothJoints; w += 32) st[w] = 0.0;
+                        if (lane == 0) {
+                            s_live[slot] = 1;
+                            s_id[slot] = pid;
+                            s_last[slot] = tick;
+                            s_mask[slot] = 0;
+                        }
+                    }
+                    if (lane == 0) s_slot[p] = slot;
+                    __syncwarp();
+                }
+            }
+        }
+        __syncthreads();
+        // 5. the (person, joint) pairs: the filter on each used joint of a person with a slot, every other joint raw
+        for (int q = tid; q < np * kSmoothJoints; q += kSmoothThreads) {
+            const int p = q / kSmoothJoints, g = q - p * kSmoothJoints;
+            const double *pr = row0 + (size_t)p * kRowWords;
+            double x = pr[2 * g], y = pr[2 * g + 1];
+            const int slot = s_slot[p];
+            if (slot >= 0 && ((s_used[p] >> g) & 1)) {
+                double *st = tb->slots[slot].joint[g];
+                const double dt = t - st[4];
+                double xh = x, yh = y, dxh = 0.0, dyh = 0.0;
+                if (((s_mask[slot] >> g) & 1) && dt > 0.0 && isfinite(dt)) {
+                    const double sc = s_scale[p];
+                    const double vx = (x - st[0]) / dt / sc, vy = (y - st[1]) / dt / sc;
+                    const double ad = 1.0 / (1.0 + 1.0 / (kTwoPi * d_cutoff * dt));
+                    dxh = ad * vx + (1.0 - ad) * st[2];
+                    dyh = ad * vy + (1.0 - ad) * st[3];
+                    const double fc = min_cutoff + beta * sqrt(dxh * dxh + dyh * dyh);
+                    const double a = 1.0 / (1.0 + 1.0 / (kTwoPi * fc * dt));
+                    xh = a * x + (1.0 - a) * st[0];
+                    yh = a * y + (1.0 - a) * st[1];
+                }
+                st[0] = xh, st[1] = yh, st[2] = dxh, st[3] = dyh, st[4] = t;
+                x = xh, y = yh;
+            }
+            f.xy[2 * q] = x;
+            f.xy[2 * q + 1] = y;
+        }
+        __syncthreads();
+        for (int p = tid; p < np; p += kSmoothThreads)  // one row per slot: the rows' used joints now have state
+            if (s_slot[p] >= 0) s_mask[s_slot[p]] |= s_used[p];
+        __syncthreads();
+    }
+    if (tid < kSmoothSlots) {
+        tb->slots[tid].id = s_id[tid];
+        tb->slots[tid].last = s_last[tid];
+        tb->slots[tid].live = s_live[tid];
+        tb->slots[tid].mask = s_mask[tid];
+    }
+    if (tid == 0) tb->clock = tick;
+}
+
 }  // namespace spg
 
 using namespace spg;
@@ -257,6 +439,49 @@ int spg_track_frames(spg_handle *h, const spg_track_frame *frames, int32_t n, sp
         fill_table(table, ms, first, g);
         if ((rc = launch(h, kStageTrack, "track_kernel", track_kernel, dim3(g.ctas), kTrackThreads, kTrackSmem,
                          static_cast<cudaStream_t>(stream), table, tables, n_tables, oks_threshold, max_age, rows)))
+            return rc;
+    }
+    return SPG_OK;
+}
+
+int spg_smooth_frames(spg_handle *h, const spg_smooth_frame *frames, int32_t n, spg_smooth_table *tables, int32_t n_tables,
+                      double min_cutoff, double beta, double d_cutoff, void *stream) {
+    if (!h) return SPG_E_INVALID;
+    if (n < 0 || (n > 0 && !frames)) return fail(h, SPG_E_INVALID, "frames is NULL or n negative");
+    if (n > 0 && (n_tables < 1 || !tables)) return fail(h, SPG_E_INVALID, "tables is NULL or n_tables below 1");
+    if ((reinterpret_cast<uintptr_t>(tables) & 7) != 0) return fail(h, SPG_E_INVALID, "tables must be 8-byte aligned");
+    if (!std::isfinite(min_cutoff) || !(min_cutoff > 0.0)) return fail(h, SPG_E_INVALID, "min_cutoff %g must be finite and above 0", min_cutoff);
+    if (!std::isfinite(d_cutoff) || !(d_cutoff > 0.0)) return fail(h, SPG_E_INVALID, "d_cutoff %g must be finite and above 0", d_cutoff);
+    if (!std::isfinite(beta) || !(beta >= 0.0)) return fail(h, SPG_E_INVALID, "beta %g must be finite and at least 0", beta);
+    if (h->ws.J != kSmoothJoints) return fail(h, SPG_E_INVALID, "smoothing needs 17 output joints (the handle has %d)", h->ws.J);
+    std::vector<SmoothFrame> ms((size_t)n);
+    for (int i = 0; i < n; i++) {  // validate every frame before the first launch
+        const spg_smooth_frame &s = frames[i];
+        if (!s.record || !s.stream || !s.ids || !s.time || !s.xy)
+            return fail(h, SPG_E_INVALID, "frame %d: record, stream, ids, time or xy is NULL", i);
+        if ((reinterpret_cast<uintptr_t>(s.record) & 7) || (reinterpret_cast<uintptr_t>(s.ids) & 7) ||
+            (reinterpret_cast<uintptr_t>(s.time) & 7) || (reinterpret_cast<uintptr_t>(s.xy) & 7) ||
+            (reinterpret_cast<uintptr_t>(s.stream) & 3))
+            return fail(h, SPG_E_INVALID, "frame %d: record, ids, time and xy must be 8-byte aligned, stream 4-byte", i);
+        ms[i] = SmoothFrame{static_cast<const unsigned char *>(s.record), s.stream, reinterpret_cast<const long long *>(s.ids),
+                            s.time, s.xy, 0};
+    }
+    if (ms.empty()) return SPG_OK;
+    const int rows = h->ws.wire_rows > 0 ? h->ws.wire_rows : h->ws.capR;
+    const size_t smem = (size_t)rows * kSmoothRowBytes;
+    if (smem > smem_room(h, smooth_kernel))
+        return fail(h, SPG_E_INVALID, "the smoothing kernel's %zu B of shared memory for %d rows exceed the device's room", smem, rows);
+    std::vector<long long> ctas((size_t)n, 1);
+    std::vector<RaggedRange> ranges;
+    std::vector<int> first;
+    int rc;
+    if ((rc = deal_ragged(h, ctas, kSmoothTableMax, "frame", nullptr, ranges, first))) return rc;
+    DeviceGuard guard(h->device);
+    SmoothRagged table{};
+    for (const RaggedRange &g : ranges) {
+        fill_table(table, ms, first, g);
+        if ((rc = launch(h, kStageSmooth, "smooth_kernel", smooth_kernel, dim3(g.ctas), kSmoothThreads, smem,
+                         static_cast<cudaStream_t>(stream), table, tables, n_tables, min_cutoff, beta, d_cutoff, rows)))
             return rc;
     }
     return SPG_OK;

@@ -25,8 +25,9 @@ from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 import numpy as np
 
 from . import sharding, wire
-from .grouping import (JPEG_OK, JPEG_RECORD, ST_MEANING, TRACK_FRAME, TRACK_TABLE, YUV_I420, YUV_MEMBER, YUV_NV12, YUV_YUYV,
-                       Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse, prenet_item)
+from .grouping import (JPEG_OK, JPEG_RECORD, SMOOTH_FRAME, SMOOTH_TABLE, ST_MEANING, TRACK_FRAME, TRACK_TABLE, YUV_I420,
+                       YUV_MEMBER, YUV_NV12, YUV_YUYV, Grouper, GroupingError, clamp_scale, input_geometry, jpeg_parse,
+                       prenet_item)
 from .skeleton import COCO_FROM_PART, LIMBS, NUM_PARTS, GroupParams
 
 _limbs: Tuple[Tuple[int, int], ...] = LIMBS
@@ -623,6 +624,31 @@ class TrackParams:
             raise ValueError(f"TrackParams.oks_threshold must be a number in [0, 1], not {t!r}")
 
 
+def _number(v) -> bool:
+    return not isinstance(v, bool) and isinstance(v, (int, float, np.integer, np.floating)) and bool(np.isfinite(v))
+
+
+@dataclasses.dataclass(frozen=True)
+class SmoothParams:
+    """``FrameStream``'s smoothing of tracked people's keypoints: a One-Euro filter (Casiez, Roussel and Vogel, CHI 2012)
+    per track and joint.  ``min_cutoff`` (Hz) is the cut-off at rest: lower removes more jitter; ``beta`` raises the
+    cut-off with the joint's filtered speed in person sizes per second: higher lags less in motion; ``d_cutoff`` (Hz)
+    filters that speed; ``rate`` (frames per second) spaces the frames submitted without a time
+    (``include/spgroup.h`` "smoothing" has the rules).  The defaults are a starting point, not tuned on real video."""
+    min_cutoff: float = 1.0
+    beta: float = 1.0
+    d_cutoff: float = 1.0
+    rate: float = 30.0
+
+    def __post_init__(self):
+        for name in ("min_cutoff", "d_cutoff", "rate"):
+            v = getattr(self, name)
+            if not _number(v) or not float(v) > 0.0:
+                raise ValueError(f"SmoothParams.{name} must be a finite number above 0, not {v!r}")
+        if not _number(self.beta) or not float(self.beta) >= 0.0:
+            raise ValueError(f"SmoothParams.beta must be a finite number at least 0, not {self.beta!r}")
+
+
 class _Key(NamedTuple):
     """A frame's part of a tick key: its size, its source -- a host or CUDA BGR image (``"image"``, ``"cuda"``), JPEG
     bytes the device decodes (``"jpeg"``), a ``YUVFrame`` with host or CUDA planes (``"yuv"``, ``"yuv_cuda"``) -- and its
@@ -635,18 +661,24 @@ class _Key(NamedTuple):
 
 class _Frame(NamedTuple):
     """A frame ``_admit`` took: its key, what is staged (a contiguous host or a CUDA image, JPEG bytes as uint8, the
-    ``YUVFrame``), its parsed JPEG record, and the image cv2 decoded or converted it to at submit, if it did."""
+    ``YUVFrame``), its parsed JPEG record, the image cv2 decoded or converted it to at submit, if it did, and with
+    smoothing its time in seconds."""
     key: _Key
     data: object
     rec: Optional[np.ndarray] = None
     decoded: Optional[np.ndarray] = None
+    t: Optional[float] = None
 
 
-def _admit(frames, streams, *, input_stage: str, device: int, n_streams: Optional[int]):
-    """A tick's frames and stream indices checked before anything is staged: per frame its ``_Frame``, the stream
-    indices as ints, and how many frames ``cv2.imdecode`` decoded.  ``n_streams``: ``TrackParams.streams``, or None
-    without tracking (only stream 0 exists).  A JPEG file the parser refuses, and with ``input_stage="host"`` every
-    JPEG or YUV frame, is staged as cv2's image of it."""
+def _admit(frames, streams, *, input_stage: str, device: int, n_streams: Optional[int], times=None, previous=None,
+           step: float = 0.0):
+    """A tick's frames, stream indices and times checked before anything is staged: per frame its ``_Frame``, the
+    stream indices as ints, and how many frames ``cv2.imdecode`` decoded.  ``n_streams``: ``TrackParams.streams``, or
+    None without tracking (only stream 0 exists).  ``times``: None or per frame its time or None; ``previous``: with
+    smoothing, per stream the time of its last frame (None before its first), and None without, when every time must
+    be None.  With smoothing each frame's ``t`` is its time, or its stream's previous one plus ``step`` (0.0 for the
+    stream's first frame), and must be finite and later than its stream's previous time.  A JPEG file the parser
+    refuses, and with ``input_stage="host"`` every JPEG or YUV frame, is staged as cv2's image of it."""
     import torch
     checked = []
     for s in streams:
@@ -658,6 +690,22 @@ def _admit(frames, streams, *, input_stage: str, device: int, n_streams: Optiona
         elif not 0 <= s < n_streams:
             raise ValueError(f"stream {s} is outside [0, {n_streams})")
         checked.append(int(s))
+    times = [None] * len(checked) if times is None else list(times)
+    if previous is None and any(t is not None for t in times):
+        raise ValueError("a frame's time needs smoothing (FrameStream(smooth=SmoothParams(...)))")
+    resolved, last = [], {}
+    if previous is not None:
+        for s, t in zip(checked, times):
+            prev = last.get(s, previous[s])
+            if t is None:
+                t = 0.0 if prev is None else prev + float(step)
+            elif not _number(t):
+                raise ValueError(f"a frame's time is a finite number of seconds, not {t!r}")
+            t = float(t)
+            if prev is not None and not t > prev:
+                raise ValueError(f"stream {s}: time {t!r} is not later than its previous frame's {prev!r}")
+            last[s] = t
+            resolved.append(t)
     out, decodes = [], 0
     for frame in frames:
         decoded = None
@@ -693,6 +741,8 @@ def _admit(frames, streams, *, input_stage: str, device: int, n_streams: Optiona
                 raise ValueError("a frame is a [H, W, 3] uint8 BGR image")
             source = "image"
         out.append(_Frame(_Key(int(frame.shape[0]), int(frame.shape[1]), source), frame, None, decoded))
+    if resolved:
+        out = [f._replace(t=t) for f, t in zip(out, resolved)]
     return out, checked, decodes
 
 
@@ -719,13 +769,16 @@ class _Tick:
                       for k, items in zip(keys, self.plan)]
         self.jpeg = [j for j, k in enumerate(keys) if k.source == "jpeg"]
         self.yuv = [j for j, k in enumerate(keys) if k.source in ("yuv", "yuv_cuda")]
-        # the one upload: the JPEG frames' records, with tracking the frames' stream indices (int32), then per frame its
-        # bytes: a JPEG frame's capacity, a host image (with input_stage="host" the pairs cv2 built go up instead) or a
-        # host YUV frame's packed planes.  A CUDA YUV frame's planes are copied into packed planes of their own.
+        # the one upload: the JPEG frames' records, with tracking the frames' stream indices (int32), with smoothing
+        # then their times (float64), then per frame its bytes: a JPEG frame's capacity, a host image (with
+        # input_stage="host" the pairs cv2 built go up instead) or a host YUV frame's packed planes.  A CUDA YUV frame's
+        # planes are copied into packed planes of their own.
         self.at, off = {}, _align(len(self.jpeg) * JPEG_RECORD.itemsize)
-        self.streams_at = None
+        self.streams_at = self.times_at = None
         if fs._track is not None:
             self.streams_at, off = off, _align(off + 4 * len(keys))
+        if fs._smooth is not None:
+            self.times_at, off = off, _align(off + 8 * len(keys))
         for j, (H, W, source, fmt) in enumerate(keys):
             size = {"jpeg": self.caps[j], "yuv": _yuv_bytes(fmt, H, W), "image": None if host_stage else H * W * 3}
             if size.get(source) is not None:
@@ -775,16 +828,30 @@ class _Tick:
                 self.track[j]["stream"] = self.up.data_ptr() + self.streams_at + 4 * j
                 self.track[j]["jpeg_status"] = self.status.data_ptr() + 4 * self.jpeg.index(j) if j in self.jpeg else 0
                 self.track[j]["ids"] = self.ids[j].data_ptr()
+        self.smooth = None
+        if fs._smooth is not None:  # per frame its people's smoothed joints, and its spg_smooth_frames member
+            self.xy = torch.empty((len(keys), fs._g.capR, 17, 2), dtype=torch.float64, device=dev)
+            self.xy_host = torch.empty(self.xy.shape, dtype=torch.float64, pin_memory=True)
+            self.smooth = np.zeros(len(keys), SMOOTH_FRAME)
+            for j in range(len(keys)):
+                self.smooth[j]["record"] = self.rec[j].data_ptr()
+                self.smooth[j]["stream"] = self.up.data_ptr() + self.streams_at + 4 * j
+                self.smooth[j]["ids"] = self.ids[j].data_ptr()
+                self.smooth[j]["time"] = self.up.data_ptr() + self.times_at + 8 * j
+                self.smooth[j]["xy"] = self.xy[j].data_ptr()
 
     def stage(self, frames: List[_Frame], streams: List[int]) -> None:
         """Write a tick's frames into this slot's buffers: the upload's host side (with tracking the stream indices, -1
-        skipping a frame), CUDA images and planes copied on the stream ahead of the graph, and with input_stage="host"
-        each item's pair built by cv2 into the pinned copy of its input."""
+        skipping a frame, with smoothing the times), CUDA images and planes copied on the stream ahead of the graph, and
+        with input_stage="host" each item's pair built by cv2 into the pinned copy of its input."""
         import torch
         host, copies = self.up_host.numpy(), []  # copies: (slot's device buffer, caller's CUDA tensor)
         if self.track is not None:
             host[self.streams_at:self.streams_at + 4 * len(frames)] = np.asarray(streams, np.int32).view(np.uint8)
-        for j, (key, data, rec, _) in enumerate(frames):
+        if self.smooth is not None:  # a re-posed frame (stream -1) has no time: it is skipped
+            times = np.asarray([0.0 if f.t is None else f.t for f in frames], np.float64)
+            host[self.times_at:self.times_at + 8 * len(frames)] = times.view(np.uint8)
+        for j, (key, data, rec, _, _) in enumerate(frames):
             at = self.at.get(j)
             if key.source == "jpeg":
                 jj = self.jpeg.index(j)
@@ -881,12 +948,23 @@ class FrameStream:
     frames are tracked in submit order, also across slots in flight; the stream indices travel in the tick's upload, so
     frames of any streams share a graph.  A frame whose record has a status bit (a crowded frame, whose people come from
     the capacity-free tier, or a grouping error) or whose JPEG decode was flagged is unobserved: its stream's tracks age
-    and its people get id -1, also after the flagged frame is posed again."""
+    and its people get id -1, also after the flagged frame is posed again.
+
+    ``smooth=SmoothParams(...)`` (with ``track``) filters each tracked person's joints across its stream's frames: a
+    One-Euro filter per track id and joint, ``spg_smooth_frames``, recorded into the graph after the tracking, with its
+    state in one table per stream on the device.  Each frame has a time in seconds (``submit(frame, t=...)``,
+    ``submit_many(frames, times=[...])``): a frame without one comes ``1 / rate`` after its stream's previous frame (its
+    stream's first at 0.0), and a time that is not finite or not later than its stream's previous one is refused
+    before anything is staged.  ``result(ticket, smoothed=True)`` gives each present joint of a tracked person its
+    filtered position (float64).  People with id -1 (an unobserved frame, a crowded frame's, a flagged JPEG frame posed
+    again) keep their raw joints; ``FrameResult.record`` and the maps stay raw."""
 
     _track: Optional[TrackParams] = None  # the tracking parameters, or None
+    _smooth: Optional[SmoothParams] = None  # the smoothing parameters, or None
 
     def __init__(self, model, params, model_params, *, slots: int = 2, input_stage: str = "device",
-                 device: Optional[int] = None, track: Optional[TrackParams] = None):
+                 device: Optional[int] = None, track: Optional[TrackParams] = None,
+                 smooth: Optional[SmoothParams] = None):
         if int(model_params["stride"]) != 4:
             raise ValueError(f"FrameStream needs stride 4 (model_params['stride'] is {model_params['stride']}): the "
                              "ragged and rotated post-network kernels it records are stride-4 kernels")
@@ -894,6 +972,10 @@ class FrameStream:
             raise ValueError("slots must be >= 1")
         if track is not None and not isinstance(track, TrackParams):
             raise ValueError(f"track is a TrackParams or None, not {track!r}")
+        if smooth is not None and not isinstance(smooth, SmoothParams):
+            raise ValueError(f"smooth is a SmoothParams or None, not {smooth!r}")
+        if smooth is not None and track is None:
+            raise ValueError("smoothing follows tracked people: FrameStream(smooth=...) needs track=TrackParams(...)")
         import torch
         self.model, self.params, self.model_params = model, dict(params), dict(model_params)
         self.input_stage = _stage(input_stage)
@@ -917,6 +999,12 @@ class FrameStream:
         self._track = track
         if track is not None:  # every stream's table of tracks, empty
             self._tables = torch.zeros((track.streams, TRACK_TABLE.itemsize), dtype=torch.uint8, device=self.device)
+        self._smooth = smooth
+        if smooth is not None:  # every stream's filter slots, empty, and the time of its last frame
+            self._smooth_tables = torch.zeros((track.streams, SMOOTH_TABLE.itemsize), dtype=torch.uint8,
+                                              device=self.device)
+            self._times: List[Optional[float]] = [None] * track.streams
+            self._smoothed: Dict[int, list] = {}  # finished tickets' smoothed people
 
     def close(self) -> None:
         for ticks in self._ticks:
@@ -931,21 +1019,23 @@ class FrameStream:
     def __exit__(self, *exc):
         self.close()
 
-    def submit(self, frame, *, stream: int = 0) -> int:
+    def submit(self, frame, *, stream: int = 0, t: Optional[float] = None) -> int:
         """Pose ``frame`` as a tick of one frame in the next slot and return its ticket.  ``frame`` is a ``[H, W, 3]``
         uint8 BGR image (numpy, or a CUDA tensor on the stream's device), a JPEG file's bytes or a ``YUVFrame``.
         ``submit(f)`` and ``submit_many([f])`` form the same tick key, so in one slot they share one graph.  ``stream``:
-        the frame's stream with tracking (``TrackParams.streams``); without, only 0."""
-        return self._submit([frame], [stream])[0]
+        the frame's stream with tracking (``TrackParams.streams``); without, only 0.  ``t``: with smoothing, the frame's
+        time in seconds, or None for its stream's previous time plus ``1 / SmoothParams.rate``; without, None."""
+        return self._submit([frame], [stream], [t])[0]
 
-    def submit_many(self, frames, *, streams=None) -> List[int]:
+    def submit_many(self, frames, *, streams=None, times=None) -> List[int]:
         """Pose a tick of ``K >= 1`` frames -- one frame per camera, or the next K frames of a video -- through one
         CUDA graph in the next slot, and return one ticket per frame, each read with ``result``.
 
         ``frames`` may mix every kind ``submit`` takes and every shape; it needs ``input_stage="device"``.  A frame
         ``submit`` would refuse refuses the whole tick before anything is staged; if the launch or its capture raises,
         no ticket is issued.  ``streams``: with tracking, None (every frame is stream 0's: the next K frames of one
-        video) or one stream per frame (one per camera, say); without, None."""
+        video) or one stream per frame (one per camera, say); without, None.  ``times``: with smoothing, None or one
+        time (or None) per frame, as ``submit``'s ``t``; without, None."""
         if self.input_stage != "device":
             raise ValueError("submit_many needs input_stage='device': the tick's network inputs are built by "
                              "spg_prenet_ragged")
@@ -953,14 +1043,21 @@ class FrameStream:
         streams = [0] * len(frames) if streams is None else list(streams)
         if len(streams) != len(frames):
             raise ValueError(f"{len(frames)} frames but {len(streams)} streams")
+        times = [None] * len(frames) if times is None else list(times)
+        if len(times) != len(frames):
+            raise ValueError(f"{len(frames)} frames but {len(times)} times")
         if not frames:
             raise ValueError("submit_many needs at least one frame")
-        return self._submit(frames, streams)
+        return self._submit(frames, streams, times)
 
-    def _submit(self, frames: list, streams: list) -> List[int]:
-        """Admit a tick's frames and stream indices (``_admit``), launch it in the next slot and return its tickets."""
+    def _submit(self, frames: list, streams: list, times: list) -> List[int]:
+        """Admit a tick's frames, stream indices and times (``_admit``), launch it in the next slot and return its
+        tickets."""
+        sm = self._smooth
         frames, streams, decodes = _admit(frames, streams, input_stage=self.input_stage, device=self.device,
-                                          n_streams=None if self._track is None else self._track.streams)
+                                          n_streams=None if self._track is None else self._track.streams, times=times,
+                                          previous=None if sm is None else self._times,
+                                          step=0.0 if sm is None else 1.0 / float(sm.rate))
         self.host_decodes += decodes
         slot = self._calls % len(self._busy)
         if self._busy[slot] is not None:
@@ -970,6 +1067,9 @@ class FrameStream:
         self._next += len(frames)
         self._calls += 1
         self._busy[slot] = (tickets, tk, done, frames)
+        if sm is not None:
+            for f, s in zip(frames, streams):
+                self._times[s] = f.t
         return tickets
 
     def _launch(self, slot: int, frames: List[_Frame], streams: List[int]):
@@ -1053,6 +1153,11 @@ class FrameStream:
             t = self._track
             g.track_frames(tk.track, self._tables.data_ptr(), t.streams, t.oks_threshold, t.max_age)
             tk.ids_host.copy_(tk.ids, non_blocking=True)
+        if tk.smooth is not None:
+            sm = self._smooth
+            g.smooth_frames(tk.smooth, self._smooth_tables.data_ptr(), self._track.streams, sm.min_cutoff, sm.beta,
+                            sm.d_cutoff)
+            tk.xy_host.copy_(tk.xy, non_blocking=True)
         tk.rec_host.copy_(tk.rec, non_blocking=True)
 
     def _capture(self, tk: _Tick) -> None:
@@ -1080,21 +1185,24 @@ class FrameStream:
         done.synchronize()
         records = tk.rec_host.numpy().copy()
         ids = tk.ids_host.numpy().copy() if tk.track is not None else None
+        xy = tk.xy_host.numpy().copy() if self._smooth is not None else None
         for j, ticket in enumerate(tickets):
             record, heat, paf, image = records[j], tk.heat[j], tk.paf[j], frames[j].decoded
             frame_ids = None if ids is None else ids[j]
+            frame_xy = None if xy is None else xy[j]
             if j in tk.jpeg and int(tk.status_host[tk.jpeg.index(j)]) != JPEG_OK:
                 image = _imdecode(tk.up_host[tk.at[j]:tk.at[j] + frames[j].data.size].numpy())
                 self.host_decodes += 1
                 frame = _Frame(_Key(image.shape[0], image.shape[1], "image"), image, None, image)
-                # the tick tracked the frame as unobserved: posing it again tracks nothing, and its people get -1
+                # the tick tracked the frame as unobserved: posing it again tracks and smooths nothing, and its people
+                # get -1 and keep their raw joints
                 again, d = self._launch(slot, [frame], [-1])
                 d.synchronize()
                 record, heat, paf = again.rec_host[0].numpy().copy(), again.heat[0].clone(), again.paf[0].clone()
-                frame_ids = None
+                frame_ids = frame_xy = None
             elif j in tk.jpeg or j in tk.yuv:
                 image = tk.images[j]  # decoded or converted on the device: copied to the host if detail asks for it
-            self._keep(ticket, record, heat, paf, tk.keys[j].height, tk.as_f64, frame_ids)
+            self._keep(ticket, record, heat, paf, tk.keys[j].height, tk.as_f64, frame_ids, frame_xy)
             self._held[ticket] = (heat, paf, tk.as_f64, image)
             tk.held.append(ticket)
 
@@ -1111,14 +1219,17 @@ class FrameStream:
             for tk in ticks.values():
                 tk.graph = None
 
-    def result(self, ticket: int, *, detail: bool = False, ids: bool = False):
+    def result(self, ticket: int, *, detail: bool = False, ids: bool = False, smoothed: bool = False):
         """``process()``'s value for the frame of ``ticket`` (waits for it); each ticket is read once.  ``detail=True``
         returns a ``FrameResult`` with the frame's wire record and copies of its maps, which needs the frame's buffers
         to still hold them: read it before ``slots`` later calls to ``submit`` or ``submit_many``.  ``ids=True`` (with
         tracking) returns ``(value, ids)``: per person its track's id within the frame's stream, -1 for the people of an
-        unobserved frame."""
+        unobserved frame.  ``smoothed=True`` (with smoothing) gives each present joint of a tracked person its filtered
+        position as float64; ``FrameResult.record`` and the maps stay raw."""
         if ids and self._track is None:
             raise ValueError("ids=True needs tracking (FrameStream(track=TrackParams(...)))")
+        if smoothed and self._smooth is None:
+            raise ValueError("smoothed=True needs smoothing (FrameStream(smooth=SmoothParams(...)))")
         for slot, busy in enumerate(self._busy):
             if busy is not None and ticket in busy[0]:
                 self._finish(slot)
@@ -1130,9 +1241,12 @@ class FrameStream:
             raise ValueError(f"ticket {ticket}: its slot holds a later frame; read detail=True before {len(self._busy)} "
                              "later submits")
         out = self._done.pop(ticket)
+        filtered = self._smoothed.pop(ticket, None) if self._smooth is not None else None
         if isinstance(out, Exception):
             raise out
         people, record, person_ids = out
+        if smoothed:
+            people = filtered
         value = people
         if detail:
             heat, paf, as_f64, image = held
@@ -1141,10 +1255,11 @@ class FrameStream:
             value = FrameResult(people, record, DeviceMaps(heat.clone(), False), DeviceMaps(paf.clone(), as_f64), image)
         return (value, person_ids) if ids else value
 
-    def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool, ids=None) -> None:
+    def _keep(self, ticket: int, record: np.ndarray, heat, paf, H: int, as_f64: bool, ids=None, xy=None) -> None:
         """Keep the people of one frame's wire record (or the error they raise) under its ticket, with their ids: with
-        tracking, ``ids`` the frame's ids output, or None for -1 each.  A record with a capacity bit is regrouped on the
-        capacity-free tier from the frame's maps."""
+        tracking, ``ids`` the frame's ids output, or None for -1 each; and with smoothing their smoothed joints from
+        ``xy``, the frame's smoothed output, or None for the raw joints.  A record with a capacity bit is regrouped on
+        the capacity-free tier from the frame's maps."""
         rec = wire.as_records(record, self._g.J, self._g.capR)[0]
         try:
             people = _people_of_record(rec, lambda: self._tier.group_unbounded(heat, paf, H, self._gp, paf_as_f64=as_f64,
@@ -1152,9 +1267,22 @@ class FrameStream:
             person_ids = None
             if self._track is not None:
                 person_ids = [-1] * len(people) if ids is None or rec["status"] else [int(v) for v in ids[:len(people)]]
+            if self._smooth is not None:
+                self._smoothed[ticket] = people if xy is None or rec["status"] else _smoothed_people(people, rec, xy)
             self._done[ticket] = (people, record, person_ids)
         except GroupingError as e:
             self._done[ticket] = e
+
+
+def _smoothed_people(people: list, rec, xy: np.ndarray) -> list:
+    """``process()``-style people of a wire record with each present joint's ``(x, y)`` taken from ``xy`` (the frame's
+    ``spg_smooth_frames`` output, ``[rows][17][2]``) as float64; absent joints stay as they are."""
+    out = []
+    for p, (pts, score) in enumerate(people):
+        present = int(rec["rows"][p]["present"])
+        out.append(([(np.float64(xy[p, g, 0]), np.float64(xy[p, g, 1])) if (present >> g) & 1 else pt
+                     for g, pt in enumerate(pts)], score))
+    return out
 
 
 def _upload_peaks(g: Grouper, all_peaks) -> None:

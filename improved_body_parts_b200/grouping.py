@@ -167,6 +167,15 @@ TRACK = np.dtype([("id", np.int64), ("age", np.int32), ("live", np.int32), ("xy"
 TRACK_TABLE = np.dtype([("next_id", np.int64), ("reserved", np.int64), ("tracks", TRACK, (TRACK_SLOTS,))], align=True)
 TRACK_FRAME = np.dtype([(f, np.uint64) for f in ("record", "stream", "jpeg_status", "ids", "oks")], align=True)
 
+#: ``spg_smooth_slot``, ``spg_smooth_table`` and ``spg_smooth_frame`` (include/spgroup.h): a stream's One-Euro filter
+#: slots, keyed by track id (caller-owned device memory; all zeros is an empty table), and one frame of
+#: ``spg_smooth_frames`` -- the device addresses of its wire record, its stream index (int32; -1 skips the frame), its
+#: ids (int64 per row), its time (float64, seconds) and its smoothed output ([rows][17][2] float64)
+SMOOTH_SLOT = np.dtype([("id", np.int64), ("last", np.int64), ("live", np.int32), ("mask", np.uint32),
+                        ("joint", np.float64, (17, 5))], align=True)
+SMOOTH_TABLE = np.dtype([("clock", np.int64), ("reserved", np.int64), ("slots", SMOOTH_SLOT, (TRACK_SLOTS,))], align=True)
+SMOOTH_FRAME = np.dtype([(f, np.uint64) for f in ("record", "stream", "ids", "time", "xy")], align=True)
+
 
 def jpeg_parse(data) -> np.ndarray:
     """``spg_jpeg_parse`` of one file's bytes (host only): a ``JPEG_RECORD`` whose ``status`` is ``JPEG_OK`` or the
@@ -238,6 +247,7 @@ _PROTOTYPES = {
     "spg_jpeg_reserve_frames": (_int, [_ptr, _ptr, _ptr, _i32, _P(C.c_int32)]),
     "spg_yuv_to_bgr": (_int, [_ptr, _ptr, _i32, _ptr]),  # members: a YUV_MEMBER array
     "spg_track_frames": (_int, [_ptr, _ptr, _i32, _ptr, _i32, _f64, _i32, _ptr]),  # frames: a TRACK_FRAME array
+    "spg_smooth_frames": (_int, [_ptr, _ptr, _i32, _ptr, _i32, _f64, _f64, _f64, _ptr]),  # frames: a SMOOTH_FRAME array
     "spg_nms_peaks": (_int, [_ptr, _ptr, _i64, _i64, _i32, _i32, _i32, _P(_Params), _ptr]),
     "spg_limb_score": (_int, [_ptr, _ptr, _i32, _i64, _i64, _i32, _i32, _i32, _f64, _P(_Params), _ptr]),
     "spg_limb_match": (_int, [_ptr, _i32, _P(_Params), _ptr]),
@@ -1143,6 +1153,16 @@ class Grouper:
         f = self._records(frames, TRACK_FRAME)
         _check(self._lib.spg_track_frames(self._h, f.ctypes.data, len(f), int(tables), int(n_tables), float(oks_threshold),
                                           int(max_age), self._stream_ptr(stream)), "spg_track_frames", self._h)
+
+    def smooth_frames(self, frames: np.ndarray, tables: int, n_tables: int, min_cutoff: float, beta: float,
+                      d_cutoff: float, stream=None) -> None:
+        """``spg_smooth_frames``: ``frames`` a ``SMOOTH_FRAME`` array, ``tables`` the device address of ``n_tables``
+        ``SMOOTH_TABLE`` records.  Each frame's tracked people get their joints filtered by their track's One-Euro
+        filters, in order.  Asynchronous on ``stream``; can be recorded into a CUDA graph."""
+        f = self._records(frames, SMOOTH_FRAME)
+        _check(self._lib.spg_smooth_frames(self._h, f.ctypes.data, len(f), int(tables), int(n_tables), float(min_cutoff),
+                                           float(beta), float(d_cutoff), self._stream_ptr(stream)),
+               "spg_smooth_frames", self._h)
 
     @staticmethod
     def _records(a: np.ndarray, dtype: np.dtype) -> np.ndarray:

@@ -414,6 +414,56 @@ typedef struct spg_track_frame {
 int spg_track_frames(spg_handle *h, const spg_track_frame *frames, int32_t n, spg_track_table *tables, int32_t n_tables,
                      double oks_threshold, int32_t max_age, void *stream);
 
+/* ---- smoothing tracked people's keypoints: a One-Euro filter (Casiez, Roussel and Vogel, CHI 2012) per track and joint
+ * A stream keeps a table of SPG_TRACK_SLOTS filter slots in caller-owned device memory, keyed by track id (the ids
+ * spg_track_frames writes); a zero-filled table is empty.  A slot holds a track's filter state per joint. */
+typedef struct spg_smooth_slot {
+    int64_t id;                 /* the track id the slot holds */
+    int64_t last;               /* the table's clock when the slot was last used */
+    int32_t live;               /* 0: the slot is free */
+    uint32_t mask;              /* bit g: joint g has state */
+    double joint[17][5];        /* per joint xh, yh, dxh, dyh, tj: the filtered position and speed, and its time */
+} spg_smooth_slot;
+typedef struct spg_smooth_table {
+    int64_t clock;              /* frames of the stream seen so far */
+    int64_t reserved;
+    spg_smooth_slot slots[SPG_TRACK_SLOTS];
+} spg_smooth_table;
+/* One frame of spg_smooth_frames; every address is device memory, read or written when the launch runs. */
+typedef struct spg_smooth_frame {
+    const void *record;         /* the frame's wire record, spg_wire_record_bytes(h) bytes (the handle's wire rows) */
+    const int32_t *stream;      /* the frame's table index in [0, n_tables), or -1: the frame is skipped */
+    const int64_t *ids;         /* [wire rows]: the track id of each of the first n_persons rows, or -1 */
+    const double *time;         /* the frame's time in seconds */
+    double *xy;                 /* [wire rows][17][2]: the first n_persons rows are written */
+} spg_smooth_frame;
+/* All arithmetic is float64, one rounding per operation in the order written, no fused multiply-add; TWO_PI =
+ * 6.283185307179586.  Per frame of a stream, in call order (several frames of one stream in one call are taken in call
+ * order):
+ *   1. the table's clock advances;
+ *   2. each person with id >= 0 finds the live slot holding its id; a person whose slot an earlier row of the frame
+ *      holds (a repeated id) is passed through raw;
+ *   3. in row order, each person with id >= 0 and no slot takes the lowest free slot or, in a full table, the slot not
+ *      used by this frame of smallest last (ties: the lowest index), whose state is reset (mask and joints 0); a person
+ *      whose id an earlier row of the frame took, or who finds no slot (more than SPG_TRACK_SLOTS ids in one frame), is
+ *      passed through raw;
+ *   4. used slots get last = clock;
+ *   5. per joint of a person with a slot: the joint is used when the row's presence mask has it and its x and y are
+ *      finite; over the used joints sc = ((xmax - xmin) + (ymax - ymin)) / 2, then sc = sc if sc > 1.0 else 1.0.  A used joint without
+ *      state (its mask bit clear) or whose dt = t - tj is not positive and finite takes xh = x, yh = y, dxh = dyh = 0,
+ *      tj = t and sets its mask bit; otherwise
+ *        vx = (x - xh) / dt / sc, vy = (y - yh) / dt / sc, ad = 1 / (1 + 1 / (TWO_PI * d_cutoff * dt)),
+ *        dxh = ad * vx + (1 - ad) * dxh, dyh = ad * vy + (1 - ad) * dyh, fc = min_cutoff + beta * sqrt(dxh * dxh +
+ *        dyh * dyh), a = 1 / (1 + 1 / (TWO_PI * fc * dt)), xh = a * x + (1 - a) * xh, yh = a * y + (1 - a) * yh, tj = t.
+ *      A used joint's output is (xh, yh); every other joint's is the row's (x, y), and its state is left alone.
+ * People with id -1 are passed through raw and change nothing.  A skipped frame (stream -1) changes no table; its rows
+ * are passed through raw.  The handle must have 17 output joints; min_cutoff > 0, d_cutoff > 0 and beta >= 0, all
+ * finite.  One CTA per stream of the call, from the first frame of it.  Asynchronous on `stream`; allocates nothing and
+ * never synchronises, and its launches depend on n alone, so it can be recorded into a CUDA graph and replayed with new
+ * records, ids, stream indices and times at the same addresses.  Frames may be reused as soon as the call returns. */
+int spg_smooth_frames(spg_handle *h, const spg_smooth_frame *frames, int32_t n, spg_smooth_table *tables, int32_t n_tables,
+                      double min_cutoff, double beta, double d_cutoff, void *stream);
+
 /* ---- training samples: the reference data server's Transformer.transform and Heatmapper.create_heatmaps ------
  * (py_cocodata_server/py_data_transformer.py:112-184, py_data_heatmapper.py:50-97).  What a call's samples share, the
  * reference's CanonicalConfig / TransformationParams: */
@@ -770,7 +820,7 @@ int spg_wire_wait(int32_t device, const uint64_t *word_dev, uint64_t value, void
 int64_t spg_launch_count(const spg_handle *h);
 /* name of the kernel variant the last launch of a stage used (0 nms_peaks, 1 limb_score, 2 limb_match, 3 assemble,
  * 4 post-network stage, 5 pre-network stage, 6 training samples, 7 training loss, 8 keypoint evaluation, 9 JPEG decode,
- * 10 YUV conversion, 11 tracking);
+ * 10 YUV conversion, 11 tracking, 12 smoothing);
  * "" before the first launch.  Profiling aid: lets bench.py label its per-kernel numbers with the ncu kernel name. */
 const char *spg_stage_kernel(const spg_handle *h, int32_t stage);
 
